@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- RAG /retrieve queries/sec on B200 (BASELINE.json metric).
+"""bench.py -- RAG /retrieve queries/sec on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Workload (config.workload): BASELINE.json configs[2] "hybrid dense+BM25+RRF /retrieve, 10M docs
 (768-d fp32 vectors + postings), top-10" -- the largest single-GPU configuration (the 100M x 768
-headline corpus is 307 GB in fp32 and does not fit one B200).  A step = one batch of 256 queries
+headline corpus is 307 GB in fp32 and does not fit one 80 GB H100).  A step = one batch of 256 queries
 through dense top-P + BM25 top-P + fuse.  N GPUs shard the SAME corpus by document (strong
 scaling): local candidates, one NCCL all-gather, merge + fuse on every rank.
 
@@ -15,6 +15,9 @@ One JSON line on rank 0:
   e2e     : queries/s through the public host-buffer API, H2D + D2H inside the timed region
   batch1  : the same two numbers at batch 1
   roofline: dominant kernel (dense scan) algorithmic GB/s against MEASURED_PEAKS.json
+  --dump-outputs DIR: after the timed steps, the fused results of the last timed step (what a caller of
+            retrieve_dev receives) as DIR/<name>.npy; the inputs are seeded, so two builds compare output for output.
+            A node without a dense / BM25 score (NaN in the API) is written as 0 with a 0/1 <name>_present mask.
   cpu_baseline / --impl reference: the CPU oracle (restated reference path; faiss/bm25s are not
             installable offline) on all host cores over a bounded sample, extrapolated linearly in N.
 """
@@ -78,7 +81,7 @@ WORKLOADS = {
     # name: (docs, dim, hybrid)
     "c3": (10_000_000, 768, True),
     "c2": (1_000_000, 768, False),
-    "headline": (100_000_000, 768, True),    # BASELINE.json metric corpus: needs >= 4 GPUs in fp32 (8 recommended)
+    "headline": (100_000_000, 768, True),    # BASELINE.json metric corpus: 8 x 80 GB GPUs in fp32 (38.4 GB of rows per GPU)
     "c4": (100_000_000, 1024, False),        # BASELINE.json configs[3]: 100M x 1024 dense, 8 GPUs (51.2 GB fp32 per GPU)
     "tiny": (200_000, 768, True),            # functional check of the harness
 }
@@ -93,13 +96,16 @@ def parse():
     ap.add_argument("--workload", default=os.environ.get("KRAG_BENCH_WORKLOAD", "c3"), choices=list(WORKLOADS))
     ap.add_argument("--batch", type=int, default=256)
     ap.add_argument("--k", type=int, default=10)
-    ap.add_argument("--dense-mode", type=int, default=0, help="0 auto, 1 scan (K1), 2 tensor-core TF32 (K2), 3 K2 pruning on a bf16 shadow (opt-in, +50%% memory)")
+    ap.add_argument("--dense-mode", type=int, default=0, help="0 auto, 1 scan (K1), 2 tensor-core K2 (bf16 prune pass), 3 K2 pruning on a bf16 shadow (opt-in, +50%% memory), 4 K2 TF32 prune pass")
     ap.add_argument("--embedding", default="auto", choices=["auto", "none", "bge-small", "bge-base", "bge-large"],
                     help="query embedding forward (K5) inside the step; auto = the bge model whose width is the corpus dim")
     ap.add_argument("--query-tokens", type=int, default=32, help="WordPiece tokens per query incl. [CLS]/[SEP]")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-optin", action="store_true", help="skip the extra OPT-IN measurement (bf16 shadow prune pass) after the default one")
     ap.add_argument("--cpu-sample-rows", type=int, default=40_000)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's results (final, dense, sparse, rank, ordinal, count; absent dense / sparse scores "
+                         "as 0 with dense_present / sparse_present masks) as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -109,7 +115,7 @@ def load_peaks():
     if os.path.exists(p):
         j = json.load(open(p))
         return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 class ClockSampler:
@@ -476,6 +482,8 @@ def run_ours(args):
             return sr.retrieve(None, terms_list, k, embedder=embedder, tokens=(flat_tok, tok_off))
         return sr.retrieve(qh, terms_list, k)
 
+    last = [None]      # what fn returned in the last timed step
+
     def timed(fn, steps, warmup):
         for _ in range(warmup):
             fn()
@@ -483,7 +491,7 @@ def run_ours(args):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(steps):
-            fn()
+            last[0] = fn()
         e1.record()
         barrier()
         ms = torch.tensor([e0.elapsed_time(e1)], dtype=torch.float64, device=dev)
@@ -497,6 +505,8 @@ def run_ours(args):
     l0 = ctx.launch_count()
     trace("timed ms_dev")
     ms_dev = timed(step_dev, args.steps, args.warmup)
+    # the result buffers are reused by later calls: copy the last timed step's results out now
+    dev_out = {name: t.cpu().numpy() for name, t in last[0].items()} if args.dump_outputs and rank == 0 else None
     launches = (ctx.launch_count() - l0) // (args.steps + args.warmup) * args.steps
     trace("timed ms_e2e")
     ms_e2e = timed(step_e2e, args.steps, args.warmup)
@@ -555,7 +565,7 @@ def run_ours(args):
     # shadow of the corpus (+50% memory, built here by one conversion pass); returned distances stay exact fp32.
     trace("default legs done")
     optin = None
-    if args.dense_mode == 0 and not args.no_optin and kern_id in (2, 3, 5):
+    if args.dense_mode == 0 and not args.no_optin and kern_id in (3, 5):
         t_sh = time.perf_counter()
         ix.set_dense_mode(_native.DENSE_TC_BF16)
         t_sh = time.perf_counter() - t_sh
@@ -588,23 +598,16 @@ def run_ours(args):
         gbs = kern_bytes / (kern_ms * 1e-3) / 1e9
         gbs1 = kern1_bytes / (kern1_ms * 1e-3) / 1e9
         tflops = kern_flops / (kern_ms * 1e-3) / 1e12
-        tf32_peak = float(peaks.get("bf16_tflops", 1590.0)) / 2.0   # TF32 dense = half the measured bf16 rate
-        if kern_id in (4, 5):     # kind::f16 prune pass (bf16 operands), timed back to back: the sustained bf16 figure
-            tensor_peak = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 1590.0)))
-            tensor_peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (kind::f16 MMAs)"
+        tf32_peak = float(peaks.get("bf16_tflops", 989.0)) / 2.0   # TF32 dense = half the bf16 rate
+        if kern_id in (4, 5):     # bf16 wgmma prune pass, timed back to back: the sustained bf16 figure
+            tensor_peak = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 989.0)))
+            tensor_peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (bf16 wgmma), else the H100 SXM data sheet"
         else:
-            tensor_peak, tensor_peak_src = tf32_peak, "MEASURED_PEAKS.json bf16_tflops / 2 (TF32 dense rate)"
-        # dram__bytes_read.sum + dram__bytes_write.sum of the same kernel on the same workload from the committed
-        # ncu --set full capture (profiles/traffic.json names the report); null when no capture matches this run
-        traffic = None
-        tpath = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.exists(tpath) and world == 1:
-            traffic = json.load(open(tpath)).get(args.workload, {}).get(str(kern_id))
+            tensor_peak, tensor_peak_src = tf32_peak, "MEASURED_PEAKS.json bf16_tflops / 2 (TF32 dense rate), else the H100 SXM data sheet"
         kname = {1: "K1 dense_scan_kernel (exact fp32 L2^2 scan + fused top-P)",
-                 2: "K2 dense_tc_kernel (tcgen05 cta_group::1 TF32 prune pass; exact fp32 rescoring follows)",
-                 3: "K2 dense_tc2_kernel (tcgen05 cta_group::2 TF32 prune pass, CTA pairs; exact fp32 rescoring follows)",
-                 5: "K2 dense_tc2cvt_kernel (tcgen05 cta_group::2 kind::f16 prune pass; fp32 corpus rows staged by TMA and rounded to bf16 in shared memory -- no shadow copy, 4 B/element from HBM; exact fp32 rescoring follows)",
-                 4: "K2 dense_tc2_kernel<bf16> (OPT-IN: prune pass over a bf16 shadow of the corpus, kind::f16; exact fp32 rescoring of the fp32 corpus follows)"}
+                 3: "K2 dense_tc_kernel<TC_TF32> (tf32 wgmma prune pass; exact fp32 rescoring follows)",
+                 5: "K2 dense_tc_kernel<TC_CVT> (bf16 wgmma prune pass; fp32 corpus rows staged by TMA and rounded to bf16 on their way into the A registers -- no shadow copy, 4 B/element from HBM; exact fp32 rescoring follows)",
+                 4: "K2 dense_tc_kernel<TC_BF16> (OPT-IN: bf16 wgmma prune pass over a bf16 shadow of the corpus; exact fp32 rescoring of the fp32 corpus follows)"}
         qps = B * args.steps / (ms_dev * 1e-3)
         qps_e2e = B * args.steps / (ms_e2e * 1e-3)
         h2d, d2h = ShardedRetriever.io_bytes(B, dim, n_terms, k)
@@ -616,9 +619,9 @@ def run_ours(args):
             embed_info = {"model_shape": emb_name, "weights": "random init N(0, 0.02) (no checkpoints offline)", "tokens_per_query": args.query_tokens,
                           "batch_ms": ms_embed / args.steps, "batch1_ms": ms_embed1 / (args.steps * 4), "flops_per_batch": fl,
                           "tflops": etf, "tflops_per_gpu": etf / world,
-                          "arithmetic": "split-fp16 operands (hi + lo*2^-11), 3 kind::f16 MMAs per step: fp32-accurate products; "
+                          "arithmetic": "split-fp16 operands (hi + lo*2^-11), 3 fp16 wgmma per step: fp32-accurate products; "
                                         "tflops counts the fp32-equivalent flops L(24 S d^2 + 4 S^2 d), the tensor pipe executes 3x the GEMM part",
-                          "tensor_frac_of_f16_peak_per_gpu": 3.0 * etf / world / float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 1590.0))),
+                          "tensor_frac_of_f16_peak_per_gpu": 3.0 * etf / world / float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 989.0))),
                           "queries_per_s": B / (ms_embed / args.steps * 1e-3)}
         line = {
             "metric": "rag_retrieve_queries_per_sec", "value": qps, "unit": "queries/s", "n_gpus": world,
@@ -627,7 +630,7 @@ def run_ours(args):
             "config": {"workload": f"{args.workload}: {docs} docs x {dim} fp32 resident" + (" (+ bf16 shadow for the prune pass: OPT-IN mode, not the default)" if args.dense_mode == 3 else "") +
                                    (f" + BM25 postings nnz={st.nnz} (local), vocab 2^20, hybrid weighted fusion" if hybrid else ", dense only"),
                        "global_batch": B, "top_k": k, "candidate_pool": P, "parallelism": f"doc-shard x{world}",
-                       "rows_per_gpu": n_local, "cache": "inputs larger than L2 (corpus >> 126 MB); no explicit flush",
+                       "rows_per_gpu": n_local, "cache": "inputs larger than L2 (corpus >> 50 MB); no explicit flush",
                        "query_embedding": (f"K5 BERT forward ({emb_name} shapes, {args.query_tokens} tokens/query, random-init weights) "
                                            "INSIDE the timed region of value, e2e and batch1") if embedder else
                                           "precomputed query vectors (embedding forward not in the timed region)",
@@ -639,7 +642,7 @@ def run_ours(args):
             "batch1": {"value": args.steps * 4 / (ms_b1 * 1e-3), "e2e": args.steps * 4 / (ms_b1_e2e * 1e-3), "unit": "queries/s",
                        "ms_per_query": ms_b1 / (args.steps * 4), "dense_kernel_ms": kern1_ms, "dense_kernel_gbs": gbs1, "dense_frac": gbs1 / peak},
             "gpu_launches": int(launches),
-            "roofline": {"bound": "hbm", "achieved": gbs, "peak": peak, "unit": "GB/s", "frac": gbs / peak, "traffic": traffic,
+            "roofline": {"bound": "hbm", "achieved": gbs, "peak": peak, "unit": "GB/s", "frac": gbs / peak,
                          "kernel": kname[kern_id], "peak_source": peak_src, "kernel_ms": kern_ms,
                          "algorithmic_bytes_per_launch": kern_bytes, "flops_per_launch": kern_flops,
                          "tensor_tflops": tflops, "tensor_peak": tensor_peak, "tensor_frac": tflops / tensor_peak,
@@ -658,6 +661,16 @@ def run_ours(args):
         if not args.no_cpu_baseline and world == 1:      # the CPU leg is reported at N = 1 only (rank 0 would stall the other ranks)
             line["cpu_baseline"] = cpu_reference_qps(docs, dim, hybrid, k, args.cpu_sample_rows, emb_name, args.query_tokens, n_queries=B)
         print(json.dumps(line), flush=True)
+        if dev_out is not None:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            for name, a in dev_out.items():   # ordinals (< 2^32) are exact in float64, ranks and counts in float32
+                a = a.astype(np.float64 if a.dtype in (np.float64, np.int64) else np.float32)
+                if name in ("dense", "sparse"):
+                    # NaN marks a node without that score (include/kaito_rag.h): written as 0 plus a 0/1 presence mask
+                    present = np.isfinite(a)
+                    np.save(os.path.join(args.dump_outputs, f"{name}_present.npy"), present.astype(np.float32))
+                    a = np.where(present, a, 0).astype(a.dtype)
+                np.save(os.path.join(args.dump_outputs, f"{name}.npy"), a)
     trace("line printed; teardown")
     barrier()
     if embedder:

@@ -9,7 +9,7 @@
 
 Reports chunks/s per stage and end to end (max over ranks, CUDA-synchronised wall clock), the K5 rate, and -- the bar
 SURVEY.md section 2.3 sets for K5 -- the same forward through torch's own bf16 BertModel (SDPA attention, cuBLAS GEMMs) on
-the same GPU.  Not the driver's bench (that is bench.py, /retrieve); numbers from this script go to profiles/ and DESIGN.md."""
+the same GPU.  Not the /retrieve bench (that is bench.py); prints one JSON line."""
 import argparse
 import json
 import os
@@ -122,7 +122,7 @@ if not a.no_torch and rank == 0:
 if rank == 0:
     fl = bench.bert_flops(cfg, a.seq) * a.chunks
     peaks = json.load(open("MEASURED_PEAKS.json")) if os.path.exists("MEASURED_PEAKS.json") else {}
-    f16_peak = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 1590.0)))
+    f16_peak = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 989.0)))   # else the H100 SXM data sheet (dense bf16)
     k5_rate = a.chunks / t_embed
     print(json.dumps({
         "metric": "index_chunks_per_sec", "unit": "chunks/s", "n_gpus": world, "data": "synthetic", "scaling": "strong",
@@ -131,7 +131,7 @@ if rank == 0:
         "value": a.chunks / (t_embed + t_add + t_commit),
         "embed": {"chunks_per_s": k5_rate, "chunks_per_s_per_gpu": k5_rate / world, "tflops_fp32_equivalent": fl / t_embed / 1e12,
                   "tensor_frac_of_f16_peak_per_gpu": 3.0 * fl / t_embed / 1e12 / world / f16_peak,
-                  "arithmetic": "split-fp16 operands, 3 kind::f16 MMAs per step (fp32-accurate); includes D2H of the embeddings",
+                  "arithmetic": "split-fp16 operands, 3 fp16 wgmma per step (fp32-accurate); includes D2H of the embeddings",
                   "flops_formula": "L*(24*S*d^2 + 4*S^2*d) per chunk (SURVEY.md 8d)"},
         "torch_same_gpu": torch_ref,
         "k5_vs_torch": None if torch_ref is None else {k: (k5_rate / world) / v["chunks_per_s"] for k, v in torch_ref.items() if isinstance(v, dict)},

@@ -2,7 +2,7 @@
  * create an index, add a few nodes (dense rows + term lists), commit, run the hybrid /retrieve path, print the result.
  *
  *   gcc -std=c99 -Iinclude examples/krag_demo.c -o krag_demo -Lkaito_b200 -lkaito_rag -Wl,-rpath,$PWD/kaito_b200 -lm
- *   ./krag_demo            # needs an sm_100 GPU: krag_init fails with KRAG_E_NO_DEVICE otherwise (no CPU fallback)
+ *   ./krag_demo            # needs an sm_90 (H100) GPU: krag_init fails with KRAG_E_NO_DEVICE otherwise (no CPU fallback)
  */
 #include <math.h>
 #include <stdio.h>

@@ -1,5 +1,5 @@
 /*
- * kaito_rag.h -- C ABI of libkaito_rag.so, the B200 (sm_100a) retrieval engine behind
+ * kaito_rag.h -- C ABI of libkaito_rag.so, the H100 (sm_90a) retrieval engine behind
  * KAITO's RAGService /retrieve and /index.
  *
  * The reference has no in-process FFI seam: its service is Python calling pip wheels
@@ -11,7 +11,7 @@
  *   - every call returns int32 status: 0 = KRAG_OK, negative = KRAG_E_*;
  *     krag_last_error() returns a thread-local UTF-8 message for the last failure.
  *   - caller owns host buffers; the library owns device memory; handles are opaque.
- *   - NO CPU FALLBACK: without an sm_100 device krag_init fails with KRAG_E_NO_DEVICE.
+ *   - NO CPU FALLBACK: without an sm_90 device krag_init fails with KRAG_E_NO_DEVICE.
  *   - thread-safety mirrors the reference's aiorwlock (vector_store/base.py:77-79):
  *     searches on one index may run concurrently, mutations are exclusive.
  *   - "ordinal" = position of a node in insertion order (global across shards:
@@ -31,7 +31,7 @@ extern "C" {
 
 #define KRAG_OK 0
 #define KRAG_E_INVALID (-1)     /* bad argument */
-#define KRAG_E_NO_DEVICE (-2)   /* no sm_100 CUDA device / driver */
+#define KRAG_E_NO_DEVICE (-2)   /* no sm_90 CUDA device / driver */
 #define KRAG_E_CUDA (-3)        /* CUDA runtime error (message has details) */
 #define KRAG_E_OOM (-4)         /* device or host allocation failed */
 #define KRAG_E_NOT_FOUND (-5)   /* unknown index / node id */
@@ -52,12 +52,12 @@ extern "C" {
 
 #define KRAG_DENSE_AUTO 0   /* exact fp32 scan for small batches, tensor-core path for large */
 #define KRAG_DENSE_SCAN 1   /* K1: exact fp32 CUDA-core scan */
-#define KRAG_DENSE_TC 2     /* K2: tcgen05 prune pass (fp32 rows rounded to bf16 in shared memory, kind::f16; TF32 when the
+#define KRAG_DENSE_TC 2     /* K2: wgmma prune pass (fp32 rows rounded to bf16 on chip, bf16 wgmma; TF32 when the
                                padded dimension is not a multiple of 64) + exact fp32 rescoring */
 #define KRAG_DENSE_TC_BF16 3 /* K2 pruning on a bf16 SHADOW copy of the corpus (+50% memory); the returned distances are
                                still exact fp32 re-scores of the fp32 corpus and carry the same exactness certificate */
 
-#define KRAG_DENSE_TC_TF32 4 /* K2 with the fp32 rows consumed directly as TF32 (kind::tf32): the earlier default, kept for comparison */
+#define KRAG_DENSE_TC_TF32 4 /* K2 with the fp32 rows consumed directly as TF32 (tf32 wgmma), kept for comparison */
 
 typedef struct krag_ctx krag_ctx;
 typedef struct krag_index krag_index;
@@ -264,7 +264,7 @@ int32_t krag_wordpiece_encode_batch(const krag_wordpiece* w, int64_t n, const ch
 int32_t krag_wordpiece_destroy(krag_wordpiece* w);
 
 /* ------------------------------------------------------------------- diagnostics */
-/* C[M,N] = A[M,K] . B[N,K]^T + bias (+erf-GELU) (+residual) through K5's tcgen05 TF32 GEMM; host buffers.
+/* C[M,N] = A[M,K] . B[N,K]^T + bias (+erf-GELU) (+residual) through K5's split-fp16 wgmma GEMM; host buffers.
  * N % 128 == 0, K % 32 == 0.  Test hook. */
 int32_t krag_debug_gemm_tf32(krag_ctx* ctx, int32_t M, int32_t N, int32_t K, const float* A, const float* B,
                              const float* bias, const float* residual, int32_t gelu, float* C_out);
@@ -281,11 +281,11 @@ int32_t krag_index_set_dense_mode(krag_index* idx, int32_t dense_mode, int32_t r
  * exact scan kernel (process-wide counter) */
 int64_t krag_tc_fallback_queries(void);
 /* CUDA-event duration of the dominant dense kernel of the last search on this process
- * (kernel_id 1 = K1 exact scan, 2 = K2 tcgen05 main pass), with the algorithmic bytes and
+ * (kernel_id 1 = K1 exact scan; K2 main pass: 3 = TF32, 4 = bf16 shadow, 5 = fp32 rows rounded to bf16 on chip), with the algorithmic bytes and
  * flops of that launch -- bench.py's roofline line is computed from it. */
 int32_t krag_last_dense_kernel(float* ms, int32_t* kernel_id, int64_t* algorithmic_bytes, int64_t* flops);
 /* raw K2 output a[j][r] = |x_r|^2 - 2 x_r.q_j (TF32) for every row, [nq_pad][S] row-major;
- * call with out == NULL to query S and nq_pad.  Test hook for the tcgen05 kernel. */
+ * call with out == NULL to query S and nq_pad.  Test hook for the tensor-core kernel. */
 int32_t krag_debug_tc_dump(krag_index* idx, int32_t nq, const float* q, float* out, int64_t out_elems,
                            int64_t* S_out, int32_t* nq_pad_out);
 

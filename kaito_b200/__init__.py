@@ -1,6 +1,6 @@
-"""kaito_b200 -- B200-native retrieval engine behind KAITO's RAGService /retrieve and /index.
+"""kaito_b200 -- H100-native retrieval engine behind KAITO's RAGService /retrieve and /index.
 
-`kaito_b200._native` binds libkaito_rag.so (hand-written sm_100a CUDA, C ABI in
+`kaito_b200._native` binds libkaito_rag.so (hand-written sm_90a CUDA, C ABI in
 include/kaito_rag.h).  The host-side mirror of the reference's RAGService classes lives in
 `kaito_b200.vector_store` / `kaito_b200.retriever`.  There is no CPU fallback.
 """

@@ -1,7 +1,7 @@
 """ctypes binding of libkaito_rag.so (include/kaito_rag.h).
 
 The CUDA library IS the product path: there is no CPU or PyTorch fallback.  Importing this
-module without the built library, or initialising it without an sm_100 GPU, raises.
+module without the built library, or initialising it without an sm_90 (H100) GPU, raises.
 """
 from __future__ import annotations
 

@@ -387,9 +387,9 @@ int32_t krag_init(const krag_config* cfg, krag_ctx** out)
         KRAG_CUDA(cudaSetDevice(cfg->device_id));
         cudaDeviceProp p;
         KRAG_CUDA(cudaGetDeviceProperties(&p, cfg->device_id));
-        KRAG_REQUIRE(p.major == 10, KRAG_E_NO_DEVICE,
+        KRAG_REQUIRE(p.major == 9 && p.minor == 0, KRAG_E_NO_DEVICE,
                      std::string("device is sm_") + std::to_string(p.major) + std::to_string(p.minor) +
-                         "; libkaito_rag is built for sm_100a only");
+                         "; libkaito_rag is built for sm_90a only");
         krag_ctx* c = new krag_ctx();
         c->cfg = *cfg;
         if (c->cfg.world_size <= 0) c->cfg.world_size = 1;

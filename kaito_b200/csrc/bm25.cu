@@ -58,7 +58,7 @@ void launch_df_histogram(const uint32_t* term_ids, const uint32_t* entry_doc, co
                          uint32_t* df, cudaStream_t st)
 {
     if (nnz == 0) return;
-    df_hist_kernel<<<148 * 8, 256, 0, st>>>(term_ids, entry_doc, alive, nnz, df);
+    df_hist_kernel<<<132 * 8, 256, 0, st>>>(term_ids, entry_doc, alive, nnz, df);
     KRAG_CUDA(cudaGetLastError());
     count_launch();
 }
@@ -350,10 +350,10 @@ void build_postings(const uint32_t* term_ids, const uint16_t* term_tf, const uin
             size_t sb = sort_bytes;
             cub::DeviceRadixSort::SortPairs(sort_tmp, sb, k_in, k_out, v_in, v_out, m, 0, end_bit, st);
             count_launch();
-            score_postings_kernel<<<148 * 8, 256, 0, st>>>(k_out, v_out, doc_len, idf, avgdl, m, post_doc + p_base, post_score + p_base);
+            score_postings_kernel<<<132 * 8, 256, 0, st>>>(k_out, v_out, doc_len, idf, avgdl, m, post_doc + p_base, post_score + p_base);
             count_launch();
             if (out.n_slots > 0) {
-                tile_index_kernel<<<148 * 8, 256, 0, st>>>(k_out, post_doc, off, out.tile_slot, p_base, m, out.n_tiles, out.tile_off);
+                tile_index_kernel<<<132 * 8, 256, 0, st>>>(k_out, post_doc, off, out.tile_slot, p_base, m, out.n_tiles, out.tile_off);
                 KRAG_CUDA(cudaGetLastError());
                 count_launch();
             }

@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host helpers for libkaito_rag (sm_100a only).
+// common.cuh -- shared device/host helpers for libkaito_rag (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

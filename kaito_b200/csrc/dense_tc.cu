@@ -1,27 +1,29 @@
-// dense_tc.cu -- K2: batched dense search on the 5th-gen tensor cores.
+// dense_tc.cu -- K2: batched dense search on the Hopper tensor cores (wgmma).
 //
 // Replaces faiss IndexFlatL2.search for query batches (its nq >= 20 sgemm path; reference
 // call site presets/ragengine/vector_store/faiss_store.py:44-49 via hybrid_retriever.py:209-213).
 //
-//   1. dense_tc_kernel<NQ, DUMP>  (tcgen05.mma kind::tf32, TMA-staged, accumulators in TMEM)
-//        D[128 corpus rows x NQ queries] = X_tile . Q^T, fp32 corpus fed as TF32 straight
-//        from HBM (no conversion pass; the corpus is streamed exactly once per pass).
+//   1. dense_tc_kernel<NQ, MODE, DUMP>  (wgmma, TMA-staged, accumulators in registers)
+//        D[128 corpus rows x NQ queries] = X_tile . Q^T.  The prune pass has three operand modes:
+//          TC_CVT  (default) fp32 corpus rows staged by TMA, rounded to bf16 while they are loaded into the
+//                  A-operand registers, bf16 queries from shared memory: 4 bytes/element from HBM, bf16 tensor rate
+//          TC_TF32 fp32 corpus and queries consumed as TF32 straight from shared memory
+//          TC_BF16 (opt-in) a bf16 shadow of the corpus: half the HBM bytes
 //        epilogue: a = |x|^2 - 2 x.q  per (row, query), compared with a per-query threshold;
 //        rows below it are appended to that query's candidate list (rare: ~C of N rows).
-//        DUMP mode writes `a` for a strided 1/64 sample of the tiles instead.
+//        DUMP mode writes `a` (TF32) for a strided 1/64 sample of the tiles instead.
 //   2. sample_threshold_kernel: per query, the m-th smallest sampled `a` -> threshold that
 //        admits ~C = max(512, 4P) rows of the full corpus.
 //   3. rescore_kernel: EXACT fp32 squared L2 of every candidate in K1's operation order
 //        (bit-identical to dense_scan.cu / the oracle), then the ordinary top-P merge.
 //   4. certify_kernel: a query's result is exact if every non-candidate row is provably
 //        farther than the P-th exact distance:  D_P <= thr + |q|^2 - 2 eps,  eps = worst-case
-//        TF32 dot-product error (2^-9 + 2^-12) |x|_max |q|.  Queries that fail (candidate
+//        TF32 / bf16 dot-product error times |x|_max |q|.  Queries that fail (candidate
 //        overflow, adversarial near-duplicates) are re-run on the exact scan kernel K1.
 //
 // So the tensor cores only PRUNE; every returned score is an exact fp32 distance.
 //
-// Roofline: bytes = n_rows*dpad*4 per pass (HBM), flops = 2*NQ*n_rows*dpad (TF32 pipe).
-// At NQ = 256 the kernel sits on the HBM/TF32 ridge (128 flop/byte).
+// Roofline: bytes = n_rows*dpad*4 per pass (HBM; 2 with the bf16 shadow), flops = 2*NQ*n_rows*dpad.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <math_constants.h>
@@ -39,227 +41,201 @@
 namespace krag {
 
 // ------------------------------------------------------------------------- the kernel
-constexpr int TC_TILE_M = 128;          // corpus rows per tile (UMMA M)
+constexpr int TC_TILE_M = 128;          // corpus rows per tile: two consumer warpgroups x wgmma M = 64
 constexpr int TC_KBLOCK = 32;           // fp32 elements per k-block = one 128-byte swizzle row
-constexpr int TC_THREADS = 352;         // warp 0: corpus TMA, warp 1: MMA issuer, warp 2: query TMA, warps 3-10: epilogue
+constexpr int TC_THREADS = 384;         // warpgroup 0: TMA producer, warpgroups 1-2: wgmma + epilogue
 constexpr int TC_SAMPLE_STRIDE = 64;    // DUMP mode visits every 64th tile
-constexpr int TC_A_BYTES = TC_TILE_M * TC_KBLOCK * 4;  // 16 KB
+constexpr int TC_A_BYTES = TC_TILE_M * 128;  // 16 KB: 128 rows x one 128-byte swizzle row
+constexpr int TC_DUMP_GROUP = 16;       // rows per minimum in the threshold-sampling dump (one warp's wgmma rows)
 
-// Two independent shared-memory rings.  The corpus ring is deep because its slabs come from
-// HBM (latency ~2 us under load: ~100 KB must be in flight per SM to sustain 6.5 TB/s); the
-// query ring is shallow because its slabs are L2 hits re-read for every tile.
-template <int NQ> struct TcCfg {
-    static constexpr int Q_BYTES = NQ * TC_KBLOCK * 4;
-    static constexpr int Q_STAGES = (NQ == 256) ? 3 : 4;
-    static constexpr int A_STAGES = (NQ == 256) ? 7 : (NQ == 128 ? 9 : 11);
-    static constexpr int TMEM_COLS = (2 * NQ < 32) ? 32 : 2 * NQ;  // double-buffered accumulators
-    static constexpr int BAR_BYTES = 512;
-    static constexpr size_t SMEM = (size_t)A_STAGES * TC_A_BYTES + (size_t)Q_STAGES * Q_BYTES + 1024 /*align*/ + BAR_BYTES + NQ * 4;
+enum { TC_TF32 = 0, TC_BF16 = 1, TC_CVT = 2 };
+
+// One ring; a stage holds the corpus rows of the tile and all NQ query rows for 32 (TF32) or 64 (bf16) elements of
+// the dimension: 4 wgmma K steps either way.  In TC_CVT mode the corpus part is two fp32 k-blocks.
+template <int NQ, int MODE> struct TcCfg {
+    static constexpr int A_BYTES = (MODE == TC_CVT ? 2 : 1) * TC_A_BYTES;
+    static constexpr int Q_BYTES = NQ * 128;
+    static constexpr int STAGE_BYTES = A_BYTES + Q_BYTES;
+    static constexpr int STAGES = (200 * 1024) / STAGE_BYTES > 8 ? 8 : (200 * 1024) / STAGE_BYTES;
+    static constexpr int ELEMS = MODE == TC_TF32 ? TC_KBLOCK : 2 * TC_KBLOCK;   // dimension elements per stage
+    static constexpr int BAR_BYTES = 256;
+    static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + 1024 /*align*/ + BAR_BYTES + NQ * 4;
 };
 
-template <int NQ, bool DUMP>
+// bf16 A fragment (mma.sync / wgmma register layout) of K step s from a TMA-swizzled fp32 staging stage: this thread's
+// rows r and r + 8 (r & 7 == g), elements 16 s + 2 q (+1) and 16 s + 8 + 2 q (+1), rounded to nearest even
+__device__ __forceinline__ void cvt_a_fragment(const unsigned char* stage_a, int r, int g, int q, int s, uint32_t* a)
+{
+    const unsigned char* box = stage_a + (s >> 1) * TC_A_BYTES;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {              // h = 0: elements e, e + 1; h = 1: e + 8, e + 9
+        const int e = 16 * (s & 1) + 8 * h + 2 * q;
+        const int off = (((e >> 2) ^ g) << 4) + ((e & 3) << 2);
+        const float2 v0 = *reinterpret_cast<const float2*>(box + r * 128 + off);
+        const float2 v1 = *reinterpret_cast<const float2*>(box + (r + 8) * 128 + off);
+        const __nv_bfloat162 b0 = __floats2bfloat162_rn(v0.x, v0.y), b1 = __floats2bfloat162_rn(v1.x, v1.y);
+        a[2 * h + 0] = *reinterpret_cast<const uint32_t*>(&b0);
+        a[2 * h + 1] = *reinterpret_cast<const uint32_t*>(&b1);
+    }
+}
+
+template <int NQ, int MODE, bool DUMP>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 dense_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmQ, int64_t n_rows,
-                int kblocks, int64_t n_ltiles, int tile_stride, const float* __restrict__ xnorm,
+                int kblocks /*stages per tile*/, int64_t n_ltiles, int tile_stride, const float* __restrict__ xnorm,
                 const uint32_t* __restrict__ alive, const float* __restrict__ thr_g, uint32_t* __restrict__ cand_count,
                 uint32_t* __restrict__ cand_rows, int cap, float* __restrict__ dump, int64_t S, int dump_min)
 {
-    using Cfg = TcCfg<NQ>;
+    using Cfg = TcCfg<NQ, MODE>;
+    constexpr int R = NQ / 2;                   // accumulators per thread
     extern __shared__ unsigned char tc_smem_raw[];
-    unsigned char* smem_a = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~(uintptr_t)1023);
-    unsigned char* smem_q = smem_a + (size_t)Cfg::A_STAGES * TC_A_BYTES;
-    unsigned char* tail = smem_q + (size_t)Cfg::Q_STAGES * Cfg::Q_BYTES;
-    uint64_t* afull = reinterpret_cast<uint64_t*>(tail);               // [A_STAGES]
-    uint64_t* aempty = afull + Cfg::A_STAGES;                           // [A_STAGES]
-    uint64_t* qfull = aempty + Cfg::A_STAGES;                           // [Q_STAGES]
-    uint64_t* qempty = qfull + Cfg::Q_STAGES;                           // [Q_STAGES]
-    uint64_t* tfull_bar = qempty + Cfg::Q_STAGES;                       // [2]
-    uint64_t* tempty_bar = tfull_bar + 2;                               // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
+    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~(uintptr_t)1023);
+    unsigned char* tail = smem + (size_t)Cfg::STAGES * Cfg::STAGE_BYTES;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);            // [STAGES] producer arrival + TMA bytes
+    uint64_t* empty_bar = full_bar + Cfg::STAGES;                       // [STAGES] one arrival per consumer warp
     float* s_thr = reinterpret_cast<float*>(tail + Cfg::BAR_BYTES);     // [NQ]
-    static_assert((2 * (Cfg::A_STAGES + Cfg::Q_STAGES) + 4) * 8 + 8 <= Cfg::BAR_BYTES, "barrier area too small");
+    static_assert(2 * Cfg::STAGES * 8 <= Cfg::BAR_BYTES, "barrier area too small");
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmX);
         tma_prefetch_desc(&tmQ);
-        for (int s = 0; s < Cfg::A_STAGES; ++s) { mbar_init(&afull[s], 1); mbar_init(&aempty[s], 1); }
-        for (int s = 0; s < Cfg::Q_STAGES; ++s) { mbar_init(&qfull[s], 1); mbar_init(&qempty[s], 1); }
-        for (int b = 0; b < 2; ++b) { mbar_init(&tfull_bar[b], 1); mbar_init(&tempty_bar[b], 8); }
+        for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
         fence_barrier_init();
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)Cfg::TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
     }
     // s_thr[j] = thr_j / 2:  a = |x|^2 - 2 x.q < thr_j   <=>   x.q + thr_j/2 > |x|^2/2
     if (!DUMP) for (int j = threadIdx.x; j < NQ; j += TC_THREADS) s_thr[j] = 0.5f * thr_g[j];
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
-        // ===================== corpus producer (HBM stream, read once) =====================
-        int stage = 0; uint32_t phase = 0;
-        for (int64_t lt = blockIdx.x; lt < n_ltiles; lt += gridDim.x) {
-            const int row0 = (int)(lt * tile_stride * TC_TILE_M);
-            for (int kb = 0; kb < kblocks; ++kb) {
-                mbar_wait(&aempty[stage], phase ^ 1);
-                if (lane == 0) {
-                    mbar_expect_tx(&afull[stage], TC_A_BYTES);
-                    tma_load_2d(smem_a + (size_t)stage * TC_A_BYTES, &tmX, &afull[stage], kb * TC_KBLOCK, row0, TMA_EVICT_FIRST);
-                }
-                __syncwarp();
-                if (++stage == Cfg::A_STAGES) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else if (warp == 2) {
-        // ===================== query producer (L2-resident, re-read per tile) =====================
-        int stage = 0; uint32_t phase = 0;
-        for (int64_t lt = blockIdx.x; lt < n_ltiles; lt += gridDim.x) {
-            for (int kb = 0; kb < kblocks; ++kb) {
-                mbar_wait(&qempty[stage], phase ^ 1);
-                if (lane == 0) {
-                    mbar_expect_tx(&qfull[stage], Cfg::Q_BYTES);
-                    tma_load_2d(smem_q + (size_t)stage * Cfg::Q_BYTES, &tmQ, &qfull[stage], kb * TC_KBLOCK, 0, TMA_EVICT_LAST);
-                }
-                __syncwarp();
-                if (++stage == Cfg::Q_STAGES) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        constexpr uint32_t idesc = umma_idesc_tf32(TC_TILE_M, NQ);
-        int sa = 0, sq = 0; uint32_t pa = 0, pq = 0; int acc = 0; uint32_t acc_phase = 0;
-        for (int64_t lt = blockIdx.x; lt < n_ltiles; lt += gridDim.x) {
-            mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-            tc_fence_after();
-            const uint32_t d_tmem = tmem_base + (uint32_t)(acc * NQ);
-            for (int kb = 0; kb < kblocks; ++kb) {
-                mbar_wait(&qfull[sq], pq);
-                mbar_wait(&afull[sa], pa);
-                tc_fence_after();
-                if (lane == 0) {
-                    const uint32_t a_base = smem_u32(smem_a + (size_t)sa * TC_A_BYTES);
-                    const uint32_t b_base = smem_u32(smem_q + (size_t)sq * Cfg::Q_BYTES);
-#pragma unroll
-                    for (int k = 0; k < TC_KBLOCK / 8; ++k) {   // UMMA K = 8 for tf32 (32 bytes)
-                        umma_tf32(d_tmem, umma_desc_sw128(a_base + k * 32), umma_desc_sw128(b_base + k * 32), idesc,
-                                  (uint32_t)((kb | k) != 0));
+    if (warp < 4) {
+        // ===================== producer: corpus rows (HBM stream, read once) + query rows (L2-resident) =====================
+        regs_dealloc<40>();
+        if (threadIdx.x == 0) {
+            int stage = 0; uint32_t phase = 0;
+            for (int64_t lt = blockIdx.x; lt < n_ltiles; lt += gridDim.x) {
+                const int row0 = (int)(lt * tile_stride * TC_TILE_M);
+                for (int kb = 0; kb < kblocks; ++kb) {
+                    mbar_wait(&empty_bar[stage], phase ^ 1);
+                    unsigned char* sa = smem + (size_t)stage * Cfg::STAGE_BYTES;
+                    mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+                    if (MODE == TC_CVT) {
+                        tma_load_2d(sa, &tmX, &full_bar[stage], (2 * kb) * TC_KBLOCK, row0, TMA_EVICT_FIRST);
+                        tma_load_2d(sa + TC_A_BYTES, &tmX, &full_bar[stage], (2 * kb + 1) * TC_KBLOCK, row0, TMA_EVICT_FIRST);
+                    } else {
+                        tma_load_2d(sa, &tmX, &full_bar[stage], kb * Cfg::ELEMS, row0, TMA_EVICT_FIRST);
                     }
-                    umma_commit(&aempty[sa]);                // slots are free once these MMAs retire
-                    umma_commit(&qempty[sq]);
-                    if (kb == kblocks - 1) umma_commit(&tfull_bar[acc]);
+                    tma_load_2d(sa + Cfg::A_BYTES, &tmQ, &full_bar[stage], kb * Cfg::ELEMS, 0, TMA_EVICT_LAST);
+                    if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
                 }
-                __syncwarp();
-                if (++sa == Cfg::A_STAGES) { sa = 0; pa ^= 1; }
-                if (++sq == Cfg::Q_STAGES) { sq = 0; pq ^= 1; }
             }
-            acc ^= 1;
-            if (acc == 0) acc_phase ^= 1;
         }
     } else {
-        // ===================== epilogue: 8 warps, two per TMEM lane group, half of the columns each =====
-        // (the epilogue paces the kernel when it is slower than the 96 MMAs of a tile, so it is kept to
-        //  ~2 instructions per (row, query) pair: one add and one 3-input max; hits are ~1 in 20000)
-        const int lg = warp & 3;                         // TMEM lane group this warp may access
-        const int col_half = (warp - 3) >> 2;            // 0: columns [0, NQ/2), 1: [NQ/2, NQ)
-        const int row_in_tile = lg * 32 + lane;
-        int acc = 0; uint32_t acc_phase = 0;
+        // ===================== consumers: warpgroup wg owns tile rows [64 wg, 64 wg + 64) =====================
+        regs_alloc<232>();
+        const int wg = (warp >> 2) - 1, w = warp & 3;
+        const int g = lane >> 2, q = lane & 3;
+        const int r_lo = 64 * wg + 16 * w + g;                 // this thread's accumulator rows: r_lo and r_lo + 8
+        float acc[R];
+        int stage = 0; uint32_t phase = 0;
         for (int64_t lt = blockIdx.x; lt < n_ltiles; lt += gridDim.x) {
-            const int64_t row = lt * tile_stride * TC_TILE_M + row_in_tile;
-            float xn = CUDART_INF_F;
-            if (row < n_rows && (alive == nullptr || bit_test(alive, (uint32_t)row))) xn = xnorm[row];
-            mbar_wait(&tfull_bar[acc], acc_phase);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)(acc * NQ);
-            const float half_xn = 0.5f * xn;
-#pragma unroll 1
-            for (int c0 = col_half * (NQ / 2); c0 < (col_half + 1) * (NQ / 2); c0 += 32) {
-                uint32_t v[32];
-                tmem_ld_x32(taddr + c0, v);
-                tmem_wait_ld();
-                if (DUMP) {
-                    if (dump_min) {
-                        // threshold sampling: per query only the MINIMUM over this warp's 32 rows is kept (one REDUX per
-                        // column) -- the few smallest values of the sample, which is all the threshold needs, survive
-                        // (two of them share a 32-row group with probability ~m^2 / (2 groups)); 40x less dump traffic
-                        uint32_t mine = 0xFFFFFFFFu;
+            for (int kb = 0; kb < kblocks; ++kb) {
+                mbar_wait(&full_bar[stage], phase);
+                unsigned char* sa = smem + (size_t)stage * Cfg::STAGE_BYTES;
+                const uint64_t bdesc = wgmma_desc_sw128(smem_u32(sa + Cfg::A_BYTES));
+                if (MODE == TC_CVT) {
+                    uint32_t af[4][4];
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            const uint32_t mn = __reduce_min_sync(0xffffffffu, f32_ordered_bits(fmaf(-2.f, __uint_as_float(v[j]), xn)));
-                            if (lane == j) mine = mn;
+                    for (int s = 0; s < 4; ++s) cvt_a_fragment(sa, r_lo, g, q, s, af[s]);
+                    wgmma_fence();
+#pragma unroll
+                    for (int s = 0; s < 4; ++s) wgmma_bf16_rs<NQ>(acc, af[s], bdesc + 2 * s, (uint32_t)((kb | s) != 0));
+                    wgmma_commit();
+                    wgmma_wait<0>();                           // the A registers are reused by the next stage
+                } else {
+                    const uint64_t adesc = wgmma_desc_sw128(smem_u32(sa + wg * 64 * 128));
+                    wgmma_fence();
+#pragma unroll
+                    for (int s = 0; s < 4; ++s) {              // K steps of 32 bytes: 8 tf32 or 16 bf16
+                        if (MODE == TC_TF32) wgmma_tf32_ss<NQ>(acc, adesc + 2 * s, bdesc + 2 * s, (uint32_t)((kb | s) != 0));
+                        else wgmma_bf16_ss<NQ>(acc, adesc + 2 * s, bdesc + 2 * s, (uint32_t)((kb | s) != 0));
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                }
+                wgmma_fence_operands<R>(acc);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[stage]);
+                if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+            }
+            // ===================== epilogue straight from the accumulator registers =====================
+            // acc[4i + 2h + c] is (row r_lo + 8h, query 8i + 2q + c)
+            const int64_t tile_row0 = lt * tile_stride * TC_TILE_M;
+            float xn[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int64_t row = tile_row0 + r_lo + 8 * h;
+                xn[h] = CUDART_INF_F;
+                if (row < n_rows && (alive == nullptr || bit_test(alive, (uint32_t)row))) xn[h] = xnorm[row];
+            }
+            if (DUMP) {
+                if (dump_min) {
+                    // threshold sampling: per query only the MINIMUM over this warp's 16 rows is kept -- the few smallest
+                    // values of the sample, which is all the threshold needs, survive
+                    const int64_t grp = lt * (TC_TILE_M / TC_DUMP_GROUP) + 4 * wg + w;
+#pragma unroll
+                    for (int i = 0; i < R / 4; ++i) {
+#pragma unroll
+                        for (int c = 0; c < 2; ++c) {
+                            float v = fminf(fmaf(-2.f, acc[4 * i + c], xn[0]), fmaf(-2.f, acc[4 * i + 2 + c], xn[1]));
+                            v = fminf(v, __shfl_xor_sync(0xffffffffu, v, 4));
+                            v = fminf(v, __shfl_xor_sync(0xffffffffu, v, 8));
+                            v = fminf(v, __shfl_xor_sync(0xffffffffu, v, 16));
+                            if (g == 0) dump[(int64_t)(8 * i + 2 * q + c) * S + grp] = v;
                         }
-                        dump[(int64_t)(c0 + lane) * S + lt * (TC_TILE_M / 32) + lg] = f32_from_ordered_bits(mine);
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            dump[(int64_t)(c0 + j) * S + lt * TC_TILE_M + row_in_tile] = fmaf(-2.f, __uint_as_float(v[j]), xn);
                     }
                 } else {
-                    float t[32];
-                    float mx = -CUDART_INF_F;
 #pragma unroll
-                    for (int j4 = 0; j4 < 32; j4 += 4) {
-                        const float4 h = *reinterpret_cast<const float4*>(s_thr + c0 + j4);   // warp-uniform: broadcast
-                        t[j4 + 0] = __uint_as_float(v[j4 + 0]) + h.x;
-                        t[j4 + 1] = __uint_as_float(v[j4 + 1]) + h.y;
-                        t[j4 + 2] = __uint_as_float(v[j4 + 2]) + h.z;
-                        t[j4 + 3] = __uint_as_float(v[j4 + 3]) + h.w;
-                        mx = fmaxf(mx, fmaxf(fmaxf(t[j4 + 0], t[j4 + 1]), fmaxf(t[j4 + 2], t[j4 + 3])));
-                    }
-                    if (mx > half_xn) {   // rare: some pair in this chunk passes  x.q + thr/2 > |x|^2/2
+                    for (int i = 0; i < R / 4; ++i)
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            if (t[j] > half_xn) {
-                                const uint32_t pos = atomicAdd(&cand_count[c0 + j], 1u);
-                                if (pos < (uint32_t)cap) cand_rows[(size_t)(c0 + j) * cap + pos] = (uint32_t)row;
+                        for (int h = 0; h < 2; ++h)
+#pragma unroll
+                            for (int c = 0; c < 2; ++c)
+                                dump[(int64_t)(8 * i + 2 * q + c) * S + lt * TC_TILE_M + r_lo + 8 * h] =
+                                    fmaf(-2.f, acc[4 * i + 2 * h + c], xn[h]);
+                }
+            } else {
+                // ~2 instructions per (row, query) pair on the common path: one add and one max; hits are ~1 in 20000
+                const float half0 = 0.5f * xn[0], half1 = 0.5f * xn[1];
+                float mx0 = -CUDART_INF_F, mx1 = -CUDART_INF_F;
+#pragma unroll
+                for (int i = 0; i < R / 4; ++i) {
+                    const float2 t = *reinterpret_cast<const float2*>(s_thr + 8 * i + 2 * q);
+                    acc[4 * i + 0] += t.x; acc[4 * i + 1] += t.y; acc[4 * i + 2] += t.x; acc[4 * i + 3] += t.y;
+                    mx0 = fmaxf(mx0, fmaxf(acc[4 * i + 0], acc[4 * i + 1]));
+                    mx1 = fmaxf(mx1, fmaxf(acc[4 * i + 2], acc[4 * i + 3]));
+                }
+                if (mx0 > half0 || mx1 > half1) {   // rare: some pair passes  x.q + thr/2 > |x|^2/2
+#pragma unroll
+                    for (int i = 0; i < R / 4; ++i) {
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                            for (int c = 0; c < 2; ++c) {
+                                if (acc[4 * i + 2 * h + c] > (h ? half1 : half0)) {
+                                    const int j = 8 * i + 2 * q + c;
+                                    const uint32_t pos = atomicAdd(&cand_count[j], 1u);
+                                    if (pos < (uint32_t)cap) cand_rows[(size_t)j * cap + pos] = (uint32_t)(tile_row0 + r_lo + 8 * h);
+                                }
                             }
                         }
                     }
                 }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-            acc ^= 1;
-            if (acc == 0) acc_phase ^= 1;
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)Cfg::TMEM_COLS) : "memory");
     }
 }
 
-// ---------------------------------------------------------- 2-CTA main pass (cta_group::2)
-// A CTA pair (one cluster of 2, one CTA per SM of a TPC) computes D[256 rows x NQ] per pair-tile with
-// tcgen05.mma.cta_group::2 (M = 256): each CTA stages ITS 128 corpus rows and HALF of the query slab,
-// the pair's tensor cores share the operands.  Per 128-cycle MMA each SM now reads 8 KB of operands
-// (A 4 KB + B half 4 KB) and TMA writes 32 KB per 512 cycles: 64 + 64 B/clk against the 128 B/clk
-// shared-memory port, versus 96 + 96 for the 1-CTA kernel (which caps its tensor pipe at 67%).
-// The halved query slab also doubles the query ring depth (6 stages) and halves L2->SM traffic.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N)
-{
-    return (1u << 4) /* D f32 */ | (1u << 7) /* A bf16 */ | (1u << 10) /* B bf16 */ | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-template <bool BF16>
-__device__ __forceinline__ void umma_2sm(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    if (BF16) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-            ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-    } else {
-        umma_tf32_2sm(d_tmem, adesc, bdesc, idesc, accumulate);
-    }
-}
 // fp32 -> bf16 (round to nearest even) shadow rows; n4 = number of float4 groups
 __global__ void f32_to_bf16_kernel(const float4* __restrict__ in, uint2* __restrict__ out, int64_t n4)
 {
@@ -276,427 +252,10 @@ void launch_f32_to_bf16(const float* in, uint16_t* out, int64_t n_elems, cudaStr
     if (n_elems == 0) return;
     const int64_t n4 = n_elems / 4;
     int64_t blocks = (n4 + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     f32_to_bf16_kernel<<<(unsigned)blocks, 256, 0, st>>>(reinterpret_cast<const float4*>(in), reinterpret_cast<uint2*>(out), n4);
     KRAG_CUDA(cudaGetLastError());
     count_launch();
-}
-
-// One ring; a stage holds TC2_KB_PER_STAGE k-blocks of this CTA's corpus rows and of its half of the
-// query rows, so the single MMA-issuing thread pays one barrier wait and one commit per 8 MMAs (it was
-// the bottleneck at 2 waits + 2 commits per 4 MMAs: ~770 cycles per k-block against 512 cycles of MMA work).
-constexpr int TC2_KB_PER_STAGE = 2;
-template <int NQ> struct Tc2Cfg {
-    static constexpr int QH_BYTES = (NQ / 2) * TC_KBLOCK * 4;          // this CTA's half of one query k-block
-    static constexpr int STAGE_BYTES = TC2_KB_PER_STAGE * (TC_A_BYTES + QH_BYTES);
-    static constexpr int STAGES = (200 * 1024) / STAGE_BYTES;          // 3 at NQ = 256, 4 at NQ = 128, 5 at NQ = 64
-    static constexpr int TMEM_COLS = (2 * NQ < 32) ? 32 : 2 * NQ;
-    static constexpr int BAR_BYTES = 256;
-    static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + 1024 + BAR_BYTES + NQ * 4;
-};
-
-__device__ __forceinline__ uint64_t desc_with_lo(uint64_t base_desc, uint32_t lo)
-{
-    return (base_desc & 0xFFFFFFFF00000000ull) | (uint64_t)lo;
-}
-
-// BF16 = true: the operands are a bf16 SHADOW of the corpus (and of the queries): k-blocks are still 128 bytes per row
-// (64 elements), the MMA is kind::f16 with K = 16 -- half the HBM bytes and half the tensor time of the TF32 pass.
-// Only the pruning changes; the rescoring that produces the returned distances always reads the fp32 corpus.
-template <int NQ, bool BF16>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-dense_tc2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmQh, int64_t n_rows,
-                 int kblocks, int64_t n_ptiles, const float* __restrict__ xnorm, const uint32_t* __restrict__ alive,
-                 const float* __restrict__ thr_g, uint32_t* __restrict__ cand_count, uint32_t* __restrict__ cand_rows, int cap)
-{
-    using Cfg = Tc2Cfg<NQ>;
-    extern __shared__ unsigned char tc_smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~(uintptr_t)1023);
-    unsigned char* tail = smem + (size_t)Cfg::STAGES * Cfg::STAGE_BYTES;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);             // used in the leader only (2 arrivals + tx of both CTAs)
-    uint64_t* empty_bar = full_bar + Cfg::STAGES;                        // per CTA
-    uint64_t* tfull_bar = empty_bar + Cfg::STAGES;                       // per CTA   [2]
-    uint64_t* tempty_bar = tfull_bar + 2;                                // leader only [2], 16 arrivals (8 warps x 2 CTAs)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-    float* s_thr = reinterpret_cast<float*>(tail + Cfg::BAR_BYTES);
-    static_assert((2 * Cfg::STAGES + 4) * 8 + 8 <= Cfg::BAR_BYTES, "barrier area too small");
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();          // 0 = pair leader
-    const int pair = blockIdx.x >> 1, n_pairs = gridDim.x >> 1;
-    const int n_stages_per_tile = (kblocks + TC2_KB_PER_STAGE - 1) / TC2_KB_PER_STAGE;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmX);
-        tma_prefetch_desc(&tmQh);
-        for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full_bar[s], 2); mbar_init(&empty_bar[s], 1); }
-        for (int b = 0; b < 2; ++b) { mbar_init(&tfull_bar[b], 1); mbar_init(&tempty_bar[b], 16); }
-        fence_barrier_init();
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)Cfg::TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    for (int j = threadIdx.x; j < NQ; j += TC_THREADS) s_thr[j] = 0.5f * thr_g[j];
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();                                // both CTAs' barriers are initialised before any remote signal
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        // ===================== producer: this CTA's 128 corpus rows + its half of the query rows =====================
-        int stage = 0; uint32_t phase = 0;
-        for (int64_t pt = pair; pt < n_ptiles; pt += n_pairs) {
-            const int row0 = (int)(pt * (2 * TC_TILE_M) + rank * TC_TILE_M);
-            for (int sk = 0; sk < n_stages_per_tile; ++sk) {
-                const int nkb = min(TC2_KB_PER_STAGE, kblocks - sk * TC2_KB_PER_STAGE);
-                mbar_wait(&empty_bar[stage], phase ^ 1);
-                if (lane == 0) {
-                    unsigned char* sa = smem + (size_t)stage * Cfg::STAGE_BYTES;
-                    unsigned char* sq = sa + TC2_KB_PER_STAGE * TC_A_BYTES;
-                    if (rank == 0) mbar_expect_tx(&full_bar[stage], 2 * nkb * (TC_A_BYTES + Cfg::QH_BYTES));   // both CTAs' bytes
-                    else mbar_arrive_remote(&full_bar[stage], 0);
-                    for (int u = 0; u < nkb; ++u) {
-                        const int kb = sk * TC2_KB_PER_STAGE + u;
-                        constexpr int KBE = BF16 ? 2 * TC_KBLOCK : TC_KBLOCK;   // elements per 128-byte k-block
-                        tma_load_2d_2sm(sa + (size_t)u * TC_A_BYTES, &tmX, &full_bar[stage], kb * KBE, row0, TMA_EVICT_FIRST);
-                        tma_load_2d_2sm(sq + (size_t)u * Cfg::QH_BYTES, &tmQh, &full_bar[stage], kb * KBE, (int)rank * (NQ / 2),
-                                        TMA_EVICT_LAST);
-                    }
-                }
-                __syncwarp();
-                if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else if (warp == 1) {
-        if (rank == 0) {
-            // ===================== MMA issuer (pair leader only) =====================
-            constexpr uint32_t idesc = BF16 ? umma_idesc_bf16(2 * TC_TILE_M, NQ) : umma_idesc_tf32(2 * TC_TILE_M, NQ);
-            const uint64_t desc0 = umma_desc_sw128(smem_u32(smem));      // descriptor of ring byte 0; only the low word moves
-            const uint32_t lo0 = (uint32_t)desc0;
-            int stage = 0; uint32_t phase = 0; int acc = 0; uint32_t acc_phase = 0;
-            for (int64_t pt = pair; pt < n_ptiles; pt += n_pairs) {
-                mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * NQ);
-                for (int sk = 0; sk < n_stages_per_tile; ++sk) {
-                    const int nkb = min(TC2_KB_PER_STAGE, kblocks - sk * TC2_KB_PER_STAGE);
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    if (lane == 0) {
-                        const uint32_t a_lo = lo0 + (uint32_t)((stage * Cfg::STAGE_BYTES) >> 4);
-                        const uint32_t q_lo = a_lo + (uint32_t)((TC2_KB_PER_STAGE * TC_A_BYTES) >> 4);
-#pragma unroll
-                        for (int u = 0; u < TC2_KB_PER_STAGE; ++u) {
-                            if (u < nkb) {
-#pragma unroll
-                                for (int k = 0; k < TC_KBLOCK / 8; ++k)   // UMMA K = 8 (32 bytes = 2 descriptor units)
-                                    umma_2sm<BF16>(d_tmem, desc_with_lo(desc0, a_lo + (uint32_t)((u * TC_A_BYTES) >> 4) + 2 * k),
-                                                  desc_with_lo(desc0, q_lo + (uint32_t)((u * Cfg::QH_BYTES) >> 4) + 2 * k), idesc,
-                                                  (uint32_t)((sk | u | k) != 0));
-                            }
-                        }
-                        umma_commit_2sm(&empty_bar[stage]);            // frees the stage in both CTAs
-                        if (sk == n_stages_per_tile - 1) umma_commit_2sm(&tfull_bar[acc]);
-                    }
-                    __syncwarp();
-                    if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-                }
-                acc ^= 1;
-                if (acc == 0) acc_phase ^= 1;
-            }
-        }
-    } else if (warp >= 3) {
-        // ===================== epilogue: 8 warps per CTA over this CTA's 128 TMEM lanes =====================
-        const int lg = warp & 3;
-        const int col_half = (warp - 3) >> 2;
-        const int row_in_tile = lg * 32 + lane;
-        int acc = 0; uint32_t acc_phase = 0;
-        for (int64_t pt = pair; pt < n_ptiles; pt += n_pairs) {
-            const int64_t row = pt * (2 * TC_TILE_M) + rank * TC_TILE_M + row_in_tile;
-            float xn = CUDART_INF_F;
-            if (row < n_rows && (alive == nullptr || bit_test(alive, (uint32_t)row))) xn = xnorm[row];
-            mbar_wait(&tfull_bar[acc], acc_phase);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)(acc * NQ);
-            const float half_xn = 0.5f * xn;
-#pragma unroll 1
-            for (int c0 = col_half * (NQ / 2); c0 < (col_half + 1) * (NQ / 2); c0 += 32) {
-                uint32_t v[32];
-                tmem_ld_x32(taddr + c0, v);
-                tmem_wait_ld();
-                float t[32];
-                float mx = -CUDART_INF_F;
-#pragma unroll
-                for (int j4 = 0; j4 < 32; j4 += 4) {
-                    const float4 h = *reinterpret_cast<const float4*>(s_thr + c0 + j4);
-                    t[j4 + 0] = __uint_as_float(v[j4 + 0]) + h.x;
-                    t[j4 + 1] = __uint_as_float(v[j4 + 1]) + h.y;
-                    t[j4 + 2] = __uint_as_float(v[j4 + 2]) + h.z;
-                    t[j4 + 3] = __uint_as_float(v[j4 + 3]) + h.w;
-                    mx = fmaxf(mx, fmaxf(fmaxf(t[j4 + 0], t[j4 + 1]), fmaxf(t[j4 + 2], t[j4 + 3])));
-                }
-                if (mx > half_xn) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        if (t[j] > half_xn) {
-                            const uint32_t pos = atomicAdd(&cand_count[c0 + j], 1u);
-                            if (pos < (uint32_t)cap) cand_rows[(size_t)(c0 + j) * cap + pos] = (uint32_t)row;
-                        }
-                    }
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                if (rank == 0) mbar_arrive(&tempty_bar[acc]);
-                else mbar_arrive_remote(&tempty_bar[acc], 0);
-            }
-            acc ^= 1;
-            if (acc == 0) acc_phase ^= 1;
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();                                // the peer may still be reading operands from this CTA's smem
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)Cfg::TMEM_COLS) : "memory");
-    }
-}
-
-// ------------------------------------------------- K2, default: fp32 rows -> bf16 IN SHARED MEMORY -> kind::f16
-// The TF32 pass above runs at 97-99% tensor-pipe activity with the SM clock held at 1.2-1.3 GHz by the power cap:
-// it is bound by tensor energy, not by HBM.  This variant keeps the corpus fp32 in HBM (no shadow copy, same
-// 4 bytes/element of traffic) but halves the tensor work: TMA lands the fp32 k-blocks in a staging ring, four
-// converter warps round them to bf16 (cvt.rn.bf16x2, the same rounding as the shadow mode) straight into the
-// 128B-swizzled operand ring, and the pair's MMAs are kind::f16 (K = 16).  The pass becomes HBM-bound.
-// Pruning only, as before: candidates are re-scored in exact fp32 and certified with the bf16 error bound.
-//   warp 0: corpus TMA (fp32 staging ring, per CTA)      warp 1: MMA issuer (pair leader)
-//   warp 2: query TMA (bf16 queries, operand ring)       warps 3-10: epilogue      warps 11-13: converters, warp w owns
-//   operand stage w: the three conversions in flight hide each other's shared-memory and barrier latency
-constexpr int TCV_THREADS = 448;
-constexpr int TCV_A_STAGES = 8;            // fp32 staging k-blocks (16 KB each): 128 KB of corpus in flight per SM covers the HBM latency
-constexpr int TCV_B_STAGES = 3;            // bf16 operand k-blocks: 16 KB corpus + this CTA's half of the queries
-template <int NQ> struct TcvCfg {
-    static constexpr int QH_BYTES = (NQ / 2) * 128;                    // 64 bf16 per row
-    static constexpr int B_STAGE = TC_A_BYTES + QH_BYTES;
-    static constexpr int TMEM_COLS = (2 * NQ < 32) ? 32 : 2 * NQ;
-    static constexpr int BAR_BYTES = 256;
-    static constexpr size_t SMEM = (size_t)TCV_A_STAGES * TC_A_BYTES + (size_t)TCV_B_STAGES * B_STAGE + 1024 + BAR_BYTES + NQ * 4;
-};
-
-template <int NQ>
-__global__ void __launch_bounds__(TCV_THREADS, 1)
-dense_tc2cvt_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmQh, int64_t n_rows,
-                    int kblocks /*fp32 k-blocks, even*/, int64_t n_ptiles, const float* __restrict__ xnorm,
-                    const uint32_t* __restrict__ alive, const float* __restrict__ thr_g, uint32_t* __restrict__ cand_count,
-                    uint32_t* __restrict__ cand_rows, int cap)
-{
-    using Cfg = TcvCfg<NQ>;
-    extern __shared__ unsigned char tc_smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~(uintptr_t)1023);
-    unsigned char* ring_a = smem;                                            // fp32 staging
-    unsigned char* ring_b = smem + (size_t)TCV_A_STAGES * TC_A_BYTES;        // bf16 operands
-    unsigned char* tail = ring_b + (size_t)TCV_B_STAGES * Cfg::B_STAGE;
-    uint64_t* a_full = reinterpret_cast<uint64_t*>(tail);                    // per CTA
-    uint64_t* a_empty = a_full + TCV_A_STAGES;                               // per CTA, the converter warp that read the slot
-    uint64_t* b_full = a_empty + TCV_A_STAGES;                               // leader only: 2 query producers + 2 converter warps + tx
-    uint64_t* b_empty = b_full + TCV_B_STAGES;                               // per CTA (multicast commit)
-    uint64_t* tfull_bar = b_empty + TCV_B_STAGES;                            // per CTA [2]
-    uint64_t* tempty_bar = tfull_bar + 2;                                    // leader only [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-    float* s_thr = reinterpret_cast<float*>(tail + Cfg::BAR_BYTES);
-    static_assert((2 * TCV_A_STAGES + 2 * TCV_B_STAGES + 4) * 8 + 8 <= Cfg::BAR_BYTES, "barrier area too small");
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const int pair = blockIdx.x >> 1, n_pairs = gridDim.x >> 1;
-    const int kb2 = kblocks >> 1;                                            // bf16 k-blocks per tile
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmX);
-        tma_prefetch_desc(&tmQh);
-        for (int s = 0; s < TCV_A_STAGES; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 1); }
-        for (int s = 0; s < TCV_B_STAGES; ++s) { mbar_init(&b_full[s], 4); mbar_init(&b_empty[s], 1); }
-        for (int b = 0; b < 2; ++b) { mbar_init(&tfull_bar[b], 1); mbar_init(&tempty_bar[b], 16); }
-        fence_barrier_init();
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)Cfg::TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    for (int j = threadIdx.x; j < NQ; j += TCV_THREADS) s_thr[j] = 0.5f * thr_g[j];
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        // ===================== corpus producer: fp32 k-blocks of this CTA's 128 rows =====================
-        if (lane == 0) {
-            int stage = 0; uint32_t phase = 0;
-            for (int64_t pt = pair; pt < n_ptiles; pt += n_pairs) {
-                const int row0 = (int)(pt * (2 * TC_TILE_M) + rank * TC_TILE_M);
-                for (int kb = 0; kb < kblocks; ++kb) {
-                    mbar_wait(&a_empty[stage], phase ^ 1);
-                    mbar_expect_tx(&a_full[stage], TC_A_BYTES);
-                    tma_load_2d(ring_a + (size_t)stage * TC_A_BYTES, &tmX, &a_full[stage], kb * TC_KBLOCK, row0, TMA_EVICT_FIRST);
-                    if (++stage == TCV_A_STAGES) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else if (warp == 2) {
-        // ===================== query producer: this CTA's half of the bf16 query rows =====================
-        if (lane == 0) {
-            int stage = 0; uint32_t phase = 0;
-            for (int64_t pt = pair; pt < n_ptiles; pt += n_pairs) {
-                for (int jb = 0; jb < kb2; ++jb) {
-                    mbar_wait(&b_empty[stage], phase ^ 1);
-                    if (rank == 0) mbar_expect_tx(&b_full[stage], 2 * Cfg::QH_BYTES);
-                    else mbar_arrive_remote(&b_full[stage], 0);
-                    tma_load_2d_2sm(ring_b + (size_t)stage * Cfg::B_STAGE + TC_A_BYTES, &tmQh, &b_full[stage], jb * 64, (int)rank * (NQ / 2),
-                                    TMA_EVICT_LAST);
-                    if (++stage == TCV_B_STAGES) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (rank == 0) {
-            // ===================== MMA issuer (pair leader) =====================
-            constexpr uint32_t idesc = umma_idesc_bf16(2 * TC_TILE_M, NQ);
-            const uint64_t desc0 = umma_desc_sw128(smem_u32(ring_b));
-            const uint32_t lo0 = (uint32_t)desc0;
-            int stage = 0; uint32_t phase = 0; int acc = 0; uint32_t acc_phase = 0;
-            for (int64_t pt = pair; pt < n_ptiles; pt += n_pairs) {
-                mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * NQ);
-                for (int jb = 0; jb < kb2; ++jb) {
-                    mbar_wait(&b_full[stage], phase);
-                    tc_fence_after();
-                    if (lane == 0) {
-                        const uint32_t a_lo = lo0 + (uint32_t)((stage * Cfg::B_STAGE) >> 4);
-                        const uint32_t q_lo = a_lo + (uint32_t)(TC_A_BYTES >> 4);
-#pragma unroll
-                        for (int k = 0; k < 4; ++k)      // UMMA K = 16 bf16 (32 bytes = 2 descriptor units)
-                            umma_2sm<true>(d_tmem, desc_with_lo(desc0, a_lo + 2 * k), desc_with_lo(desc0, q_lo + 2 * k), idesc,
-                                           (uint32_t)((jb | k) != 0));
-                        umma_commit_2sm(&b_empty[stage]);
-                        if (jb == kb2 - 1) umma_commit_2sm(&tfull_bar[acc]);
-                    }
-                    __syncwarp();
-                    if (++stage == TCV_B_STAGES) { stage = 0; phase ^= 1; }
-                }
-                acc ^= 1;
-                if (acc == 0) acc_phase ^= 1;
-            }
-        }
-    } else if (warp >= 11) {
-        // ===================== converters: two fp32 staging k-blocks -> one bf16 operand k-block =====================
-        static_assert(TCV_B_STAGES == 3 && TCV_A_STAGES == 8, "converter warp w owns operand stage w; staging ring of 8");
-        const int w = warp - 11;                                // operand stage owned by this warp
-        const int c = lane & 7;                                 // 16-byte chunk of the fp32 row
-        // rows handled by a lane: base {0,4,1,5}[lane >> 3] + 2 (it & 1) + 8 (it >> 1).  The two rows of a half-warp differ in
-        // bit 2, so their swizzled 64-byte bf16 halves fall into opposite bank halves (conflict-free 64-bit stores)
-        const int rr = (((lane >> 3) & 1) << 2) | (lane >> 4);
-        const int64_t my_tiles = (n_ptiles - pair + n_pairs - 1) / n_pairs;
-        const int64_t total = my_tiles * kb2;                   // bf16 k-blocks this CTA converts
-        unsigned char* dst = ring_b + (size_t)w * Cfg::B_STAGE;
-        uint32_t pbe = 1;                                       // parity to wait for on b_empty[w]
-        for (int64_t g = w; g < total; g += TCV_B_STAGES) {
-            mbar_wait(&b_empty[w], pbe);                        // the MMAs that read this operand stage have retired
-            pbe ^= 1;
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int64_t i = 2 * g + h;                    // fp32 k-block counter of this CTA
-                const int sa = (int)(i & 7);
-                mbar_wait(&a_full[sa], (uint32_t)((i >> 3) & 1));
-                const unsigned char* src = ring_a + (size_t)sa * TC_A_BYTES;
-                const int cd = (h << 2) | (c >> 1);             // 16-byte chunk of the bf16 row
-#pragma unroll
-                for (int b8 = 0; b8 < 4; ++b8) {
-                    float4 v[8];
-#pragma unroll
-                    for (int it = 0; it < 8; ++it) {
-                        const int r = rr + 2 * (it & 1) + 8 * (b8 * 4 + (it >> 1));
-                        v[it] = *reinterpret_cast<const float4*>(src + r * 128 + ((c ^ (r & 7)) << 4));
-                    }
-#pragma unroll
-                    for (int it = 0; it < 8; ++it) {
-                        const int r = rr + 2 * (it & 1) + 8 * (b8 * 4 + (it >> 1));
-                        const __nv_bfloat162 lo = __floats2bfloat162_rn(v[it].x, v[it].y), hi = __floats2bfloat162_rn(v[it].z, v[it].w);
-                        uint2 o;
-                        o.x = *reinterpret_cast<const uint32_t*>(&lo); o.y = *reinterpret_cast<const uint32_t*>(&hi);
-                        *reinterpret_cast<uint2*>(dst + r * 128 + ((cd ^ (r & 7)) << 4) + ((c & 1) << 3)) = o;
-                    }
-                }
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&a_empty[sa]);        // staging slot read: TMA may refill it
-            }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the MMA's async proxy
-            __syncwarp();
-            if (lane == 0) { if (rank == 0) mbar_arrive(&b_full[w]); else mbar_arrive_remote(&b_full[w], 0); }
-        }
-    } else {
-        // ===================== epilogue (warps 3-10): as dense_tc2_kernel =====================
-        const int lg = warp & 3;
-        const int col_half = (warp - 3) >> 2;
-        const int row_in_tile = lg * 32 + lane;
-        int acc = 0; uint32_t acc_phase = 0;
-        for (int64_t pt = pair; pt < n_ptiles; pt += n_pairs) {
-            const int64_t row = pt * (2 * TC_TILE_M) + rank * TC_TILE_M + row_in_tile;
-            float xn = CUDART_INF_F;
-            if (row < n_rows && (alive == nullptr || bit_test(alive, (uint32_t)row))) xn = xnorm[row];
-            mbar_wait(&tfull_bar[acc], acc_phase);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)(acc * NQ);
-            const float half_xn = 0.5f * xn;
-#pragma unroll 1
-            for (int c0 = col_half * (NQ / 2); c0 < (col_half + 1) * (NQ / 2); c0 += 32) {
-                uint32_t v[32];
-                tmem_ld_x32(taddr + c0, v);
-                tmem_wait_ld();
-                float t[32];
-                float mx = -CUDART_INF_F;
-#pragma unroll
-                for (int j4 = 0; j4 < 32; j4 += 4) {
-                    const float4 h = *reinterpret_cast<const float4*>(s_thr + c0 + j4);
-                    t[j4 + 0] = __uint_as_float(v[j4 + 0]) + h.x;
-                    t[j4 + 1] = __uint_as_float(v[j4 + 1]) + h.y;
-                    t[j4 + 2] = __uint_as_float(v[j4 + 2]) + h.z;
-                    t[j4 + 3] = __uint_as_float(v[j4 + 3]) + h.w;
-                    mx = fmaxf(mx, fmaxf(fmaxf(t[j4 + 0], t[j4 + 1]), fmaxf(t[j4 + 2], t[j4 + 3])));
-                }
-                if (mx > half_xn) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        if (t[j] > half_xn) {
-                            const uint32_t pos = atomicAdd(&cand_count[c0 + j], 1u);
-                            if (pos < (uint32_t)cap) cand_rows[(size_t)(c0 + j) * cap + pos] = (uint32_t)row;
-                        }
-                    }
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                if (rank == 0) mbar_arrive(&tempty_bar[acc]);
-                else mbar_arrive_remote(&tempty_bar[acc], 0);
-            }
-            acc ^= 1;
-            if (acc == 0) acc_phase ^= 1;
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)Cfg::TMEM_COLS) : "memory");
-    }
 }
 
 // ------------------------------------------------------------- row norms (index time)
@@ -869,7 +428,7 @@ constexpr int64_t TC_MIN_ROWS = 262144;   // below this the exact scan is cheape
 
 bool dense_tc_supported(const DeviceInfo& di, int dpad)
 {
-    return di.cc_major == 10 && dpad % TC_KBLOCK == 0 && di.smem_optin >= TcCfg<256>::SMEM && get_encode() != nullptr;
+    return di.cc_major == 9 && dpad % TC_KBLOCK == 0 && di.smem_optin >= TcCfg<256, TC_CVT>::SMEM && get_encode() != nullptr;
 }
 
 static int tc_target(int P, bool bf16 = false)
@@ -908,11 +467,21 @@ size_t dense_tc_workspace_bytes(const DeviceInfo&, int64_t n_rows, int P)
 }
 bool dense_tc_wants(int64_t n_rows, int batch) { return n_rows >= TC_MIN_ROWS && batch >= 16; }
 
-static bool tc_use_2cta()
+// one launch of the prune kernel (sample pass: MODE = TC_TF32, DUMP) over n_ltiles tiles of 128 rows, tile_stride apart
+template <int NQ, int MODE, bool DUMP>
+static void tc_launch(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensorMap& tmQ, int64_t n_rows, int dpad,
+                      int64_t n_ltiles, int tile_stride, const float* xnorm, const uint32_t* alive, const float* thr,
+                      uint32_t* cand_count, uint32_t* cand_rows, int cap, float* dump, int64_t S, int dump_min, cudaStream_t st)
 {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("KRAG_TC_2CTA"); v = (e == nullptr || e[0] != '0') ? 1 : 0; }
-    return v == 1;
+    using Cfg = TcCfg<NQ, MODE>;
+    static bool attr_set = false;
+    if (!attr_set) {
+        KRAG_CUDA(cudaFuncSetAttribute(dense_tc_kernel<NQ, MODE, DUMP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM));
+        attr_set = true;
+    }
+    const int grid = (int)(n_ltiles < di.sm_count ? n_ltiles : di.sm_count);
+    dense_tc_kernel<NQ, MODE, DUMP><<<grid, TC_THREADS, Cfg::SMEM, st>>>(tmX, tmQ, n_rows, dpad / Cfg::ELEMS, n_ltiles, tile_stride,
+                                                                         xnorm, alive, thr, cand_count, cand_rows, cap, dump, S, dump_min);
 }
 
 template <int NQ>
@@ -921,25 +490,15 @@ static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensor
                     int nq, int P, OrdMap ord_base, const TcWorkspace& w, int cap, int64_t S, uint64_t* keys_out,
                     const uint16_t* Xh, bool cvt, cudaStream_t st)
 {
-    using Cfg = TcCfg<NQ>;
     const bool bf16 = Xh != nullptr || cvt;      // bf16 operands in the prune pass (shadow copy, or converted on chip)
-    static bool attr_set = false;
-    if (!attr_set) {
-        KRAG_CUDA(cudaFuncSetAttribute(dense_tc_kernel<NQ, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM));
-        KRAG_CUDA(cudaFuncSetAttribute(dense_tc_kernel<NQ, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM));
-        attr_set = true;
-    }
-    const int kblocks = dpad / TC_KBLOCK;
     const int64_t n_tiles = (n_rows + TC_TILE_M - 1) / TC_TILE_M;
     const int64_t s_tiles = tc_sample_tiles(n_rows);
-    const int grid_s = (int)(s_tiles < di.sm_count ? s_tiles : di.sm_count);
-    const int grid_m = (int)(n_tiles < di.sm_count ? n_tiles : di.sm_count);
     // 1. sample pass (1/64 of the tiles), dump a = |x|^2 - 2 x.q
-    // the dump holds one value per (32-row group of a sampled tile, query): S_min per query
-    const int64_t S_min = s_tiles * (TC_TILE_M / 32);
+    // the dump holds one value per (16-row group of a sampled tile, query): S_min per query
+    const int64_t S_min = s_tiles * (TC_TILE_M / TC_DUMP_GROUP);
     (void)S;
-    dense_tc_kernel<NQ, true><<<grid_s, TC_THREADS, Cfg::SMEM, st>>>(tmX, tmQ, n_rows, kblocks, s_tiles, TC_SAMPLE_STRIDE, xnorm,
-                                                                     alive, nullptr, nullptr, nullptr, 0, w.dump, S_min, 1);
+    tc_launch<NQ, TC_TF32, true>(di, tmX, tmQ, n_rows, dpad, s_tiles, TC_SAMPLE_STRIDE, xnorm, alive, nullptr, nullptr, nullptr, 0,
+                                 w.dump, S_min, 1, st);
     KRAG_CUDA(cudaGetLastError());
     count_launch();
     // 2. threshold admitting ~C rows: the m-th smallest of the sample, m = C * sample_fraction
@@ -960,67 +519,23 @@ static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensor
     KRAG_CUDA(cudaMemsetAsync(w.cand_count, 0, 256 * 4, st));
     // 3. main pass: stream the corpus once, prune on the tensor cores
     if (bf16) launch_f32_to_bf16(q, w.q_bf16, (int64_t)nq * dpad, st);
-    dense_timer_begin(st, cvt ? 5 : (bf16 ? 4 : (tc_use_2cta() ? 3 : 2)), n_rows * (int64_t)dpad * ((bf16 && !cvt) ? 2 : 4),
-                      2 * (int64_t)NQ * n_rows * dpad);
-    if (cvt) {
-        using CfgV = TcvCfg<NQ>;
-        static bool attrv_set = false;
-        if (!attrv_set) {
-            KRAG_CUDA(cudaFuncSetAttribute(dense_tc2cvt_kernel<NQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CfgV::SMEM));
-            attrv_set = true;
-        }
-        CUtensorMap tmQh;
-        if (!make_map(&tmQh, (const void*)w.q_bf16, nq, dpad, NQ / 2, true))
-            throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled(Q half, bf16)", __FILE__, __LINE__};
-        const int64_t n_ptiles = (n_rows + 2 * TC_TILE_M - 1) / (2 * TC_TILE_M);
-        const int64_t max_pairs = di.sm_count / 2;
-        const int n_pairs = (int)(n_ptiles < max_pairs ? n_ptiles : max_pairs);
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3((unsigned)(2 * n_pairs));
-        cfg.blockDim = dim3(TCV_THREADS);
-        cfg.dynamicSmemBytes = CfgV::SMEM;
-        cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-        KRAG_CUDA(cudaLaunchKernelEx(&cfg, dense_tc2cvt_kernel<NQ>, tmX, tmQh, n_rows, kblocks, n_ptiles, xnorm, alive,
-                                     (const float*)w.thr, w.cand_count, w.cand_rows, cap));
-    } else if (tc_use_2cta() || bf16) {
-        using Cfg2 = Tc2Cfg<NQ>;
-        static bool attr2_set = false;
-        if (!attr2_set) {
-            KRAG_CUDA(cudaFuncSetAttribute(dense_tc2_kernel<NQ, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg2::SMEM));
-            KRAG_CUDA(cudaFuncSetAttribute(dense_tc2_kernel<NQ, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg2::SMEM));
-            attr2_set = true;
-        }
+    dense_timer_begin(st, cvt ? 5 : (bf16 ? 4 : 3), n_rows * (int64_t)dpad * ((bf16 && !cvt) ? 2 : 4), 2 * (int64_t)NQ * n_rows * dpad);
+    if (bf16) {
         CUtensorMap tmQh, tmXh;
-        if (!make_map(&tmQh, bf16 ? (const void*)w.q_bf16 : (const void*)q, nq, dpad, NQ / 2, bf16))
-            throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled(Q half)", __FILE__, __LINE__};
-        if (bf16 && !make_map(&tmXh, Xh, n_rows, dpad, TC_TILE_M, true))
-            throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled(bf16 shadow)", __FILE__, __LINE__};
-        const int kb2 = bf16 ? dpad / (2 * TC_KBLOCK) : kblocks;
-        const int64_t n_ptiles = (n_rows + 2 * TC_TILE_M - 1) / (2 * TC_TILE_M);
-        const int64_t max_pairs = di.sm_count / 2;
-        const int n_pairs = (int)(n_ptiles < max_pairs ? n_ptiles : max_pairs);
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3((unsigned)(2 * n_pairs));
-        cfg.blockDim = dim3(TC_THREADS);
-        cfg.dynamicSmemBytes = Cfg2::SMEM;
-        cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-        if (bf16)
-            KRAG_CUDA(cudaLaunchKernelEx(&cfg, dense_tc2_kernel<NQ, true>, tmXh, tmQh, n_rows, kb2, n_ptiles, xnorm, alive,
-                                         (const float*)w.thr, w.cand_count, w.cand_rows, cap));
-        else
-            KRAG_CUDA(cudaLaunchKernelEx(&cfg, dense_tc2_kernel<NQ, false>, tmX, tmQh, n_rows, kb2, n_ptiles, xnorm, alive,
-                                         (const float*)w.thr, w.cand_count, w.cand_rows, cap));
+        if (!make_map(&tmQh, (const void*)w.q_bf16, nq, dpad, NQ, true))
+            throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled(Q, bf16)", __FILE__, __LINE__};
+        if (cvt) {
+            tc_launch<NQ, TC_CVT, false>(di, tmX, tmQh, n_rows, dpad, n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap,
+                                         nullptr, 0, 0, st);
+        } else {
+            if (!make_map(&tmXh, Xh, n_rows, dpad, TC_TILE_M, true))
+                throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled(bf16 shadow)", __FILE__, __LINE__};
+            tc_launch<NQ, TC_BF16, false>(di, tmXh, tmQh, n_rows, dpad, n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap,
+                                          nullptr, 0, 0, st);
+        }
     } else {
-        dense_tc_kernel<NQ, false><<<grid_m, TC_THREADS, Cfg::SMEM, st>>>(tmX, tmQ, n_rows, kblocks, n_tiles, 1, xnorm, alive, w.thr,
-                                                                          w.cand_count, w.cand_rows, cap, nullptr, 0, 0);
+        tc_launch<NQ, TC_TF32, false>(di, tmX, tmQ, n_rows, dpad, n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap,
+                                      nullptr, 0, 0, st);
     }
     dense_timer_end(st);
     KRAG_CUDA(cudaGetLastError());
@@ -1055,9 +570,9 @@ bool launch_dense_tc(const DeviceInfo& di, const float* X, int64_t n_rows, int d
                      const uint16_t* Xh, bool allow_cvt)
 {
     if (Xh != nullptr && dpad % (2 * TC_KBLOCK) != 0) Xh = nullptr;   // bf16 k-blocks are 64 elements wide
-    // default prune pass: fp32 rows converted to bf16 in shared memory (no shadow); KRAG_TC_CVT=0 keeps the TF32 pass
-    const bool cvt = Xh == nullptr && allow_cvt && tc_use_cvt() && tc_use_2cta() && dpad % (2 * TC_KBLOCK) == 0 &&
-                     di.smem_optin >= TcvCfg<256>::SMEM;
+    // default prune pass: fp32 rows rounded to bf16 on their way into the wgmma A registers (no shadow); KRAG_TC_CVT=0
+    // keeps the TF32 pass
+    const bool cvt = Xh == nullptr && allow_cvt && tc_use_cvt() && dpad % (2 * TC_KBLOCK) == 0;
     if (n_rows < TC_MIN_ROWS || n_rows >= (1ll << 31) || xnorm == nullptr) return false;
     const int cap = tc_cap(P);
     const int64_t S = tc_sample_tiles(n_rows) * TC_TILE_M;
@@ -1100,14 +615,8 @@ bool dense_tc_debug_dump(const DeviceInfo& di, const float* X, int64_t n_rows, i
     if (dump_out == nullptr) return true;   // size query
     CUtensorMap tmX, tmQ;
     if (!make_map(&tmX, X, n_rows, dpad, TC_TILE_M) || !make_map(&tmQ, q, nq, dpad, NQ)) return false;
-    const int kblocks = dpad / TC_KBLOCK;
-    const int grid = (int)(n_tiles < di.sm_count ? n_tiles : di.sm_count);
 #define KRAG_TC_DUMP(N)                                                                                                    \
-    do {                                                                                                                   \
-        KRAG_CUDA(cudaFuncSetAttribute(dense_tc_kernel<N, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcCfg<N>::SMEM)); \
-        dense_tc_kernel<N, true><<<grid, TC_THREADS, TcCfg<N>::SMEM, st>>>(tmX, tmQ, n_rows, kblocks, n_tiles, 1, xnorm, nullptr,   \
-                                                                           nullptr, nullptr, nullptr, 0, dump_out, S, 0);  \
-    } while (0)
+    tc_launch<N, TC_TF32, true>(di, tmX, tmQ, n_rows, dpad, n_tiles, 1, xnorm, nullptr, nullptr, nullptr, nullptr, 0, dump_out, S, 0, st)
     if (NQ == 64) KRAG_TC_DUMP(64); else if (NQ == 128) KRAG_TC_DUMP(128); else KRAG_TC_DUMP(256);
 #undef KRAG_TC_DUMP
     KRAG_CUDA(cudaGetLastError());

@@ -9,10 +9,10 @@
 //   L x [ QKV GEMM -> attention -> O GEMM (+bias +residual) -> LayerNorm -> FFN1 GEMM (+bias, erf-GELU)
 //         -> FFN2 GEMM (+bias +residual) -> LayerNorm ]  ->  CLS row  ->  L2 normalise
 //
-// The four GEMMs per layer (24 S d^2 of the 24 S d^2 + 4 S^2 d flops) run on tcgen05.mma kind::tf32 with
-// fp32 accumulation in TMEM, operands staged by TMA (fp32 weights/activations are consumed as TF32, no
-// conversion pass); bias / GELU / residual are fused into the TMEM epilogue.  LayerNorm, softmax and the
-// attention products are fp32 CUDA-core code (attention is 4 S^2 d: 2% of the flops at S = 32 queries).
+// The four GEMMs per layer (24 S d^2 of the 24 S d^2 + 4 S^2 d flops) run on fp16 wgmma over split operands (see
+// gemm_f16s_kernel) with fp32 accumulation in registers, operands staged by TMA; bias / GELU / residual are fused into
+// the register epilogue.  LayerNorm and softmax are fp32 CUDA-core code; the attention products run on mma.sync
+// (attention is 4 S^2 d: 2% of the flops at S = 32 queries).
 #include <cuda_fp16.h>
 #include <math_constants.h>
 #include <stdlib.h>
@@ -36,34 +36,26 @@ namespace krag {
 //     hi = fp16(v),   lo = fp16((v - hi) * 2^11)          v = hi + lo * 2^-11  to ~2^-22 relative
 // ("split" operands: producers write them next to / instead of the fp32 tensor, weights are split once at load time), and
 //     A . B^T  =  hi_A . hi_B^T  +  2^-11 (hi_A . lo_B^T + lo_A . hi_B^T)          (lo . lo term: 2^-22, dropped)
-// is three kind::f16 MMAs per K = 16 step into two TMEM accumulators (main term / correction terms, combined in the
+// is three fp16 wgmma per K = 16 step into two register accumulators (main term / correction terms, combined in the
 // epilogue; the scaling keeps the lo parts out of the fp16 subnormal range and the small terms out of the big
 // accumulator's rounding).  fp16 products are exact in fp32, so what is left is the accumulation order -- the same kind of
-// error an fp32 SIMT GEMM has.  Operand bytes per element are those of fp32 (2 + 2), the tensor work is 1.5x a TF32 GEMM's:
-// with these layer shapes the kernels stay bound by L2 -> shared-memory operand traffic, as the TF32 kernels they replace
-// were, but now meet the reference's fp32 arithmetic (TF32 carried 10 mantissa bits: ~5e-3 on the unit-norm embedding).
-// Persistent CTAs over 128 x 128 output tiles (n fastest so neighbouring CTAs share the A tile in L2); one TMA warp,
-// one MMA-issuing thread, four epilogue warps; stage = one k-block of 64 halfs of hi_A, lo_A, hi_B, lo_B.
+// error an fp32 SIMT GEMM has.  Operand bytes per element are those of fp32 (2 + 2), the tensor work is 1.5x a TF32 GEMM's,
+// and the result meets the reference's fp32 arithmetic (TF32 carried 10 mantissa bits: ~5e-3 on the unit-norm embedding).
+//
+// One kernel, gemm_f16s_kernel<BN>: 128 x BN output tiles (two consumer warpgroups of wgmma M = 64 rows), K cut into
+// `splits` slices.  Work items (n fastest, so neighbouring CTAs share the A tile in L2, then m, then the K slice) are
+// walked persistently by min(items, SMs) CTAs.  One TMA thread fills a ring of stages = one k-block of 64 halfs of hi_A,
+// lo_A (128 rows each) and hi_B, lo_B (BN rows each).  splits == 1: bias / GELU / residual epilogue straight to the
+// outputs; splits > 1: fp32 partials (main + 2^-11 correction) to ws[split][M][N], summed in split order by
+// splitk_reduce_kernel (deterministic), which also applies bias / residual / LayerNorm and writes the split planes.
 constexpr int GM_TILE = 128;
 constexpr int GH_KB = 64;                   // halfs per k-block (128-byte swizzle row)
 constexpr int GM_SLAB = GM_TILE * 128;      // 16 KB: 128 rows x 128 B
-constexpr int GM_STAGE_BYTES = 4 * GM_SLAB; // 64 KB
-constexpr int GM_STAGES = 3;
-constexpr int GM_THREADS = 192;
-constexpr size_t GM_SMEM = (size_t)GM_STAGES * GM_STAGE_BYTES + 1024 + 256;
+constexpr int GM_THREADS = 384;             // warpgroup 0: TMA producer, warpgroups 1-2: wgmma + epilogue
+constexpr int GM_MAX_STAGES = 16;
+constexpr int GM_SMEM_BUDGET = 200 * 1024;  // operand ring
 constexpr float GH_LO_SCALE = 2048.f, GH_LO_INV = 1.f / 2048.f;
 
-// 256-bit global accesses (sm_100): one full 32-byte sector per thread and instruction
-__device__ __forceinline__ void st_global_v8(float* p, const float* o)
-{
-    asm volatile("st.global.v8.f32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-                 ::"l"(p), "f"(o[0]), "f"(o[1]), "f"(o[2]), "f"(o[3]), "f"(o[4]), "f"(o[5]), "f"(o[6]), "f"(o[7]) : "memory");
-}
-__device__ __forceinline__ void ld_global_v8(const float* p, float* r)
-{
-    asm volatile("ld.global.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=f"(r[0]), "=f"(r[1]), "=f"(r[2]), "=f"(r[3]), "=f"(r[4]), "=f"(r[5]), "=f"(r[6]), "=f"(r[7]) : "l"(p));
-}
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
 
 // ---- split fp16 operands
@@ -111,31 +103,9 @@ void launch_split_f16(const float* in, uint16_t* hi, uint16_t* lo, int64_t n, cu
 {
     const int64_t n8 = n / 8;
     const int64_t want = (n8 + 255) / 256;
-    split_f16_kernel<<<(unsigned)(want < 148 * 16 ? (want > 0 ? want : 1) : 148 * 16), 256, 0, st>>>(in, hi, lo, n8);
+    split_f16_kernel<<<(unsigned)(want < 132 * 16 ? (want > 0 ? want : 1) : 132 * 16), 256, 0, st>>>(in, hi, lo, n8);
     KRAG_CUDA(cudaGetLastError());
     count_launch();
-}
-
-// instruction descriptor for kind::f16 with fp16 operands (format 0), fp32 accumulate, both operands K-major
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N)
-{
-    return (1u << 4) /* D f32 */ | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_f16_2sm(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
 }
 
 // what a GEMM epilogue writes: fp32 C and / or the split planes of C (operand of the next GEMM)
@@ -145,439 +115,122 @@ struct GemmOut {
     uint16_t* lo;
 };
 
-// 32 accumulator columns of one row: v = main + 2^-11 corr (+bias)(gelu)(+residual) -> outputs
-__device__ __forceinline__ void gemm_epilogue_row32(const uint32_t* v0, const uint32_t* v1, const float* __restrict__ bias_c,
-                                                    const float* rrow, int act_gelu, const GemmOut& out, size_t off)
-{
-#pragma unroll
-    for (int j = 0; j < 32; j += 8) {   // 32-byte (full-sector) vector accesses: a thread owns a row segment
-        float o[8];
-#pragma unroll
-        for (int t = 0; t < 8; t += 4) {
-            const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias_c + j + t));
-            o[t + 0] = fmaf(__uint_as_float(v1[j + t + 0]), GH_LO_INV, __uint_as_float(v0[j + t + 0])) + b4.x;
-            o[t + 1] = fmaf(__uint_as_float(v1[j + t + 1]), GH_LO_INV, __uint_as_float(v0[j + t + 1])) + b4.y;
-            o[t + 2] = fmaf(__uint_as_float(v1[j + t + 2]), GH_LO_INV, __uint_as_float(v0[j + t + 2])) + b4.z;
-            o[t + 3] = fmaf(__uint_as_float(v1[j + t + 3]), GH_LO_INV, __uint_as_float(v0[j + t + 3])) + b4.w;
-        }
-        if (act_gelu) {
-#pragma unroll
-            for (int t = 0; t < 8; ++t) o[t] = gelu_erf(o[t]);
-        }
-        if (rrow) {
-            float r[8];
-            ld_global_v8(rrow + j, r);
-#pragma unroll
-            for (int t = 0; t < 8; ++t) o[t] += r[t];
-        }
-        if (out.c) st_global_v8(out.c + off + j, o);
-        if (out.hi) split_store8(o, out.hi + off + j, out.lo + off + j);
-    }
-}
-
+template <int BN>
 __global__ void __launch_bounds__(GM_THREADS, 1)
 gemm_f16s_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmA2,
-                 const __grid_constant__ CUtensorMap tmB1, const __grid_constant__ CUtensorMap tmB2, int M, int N, int K,
-                 const float* __restrict__ bias, const float* __restrict__ residual, int act_gelu, GemmOut out)
+                 const __grid_constant__ CUtensorMap tmB1, const __grid_constant__ CUtensorMap tmB2, int M, int N, int splits,
+                 int kb_per_split, int n_stages, int b_evict_first, const float* __restrict__ bias, const float* residual,
+                 int act_gelu, GemmOut out, float* __restrict__ ws)
 {
+    constexpr int B_BYTES = BN * 128;                      // one plane of one weight k-block
+    constexpr int STAGE_BYTES = 2 * GM_SLAB + 2 * B_BYTES;
+    constexpr int R = BN / 2;                              // accumulators per thread and term
     extern __shared__ unsigned char gm_smem_raw[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(gm_smem_raw) + 1023) & ~(uintptr_t)1023);
-    unsigned char* tail = smem + (size_t)GM_STAGES * GM_STAGE_BYTES;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);
-    uint64_t* empty_bar = full_bar + GM_STAGES;
-    uint64_t* tfull_bar = empty_bar + GM_STAGES;      // [2]
-    uint64_t* tempty_bar = tfull_bar + 2;             // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)n_stages * STAGE_BYTES);
+    uint64_t* empty_bar = full_bar + GM_MAX_STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int m_tiles = (M + GM_TILE - 1) / GM_TILE, n_tiles = N / GM_TILE;
-    const int total = m_tiles * n_tiles;
-    const int kblocks = K / GH_KB;
+    const int m_tiles = (M + GM_TILE - 1) / GM_TILE, n_tiles = N / BN;
+    const int total = m_tiles * n_tiles * splits;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA1); tma_prefetch_desc(&tmA2); tma_prefetch_desc(&tmB1); tma_prefetch_desc(&tmB2);
-        for (int s = 0; s < GM_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        for (int b = 0; b < 2; ++b) { mbar_init(&tfull_bar[b], 1); mbar_init(&tempty_bar[b], 4); }
+        for (int s = 0; s < n_stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
         fence_barrier_init();
-    }
-    if (warp == 1) {   // 2 buffers x (main 128 + correction 128) columns
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        int stage = 0; uint32_t phase = 0;
-        for (int t = blockIdx.x; t < total; t += gridDim.x) {
-            const int m0 = (t / n_tiles) * GM_TILE, n0 = (t % n_tiles) * GM_TILE;
-            for (int kb = 0; kb < kblocks; ++kb) {
-                mbar_wait(&empty_bar[stage], phase ^ 1);
-                if (lane == 0) {
-                    unsigned char* s0 = smem + (size_t)stage * GM_STAGE_BYTES;
-                    mbar_expect_tx(&full_bar[stage], GM_STAGE_BYTES);
-                    const int k0 = kb * GH_KB;
-                    tma_load_2d(s0, &tmA1, &full_bar[stage], k0, m0, TMA_EVICT_FIRST);
-                    tma_load_2d(s0 + GM_SLAB, &tmA2, &full_bar[stage], k0, m0, TMA_EVICT_FIRST);
-                    tma_load_2d(s0 + 2 * GM_SLAB, &tmB1, &full_bar[stage], k0, n0, TMA_EVICT_LAST);
-                    tma_load_2d(s0 + 3 * GM_SLAB, &tmB2, &full_bar[stage], k0, n0, TMA_EVICT_LAST);
-                }
-                __syncwarp();
-                if (++stage == GM_STAGES) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else if (warp == 1) {
-        constexpr uint32_t idesc = umma_idesc_f16(GM_TILE, GM_TILE);
-        const uint64_t desc0 = umma_desc_sw128(smem_u32(smem));
-        const uint64_t dhi = desc0 & 0xFFFFFFFF00000000ull;
-        const uint32_t lo0 = (uint32_t)desc0;
-        int stage = 0; uint32_t phase = 0; int acc = 0; uint32_t acc_phase = 0;
-        for (int t = blockIdx.x; t < total; t += gridDim.x) {
-            mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-            tc_fence_after();
-            const uint32_t d_main = tmem_base + (uint32_t)(acc * 2 * GM_TILE), d_corr = d_main + GM_TILE;
-            for (int kb = 0; kb < kblocks; ++kb) {
-                mbar_wait(&full_bar[stage], phase);
-                tc_fence_after();
-                if (lane == 0) {
-                    const uint32_t a1 = lo0 + (uint32_t)((stage * GM_STAGE_BYTES) >> 4);
-                    const uint32_t a2 = a1 + (GM_SLAB >> 4), b1 = a1 + (2 * GM_SLAB >> 4), b2 = a1 + (3 * GM_SLAB >> 4);
-#pragma unroll
-                    for (int k = 0; k < GH_KB / 16; ++k) {
-                        const uint32_t first = (uint32_t)((kb | k) != 0);
-                        umma_f16(d_main, dhi | (uint64_t)(a1 + 2 * k), dhi | (uint64_t)(b1 + 2 * k), idesc, first);
-                        umma_f16(d_corr, dhi | (uint64_t)(a1 + 2 * k), dhi | (uint64_t)(b2 + 2 * k), idesc, first);
-                        umma_f16(d_corr, dhi | (uint64_t)(a2 + 2 * k), dhi | (uint64_t)(b1 + 2 * k), idesc, 1u);
-                    }
-                    umma_commit(&empty_bar[stage]);
-                    if (kb == kblocks - 1) umma_commit(&tfull_bar[acc]);
-                }
-                __syncwarp();
-                if (++stage == GM_STAGES) { stage = 0; phase ^= 1; }
-            }
-            acc ^= 1;
-            if (acc == 0) acc_phase ^= 1;
-        }
-    } else {
-        const int lg = warp & 3;
-        const int r_in = lg * 32 + lane;
-        int acc = 0; uint32_t acc_phase = 0;
-        for (int t = blockIdx.x; t < total; t += gridDim.x) {
-            const int m0 = (t / n_tiles) * GM_TILE, n0 = (t % n_tiles) * GM_TILE;
-            const int row = m0 + r_in;
-            mbar_wait(&tfull_bar[acc], acc_phase);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)(acc * 2 * GM_TILE);
-#pragma unroll 1
-            for (int c0 = 0; c0 < GM_TILE; c0 += 32) {
-                uint32_t v0[32], v1[32];
-                tmem_ld_x32(taddr + c0, v0);
-                tmem_ld_x32(taddr + GM_TILE + c0, v1);
-                tmem_wait_ld();
-                if (row < M) {
-                    const size_t off = (size_t)row * N + n0 + c0;
-                    gemm_epilogue_row32(v0, v1, bias + n0 + c0, residual ? residual + off : nullptr, act_gelu, out, off);
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-            acc ^= 1;
-            if (acc == 0) acc_phase ^= 1;
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-    }
-}
-
-// ---------------------------------------------------------------- 2-CTA GEMM (cta_group::2, M = 256 per pair)
-// Same structure as dense_tc2_kernel (dense_tc.cu): a CTA pair owns a 256 x BN output tile; each CTA stages its
-// 128 activation rows (hi and lo planes) and HALF of the BN weight rows (hi and lo), the pair's tensor cores share the
-// operands.  Both accumulators of the tile fill the pair's TMEM (2 x BN columns: BN = 256 -> all 512), so a tile's
-// epilogue is not overlapped with the next tile's MMAs; with 12..48 k-blocks per tile that costs a few percent.
-template <int BN> struct Gm2Cfg {
-    static constexpr int BH_BYTES = (BN / 2) * 128;                    // this CTA's half of one weight k-block (one plane)
-    static constexpr int STAGE_BYTES = 2 * GM_SLAB + 2 * BH_BYTES;     // 64 KB at BN = 256, 48 KB at BN = 128
-    static constexpr int STAGES = (200 * 1024) / STAGE_BYTES;          // 3 / 4
-    static constexpr int NBUF = BN <= 128 ? 2 : 1;                     // accumulator sets in TMEM: (main + correction) x NBUF = 512 columns
-    static constexpr int TMEM_COLS = 2 * BN * NBUF;
-    static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + 1024 + 256;
-};
-constexpr int GM2_THREADS = 320;   // warp 0: TMA, warp 1: MMA issuer (leader), warps 2-9: epilogue (2 per TMEM lane group)
-
-template <int BN>
-__global__ void __launch_bounds__(GM2_THREADS, 1)
-gemm2_f16s_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmA2,
-                  const __grid_constant__ CUtensorMap tmB1h, const __grid_constant__ CUtensorMap tmB2h, int M, int N, int K,
-                  const float* __restrict__ bias, const float* __restrict__ residual, int act_gelu, GemmOut out)
-{
-    using Cfg = Gm2Cfg<BN>;
-    extern __shared__ unsigned char gm_smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(gm_smem_raw) + 1023) & ~(uintptr_t)1023);
-    unsigned char* tail = smem + (size_t)Cfg::STAGES * Cfg::STAGE_BYTES;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);             // leader only: 2 arrivals + tx bytes of both CTAs
-    uint64_t* empty_bar = full_bar + Cfg::STAGES;                        // per CTA
-    uint64_t* tfull_bar = empty_bar + Cfg::STAGES;                       // per CTA [1]
-    uint64_t* tempty_bar = tfull_bar + 2;                                // leader only [1]: 16 arrivals
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const int pair = blockIdx.x >> 1, n_pairs = gridDim.x >> 1;
-    const int m_ptiles = (M + 2 * GM_TILE - 1) / (2 * GM_TILE), n_tiles = N / BN;
-    const int total = m_ptiles * n_tiles;
-    const int kblocks = K / GH_KB;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmA1); tma_prefetch_desc(&tmA2); tma_prefetch_desc(&tmB1h); tma_prefetch_desc(&tmB2h);
-        for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full_bar[s], 2); mbar_init(&empty_bar[s], 1); }
-        for (int b = 0; b < 2; ++b) { mbar_init(&tfull_bar[b], 1); mbar_init(&tempty_bar[b], 16); }
-        fence_barrier_init();
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)Cfg::TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        int stage = 0; uint32_t phase = 0;
-        for (int t = pair; t < total; t += n_pairs) {
-            const int m0 = (t / n_tiles) * (2 * GM_TILE) + (int)rank * GM_TILE, n0 = (t % n_tiles) * BN + (int)rank * (BN / 2);
-            for (int kb = 0; kb < kblocks; ++kb) {
-                mbar_wait(&empty_bar[stage], phase ^ 1);
-                if (lane == 0) {
-                    unsigned char* s0 = smem + (size_t)stage * Cfg::STAGE_BYTES;
-                    if (rank == 0) mbar_expect_tx(&full_bar[stage], 2 * Cfg::STAGE_BYTES);
-                    else mbar_arrive_remote(&full_bar[stage], 0);
-                    const int k0 = kb * GH_KB;
-                    tma_load_2d_2sm(s0, &tmA1, &full_bar[stage], k0, m0, TMA_EVICT_FIRST);
-                    tma_load_2d_2sm(s0 + GM_SLAB, &tmA2, &full_bar[stage], k0, m0, TMA_EVICT_FIRST);
-                    tma_load_2d_2sm(s0 + 2 * GM_SLAB, &tmB1h, &full_bar[stage], k0, n0, TMA_EVICT_LAST);
-                    tma_load_2d_2sm(s0 + 2 * GM_SLAB + Cfg::BH_BYTES, &tmB2h, &full_bar[stage], k0, n0, TMA_EVICT_LAST);
-                }
-                __syncwarp();
-                if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else if (warp == 1) {
-        if (rank == 0) {
-            constexpr uint32_t idesc = umma_idesc_f16(2 * GM_TILE, BN);
-            const uint64_t desc0 = umma_desc_sw128(smem_u32(smem));
-            const uint64_t dhi = desc0 & 0xFFFFFFFF00000000ull;
-            const uint32_t lo0 = (uint32_t)desc0;
-            int stage = 0; uint32_t phase = 0; int acc = 0; uint32_t acc_phase = 0;
-            for (int t = pair; t < total; t += n_pairs) {
-                mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t d_main = tmem_base + (uint32_t)(acc * 2 * BN), d_corr = d_main + (uint32_t)BN;
-                for (int kb = 0; kb < kblocks; ++kb) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    if (lane == 0) {
-                        const uint32_t a1 = lo0 + (uint32_t)((stage * Cfg::STAGE_BYTES) >> 4);
-                        const uint32_t a2 = a1 + (GM_SLAB >> 4), b1 = a1 + (2 * GM_SLAB >> 4), b2 = b1 + (Cfg::BH_BYTES >> 4);
-#pragma unroll
-                        for (int k = 0; k < GH_KB / 16; ++k) {
-                            const uint32_t first = (uint32_t)((kb | k) != 0);
-                            umma_f16_2sm(d_main, dhi | (uint64_t)(a1 + 2 * k), dhi | (uint64_t)(b1 + 2 * k), idesc, first);
-                            umma_f16_2sm(d_corr, dhi | (uint64_t)(a1 + 2 * k), dhi | (uint64_t)(b2 + 2 * k), idesc, first);
-                            umma_f16_2sm(d_corr, dhi | (uint64_t)(a2 + 2 * k), dhi | (uint64_t)(b1 + 2 * k), idesc, 1u);
-                        }
-                        umma_commit_2sm(&empty_bar[stage]);
-                        if (kb == kblocks - 1) umma_commit_2sm(&tfull_bar[acc]);
-                    }
-                    __syncwarp();
-                    if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-                }
-                if (++acc == Cfg::NBUF) { acc = 0; acc_phase ^= 1; }
-            }
-        }
-    } else {
-        // 8 epilogue warps: lane group = warp & 3, column half = (warp - 2) >> 2
-        const int lg = warp & 3;
-        const int col_half = (warp - 2) >> 2;
-        const int r_in = lg * 32 + lane;
-        int acc = 0; uint32_t acc_phase = 0;
-        for (int t = pair; t < total; t += n_pairs) {
-            const int m0 = (t / n_tiles) * (2 * GM_TILE) + (int)rank * GM_TILE, n0 = (t % n_tiles) * BN;
-            const int row = m0 + r_in;
-            mbar_wait(&tfull_bar[acc], acc_phase);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)(acc * 2 * BN);
-#pragma unroll 1
-            for (int c0 = col_half * (BN / 2); c0 < (col_half + 1) * (BN / 2); c0 += 32) {
-                uint32_t v0[32], v1[32];
-                tmem_ld_x32(taddr + c0, v0);
-                tmem_ld_x32(taddr + BN + c0, v1);
-                tmem_wait_ld();
-                if (row < M) {
-                    const size_t off = (size_t)row * N + n0 + c0;
-                    gemm_epilogue_row32(v0, v1, bias + n0 + c0, residual ? residual + off : nullptr, act_gelu, out, off);
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                if (rank == 0) mbar_arrive(&tempty_bar[acc]);
-                else mbar_arrive_remote(&tempty_bar[acc], 0);
-            }
-            if (++acc == Cfg::NBUF) { acc = 0; acc_phase ^= 1; }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)Cfg::TMEM_COLS) : "memory");
-    }
-}
-
-// ---------------------------------------------------------------- small-M GEMM: 128 x BN tiles, split-K
-// A handful of query tokens (batch-1 latency; the per-rank slice of a batch on 8 GPUs) gives the persistent kernels
-// above 6..24 tiles for 148 SMs, each CTA streaming up to 1.5 MB of weights through a serial K loop.  This kernel
-// cuts the output into 128 x BN tiles (BN = 32, 64 or 128) AND the K range into `splits` slices, one CTA each, so that
-// ~148 CTAs pull the weight matrix concurrently; when M < 128 only round8(M) activation rows are staged (the other
-// MMA rows compute on stale shared memory and are never stored).  splits == 1: bias / GELU / residual epilogue
-// straight to the outputs; splits > 1: fp32 partials (main + 2^-11 correction) to ws[split][M][N], summed in split order
-// by splitk_reduce_kernel (deterministic), which also applies bias / residual / LayerNorm and writes the split planes.
-// Stages are packed: round8(M) activation rows (a_bytes, hi then lo plane) + BN weight rows (hi, lo) per k-block, so that
-// for a handful of tokens the whole K slice of a CTA is in flight at once and two CTAs fit on an SM.  The MMA still
-// reads a 128-row A operand from each plane's base; the bytes past a_bytes belong to the following planes / stages (or
-// the 16 KB slack after the last one) and only feed accumulator rows that are never stored.
-constexpr int GSK_MAX_STAGES = 32;
-template <int BN> struct GskCfg {
-    static constexpr int B_BYTES = BN * 128;      // one plane of one weight k-block
-};
-static inline size_t gsk_smem_bytes(int n_stages, int stage_bytes) { return 2048 + (size_t)n_stages * stage_bytes + GM_SLAB; }
-
-template <int BN>
-__global__ void __launch_bounds__(GM_THREADS, 1)
-gemm_sk_f16s_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmA2,
-                    const __grid_constant__ CUtensorMap tmB1, const __grid_constant__ CUtensorMap tmB2, int M, int N, int kb_per_split,
-                    int a_bytes, int n_stages, int b_evict_first, const float* __restrict__ bias, const float* __restrict__ residual,
-                    int act_gelu, GemmOut out, float* __restrict__ ws)
-{
-    using Cfg = GskCfg<BN>;
-    extern __shared__ unsigned char gm_smem_raw[];
-    unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(gm_smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(base);
-    uint64_t* empty_bar = full_bar + GSK_MAX_STAGES;
-    uint64_t* tfull_bar = empty_bar + GSK_MAX_STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tfull_bar + 1);
-    unsigned char* smem = base + 1024;
-    const int stage_bytes = 2 * a_bytes + 2 * Cfg::B_BYTES;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int n0 = blockIdx.x * BN, m0 = blockIdx.y * GM_TILE, split = blockIdx.z;
-    const int kb0 = split * kb_per_split;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmA1); tma_prefetch_desc(&tmA2); tma_prefetch_desc(&tmB1); tma_prefetch_desc(&tmB2);
-        for (int s = 0; s < n_stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(tfull_bar, 1);
-        fence_barrier_init();
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)(2 * BN)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
     }
     pdl_launch_dependents();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     pdl_wait();                        // everything above overlapped the previous kernel's tail
 
-    if (warp == 0) {
-        if (lane == 0) {
-            const uint32_t tx = (uint32_t)stage_bytes;
+    if (warp < 4) {
+        regs_dealloc<40>();
+        if (threadIdx.x == 0) {
+            const uint64_t pol_b = b_evict_first ? TMA_EVICT_FIRST : TMA_EVICT_LAST;
             int stage = 0; uint32_t phase = 0;
-            for (int i = 0; i < kb_per_split; ++i) {
-                mbar_wait(&empty_bar[stage], phase ^ 1);
-                unsigned char* sa = smem + (size_t)stage * stage_bytes;
-                mbar_expect_tx(&full_bar[stage], tx);
-                const int k0 = (kb0 + i) * GH_KB;
-                const uint64_t pol = b_evict_first ? TMA_EVICT_FIRST : TMA_EVICT_LAST;
-                tma_load_2d(sa, &tmA1, &full_bar[stage], k0, m0, TMA_EVICT_LAST);
-                tma_load_2d(sa + a_bytes, &tmA2, &full_bar[stage], k0, m0, TMA_EVICT_LAST);
-                tma_load_2d(sa + 2 * a_bytes, &tmB1, &full_bar[stage], k0, n0, pol);
-                tma_load_2d(sa + 2 * a_bytes + Cfg::B_BYTES, &tmB2, &full_bar[stage], k0, n0, pol);
-                if (++stage == n_stages) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else if (warp == 1) {
-        constexpr uint32_t idesc = umma_idesc_f16(GM_TILE, BN);
-        const uint64_t desc0 = umma_desc_sw128(smem_u32(smem));
-        const uint64_t dhi = desc0 & 0xFFFFFFFF00000000ull;
-        const uint32_t lo0 = (uint32_t)desc0;
-        const uint32_t d_main = tmem_base, d_corr = tmem_base + (uint32_t)BN;
-        int stage = 0; uint32_t phase = 0;
-        for (int i = 0; i < kb_per_split; ++i) {
-            mbar_wait(&full_bar[stage], phase);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t a1 = lo0 + (uint32_t)((stage * stage_bytes) >> 4);
-                const uint32_t a2 = a1 + (uint32_t)(a_bytes >> 4), b1 = a2 + (uint32_t)(a_bytes >> 4), b2 = b1 + (Cfg::B_BYTES >> 4);
-#pragma unroll
-                for (int k = 0; k < GH_KB / 16; ++k) {
-                    const uint32_t first = (uint32_t)((i | k) != 0);
-                    umma_f16(d_main, dhi | (uint64_t)(a1 + 2 * k), dhi | (uint64_t)(b1 + 2 * k), idesc, first);
-                    umma_f16(d_corr, dhi | (uint64_t)(a1 + 2 * k), dhi | (uint64_t)(b2 + 2 * k), idesc, first);
-                    umma_f16(d_corr, dhi | (uint64_t)(a2 + 2 * k), dhi | (uint64_t)(b1 + 2 * k), idesc, 1u);
+            for (int t = blockIdx.x; t < total; t += gridDim.x) {
+                const int n0 = (t % n_tiles) * BN, m0 = ((t / n_tiles) % m_tiles) * GM_TILE;
+                const int kb0 = (t / (n_tiles * m_tiles)) * kb_per_split;
+                for (int i = 0; i < kb_per_split; ++i) {
+                    mbar_wait(&empty_bar[stage], phase ^ 1);
+                    unsigned char* s0 = smem + (size_t)stage * STAGE_BYTES;
+                    mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
+                    const int k0 = (kb0 + i) * GH_KB;
+                    tma_load_2d(s0, &tmA1, &full_bar[stage], k0, m0, TMA_EVICT_LAST);
+                    tma_load_2d(s0 + GM_SLAB, &tmA2, &full_bar[stage], k0, m0, TMA_EVICT_LAST);
+                    tma_load_2d(s0 + 2 * GM_SLAB, &tmB1, &full_bar[stage], k0, n0, pol_b);
+                    tma_load_2d(s0 + 2 * GM_SLAB + B_BYTES, &tmB2, &full_bar[stage], k0, n0, pol_b);
+                    if (++stage == n_stages) { stage = 0; phase ^= 1; }
                 }
-                umma_commit(&empty_bar[stage]);
-                if (i == kb_per_split - 1) umma_commit(tfull_bar);
             }
-            __syncwarp();
-            if (++stage == n_stages) { stage = 0; phase ^= 1; }
         }
     } else {
-        const int lg = warp & 3;
-        const int row = m0 + lg * 32 + lane;
-        mbar_wait(tfull_bar, 0);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(lg * 32) << 16);
-        const bool direct = gridDim.z == 1;
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 32) {
-            uint32_t v0[32], v1[32];
-            tmem_ld_x32(taddr + c0, v0);
-            tmem_ld_x32(taddr + BN + c0, v1);
-            tmem_wait_ld();
-            if (row < M) {
-                if (direct) {
-                    const size_t off = (size_t)row * N + n0 + c0;
-                    gemm_epilogue_row32(v0, v1, bias + n0 + c0, residual ? residual + off : nullptr, act_gelu, out, off);
-                } else {
-                    float* wrow = ws + ((size_t)split * M + row) * N + n0 + c0;
+        regs_alloc<232>();
+        const int wg = (warp >> 2) - 1, w = warp & 3;
+        const int g = lane >> 2, q = lane & 3;
+        const int r_lo = 64 * wg + 16 * w + g;             // this thread's accumulator rows: r_lo and r_lo + 8
+        float acc_m[R], acc_c[R];
+        int stage = 0; uint32_t phase = 0;
+        for (int t = blockIdx.x; t < total; t += gridDim.x) {
+            const int n0 = (t % n_tiles) * BN, m0 = ((t / n_tiles) % m_tiles) * GM_TILE;
+            const int split = t / (n_tiles * m_tiles);
+            const bool rows_here = m0 + 64 * wg < M;        // a warpgroup whose 64 rows are all past M skips its MMAs
+            for (int i = 0; i < kb_per_split; ++i) {
+                mbar_wait(&full_bar[stage], phase);
+                if (rows_here) {
+                    const uint32_t s0 = smem_u32(smem + (size_t)stage * STAGE_BYTES);
+                    const uint64_t a1 = wgmma_desc_sw128(s0 + wg * 64 * 128), a2 = wgmma_desc_sw128(s0 + GM_SLAB + wg * 64 * 128);
+                    const uint64_t b1 = wgmma_desc_sw128(s0 + 2 * GM_SLAB), b2 = wgmma_desc_sw128(s0 + 2 * GM_SLAB + B_BYTES);
+                    wgmma_fence();
 #pragma unroll
-                    for (int j = 0; j < 32; j += 8) {
-                        float o[8];
+                    for (int k = 0; k < GH_KB / 16; ++k) {   // K steps of 16 halfs = 32 bytes = 2 descriptor units
+                        const uint32_t first = (uint32_t)((i | k) != 0);
+                        wgmma_f16_ss<BN>(acc_m, a1 + 2 * k, b1 + 2 * k, first);
+                        wgmma_f16_ss<BN>(acc_c, a1 + 2 * k, b2 + 2 * k, first);
+                        wgmma_f16_ss<BN>(acc_c, a2 + 2 * k, b1 + 2 * k, 1u);
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_fence_operands<R>(acc_m);
+                    wgmma_fence_operands<R>(acc_c);
+                }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[stage]);
+                if (++stage == n_stages) { stage = 0; phase ^= 1; }
+            }
+            if (!rows_here) continue;
+            // ===== epilogue straight from the registers: acc[4j + 2h + c] is (row r_lo + 8h, column n0 + 8j + 2q + c)
 #pragma unroll
-                        for (int t = 0; t < 8; ++t) o[t] = fmaf(__uint_as_float(v1[j + t]), GH_LO_INV, __uint_as_float(v0[j + t]));
-                        st_global_v8(wrow + j, o);
+            for (int h = 0; h < 2; ++h) {
+                const int row = m0 + r_lo + 8 * h;
+                if (row >= M) continue;
+                const size_t roff = (size_t)row * N;
+#pragma unroll
+                for (int j = 0; j < R / 4; ++j) {
+                    const int col = n0 + 8 * j + 2 * q;
+                    float o0 = fmaf(acc_c[4 * j + 2 * h], GH_LO_INV, acc_m[4 * j + 2 * h]);
+                    float o1 = fmaf(acc_c[4 * j + 2 * h + 1], GH_LO_INV, acc_m[4 * j + 2 * h + 1]);
+                    if (splits > 1) {
+                        *reinterpret_cast<float2*>(ws + (size_t)split * M * N + roff + col) = make_float2(o0, o1);
+                        continue;
+                    }
+                    const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + col));
+                    o0 += b2.x; o1 += b2.y;
+                    if (act_gelu) { o0 = gelu_erf(o0); o1 = gelu_erf(o1); }
+                    if (residual) {
+                        const float2 r2 = *reinterpret_cast<const float2*>(residual + roff + col);
+                        o0 += r2.x; o1 += r2.y;
+                    }
+                    if (out.c) *reinterpret_cast<float2*>(out.c + roff + col) = make_float2(o0, o1);
+                    if (out.hi) {
+                        uint16_t h0, l0, h1, l1;
+                        split_f16(o0, h0, l0); split_f16(o1, h1, l1);
+                        *reinterpret_cast<uint32_t*>(out.hi + roff + col) = (uint32_t)h0 | ((uint32_t)h1 << 16);
+                        *reinterpret_cast<uint32_t*>(out.lo + roff + col) = (uint32_t)l0 | ((uint32_t)l1 << 16);
                     }
                 }
             }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)(2 * BN)) : "memory");
     }
 }
 
@@ -1350,86 +1003,25 @@ static void emb_map(CUtensorMap* tm, const uint16_t* base, int rows, int cols, i
         throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled failed", __FILE__, __LINE__};
 }
 
-// large-M GEMM on split operands: CTA pairs (256 x BN tiles) or single CTAs (128 x 128 tiles)
-void launch_gemm_f16s(const DeviceInfo& di, const SplitMat& A, const SplitMat& B, int M, int N, int K, const float* bias,
-                      const float* residual, bool gelu, float* C, uint16_t* C_hi, uint16_t* C_lo, cudaStream_t st)
-{
-    static bool attr_set = false;
-    if (!attr_set) {
-        KRAG_CUDA(cudaFuncSetAttribute(gemm_f16s_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GM_SMEM));
-        attr_set = true;
-    }
-    const GemmOut out{C, C_hi, C_lo};
-    CUtensorMap tmA1, tmA2, tmB1, tmB2;
-    emb_map(&tmA1, A.hi, M, K);
-    emb_map(&tmA2, A.lo, M, K);
-    static int use2 = -1;
-    if (use2 < 0) { const char* ev = getenv("KRAG_GEMM_2CTA"); use2 = (ev == nullptr || ev[0] != '0') ? 1 : 0; }
-    // CTA pairs (256 x BN tiles) win when there are enough tiles to fill the 74 pairs; small problems (few query
-    // tokens per rank) are latency-bound by the K loop of a single tile, where 128 x 128 tiles on single CTAs
-    // halve the per-tile MMA time and quadruple the number of CTAs
-    static int want_bn = -1;
-    if (want_bn < 0) { const char* ev = getenv("KRAG_GEMM_BN"); want_bn = (ev && atoi(ev) == 256) ? 256 : 128; }
-    const int BN = (want_bn == 256 && N % 256 == 0) ? 256 : 128;
-    const int pair_tiles = ((M + 2 * GM_TILE - 1) / (2 * GM_TILE)) * (N / BN);
-    if (use2 && M > GM_TILE && pair_tiles >= di.sm_count / 4) {
-        emb_map(&tmB1, B.hi, N, K, BN / 2);
-        emb_map(&tmB2, B.lo, N, K, BN / 2);
-        const int total2 = ((M + 2 * GM_TILE - 1) / (2 * GM_TILE)) * (N / BN);
-        const int max_pairs = di.sm_count / 2;
-        const int n_pairs = total2 < max_pairs ? total2 : max_pairs;
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3((unsigned)(2 * n_pairs));
-        cfg.blockDim = dim3(GM2_THREADS);
-        cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-        const int gelu_i = gelu ? 1 : 0;
-        if (BN == 256) {
-            static bool a256 = false;
-            if (!a256) { KRAG_CUDA(cudaFuncSetAttribute(gemm2_f16s_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Gm2Cfg<256>::SMEM)); a256 = true; }
-            cfg.dynamicSmemBytes = Gm2Cfg<256>::SMEM;
-            KRAG_CUDA(cudaLaunchKernelEx(&cfg, gemm2_f16s_kernel<256>, tmA1, tmA2, tmB1, tmB2, M, N, K, bias, residual, gelu_i, out));
-        } else {
-            static bool a128 = false;
-            if (!a128) { KRAG_CUDA(cudaFuncSetAttribute(gemm2_f16s_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Gm2Cfg<128>::SMEM)); a128 = true; }
-            cfg.dynamicSmemBytes = Gm2Cfg<128>::SMEM;
-            KRAG_CUDA(cudaLaunchKernelEx(&cfg, gemm2_f16s_kernel<128>, tmA1, tmA2, tmB1, tmB2, M, N, K, bias, residual, gelu_i, out));
-        }
-        count_launch();
-        return;
-    }
-    emb_map(&tmB1, B.hi, N, K);
-    emb_map(&tmB2, B.lo, N, K);
-    const int total = ((M + GM_TILE - 1) / GM_TILE) * (N / GM_TILE);
-    const int grid = total < di.sm_count ? total : di.sm_count;
-    gemm_f16s_kernel<<<grid, GM_THREADS, GM_SMEM, st>>>(tmA1, tmA2, tmB1, tmB2, M, N, K, bias, residual, gelu ? 1 : 0, out);
-    KRAG_CUDA(cudaGetLastError());
-    count_launch();
-}
-
-
-// small-M path: 128 x BN tiles x split-K slices, ~one CTA per SM (see gemm_sk_f16s_kernel)
+// gemm_f16s_kernel over the 128 x BN tiles of C and `splits` K slices, min(work items, SMs) persistent CTAs
 template <int BN>
-static void launch_gemm_sk(const CUtensorMap& tmA1, const CUtensorMap& tmA2, const CUtensorMap& tmB1, const CUtensorMap& tmB2, int M, int N,
-                           int m_tiles, int splits, int kb_per_split, int a_rows, const float* bias, const float* residual, bool gelu,
-                           const GemmOut& out, float* ws, cudaStream_t st)
+static void launch_gemm(const DeviceInfo& di, const SplitMat& A, const SplitMat& B, int M, int N, int K, int splits, const float* bias,
+                        const float* residual, bool gelu, const GemmOut& out, float* ws, cudaStream_t st)
 {
+    constexpr int stage_bytes = 2 * GM_SLAB + 2 * BN * 128;
+    constexpr int n_stages = GM_SMEM_BUDGET / stage_bytes < GM_MAX_STAGES ? GM_SMEM_BUDGET / stage_bytes : GM_MAX_STAGES;
+    constexpr size_t smem = 1024 + (size_t)n_stages * stage_bytes + 2 * GM_MAX_STAGES * 8;
     static bool attr = false;
-    if (!attr) { KRAG_CUDA(cudaFuncSetAttribute(gemm_sk_f16s_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)); attr = true; }
-    const int a_bytes = a_rows * 128, stage_bytes = 2 * a_bytes + 2 * GskCfg<BN>::B_BYTES;
-    // a few activation rows: keep a CTA under half an SM's shared memory (two CTAs per SM, the next kernel's CTAs
-    // can become resident while this one drains); full 128-row tiles take the whole SM
-    const int budget = (a_rows <= 32 ? 96 : 196) * 1024;
-    int n_stages = budget / stage_bytes;
-    n_stages = n_stages > GSK_MAX_STAGES ? GSK_MAX_STAGES : n_stages;
-    n_stages = n_stages > kb_per_split ? kb_per_split : n_stages;
-    n_stages = n_stages < 1 ? 1 : n_stages;
-    launch_pdl(gemm_sk_f16s_kernel<BN>, dim3((unsigned)(N / BN), (unsigned)m_tiles, (unsigned)splits), dim3(GM_THREADS),
-               gsk_smem_bytes(n_stages, stage_bytes), st, tmA1, tmA2, tmB1, tmB2, M, N, kb_per_split, a_bytes, n_stages, m_tiles == 1 ? 1 : 0, bias,
-               residual, gelu ? 1 : 0, out, ws);
+    if (!attr) { KRAG_CUDA(cudaFuncSetAttribute(gemm_f16s_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = true; }
+    CUtensorMap tmA1, tmA2, tmB1, tmB2;
+    emb_map(&tmA1, A.hi, M, K); emb_map(&tmA2, A.lo, M, K);
+    emb_map(&tmB1, B.hi, N, K, BN); emb_map(&tmB2, B.lo, N, K, BN);
+    const int m_tiles = (M + GM_TILE - 1) / GM_TILE;
+    const int total = m_tiles * (N / BN) * splits;
+    const int grid = total < di.sm_count ? total : di.sm_count;
+    // one activation tile: every weight byte is read once, keep it out of the way of the activations in L2
+    launch_pdl(gemm_f16s_kernel<BN>, dim3((unsigned)grid), dim3(GM_THREADS), smem, st, tmA1, tmA2, tmB1, tmB2, M, N, splits,
+               K / GH_KB / splits, n_stages, m_tiles == 1 ? 1 : 0, bias, residual, gelu ? 1 : 0, out, ws);
 }
 
 // Linear layer on split operands: C = A . B^T + bias (+GELU) (+residual) -> fp32 C and / or split planes of C; with ln_g the
@@ -1456,23 +1048,19 @@ void launch_linear(const DeviceInfo& di, const SplitMat& A, const SplitMat& B, i
             for (int sp = want; sp >= 2; --sp)
                 if (kblocks % sp == 0 && kblocks / sp >= 2 && (size_t)sp * M * N <= ws_floats) { splits = sp; break; }
         }
-        const int a_rows = m_tiles == 1 ? ((M + 7) / 8) * 8 : GM_TILE;
-        CUtensorMap tmA1, tmA2, tmB1, tmB2;
-        emb_map(&tmA1, A.hi, M, K, a_rows); emb_map(&tmA2, A.lo, M, K, a_rows);
-        emb_map(&tmB1, B.hi, N, K, BN); emb_map(&tmB2, B.lo, N, K, BN);
         // splits == 1 and a LayerNorm to follow: the GEMM writes fp32 C (scratch), the LayerNorm kernel writes Y + planes
         const GemmOut direct = ln_g ? GemmOut{C, nullptr, nullptr} : GemmOut{C, C_hi, C_lo};
-        if (BN == 32) launch_gemm_sk<32>(tmA1, tmA2, tmB1, tmB2, M, N, m_tiles, splits, kblocks / splits, a_rows, bias, residual, gelu, direct, ws, st);
-        else if (BN == 128) launch_gemm_sk<128>(tmA1, tmA2, tmB1, tmB2, M, N, m_tiles, splits, kblocks / splits, a_rows, bias, residual, gelu, direct, ws, st);
-        else launch_gemm_sk<64>(tmA1, tmA2, tmB1, tmB2, M, N, m_tiles, splits, kblocks / splits, a_rows, bias, residual, gelu, direct, ws, st);
+        if (BN == 32) launch_gemm<32>(di, A, B, M, N, K, splits, bias, residual, gelu, direct, ws, st);
+        else if (BN == 128) launch_gemm<128>(di, A, B, M, N, K, splits, bias, residual, gelu, direct, ws, st);
+        else launch_gemm<64>(di, A, B, M, N, K, splits, bias, residual, gelu, direct, ws, st);
         if (splits > 1) {
             launch_pdl(splitk_reduce_kernel, dim3((unsigned)M), dim3(256), 0, st, ws, splits, M, N, bias, residual, gelu ? 1 : 0, ln_g, ln_b, eps,
                        ln_g ? Y : C, ln_g ? Y_hi : C_hi, ln_g ? Y_lo : C_lo);
             return;
         }
     } else {
-        if (ln_g) launch_gemm_f16s(di, A, B, M, N, K, bias, residual, gelu, C, nullptr, nullptr, st);
-        else launch_gemm_f16s(di, A, B, M, N, K, bias, residual, gelu, C, C_hi, C_lo, st);
+        launch_gemm<128>(di, A, B, M, N, K, 1, bias, residual, gelu, ln_g ? GemmOut{C, nullptr, nullptr} : GemmOut{C, C_hi, C_lo},
+                         nullptr, st);
     }
     if (ln_g) {
         launch_pdl(layernorm_kernel, dim3((unsigned)((M * 32 + 255) / 256)), dim3(256), 0, st, C, Y, Y_hi, Y_lo, ln_g, ln_b, M, N, eps);

@@ -19,7 +19,7 @@ struct OrdMap {
 
 struct DeviceInfo {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     int cc_major = 0, cc_minor = 0;
     size_t smem_optin = 0;
 };
@@ -42,7 +42,7 @@ void launch_dense_scan(const DeviceInfo& di, const float* X, int64_t n_rows, int
                        const float* q, int batch, int P, OrdMap ord_base, uint64_t* part, uint64_t* keys_out,
                        cudaStream_t st);
 
-// ---- K2: tcgen05 TF32 candidate generation + exact fp32 rescoring (dense_tc.cu)
+// ---- K2: wgmma candidate generation + exact fp32 rescoring (dense_tc.cu)
 bool dense_tc_supported(const DeviceInfo& di, int dpad);
 bool dense_tc_wants(int64_t n_rows, int batch);   // size heuristics: is K2 the better kernel for this call?
 size_t dense_tc_workspace_bytes(const DeviceInfo& di, int64_t n_rows, int P);
@@ -54,7 +54,7 @@ bool launch_dense_tc(const DeviceInfo& di, const float* X, int64_t n_rows, int d
                      const float* xnorm, const uint32_t* xn_max_bits, const float* q, int batch, int P,
                      OrdMap ord_base, void* workspace, size_t workspace_bytes, uint64_t* part, uint64_t* keys_out,
                      cudaStream_t st, const uint16_t* Xh = nullptr /* optional bf16 shadow of X for the prune pass */,
-                     bool allow_cvt = true /* fp32 rows rounded to bf16 on chip (kind::f16) instead of kind::tf32 */);
+                     bool allow_cvt = true /* fp32 rows rounded to bf16 on chip (bf16 wgmma) instead of tf32 wgmma */);
 void launch_f32_to_bf16(const float* in, uint16_t* out, int64_t n_elems, cudaStream_t st);
 int64_t dense_tc_fallback_queries();   // queries re-run on K1 because the exactness certificate failed
 // diagnostics: a[j][r] = |x_r|^2 - 2 x_r.q_j for ALL rows through the tensor-core kernel (tests only)
@@ -125,9 +125,9 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
 // A fp32 matrix carried as two fp16 planes: v = hi + lo * 2^-11 (see embed.cu: split operands of the K5 GEMMs)
 struct SplitMat { uint16_t* hi; uint16_t* lo; };
 void launch_split_f16(const float* in, uint16_t* hi, uint16_t* lo, int64_t n /* % 8 == 0 */, cudaStream_t st);
-// Linear layer on split operands: C = A . B^T + bias (+GELU) (+residual), fp32-accurate (three kind::f16 MMAs per step);
+// Linear layer on split operands: C = A . B^T + bias (+GELU) (+residual), fp32-accurate (three fp16 wgmma per step);
 // outputs: fp32 C and / or the split planes of C; with ln_g the row LayerNorm of that goes to Y / Y planes (C is scratch).
-// Picks CTA pairs / 128x128 tiles / 128xBN split-K tiles by problem size; ws = split-K workspace (may be null).
+// Picks 128x128 tiles / 128xBN split-K tiles by problem size; ws = split-K workspace (may be null).
 void launch_linear(const DeviceInfo& di, const SplitMat& A, const SplitMat& B, int M, int N, int K, const float* bias, const float* residual,
                    bool gelu, float* C, uint16_t* C_hi, uint16_t* C_lo, const float* ln_g, const float* ln_b, float eps, float* Y,
                    uint16_t* Y_hi, uint16_t* Y_lo, float* ws, size_t ws_floats, cudaStream_t st);

@@ -1,6 +1,6 @@
-// tc_ptx.cuh -- inline-PTX wrappers for the Blackwell async machinery used by the tensor-core kernels:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc/mma/commit/ld/fences) and UMMA descriptors.
-// Bit layouts follow cute/arch/mma_sm100_desc.hpp (SmemDescriptor, InstrDescriptor).
+// tc_ptx.cuh -- inline-PTX wrappers for the Hopper async machinery used by the tensor-core kernels:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (fences, commit / wait groups) and the wgmma shared-memory descriptor.
+// The wgmma instructions themselves are in wgmma.cuh.
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
@@ -32,18 +32,17 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity)
         : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
     return ok != 0;
 }
-// bounded wait: a protocol bug traps instead of hanging the GPU
+// bounded wait: a protocol bug traps instead of hanging the GPU (no printf here: a function call inside the wgmma
+// loop would make ptxas serialise the wgmma pipeline)
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity)
 {
     if (mbar_try_wait(bar, parity)) return;
     const long long t0 = clock64();
     while (!mbar_try_wait(bar, parity)) {
-        if (clock64() - t0 > 4000000000ll) { printf("dense_tc: mbarrier wait timed out (block %d thread %d)\n", blockIdx.x, threadIdx.x); __trap(); }
+        if (clock64() - t0 > 4000000000ll) __trap();
     }
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 constexpr uint64_t TMA_EVICT_FIRST = 0x12F0000000000000ull;
 constexpr uint64_t TMA_EVICT_LAST = 0x14F0000000000000ull;
@@ -61,122 +60,29 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* tm)
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tm)) : "memory");
 }
 
-// UMMA shared-memory descriptor, K-major operand, SWIZZLE_128B, 8-row groups 1024 B apart
-// (bit layout: cute/arch/mma_sm100_desc.hpp SmemDescriptor)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr)
+// wgmma shared-memory descriptor, K-major operand, SWIZZLE_128B, 8-row groups 1024 B apart.  The operand tile starts
+// 1024-byte aligned; a K step inside the 128-byte swizzle row adds its byte offset / 16 to the start-address field.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr)
 {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);   // start address, 16-byte units   [0,14)
     d |= (uint64_t)1 << 16;                         // leading byte offset (unused for swizzled K-major)
     d |= (uint64_t)(1024 >> 4) << 32;               // stride byte offset = 1024 B     [32,46)
-    d |= (uint64_t)1 << 46;                         // descriptor version 1 (sm_100)   [46,48)
-    d |= (uint64_t)2 << 61;                         // layout type SWIZZLE_128B        [61,64)
+    d |= (uint64_t)1 << 62;                         // layout type SWIZZLE_128B        [62,64)
     return d;
 }
-// instruction descriptor for kind::tf32, fp32 accumulate, both operands K-major
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(int M, int N)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of accumulator registers across wgmma issue / wait
+template <int R> __device__ __forceinline__ void wgmma_fence_operands(float* d)
 {
-    return (1u << 4)      /* D format f32 */
-         | (2u << 7)      /* A format tf32 */
-         | (2u << 10)     /* B format tf32 */
-         | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t* v)
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-
-// ---- CTA-pair (cta_group::2) helpers
-__device__ __forceinline__ uint32_t cluster_ctarank()
-{
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all()
-{
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta)
-{
-    asm volatile(
-        "{\n\t.reg .b32 ra;\n\t"
-        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-        "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
-        ::"r"(smem_u32(bar)), "r"(cta) : "memory");
-}
-// cluster-scope release / acquire: the payload is shared memory of the PEER CTA written by its threads
-__device__ __forceinline__ void mbar_arrive_remote_release(uint64_t* bar, uint32_t cta)
-{
-    asm volatile(
-        "{\n\t.reg .b32 ra;\n\t"
-        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
-        ::"r"(smem_u32(bar)), "r"(cta) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity)
-{
-    const long long t0 = clock64();
-    for (;;) {
-        uint32_t ok;
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-        if (ok) return;
-        if (clock64() - t0 > 4000000000ll) { printf("dense_tc: cluster mbarrier wait timed out (block %d thread %d)\n", blockIdx.x, threadIdx.x); __trap(); }
-    }
-}
-constexpr uint32_t TC_PEER_MASK = 0xFEFFFFFFu;   // clears the CTA-rank bit: the pair leader's copy of a barrier
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* tm, uint64_t* leader_bar, int c0, int c1,
-                                                uint64_t policy)
-{
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-        " [%0], [%1, {%3, %4}], [%2], %5;"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(leader_bar) & TC_PEER_MASK), "r"(c0),
-          "r"(c1), "l"(policy)
-        : "memory");
-}
-__device__ __forceinline__ void umma_tf32_2sm(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar)   // arrives on `bar` in BOTH CTAs of the pair
-{
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-
-
+// warp-specialised kernels: the producer warpgroup gives registers to the consumer (accumulator) warpgroups
+template <int R> __device__ __forceinline__ void regs_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void regs_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // programmatic dependent launch: let the next kernel of the stream become resident and run its prologue while this
 // grid drains; every thread of a kernel launched that way calls pdl_wait() before it touches global memory written by
@@ -184,3 +90,5 @@ __device__ __forceinline__ void umma_commit_2sm(uint64_t* bar)   // arrives on `
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 }  // namespace krag
+
+#include "wgmma.cuh"

@@ -188,7 +188,7 @@ def create_app(store: vs.VectorStore, cfg: dict | None = None, llm=None) -> Fast
     chat_cfg = {**_chat.chat_config(), **{k: v for k, v in cfg.items() if k in _chat.chat_config()}}
     if llm is None and chat_cfg.get("llm_inference_url"):
         llm = _chat.LLMClient(chat_cfg["llm_inference_url"], chat_cfg["llm_access_secret"], chat_cfg["llm_context_window"])
-    app = FastAPI(title="KAITO RAGEngine service (B200-native)")
+    app = FastAPI(title="KAITO RAGEngine service (H100-native)")
     reg = CollectorRegistry()
     mx = build_metrics(reg)
     M = {"index": ("rag_index_latency_seconds", "rag_index_requests"), "indexes": ("rag_indexes_latency_seconds", "rag_indexes_requests"),

@@ -1,7 +1,7 @@
 """Host-side mirror of the reference RAGService store classes for the /index and /retrieve
 paths, backed by libkaito_rag (CUDA) instead of LlamaIndex + FAISS + bm25s.
 
-Mirrors (paths relative to /root/reference/presets/ragengine/):
+Mirrors (paths relative to the reference's presets/ragengine/):
   BaseVectorStore            vector_store/base.py:60-978   (index_documents, retrieve, CRUD, persist/load)
   FaissVectorStoreHandler    vector_store/faiss_store.py:25-50
   HybridRetriever            vector_store/retriever/hybrid_retriever.py:60-237

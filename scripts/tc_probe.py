@@ -1,4 +1,4 @@
-"""Small driver for ncu: K2 (tcgen05) dense search, batch 256, over a device-generated corpus."""
+"""Small driver for ncu: K2 (wgmma) dense search, batch 256, over a device-generated corpus."""
 import sys
 import numpy as np
 sys.path.insert(0, ".")

@@ -74,7 +74,7 @@ def test_header_is_plain_c99_and_links(tmp_path):
 
 def test_c_example_builds_and_fails_loudly_without_a_gpu(tmp_path):
     """examples/krag_demo.c (the cgo-equivalent call sequence in plain C) compiles as pedantic C99 and links; on a machine
-    without an sm_100 GPU it stops at krag_init with KRAG_E_NO_DEVICE -- there is no CPU path to fall back to."""
+    without an sm_90 GPU it stops at krag_init with KRAG_E_NO_DEVICE -- there is no CPU path to fall back to."""
     import shutil
     import subprocess
     gcc = "/usr/bin/gcc" if os.path.exists("/usr/bin/gcc") else shutil.which("gcc")

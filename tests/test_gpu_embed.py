@@ -1,4 +1,4 @@
-"""K5 (BERT encoder forward; linear layers on tcgen05 kind::f16 with split fp16 operands = fp32-accurate products) against
+"""K5 (BERT encoder forward; linear layers on fp16 wgmma with split fp16 operands = fp32-accurate products) against
 transformers.BertModel in fp32 on the CPU with the same seeded random weights (the real bge weights are not available
 offline; an opt-in test at the bottom runs the reference's own golden when a local snapshot is given), CLS pooling + L2 norm
 as sentence-transformers does for bge (embedding/huggingface_local_embedding.py:34-53).  Tolerances are written out: the

@@ -1,4 +1,4 @@
-"""GPU tests of K2, the tcgen05 TF32 kernel: raw tensor-core output against numpy, and the
+"""GPU tests of K2, the wgmma prune kernel: raw tensor-core output against numpy, and the
 full prune -> exact-rescore -> certify pipeline bit-exact against the oracle."""
 import ctypes as C
 
@@ -10,8 +10,8 @@ pytestmark = pytest.mark.gpu
 
 @pytest.fixture(scope="module", params=["cvt", "tf32"])
 def ctx_tc(request):
-    """K2 forced for every batch size: the default prune pass (fp32 rows rounded to bf16 in shared memory, kind::f16) and
-    the direct TF32 pass (kind::tf32) it replaced"""
+    """K2 forced for every batch size: the default prune pass (fp32 rows rounded to bf16 on chip, bf16 wgmma) and
+    the direct TF32 pass (tf32 wgmma)"""
     from kaito_b200 import _native
     c = _native.Context(device_id=0, dense_mode=_native.DENSE_TC if request.param == "cvt" else _native.DENSE_TC_TF32)
     yield c
@@ -108,7 +108,7 @@ def test_bf16_shadow_pruning_still_returns_exact_fp32(ctx_bf16, oracle, batch, P
         rd, ro = oracle.dense_topk(x, q, P)
         assert np.array_equal(ordn, ro) and np.array_equal(dist, rd)
         assert fb <= max(1, batch // 10), fb
-        assert _native.last_dense_kernel()[1] == 4      # the bf16 cta_group::2 kernel really ran
+        assert _native.last_dense_kernel()[1] == 4      # the bf16-shadow prune pass really ran
     finally:
         ix.drop()
 
@@ -147,7 +147,7 @@ def test_dense_mode_switch_builds_shadow_on_demand(oracle):
 # ---------------------------------------------------------------- K2 at the shapes it is benchmarked on
 # bench.py runs K2 at d = 768 (24 fp32 / 12 bf16 k-blocks per tile: the staging ring wraps several times per tile and the
 # mbarrier phases flip, unlike d = 128) over millions of rows with NQ = 256.  These cases pin the whole pipeline (sample ->
-# threshold -> prune on tcgen05 -> exact rescoring -> certificate) bit-exact against the oracle at those shapes, for both
+# threshold -> prune on the tensor cores -> exact rescoring -> certificate) bit-exact against the oracle at those shapes, for both
 # the default pass (kernel id 5, fp32 rows rounded to bf16 on chip) and the TF32 pass (id 3).
 _BIG = {}
 
@@ -185,7 +185,7 @@ def test_tc_pipeline_bit_exact_at_bench_shapes(ctx_tc, oracle, n, d, batch, pool
             dist, ordn = ix.search_dense(q, P)
             fb = _native.load().krag_tc_fallback_queries() - fb0
             kid = _native.last_dense_kernel()[1]
-            assert kid in (3, 5), kid                                   # the cta_group::2 pass that bench.py times
+            assert kid in (3, 5), kid                                   # the prune pass that bench.py times
             assert np.array_equal(ordn, ro_all[:, :P]), f"ids differ at P={P} (kernel {kid})"
             assert np.array_equal(dist, rd_all[:, :P]), f"distances differ at P={P} (kernel {kid})"
             assert fb <= batch // 20, f"{fb} of {batch} queries fell back to the exact scan on random data"

@@ -102,47 +102,83 @@ def test_prestop_snapshot_and_poststart_restore(oracle, tmp_path, monkeypatch):
         th.join(timeout=5)
 
 
-REF_MANAGER = "/root/reference/presets/ragengine/lifecycle/manager.py"
+LIFECYCLE_GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "lifecycle_reference.json")
+TS_RE = r"\d{4}-\d\d-\d\dT\d\d-\d\d-\d\d"
 
 
-@pytest.mark.skipif(not os.path.exists(REF_MANAGER), reason="reference tree not present (it never is on the GPU box)")
+def _replay(url, requests, snap):
+    """send recorded (method, path) pairs with <snap> filled in; every one must answer 200"""
+    import urllib.request
+    out = []
+    for method, path in requests:
+        req = urllib.request.Request(url + path.replace("<snap>", snap), method=method, data=b"" if method == "POST" else None)
+        with urllib.request.urlopen(req, timeout=30) as r:
+            assert r.status == 200, (method, path)
+            out.append(json.loads(r.read() or b"null"))
+    return out
+
+
 def test_reference_lifecycle_manager_drives_this_service(oracle, tmp_path, monkeypatch):
-    """Drop-in check with the reference in the loop: its own PreStop/PostStart handlers (lifecycle/manager.py, executed
-    unmodified, only pointed at the test server) persist and restore this service's indexes, and snapshots written by
-    either implementation restore under the other."""
+    """Drop-in check against the reference's own PreStop / PostStart handlers (lifecycle/manager.py), recorded in
+    tests/golden/lifecycle_reference.json by oracle/gen_golden_lifecycle.py: the requests they send (unquoted snapshot
+    paths, URL-quoted index names) work against this service, a snapshot laid out as theirs restores under our PostStart,
+    and a snapshot written by our PreStop satisfies what their PostStart reads (LATEST, metadata.json index_names)."""
     from starlette.testclient import TestClient
     from tests.oracle_engine import OracleEngine
+    gold = json.load(open(LIFECYCLE_GOLD))
+    names = gold["indexes"]
     port = _free_port()
     url = f"http://127.0.0.1:{port}"
     app = create_app(VectorStore(HashingEmbedding(64), OracleEngine(oracle)), {"persist_dir": str(tmp_path), "llm_inference_url": None})
     server, th = _serve(app, port)
     try:
-        spec = importlib.util.spec_from_file_location("ref_lifecycle_manager", REF_MANAGER)
-        ref = importlib.util.module_from_spec(spec)
-        spec.loader.exec_module(ref)
-        ref.wait_for_service.__defaults__ = (url + "/indexes", 60)
-        for fn in (ref.get_indexes, ref.load_index, ref.persist_index):
-            fn.__defaults__ = (url,)
-        import types
-        monkeypatch.setattr(ref, "time", types.SimpleNamespace(sleep=lambda s: None, time=time.time))   # its 0.5 s rate limiting
-        monkeypatch.setenv("POD_UID", "feedfacecafe")
         c = TestClient(app)
         docs = [{"text": "First document about retrieval engines"}, {"text": "Second document about Kubernetes operators"}]
-        assert c.post("/index", json={"index_name": "idx_a", "documents": docs}).status_code == 200
-        before = c.post("/retrieve", json={"index_name": "idx_a", "query": "retrieval engines", "max_node_count": 2}).json()
-        # reference PreStop -> our PostStart
-        assert ref.prestop_handler(str(tmp_path)) == 0
-        assert c.delete("/indexes/idx_a").status_code == 200
+        for name in names:
+            assert c.post("/index", json={"index_name": name, "documents": docs}).status_code == 200
+        query = {"index_name": names[0], "query": "retrieval engines", "max_node_count": 2}
+        before = c.post("/retrieve", json=query).json()
+
+        # reference PreStop (replayed) -> our PostStart
+        pre = gold["prestop"]
+        ts = "2000-01-01T00-00-00"                                    # older than any snapshot our PreStop writes below
+        rel = pre["snapshot_dir"].replace("<ts>", ts)
+        snap = str(tmp_path / rel)
+        os.makedirs(snap)
+        listed = _replay(url, pre["requests"], snap)
+        assert listed[0] == names                                      # GET /indexes: the names it persists
+        meta = dict(pre["metadata"], timestamp="2000-01-01T00:00:00.000000")
+        json.dump(meta, open(os.path.join(snap, "metadata.json"), "w"), indent=2)
+        os.symlink(pre["latest_link"].replace("<ts>", ts), tmp_path / "LATEST")
+        assert sorted(os.listdir(snap)) == sorted(pre["snapshot_entries"] + names)
+        for name in names:
+            assert c.delete(f"/indexes/{name}").status_code == 200
         hooks = _load_hooks(monkeypatch, port, tmp_path, "feedfacecafe")
         assert hooks.poststart() == 0
-        assert c.post("/retrieve", json={"index_name": "idx_a", "query": "retrieval engines", "max_node_count": 2}).json() == before
-        # our PreStop -> reference PostStart
-        time.sleep(1.1)
+        assert sorted(c.get("/indexes").json()) == sorted(names)
+        assert c.post("/retrieve", json=query).json() == before
+
+        # our PreStop -> reference PostStart (its reader rules, then its recorded requests)
         assert hooks.prestop() == 0
-        assert c.delete("/indexes/idx_a").status_code == 200
-        assert ref.poststart_handler(str(tmp_path)) == 0
-        assert c.get("/indexes").json() == ["idx_a"]
-        assert c.post("/retrieve", json={"index_name": "idx_a", "query": "retrieval engines", "max_node_count": 2}).json() == before
+        link = os.readlink(tmp_path / "LATEST")
+        want = re.escape(pre["latest_link"]).replace(re.escape("<ts>"), TS_RE).replace(re.escape("pod-" + gold["env"]["POD_UID"][:8]), "pod-feedface")
+        assert re.fullmatch(want, link), link                           # relative, systemsnapshots/<ts>_pod-<uid8>
+        ours = os.path.realpath(tmp_path / "LATEST")
+        ours_meta = json.load(open(os.path.join(ours, "metadata.json")))
+        assert set(ours_meta) == set(pre["metadata"]) and ours_meta["version"] == pre["metadata"]["version"]
+        assert ours_meta["index_names"] == names
+        for name in names:
+            assert c.delete(f"/indexes/{name}").status_code == 200
+        _replay(url, gold["poststart"]["requests"], ours)
+        assert sorted(c.get("/indexes").json()) == sorted(names)
+        assert c.post("/retrieve", json=query).json() == before
+        # LATEST lost: the reference falls back to the newest snapshot directory by name -- ours
+        os.remove(tmp_path / "LATEST")
+        newest = sorted(os.listdir(tmp_path / "systemsnapshots"), reverse=True)[0]
+        assert os.path.realpath(tmp_path / "systemsnapshots" / newest) == ours
+        assert gold["poststart_without_latest"]["latest_link"] == pre["latest_link"]
+        _replay(url, gold["poststart_without_latest"]["requests"], ours)
+        assert c.post("/retrieve", json=query).json() == before
         assert len(os.listdir(tmp_path / "systemsnapshots")) == 2
     finally:
         server.should_exit = True
@@ -183,30 +219,27 @@ def test_resolve_model_dir(tmp_path, monkeypatch):
     assert resolve_model_dir("BAAI/bge-small-en-v1.5") == str(tmp_path / "explicit")
 
 
-REF_GO = "/root/reference/pkg/ragengine"
+POD_CONTRACT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "controller_pod_contract.json")
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_GO), reason="reference tree not present")
 def test_deploy_tree_satisfies_the_controllers_pod_contract():
-    """The literals the unmodified controller puts into the pod spec (pkg/ragengine/manifests/manifests.go:116-134, 146-279;
-    pkg/ragengine/controllers/preset_rag.go:33-64, 186) resolve inside deploy/: hook script path and verbs, `python3 main.py` in
-    the image WORKDIR, port and probe path, and the environment variables the hooks read."""
+    """The literals the unmodified controller puts into the pod spec (tests/golden/controller_pod_contract.json, extracted
+    from pkg/ragengine/manifests/manifests.go:116-134, 146-279 and pkg/ragengine/controllers/preset_rag.go:33-64, 186) resolve
+    inside deploy/: hook script path and verbs, `python3 main.py` in the image WORKDIR, port and probe path, and the
+    environment variables the hooks read."""
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    man = open(os.path.join(REF_GO, "manifests", "manifests.go")).read()
-    pre = open(os.path.join(REF_GO, "controllers", "preset_rag.go")).read()
-    hook_path = re.search(r'"(/app/ragengine/lifecycle/hooks\.py)"', man).group(1)
+    pc = json.load(open(POD_CONTRACT))
+    hook_path = pc["hook_path"]
     assert os.path.isfile(os.path.join(root, "deploy", hook_path.lstrip("/")))
-    assert "python3 /app/ragengine/lifecycle/hooks.py prestop" in man and '"poststart"' in man
+    assert pc["hook_verbs"] == ["poststart", "prestop"]
     hooks_src = open(os.path.join(root, "deploy", hook_path.lstrip("/"))).read()
-    for verb in ("poststart", "prestop"):
+    for verb in pc["hook_verbs"]:
         assert f'"{verb}"' in hooks_src
-    for env in ("POD_NAME", "POD_UID", "DEFAULT_VECTOR_DB_PERSIST_DIR"):
-        assert f'Name:  "{env}"' in man or f'Name: "{env}"' in man
+    assert pc["env"] == ["POD_NAME", "POD_UID", "DEFAULT_VECTOR_DB_PERSIST_DIR"]
+    for env in pc["env"]:
         assert env in hooks_src
-    assert 'utils.ShellCmd("python3 main.py")' in pre and os.path.isfile(os.path.join(root, "deploy", "app", "ragengine", "main.py"))
+    assert pc["command"] == "python3 main.py" and os.path.isfile(os.path.join(root, "deploy", "app", "ragengine", "main.py"))
     dockerfile = open(os.path.join(root, "deploy", "Dockerfile")).read()
-    assert "WORKDIR /app/ragengine" in dockerfile and "python3 main.py" in dockerfile and "EXPOSE 5000" in dockerfile
-    port = int(re.search(r"PortInferenceServer\s*=\s*(\d+)", pre).group(1))
-    probe = re.search(r'ProbePath\s*=\s*"([^"]+)"', pre).group(1)
+    assert "WORKDIR /app/ragengine" in dockerfile and pc["command"] in dockerfile and f"EXPOSE {pc['port']}" in dockerfile
     svc = open(os.path.join(root, "kaito_b200", "service.py")).read()
-    assert f"port={port}" in svc and f'@app.get("{probe}"' in svc
+    assert f"port={pc['port']}" in svc and f'@app.get("{pc["probe_path"]}"' in svc

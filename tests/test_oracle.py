@@ -1,5 +1,5 @@
 """CPU tests: the oracle against the reference-generated golden fixtures and against
-independent restatements.  No GPU, no /root/reference at run time."""
+independent restatements.  No GPU, no reference checkout at run time."""
 import json
 import math
 import os
