@@ -94,6 +94,8 @@ int32_t krag_init(const krag_config* cfg, krag_ctx** out);
 int32_t krag_shutdown(krag_ctx* ctx);
 /* number of kernels this library has launched since krag_init (bench.py gpu_launches) */
 int64_t krag_launch_count(krag_ctx* ctx);
+/* device memory this process currently holds through libkaito_rag, in bytes (every context, index and embedder) */
+int64_t krag_device_bytes(void);
 void* krag_ctx_stream(krag_ctx* ctx);  /* cudaStream_t of search slot 0 (for event timing) */
 
 /* ------------------------------------------------------------------------- index */

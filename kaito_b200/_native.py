@@ -25,7 +25,7 @@ DENSE_AUTO, DENSE_SCAN, DENSE_TC, DENSE_TC_BF16, DENSE_TC_TF32 = 0, 1, 2, 3, 4
 
 # every symbol include/kaito_rag.h declares (tests check the export table against this)
 SYMBOLS = [
-    "krag_version", "krag_last_error", "krag_init", "krag_shutdown", "krag_launch_count", "krag_ctx_stream",
+    "krag_version", "krag_last_error", "krag_init", "krag_shutdown", "krag_launch_count", "krag_device_bytes", "krag_ctx_stream",
     "krag_index_create", "krag_index_drop", "krag_index_reserve", "krag_index_add", "krag_index_remove",
     "krag_index_commit", "krag_index_commit_local", "krag_index_commit_global", "krag_index_stats",
     "krag_index_node_ids", "krag_index_set_ordinal_map", "krag_index_persist", "krag_index_load", "krag_search_dense", "krag_search_bm25",
@@ -80,6 +80,7 @@ def load() -> C.CDLL:
     L.krag_shutdown.argtypes = [vp]
     L.krag_launch_count.argtypes = [vp]
     L.krag_launch_count.restype = i64
+    L.krag_device_bytes.restype = i64
     L.krag_ctx_stream.argtypes = [vp]
     L.krag_ctx_stream.restype = vp
     L.krag_index_create.argtypes = [vp, C.c_char_p, i32, C.POINTER(vp)]
@@ -152,6 +153,11 @@ def last_dense_kernel():
     ms, kid, by, fl = C.c_float(0), C.c_int32(0), C.c_int64(0), C.c_int64(0)
     check(load().krag_last_dense_kernel(C.byref(ms), C.byref(kid), C.byref(by), C.byref(fl)))
     return ms.value, kid.value, by.value, fl.value
+
+
+def device_bytes() -> int:
+    """device memory, in bytes, this process currently holds through the library (every context, index and embedder)"""
+    return int(load().krag_device_bytes())
 
 
 class Context:

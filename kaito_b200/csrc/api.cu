@@ -7,6 +7,7 @@
 
 #include <atomic>
 #include <condition_variable>
+#include <memory>
 #include <mutex>
 #include <shared_mutex>
 #include <string>
@@ -25,6 +26,9 @@ void set_error(const std::string& msg) { g_err = msg; }
 static std::atomic<int64_t> g_launches{0};
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 int64_t launch_count() { return g_launches.load(std::memory_order_relaxed); }
+static std::atomic<int64_t> g_device_bytes{0};
+void count_device_bytes(int64_t delta) { g_device_bytes.fetch_add(delta, std::memory_order_relaxed); }
+int64_t device_bytes() { return g_device_bytes.load(std::memory_order_relaxed); }
 
 // "last dense kernel" diagnostics (krag_last_dense_kernel, read by bench.py).  Process-wide and last-writer-wins: with
 // concurrent searches the numbers describe one of them; the mutex only keeps the record itself consistent.
@@ -87,33 +91,6 @@ static int32_t guarded(F&& f)
     }
 }
 
-// growable device array (copy-on-grow; krag_index_reserve avoids the copies for big corpora)
-template <class T>
-struct DevArray {
-    T* p = nullptr;
-    int64_t cap = 0;
-    void reserve(int64_t n, int64_t used, cudaStream_t st)
-    {
-        if (n <= cap) return;
-        int64_t ncap = cap + cap / 2;
-        if (ncap < n) ncap = n;
-        T* np = nullptr;
-        KRAG_CUDA(cudaMalloc(&np, sizeof(T) * (size_t)ncap));
-        if (p && used > 0) KRAG_CUDA(cudaMemcpyAsync(np, p, sizeof(T) * (size_t)used, cudaMemcpyDeviceToDevice, st));
-        KRAG_CUDA(cudaStreamSynchronize(st));
-        if (p) KRAG_CUDA(cudaFree(p));
-        p = np;
-        cap = ncap;
-    }
-    void release()
-    {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-    }
-    int64_t bytes() const { return (int64_t)sizeof(T) * cap; }
-};
-
 // per-call search workspace
 struct Slot {
     cudaStream_t st = nullptr;
@@ -128,6 +105,7 @@ struct Slot {
     DevArray<int32_t> out_rank, out_count;
     DevArray<int64_t> out_ord;
     std::vector<float> hq;  // padded query staging
+    ~Slot() { if (st) cudaStreamDestroy(st); }
 };
 
 }  // namespace krag
@@ -139,8 +117,10 @@ struct krag_ctx {
     krag_config cfg;
     std::mutex mu;
     std::condition_variable cv;
-    std::vector<Slot*> all_slots, free_slots;
+    std::vector<std::unique_ptr<Slot>> all_slots;
+    std::vector<Slot*> free_slots;
     cudaStream_t admin = nullptr;  // mutation / build stream
+    ~krag_ctx() { if (admin) cudaStreamDestroy(admin); }
 };
 
 struct krag_index {
@@ -308,22 +288,22 @@ void commit_local_impl(krag_index* ix, int64_t vocab, uint32_t* df_out, int64_t*
     KRAG_REQUIRE(vocab > 0 && vocab < 0x7fffffffll, KRAG_E_INVALID, "vocab out of range");
     ix->entry_doc.reserve(ix->nnz > 0 ? ix->nnz : 1, 0, st);
     if (ix->n_rows > 0) launch_expand_entry_doc(ix->toff.p, ix->n_rows, ix->entry_doc.p, st);
-    uint32_t* df = nullptr;
-    KRAG_CUDA(cudaMalloc(&df, sizeof(uint32_t) * (size_t)vocab));
-    KRAG_CUDA(cudaMemsetAsync(df, 0, sizeof(uint32_t) * (size_t)vocab, st));
+    DevArray<uint32_t> df;
+    df.alloc(vocab);
+    KRAG_CUDA(cudaMemsetAsync(df.p, 0, sizeof(uint32_t) * (size_t)vocab, st));
     // term ids >= vocab would make the df kernel write out of bounds: the largest id is tracked on the host at add time
     KRAG_REQUIRE(ix->nnz == 0 || vocab > (int64_t)ix->max_term_id, KRAG_E_INVALID,
                  "vocab must exceed the largest term id added to the index");
     if (ix->nnz > 0) {
-        launch_df_histogram(ix->tid.p, ix->entry_doc.p, alive_ptr(ix), ix->nnz, df, st);
+        launch_df_histogram(ix->tid.p, ix->entry_doc.p, alive_ptr(ix), ix->nnz, df.p, st);
     }
-    KRAG_CUDA(cudaMemcpyAsync(df_out, df, sizeof(uint32_t) * (size_t)vocab, cudaMemcpyDeviceToHost, st));
+    KRAG_CUDA(cudaMemcpyAsync(df_out, df.p, sizeof(uint32_t) * (size_t)vocab, cudaMemcpyDeviceToHost, st));
     // total length over live docs (host side: doc_len is small)
     std::vector<uint32_t> dl((size_t)ix->n_rows);
     if (ix->n_rows > 0)
         KRAG_CUDA(cudaMemcpyAsync(dl.data(), ix->dlen.p, sizeof(uint32_t) * (size_t)ix->n_rows, cudaMemcpyDeviceToHost, st));
     KRAG_CUDA(cudaStreamSynchronize(st));
-    KRAG_CUDA(cudaFree(df));
+    df.release();
     int64_t total = 0, live = 0;
     for (int64_t r = 0; r < ix->n_rows; ++r)
         if ((ix->alive_h[(size_t)(r >> 5)] >> (r & 31)) & 1u) { total += dl[(size_t)r]; ++live; }
@@ -347,18 +327,18 @@ void commit_global_impl(krag_index* ix, int64_t vocab, const uint32_t* df_global
         double dfd = (double)df_global[t];
         idf[(size_t)t] = (float)log(1.0 + ((double)n_docs_global - dfd + 0.5) / (dfd + 0.5));
     }
-    float* d_idf = nullptr;
-    KRAG_CUDA(cudaMalloc(&d_idf, sizeof(float) * (size_t)vocab));
-    KRAG_CUDA(cudaMemcpyAsync(d_idf, idf.data(), sizeof(float) * (size_t)vocab, cudaMemcpyHostToDevice, st));
+    DevArray<float> d_idf;
+    d_idf.alloc(vocab);
+    KRAG_CUDA(cudaMemcpyAsync(d_idf.p, idf.data(), sizeof(float) * (size_t)vocab, cudaMemcpyHostToDevice, st));
     const double avgdl = n_docs_global > 0 ? (double)total_len_global / (double)n_docs_global : 1.0;
     if (ix->entry_doc.cap < (ix->nnz > 0 ? ix->nnz : 1)) {
         ix->entry_doc.reserve(ix->nnz > 0 ? ix->nnz : 1, 0, st);
         if (ix->n_rows > 0) launch_expand_entry_doc(ix->toff.p, ix->n_rows, ix->entry_doc.p, st);
     }
-    build_postings(ix->tid.p, ix->ttf.p, ix->entry_doc.p, ix->dlen.p, alive_ptr(ix), ix->nnz, vocab, d_idf, avgdl,
+    build_postings(ix->tid.p, ix->ttf.p, ix->entry_doc.p, ix->dlen.p, alive_ptr(ix), ix->nnz, vocab, d_idf.p, avgdl,
                    ix->n_rows, ix->post, st);
     KRAG_CUDA(cudaStreamSynchronize(st));
-    KRAG_CUDA(cudaFree(d_idf));
+    d_idf.release();
     ix->entry_doc.release();
     ix->vocab = vocab;
     ix->n_docs_global = n_docs_global;
@@ -390,7 +370,7 @@ int32_t krag_init(const krag_config* cfg, krag_ctx** out)
         KRAG_REQUIRE(p.major == 9 && p.minor == 0, KRAG_E_NO_DEVICE,
                      std::string("device is sm_") + std::to_string(p.major) + std::to_string(p.minor) +
                          "; libkaito_rag is built for sm_90a only");
-        krag_ctx* c = new krag_ctx();
+        auto c = std::make_unique<krag_ctx>();
         c->cfg = *cfg;
         if (c->cfg.world_size <= 0) c->cfg.world_size = 1;
         c->di.device = cfg->device_id;
@@ -401,12 +381,11 @@ int32_t krag_init(const krag_config* cfg, krag_ctx** out)
         KRAG_CUDA(cudaStreamCreateWithFlags(&c->admin, cudaStreamNonBlocking));
         int ns = cfg->search_slots > 0 ? cfg->search_slots : 4;
         for (int i = 0; i < ns; ++i) {
-            Slot* s = new Slot();
-            KRAG_CUDA(cudaStreamCreateWithFlags(&s->st, cudaStreamNonBlocking));
-            c->all_slots.push_back(s);
-            c->free_slots.push_back(s);
+            c->all_slots.push_back(std::make_unique<Slot>());
+            KRAG_CUDA(cudaStreamCreateWithFlags(&c->all_slots.back()->st, cudaStreamNonBlocking));
+            c->free_slots.push_back(c->all_slots.back().get());
         }
-        *out = c;
+        *out = c.release();
     });
 }
 
@@ -416,19 +395,12 @@ int32_t krag_shutdown(krag_ctx* c)
         KRAG_REQUIRE(c, KRAG_E_INVALID, "null context");
         cudaSetDevice(c->di.device);
         cudaDeviceSynchronize();
-        for (Slot* s : c->all_slots) {
-            s->q.release(); s->terms.release(); s->toff.release(); s->dense_keys.release(); s->bm25_keys.release();
-            s->part.release(); s->tc_ws.release(); s->bm25_res.release(); s->allow.release(); s->out_final.release(); s->out_dense.release();
-            s->out_sparse.release(); s->out_rank.release(); s->out_count.release(); s->out_ord.release();
-            cudaStreamDestroy(s->st);
-            delete s;
-        }
-        cudaStreamDestroy(c->admin);
         delete c;
     });
 }
 
 int64_t krag_launch_count(krag_ctx*) { return launch_count(); }
+int64_t krag_device_bytes(void) { return device_bytes(); }
 void* krag_ctx_stream(krag_ctx* c) { return c ? (void*)c->all_slots[0]->st : nullptr; }
 
 int32_t krag_index_create(krag_ctx* c, const char* name, int32_t dim, krag_index** out)
@@ -454,13 +426,6 @@ int32_t krag_index_drop(krag_index* ix)
             std::unique_lock<std::shared_mutex> lk(ix->mu);
             cudaSetDevice(ix->ctx->di.device);
             cudaDeviceSynchronize();
-            ix->X.release(); ix->Xh.release(); ix->xnorm.release(); ix->xn_max.release(); ix->alive_d.release(); ix->toff.release(); ix->tid.release(); ix->ttf.release();
-            ix->dlen.release(); ix->entry_doc.release();
-            if (ix->post.off) cudaFree(ix->post.off);
-            if (ix->post.doc) cudaFree(ix->post.doc);
-            if (ix->post.score) cudaFree(ix->post.score);
-            if (ix->post.tile_slot) cudaFree(ix->post.tile_slot);
-            if (ix->post.tile_off) cudaFree(ix->post.tile_off);
         }
         delete ix;
     });
@@ -825,13 +790,9 @@ int32_t krag_synth_fill(krag_index* ix, int64_t n, int64_t row_base, uint64_t se
         launch_row_norms(ix->X.p, 0, n, ix->dpad, ix->xnorm.p, ix->xn_max.p, st);
         if (ix->Xh.p) launch_f32_to_bf16(ix->X.p, ix->Xh.p, n * ix->dpad, st);
         if (vocab > 0) {
-            int64_t* off = nullptr; uint32_t* ids = nullptr; uint16_t* tf = nullptr; uint32_t* dl = nullptr; int64_t nnz = 0;
-            synth_sparse(n, row_base, seed, vocab, &off, &ids, &tf, &dl, &nnz, st);
-            ix->toff.release(); ix->tid.release(); ix->ttf.release(); ix->dlen.release();
-            ix->toff.p = off; ix->toff.cap = n + 1;
-            ix->tid.p = ids; ix->tid.cap = nnz > 0 ? nnz : 1;
-            ix->ttf.p = tf; ix->ttf.cap = nnz > 0 ? nnz : 1;
-            ix->dlen.p = dl; ix->dlen.cap = n > 0 ? n : 1;
+            DevArray<int64_t> off; DevArray<uint32_t> ids; DevArray<uint16_t> tf; DevArray<uint32_t> dl; int64_t nnz = 0;
+            synth_sparse(n, row_base, seed, vocab, off, ids, tf, dl, &nnz, st);
+            ix->toff = std::move(off); ix->tid = std::move(ids); ix->ttf = std::move(tf); ix->dlen = std::move(dl);
             ix->nnz = nnz;
             ix->max_term_id = (uint32_t)(vocab - 1);     // the generator draws ids in [0, vocab)
             ix->has_sparse = true;
@@ -865,12 +826,12 @@ int32_t krag_index_read_postings(krag_index* ix, uint32_t term, int64_t cap, uin
         KRAG_REQUIRE((int64_t)term < ix->post.vocab, KRAG_E_INVALID, "term id out of range");
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         int64_t be[2];
-        KRAG_CUDA(cudaMemcpy(be, ix->post.off + term, sizeof be, cudaMemcpyDeviceToHost));
+        KRAG_CUDA(cudaMemcpy(be, ix->post.off.p + term, sizeof be, cudaMemcpyDeviceToHost));
         int64_t cnt = be[1] - be[0];
         *n_out = cnt;
         int64_t m = cnt < cap ? cnt : cap;
-        if (m > 0 && docs_out) KRAG_CUDA(cudaMemcpy(docs_out, ix->post.doc + be[0], sizeof(uint32_t) * (size_t)m, cudaMemcpyDeviceToHost));
-        if (m > 0 && scores_out) KRAG_CUDA(cudaMemcpy(scores_out, ix->post.score + be[0], sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost));
+        if (m > 0 && docs_out) KRAG_CUDA(cudaMemcpy(docs_out, ix->post.doc.p + be[0], sizeof(uint32_t) * (size_t)m, cudaMemcpyDeviceToHost));
+        if (m > 0 && scores_out) KRAG_CUDA(cudaMemcpy(scores_out, ix->post.score.p + be[0], sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost));
     });
 }
 
@@ -929,9 +890,9 @@ int32_t krag_debug_tc_dump(krag_index* ix, int32_t nq, const float* q, float* ou
 // ------------------------------------------------------------- peer-memory exchange (one process per GPU)
 struct krag_p2p {
     krag_ctx* ctx; int rank, world, nl, max_batch, max_P; int64_t slot_words;
-    uint64_t* own = nullptr;                 // this rank's mailbox (cudaMalloc, IPC-exported)
+    DevArray<uint64_t> own;                  // this rank's mailbox (IPC-exported)
     std::vector<uint64_t*> peers;            // [world] device pointers: own + IPC-opened peers
-    uint64_t** d_peers = nullptr;            // device copy of the pointer table
+    DevArray<uint64_t*> d_peers;             // device copy of the pointer table
     unsigned long long seq = 0;
 };
 
@@ -940,19 +901,19 @@ int32_t krag_p2p_create(krag_ctx* c, int32_t rank, int32_t world, int32_t max_ba
     return guarded([&] {
         KRAG_REQUIRE(c && out && handle_out && world >= 1 && world <= 64 && rank >= 0 && rank < world, KRAG_E_INVALID, "bad argument");
         KRAG_CUDA(cudaSetDevice(c->di.device));
-        krag_p2p* p = new krag_p2p();
+        auto p = std::make_unique<krag_p2p>();
         p->ctx = c; p->rank = rank; p->world = world; p->nl = 2; p->max_batch = max_batch; p->max_P = max_P;
         p->slot_words = (int64_t)2 * max_batch * max_P;
         const size_t words = p2p_mailbox_words(world, 2, max_batch, max_P);
-        KRAG_CUDA(cudaMalloc(&p->own, words * 8));
-        KRAG_CUDA(cudaMemset(p->own, 0, words * 8));
+        p->own.alloc((int64_t)words);
+        KRAG_CUDA(cudaMemset(p->own.p, 0, words * 8));
         cudaIpcMemHandle_t h;
-        KRAG_CUDA(cudaIpcGetMemHandle(&h, p->own));
+        KRAG_CUDA(cudaIpcGetMemHandle(&h, p->own.p));
         static_assert(sizeof(h) == 64, "cudaIpcMemHandle_t is 64 bytes");
         memcpy(handle_out, &h, 64);
         p->peers.assign((size_t)world, nullptr);
-        p->peers[(size_t)rank] = p->own;
-        *out = p;
+        p->peers[(size_t)rank] = p->own.p;
+        *out = p.release();
     });
 }
 
@@ -969,21 +930,21 @@ int32_t krag_p2p_connect(krag_p2p* p, const uint8_t* handles /*[world][64]*/)
             KRAG_CUDA(cudaIpcOpenMemHandle(&ptr, h, cudaIpcMemLazyEnablePeerAccess));
             p->peers[(size_t)r] = (uint64_t*)ptr;
         }
-        KRAG_CUDA(cudaMalloc(&p->d_peers, sizeof(uint64_t*) * (size_t)p->world));
-        KRAG_CUDA(cudaMemcpy(p->d_peers, p->peers.data(), sizeof(uint64_t*) * (size_t)p->world, cudaMemcpyHostToDevice));
+        p->d_peers.alloc(p->world);
+        KRAG_CUDA(cudaMemcpy(p->d_peers.p, p->peers.data(), sizeof(uint64_t*) * (size_t)p->world, cudaMemcpyHostToDevice));
     });
 }
 
 int32_t krag_dev_exchange_merge(krag_p2p* p, int32_t n_lists, int32_t batch, int32_t P, const uint64_t* d_local, uint64_t* d_merged, void* stream)
 {
     return guarded([&] {
-        KRAG_REQUIRE(p && p->d_peers && d_local && d_merged, KRAG_E_INVALID, "bad argument / not connected");
+        KRAG_REQUIRE(p && p->d_peers.p && d_local && d_merged, KRAG_E_INVALID, "bad argument / not connected");
         KRAG_REQUIRE(n_lists >= 1 && n_lists <= 2 && batch >= 1 && (int64_t)n_lists * batch * P <= p->slot_words, KRAG_E_INVALID,
                      "exchange exceeds the mailbox the ranks agreed on");
         check_P(P);
         KRAG_CUDA(cudaSetDevice(p->ctx->di.device));
         ++p->seq;
-        launch_p2p_exchange_merge(p->d_peers, p->own, p->rank, p->world, p->slot_words, p->seq, n_lists, batch, P, d_local, d_merged,
+        launch_p2p_exchange_merge(p->d_peers.p, p->own.p, p->rank, p->world, p->slot_words, p->seq, n_lists, batch, P, d_local, d_merged,
                                   (cudaStream_t)stream);
     });
 }
@@ -995,8 +956,6 @@ int32_t krag_p2p_destroy(krag_p2p* p)
         cudaSetDevice(p->ctx->di.device);
         cudaDeviceSynchronize();
         for (int r = 0; r < p->world; ++r) if (r != p->rank && p->peers[(size_t)r]) cudaIpcCloseMemHandle(p->peers[(size_t)r]);
-        if (p->d_peers) cudaFree(p->d_peers);
-        if (p->own) cudaFree(p->own);
         delete p;
     });
 }
@@ -1063,23 +1022,19 @@ static void debug_linear(krag_ctx* c, int32_t M, int32_t N, int32_t K, const flo
 {
     KRAG_REQUIRE(c && A && B && bias && out && M >= 1 && N % 128 == 0 && K % 64 == 0, KRAG_E_INVALID, "bad argument (N % 128, K % 64)");
     KRAG_CUDA(cudaSetDevice(c->di.device));
-    float *dA, *dB, *db, *dr = nullptr, *dC, *dY = nullptr, *dg = nullptr, *dlb = nullptr, *ws;
+    DevArray<float> dA, dB, db, dr, dC, dY, dg, dlb, ws;
     const size_t ws_floats = (size_t)4 << 20;
-    KRAG_CUDA(cudaMalloc(&dA, 4 * (size_t)M * K)); KRAG_CUDA(cudaMalloc(&dB, 4 * (size_t)N * K)); KRAG_CUDA(cudaMalloc(&db, 4 * (size_t)N));
-    KRAG_CUDA(cudaMalloc(&dC, 4 * (size_t)M * N)); KRAG_CUDA(cudaMalloc(&ws, 4 * ws_floats));
-    KRAG_CUDA(cudaMemcpy(dA, A, 4 * (size_t)M * K, cudaMemcpyHostToDevice)); KRAG_CUDA(cudaMemcpy(dB, B, 4 * (size_t)N * K, cudaMemcpyHostToDevice));
-    KRAG_CUDA(cudaMemcpy(db, bias, 4 * (size_t)N, cudaMemcpyHostToDevice));
-    if (residual) { KRAG_CUDA(cudaMalloc(&dr, 4 * (size_t)M * N)); KRAG_CUDA(cudaMemcpy(dr, residual, 4 * (size_t)M * N, cudaMemcpyHostToDevice)); }
+    dA.alloc((int64_t)M * K); dB.alloc((int64_t)N * K); db.alloc(N); dC.alloc((int64_t)M * N); ws.alloc((int64_t)ws_floats);
+    KRAG_CUDA(cudaMemcpy(dA.p, A, 4 * (size_t)M * K, cudaMemcpyHostToDevice)); KRAG_CUDA(cudaMemcpy(dB.p, B, 4 * (size_t)N * K, cudaMemcpyHostToDevice));
+    KRAG_CUDA(cudaMemcpy(db.p, bias, 4 * (size_t)N, cudaMemcpyHostToDevice));
+    if (residual) { dr.alloc((int64_t)M * N); KRAG_CUDA(cudaMemcpy(dr.p, residual, 4 * (size_t)M * N, cudaMemcpyHostToDevice)); }
     if (ln_g) {
-        KRAG_CUDA(cudaMalloc(&dg, 4 * (size_t)N)); KRAG_CUDA(cudaMalloc(&dlb, 4 * (size_t)N)); KRAG_CUDA(cudaMalloc(&dY, 4 * (size_t)M * N));
-        KRAG_CUDA(cudaMemcpy(dg, ln_g, 4 * (size_t)N, cudaMemcpyHostToDevice)); KRAG_CUDA(cudaMemcpy(dlb, ln_b, 4 * (size_t)N, cudaMemcpyHostToDevice));
+        dg.alloc(N); dlb.alloc(N); dY.alloc((int64_t)M * N);
+        KRAG_CUDA(cudaMemcpy(dg.p, ln_g, 4 * (size_t)N, cudaMemcpyHostToDevice)); KRAG_CUDA(cudaMemcpy(dlb.p, ln_b, 4 * (size_t)N, cudaMemcpyHostToDevice));
     }
-    launch_linear_f32(c->di, dA, dB, M, N, K, db, dr, gelu != 0, dC, dg, dlb, eps, dY, ws, ws_floats, c->admin);
+    launch_linear_f32(c->di, dA.p, dB.p, M, N, K, db.p, dr.p, gelu != 0, dC.p, dg.p, dlb.p, eps, dY.p, ws.p, ws_floats, c->admin);
     KRAG_CUDA(cudaStreamSynchronize(c->admin));
-    KRAG_CUDA(cudaMemcpy(out, ln_g ? dY : dC, 4 * (size_t)M * N, cudaMemcpyDeviceToHost));
-    cudaFree(dA); cudaFree(dB); cudaFree(db); cudaFree(dC); cudaFree(ws);
-    if (dr) cudaFree(dr);
-    if (dg) { cudaFree(dg); cudaFree(dlb); cudaFree(dY); }
+    KRAG_CUDA(cudaMemcpy(out, ln_g ? dY.p : dC.p, 4 * (size_t)M * N, cudaMemcpyDeviceToHost));
 }
 
 int32_t krag_debug_gemm_tf32(krag_ctx* c, int32_t M, int32_t N, int32_t K, const float* A, const float* B, const float* bias,

@@ -177,67 +177,35 @@ __global__ void tile_index_kernel(const uint32_t* __restrict__ sorted_terms, con
         if (p == e - 1) for (int64_t tl = tile_d + 1; tl <= n_tiles; ++tl) row[tl] = (uint32_t)(e - b);
     }
 }
-// device scratch of the index build: everything allocated through it is freed on scope exit (also when a CUDA call
-// throws half-way), except what keep() hands over to the Postings
-struct DevScratch {
-    std::vector<void*> ptrs;
-    template <typename T> T* alloc(size_t n)
-    {
-        void* p = nullptr;
-        const size_t bytes = sizeof(T) * (n ? n : 1);
-        const cudaError_t e = cudaMalloc(&p, bytes);
-        if (e == cudaErrorMemoryAllocation) {          // say how much was asked for and what was left: the build is the memory peak
-            cudaGetLastError();
-            size_t free_b = 0, total_b = 0;
-            cudaMemGetInfo(&free_b, &total_b);
-            char msg[256];
-            snprintf(msg, sizeof msg, "bm25 index build: out of device memory (wanted %.2f GB, %.2f of %.2f GB free)", bytes / 1e9, free_b / 1e9,
-                     total_b / 1e9);
-            throw DevOom{msg};
-        }
-        KRAG_CUDA(e);
-        ptrs.push_back(p);
-        return static_cast<T*>(p);
-    }
-    void free_now(void* p)
-    {
-        for (auto& q : ptrs) if (q == p && q) { cudaFree(q); q = nullptr; }
-    }
-    template <typename T> T* keep(T* p)
-    {
-        for (auto& q : ptrs) if (q == static_cast<void*>(p)) q = nullptr;
-        return p;
-    }
-    ~DevScratch() { for (void* p : ptrs) if (p) cudaFree(p); }
-};
+// cub temporary storage: never a null pointer, which cub would take for a size query
+static size_t cub_tmp_bytes(size_t bytes) { return bytes ? bytes : 1; }
 
 // slots of the frequent terms (df > BM25_RARE_MAX) and the (still empty) boundary table; filled range by range below
 static void prepare_tile_index(const int64_t* off, int64_t vocab, int64_t n_rows, Postings& out, cudaStream_t st)
 {
-    DevScratch sc;
-    int32_t* flag = sc.alloc<int32_t>((size_t)(vocab + 1));
-    int32_t* scan = sc.alloc<int32_t>((size_t)(vocab + 1));
-    int32_t* slot = sc.alloc<int32_t>((size_t)vocab);
-    tile_flag_kernel<<<256, 256, 0, st>>>(off, vocab, flag);
+    DevArray<int32_t> flag, scan, slot;
+    flag.alloc(vocab + 1);
+    scan.alloc(vocab + 1);
+    slot.alloc(vocab);
+    tile_flag_kernel<<<256, 256, 0, st>>>(off, vocab, flag.p);
     count_launch();
     size_t bytes = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, bytes, flag, scan, (int)(vocab + 1), st);
-    void* tmp = sc.alloc<unsigned char>(bytes);
-    cub::DeviceScan::ExclusiveSum(tmp, bytes, flag, scan, (int)(vocab + 1), st);
+    cub::DeviceScan::ExclusiveSum(nullptr, bytes, flag.p, scan.p, (int)(vocab + 1), st);
+    DevArray<unsigned char> tmp;
+    tmp.alloc(cub_tmp_bytes(bytes));
+    cub::DeviceScan::ExclusiveSum(tmp.p, bytes, flag.p, scan.p, (int)(vocab + 1), st);
     count_launch();
-    tile_slot_kernel<<<256, 256, 0, st>>>(flag, scan, vocab, slot);
+    tile_slot_kernel<<<256, 256, 0, st>>>(flag.p, scan.p, vocab, slot.p);
     count_launch();
     int32_t n_slots = 0;
-    KRAG_CUDA(cudaMemcpyAsync(&n_slots, scan + vocab, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    KRAG_CUDA(cudaMemcpyAsync(&n_slots, scan.p + vocab, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     KRAG_CUDA(cudaStreamSynchronize(st));
-    sc.free_now(tmp); sc.free_now(flag); sc.free_now(scan);
+    tmp.release(); flag.release(); scan.release();
     int64_t n_tiles = (n_rows + BM25_SUB_DOCS - 1) / BM25_SUB_DOCS;
     if (n_tiles < 1) n_tiles = 1;
-    uint32_t* tile_off = sc.alloc<uint32_t>((size_t)((int64_t)(n_slots > 0 ? n_slots : 1) * (n_tiles + 1)));
-    if (out.tile_slot) cudaFree(out.tile_slot);
-    if (out.tile_off) cudaFree(out.tile_off);
-    sc.keep(slot); sc.keep(tile_off);
-    out.tile_slot = slot; out.tile_off = tile_off; out.n_slots = n_slots; out.n_tiles = n_tiles;
+    DevArray<uint32_t> tile_off;
+    tile_off.alloc((int64_t)(n_slots > 0 ? n_slots : 1) * (n_tiles + 1));
+    out.tile_slot = std::move(slot); out.tile_off = std::move(tile_off); out.n_slots = n_slots; out.n_tiles = n_tiles;
 }
 
 // postings per term range of the build: KRAG_BM25_BUILD_CHUNK, else what fits in 70 % of the free device memory at 24 bytes
@@ -262,47 +230,53 @@ void build_postings(const uint32_t* term_ids, const uint16_t* term_tf, const uin
                     double avgdl, int64_t n_docs_rows, Postings& out, cudaStream_t st)
 {
     // local df (live docs only) -> exclusive scan -> offsets
-    DevScratch sc;
-    uint32_t* df_local = sc.alloc<uint32_t>((size_t)(vocab + 1));
-    KRAG_CUDA(cudaMemsetAsync(df_local, 0, sizeof(uint32_t) * (size_t)(vocab + 1), st));
-    launch_df_histogram(term_ids, entry_doc, alive, nnz, df_local, st);
-    int64_t* off = sc.alloc<int64_t>((size_t)(vocab + 1));
-    int64_t* tmp64 = sc.alloc<int64_t>((size_t)(vocab + 1));
-    df_to_i64_kernel<<<256, 256, 0, st>>>(df_local, vocab, tmp64);
+    DevArray<uint32_t> df_local;
+    df_local.alloc(vocab + 1);
+    KRAG_CUDA(cudaMemsetAsync(df_local.p, 0, sizeof(uint32_t) * (size_t)(vocab + 1), st));
+    launch_df_histogram(term_ids, entry_doc, alive, nnz, df_local.p, st);
+    DevArray<int64_t> off, tmp64;
+    off.alloc(vocab + 1);
+    tmp64.alloc(vocab + 1);
+    df_to_i64_kernel<<<256, 256, 0, st>>>(df_local.p, vocab, tmp64.p);
     count_launch();
     size_t scan_bytes = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, tmp64, off, (int)(vocab + 1), st);
-    void* scan_tmp = sc.alloc<unsigned char>(scan_bytes);
-    cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, tmp64, off, (int)(vocab + 1), st);
+    cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, tmp64.p, off.p, (int)(vocab + 1), st);
+    DevArray<unsigned char> scan_tmp;
+    scan_tmp.alloc(cub_tmp_bytes(scan_bytes));
+    cub::DeviceScan::ExclusiveSum(scan_tmp.p, scan_bytes, tmp64.p, off.p, (int)(vocab + 1), st);
     count_launch();
     std::vector<int64_t> h_off((size_t)(vocab + 1));
-    KRAG_CUDA(cudaMemcpyAsync(h_off.data(), off, sizeof(int64_t) * (size_t)(vocab + 1), cudaMemcpyDeviceToHost, st));
+    KRAG_CUDA(cudaMemcpyAsync(h_off.data(), off.p, sizeof(int64_t) * (size_t)(vocab + 1), cudaMemcpyDeviceToHost, st));
     KRAG_CUDA(cudaStreamSynchronize(st));
     const int64_t nnz_live = h_off[(size_t)vocab];
-    sc.free_now(scan_tmp); sc.free_now(tmp64); sc.free_now(df_local);
+    scan_tmp.release(); tmp64.release(); df_local.release();
 
-    uint32_t* post_doc = sc.alloc<uint32_t>((size_t)(nnz_live > 0 ? nnz_live : 1));
-    float* post_score = sc.alloc<float>((size_t)(nnz_live > 0 ? nnz_live : 1));
+    DevArray<uint32_t> post_doc;
+    DevArray<float> post_score;
+    post_doc.alloc(nnz_live > 0 ? nnz_live : 1);
+    post_score.alloc(nnz_live > 0 ? nnz_live : 1);
 
     if (nnz > 0 && nnz_live > 0) {
-        prepare_tile_index(off, vocab, n_docs_rows, out, st);
+        prepare_tile_index(off.p, vocab, n_docs_rows, out, st);
         // term ranges [t_lo, t_hi) of at most `cap` postings each (a single term longer than that is a range of its own).  The
         // sort buffers are sized for the widest range; if they do not fit after all (fragmentation, another context on the
         // device), the ranges are halved until they do
         int64_t cap = build_chunk_cap(nnz_live);
         const int64_t n_blocks = (nnz + (int64_t)CC_THREADS * CC_ITEMS - 1) / ((int64_t)CC_THREADS * CC_ITEMS);
         if (n_blocks >= ((int64_t)1 << 31)) throw std::runtime_error("bm25 build: too many index entries on one shard");
-        uint32_t* block_cnt = sc.alloc<uint32_t>((size_t)n_blocks);
-        uint32_t* block_off = sc.alloc<uint32_t>((size_t)n_blocks);
+        DevArray<uint32_t> block_cnt, block_off;
+        block_cnt.alloc(n_blocks);
+        block_off.alloc(n_blocks);
         size_t bscan_bytes = 0;
-        cub::DeviceScan::ExclusiveSum(nullptr, bscan_bytes, block_cnt, block_off, (int)n_blocks, st);
-        void* bscan_tmp = sc.alloc<unsigned char>(bscan_bytes);
+        cub::DeviceScan::ExclusiveSum(nullptr, bscan_bytes, block_cnt.p, block_off.p, (int)n_blocks, st);
+        DevArray<unsigned char> bscan_tmp;
+        bscan_tmp.alloc(cub_tmp_bytes(bscan_bytes));
         int end_bit = 1;
         while (((int64_t)1 << end_bit) < vocab) ++end_bit;  // keys range over [0, vocab)
         std::vector<int64_t> cuts;
-        uint32_t *k_in = nullptr, *k_out = nullptr;
-        uint64_t *v_in = nullptr, *v_out = nullptr;
-        void* sort_tmp = nullptr;
+        DevArray<uint32_t> k_in, k_out;
+        DevArray<uint64_t> v_in, v_out;
+        DevArray<unsigned char> sort_tmp;
         size_t sort_bytes = 0;
         for (;;) {
             cuts.assign(1, 0);
@@ -318,17 +292,16 @@ void build_postings(const uint32_t* term_ids, const uint16_t* term_tf, const uin
             if (widest >= ((int64_t)1 << 31)) throw std::runtime_error("bm25 build: a single term has too many postings for one build range");
             try {
                 // stable LSD radix sort by term id keeps documents ascending inside every term
-                k_in = sc.alloc<uint32_t>((size_t)widest);
-                k_out = sc.alloc<uint32_t>((size_t)widest);
-                v_in = sc.alloc<uint64_t>((size_t)widest);
-                v_out = sc.alloc<uint64_t>((size_t)widest);
+                k_in.alloc(widest);
+                k_out.alloc(widest);
+                v_in.alloc(widest);
+                v_out.alloc(widest);
                 sort_bytes = 0;
-                cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, k_in, k_out, v_in, v_out, widest, 0, end_bit, st);
-                sort_tmp = sc.alloc<unsigned char>(sort_bytes);
+                cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, k_in.p, k_out.p, v_in.p, v_out.p, widest, 0, end_bit, st);
+                sort_tmp.alloc(cub_tmp_bytes(sort_bytes));
                 break;
             } catch (const DevOom&) {
-                sc.free_now(k_in); sc.free_now(k_out); sc.free_now(v_in); sc.free_now(v_out);
-                k_in = k_out = nullptr; v_in = v_out = nullptr;
+                k_in.release(); k_out.release(); v_in.release(); v_out.release();
                 if (cap <= ((int64_t)1 << 22) || widest > cap) throw;      // cannot get smaller: the widest range is one term
                 cap /= 2;
             }
@@ -338,22 +311,22 @@ void build_postings(const uint32_t* term_ids, const uint16_t* term_tf, const uin
             const int64_t p_base = h_off[(size_t)t_lo], m = h_off[(size_t)t_hi] - p_base;
             if (m == 0) continue;
             chunk_count_kernel<<<(unsigned)n_blocks, CC_THREADS, 0, st>>>(term_ids, entry_doc, alive, nnz, (uint32_t)t_lo, (uint32_t)t_hi,
-                                                                         block_cnt);
+                                                                         block_cnt.p);
             KRAG_CUDA(cudaGetLastError());
             count_launch();
-            cub::DeviceScan::ExclusiveSum(bscan_tmp, bscan_bytes, block_cnt, block_off, (int)n_blocks, st);
+            cub::DeviceScan::ExclusiveSum(bscan_tmp.p, bscan_bytes, block_cnt.p, block_off.p, (int)n_blocks, st);
             count_launch();
             chunk_scatter_kernel<<<(unsigned)n_blocks, CC_THREADS, 0, st>>>(term_ids, term_tf, entry_doc, alive, nnz, (uint32_t)t_lo,
-                                                                           (uint32_t)t_hi, block_off, k_in, v_in);
+                                                                           (uint32_t)t_hi, block_off.p, k_in.p, v_in.p);
             KRAG_CUDA(cudaGetLastError());
             count_launch();
             size_t sb = sort_bytes;
-            cub::DeviceRadixSort::SortPairs(sort_tmp, sb, k_in, k_out, v_in, v_out, m, 0, end_bit, st);
+            cub::DeviceRadixSort::SortPairs(sort_tmp.p, sb, k_in.p, k_out.p, v_in.p, v_out.p, m, 0, end_bit, st);
             count_launch();
-            score_postings_kernel<<<132 * 8, 256, 0, st>>>(k_out, v_out, doc_len, idf, avgdl, m, post_doc + p_base, post_score + p_base);
+            score_postings_kernel<<<132 * 8, 256, 0, st>>>(k_out.p, v_out.p, doc_len, idf, avgdl, m, post_doc.p + p_base, post_score.p + p_base);
             count_launch();
             if (out.n_slots > 0) {
-                tile_index_kernel<<<132 * 8, 256, 0, st>>>(k_out, post_doc, off, out.tile_slot, p_base, m, out.n_tiles, out.tile_off);
+                tile_index_kernel<<<132 * 8, 256, 0, st>>>(k_out.p, post_doc.p, off.p, out.tile_slot.p, p_base, m, out.n_tiles, out.tile_off.p);
                 KRAG_CUDA(cudaGetLastError());
                 count_launch();
             }
@@ -361,19 +334,15 @@ void build_postings(const uint32_t* term_ids, const uint16_t* term_tf, const uin
         KRAG_CUDA(cudaStreamSynchronize(st));
     }
     if (nnz_live == 0 || nnz == 0) {   // no postings: every term is "rare" with an empty list
-        int32_t* slot = sc.alloc<int32_t>((size_t)vocab);
-        KRAG_CUDA(cudaMemset(slot, 0xFF, sizeof(int32_t) * (size_t)vocab));
-        uint32_t* toff = sc.alloc<uint32_t>(4);
-        if (out.tile_slot) cudaFree(out.tile_slot);
-        if (out.tile_off) cudaFree(out.tile_off);
-        out.tile_slot = sc.keep(slot); out.tile_off = sc.keep(toff); out.n_slots = 0;
+        DevArray<int32_t> slot;
+        slot.alloc(vocab);
+        KRAG_CUDA(cudaMemset(slot.p, 0xFF, sizeof(int32_t) * (size_t)vocab));
+        DevArray<uint32_t> toff;
+        toff.alloc(4);
+        out.tile_slot = std::move(slot); out.tile_off = std::move(toff); out.n_slots = 0;
         out.n_tiles = (n_docs_rows + BM25_SUB_DOCS - 1) / BM25_SUB_DOCS < 1 ? 1 : (n_docs_rows + BM25_SUB_DOCS - 1) / BM25_SUB_DOCS;
     }
-    if (out.off) cudaFree(out.off);
-    if (out.doc) cudaFree(out.doc);
-    if (out.score) cudaFree(out.score);
-    sc.keep(off); sc.keep(post_doc); sc.keep(post_score);
-    out.off = off; out.doc = post_doc; out.score = post_score; out.vocab = vocab; out.nnz = nnz_live;
+    out.off = std::move(off); out.doc = std::move(post_doc); out.score = std::move(post_score); out.vocab = vocab; out.nnz = nnz_live;
 }
 
 // -------------------------------------------------------------------------- query time
@@ -1085,7 +1054,7 @@ void launch_bm25(const DeviceInfo& di, const Postings& post, int64_t n_rows, con
     int32_t* q_rare = q_slot + nt;
     uint32_t* scratch_rows = reinterpret_cast<uint32_t*>(q_rare + nt);
     if (n_terms_total > 0) {
-        bm25_resolve_kernel<<<n_terms_total, 256, 0, st>>>(q_terms, n_terms_total, post.off, post.doc, post.tile_slot, post.tile_off,
+        bm25_resolve_kernel<<<n_terms_total, 256, 0, st>>>(q_terms, n_terms_total, post.off.p, post.doc.p, post.tile_slot.p, post.tile_off.p,
                                                            post.vocab, n_sub, scratch_rows, q_row, q_base, q_slot, q_rare);
         KRAG_CUDA(cudaGetLastError());
         count_launch();
@@ -1116,7 +1085,7 @@ void launch_bm25(const DeviceInfo& di, const Postings& post, int64_t n_rows, con
             const long long want = (units + BW_WARPS - 1) / BW_WARPS;
             const long long max_grid = 2LL * di.sm_count;
             const int grid = (int)(want < max_grid ? (want > 0 ? want : 1) : max_grid);
-            bm25_warp_kernel<<<grid, BW_THREADS, smem, st>>>(post.doc, post.score, q_term_offsets, q_row, q_base, n_rows, alive, ord_base,
+            bm25_warp_kernel<<<grid, BW_THREADS, smem, st>>>(post.doc.p, post.score.p, q_term_offsets, q_row, q_base, n_rows, alive, ord_base,
                                                              batch, n_s, stride, thr, cand, cand_cnt, L.capq, counter);
             KRAG_CUDA(cudaGetLastError());
             count_launch();
@@ -1157,7 +1126,7 @@ void launch_bm25(const DeviceInfo& di, const Postings& post, int64_t n_rows, con
         const int64_t max_grid = (int64_t)per_sm * di.sm_count;
         const int grid = (int)(n_items < max_grid ? n_items : max_grid);
         const uint32_t* only = legacy_only ? nullptr : flags;
-        bm25_tile_kernel<<<grid, BQ_THREADS, smem, st>>>(post.off, post.doc, post.score, post.tile_slot, post.tile_off,
+        bm25_tile_kernel<<<grid, BQ_THREADS, smem, st>>>(post.off.p, post.doc.p, post.score.p, post.tile_slot.p, post.tile_off.p,
                                                          post.n_tiles, post.vocab, q_terms, q_term_offsets, q_slot, q_base, q_rare, n_rows,
                                                          alive, P, cap, ord_base, batch, (int)L.n_tiles, bq_group(), part + L.legacy_part, g_thr, only);
         KRAG_CUDA(cudaGetLastError());

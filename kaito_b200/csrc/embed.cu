@@ -18,6 +18,7 @@
 #include <stdlib.h>
 
 #include <map>
+#include <memory>
 #include <stdexcept>
 #include <tuple>
 #include <string>
@@ -1072,28 +1073,25 @@ void launch_linear_f32(const DeviceInfo& di, const float* A, const float* B, int
                        bool gelu, float* C, const float* ln_g, const float* ln_b, float eps, float* Y, float* ws, size_t ws_floats,
                        cudaStream_t st)
 {
-    uint16_t* planes = nullptr;
     const size_t na = (size_t)M * K, nb = (size_t)N * K;
-    KRAG_CUDA(cudaMalloc(&planes, 2 * (2 * na + 2 * nb)));
-    SplitMat As{planes, planes + na}, Bs{planes + 2 * na, planes + 2 * na + nb};
-    try {
-        launch_split_f16(A, As.hi, As.lo, (int64_t)na, st);
-        launch_split_f16(B, Bs.hi, Bs.lo, (int64_t)nb, st);
-        launch_linear(di, As, Bs, M, N, K, bias, residual, gelu, C, nullptr, nullptr, ln_g, ln_b, eps, Y, nullptr, nullptr, ws, ws_floats, st);
-        KRAG_CUDA(cudaStreamSynchronize(st));
-    } catch (...) { cudaFree(planes); throw; }
-    cudaFree(planes);
+    DevArray<uint16_t> planes;
+    planes.alloc((int64_t)(2 * na + 2 * nb));
+    SplitMat As{planes.p, planes.p + na}, Bs{planes.p + 2 * na, planes.p + 2 * na + nb};
+    launch_split_f16(A, As.hi, As.lo, (int64_t)na, st);
+    launch_split_f16(B, Bs.hi, Bs.lo, (int64_t)nb, st);
+    launch_linear(di, As, Bs, M, N, K, bias, residual, gelu, C, nullptr, nullptr, ln_g, ln_b, eps, Y, nullptr, nullptr, ws, ws_floats, st);
+    KRAG_CUDA(cudaStreamSynchronize(st));
 }
 
 
 struct Embedder {
     DeviceInfo di;
     BertConfig cfg;
-    std::map<std::string, float*> t;      // HF tensor name -> device copy
-    std::vector<float*> bqkv;             // fused Q|K|V bias per layer (finalize)
+    std::map<std::string, DevArray<float>> t;   // HF tensor name -> device copy
+    std::vector<DevArray<float>> bqkv;          // fused Q|K|V bias per layer (finalize)
     // split fp16 planes of the GEMM weights (finalize): per layer QKV (fused), attention output, FFN1, FFN2
     std::vector<SplitMat> s_qkv, s_o, s_f1, s_f2;
-    std::vector<uint16_t*> planes;        // owning pointers of all weight planes
+    std::vector<DevArray<uint16_t>> planes;     // the buffers all weight planes live in
     bool finalized = false;
     cudaStream_t st = nullptr;
     cudaEvent_t done = nullptr, in_ev = nullptr;
@@ -1101,19 +1099,32 @@ struct Embedder {
     std::map<std::tuple<int, int, int>, int> seen;
     // workspaces, grown on demand
     int cap_tok = 0, cap_batch = 0;
-    int32_t *d_tok = nullptr, *d_pos = nullptr, *d_off = nullptr;
-    float *x = nullptr, *x2 = nullptr, *qkv = nullptr, *out = nullptr;
-    uint16_t *xs = nullptr, *cs = nullptr, *fs = nullptr;   // split planes [2][T][*] of x (LayerNorm outputs), attention context, FFN1 output
-    float* ws = nullptr;                  // split-K partials (small token counts)
+    DevArray<int32_t> d_tok, d_pos, d_off;
+    DevArray<float> x, x2, qkv, out;
+    DevArray<uint16_t> xs, cs, fs;        // split planes [2][T][*] of x (LayerNorm outputs), attention context, FFN1 output
+    DevArray<float> ws;                   // split-K partials (small token counts)
     static constexpr size_t WS_FLOATS = (size_t)4 << 20;
+
+    void drop_graphs()
+    {
+        for (auto& kv : graphs) cudaGraphExecDestroy(kv.second);
+        graphs.clear();
+    }
+    ~Embedder()
+    {
+        drop_graphs();
+        if (done) cudaEventDestroy(done);
+        if (in_ev) cudaEventDestroy(in_ev);
+        if (st) cudaStreamDestroy(st);
+    }
 };
 
 static float* emb_get(Embedder* e, const std::string& name, int64_t n)
 {
     auto it = e->t.find(name);
-    if (it == e->t.end() || it->second == nullptr) throw std::runtime_error("embedder: tensor not loaded: " + name);
+    if (it == e->t.end() || it->second.p == nullptr) throw std::runtime_error("embedder: tensor not loaded: " + name);
     (void)n;
-    return it->second;
+    return it->second.p;
 }
 static std::string lname(int l, const char* s) { return "encoder.layer." + std::to_string(l) + "." + s; }
 
@@ -1121,29 +1132,27 @@ Embedder* embedder_create(const DeviceInfo& di, const BertConfig& cfg)
 {
     if (cfg.hidden % 128 || cfg.inter % 128 || cfg.hidden % cfg.heads || cfg.hidden / cfg.heads > 64 || (cfg.hidden / cfg.heads) % 32 || cfg.hidden > 1024)
         throw std::runtime_error("embedder: hidden/intermediate must be multiples of 128, hidden <= 1024 and head_dim 32 or 64");
-    Embedder* e = new Embedder();
+    auto e = std::make_unique<Embedder>();
     e->di = di; e->cfg = cfg;
     KRAG_CUDA(cudaStreamCreateWithFlags(&e->st, cudaStreamNonBlocking));
-    return e;
+    return e.release();
 }
 
 void embedder_load(Embedder* e, const char* name, const float* data, int64_t n)
 {
-    float* p = nullptr;
-    KRAG_CUDA(cudaMalloc(&p, sizeof(float) * (size_t)n));
-    KRAG_CUDA(cudaMemcpy(p, data, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice));
-    auto it = e->t.find(name);
-    if (it != e->t.end()) cudaFree(it->second);
-    e->t[name] = p;
+    DevArray<float> p;
+    p.alloc(n);
+    KRAG_CUDA(cudaMemcpy(p.p, data, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice));
+    e->t[name] = std::move(p);
     e->finalized = false;
 }
 
 static SplitMat emb_split_weight(Embedder* e, const float* w, size_t n)
 {
-    uint16_t* p = nullptr;
-    KRAG_CUDA(cudaMalloc(&p, 2 * 2 * n));
-    e->planes.push_back(p);
-    SplitMat m{p, p + n};
+    DevArray<uint16_t> p;
+    p.alloc((int64_t)(2 * n));
+    SplitMat m{p.p, p.p + n};
+    e->planes.push_back(std::move(p));
     launch_split_f16(w, m.hi, m.lo, (int64_t)n, e->st);
     return m;
 }
@@ -1151,26 +1160,24 @@ static SplitMat emb_split_weight(Embedder* e, const float* w, size_t n)
 void embedder_finalize(Embedder* e)
 {
     const int d = e->cfg.hidden, inter = e->cfg.inter;
-    for (float* p : e->bqkv) cudaFree(p);
-    for (uint16_t* p : e->planes) cudaFree(p);
+    e->finalized = false;
     e->bqkv.clear(); e->planes.clear(); e->s_qkv.clear(); e->s_o.clear(); e->s_f1.clear(); e->s_f2.clear();
-    for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second);   // captured weight pointers are about to change
-    e->graphs.clear(); e->seen.clear();
+    e->drop_graphs(); e->seen.clear();   // captured weight pointers are about to change
     emb_get(e, "embeddings.word_embeddings.weight", 0); emb_get(e, "embeddings.position_embeddings.weight", 0);
     emb_get(e, "embeddings.token_type_embeddings.weight", 0); emb_get(e, "embeddings.LayerNorm.weight", 0);
     emb_get(e, "embeddings.LayerNorm.bias", 0);
-    float* wtmp = nullptr;
-    KRAG_CUDA(cudaMalloc(&wtmp, sizeof(float) * (size_t)3 * d * d));
+    DevArray<float> wtmp;
+    wtmp.alloc((int64_t)3 * d * d);
     for (int l = 0; l < e->cfg.layers; ++l) {
-        float* b = nullptr;
-        KRAG_CUDA(cudaMalloc(&b, sizeof(float) * (size_t)3 * d));
+        DevArray<float> b;
+        b.alloc((int64_t)3 * d);
         const char* names[3] = {"attention.self.query", "attention.self.key", "attention.self.value"};
         for (int j = 0; j < 3; ++j) {
-            KRAG_CUDA(cudaMemcpyAsync(wtmp + (size_t)j * d * d, emb_get(e, lname(l, names[j]) + ".weight", 0), sizeof(float) * (size_t)d * d, cudaMemcpyDeviceToDevice, e->st));
-            KRAG_CUDA(cudaMemcpyAsync(b + (size_t)j * d, emb_get(e, lname(l, names[j]) + ".bias", 0), sizeof(float) * (size_t)d, cudaMemcpyDeviceToDevice, e->st));
+            KRAG_CUDA(cudaMemcpyAsync(wtmp.p + (size_t)j * d * d, emb_get(e, lname(l, names[j]) + ".weight", 0), sizeof(float) * (size_t)d * d, cudaMemcpyDeviceToDevice, e->st));
+            KRAG_CUDA(cudaMemcpyAsync(b.p + (size_t)j * d, emb_get(e, lname(l, names[j]) + ".bias", 0), sizeof(float) * (size_t)d, cudaMemcpyDeviceToDevice, e->st));
         }
-        e->bqkv.push_back(b);
-        e->s_qkv.push_back(emb_split_weight(e, wtmp, (size_t)3 * d * d));       // stream order: the split reads wtmp before the next layer overwrites it
+        e->bqkv.push_back(std::move(b));
+        e->s_qkv.push_back(emb_split_weight(e, wtmp.p, (size_t)3 * d * d));       // stream order: the split reads wtmp before the next layer overwrites it
         for (const char* nm : {"attention.output.dense.bias", "attention.output.LayerNorm.weight", "attention.output.LayerNorm.bias",
                                "intermediate.dense.bias", "output.dense.bias", "output.LayerNorm.weight", "output.LayerNorm.bias"})
             emb_get(e, lname(l, nm), 0);
@@ -1179,32 +1186,19 @@ void embedder_finalize(Embedder* e)
         e->s_f2.push_back(emb_split_weight(e, emb_get(e, lname(l, "output.dense.weight"), 0), (size_t)d * inter));
     }
     KRAG_CUDA(cudaStreamSynchronize(e->st));
-    cudaFree(wtmp);
+    wtmp.release();
     // the fp32 copies of the GEMM weights are not read again: free them (the split planes hold the same bytes per element)
     for (int l = 0; l < e->cfg.layers; ++l)
         for (const char* nm : {"attention.self.query.weight", "attention.self.key.weight", "attention.self.value.weight",
                                "attention.output.dense.weight", "intermediate.dense.weight", "output.dense.weight"}) {
             auto it = e->t.find(lname(l, nm));
-            if (it != e->t.end() && it->second) { cudaFree(it->second); it->second = nullptr; }
+            if (it != e->t.end()) it->second.release();
         }
-    if (!e->ws) KRAG_CUDA(cudaMalloc(&e->ws, sizeof(float) * Embedder::WS_FLOATS));
+    if (!e->ws.p) e->ws.alloc((int64_t)Embedder::WS_FLOATS);
     e->finalized = true;
 }
 
-void embedder_destroy(Embedder* e)
-{
-    for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second);
-    for (auto& kv : e->t) if (kv.second) cudaFree(kv.second);
-    for (float* p : e->bqkv) cudaFree(p);
-    for (uint16_t* p : e->planes) cudaFree(p);
-    for (void* p : {(void*)e->d_tok, (void*)e->d_pos, (void*)e->d_off, (void*)e->x, (void*)e->x2, (void*)e->qkv, (void*)e->xs, (void*)e->cs, (void*)e->fs, (void*)e->out})
-        if (p) cudaFree(p);
-    if (e->ws) cudaFree(e->ws);
-    if (e->done) cudaEventDestroy(e->done);
-    if (e->in_ev) cudaEventDestroy(e->in_ev);
-    if (e->st) cudaStreamDestroy(e->st);
-    delete e;
-}
+void embedder_destroy(Embedder* e) { delete e; }
 
 int embedder_hidden(const Embedder* e) { return e->cfg.hidden; }
 
@@ -1228,31 +1222,33 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
         for (int i = 0; i < len; ++i) pos[(size_t)tok_offsets[b] + i] = i;
     }
     if (n_tok > e->cap_tok || batch > e->cap_batch) {
-        for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second);   // captured pointers are about to change
-        e->graphs.clear(); e->seen.clear();
+        const int64_t T = n_tok > e->cap_tok ? n_tok : e->cap_tok, Bc = batch > e->cap_batch ? batch : e->cap_batch;
+        e->drop_graphs(); e->seen.clear();   // captured pointers are about to change
         KRAG_CUDA(cudaStreamSynchronize(st));
-        for (void* p : {(void*)e->d_tok, (void*)e->d_pos, (void*)e->d_off, (void*)e->x, (void*)e->x2, (void*)e->qkv, (void*)e->xs, (void*)e->cs, (void*)e->fs, (void*)e->out})
-            if (p) cudaFree(p);
-        const size_t T = (size_t)(n_tok > e->cap_tok ? n_tok : e->cap_tok), Bc = (size_t)(batch > e->cap_batch ? batch : e->cap_batch);
-        KRAG_CUDA(cudaMalloc(&e->d_tok, 4 * T)); KRAG_CUDA(cudaMalloc(&e->d_pos, 4 * T)); KRAG_CUDA(cudaMalloc(&e->d_off, 4 * (Bc + 1)));
-        KRAG_CUDA(cudaMalloc(&e->x, 4 * T * d)); KRAG_CUDA(cudaMalloc(&e->x2, 4 * T * d)); KRAG_CUDA(cudaMalloc(&e->qkv, 4 * T * 3 * d));
-        KRAG_CUDA(cudaMalloc(&e->xs, 2 * 2 * T * d)); KRAG_CUDA(cudaMalloc(&e->cs, 2 * 2 * T * d)); KRAG_CUDA(cudaMalloc(&e->fs, 2 * 2 * T * c.inter));
-        KRAG_CUDA(cudaMalloc(&e->out, 4 * Bc * d));
+        // all old buffers go before the first new one is allocated (the peak is the new set only); a grow that fails
+        // half-way leaves no workspace and capacity 0, so the next call grows again
+        e->cap_tok = e->cap_batch = 0;
+        e->d_tok.release(); e->d_pos.release(); e->d_off.release(); e->x.release(); e->x2.release(); e->qkv.release();
+        e->xs.release(); e->cs.release(); e->fs.release(); e->out.release();
+        e->d_tok.alloc(T); e->d_pos.alloc(T); e->d_off.alloc(Bc + 1);
+        e->x.alloc(T * d); e->x2.alloc(T * d); e->qkv.alloc(T * 3 * d);
+        e->xs.alloc(2 * T * d); e->cs.alloc(2 * T * d); e->fs.alloc(2 * T * c.inter);
+        e->out.alloc(Bc * d);
         e->cap_tok = (int)T; e->cap_batch = (int)Bc;
     }
     // split planes: [hi plane | lo plane], each cap_tok rows
-    const SplitMat xs{e->xs, e->xs + (size_t)e->cap_tok * d}, cs{e->cs, e->cs + (size_t)e->cap_tok * d},
-                   fs{e->fs, e->fs + (size_t)e->cap_tok * c.inter};
-    KRAG_CUDA(cudaMemcpyAsync(e->d_tok, tok_ids, 4 * (size_t)n_tok, cudaMemcpyHostToDevice, st));
-    KRAG_CUDA(cudaMemcpyAsync(e->d_pos, pos.data(), 4 * (size_t)n_tok, cudaMemcpyHostToDevice, st));
-    KRAG_CUDA(cudaMemcpyAsync(e->d_off, tok_offsets, 4 * (size_t)(batch + 1), cudaMemcpyHostToDevice, st));
+    const SplitMat xs{e->xs.p, e->xs.p + (size_t)e->cap_tok * d}, cs{e->cs.p, e->cs.p + (size_t)e->cap_tok * d},
+                   fs{e->fs.p, e->fs.p + (size_t)e->cap_tok * c.inter};
+    KRAG_CUDA(cudaMemcpyAsync(e->d_tok.p, tok_ids, 4 * (size_t)n_tok, cudaMemcpyHostToDevice, st));
+    KRAG_CUDA(cudaMemcpyAsync(e->d_pos.p, pos.data(), 4 * (size_t)n_tok, cudaMemcpyHostToDevice, st));
+    KRAG_CUDA(cudaMemcpyAsync(e->d_off.p, tok_offsets, 4 * (size_t)(batch + 1), cudaMemcpyHostToDevice, st));
 
     // The forward is ~7 kernels per layer; for a handful of query tokens it is bound by launch gaps and kernel
     // prologues, so each (n_tok, batch, max_len) shape is captured into a CUDA graph the second time it is seen.
     auto run_layers = [&]() {
-    launch_pdl(embed_ln_kernel, dim3((unsigned)((n_tok + 7) / 8)), dim3(256), (size_t)8 * d * 4, st, e->d_tok, e->d_pos,
-               e->t["embeddings.word_embeddings.weight"], e->t["embeddings.position_embeddings.weight"],
-               e->t["embeddings.token_type_embeddings.weight"], e->t["embeddings.LayerNorm.weight"], e->t["embeddings.LayerNorm.bias"], e->x,
+    launch_pdl(embed_ln_kernel, dim3((unsigned)((n_tok + 7) / 8)), dim3(256), (size_t)8 * d * 4, st, e->d_tok.p, e->d_pos.p,
+               e->t["embeddings.word_embeddings.weight"].p, e->t["embeddings.position_embeddings.weight"].p,
+               e->t["embeddings.token_type_embeddings.weight"].p, e->t["embeddings.LayerNorm.weight"].p, e->t["embeddings.LayerNorm.bias"].p, e->x.p,
                xs.hi, xs.lo, n_tok, d, c.vocab, c.eps);
     const int dh = d / c.heads;
     const size_t at_smem = sizeof(float) * ((size_t)AT_ROWS * dh + (size_t)dh * (AT_CHUNK + 1) + (size_t)AT_CHUNK * dh + (size_t)AT_ROWS * max_len);
@@ -1274,41 +1270,41 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
         const size_t L = (size_t)l;
         if (use_mma) {
             // QKV projection writes the split planes only (same bytes as the fp32 matrix they replace); attention on the tensor cores
-            uint16_t* q_hi = reinterpret_cast<uint16_t*>(e->qkv);
+            uint16_t* q_hi = reinterpret_cast<uint16_t*>(e->qkv.p);
             uint16_t* q_lo = q_hi + (size_t)n_tok * 3 * d;
-            launch_linear(e->di, xs, e->s_qkv[L], n_tok, 3 * d, d, e->bqkv[L], nullptr, false, nullptr, q_hi, q_lo, nullptr, nullptr, 0.f,
-                          nullptr, nullptr, nullptr, e->ws, Embedder::WS_FLOATS, st);
-            if (dh == 64) attention_mma<64>(q_hi, q_lo, e->d_off, cs.hi, cs.lo, d, c.heads, batch, max_len, st);
-            else attention_mma<32>(q_hi, q_lo, e->d_off, cs.hi, cs.lo, d, c.heads, batch, max_len, st);
+            launch_linear(e->di, xs, e->s_qkv[L], n_tok, 3 * d, d, e->bqkv[L].p, nullptr, false, nullptr, q_hi, q_lo, nullptr, nullptr, 0.f,
+                          nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st);
+            if (dh == 64) attention_mma<64>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, st);
+            else attention_mma<32>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, st);
         } else {
         // KRAG_ATTN_MMA=0: fp32 qkv and the fp32 CUDA-core attention kernels
-        launch_linear(e->di, xs, e->s_qkv[L], n_tok, 3 * d, d, e->bqkv[L], nullptr, false, e->qkv, nullptr, nullptr, nullptr, nullptr, 0.f,
-                      nullptr, nullptr, nullptr, e->ws, Embedder::WS_FLOATS, st);
+        launch_linear(e->di, xs, e->s_qkv[L], n_tok, 3 * d, d, e->bqkv[L].p, nullptr, false, e->qkv.p, nullptr, nullptr, nullptr, nullptr, 0.f,
+                      nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st);
         if (max_len <= 32) {
-            launch_pdl(attention_tiled_kernel<32>, dim3((unsigned)batch, (unsigned)c.heads), dim3(128), ats_smem32, st, e->qkv, e->d_off, cs.hi, cs.lo, d, c.heads);
+            launch_pdl(attention_tiled_kernel<32>, dim3((unsigned)batch, (unsigned)c.heads), dim3(128), ats_smem32, st, e->qkv.p, e->d_off.p, cs.hi, cs.lo, d, c.heads);
         } else if (max_len <= ATS_MAX) {
-            launch_pdl(attention_tiled_kernel<64>, dim3((unsigned)batch, (unsigned)c.heads), dim3(128), ats_smem64, st, e->qkv, e->d_off, cs.hi, cs.lo, d, c.heads);
+            launch_pdl(attention_tiled_kernel<64>, dim3((unsigned)batch, (unsigned)c.heads), dim3(128), ats_smem64, st, e->qkv.p, e->d_off.p, cs.hi, cs.lo, d, c.heads);
         } else {
             if (use_flash)
                 attention_flash_kernel<<<dim3((unsigned)((max_len + 63) / 64), (unsigned)c.heads, (unsigned)batch), 128, ats_smem64, st>>>(
-                    e->qkv, e->d_off, cs.hi, cs.lo, d, c.heads);
+                    e->qkv.p, e->d_off.p, cs.hi, cs.lo, d, c.heads);
             else
                 attention_kernel<<<dim3((unsigned)((max_len + AT_ROWS - 1) / AT_ROWS), (unsigned)c.heads, (unsigned)batch), 256, at_smem, st>>>(
-                    e->qkv, e->d_off, cs.hi, cs.lo, d, c.heads, max_len);
+                    e->qkv.p, e->d_off.p, cs.hi, cs.lo, d, c.heads, max_len);
             KRAG_CUDA(cudaGetLastError());
             count_launch();
         }
         }
         // O projection (+bias +residual) -> LayerNorm -> x (fp32 residual stream) + its split planes
-        launch_linear(e->di, cs, e->s_o[L], n_tok, d, d, e->t[lname(l, "attention.output.dense.bias")], e->x, false, e->x2, nullptr, nullptr,
-                      e->t[lname(l, "attention.output.LayerNorm.weight")], e->t[lname(l, "attention.output.LayerNorm.bias")], c.eps, e->x, xs.hi, xs.lo,
-                      e->ws, Embedder::WS_FLOATS, st);
+        launch_linear(e->di, cs, e->s_o[L], n_tok, d, d, e->t[lname(l, "attention.output.dense.bias")].p, e->x.p, false, e->x2.p, nullptr, nullptr,
+                      e->t[lname(l, "attention.output.LayerNorm.weight")].p, e->t[lname(l, "attention.output.LayerNorm.bias")].p, c.eps, e->x.p, xs.hi, xs.lo,
+                      e->ws.p, Embedder::WS_FLOATS, st);
         // FFN1 (+bias, GELU): only the split planes are written (FFN2 is the sole consumer)
-        launch_linear(e->di, xs, e->s_f1[L], n_tok, c.inter, d, e->t[lname(l, "intermediate.dense.bias")], nullptr, true, nullptr, fs.hi, fs.lo,
-                      nullptr, nullptr, 0.f, nullptr, nullptr, nullptr, e->ws, Embedder::WS_FLOATS, st);
+        launch_linear(e->di, xs, e->s_f1[L], n_tok, c.inter, d, e->t[lname(l, "intermediate.dense.bias")].p, nullptr, true, nullptr, fs.hi, fs.lo,
+                      nullptr, nullptr, 0.f, nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st);
         // FFN2 (+bias +residual) -> LayerNorm -> x + split planes
-        launch_linear(e->di, fs, e->s_f2[L], n_tok, d, c.inter, e->t[lname(l, "output.dense.bias")], e->x, false, e->x2, nullptr, nullptr,
-                      e->t[lname(l, "output.LayerNorm.weight")], e->t[lname(l, "output.LayerNorm.bias")], c.eps, e->x, xs.hi, xs.lo, e->ws,
+        launch_linear(e->di, fs, e->s_f2[L], n_tok, d, c.inter, e->t[lname(l, "output.dense.bias")].p, e->x.p, false, e->x2.p, nullptr, nullptr,
+                      e->t[lname(l, "output.LayerNorm.weight")].p, e->t[lname(l, "output.LayerNorm.bias")].p, c.eps, e->x.p, xs.hi, xs.lo, e->ws.p,
                       Embedder::WS_FLOATS, st);
     }
     };   // run_layers
@@ -1320,7 +1316,7 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
         KRAG_CUDA(cudaGraphLaunch(git->second, st));
         count_launch(1 + 7 * c.layers);
     } else if (use_graph && (e->seen.size() > 4096 ? (e->seen.clear(), false) : e->seen[key]++ >= 1)) {
-        if (e->graphs.size() >= 64) { for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second); e->graphs.clear(); }
+        if (e->graphs.size() >= 64) e->drop_graphs();
         cudaGraph_t g = nullptr;
         cudaGraphExec_t ex = nullptr;
         KRAG_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
@@ -1339,7 +1335,7 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
         if (!e->in_ev) KRAG_CUDA(cudaEventCreateWithFlags(&e->in_ev, cudaEventDisableTiming));
         KRAG_CUDA(cudaEventRecord(e->in_ev, consumer));
         KRAG_CUDA(cudaStreamWaitEvent(st, e->in_ev, 0));
-        cls_normalize_kernel<<<(batch * 32 + 255) / 256, 256, 0, st>>>(e->x, e->d_off, out_dev, batch, d, ld_out);
+        cls_normalize_kernel<<<(batch * 32 + 255) / 256, 256, 0, st>>>(e->x.p, e->d_off.p, out_dev, batch, d, ld_out);
         KRAG_CUDA(cudaGetLastError());
         count_launch();
         if (!e->done) KRAG_CUDA(cudaEventCreateWithFlags(&e->done, cudaEventDisableTiming));
@@ -1347,10 +1343,10 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
         KRAG_CUDA(cudaStreamWaitEvent(consumer, e->done, 0));
     }
     if (out_host) {
-        cls_normalize_kernel<<<(batch * 32 + 255) / 256, 256, 0, st>>>(e->x, e->d_off, e->out, batch, d, d);
+        cls_normalize_kernel<<<(batch * 32 + 255) / 256, 256, 0, st>>>(e->x.p, e->d_off.p, e->out.p, batch, d, d);
         KRAG_CUDA(cudaGetLastError());
         count_launch();
-        KRAG_CUDA(cudaMemcpyAsync(out_host, e->out, 4 * (size_t)batch * d, cudaMemcpyDeviceToHost, st));
+        KRAG_CUDA(cudaMemcpyAsync(out_host, e->out.p, 4 * (size_t)batch * d, cudaMemcpyDeviceToHost, st));
         KRAG_CUDA(cudaStreamSynchronize(st));
     }
 }

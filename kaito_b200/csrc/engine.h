@@ -2,12 +2,87 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <stdio.h>
 
 #include <stdexcept>
+#include <utility>
+
+#include "common.cuh"
 namespace krag {
 
 // device allocation failure with a message that says what was asked for and what was free (KRAG_E_OOM at the C ABI)
 struct DevOom : std::runtime_error { using std::runtime_error::runtime_error; };
+
+// bytes of device memory currently held through DevArray, process-wide (krag_device_bytes)
+void count_device_bytes(int64_t delta);
+int64_t device_bytes();
+
+// Owning device buffer: the only code of the library that allocates or frees device memory.  Move-only; the destructor frees.
+// An allocation that does not fit throws DevOom, saying how much was asked for and what was left.
+template <class T>
+struct DevArray {
+    T* p = nullptr;
+    int64_t cap = 0;
+
+    DevArray() = default;
+    DevArray(const DevArray&) = delete;
+    DevArray& operator=(const DevArray&) = delete;
+    DevArray(DevArray&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    DevArray& operator=(DevArray&& o) noexcept
+    {
+        if (this != &o) { release(); std::swap(p, o.p); std::swap(cap, o.cap); }
+        return *this;
+    }
+    ~DevArray() { release(); }
+
+    // a fresh buffer of exactly n elements; the old one is freed first
+    void alloc(int64_t n)
+    {
+        release();
+        p = allocate(n);
+        cap = n;
+    }
+    // grow to at least n elements keeping the first `used` (copy-on-grow; krag_index_reserve avoids the copies for big corpora)
+    void reserve(int64_t n, int64_t used, cudaStream_t st)
+    {
+        if (n <= cap) return;
+        DevArray grown;
+        grown.alloc(cap + cap / 2 > n ? cap + cap / 2 : n);
+        if (p && used > 0) KRAG_CUDA(cudaMemcpyAsync(grown.p, p, sizeof(T) * (size_t)used, cudaMemcpyDeviceToDevice, st));
+        KRAG_CUDA(cudaStreamSynchronize(st));
+        *this = std::move(grown);
+    }
+    void release()
+    {
+        if (p) {
+            cudaFree(p);
+            count_device_bytes(-bytes());
+        }
+        p = nullptr;
+        cap = 0;
+    }
+    int64_t bytes() const { return (int64_t)sizeof(T) * cap; }
+
+private:
+    static T* allocate(int64_t n)
+    {
+        void* q = nullptr;
+        const size_t bytes = sizeof(T) * (size_t)n;
+        const cudaError_t e = cudaMalloc(&q, bytes);
+        if (e == cudaErrorMemoryAllocation) {
+            cudaGetLastError();
+            size_t free_b = 0, total_b = 0;
+            cudaMemGetInfo(&free_b, &total_b);
+            char msg[160];
+            snprintf(msg, sizeof msg, "out of device memory (wanted %.2f GB, %.2f of %.2f GB free)", bytes / 1e9, free_b / 1e9,
+                     total_b / 1e9);
+            throw DevOom{msg};
+        }
+        KRAG_CUDA(e);
+        count_device_bytes((int64_t)bytes);
+        return static_cast<T*>(q);
+    }
+};
 
 // global ordinal of a local row: base + row * stride.  Contiguous shards (bench, one GPU) use stride 1; the multi-GPU
 // service deals nodes round-robin (node o -> shard o % G, row o / G), so base = shard, stride = G and ordinals -- hence
@@ -86,16 +161,16 @@ constexpr int BM25_SUB_DOCS = 2048;      // doc range of one tile-index column =
 constexpr int BM25_SUBS_PER_TILE = 8;
 constexpr int BM25_TILE_DOCS = BM25_SUB_DOCS * BM25_SUBS_PER_TILE;   // doc range of one CTA in the legacy kernel (safety net)
 struct Postings {
-    int64_t* off = nullptr;    // [vocab+1]
-    uint32_t* doc = nullptr;   // [nnz] local rows ascending inside a term
-    float* score = nullptr;    // [nnz]
+    DevArray<int64_t> off;     // [vocab+1]
+    DevArray<uint32_t> doc;    // [nnz] local rows ascending inside a term
+    DevArray<float> score;     // [nnz]
     int64_t vocab = 0, nnz = 0;
     // tile index: for terms with more than BM25_RARE_MAX postings, the offset (relative to off[t]) of the
     // first posting whose doc lies in each BM25_SUB_DOCS-sized doc range; removes per-query searches.  Terms below the
     // threshold get the same kind of row built per batch by bm25_resolve_kernel (a row costs 4 B per sub-tile, more than
     // the postings of a short list)
-    int32_t* tile_slot = nullptr;   // [vocab]  slot of a frequent term, -1 for the others
-    uint32_t* tile_off = nullptr;   // [n_slots][n_tiles + 1]
+    DevArray<int32_t> tile_slot;    // [vocab]  slot of a frequent term, -1 for the others
+    DevArray<uint32_t> tile_off;    // [n_slots][n_tiles + 1]
     int64_t n_slots = 0, n_tiles = 0;   // n_tiles = number of BM25_SUB_DOCS ranges
 };
 constexpr int BM25_RARE_MAX = 2048;
@@ -139,8 +214,8 @@ void launch_linear_f32(const DeviceInfo& di, const float* A, const float* B, int
 // ---- synthetic data (synth.cu)
 void launch_synth_dense(float* X, int64_t n, int d, int dpad, int64_t row_base, uint64_t seed, cudaStream_t st);
 // two-pass: lengths -> offsets (host scan by caller via cub) -> fill
-void synth_sparse(int64_t n, int64_t row_base, uint64_t seed, int64_t vocab, int64_t** term_offsets_out,
-                  uint32_t** term_ids_out, uint16_t** term_tf_out, uint32_t** doc_len_out, int64_t* nnz_out,
+void synth_sparse(int64_t n, int64_t row_base, uint64_t seed, int64_t vocab, DevArray<int64_t>& term_offsets,
+                  DevArray<uint32_t>& term_ids, DevArray<uint16_t>& term_tf, DevArray<uint32_t>& doc_len, int64_t* nnz_out,
                   cudaStream_t st);
 
 }  // namespace krag

@@ -145,49 +145,46 @@ synth_sparse_kernel(int64_t n, int64_t row_base, uint64_t seed, int64_t vocab, f
     if (MODE == 0 && lane == 0) { uniq[d] = runs_before; doc_len[d] = (uint32_t)dl; }
 }
 
-void synth_sparse(int64_t n, int64_t row_base, uint64_t seed, int64_t vocab, int64_t** term_offsets_out,
-                  uint32_t** term_ids_out, uint16_t** term_tf_out, uint32_t** doc_len_out, int64_t* nnz_out,
+void synth_sparse(int64_t n, int64_t row_base, uint64_t seed, int64_t vocab, DevArray<int64_t>& offsets,
+                  DevArray<uint32_t>& term_ids, DevArray<uint16_t>& term_tf, DevArray<uint32_t>& doc_len, int64_t* nnz_out,
                   cudaStream_t st)
 {
     const float s = 1.07f;
     const float vmax_pow = powf((float)(vocab + 1), 1.f - s);
     const float inv_exp = 1.f / (1.f - s);
-    int64_t *uniq = nullptr, *offsets = nullptr;
-    uint32_t* doc_len = nullptr;
-    KRAG_CUDA(cudaMalloc(&uniq, sizeof(int64_t) * (size_t)(n + 1)));
-    KRAG_CUDA(cudaMemsetAsync(uniq, 0, sizeof(int64_t) * (size_t)(n + 1), st));
-    KRAG_CUDA(cudaMalloc(&offsets, sizeof(int64_t) * (size_t)(n + 1)));
-    KRAG_CUDA(cudaMalloc(&doc_len, sizeof(uint32_t) * (size_t)(n > 0 ? n : 1)));
+    DevArray<int64_t> uniq;
+    uniq.alloc(n + 1);
+    KRAG_CUDA(cudaMemsetAsync(uniq.p, 0, sizeof(int64_t) * (size_t)(n + 1), st));
+    offsets.alloc(n + 1);
+    doc_len.alloc(n > 0 ? n : 1);
     const unsigned grid = (unsigned)((n + SY_WARPS - 1) / SY_WARPS);
     if (n > 0) {
-        synth_sparse_kernel<0><<<grid, SY_WARPS * 32, 0, st>>>(n, row_base, seed, vocab, vmax_pow, inv_exp, uniq, doc_len,
+        synth_sparse_kernel<0><<<grid, SY_WARPS * 32, 0, st>>>(n, row_base, seed, vocab, vmax_pow, inv_exp, uniq.p, doc_len.p,
                                                                nullptr, nullptr, nullptr);
         KRAG_CUDA(cudaGetLastError());
         count_launch();
     }
     size_t tmp_bytes = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, uniq, offsets, (int64_t)(n + 1), st);
-    void* tmp = nullptr;
-    KRAG_CUDA(cudaMalloc(&tmp, tmp_bytes ? tmp_bytes : 16));
-    cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, uniq, offsets, (int64_t)(n + 1), st);
+    cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, uniq.p, offsets.p, (int64_t)(n + 1), st);
+    DevArray<unsigned char> tmp;
+    tmp.alloc(tmp_bytes ? tmp_bytes : 16);
+    cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, uniq.p, offsets.p, (int64_t)(n + 1), st);
     count_launch();
     int64_t nnz = 0;
-    KRAG_CUDA(cudaMemcpyAsync(&nnz, offsets + n, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    KRAG_CUDA(cudaMemcpyAsync(&nnz, offsets.p + n, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     KRAG_CUDA(cudaStreamSynchronize(st));
-    KRAG_CUDA(cudaFree(tmp));
-    KRAG_CUDA(cudaFree(uniq));
-    uint32_t* term_ids = nullptr;
-    uint16_t* term_tf = nullptr;
-    KRAG_CUDA(cudaMalloc(&term_ids, sizeof(uint32_t) * (size_t)(nnz > 0 ? nnz : 1)));
-    KRAG_CUDA(cudaMalloc(&term_tf, sizeof(uint16_t) * (size_t)(nnz > 0 ? nnz : 1)));
+    tmp.release();
+    uniq.release();
+    term_ids.alloc(nnz > 0 ? nnz : 1);
+    term_tf.alloc(nnz > 0 ? nnz : 1);
     if (n > 0) {
         synth_sparse_kernel<1><<<grid, SY_WARPS * 32, 0, st>>>(n, row_base, seed, vocab, vmax_pow, inv_exp, nullptr,
-                                                               nullptr, offsets, term_ids, term_tf);
+                                                               nullptr, offsets.p, term_ids.p, term_tf.p);
         KRAG_CUDA(cudaGetLastError());
         count_launch();
     }
     KRAG_CUDA(cudaStreamSynchronize(st));
-    *term_offsets_out = offsets; *term_ids_out = term_ids; *term_tf_out = term_tf; *doc_len_out = doc_len; *nnz_out = nnz;
+    *nnz_out = nnz;
 }
 
 }  // namespace krag
