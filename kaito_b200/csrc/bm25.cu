@@ -349,21 +349,17 @@ void build_postings(const uint32_t* term_ids, const uint16_t* term_tf, const uin
 // Two kernels.  bm25_warp_kernel (further down) is the one that runs: warp-autonomous sub-tiles, a sampled per-query
 // admission threshold, global candidate lists.  bm25_tile_kernel below is the first-generation CTA-per-tile kernel, kept as
 // the exact SAFETY NET for queries whose candidate list overflows (launched after every batch, it skips every query whose
-// overflow flag is 0) and selectable as a whole with KRAG_BM25_LEGACY=1.
+// overflow flag is 0) and selectable as a whole with KRAG_BM25_KERNEL=legacy.
 constexpr int BQ_THREADS = 256;   // a term contributes ~200 postings to a 16384-doc tile: 256-wide slabs keep the lanes busy
 constexpr int BQ_MAX_TERMS = 32;    // query terms resolved per pass; longer queries loop
 constexpr int BQ_MAX_SLABS = 96;    // 512-posting slabs per pass
 constexpr int BQ_PREFETCH = 8;      // slabs held in registers at a time
 constexpr int BQ_GROUP_MAX = 32;    // upper bound of the group size (shared-memory table)
-// consecutive doc tiles handled by one work item (same query): one resolve, one select, one store.  Runtime value
-// (KRAG_BM25_GROUP, default 8): larger groups mean fewer per-item sorts/stores and tighter own thresholds, smaller
-// ones more items to balance over the 444 resident CTAs
-static int bq_group()
-{
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("KRAG_BM25_GROUP"); int g = e ? atoi(e) : 8; v = g < 1 ? 1 : (g > BQ_GROUP_MAX ? BQ_GROUP_MAX : g); }
-    return v;
-}
+// consecutive doc tiles handled by one work item (same query): one resolve, one select, one store.  Larger groups mean
+// fewer per-item sorts/stores and tighter own thresholds, smaller ones more items to balance over the 444 resident CTAs.
+// bm25_tile_kernel takes it as a run-time argument (up to BQ_GROUP_MAX)
+constexpr int BQ_GROUP = 8;
+static_assert(BQ_GROUP >= 1 && BQ_GROUP <= BQ_GROUP_MAX, "BQ_GROUP must fit the kernel's shared-memory table");
 
 // A "slab" is up to 512 consecutive postings of one query term that fall into this CTA's doc
 // range (frequent terms: looked up in the tile index; rare terms: the whole <= 256-entry list,
@@ -994,14 +990,13 @@ static int bw_capq(int P)
     while (c < 256 * P && c < 262144) c <<= 1;
     return c;
 }
-// which query kernel serves a shard: KRAG_BM25_KERNEL = auto (default) | warp | legacy; KRAG_BM25_LEGACY=1 == legacy.
+// which query kernel serves a shard: KRAG_BM25_KERNEL = auto (default) | warp | legacy.
 // auto: the warp kernel's fixed passes (resolve, sample pass, two selects) cost ~0.5 ms per batch whatever the shard size,
 // the first-generation kernel has almost none but ~1.5x the per-posting cost: the curves cross near 3M rows per shard
 // (measured: 10M rows 2.2 vs 3.1 ms, 1.25M rows 0.75 vs 0.50 ms per 256-query batch).
 constexpr int64_t BW_AUTO_MIN_ROWS = 3000000;
 static bool bw_legacy(int64_t n_rows)
 {
-    if (env_int("KRAG_BM25_LEGACY", 0) != 0) return true;
     const char* k = getenv("KRAG_BM25_KERNEL");
     if (k && k[0] == 'w') return false;
     if (k && k[0] == 'l') return true;
@@ -1018,7 +1013,7 @@ static BmLayout bm_layout(int64_t n_rows, int batch, int P)
     BmLayout L;
     L.n_tiles = (n_rows + BM25_TILE_DOCS - 1) / BM25_TILE_DOCS;
     if (L.n_tiles < 1) L.n_tiles = 1;
-    L.n_groups = (L.n_tiles + bq_group() - 1) / bq_group();
+    L.n_groups = (L.n_tiles + BQ_GROUP - 1) / BQ_GROUP;
     L.capq = bw_capq(P);
     size_t o = 0;
     L.legacy_part = o; o += (size_t)L.n_groups * batch * P;
@@ -1111,8 +1106,8 @@ void launch_bm25(const DeviceInfo& di, const Postings& post, int64_t n_rows, con
         count_launch();
     }
     if (need_safety_net) {
-        // legacy kernel: every query (KRAG_BM25_LEGACY=1) or only the queries whose list overflowed (normally none: its
-        // CTAs read one flag per work item and leave)
+        // legacy kernel: every query (KRAG_BM25_KERNEL=legacy, or auto on a small shard) or only the queries whose list
+        // overflowed (normally none: its CTAs read one flag per work item and leave)
         const int cap = bq_cap(P);
         const size_t smem = (size_t)BM25_TILE_DOCS * 4 + (size_t)cap * 8;
         static bool attr_set = false;
@@ -1128,7 +1123,7 @@ void launch_bm25(const DeviceInfo& di, const Postings& post, int64_t n_rows, con
         const uint32_t* only = legacy_only ? nullptr : flags;
         bm25_tile_kernel<<<grid, BQ_THREADS, smem, st>>>(post.off.p, post.doc.p, post.score.p, post.tile_slot.p, post.tile_off.p,
                                                          post.n_tiles, post.vocab, q_terms, q_term_offsets, q_slot, q_base, q_rare, n_rows,
-                                                         alive, P, cap, ord_base, batch, (int)L.n_tiles, bq_group(), part + L.legacy_part, g_thr, only);
+                                                         alive, P, cap, ord_base, batch, (int)L.n_tiles, BQ_GROUP, part + L.legacy_part, g_thr, only);
         KRAG_CUDA(cudaGetLastError());
         count_launch();
         launch_merge(part + L.legacy_part, (int)L.n_groups, P, batch, P, /*list_stride=*/P, /*batch_stride=*/L.n_groups * P, keys_out, st,

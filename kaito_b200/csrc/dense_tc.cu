@@ -28,8 +28,6 @@
 #include <cuda_bf16.h>
 #include <math_constants.h>
 
-#include <stdlib.h>
-
 #include <atomic>
 #include <mutex>
 #include <vector>
@@ -554,13 +552,6 @@ static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensor
     count_launch();
 }
 
-static bool tc_use_cvt()
-{
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("KRAG_TC_CVT"); v = (e == nullptr || e[0] != '0') ? 1 : 0; }
-    return v == 1;
-}
-
 static std::atomic<int64_t> g_tc_fallback_queries{0};   // searches run concurrently (reader lock)
 int64_t dense_tc_fallback_queries() { return g_tc_fallback_queries.load(); }
 
@@ -570,9 +561,9 @@ bool launch_dense_tc(const DeviceInfo& di, const float* X, int64_t n_rows, int d
                      const uint16_t* Xh, bool allow_cvt)
 {
     if (Xh != nullptr && dpad % (2 * TC_KBLOCK) != 0) Xh = nullptr;   // bf16 k-blocks are 64 elements wide
-    // default prune pass: fp32 rows rounded to bf16 on their way into the wgmma A registers (no shadow); KRAG_TC_CVT=0
+    // default prune pass: fp32 rows rounded to bf16 on their way into the wgmma A registers (no shadow); allow_cvt = false
     // keeps the TF32 pass
-    const bool cvt = Xh == nullptr && allow_cvt && tc_use_cvt() && dpad % (2 * TC_KBLOCK) == 0;
+    const bool cvt = Xh == nullptr && allow_cvt && dpad % (2 * TC_KBLOCK) == 0;
     if (n_rows < TC_MIN_ROWS || n_rows >= (1ll << 31) || xnorm == nullptr) return false;
     const int cap = tc_cap(P);
     const int64_t S = tc_sample_tiles(n_rows) * TC_TILE_M;

@@ -15,7 +15,6 @@
 // (attention is 4 S^2 d: 2% of the flops at S = 32 queries).
 #include <cuda_fp16.h>
 #include <math_constants.h>
-#include <stdlib.h>
 
 #include <map>
 #include <memory>
@@ -328,9 +327,6 @@ embed_ln_kernel(const int32_t* __restrict__ tok, const int32_t* __restrict__ pos
     warp_layernorm_row(row, x + (size_t)t * d, x_hi + (size_t)t * d, x_lo + (size_t)t * d, g, b, d, eps, lane);
 }
 
-// ------------------------------------------------------------------------------- attention
-// packed variable-length sequences: qkv [n_tok, 3d] (Q | K | V, heads contiguous inside each), out [n_tok, d].
-// grid (ceil(max_len / 16), heads, batch); 8 warps, 2 query rows per warp; keys processed in chunks of 64.
 // split-K epilogue: out[row] = f(sum_s ws[s][row] + bias) (+GELU) (+residual), optionally followed by LayerNorm over
 // the row (N <= 1024).  One 256-thread block per row, one float4 column group per thread: the `splits` partial loads
 // of a thread are independent (all in flight at once) -- with a few rows this kernel is pure load latency.
@@ -406,317 +402,7 @@ splitk_reduce_kernel(const float* __restrict__ ws, int splits, int M, int N, con
     }
 }
 
-constexpr int AT_ROWS = 16;
-constexpr int AT_CHUNK = 64;
-__global__ void __launch_bounds__(256)
-attention_kernel(const float* __restrict__ qkv, const int32_t* __restrict__ seq_off, uint16_t* __restrict__ out_hi,
-                 uint16_t* __restrict__ out_lo, int d, int heads, int max_len)
-{
-    extern __shared__ float a_sm[];
-    const int dh = d / heads;
-    const int b = blockIdx.z, h = blockIdx.y;
-    const int t0 = seq_off[b], len = seq_off[b + 1] - t0;
-    const int r0 = blockIdx.x * AT_ROWS;
-    if (r0 >= len) return;
-    float* s_q = a_sm;                                  // [AT_ROWS][dh]
-    float* s_kT = s_q + AT_ROWS * dh;                   // [dh][AT_CHUNK + 1]
-    float* s_v = s_kT + dh * (AT_CHUNK + 1);            // [AT_CHUNK][dh]
-    float* s_p = s_v + AT_CHUNK * dh;                   // [AT_ROWS][max_len] scores / probabilities
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const float scale = rsqrtf((float)dh);
-    const int nrows = min(AT_ROWS, len - r0);
-    for (int i = tid; i < nrows * dh; i += 256) {
-        const int r = i / dh, c = i % dh;
-        s_q[i] = qkv[(size_t)(t0 + r0 + r) * 3 * d + h * dh + c];
-    }
-    // pass 1: scores
-    for (int k0 = 0; k0 < len; k0 += AT_CHUNK) {
-        const int nk = min(AT_CHUNK, len - k0);
-        __syncthreads();
-        for (int i = tid; i < nk * dh; i += 256) {
-            const int kk = i / dh, c = i % dh;
-            s_kT[c * (AT_CHUNK + 1) + kk] = qkv[(size_t)(t0 + k0 + kk) * 3 * d + d + h * dh + c];
-        }
-        __syncthreads();
-        for (int rr = 0; rr < 2; ++rr) {
-            const int r = warp * 2 + rr;
-            if (r >= nrows) break;
-            for (int kk = lane; kk < nk; kk += 32) {
-                float acc = 0.f;
-                for (int c = 0; c < dh; ++c) acc = fmaf(s_q[r * dh + c], s_kT[c * (AT_CHUNK + 1) + kk], acc);
-                s_p[r * max_len + k0 + kk] = acc * scale;
-            }
-        }
-    }
-    __syncthreads();
-    // softmax per row (fp32, max-subtracted like torch)
-    for (int rr = 0; rr < 2; ++rr) {
-        const int r = warp * 2 + rr;
-        if (r >= nrows) break;
-        float* p = s_p + r * max_len;
-        float m = -CUDART_INF_F;
-        for (int k = lane; k < len; k += 32) m = fmaxf(m, p[k]);
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-        float s = 0.f;
-        for (int k = lane; k < len; k += 32) { float e = expf(p[k] - m); p[k] = e; s += e; }
-        s = warp_sum(s);
-        const float inv = 1.f / s;
-        for (int k = lane; k < len; k += 32) p[k] *= inv;
-    }
-    // pass 2: out = P . V
-    float o_acc[2][2] = {{0.f, 0.f}, {0.f, 0.f}};      // [row of the warp][dh / 32 columns per lane, dh <= 64]
-    for (int k0 = 0; k0 < len; k0 += AT_CHUNK) {
-        const int nk = min(AT_CHUNK, len - k0);
-        __syncthreads();
-        for (int i = tid; i < nk * dh; i += 256) {
-            const int kk = i / dh, c = i % dh;
-            s_v[kk * dh + c] = qkv[(size_t)(t0 + k0 + kk) * 3 * d + 2 * d + h * dh + c];
-        }
-        __syncthreads();
-        for (int rr = 0; rr < 2; ++rr) {
-            const int r = warp * 2 + rr;
-            if (r >= nrows) break;
-            for (int kk = 0; kk < nk; ++kk) {
-                const float p = s_p[r * max_len + k0 + kk];
-                if (lane < dh) o_acc[rr][0] = fmaf(p, s_v[kk * dh + lane], o_acc[rr][0]);
-                if (lane + 32 < dh) o_acc[rr][1] = fmaf(p, s_v[kk * dh + lane + 32], o_acc[rr][1]);
-            }
-        }
-    }
-    for (int rr = 0; rr < 2; ++rr) {
-        const int r = warp * 2 + rr;
-        if (r >= nrows) break;
-        const size_t ob = (size_t)(t0 + r0 + r) * d + h * dh;
-        if (lane < dh) split_f16(o_acc[rr][0], out_hi[ob + lane], out_lo[ob + lane]);
-        if (lane + 32 < dh) split_f16(o_acc[rr][1], out_hi[ob + lane + 32], out_lo[ob + lane + 32]);
-    }
-}
-
-// short sequences (queries; len <= S2 in {32, 64}): one CTA of 128 threads per (sequence, head).  Both products
-// are register-tiled out of shared memory: thread (ty, tx) owns S2/8 rows x S2/16 score columns, then S2/8 rows x 4
-// output columns; operands are stored transposed where needed so every shared-memory read is a conflict-free
-// vector load.  fp32 throughout (scores, max-subtracted softmax, P.V) like torch's math path.
-constexpr int ATS_MAX = 64;
-template <int S2>
-__global__ void __launch_bounds__(128)
-attention_tiled_kernel(const float* __restrict__ qkv, const int32_t* __restrict__ seq_off, uint16_t* __restrict__ out_hi,
-                       uint16_t* __restrict__ out_lo, int d, int heads)
-{
-    constexpr int RPT = S2 / 8;        // rows per thread
-    constexpr int CPT = S2 / 16;       // score columns per thread
-    constexpr int LD = S2 + 4;         // padded leading dimension (keeps 16-byte alignment, staggers banks)
-    extern __shared__ __align__(16) float as_sm[];
-    const int dh = d / heads;          // 32 or 64
-    float* s_qT = as_sm;               // [dh][LD]   q transposed: s_qT[c][r]
-    float* s_kT = s_qT + 64 * LD;      // [dh][LD]   k transposed: s_kT[c][key]
-    float* s_v = s_kT + 64 * LD;       // [S2][64]   v: s_v[key][c]
-    float* s_pT = s_v + S2 * 64;       // [S2][LD]   probabilities transposed: s_pT[key][r]
-    pdl_launch_dependents();
-    pdl_wait();
-    const int b = blockIdx.x, h = blockIdx.y;
-    const int t0 = seq_off[b], len = seq_off[b + 1] - t0;
-    const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
-    {   // a warp moves 4 rows x 8 columns per step: 32-byte global segments, and with LD = S2 + 4 the
-        // transposed stores (bank = 4 c + r) touch 32 distinct banks
-        const int warp = tid >> 5, lane = tid & 31, cl = lane & 7, rl = lane >> 3;
-        const int cblocks = dh / 8;
-        for (int blk = warp; blk < cblocks * (S2 / 4); blk += 4) {
-            const int c = (blk % cblocks) * 8 + cl, r = (blk / cblocks) * 4 + rl;
-            float q = 0.f, k = 0.f, v = 0.f;
-            if (r < len) {
-                const float* base = qkv + (size_t)(t0 + r) * 3 * d + h * dh + c;
-                q = base[0]; k = base[d]; v = base[2 * d];
-            }
-            s_qT[c * LD + r] = q; s_kT[c * LD + r] = k; s_v[r * 64 + c] = v;
-        }
-    }
-    __syncthreads();
-    // ---- scores
-    float acc[RPT][CPT];
-#pragma unroll
-    for (int i = 0; i < RPT; ++i)
-#pragma unroll
-        for (int j = 0; j < CPT; ++j) acc[i][j] = 0.f;
-    for (int c = 0; c < dh; ++c) {
-        float qv[RPT], kv[CPT];
-#pragma unroll
-        for (int i = 0; i < RPT; ++i) qv[i] = s_qT[c * LD + ty * RPT + i];
-#pragma unroll
-        for (int j = 0; j < CPT; ++j) kv[j] = s_kT[c * LD + tx * CPT + j];
-#pragma unroll
-        for (int i = 0; i < RPT; ++i)
-#pragma unroll
-            for (int j = 0; j < CPT; ++j) acc[i][j] = fmaf(qv[i], kv[j], acc[i][j]);
-    }
-    const float scale = rsqrtf((float)dh);
-    // ---- softmax over each row: its S2 columns live in the 16 threads tx = 0..15 of one half-warp
-#pragma unroll
-    for (int i = 0; i < RPT; ++i) {
-        float m = -CUDART_INF_F;
-#pragma unroll
-        for (int j = 0; j < CPT; ++j) {
-            acc[i][j] = (tx * CPT + j < len) ? acc[i][j] * scale : -CUDART_INF_F;
-            m = fmaxf(m, acc[i][j]);
-        }
-#pragma unroll
-        for (int o = 8; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-        float sum = 0.f;
-#pragma unroll
-        for (int j = 0; j < CPT; ++j) { acc[i][j] = (tx * CPT + j < len) ? expf(acc[i][j] - m) : 0.f; sum += acc[i][j]; }
-#pragma unroll
-        for (int o = 8; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-        const float inv = 1.f / sum;
-#pragma unroll
-        for (int j = 0; j < CPT; ++j) s_pT[(tx * CPT + j) * LD + ty * RPT + i] = acc[i][j] * inv;
-    }
-    __syncthreads();
-    // ---- out = P . V : thread (ty, tx) owns rows ty*RPT.. and columns tx*4.. (dh = 64) / tx*2.. (dh = 32)
-    const int cw = dh / 16;            // 4 or 2 output columns per thread
-    float o_acc[RPT][4];
-#pragma unroll
-    for (int i = 0; i < RPT; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) o_acc[i][j] = 0.f;
-    for (int k = 0; k < len; ++k) {
-        float pv[RPT], vv[4];
-#pragma unroll
-        for (int i = 0; i < RPT; ++i) pv[i] = s_pT[k * LD + ty * RPT + i];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) vv[j] = j < cw ? s_v[k * 64 + tx * cw + j] : 0.f;
-#pragma unroll
-        for (int i = 0; i < RPT; ++i)
-#pragma unroll
-            for (int j = 0; j < 4; ++j) o_acc[i][j] = fmaf(pv[i], vv[j], o_acc[i][j]);
-    }
-#pragma unroll
-    for (int i = 0; i < RPT; ++i) {
-        const int r = ty * RPT + i;
-        if (r < len) {
-            const size_t ob = (size_t)(t0 + r) * d + h * dh + tx * cw;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) if (j < cw) split_f16(o_acc[i][j], out_hi[ob + j], out_lo[ob + j]);
-        }
-    }
-}
-
-// long sequences (chunks on the /index path; len up to max_position): flash-style fp32 attention.
-// One CTA of 128 threads per (sequence, head, block of 64 query rows); keys are visited in chunks of 64 with an
-// online (running max / running sum) softmax, so no S x S score matrix is materialised.  Both products are
-// register-tiled exactly like attention_tiled_kernel<64>: thread (ty, tx) owns 8 rows x 4 score columns and
-// 8 rows x (dh/16) output columns.
-__global__ void __launch_bounds__(128)
-attention_flash_kernel(const float* __restrict__ qkv, const int32_t* __restrict__ seq_off, uint16_t* __restrict__ out_hi,
-                       uint16_t* __restrict__ out_lo, int d, int heads)
-{
-    constexpr int S2 = 64, RPT = 8, CPT = 4, LD = S2 + 4;
-    extern __shared__ __align__(16) float af_sm[];
-    const int dh = d / heads;
-    float* s_qT = af_sm;               // [dh][LD]
-    float* s_kT = s_qT + 64 * LD;      // [dh][LD]
-    float* s_v = s_kT + 64 * LD;       // [64][64]
-    float* s_pT = s_v + S2 * 64;       // [64 keys][LD rows]
-    const int b = blockIdx.z, h = blockIdx.y;
-    const int t0 = seq_off[b], len = seq_off[b + 1] - t0;
-    const int r0 = blockIdx.x * S2;
-    if (r0 >= len) return;
-    const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
-    const int warp = tid >> 5, lane = tid & 31, cl = lane & 7, rl = lane >> 3;
-    const int cblocks = dh / 8;
-    for (int blk = warp; blk < cblocks * (S2 / 4); blk += 4) {       // Q rows of this block, transposed
-        const int c = (blk % cblocks) * 8 + cl, r = (blk / cblocks) * 4 + rl;
-        s_qT[c * LD + r] = (r0 + r < len) ? qkv[(size_t)(t0 + r0 + r) * 3 * d + h * dh + c] : 0.f;
-    }
-    const float scale = rsqrtf((float)dh);
-    const int cw = dh / 16;
-    float m_run[RPT], l_run[RPT], o_acc[RPT][4];
-#pragma unroll
-    for (int i = 0; i < RPT; ++i) {
-        m_run[i] = -CUDART_INF_F; l_run[i] = 0.f;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) o_acc[i][j] = 0.f;
-    }
-    for (int k0 = 0; k0 < len; k0 += S2) {
-        __syncthreads();                                             // previous chunk fully consumed (s_kT, s_v, s_pT)
-        for (int blk = warp; blk < cblocks * (S2 / 4); blk += 4) {
-            const int c = (blk % cblocks) * 8 + cl, r = (blk / cblocks) * 4 + rl;
-            float k = 0.f, v = 0.f;
-            if (k0 + r < len) {
-                const float* base = qkv + (size_t)(t0 + k0 + r) * 3 * d + d + h * dh + c;
-                k = base[0]; v = base[d];
-            }
-            s_kT[c * LD + r] = k; s_v[r * 64 + c] = v;
-        }
-        __syncthreads();
-        float acc[RPT][CPT];
-#pragma unroll
-        for (int i = 0; i < RPT; ++i)
-#pragma unroll
-            for (int j = 0; j < CPT; ++j) acc[i][j] = 0.f;
-        for (int c = 0; c < dh; ++c) {
-            float qv[RPT], kv[CPT];
-#pragma unroll
-            for (int i = 0; i < RPT; ++i) qv[i] = s_qT[c * LD + ty * RPT + i];
-#pragma unroll
-            for (int j = 0; j < CPT; ++j) kv[j] = s_kT[c * LD + tx * CPT + j];
-#pragma unroll
-            for (int i = 0; i < RPT; ++i)
-#pragma unroll
-                for (int j = 0; j < CPT; ++j) acc[i][j] = fmaf(qv[i], kv[j], acc[i][j]);
-        }
-        // online softmax: a row's 64 chunk columns live in the 16 threads tx = 0..15 of one half-warp
-#pragma unroll
-        for (int i = 0; i < RPT; ++i) {
-            float m = -CUDART_INF_F;
-#pragma unroll
-            for (int j = 0; j < CPT; ++j) {
-                acc[i][j] = (k0 + tx * CPT + j < len) ? acc[i][j] * scale : -CUDART_INF_F;
-                m = fmaxf(m, acc[i][j]);
-            }
-#pragma unroll
-            for (int o = 8; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-            const float m_new = fmaxf(m_run[i], m);                  // finite: every chunk holds at least one valid key
-            const float corr = expf(m_run[i] - m_new);               // exp(-inf) = 0 on the first chunk
-            float sum = 0.f;
-#pragma unroll
-            for (int j = 0; j < CPT; ++j) {
-                const float p = (k0 + tx * CPT + j < len) ? expf(acc[i][j] - m_new) : 0.f;
-                sum += p;
-                s_pT[(tx * CPT + j) * LD + ty * RPT + i] = p;
-            }
-#pragma unroll
-            for (int o = 8; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-            l_run[i] = l_run[i] * corr + sum;
-            m_run[i] = m_new;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) o_acc[i][j] *= corr;
-        }
-        __syncthreads();
-        const int nk = min(S2, len - k0);
-        for (int k = 0; k < nk; ++k) {
-            float pv[RPT], vv[4];
-#pragma unroll
-            for (int i = 0; i < RPT; ++i) pv[i] = s_pT[k * LD + ty * RPT + i];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) vv[j] = j < cw ? s_v[k * 64 + tx * cw + j] : 0.f;
-#pragma unroll
-            for (int i = 0; i < RPT; ++i)
-#pragma unroll
-                for (int j = 0; j < 4; ++j) o_acc[i][j] = fmaf(pv[i], vv[j], o_acc[i][j]);
-        }
-    }
-#pragma unroll
-    for (int i = 0; i < RPT; ++i) {
-        const int r = r0 + ty * RPT + i;
-        if (r < len) {
-            const float inv = 1.f / l_run[i];
-            const size_t ob = (size_t)(t0 + r) * d + h * dh + tx * cw;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) if (j < cw) split_f16(o_acc[i][j] * inv, out_hi[ob + j], out_lo[ob + j]);
-        }
-    }
-}
-
+// ------------------------------------------------------------------------------- attention
 // ---- tensor-core attention: mma.sync m16n8k16 on the split fp16 planes the QKV projection writes, fp32 accumulators and
 // fp32 max-subtracted softmax.  Every product is the error-compensated 3-MMA form of the GEMMs above:
 //   A . B^T = hiA.hiB + 2^-11 (hiA.loB + loA.hiB).
@@ -932,12 +618,6 @@ cls_normalize_kernel(const float* __restrict__ x, const int32_t* __restrict__ se
 }
 
 // ------------------------------------------------------------------------------------ host
-static bool pdl_enabled()
-{
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("KRAG_PDL"); v = (e == nullptr || e[0] != '0') ? 1 : 0; }
-    return v == 1;
-}
 // launch with programmatic stream serialization (see pdl_wait in tc_ptx.cuh); only for kernels that call pdl_wait()
 template <typename... KArgs, typename... Args>
 static void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args)
@@ -948,7 +628,7 @@ static void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.numAttrs = 1;
     KRAG_CUDA(cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...));
     count_launch();
 }
@@ -1031,17 +711,13 @@ void launch_linear(const DeviceInfo& di, const SplitMat& A, const SplitMat& B, i
                    bool gelu, float* C, uint16_t* C_hi, uint16_t* C_lo, const float* ln_g, const float* ln_b, float eps, float* Y,
                    uint16_t* Y_hi, uint16_t* Y_lo, float* ws, size_t ws_floats, cudaStream_t st)
 {
-    static int use_sk = -1;
-    if (use_sk < 0) { const char* ev = getenv("KRAG_GEMM_SPLITK"); use_sk = (ev == nullptr || ev[0] != '0') ? 1 : 0; }
     if (ln_g && N > 32 * LN_MAX_GROUPS * 8) throw std::runtime_error("launch_linear: fused LayerNorm rows hold at most 1024 elements");
     const int m_tiles = (M + GM_TILE - 1) / GM_TILE;
     const int tiles128 = m_tiles * (N / GM_TILE);
-    if (use_sk && ws && tiles128 < di.sm_count / 2 && N % 64 == 0 && K % GH_KB == 0 && (!ln_g || N <= 1024)) {
+    if (ws && tiles128 < di.sm_count / 2 && N % 64 == 0 && K % GH_KB == 0 && (!ln_g || N <= 1024)) {
         // long-K layers over several activation tiles (FFN2 for tens of queries): 128 x 128 tiles halve the operand
         // re-reads through L2 (the binding resource); split-K restores the CTA count
-        static int use_wide = -1;
-        if (use_wide < 0) { const char* ev = getenv("KRAG_SK_WIDE"); use_wide = (ev == nullptr || ev[0] != '0') ? 1 : 0; }
-        const int BN = m_tiles == 1 ? 32 : ((use_wide && K >= 2048 && N % 128 == 0) ? 128 : 64);
+        const int BN = m_tiles == 1 ? 32 : ((K >= 2048 && N % 128 == 0) ? 128 : 64);
         const int ctas = m_tiles * (N / BN), kblocks = K / GH_KB;
         int splits = 1;
         if (ctas <= di.sm_count / 3) {              // 72 CTAs with the whole K range beat 144 + a reduce kernel
@@ -1100,8 +776,9 @@ struct Embedder {
     // workspaces, grown on demand
     int cap_tok = 0, cap_batch = 0;
     DevArray<int32_t> d_tok, d_pos, d_off;
-    DevArray<float> x, x2, qkv, out;
+    DevArray<float> x, x2, out;
     DevArray<uint16_t> xs, cs, fs;        // split planes [2][T][*] of x (LayerNorm outputs), attention context, FFN1 output
+    DevArray<uint16_t> qkv;               // split planes [2][n_tok][3d] of the QKV projection (the lo plane starts at n_tok rows)
     DevArray<float> ws;                   // split-K partials (small token counts)
     static constexpr size_t WS_FLOATS = (size_t)4 << 20;
 
@@ -1231,7 +908,7 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
         e->d_tok.release(); e->d_pos.release(); e->d_off.release(); e->x.release(); e->x2.release(); e->qkv.release();
         e->xs.release(); e->cs.release(); e->fs.release(); e->out.release();
         e->d_tok.alloc(T); e->d_pos.alloc(T); e->d_off.alloc(Bc + 1);
-        e->x.alloc(T * d); e->x2.alloc(T * d); e->qkv.alloc(T * 3 * d);
+        e->x.alloc(T * d); e->x2.alloc(T * d); e->qkv.alloc(2 * T * 3 * d);
         e->xs.alloc(2 * T * d); e->cs.alloc(2 * T * d); e->fs.alloc(2 * T * c.inter);
         e->out.alloc(Bc * d);
         e->cap_tok = (int)T; e->cap_batch = (int)Bc;
@@ -1251,50 +928,15 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
                e->t["embeddings.token_type_embeddings.weight"].p, e->t["embeddings.LayerNorm.weight"].p, e->t["embeddings.LayerNorm.bias"].p, e->x.p,
                xs.hi, xs.lo, n_tok, d, c.vocab, c.eps);
     const int dh = d / c.heads;
-    const size_t at_smem = sizeof(float) * ((size_t)AT_ROWS * dh + (size_t)dh * (AT_CHUNK + 1) + (size_t)AT_CHUNK * dh + (size_t)AT_ROWS * max_len);
-    const size_t ats_smem32 = sizeof(float) * ((size_t)2 * 64 * (32 + 4) + (size_t)32 * 64 + (size_t)32 * (32 + 4));
-    const size_t ats_smem64 = sizeof(float) * ((size_t)2 * 64 * (64 + 4) + (size_t)64 * 64 + (size_t)64 * (64 + 4));
-    static bool at_attr = false;
-    if (!at_attr) {
-        KRAG_CUDA(cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-        KRAG_CUDA(cudaFuncSetAttribute(attention_tiled_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 80 * 1024));
-        KRAG_CUDA(cudaFuncSetAttribute(attention_tiled_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 80 * 1024));
-        KRAG_CUDA(cudaFuncSetAttribute(attention_flash_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 80 * 1024));
-        at_attr = true;
-    }
-    static int use_mma = -1;
-    if (use_mma < 0) { const char* ev = getenv("KRAG_ATTN_MMA"); use_mma = (ev == nullptr || ev[0] != '0') ? 1 : 0; }
-    static int use_flash = -1;
-    if (use_flash < 0) { const char* ev = getenv("KRAG_ATTN_FLASH"); use_flash = (ev == nullptr || ev[0] != '0') ? 1 : 0; }
+    // the QKV projection writes the split planes only (same bytes as an fp32 matrix); attention reads them on the tensor cores
+    uint16_t* q_hi = e->qkv.p;
+    uint16_t* q_lo = q_hi + (size_t)n_tok * 3 * d;
     for (int l = 0; l < c.layers; ++l) {
         const size_t L = (size_t)l;
-        if (use_mma) {
-            // QKV projection writes the split planes only (same bytes as the fp32 matrix they replace); attention on the tensor cores
-            uint16_t* q_hi = reinterpret_cast<uint16_t*>(e->qkv.p);
-            uint16_t* q_lo = q_hi + (size_t)n_tok * 3 * d;
-            launch_linear(e->di, xs, e->s_qkv[L], n_tok, 3 * d, d, e->bqkv[L].p, nullptr, false, nullptr, q_hi, q_lo, nullptr, nullptr, 0.f,
-                          nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st);
-            if (dh == 64) attention_mma<64>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, st);
-            else attention_mma<32>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, st);
-        } else {
-        // KRAG_ATTN_MMA=0: fp32 qkv and the fp32 CUDA-core attention kernels
-        launch_linear(e->di, xs, e->s_qkv[L], n_tok, 3 * d, d, e->bqkv[L].p, nullptr, false, e->qkv.p, nullptr, nullptr, nullptr, nullptr, 0.f,
+        launch_linear(e->di, xs, e->s_qkv[L], n_tok, 3 * d, d, e->bqkv[L].p, nullptr, false, nullptr, q_hi, q_lo, nullptr, nullptr, 0.f,
                       nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st);
-        if (max_len <= 32) {
-            launch_pdl(attention_tiled_kernel<32>, dim3((unsigned)batch, (unsigned)c.heads), dim3(128), ats_smem32, st, e->qkv.p, e->d_off.p, cs.hi, cs.lo, d, c.heads);
-        } else if (max_len <= ATS_MAX) {
-            launch_pdl(attention_tiled_kernel<64>, dim3((unsigned)batch, (unsigned)c.heads), dim3(128), ats_smem64, st, e->qkv.p, e->d_off.p, cs.hi, cs.lo, d, c.heads);
-        } else {
-            if (use_flash)
-                attention_flash_kernel<<<dim3((unsigned)((max_len + 63) / 64), (unsigned)c.heads, (unsigned)batch), 128, ats_smem64, st>>>(
-                    e->qkv.p, e->d_off.p, cs.hi, cs.lo, d, c.heads);
-            else
-                attention_kernel<<<dim3((unsigned)((max_len + AT_ROWS - 1) / AT_ROWS), (unsigned)c.heads, (unsigned)batch), 256, at_smem, st>>>(
-                    e->qkv.p, e->d_off.p, cs.hi, cs.lo, d, c.heads, max_len);
-            KRAG_CUDA(cudaGetLastError());
-            count_launch();
-        }
-        }
+        if (dh == 64) attention_mma<64>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, st);
+        else attention_mma<32>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, st);
         // O projection (+bias +residual) -> LayerNorm -> x (fp32 residual stream) + its split planes
         launch_linear(e->di, cs, e->s_o[L], n_tok, d, d, e->t[lname(l, "attention.output.dense.bias")].p, e->x.p, false, e->x2.p, nullptr, nullptr,
                       e->t[lname(l, "attention.output.LayerNorm.weight")].p, e->t[lname(l, "attention.output.LayerNorm.bias")].p, c.eps, e->x.p, xs.hi, xs.lo,
@@ -1308,14 +950,12 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
                       Embedder::WS_FLOATS, st);
     }
     };   // run_layers
-    static int use_graph = -1;
-    if (use_graph < 0) { const char* ev = getenv("KRAG_EMBED_GRAPH"); use_graph = (ev == nullptr || ev[0] != '0') ? 1 : 0; }
     const std::tuple<int, int, int> key(n_tok, batch, max_len);
     auto git = e->graphs.find(key);
-    if (use_graph && git != e->graphs.end()) {
+    if (git != e->graphs.end()) {
         KRAG_CUDA(cudaGraphLaunch(git->second, st));
         count_launch(1 + 7 * c.layers);
-    } else if (use_graph && (e->seen.size() > 4096 ? (e->seen.clear(), false) : e->seen[key]++ >= 1)) {
+    } else if (e->seen.size() > 4096 ? (e->seen.clear(), false) : e->seen[key]++ >= 1) {
         if (e->graphs.size() >= 64) e->drop_graphs();
         cudaGraph_t g = nullptr;
         cudaGraphExec_t ex = nullptr;

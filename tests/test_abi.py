@@ -48,6 +48,27 @@ def test_product_package_never_imports_oracle():
                 assert "libkrag_oracle" not in txt and not re.search(r'#include\s*"[^"]*oracle', txt), f
 
 
+def test_every_env_variable_the_library_reads_is_documented():
+    """each KRAG_* variable the native library reads is a supported setting, listed in INTEGRATION.md's variable table"""
+    read = set()
+    csrc = os.path.join(ROOT, "kaito_b200", "csrc")
+    for f in sorted(os.listdir(csrc)):
+        if not f.endswith((".cu", ".cuh", ".h", ".cpp")):
+            continue
+        txt = open(os.path.join(csrc, f)).read()
+        read |= set(re.findall(r'\b(?:getenv|env_int)\(\s*"(KRAG_[A-Z0-9_]+)"', txt))
+    assert read, "no getenv(\"KRAG_...\") found: the pattern no longer matches the sources"
+    lines = open(os.path.join(ROOT, "INTEGRATION.md")).read().splitlines()
+    start = lines.index("| variable | default | effect |")
+    table = []
+    for line in lines[start + 2:]:
+        if not line.startswith("|"):
+            break
+        table.append(line.split("|")[1])
+    documented = set(re.findall(r"`(KRAG_[A-Z0-9_]+)`", "\n".join(table)))
+    assert sorted(read - documented) == []
+
+
 def test_header_is_plain_c99_and_links(tmp_path):
     """include/kaito_rag.h is consumed by cgo: it must compile as C99 (no C++-isms, no torch/CUDA types) and a C program
     calling an entry point must link against libkaito_rag.so (no compute call: there is no GPU here)."""

@@ -200,11 +200,11 @@ def test_bm25_overflow_takes_the_exact_safety_net(sparse_400k, oracle, monkeypat
 
 
 def test_bm25_legacy_kernel_still_exact(sparse_400k, oracle, monkeypatch):
-    """KRAG_BM25_LEGACY=1: the CTA-per-tile kernel alone (the safety net) on the 4096-doc tile index and 2048-posting short lists"""
+    """KRAG_BM25_KERNEL=legacy: the CTA-per-tile kernel alone (the safety net) on the 4096-doc tile index and 2048-posting short lists"""
     ix, post, n, vocab = sparse_400k
     qs = oracle.synth_query_terms(vocab, 10, seed=7, rank_offset=20)
     qs[1] = np.random.default_rng(9).integers(0, 3000, 40).astype(np.uint32)
-    monkeypatch.setenv("KRAG_BM25_LEGACY", "1")
+    monkeypatch.setenv("KRAG_BM25_KERNEL", "legacy")
     _bm25_batch_vs_oracle(ix, oracle, post, qs, (30, 300))
 
 
