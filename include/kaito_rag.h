@@ -59,6 +59,13 @@ extern "C" {
 
 #define KRAG_DENSE_TC_TF32 4 /* K2 with the fp32 rows consumed directly as TF32 (tf32 wgmma), kept for comparison */
 
+/* Where an index keeps its fp32 rows (krag_config.row_storage; every index created or loaded in the context).
+ * HOST: the fp32 rows live in pinned host memory; the device holds a bf16 copy (2 B per element) plus 8 B per row of
+ * metadata.  Searches prune on the bf16 copy and rescore exactly from the host rows: returned distances and ids are
+ * bit-identical to DEVICE mode, ties included.  KRAG_DENSE_SCAN streams the host rows through the exact scan instead. */
+#define KRAG_ROWS_DEVICE 0
+#define KRAG_ROWS_HOST 1
+
 typedef struct krag_ctx krag_ctx;
 typedef struct krag_index krag_index;
 
@@ -68,7 +75,8 @@ typedef struct krag_config {
     int32_t world_size;     /* number of shards (1 when single GPU) */
     int32_t dense_mode;     /* KRAG_DENSE_* */
     int32_t search_slots;   /* concurrent search workspaces (0 = default 4) */
-    int32_t reserved[3];
+    int32_t row_storage;    /* KRAG_ROWS_* (0 = device) */
+    int32_t reserved[2];
 } krag_config;
 
 typedef struct krag_stats_t {
@@ -96,6 +104,8 @@ int32_t krag_shutdown(krag_ctx* ctx);
 int64_t krag_launch_count(krag_ctx* ctx);
 /* device memory this process currently holds through libkaito_rag, in bytes (every context, index and embedder) */
 int64_t krag_device_bytes(void);
+/* pinned host memory this process currently holds through libkaito_rag, in bytes (KRAG_ROWS_HOST rows) */
+int64_t krag_host_pinned_bytes(void);
 void* krag_ctx_stream(krag_ctx* ctx);  /* cudaStream_t of search slot 0 (for event timing) */
 
 /* ------------------------------------------------------------------------- index */
@@ -277,17 +287,22 @@ int32_t krag_debug_linear_ln(krag_ctx* ctx, int32_t M, int32_t N, int32_t K, con
                              float eps, float* Y_out);
 /* Switch the dense kernel policy (KRAG_DENSE_*) of the context this index lives in.  Switching to KRAG_DENSE_TC_BF16
  * builds the index's bf16 shadow if it does not exist yet (one conversion pass over the fp32 rows); switching away
- * keeps the shadow unless release_shadow != 0.  Results never change: every mode returns exact fp32 distances. */
+ * keeps the shadow unless release_shadow != 0.  Results never change: every mode returns exact fp32 distances.
+ * A KRAG_ROWS_HOST index always keeps its bf16 rows (they are its device copy): release_shadow is ignored there. */
 int32_t krag_index_set_dense_mode(krag_index* idx, int32_t dense_mode, int32_t release_shadow);
 /* queries whose tensor-core result failed the exactness certificate and were re-run on the
  * exact scan kernel (process-wide counter) */
 int64_t krag_tc_fallback_queries(void);
+/* rows rescored from host memory by KRAG_ROWS_HOST searches (process-wide counter) */
+int64_t krag_host_rows_fetched(void);
 /* CUDA-event duration of the dominant dense kernel of the last search on this process
- * (kernel_id 1 = K1 exact scan; K2 main pass: 3 = TF32, 4 = bf16 shadow, 5 = fp32 rows rounded to bf16 on chip), with the algorithmic bytes and
+ * (kernel_id 1 = K1 exact scan; K2 main pass: 3 = TF32, 4 = bf16 shadow, 5 = fp32 rows rounded to bf16 on chip,
+ * 6 = device bf16 rows of a KRAG_ROWS_HOST index), with the algorithmic bytes and
  * flops of that launch -- bench.py's roofline line is computed from it. */
 int32_t krag_last_dense_kernel(float* ms, int32_t* kernel_id, int64_t* algorithmic_bytes, int64_t* flops);
 /* raw K2 output a[j][r] = |x_r|^2 - 2 x_r.q_j (TF32) for every row, [nq_pad][S] row-major;
- * call with out == NULL to query S and nq_pad.  Test hook for the tensor-core kernel. */
+ * call with out == NULL to query S and nq_pad.  Test hook for the tensor-core kernel; KRAG_E_UNSUPPORTED for
+ * KRAG_ROWS_HOST indexes. */
 int32_t krag_debug_tc_dump(krag_index* idx, int32_t nq, const float* q, float* out, int64_t out_elems,
                            int64_t* S_out, int32_t* nq_pad_out);
 

@@ -22,6 +22,7 @@ KRAG_MAX_POOL = 1024
 FUSION_REFERENCE, FUSION_SIMILARITY = 0, 1
 FILTER_PUSHDOWN = 0x100   # OR into fusion_mode: the allow bitmap restricts the dense and BM25 scans themselves
 DENSE_AUTO, DENSE_SCAN, DENSE_TC, DENSE_TC_BF16, DENSE_TC_TF32 = 0, 1, 2, 3, 4
+ROWS_DEVICE, ROWS_HOST = 0, 1   # krag_config.row_storage: fp32 rows in HBM, or in pinned host memory with a bf16 device copy
 
 # every symbol include/kaito_rag.h declares (tests check the export table against this)
 SYMBOLS = [
@@ -35,6 +36,7 @@ SYMBOLS = [
     "krag_embedder_finalize", "krag_embed", "krag_embed_dev", "krag_embedder_destroy", "krag_debug_gemm_tf32",
     "krag_debug_linear_ln", "krag_index_set_dense_mode", "krag_text_analyze", "krag_wordpiece_create",
     "krag_wordpiece_encode_batch", "krag_wordpiece_destroy", "krag_p2p_create", "krag_p2p_connect", "krag_dev_exchange_merge", "krag_p2p_destroy",
+    "krag_host_pinned_bytes", "krag_host_rows_fetched",
 ]
 
 
@@ -46,7 +48,7 @@ class KragError(RuntimeError):
 
 class Config(C.Structure):
     _fields_ = [("device_id", C.c_int32), ("rank", C.c_int32), ("world_size", C.c_int32), ("dense_mode", C.c_int32),
-                ("search_slots", C.c_int32), ("reserved", C.c_int32 * 3)]
+                ("search_slots", C.c_int32), ("row_storage", C.c_int32), ("reserved", C.c_int32 * 2)]
 
 
 class Stats(C.Structure):
@@ -81,6 +83,8 @@ def load() -> C.CDLL:
     L.krag_launch_count.argtypes = [vp]
     L.krag_launch_count.restype = i64
     L.krag_device_bytes.restype = i64
+    L.krag_host_pinned_bytes.restype = i64
+    L.krag_host_rows_fetched.restype = i64
     L.krag_ctx_stream.argtypes = [vp]
     L.krag_ctx_stream.restype = vp
     L.krag_index_create.argtypes = [vp, C.c_char_p, i32, C.POINTER(vp)]
@@ -160,14 +164,32 @@ def device_bytes() -> int:
     return int(load().krag_device_bytes())
 
 
+def row_storage_from_env(environ=None) -> int:
+    """KRAG_ROW_STORAGE=device|host (default device) -> ROWS_DEVICE / ROWS_HOST; any other value raises ValueError"""
+    v = (os.environ if environ is None else environ).get("KRAG_ROW_STORAGE", "device").strip().lower()
+    if v not in ("device", "host"):
+        raise ValueError(f"KRAG_ROW_STORAGE={v!r}: expected 'device' or 'host'")
+    return ROWS_HOST if v == "host" else ROWS_DEVICE
+
+
+def host_pinned_bytes() -> int:
+    """pinned host memory, in bytes, this process currently holds through the library (ROWS_HOST rows)"""
+    return int(load().krag_host_pinned_bytes())
+
+
+def host_rows_fetched() -> int:
+    """rows rescored from host memory by ROWS_HOST searches so far (process-wide)"""
+    return int(load().krag_host_rows_fetched())
+
+
 class Context:
-    """krag_ctx: one per process per GPU."""
+    """krag_ctx: one per process per GPU.  row_storage applies to every index created or loaded in the context."""
 
     def __init__(self, device_id: int = 0, rank: int = 0, world_size: int = 1, dense_mode: int = DENSE_AUTO,
-                 search_slots: int = 0):
+                 search_slots: int = 0, row_storage: int = ROWS_DEVICE):
         L = load()
         cfg = Config(device_id=device_id, rank=rank, world_size=world_size, dense_mode=dense_mode,
-                     search_slots=search_slots)
+                     search_slots=search_slots, row_storage=row_storage)
         h = C.c_void_p()
         check(L.krag_init(C.byref(cfg), C.byref(h)))
         self._h, self._L = h, L

@@ -29,6 +29,9 @@ int64_t launch_count() { return g_launches.load(std::memory_order_relaxed); }
 static std::atomic<int64_t> g_device_bytes{0};
 void count_device_bytes(int64_t delta) { g_device_bytes.fetch_add(delta, std::memory_order_relaxed); }
 int64_t device_bytes() { return g_device_bytes.load(std::memory_order_relaxed); }
+static std::atomic<int64_t> g_host_pinned_bytes{0};
+void count_host_pinned_bytes(int64_t delta) { g_host_pinned_bytes.fetch_add(delta, std::memory_order_relaxed); }
+int64_t host_pinned_bytes() { return g_host_pinned_bytes.load(std::memory_order_relaxed); }
 
 // "last dense kernel" diagnostics (krag_last_dense_kernel, read by bench.py).  Process-wide and last-writer-wins: with
 // concurrent searches the numbers describe one of them; the mutex only keeps the record itself consistent.
@@ -105,7 +108,18 @@ struct Slot {
     DevArray<int32_t> out_rank, out_count;
     DevArray<int64_t> out_ord;
     std::vector<float> hq;  // padded query staging
-    ~Slot() { if (st) cudaStreamDestroy(st); }
+    // streamed exact scan over host-resident rows (created on first use)
+    DevArray<float> stage;
+    DevArray<uint64_t> fold, k_sel;
+    DevArray<float> q_sel;
+    cudaStream_t copy_st = nullptr;
+    cudaEvent_t copied[2] = {nullptr, nullptr}, freed[2] = {nullptr, nullptr};
+    ~Slot()
+    {
+        for (cudaEvent_t e : {copied[0], copied[1], freed[0], freed[1]}) if (e) cudaEventDestroy(e);
+        if (copy_st) cudaStreamDestroy(copy_st);
+        if (st) cudaStreamDestroy(st);
+    }
 };
 
 }  // namespace krag
@@ -129,9 +143,12 @@ struct krag_index {
     int dim = 0, dpad = 0;
     std::shared_mutex mu;
     // dense shard
+    bool host_rows = false;         // KRAG_ROWS_HOST: the fp32 rows are Xp (pinned host memory) and X stays empty
     DevArray<float> X;
-    DevArray<float> xnorm;          // |x|^2 per row (K2 epilogue)
-    DevArray<uint16_t> Xh;          // optional bf16 shadow of X (KRAG_DENSE_TC_BF16): prune pass only
+    HostArray<float> Xp;            // host-resident fp32 rows [rows, dpad], zero padded
+    DevArray<float> xnorm;          // |x|^2 per row (K2 epilogue), from the fp32 rows in either storage
+    DevArray<uint16_t> Xh;          // bf16 copy of the rows: optional shadow (KRAG_DENSE_TC_BF16), always present for host rows
+    DevArray<float> xres;           // host rows only: |x - bf16(x)| per row, rounded up (refine bound)
     DevArray<uint32_t> xn_max;      // [1] bits of max |x|^2 (K2 certificate)
     int64_t n_rows = 0, n_live = 0;
     std::vector<uint32_t> alive_h;
@@ -184,6 +201,24 @@ int64_t ord_last(const krag_index* ix) { return ix->ord_base + (ix->n_rows > 0 ?
 
 void check_P(int P) { KRAG_REQUIRE(P >= 1 && P <= KRAG_MAX_POOL, KRAG_E_INVALID, "candidate pool must be in [1, 1024]"); }
 
+// the slot's staging for the streamed scan of a host-rows index, grown to this call's shape
+ScanStaging scan_staging(const krag_index* ix, Slot* s, int batch, int P)
+{
+    if (!s->copy_st) {
+        KRAG_CUDA(cudaStreamCreateWithFlags(&s->copy_st, cudaStreamNonBlocking));
+        for (cudaEvent_t* e : {&s->copied[0], &s->copied[1], &s->freed[0], &s->freed[1]})
+            KRAG_CUDA(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    }
+    const int64_t R = stream_scan_chunk_rows(ix->dpad);
+    const int64_t half = (R < ix->n_rows ? R : ix->n_rows) * ix->dpad;
+    s->stage.reserve(2 * half, 0, s->st);
+    s->fold.reserve(2 * (int64_t)(batch > 256 ? batch : 256) * P, 0, s->st);
+    s->q_sel.reserve((int64_t)256 * ix->dpad, 0, s->st);
+    s->k_sel.reserve((int64_t)256 * P, 0, s->st);
+    return ScanStaging{{s->stage.p, s->stage.p + half}, R, s->copy_st, {s->copied[0], s->copied[1]}, {s->freed[0], s->freed[1]},
+                       s->fold.p, s->q_sel.p, s->k_sel.p};
+}
+
 // dense candidates for device-resident padded queries
 void dense_candidates_dev(krag_index* ix, Slot* s, const float* d_q, int batch, int P, uint64_t* d_keys, cudaStream_t st,
                           const uint32_t* eligible = nullptr)
@@ -197,6 +232,19 @@ void dense_candidates_dev(krag_index* ix, Slot* s, const float* d_q, int batch, 
     KRAG_REQUIRE(ord_last(ix) < 0xFFFFFFFFll, KRAG_E_UNSUPPORTED, "global ordinal exceeds 32 bits");
     s->part.reserve((int64_t)dense_scan_part_elems(c->di, P), 0, st);
     int mode = c->cfg.dense_mode;
+    if (ix->host_rows) {
+        const HostRowsView hr{ix->Xp.h, ix->Xp.d, ix->Xh.p, ix->xres.p};
+        const ScanStaging sg = scan_staging(ix, s, batch, P);
+        if (mode != KRAG_DENSE_SCAN && dense_tc_host_rows_supported(c->di, ix->n_rows, ix->dpad)) {
+            const size_t ws = dense_tc_workspace_bytes(c->di, ix->n_rows, P, true);
+            s->tc_ws.reserve((int64_t)ws, 0, st);
+            if (launch_dense_tc_host(c->di, hr, ix->n_rows, ix->dpad, alive, ix->xnorm.p, ix->xn_max.p, d_q, batch, P, ord_map(ix),
+                                     s->tc_ws.p, ws, s->part.p, sg, d_keys, st))
+                return;
+        }
+        launch_dense_scan_streamed(c->di, ix->Xp.h, ix->n_rows, ix->dpad, alive, d_q, batch, P, ord_map(ix), s->part.p, sg, d_keys, st);
+        return;
+    }
     bool use_tc = (mode == KRAG_DENSE_TC) || (mode == KRAG_DENSE_TC_TF32) || (mode == KRAG_DENSE_TC_BF16 && dense_tc_wants(ix->n_rows, batch)) ||
                   (mode == KRAG_DENSE_AUTO && dense_tc_wants(ix->n_rows, batch));
     if (use_tc && dense_tc_supported(c->di, ix->dpad)) {
@@ -266,9 +314,14 @@ void mark_alive(krag_index* ix, int64_t row0, int64_t n, cudaStream_t st)
 
 void ensure_capacity(krag_index* ix, int64_t rows, int64_t nnz, cudaStream_t st)
 {
-    ix->X.reserve(rows * ix->dpad, ix->n_rows * ix->dpad, st);
+    if (ix->host_rows) {
+        ix->Xp.reserve(rows * ix->dpad, ix->n_rows * ix->dpad);
+        ix->xres.reserve(rows, ix->n_rows, st);
+    } else {
+        ix->X.reserve(rows * ix->dpad, ix->n_rows * ix->dpad, st);
+    }
     ix->xnorm.reserve(rows, ix->n_rows, st);
-    if (ix->ctx->cfg.dense_mode == KRAG_DENSE_TC_BF16 || ix->Xh.p) ix->Xh.reserve(rows * ix->dpad, ix->n_rows * ix->dpad, st);
+    if (ix->ctx->cfg.dense_mode == KRAG_DENSE_TC_BF16 || ix->Xh.p || ix->host_rows) ix->Xh.reserve(rows * ix->dpad, ix->n_rows * ix->dpad, st);
     if (ix->xn_max.p == nullptr) {
         ix->xn_max.reserve(1, 0, st);
         KRAG_CUDA(cudaMemsetAsync(ix->xn_max.p, 0, sizeof(uint32_t), st));
@@ -279,6 +332,32 @@ void ensure_capacity(krag_index* ix, int64_t rows, int64_t nnz, cudaStream_t st)
         ix->tid.reserve(nnz > 0 ? nnz : 1, ix->nnz, st);
         ix->ttf.reserve(nnz > 0 ? nnz : 1, ix->nnz, st);
     }
+}
+
+// Host rows [row0, row0 + n) -> xnorm (row_norms_kernel, as for device rows), the bf16 copy and xres, streamed through a
+// device staging buffer that is freed before returning.  gen_seed != nullptr: the rows are first generated on the device
+// (krag_synth_fill, global rows row_base + r) and copied to the pinned rows; otherwise they are already there.
+void derive_host_rows(krag_index* ix, int64_t row0, int64_t n, cudaStream_t st, const uint64_t* gen_seed = nullptr,
+                      int64_t row_base = 0)
+{
+    if (n == 0) return;
+    const int64_t R = stream_scan_chunk_rows(ix->dpad);
+    const int dp = ix->dpad;
+    DevArray<float> stage;
+    stage.alloc((n < R ? n : R) * dp);
+    for (int64_t r = row0; r < row0 + n; r += R) {
+        const int64_t m = row0 + n - r < R ? row0 + n - r : R;
+        float* host = ix->Xp.h + r * dp;
+        if (gen_seed) {
+            launch_synth_dense(stage.p, m, ix->dim, dp, row_base + r, *gen_seed, st);
+            KRAG_CUDA(cudaMemcpyAsync(host, stage.p, sizeof(float) * (size_t)(m * dp), cudaMemcpyDeviceToHost, st));
+        } else {
+            KRAG_CUDA(cudaMemcpyAsync(stage.p, host, sizeof(float) * (size_t)(m * dp), cudaMemcpyHostToDevice, st));
+        }
+        launch_row_norms(stage.p, 0, m, dp, ix->xnorm.p + r, ix->xn_max.p, st);
+        launch_bf16_residual(stage.p, m, dp, ix->Xh.p + r * dp, ix->xres.p + r, st);
+    }
+    KRAG_CUDA(cudaStreamSynchronize(st));
 }
 
 void commit_local_impl(krag_index* ix, int64_t vocab, uint32_t* df_out, int64_t* n_live_out, int64_t* total_len_out)
@@ -364,6 +443,8 @@ int32_t krag_init(const krag_config* cfg, krag_ctx** out)
         KRAG_REQUIRE(e == cudaSuccess && n > 0, KRAG_E_NO_DEVICE,
                      std::string("no CUDA device: ") + cudaGetErrorString(e) + " (libkaito_rag has no CPU fallback)");
         KRAG_REQUIRE(cfg->device_id >= 0 && cfg->device_id < n, KRAG_E_INVALID, "device_id out of range");
+        KRAG_REQUIRE(cfg->row_storage == KRAG_ROWS_DEVICE || cfg->row_storage == KRAG_ROWS_HOST, KRAG_E_INVALID,
+                     "row_storage must be KRAG_ROWS_DEVICE or KRAG_ROWS_HOST");
         KRAG_CUDA(cudaSetDevice(cfg->device_id));
         cudaDeviceProp p;
         KRAG_CUDA(cudaGetDeviceProperties(&p, cfg->device_id));
@@ -401,6 +482,7 @@ int32_t krag_shutdown(krag_ctx* c)
 
 int64_t krag_launch_count(krag_ctx*) { return launch_count(); }
 int64_t krag_device_bytes(void) { return device_bytes(); }
+int64_t krag_host_pinned_bytes(void) { return host_pinned_bytes(); }
 void* krag_ctx_stream(krag_ctx* c) { return c ? (void*)c->all_slots[0]->st : nullptr; }
 
 int32_t krag_index_create(krag_ctx* c, const char* name, int32_t dim, krag_index** out)
@@ -414,6 +496,7 @@ int32_t krag_index_create(krag_ctx* c, const char* name, int32_t dim, krag_index
         ix->dim = dim;
         ix->dpad = (dim + KRAG_LANES - 1) / KRAG_LANES * KRAG_LANES;
         ix->ord_base = 0;
+        ix->host_rows = c->cfg.row_storage == KRAG_ROWS_HOST;
         *out = ix;
     });
 }
@@ -468,15 +551,28 @@ int32_t krag_index_add(krag_index* ix, int64_t n, const uint64_t* node_ids, cons
         KRAG_REQUIRE(!sparse || (term_offsets[0] == 0 && add_nnz >= 0), KRAG_E_INVALID, "term_offsets must start at 0");
         ensure_capacity(ix, ix->n_rows + n, sparse ? ix->nnz + add_nnz : -1, st);
         float* dst = ix->X.p + ix->n_rows * ix->dpad;
-        if (ix->dim == ix->dpad) {
+        if (ix->host_rows) {
+            float* h = ix->Xp.h + ix->n_rows * ix->dpad;
+            if (ix->dim == ix->dpad) {
+                memcpy(h, vecs, sizeof(float) * (size_t)n * ix->dim);
+            } else {
+                for (int64_t i = 0; i < n; ++i) {
+                    memcpy(h + i * ix->dpad, vecs + i * ix->dim, sizeof(float) * ix->dim);
+                    memset(h + i * ix->dpad + ix->dim, 0, sizeof(float) * (ix->dpad - ix->dim));
+                }
+            }
+            derive_host_rows(ix, ix->n_rows, n, st);
+        } else if (ix->dim == ix->dpad) {
             KRAG_CUDA(cudaMemcpyAsync(dst, vecs, sizeof(float) * (size_t)n * ix->dim, cudaMemcpyHostToDevice, st));
         } else {
             KRAG_CUDA(cudaMemsetAsync(dst, 0, sizeof(float) * (size_t)n * ix->dpad, st));
             KRAG_CUDA(cudaMemcpy2DAsync(dst, sizeof(float) * ix->dpad, vecs, sizeof(float) * ix->dim, sizeof(float) * ix->dim,
                                         (size_t)n, cudaMemcpyHostToDevice, st));
         }
-        launch_row_norms(ix->X.p, ix->n_rows, n, ix->dpad, ix->xnorm.p, ix->xn_max.p, st);
-        if (ix->Xh.p) launch_f32_to_bf16(dst, ix->Xh.p + ix->n_rows * ix->dpad, n * ix->dpad, st);
+        if (!ix->host_rows) {
+            launch_row_norms(ix->X.p, ix->n_rows, n, ix->dpad, ix->xnorm.p, ix->xn_max.p, st);
+            if (ix->Xh.p) launch_f32_to_bf16(dst, ix->Xh.p + ix->n_rows * ix->dpad, n * ix->dpad, st);
+        }
         std::vector<int64_t> shifted;
         if (sparse) {
             shifted.resize((size_t)n + 1);
@@ -587,7 +683,7 @@ int32_t krag_index_stats(krag_index* ix, krag_stats_t* out)
         out->n_docs_global = ix->n_docs_global; out->total_len_global = ix->total_len_global; out->vocab = ix->vocab;
         out->ordinal_base = ix->ord_base; out->dim = ix->dim; out->dim_padded = ix->dpad;
         out->committed = ix->committed && ix->committed_rows == ix->n_rows;
-        out->device_bytes = ix->X.bytes() + ix->Xh.bytes() + ix->xnorm.bytes() + ix->alive_d.bytes() + ix->toff.bytes() + ix->tid.bytes() + ix->ttf.bytes() +
+        out->device_bytes = ix->X.bytes() + ix->Xh.bytes() + ix->xres.bytes() + ix->xnorm.bytes() + ix->alive_d.bytes() + ix->toff.bytes() + ix->tid.bytes() + ix->ttf.bytes() +
                             ix->dlen.bytes() + (ix->committed ? (int64_t)(ix->post.nnz * 8 + (ix->post.vocab + 1) * 8) : 0);
     });
 }
@@ -786,9 +882,13 @@ int32_t krag_synth_fill(krag_index* ix, int64_t n, int64_t row_base, uint64_t se
         cudaStream_t st = ix->ctx->admin;
         KRAG_REQUIRE(ix->n_rows == 0, KRAG_E_STATE, "synthetic fill needs an empty index");
         ensure_capacity(ix, n, -1, st);
-        launch_synth_dense(ix->X.p, n, ix->dim, ix->dpad, row_base, seed, st);
-        launch_row_norms(ix->X.p, 0, n, ix->dpad, ix->xnorm.p, ix->xn_max.p, st);
-        if (ix->Xh.p) launch_f32_to_bf16(ix->X.p, ix->Xh.p, n * ix->dpad, st);
+        if (ix->host_rows) {
+            derive_host_rows(ix, 0, n, st, &seed, row_base);
+        } else {
+            launch_synth_dense(ix->X.p, n, ix->dim, ix->dpad, row_base, seed, st);
+            launch_row_norms(ix->X.p, 0, n, ix->dpad, ix->xnorm.p, ix->xn_max.p, st);
+            if (ix->Xh.p) launch_f32_to_bf16(ix->X.p, ix->Xh.p, n * ix->dpad, st);
+        }
         if (vocab > 0) {
             DevArray<int64_t> off; DevArray<uint32_t> ids; DevArray<uint16_t> tf; DevArray<uint32_t> dl; int64_t nnz = 0;
             synth_sparse(n, row_base, seed, vocab, off, ids, tf, dl, &nnz, st);
@@ -812,6 +912,10 @@ int32_t krag_index_read_rows(krag_index* ix, int64_t row0, int64_t n, float* out
         std::shared_lock<std::shared_mutex> lk(ix->mu);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         if (n == 0) return;
+        if (ix->host_rows) {
+            for (int64_t i = 0; i < n; ++i) memcpy(out + i * ix->dim, ix->Xp.h + (row0 + i) * ix->dpad, sizeof(float) * ix->dim);
+            return;
+        }
         KRAG_CUDA(cudaMemcpy2D(out, sizeof(float) * ix->dim, ix->X.p + row0 * ix->dpad, sizeof(float) * ix->dpad,
                                sizeof(float) * ix->dim, (size_t)n, cudaMemcpyDeviceToHost));
     });
@@ -846,13 +950,14 @@ int32_t krag_index_set_dense_mode(krag_index* ix, int32_t dense_mode, int32_t re
             ix->Xh.reserve(ix->X.cap, 0, st);                     // same capacity as the fp32 rows: later appends convert in place
             launch_f32_to_bf16(ix->X.p, ix->Xh.p, ix->n_rows * ix->dpad, st);
         }
-        if (dense_mode != KRAG_DENSE_TC_BF16 && release_shadow) ix->Xh.release();
+        if (dense_mode != KRAG_DENSE_TC_BF16 && release_shadow && !ix->host_rows) ix->Xh.release();   // host rows: Xh is the device copy
         KRAG_CUDA(cudaStreamSynchronize(st));
         ix->ctx->cfg.dense_mode = dense_mode;
     });
 }
 
 int64_t krag_tc_fallback_queries(void) { return dense_tc_fallback_queries(); }
+int64_t krag_host_rows_fetched(void) { return host_rows_fetched(); }
 
 int32_t krag_last_dense_kernel(float* ms, int32_t* kernel_id, int64_t* algorithmic_bytes, int64_t* flops)
 {
@@ -869,6 +974,7 @@ int32_t krag_debug_tc_dump(krag_index* ix, int32_t nq, const float* q, float* ou
     return guarded([&] {
         KRAG_REQUIRE(ix && q && S_out && nq_pad_out && nq >= 1 && nq <= 256, KRAG_E_INVALID, "bad argument");
         std::shared_lock<std::shared_mutex> lk(ix->mu);
+        KRAG_REQUIRE(!ix->host_rows, KRAG_E_UNSUPPORTED, "the fp32 tensor-core dump needs device-resident rows");
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         SlotLease lease(ix->ctx);
         Slot* s = lease.s;
@@ -1074,8 +1180,13 @@ int32_t krag_index_persist(krag_index* ix, const char* dir)
         std::vector<float> rows((size_t)chunk * ix->dim);
         for (int64_t r = 0; r < ix->n_rows; r += chunk) {
             int64_t m = ix->n_rows - r < chunk ? ix->n_rows - r : chunk;
-            KRAG_CUDA(cudaMemcpy2D(rows.data(), sizeof(float) * ix->dim, ix->X.p + r * ix->dpad, sizeof(float) * ix->dpad,
-                                   sizeof(float) * ix->dim, (size_t)m, cudaMemcpyDeviceToHost));
+            if (ix->host_rows) {
+                for (int64_t i = 0; i < m; ++i)
+                    memcpy(rows.data() + i * ix->dim, ix->Xp.h + (r + i) * ix->dpad, sizeof(float) * ix->dim);
+            } else {
+                KRAG_CUDA(cudaMemcpy2D(rows.data(), sizeof(float) * ix->dim, ix->X.p + r * ix->dpad, sizeof(float) * ix->dpad,
+                                       sizeof(float) * ix->dim, (size_t)m, cudaMemcpyDeviceToHost));
+            }
             W(rows.data(), sizeof(float) * (size_t)m * ix->dim);
         }
         if (ix->has_sparse) {

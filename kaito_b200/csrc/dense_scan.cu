@@ -173,4 +173,42 @@ void launch_dense_scan(const DeviceInfo& di, const float* X, int64_t n_rows, int
     }
 }
 
+// chunks of the streamed scan: up to 64 MB or 64K rows, a multiple of 32 rows so a chunk's tombstone words start on a word
+int64_t stream_scan_chunk_rows(int dpad)
+{
+    int64_t r = ((int64_t)64 << 20) / ((int64_t)dpad * 4);
+    if (r > 65536) r = 65536;
+    return r / 32 * 32;
+}
+
+void launch_dense_scan_streamed(const DeviceInfo& di, const float* X_host, int64_t n_rows, int dpad, const uint32_t* alive,
+                                const float* q, int batch, int P, OrdMap ord_base, uint64_t* part, const ScanStaging& sg,
+                                uint64_t* keys_out, cudaStream_t st)
+{
+    const int64_t R = sg.chunk_rows;
+    const int64_t list = (int64_t)batch * P;
+    uint64_t* run = sg.fold;            // running top P
+    uint64_t* chk = sg.fold + list;     // this chunk's top P
+    // the staging buffers are free once the work already queued on st is done
+    KRAG_CUDA(cudaEventRecord(sg.freed[0], st));
+    KRAG_CUDA(cudaEventRecord(sg.freed[1], st));
+    int64_t i = 0;
+    for (int64_t r0 = 0; r0 < n_rows; r0 += R, ++i) {
+        const int b = (int)(i & 1);
+        const int64_t m = n_rows - r0 < R ? n_rows - r0 : R;
+        KRAG_CUDA(cudaStreamWaitEvent(sg.copy, sg.freed[b], 0));
+        KRAG_CUDA(cudaMemcpyAsync(sg.buf[b], X_host + r0 * dpad, sizeof(float) * (size_t)(m * dpad), cudaMemcpyHostToDevice, sg.copy));
+        KRAG_CUDA(cudaEventRecord(sg.copied[b], sg.copy));
+        KRAG_CUDA(cudaStreamWaitEvent(st, sg.copied[b], 0));
+        const OrdMap om{ord_base + (uint32_t)r0, ord_base.stride};
+        launch_dense_scan(di, sg.buf[b], m, dpad, alive ? alive + r0 / 32 : nullptr, q, batch, P, om, part, i == 0 ? run : chk, st);
+        KRAG_CUDA(cudaEventRecord(sg.freed[b], st));
+        if (i > 0) {
+            launch_merge(run, 2, P, batch, P, list, P, keys_out, st);
+            if (r0 + R < n_rows) KRAG_CUDA(cudaMemcpyAsync(run, keys_out, sizeof(uint64_t) * (size_t)list, cudaMemcpyDeviceToDevice, st));
+        }
+    }
+    if (i == 1) KRAG_CUDA(cudaMemcpyAsync(keys_out, run, sizeof(uint64_t) * (size_t)list, cudaMemcpyDeviceToDevice, st));
+}
+
 }  // namespace krag

@@ -256,6 +256,38 @@ void launch_f32_to_bf16(const float* in, uint16_t* out, int64_t n_elems, cudaStr
     count_launch();
 }
 
+// host-resident rows: bf16 copy (round to nearest even, as f32_to_bf16_kernel) and r = |x - bf16(x)| rounded up, one warp per
+// row.  x - bf16(x) is exact in fp32 (the two are within a factor of 2: Sterbenz), so only the sum and the root round, upwards.
+__global__ void __launch_bounds__(256)
+bf16_residual_kernel(const float* __restrict__ X, int64_t n, int dpad, uint16_t* __restrict__ Xh, float* __restrict__ xres)
+{
+    const int lane = threadIdx.x & 31;
+    const int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (r >= n) return;
+    const float4* p = reinterpret_cast<const float4*>(X + r * dpad);
+    uint2* o = reinterpret_cast<uint2*>(Xh + r * dpad);
+    float s = 0.f;
+    for (int i = lane; i < dpad / 4; i += 32) {
+        const float4 v = p[i];
+        const __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
+        const float e0 = v.x - __low2float(a), e1 = v.y - __high2float(a), e2 = v.z - __low2float(b), e3 = v.w - __high2float(b);
+        s = __fmaf_ru(e0, e0, s); s = __fmaf_ru(e1, e1, s); s = __fmaf_ru(e2, e2, s); s = __fmaf_ru(e3, e3, s);
+        uint2 w;
+        w.x = *reinterpret_cast<const uint32_t*>(&a); w.y = *reinterpret_cast<const uint32_t*>(&b);
+        o[i] = w;
+    }
+#pragma unroll
+    for (int k = 16; k > 0; k >>= 1) s = __fadd_ru(s, __shfl_xor_sync(0xffffffffu, s, k));
+    if (lane == 0) xres[r] = __fsqrt_ru(s);
+}
+void launch_bf16_residual(const float* X, int64_t n, int dpad, uint16_t* Xh, float* xres, cudaStream_t st)
+{
+    if (n == 0) return;
+    bf16_residual_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, st>>>(X, n, dpad, Xh, xres);
+    KRAG_CUDA(cudaGetLastError());
+    count_launch();
+}
+
 // ------------------------------------------------------------- row norms (index time)
 __global__ void __launch_bounds__(256)
 row_norms_kernel(const float* __restrict__ X, int64_t row0, int64_t n, int dpad, float* __restrict__ xnorm,
@@ -365,6 +397,126 @@ rescore_kernel(const float* __restrict__ X, int dpad, const float* __restrict__ 
     if (l8 == 0 && c < cap) exact_keys[(size_t)j * cap + c] = valid ? make_key_asc(s, ord_base + row) : KEY_PAD;
 }
 
+// rescore_kernel's arithmetic on rows in pinned host memory, read through their mapped device address (zero-copy over the
+// host link) with plain ld.global: the non-coherent path is not relied on for host-mapped memory
+__global__ void __launch_bounds__(256)
+rescore_mapped_kernel(const float* __restrict__ X, int dpad, const float* __restrict__ Q, const uint32_t* __restrict__ cand_count,
+                      const uint32_t* __restrict__ cand_rows, int cap, OrdMap ord_base, uint64_t* __restrict__ exact_keys)
+{
+    extern __shared__ __align__(16) float rm_q[];   // [dpad]
+    const int j = blockIdx.y, tid = threadIdx.x, lane = tid & 31, l8 = lane & 7;
+    const int cnt = (int)min(cand_count[j], (uint32_t)cap);
+    const int c = blockIdx.x * 32 + (tid >> 3);
+    if (blockIdx.x * 32 >= cnt) {
+        if (l8 == 0 && c < cap) exact_keys[(size_t)j * cap + c] = KEY_PAD;
+        return;
+    }
+    for (int i = tid; i < dpad; i += 256) rm_q[i] = Q[(size_t)j * dpad + i];
+    __syncthreads();
+    const bool valid = c < cnt;
+    const uint32_t row = valid ? cand_rows[(size_t)j * cap + c] : 0u;
+    const float4* p = reinterpret_cast<const float4*>(X + (size_t)row * dpad) + l8;
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    const int steps = dpad / KRAG_LANES;
+#pragma unroll 4
+    for (int i = 0; i < steps; ++i) {
+        float4 a;
+        asm("ld.global.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(a.x), "=f"(a.y), "=f"(a.z), "=f"(a.w) : "l"(p + i * 8));
+        const float4 qv = *reinterpret_cast<const float4*>(rm_q + i * KRAG_LANES + l8 * 4);
+        float t;
+        t = a.x - qv.x; acc.x = fmaf(t, t, acc.x);
+        t = a.y - qv.y; acc.y = fmaf(t, t, acc.y);
+        t = a.z - qv.z; acc.z = fmaf(t, t, acc.z);
+        t = a.w - qv.w; acc.w = fmaf(t, t, acc.w);
+    }
+    float s = (acc.x + acc.y) + (acc.z + acc.w);
+    s += __shfl_xor_sync(0xffffffffu, s, 4);
+    s += __shfl_xor_sync(0xffffffffu, s, 2);
+    s += __shfl_xor_sync(0xffffffffu, s, 1);
+    if (l8 == 0 && c < cap) exact_keys[(size_t)j * cap + c] = valid ? make_key_asc(s, ord_base + row) : KEY_PAD;
+}
+
+// ------------------------------------------------------------- refine (host-resident rows)
+// For every candidate of the main pass, an interval [L, U] that holds its exact distance D = |x - q|^2, computed from the
+// device bf16 copy b = bf16(x) and r >= |x - b| (xres):  |b - q| - r <= |x - q| <= |b - q| + r  (triangle inequality).
+// d_lo <= |b - q|^2 <= d_hi come from directed rounding throughout (no error model needed); then
+//   L = max(0, sqrt_rd(d_lo) - r)^2 rounded down,   U = (sqrt_ru(d_hi) + r)^2 rounded up.
+// One 8-lane group per candidate as in rescore_kernel; lane l8 reads 8 bf16 elements (16 bytes) per 64-element step.
+__device__ __forceinline__ void refine_acc(float b, float q, float& lo, float& hi)
+{
+    // b - q rounded both ways: both results carry the sign of the exact difference (or are zero)
+    const float t_lo = __fsub_rd(b, q), t_hi = __fsub_ru(b, q);
+    const float m_lo = t_lo >= 0.f ? t_lo : -t_hi, m_hi = t_lo >= 0.f ? t_hi : -t_lo;
+    lo = __fmaf_rd(m_lo, m_lo, lo);
+    hi = __fmaf_ru(m_hi, m_hi, hi);
+}
+__global__ void __launch_bounds__(256)
+refine_kernel(const uint16_t* __restrict__ Xh, const float* __restrict__ xres, int dpad, const float* __restrict__ Q,
+              const uint32_t* __restrict__ cand_count, const uint32_t* __restrict__ cand_rows, int cap,
+              float* __restrict__ lo_out, uint64_t* __restrict__ u_keys)
+{
+    extern __shared__ __align__(16) float rf_q[];   // [dpad]
+    const int j = blockIdx.y, tid = threadIdx.x, lane = tid & 31, l8 = lane & 7;
+    const int cnt = (int)min(cand_count[j], (uint32_t)cap);
+    const int c = blockIdx.x * 32 + (tid >> 3);
+    if (blockIdx.x * 32 >= cnt) {
+        if (l8 == 0 && c < cap) u_keys[(size_t)j * cap + c] = KEY_PAD;
+        return;
+    }
+    for (int i = tid; i < dpad; i += 256) rf_q[i] = Q[(size_t)j * dpad + i];
+    __syncthreads();
+    const bool valid = c < cnt;
+    const uint32_t row = valid ? cand_rows[(size_t)j * cap + c] : 0u;
+    const uint4* p = reinterpret_cast<const uint4*>(Xh + (size_t)row * dpad) + l8;
+    float lo = 0.f, hi = 0.f;
+    for (int i = 0; i < dpad / 64; ++i) {
+        const uint4 v = p[i * 8];
+        const float* qv = rf_q + i * 64 + l8 * 8;
+        const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {   // element 2e in the low half of the word, 2e + 1 in the high half
+            refine_acc(__uint_as_float(w[e] << 16), qv[2 * e], lo, hi);
+            refine_acc(__uint_as_float(w[e] & 0xFFFF0000u), qv[2 * e + 1], lo, hi);
+        }
+    }
+#pragma unroll
+    for (int o = 4; o > 0; o >>= 1) {
+        lo = __fadd_rd(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+        hi = __fadd_ru(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+    }
+    if (l8 == 0 && c < cap) {
+        if (valid) {
+            const float r = xres[row];
+            const float a = fmaxf(__fsub_rd(__fsqrt_rd(lo), r), 0.f), b = __fadd_ru(__fsqrt_ru(hi), r);
+            lo_out[(size_t)j * cap + c] = __fmul_rd(a, a);
+            u_keys[(size_t)j * cap + c] = make_key_asc(__fmul_ru(b, b), (uint32_t)c);
+        } else {
+            u_keys[(size_t)j * cap + c] = KEY_PAD;
+        }
+    }
+}
+
+// Fetch rule.  u_top[j * P + P - 1] is U_(P), the P-th smallest U of query j (KEY_PAD: fewer than P candidates, fetch all).
+// K1 rounds a distance D to D1 with |D1 - D| <= gamma D + eta (see fetch_rule_constants).  The P candidates of smallest U
+// have D1 <= (1 + gamma) U_(P) + eta; a candidate with L > T = ((1 + gamma) U_(P) + 2 eta) / (1 - gamma) has
+// D1 >= (1 - gamma) L - eta > (1 + gamma) U_(P) + eta: strictly worse, after K1's own rounding, than P fetched rows, so it
+// cannot be in the top P whatever its ordinal.  Every candidate with L <= T is fetched (those P included: L <= U <= U_(P)).
+__global__ void __launch_bounds__(256)
+fetch_compact_kernel(const uint32_t* __restrict__ cand_count, const uint32_t* __restrict__ cand_rows, int cap,
+                     const float* __restrict__ lo, const uint64_t* __restrict__ u_top, int P, float scale, float eta2,
+                     uint32_t* __restrict__ fetch_count, uint32_t* __restrict__ fetch_rows)
+{
+    const int j = blockIdx.y, c = blockIdx.x * 256 + threadIdx.x;
+    const int cnt = (int)min(cand_count[j], (uint32_t)cap);
+    if (c >= cnt) return;
+    const uint64_t kP = u_top[(size_t)j * P + (P - 1)];
+    const float T = kP == KEY_PAD ? CUDART_INF_F : __fadd_ru(__fmul_ru(key_value_asc(kP), scale), eta2);
+    if (lo[(size_t)j * cap + c] <= T) {
+        const uint32_t pos = atomicAdd(&fetch_count[j], 1u);
+        fetch_rows[(size_t)j * cap + pos] = cand_rows[(size_t)j * cap + c];
+    }
+}
+
 // ------------------------------------------------------------------------ certificate
 __global__ void certify_kernel(const float* __restrict__ Q, int dpad, int nq, int P, const float* __restrict__ thr,
                                const uint32_t* __restrict__ cand_count, int cap, const uint64_t* __restrict__ keys_out,
@@ -442,8 +594,9 @@ static int tc_cap(int P) { return 4 * tc_target(P, true); }   // sized for eithe
 
 struct TcWorkspace {   // carved out of the caller's byte buffer
     float* thr; uint32_t* cand_count; int32_t* flags; uint32_t* cand_rows; uint64_t* exact_keys; float* dump; uint16_t* q_bf16;
+    float* lo; uint32_t* fetch_count; uint32_t* fetch_rows;   // host-resident rows only: refine bounds and fetch lists
 };
-static size_t tc_carve(TcWorkspace* w, unsigned char* base, int cap, int64_t S)
+static size_t tc_carve(TcWorkspace* w, unsigned char* base, int cap, int64_t S, bool host_rows = false)
 {
     size_t o = 0;
     auto take = [&](size_t bytes) { size_t at = o; o = (o + bytes + 255) & ~(size_t)255; return base ? base + at : nullptr; };
@@ -455,6 +608,11 @@ static size_t tc_carve(TcWorkspace* w, unsigned char* base, int cap, int64_t S)
     p = take((size_t)256 * cap * 8); if (w) w->exact_keys = (uint64_t*)p;
     p = take((size_t)256 * S * 4); if (w) w->dump = (float*)p;
     p = take((size_t)256 * 16384 * 2); if (w) w->q_bf16 = (uint16_t*)p;   // queries as bf16 (dim <= 16384)
+    if (host_rows) {
+        p = take((size_t)256 * cap * 4); if (w) w->lo = (float*)p;
+        p = take(256 * 4); if (w) w->fetch_count = (uint32_t*)p;
+        p = take((size_t)256 * cap * 4); if (w) w->fetch_rows = (uint32_t*)p;
+    }
     return o;
 }
 static int64_t tc_sample_tiles(int64_t n_rows)
@@ -462,11 +620,33 @@ static int64_t tc_sample_tiles(int64_t n_rows)
     int64_t n_tiles = (n_rows + TC_TILE_M - 1) / TC_TILE_M;
     return (n_tiles + TC_SAMPLE_STRIDE - 1) / TC_SAMPLE_STRIDE;
 }
-size_t dense_tc_workspace_bytes(const DeviceInfo&, int64_t n_rows, int P)
+size_t dense_tc_workspace_bytes(const DeviceInfo&, int64_t n_rows, int P, bool host_rows)
 {
-    return tc_carve(nullptr, nullptr, tc_cap(P), tc_sample_tiles(n_rows) * TC_TILE_M);
+    return tc_carve(nullptr, nullptr, tc_cap(P), tc_sample_tiles(n_rows) * TC_TILE_M, host_rows);
 }
 bool dense_tc_wants(int64_t n_rows, int batch) { return n_rows >= TC_MIN_ROWS && batch >= 16; }
+bool dense_tc_host_rows_supported(const DeviceInfo& di, int64_t n_rows, int dpad)
+{
+    return n_rows >= TC_MIN_ROWS && n_rows < (1ll << 31) && dpad % (2 * TC_KBLOCK) == 0 && dense_tc_supported(di, dpad);
+}
+
+// Constants of the fetch rule (fetch_compact_kernel).  K1 (dense_scan_kernel, rescore_kernel) computes D = sum (x_i - q_i)^2
+// over nonnegative terms; every term passes through at most m = dpad / 32 + 7 roundings to nearest: its difference (squared:
+// 2), its lane's FFMA chain (dpad / 32 steps), (p0 + p1) + (p2 + p3) (2) and the butterfly over lanes 4, 2, 1 (3).  With
+// u = 2^-24 this gives |D1 - D| <= gamma D + eta, gamma = m u / (1 - m u) (Higham, Lemma 3.1); eta bounds what subnormal
+// results add, at most 2^-150 each over at most dpad + 64 roundings (doubled to cover their propagation through later
+// roundings).  scale >= (1 + gamma) / (1 - gamma) and eta2 >= 2 eta / (1 - gamma), both rounded up.
+static void fetch_rule_constants(int dpad, float* scale, float* eta2)
+{
+    const double u = ldexp(1.0, -24), m = dpad / KRAG_LANES + 7;
+    const double gamma = m * u / (1.0 - m * u);
+    const double eta = (dpad + 64) * ldexp(1.0, -149);
+    *scale = nextafterf((float)((1.0 + gamma) / (1.0 - gamma)), INFINITY);
+    *eta2 = nextafterf((float)(2.0 * eta / (1.0 - gamma)), INFINITY);
+}
+
+static std::atomic<int64_t> g_host_rows_fetched{0};
+int64_t host_rows_fetched() { return g_host_rows_fetched.load(); }
 
 // one launch of the prune kernel (sample pass: MODE = TC_TF32, DUMP) over n_ltiles tiles of 128 rows, tile_stride apart
 template <int NQ, int MODE, bool DUMP>
@@ -489,8 +669,9 @@ template <int NQ>
 static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensorMap& tmQ, const float* X, int64_t n_rows,
                     int dpad, const float* xnorm, const uint32_t* xn_max_bits, const uint32_t* alive, const float* q,
                     int nq, int P, OrdMap ord_base, const TcWorkspace& w, int cap, int64_t S, uint64_t* keys_out,
-                    const uint16_t* Xh, bool cvt, cudaStream_t st)
+                    const uint16_t* Xh, bool cvt, const HostRowsView* hr, cudaStream_t st)
 {
+    const bool host = hr != nullptr;             // fp32 rows in pinned host memory: both passes read the bf16 copy Xh
     const bool bf16 = Xh != nullptr || cvt;      // bf16 operands in the prune pass (shadow copy, or converted on chip)
     const int64_t n_tiles = (n_rows + TC_TILE_M - 1) / TC_TILE_M;
     const int64_t s_tiles = tc_sample_tiles(n_rows);
@@ -498,8 +679,17 @@ static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensor
     // the dump holds one value per (16-row group of a sampled tile, query): S_min per query
     const int64_t S_min = s_tiles * (TC_TILE_M / TC_DUMP_GROUP);
     (void)S;
-    tc_launch<NQ, TC_TF32, true>(di, tmX, tmQ, n_rows, dpad, s_tiles, TC_SAMPLE_STRIDE, xnorm, alive, nullptr, nullptr, nullptr, 0,
-                                 w.dump, S_min, 1, st);
+    if (host) {   // the sample pass only chooses thr: bf16 operands do not enter soundness
+        CUtensorMap tmQh, tmXh;
+        launch_f32_to_bf16(q, w.q_bf16, (int64_t)nq * dpad, st);
+        if (!make_map(&tmQh, (const void*)w.q_bf16, nq, dpad, NQ, true) || !make_map(&tmXh, Xh, n_rows, dpad, TC_TILE_M, true))
+            throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled(bf16 rows)", __FILE__, __LINE__};
+        tc_launch<NQ, TC_BF16, true>(di, tmXh, tmQh, n_rows, dpad, s_tiles, TC_SAMPLE_STRIDE, xnorm, alive, nullptr, nullptr, nullptr, 0,
+                                     w.dump, S_min, 1, st);
+    } else {
+        tc_launch<NQ, TC_TF32, true>(di, tmX, tmQ, n_rows, dpad, s_tiles, TC_SAMPLE_STRIDE, xnorm, alive, nullptr, nullptr, nullptr, 0,
+                                     w.dump, S_min, 1, st);
+    }
     KRAG_CUDA(cudaGetLastError());
     count_launch();
     // 2. threshold admitting ~C rows: the m-th smallest of the sample, m = C * sample_fraction
@@ -519,8 +709,9 @@ static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensor
     count_launch();
     KRAG_CUDA(cudaMemsetAsync(w.cand_count, 0, 256 * 4, st));
     // 3. main pass: stream the corpus once, prune on the tensor cores
-    if (bf16) launch_f32_to_bf16(q, w.q_bf16, (int64_t)nq * dpad, st);
-    dense_timer_begin(st, cvt ? 5 : (bf16 ? 4 : 3), n_rows * (int64_t)dpad * ((bf16 && !cvt) ? 2 : 4), 2 * (int64_t)NQ * n_rows * dpad);
+    if (bf16 && !host) launch_f32_to_bf16(q, w.q_bf16, (int64_t)nq * dpad, st);
+    dense_timer_begin(st, host ? 6 : (cvt ? 5 : (bf16 ? 4 : 3)), n_rows * (int64_t)dpad * ((bf16 && !cvt) ? 2 : 4),
+                      2 * (int64_t)NQ * n_rows * dpad);
     if (bf16) {
         CUtensorMap tmQh, tmXh;
         if (!make_map(&tmQh, (const void*)w.q_bf16, nq, dpad, NQ, true))
@@ -548,7 +739,31 @@ static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensor
         rs_attr_set = true;
     }
     dim3 rg((unsigned)((cap + 31) / 32), (unsigned)nq);
-    rescore_kernel<<<rg, 256, (size_t)dpad * 4, st>>>(X, dpad, q, w.cand_count, w.cand_rows, cap, ord_base, w.exact_keys);
+    if (host) {
+        // refine on the bf16 copy, U_(P) per query (merged into keys_out, overwritten below), compact the candidates that
+        // may be in the top P, rescore only those from the host rows
+        static bool rf_attr_set = false;
+        if (!rf_attr_set) {
+            KRAG_CUDA(cudaFuncSetAttribute(refine_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 4));
+            KRAG_CUDA(cudaFuncSetAttribute(rescore_mapped_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 4));
+            rf_attr_set = true;
+        }
+        refine_kernel<<<rg, 256, (size_t)dpad * 4, st>>>(Xh, hr->xres, dpad, q, w.cand_count, w.cand_rows, cap, w.lo, w.exact_keys);
+        KRAG_CUDA(cudaGetLastError());
+        count_launch();
+        launch_merge(w.exact_keys, 1, cap, nq, P, cap, cap, keys_out, st);
+        float scale, eta2;
+        fetch_rule_constants(dpad, &scale, &eta2);
+        KRAG_CUDA(cudaMemsetAsync(w.fetch_count, 0, 256 * 4, st));
+        fetch_compact_kernel<<<dim3((unsigned)((cap + 255) / 256), (unsigned)nq), 256, 0, st>>>(
+            w.cand_count, w.cand_rows, cap, w.lo, keys_out, P, scale, eta2, w.fetch_count, w.fetch_rows);
+        KRAG_CUDA(cudaGetLastError());
+        count_launch();
+        rescore_mapped_kernel<<<rg, 256, (size_t)dpad * 4, st>>>(hr->d, dpad, q, w.fetch_count, w.fetch_rows, cap, ord_base,
+                                                                 w.exact_keys);
+    } else {
+        rescore_kernel<<<rg, 256, (size_t)dpad * 4, st>>>(X, dpad, q, w.cand_count, w.cand_rows, cap, ord_base, w.exact_keys);
+    }
     KRAG_CUDA(cudaGetLastError());
     count_launch();
     launch_merge(w.exact_keys, 1, cap, nq, P, cap, cap, keys_out, st);
@@ -586,9 +801,9 @@ bool launch_dense_tc(const DeviceInfo& di, const float* X, int64_t n_rows, int d
         CUtensorMap tmQ;
         if (!make_map(&tmQ, qb, nq, dpad, NQ)) return false;
         uint64_t* ko = keys_out + (size_t)b0 * P;
-        if (NQ == 64) tc_pass<64>(di, tmX, tmQ, X, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, Xh, cvt, st);
-        else if (NQ == 128) tc_pass<128>(di, tmX, tmQ, X, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, Xh, cvt, st);
-        else tc_pass<256>(di, tmX, tmQ, X, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, Xh, cvt, st);
+        if (NQ == 64) tc_pass<64>(di, tmX, tmQ, X, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, Xh, cvt, nullptr, st);
+        else if (NQ == 128) tc_pass<128>(di, tmX, tmQ, X, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, Xh, cvt, nullptr, st);
+        else tc_pass<256>(di, tmX, tmQ, X, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, Xh, cvt, nullptr, st);
         // uncertified queries (rare) are re-run on the exact scan kernel -- still on the GPU
         KRAG_CUDA(cudaMemcpyAsync(flags.data(), w.flags, sizeof(int32_t) * (size_t)nq, cudaMemcpyDeviceToHost, st));
         KRAG_CUDA(cudaStreamSynchronize(st));
@@ -597,6 +812,52 @@ bool launch_dense_tc(const DeviceInfo& di, const float* X, int64_t n_rows, int d
             ++g_tc_fallback_queries;
             launch_dense_scan(di, X, n_rows, dpad, alive, qb + (size_t)j * dpad, 1, P, ord_base, part, ko + (size_t)j * P, st);
         }
+    }
+    return true;
+}
+
+// K2 over host-resident rows: sample and main pass on the device bf16 copy, refine + fetch + zero-copy rescoring from the
+// pinned fp32 rows, the same certificate; uncertified queries go through the streamed exact scan together
+bool launch_dense_tc_host(const DeviceInfo& di, const HostRowsView& hr, int64_t n_rows, int dpad, const uint32_t* alive,
+                          const float* xnorm, const uint32_t* xn_max_bits, const float* q, int batch, int P, OrdMap ord_base,
+                          void* workspace, size_t workspace_bytes, uint64_t* part, const ScanStaging& sg, uint64_t* keys_out,
+                          cudaStream_t st)
+{
+    if (!dense_tc_host_rows_supported(di, n_rows, dpad) || xnorm == nullptr) return false;
+    const int cap = tc_cap(P);
+    const int64_t S = tc_sample_tiles(n_rows) * TC_TILE_M;
+    TcWorkspace w;
+    if (tc_carve(&w, (unsigned char*)workspace, cap, S, true) > workspace_bytes) return false;
+    CUtensorMap unused{};   // the fp32 maps are not read in host mode
+    std::vector<int32_t> flags(256);
+    std::vector<uint32_t> fetched(256);
+    for (int b0 = 0; b0 < batch; b0 += 256) {
+        const int nq = batch - b0 < 256 ? batch - b0 : 256;
+        const int NQ = nq <= 64 ? 64 : (nq <= 128 ? 128 : 256);
+        const float* qb = q + (size_t)b0 * dpad;
+        uint64_t* ko = keys_out + (size_t)b0 * P;
+        if (NQ == 64) tc_pass<64>(di, unused, unused, nullptr, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, hr.bf16, false, &hr, st);
+        else if (NQ == 128) tc_pass<128>(di, unused, unused, nullptr, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, hr.bf16, false, &hr, st);
+        else tc_pass<256>(di, unused, unused, nullptr, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, hr.bf16, false, &hr, st);
+        KRAG_CUDA(cudaMemcpyAsync(flags.data(), w.flags, sizeof(int32_t) * (size_t)nq, cudaMemcpyDeviceToHost, st));
+        KRAG_CUDA(cudaMemcpyAsync(fetched.data(), w.fetch_count, sizeof(uint32_t) * (size_t)nq, cudaMemcpyDeviceToHost, st));
+        KRAG_CUDA(cudaStreamSynchronize(st));
+        int64_t rows = 0;
+        int nf = 0;
+        for (int j = 0; j < nq; ++j) {
+            rows += fetched[(size_t)j] < (uint32_t)cap ? fetched[(size_t)j] : (uint32_t)cap;
+            if (flags[(size_t)j]) continue;
+            KRAG_CUDA(cudaMemcpyAsync(sg.q_sel + (size_t)nf * dpad, qb + (size_t)j * dpad, sizeof(float) * (size_t)dpad,
+                                      cudaMemcpyDeviceToDevice, st));
+            flags[(size_t)nf++] = j;   // flags[0, nf) now lists the uncertified queries
+        }
+        g_host_rows_fetched += rows;
+        if (nf == 0) continue;
+        g_tc_fallback_queries += nf;
+        launch_dense_scan_streamed(di, hr.h, n_rows, dpad, alive, sg.q_sel, nf, P, ord_base, part, sg, sg.k_sel, st);
+        for (int i = 0; i < nf; ++i)
+            KRAG_CUDA(cudaMemcpyAsync(ko + (size_t)flags[(size_t)i] * P, sg.k_sel + (size_t)i * P, sizeof(uint64_t) * (size_t)P,
+                                      cudaMemcpyDeviceToDevice, st));
     }
     return true;
 }

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <string.h>
 
 #include <stdexcept>
 #include <utility>
@@ -84,6 +85,73 @@ private:
     }
 };
 
+// bytes of pinned host memory currently held through HostArray, process-wide (krag_host_pinned_bytes)
+void count_host_pinned_bytes(int64_t delta);
+int64_t host_pinned_bytes();
+
+// Owning pinned, device-mapped host buffer: the host counterpart of DevArray and the only code of the library that
+// allocates, registers or frees pinned host memory.  `h` is the host address; `d` the address kernels read it through
+// (zero-copy over the host link), taken from cudaHostGetDevicePointer, not assumed equal to `h`.  Move-only; the
+// destructor frees.  An allocation that does not fit throws DevOom.
+template <class T>
+struct HostArray {
+    T* h = nullptr;
+    T* d = nullptr;
+    int64_t cap = 0;
+
+    HostArray() = default;
+    HostArray(const HostArray&) = delete;
+    HostArray& operator=(const HostArray&) = delete;
+    HostArray(HostArray&& o) noexcept : h(o.h), d(o.d), cap(o.cap) { o.h = o.d = nullptr; o.cap = 0; }
+    HostArray& operator=(HostArray&& o) noexcept
+    {
+        if (this != &o) { release(); std::swap(h, o.h); std::swap(d, o.d); std::swap(cap, o.cap); }
+        return *this;
+    }
+    ~HostArray() { release(); }
+
+    void alloc(int64_t n)
+    {
+        release();
+        void* q = nullptr;
+        const size_t bytes = sizeof(T) * (size_t)n;
+        const cudaError_t e = cudaHostAlloc(&q, bytes, cudaHostAllocMapped | cudaHostAllocPortable);
+        if (e == cudaErrorMemoryAllocation) {
+            cudaGetLastError();
+            char msg[160];
+            snprintf(msg, sizeof msg, "out of pinned host memory (wanted %.2f GB, %.2f GB already pinned by this process)", bytes / 1e9,
+                     host_pinned_bytes() / 1e9);
+            throw DevOom{msg};
+        }
+        KRAG_CUDA(e);
+        h = static_cast<T*>(q);
+        cap = n;
+        count_host_pinned_bytes((int64_t)bytes);
+        void* dp = nullptr;
+        KRAG_CUDA(cudaHostGetDevicePointer(&dp, q, 0));
+        d = static_cast<T*>(dp);
+    }
+    // grow to at least n elements keeping the first `used` (copy-on-grow on the host)
+    void reserve(int64_t n, int64_t used)
+    {
+        if (n <= cap) return;
+        HostArray grown;
+        grown.alloc(cap + cap / 2 > n ? cap + cap / 2 : n);
+        if (h && used > 0) memcpy(grown.h, h, sizeof(T) * (size_t)used);
+        *this = std::move(grown);
+    }
+    void release()
+    {
+        if (h) {
+            cudaFreeHost(h);
+            count_host_pinned_bytes(-bytes());
+        }
+        h = d = nullptr;
+        cap = 0;
+    }
+    int64_t bytes() const { return (int64_t)sizeof(T) * cap; }
+};
+
 // global ordinal of a local row: base + row * stride.  Contiguous shards (bench, one GPU) use stride 1; the multi-GPU
 // service deals nodes round-robin (node o -> shard o % G, row o / G), so base = shard, stride = G and ordinals -- hence
 // every tie-break -- are exactly the single-GPU insertion order.
@@ -117,10 +185,41 @@ void launch_dense_scan(const DeviceInfo& di, const float* X, int64_t n_rows, int
                        const float* q, int batch, int P, OrdMap ord_base, uint64_t* part, uint64_t* keys_out,
                        cudaStream_t st);
 
+// ---- host-resident rows (KRAG_ROWS_HOST): fp32 rows in pinned host memory, bf16 copy + residual norms on the device
+struct HostRowsView {
+    const float* h;          // host address of the fp32 rows [n_rows, dpad] (DMA source)
+    const float* d;          // the same memory through its mapped device address (zero-copy reads)
+    const uint16_t* bf16;    // device bf16 copy [n_rows, dpad]
+    const float* xres;       // device |x - bf16(x)| per row, rounded up
+};
+// device staging of the streamed exact scan, owned by the search slot
+struct ScanStaging {
+    float* buf[2];           // two chunks of chunk_rows rows (double buffering)
+    int64_t chunk_rows;      // multiple of 32
+    cudaStream_t copy;       // DMA stream
+    cudaEvent_t copied[2], freed[2];
+    uint64_t* fold;          // [2, batch, P]: running top P and the current chunk's
+    float* q_sel;            // [256, dpad] uncertified queries of a K2 chunk
+    uint64_t* k_sel;         // [256, P]
+};
+int64_t stream_scan_chunk_rows(int dpad);
+// K1, unchanged, over chunks of host rows copied in by DMA; each chunk's top P folded into the running list.  Exact.
+void launch_dense_scan_streamed(const DeviceInfo& di, const float* X_host, int64_t n_rows, int dpad, const uint32_t* alive,
+                                const float* q, int batch, int P, OrdMap ord_base, uint64_t* part, const ScanStaging& sg,
+                                uint64_t* keys_out, cudaStream_t st);
+void launch_bf16_residual(const float* X, int64_t n, int dpad, uint16_t* Xh, float* xres, cudaStream_t st);
+bool dense_tc_host_rows_supported(const DeviceInfo& di, int64_t n_rows, int dpad);
+// returns false when K2 cannot serve the index (the caller runs the streamed scan)
+bool launch_dense_tc_host(const DeviceInfo& di, const HostRowsView& hr, int64_t n_rows, int dpad, const uint32_t* alive,
+                          const float* xnorm, const uint32_t* xn_max_bits, const float* q, int batch, int P, OrdMap ord_base,
+                          void* workspace, size_t workspace_bytes, uint64_t* part, const ScanStaging& sg, uint64_t* keys_out,
+                          cudaStream_t st);
+int64_t host_rows_fetched();   // rows rescored from host memory, process-wide
+
 // ---- K2: wgmma candidate generation + exact fp32 rescoring (dense_tc.cu)
 bool dense_tc_supported(const DeviceInfo& di, int dpad);
 bool dense_tc_wants(int64_t n_rows, int batch);   // size heuristics: is K2 the better kernel for this call?
-size_t dense_tc_workspace_bytes(const DeviceInfo& di, int64_t n_rows, int P);
+size_t dense_tc_workspace_bytes(const DeviceInfo& di, int64_t n_rows, int P, bool host_rows = false);
 // |x|^2 per row (+ running max) maintained at index time for K2's epilogue and certificate
 void launch_row_norms(const float* X, int64_t row0, int64_t n, int dpad, float* xnorm, uint32_t* xn_max_bits,
                       cudaStream_t st);

@@ -425,7 +425,8 @@ def main():
     if source not in ("local", "remote"):
         raise SystemExit("Invalid Embedding Type Specified (Must be Local or Remote)")          # main.py:133-141
     n_gpus = int(os.getenv("KRAG_NUM_GPUS", "0")) or _gpu_count()
-    ctx = _native.Context(device_id=cfg["device_id"], rank=0, world_size=max(1, n_gpus))
+    ctx = _native.Context(device_id=cfg["device_id"], rank=0, world_size=max(1, n_gpus),
+                          row_storage=_native.row_storage_from_env())
     engine, workers = ctx, []
     if n_gpus > 1:
         # one replica per RAGEngine (manifests.go:81): every GPU of the pod belongs to this service.  Rank 0 (this process)

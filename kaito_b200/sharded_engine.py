@@ -296,7 +296,7 @@ def worker_main():
     rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
     local_rank = int(os.environ.get("LOCAL_RANK", rank))
     ctl = init_distributed(rank, world, local_rank, int(os.environ["MASTER_PORT"]))
-    ctx = _native.Context(device_id=local_rank, rank=rank, world_size=world)
+    ctx = _native.Context(device_id=local_rank, rank=rank, world_size=world, row_storage=_native.row_storage_from_env())
     eng = ShardedEngine(native_stages_factory(ctx), torch.device("cuda", local_rank), None, ctl)
     try:
         eng.serve()
