@@ -131,6 +131,15 @@ int32_t krag_index_add(krag_index* idx, int64_t n, const uint64_t* node_ids, con
                        const uint32_t* doc_len);
 /* replaces: IndexIDMap.remove_ids via llama-index delete (vector_store/base.py:563-643) */
 int32_t krag_index_remove(krag_index* idx, int64_t n, const uint64_t* node_ids, int64_t* n_removed);
+/* Remove tombstoned rows from the index: live rows keep their relative order and move down to rows [0, n_live).
+ * Node ids, vectors, term lists, BM25 scores and every search result (ids, scores, tie order) are unchanged; only the
+ * ordinals of rows behind a removed row change.  Takes the index's writer lock.  *n_reclaimed_out = rows removed.
+ * The rows move in place on the device (a bounded staging buffer, no second copy of the index); a committed index gets
+ * its postings rebuilt with the statistics of its last commit, an uncommitted one stays uncommitted.  Buffers that shrank
+ * are reallocated at their exact size when that fits beside the old ones.  No dead rows: a no-op, 0 reclaimed.
+ * KRAG_E_UNSUPPORTED for an ordinal stride > 1 (round-robin shards, krag_index_set_ordinal_map): the index is unchanged.
+ * No counterpart in the reference, whose FAISS IndexIDMap.remove_ids compacts on every delete. */
+int32_t krag_index_compact(krag_index* idx, int64_t* n_reclaimed_out);
 /*
  * (Re)build BM25 postings for the rows added so far.  replaces the per-query
  * BM25Retriever.from_defaults rebuild (hybrid_retriever.py:104-130): same scores,
@@ -300,6 +309,10 @@ int64_t krag_host_rows_fetched(void);
  * 6 = device bf16 rows of a KRAG_ROWS_HOST index), with the algorithmic bytes and
  * flops of that launch -- bench.py's roofline line is computed from it. */
 int32_t krag_last_dense_kernel(float* ms, int32_t* kernel_id, int64_t* algorithmic_bytes, int64_t* flops);
+/* Figures of the last krag_index_compact on this process: CUDA-event duration of the row-move phase (device moves and
+ * the host-row memmoves they overlap), host-clock duration of the postings rebuild (0 if the index was not committed),
+ * live rows that changed position, and the bytes of the moved rows and term lists (each counted once). */
+int32_t krag_last_compact(float* move_ms, float* postings_ms, int64_t* rows_moved, int64_t* bytes_moved);
 /* raw K2 output a[j][r] = |x_r|^2 - 2 x_r.q_j (TF32) for every row, [nq_pad][S] row-major;
  * call with out == NULL to query S and nq_pad.  Test hook for the tensor-core kernel; KRAG_E_UNSUPPORTED for
  * KRAG_ROWS_HOST indexes. */

@@ -36,7 +36,7 @@ SYMBOLS = [
     "krag_embedder_finalize", "krag_embed", "krag_embed_dev", "krag_embedder_destroy", "krag_debug_gemm_tf32",
     "krag_debug_linear_ln", "krag_index_set_dense_mode", "krag_text_analyze", "krag_wordpiece_create",
     "krag_wordpiece_encode_batch", "krag_wordpiece_destroy", "krag_p2p_create", "krag_p2p_connect", "krag_dev_exchange_merge", "krag_p2p_destroy",
-    "krag_host_pinned_bytes", "krag_host_rows_fetched",
+    "krag_host_pinned_bytes", "krag_host_rows_fetched", "krag_index_compact", "krag_last_compact",
 ]
 
 
@@ -92,6 +92,7 @@ def load() -> C.CDLL:
     L.krag_index_reserve.argtypes = [vp, i64, i64]
     L.krag_index_add.argtypes = [vp, i64, vp, vp, vp, vp, vp, vp]
     L.krag_index_remove.argtypes = [vp, i64, vp, C.POINTER(i64)]
+    L.krag_index_compact.argtypes = [vp, C.POINTER(i64)]
     L.krag_index_commit.argtypes = [vp, i64]
     L.krag_index_commit_local.argtypes = [vp, i64, vp, C.POINTER(i64), C.POINTER(i64)]
     L.krag_index_commit_global.argtypes = [vp, i64, vp, i64, i64, i64]
@@ -129,6 +130,7 @@ def load() -> C.CDLL:
     L.krag_p2p_destroy.argtypes = [vp]
     L.krag_tc_fallback_queries.restype = i64
     L.krag_last_dense_kernel.argtypes = [C.POINTER(C.c_float), C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]
+    L.krag_last_compact.argtypes = [C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(i64), C.POINTER(i64)]
     L.krag_debug_tc_dump.argtypes = [vp, i32, vp, vp, i64, C.POINTER(i64), C.POINTER(i32)]
     for name in SYMBOLS:
         fn = getattr(L, name)
@@ -157,6 +159,14 @@ def last_dense_kernel():
     ms, kid, by, fl = C.c_float(0), C.c_int32(0), C.c_int64(0), C.c_int64(0)
     check(load().krag_last_dense_kernel(C.byref(ms), C.byref(kid), C.byref(by), C.byref(fl)))
     return ms.value, kid.value, by.value, fl.value
+
+
+def last_compact() -> dict:
+    """figures of the last Index.compact() of this process: move_ms (CUDA events around the row moves), postings_ms,
+    rows_moved, bytes_moved (moved rows and term lists, each byte counted once)"""
+    mv, po, rows, by = C.c_float(0), C.c_float(0), C.c_int64(0), C.c_int64(0)
+    check(load().krag_last_compact(C.byref(mv), C.byref(po), C.byref(rows), C.byref(by)))
+    return {"move_ms": mv.value, "postings_ms": po.value, "rows_moved": rows.value, "bytes_moved": by.value}
 
 
 def device_bytes() -> int:
@@ -358,6 +368,13 @@ class Index:
         node_ids = np.ascontiguousarray(node_ids, np.uint64)
         n = C.c_int64(0)
         check(self._L.krag_index_remove(self._h, len(node_ids), ptr(node_ids), C.byref(n)))
+        return n.value
+
+    def compact(self) -> int:
+        """remove the tombstoned rows in place; live rows keep their order (ordinals behind a removed row move down).
+        Returns the number of rows reclaimed."""
+        n = C.c_int64(0)
+        check(self._L.krag_index_compact(self._h, C.byref(n)))
         return n.value
 
     def commit(self, vocab: int):

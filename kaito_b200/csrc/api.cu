@@ -6,6 +6,7 @@
 #include <sys/stat.h>
 
 #include <atomic>
+#include <chrono>
 #include <condition_variable>
 #include <memory>
 #include <mutex>
@@ -170,6 +171,8 @@ struct krag_index {
     bool committed = false;
     int64_t committed_rows = 0;
     int64_t vocab = 0, n_docs_global = 0, total_len_global = 0;
+    std::vector<float> idf;         // [vocab] and avgdl of the last commit: compaction rebuilds the postings with them
+    double avgdl = 1.0;
     int64_t ord_base = 0, ord_stride = 1;   // global ordinal of local row r = ord_base + r * ord_stride
 };
 
@@ -419,12 +422,122 @@ void commit_global_impl(krag_index* ix, int64_t vocab, const uint32_t* df_global
     KRAG_CUDA(cudaStreamSynchronize(st));
     d_idf.release();
     ix->entry_doc.release();
+    ix->idf = std::move(idf);
+    ix->avgdl = avgdl;
     ix->vocab = vocab;
     ix->n_docs_global = n_docs_global;
     ix->total_len_global = total_len_global;
     ix->ord_base = ord_base;
     ix->committed = true;
     ix->committed_rows = ix->n_rows;
+}
+
+// figures of the last compaction (krag_last_compact): process-wide, last writer wins
+struct CompactReport { float move_ms = 0.f, postings_ms = 0.f; int64_t rows_moved = 0, bytes_moved = 0; bool valid = false; };
+std::mutex g_compact_mu;
+CompactReport g_compact;
+
+// krag_index_compact on an index with dead rows and ordinal stride 1 (writer lock held)
+void compact_impl(krag_index* ix)
+{
+    cudaStream_t st = ix->ctx->admin;
+    const int64_t dp = ix->dpad;
+    CompactPlan plan;
+    compact_plan(ix->alive_d.p, ix->n_rows, ix->has_sparse ? ix->toff.p : nullptr, plan, st);
+    const int64_t n = plan.n_live;
+    const int64_t nnz = ix->has_sparse ? plan.h_toff_new[(size_t)n] : 0;
+
+    cudaEvent_t e0, e1;
+    KRAG_CUDA(cudaEventCreate(&e0));
+    KRAG_CUDA(cudaEventCreate(&e1));
+    CompactReport rep;
+    KRAG_CUDA(cudaEventRecord(e0, st));
+    // device arrays first (asynchronous); the pinned host rows move on the CPU meanwhile
+    if (!ix->host_rows) rep.bytes_moved += compact_rows(ix->X.p, dp * (int64_t)sizeof(float), plan, st);
+    if (ix->Xh.p) rep.bytes_moved += compact_rows(ix->Xh.p, dp * (int64_t)sizeof(uint16_t), plan, st);
+    if (ix->xres.p) rep.bytes_moved += compact_rows(ix->xres.p, sizeof(float), plan, st);
+    rep.bytes_moved += compact_rows(ix->xnorm.p, sizeof(float), plan, st);
+    if (ix->has_sparse) {
+        rep.bytes_moved += compact_rows(ix->dlen.p, sizeof(uint32_t), plan, st);
+        rep.bytes_moved += compact_terms(ix->tid.p, ix->ttf.p, ix->toff.p, plan, st);
+        KRAG_CUDA(cudaMemcpyAsync(ix->toff.p, plan.toff_new.p, sizeof(int64_t) * (size_t)(n + 1), cudaMemcpyDeviceToDevice, st));
+    }
+    launch_max_bits(ix->xnorm.p, n, ix->xn_max.p, st);
+    if (ix->host_rows) {
+        // runs of consecutive live rows, ascending: a destination never lies above its source, so memmove is safe
+        for (int64_t d = plan.first; d < n;) {
+            int64_t e = d + 1;
+            while (e < n && plan.h_src[(size_t)e] == plan.h_src[(size_t)e - 1] + 1) ++e;
+            memmove(ix->Xp.h + d * dp, ix->Xp.h + (int64_t)plan.h_src[(size_t)d] * dp, sizeof(float) * (size_t)((e - d) * dp));
+            d = e;
+        }
+    }
+    KRAG_CUDA(cudaEventRecord(e1, st));
+    KRAG_CUDA(cudaEventSynchronize(e1));
+    KRAG_CUDA(cudaEventElapsedTime(&rep.move_ms, e0, e1));
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+    rep.rows_moved = n - plan.first;
+
+    // host-side state
+    std::vector<uint64_t> ids((size_t)n);
+    ix->id2row.clear();
+    ix->id2row.reserve((size_t)n);
+    for (int64_t d = 0; d < n; ++d) {
+        ids[(size_t)d] = ix->node_ids[plan.h_src[(size_t)d]];
+        ix->id2row[ids[(size_t)d]] = d;
+    }
+    ix->node_ids = std::move(ids);
+    const int64_t words = (n + 31) / 32;
+    ix->alive_h.assign((size_t)words, 0xFFFFFFFFu);
+    if (n & 31) ix->alive_h.back() = (1u << (n & 31)) - 1u;
+    if (words > 0)
+        KRAG_CUDA(cudaMemcpyAsync(ix->alive_d.p, ix->alive_h.data(), sizeof(uint32_t) * (size_t)words, cudaMemcpyHostToDevice, st));
+    KRAG_CUDA(cudaStreamSynchronize(st));
+    plan = CompactPlan{};
+    ix->n_rows = n;
+    ix->n_live = n;
+    ix->has_dead = false;
+    ix->nnz = nnz;
+    ix->entry_doc.release();
+    ix->post = Postings{};
+
+    // exact-size buffers where they fit (never empty: a null Xh means "no bf16 shadow")
+    const int64_t rows1 = n > 0 ? n : 1;
+    if (ix->host_rows) ix->Xp.shrink(rows1 * dp);
+    else ix->X.shrink(rows1 * dp, st);
+    ix->Xh.shrink(rows1 * dp, st);
+    ix->xres.shrink(rows1, st);
+    ix->xnorm.shrink(rows1, st);
+    ix->alive_d.shrink(words > 0 ? words : 1, st);
+    if (ix->has_sparse) {
+        ix->toff.shrink(n + 1, st);
+        ix->dlen.shrink(rows1, st);
+        ix->tid.shrink(nnz > 0 ? nnz : 1, st);
+        ix->ttf.shrink(nnz > 0 ? nnz : 1, st);
+    }
+
+    // postings of a committed index: rebuilt over the compacted term lists with the statistics of the last commit, so every
+    // score is the one the index returned before (including after a commit_global with multi-shard statistics)
+    const bool rebuild = ix->committed;
+    ix->committed = false;            // until the rebuild below has succeeded
+    if (rebuild) {
+        const auto t0 = std::chrono::steady_clock::now();
+        DevArray<float> d_idf;
+        d_idf.alloc(ix->vocab);
+        KRAG_CUDA(cudaMemcpyAsync(d_idf.p, ix->idf.data(), sizeof(float) * (size_t)ix->vocab, cudaMemcpyHostToDevice, st));
+        ix->entry_doc.alloc(nnz > 0 ? nnz : 1);
+        if (n > 0) launch_expand_entry_doc(ix->toff.p, n, ix->entry_doc.p, st);
+        build_postings(ix->tid.p, ix->ttf.p, ix->entry_doc.p, ix->dlen.p, nullptr, nnz, ix->vocab, d_idf.p, ix->avgdl, n, ix->post, st);
+        KRAG_CUDA(cudaStreamSynchronize(st));
+        ix->entry_doc.release();
+        ix->committed = true;
+        ix->committed_rows = n;
+        rep.postings_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    }
+    rep.valid = true;
+    std::lock_guard<std::mutex> lk(g_compact_mu);
+    g_compact = rep;
 }
 
 }  // namespace
@@ -625,6 +738,33 @@ int32_t krag_index_remove(krag_index* ix, int64_t n, const uint64_t* node_ids, i
         KRAG_CUDA(cudaStreamSynchronize(ix->ctx->admin));
         if (removed) { ix->has_dead = true; ix->n_live -= removed; }
         if (n_removed) *n_removed = removed;
+    });
+}
+
+int32_t krag_index_compact(krag_index* ix, int64_t* n_reclaimed_out)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(ix, KRAG_E_INVALID, "null index");
+        std::unique_lock<std::shared_mutex> lk(ix->mu);
+        KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
+        KRAG_REQUIRE(ix->ord_stride == 1, KRAG_E_UNSUPPORTED,
+                     "compaction needs ordinal stride 1: rows of a round-robin shard cannot move down without leaving it");
+        if (n_reclaimed_out) *n_reclaimed_out = 0;
+        if (!ix->has_dead || ix->n_live == ix->n_rows) return;
+        const int64_t before = ix->n_rows;
+        compact_impl(ix);
+        if (n_reclaimed_out) *n_reclaimed_out = before - ix->n_rows;
+    });
+}
+
+int32_t krag_last_compact(float* move_ms, float* postings_ms, int64_t* rows_moved, int64_t* bytes_moved)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(move_ms && postings_ms && rows_moved && bytes_moved, KRAG_E_INVALID, "null argument");
+        std::lock_guard<std::mutex> lk(g_compact_mu);
+        KRAG_REQUIRE(g_compact.valid, KRAG_E_STATE, "no compaction has run yet");
+        *move_ms = g_compact.move_ms; *postings_ms = g_compact.postings_ms;
+        *rows_moved = g_compact.rows_moved; *bytes_moved = g_compact.bytes_moved;
     });
 }
 

@@ -7,6 +7,7 @@
 
 #include <stdexcept>
 #include <utility>
+#include <vector>
 
 #include "common.cuh"
 namespace krag {
@@ -52,6 +53,22 @@ struct DevArray {
         if (p && used > 0) KRAG_CUDA(cudaMemcpyAsync(grown.p, p, sizeof(T) * (size_t)used, cudaMemcpyDeviceToDevice, st));
         KRAG_CUDA(cudaStreamSynchronize(st));
         *this = std::move(grown);
+    }
+    // an exact-size buffer holding the first n elements, when one fits beside the current buffer; otherwise the capacity stays
+    // (later growth reuses it).  Returns whether the buffer shrank.
+    bool shrink(int64_t n, cudaStream_t st)
+    {
+        if (!p || n >= cap) return false;
+        DevArray s;
+        try {
+            s.alloc(n);
+        } catch (const DevOom&) {
+            return false;
+        }
+        KRAG_CUDA(cudaMemcpyAsync(s.p, p, sizeof(T) * (size_t)n, cudaMemcpyDeviceToDevice, st));
+        KRAG_CUDA(cudaStreamSynchronize(st));
+        *this = std::move(s);
+        return true;
     }
     void release()
     {
@@ -139,6 +156,20 @@ struct HostArray {
         grown.alloc(cap + cap / 2 > n ? cap + cap / 2 : n);
         if (h && used > 0) memcpy(grown.h, h, sizeof(T) * (size_t)used);
         *this = std::move(grown);
+    }
+    // the host counterpart of DevArray::shrink
+    bool shrink(int64_t n)
+    {
+        if (!h || n >= cap) return false;
+        HostArray s;
+        try {
+            s.alloc(n);
+        } catch (const DevOom&) {
+            return false;
+        }
+        memcpy(s.h, h, sizeof(T) * (size_t)n);
+        *this = std::move(s);
+        return true;
     }
     void release()
     {
@@ -285,6 +316,28 @@ size_t bm25_resolve_bytes(int64_t n_rows, int n_terms_total);   // size of launc
 void launch_bm25(const DeviceInfo& di, const Postings& post, int64_t n_rows, const uint32_t* alive,
                  const uint32_t* q_terms, const int32_t* q_term_offsets, int n_terms_total, void* resolve_ws, int batch, int P,
                  OrdMap ord_base, uint64_t* part, uint64_t* keys_out, cudaStream_t st);
+
+// ---- compaction (compact.cu): tombstoned rows removed in place, live rows keep their order
+constexpr int64_t COMPACT_STAGE_BYTES = (int64_t)32 << 20;   // staging of windows whose source and destination overlap
+constexpr int64_t COMPACT_TERM_BYTES = sizeof(uint32_t) + sizeof(uint16_t);   // one CSR entry: term id + tf
+struct CompactPlan {
+    int64_t n_rows = 0, n_live = 0;
+    int64_t first = 0;                  // first destination row that moves (= the first dead row); rows before it stay
+    DevArray<uint32_t> src;             // [n_live] source row of destination row d (ascending)
+    std::vector<uint32_t> h_src;
+    DevArray<int64_t> toff_new;         // [n_live + 1] term-list offsets after compaction (hybrid indexes)
+    std::vector<int64_t> h_toff_old, h_toff_new;
+    DevArray<unsigned char> stage;      // COMPACT_STAGE_BYTES, or the longest moved term list if that is larger
+};
+// ranks of the live rows (popcount prefix over the alive words) and, with toff, the new term-list offsets.  Allocates every
+// temporary of the compaction, so an allocation failure happens before any row has moved.
+void compact_plan(const uint32_t* alive, int64_t n_rows, const int64_t* toff, CompactPlan& plan, cudaStream_t st);
+// rows of row_bytes (a multiple of 4) at base: row d <- row src[d], in place; returns the bytes of the rows that moved
+int64_t compact_rows(void* base, int64_t row_bytes, const CompactPlan& plan, cudaStream_t st);
+// CSR term lists (tid / ttf) in place under toff_old -> plan.toff_new; returns the bytes of the entries that moved
+int64_t compact_terms(uint32_t* tid, uint16_t* ttf, const int64_t* toff_old, const CompactPlan& plan, cudaStream_t st);
+// *max_bits = bits of max x[i] over [0, n), x >= 0 (the K2 certificate's max |x|^2, as row_norms_kernel keeps it)
+void launch_max_bits(const float* x, int64_t n, uint32_t* max_bits, cudaStream_t st);
 
 // ---- K5: BERT encoder forward (embed.cu)
 struct BertConfig;

@@ -24,6 +24,11 @@ from . import text as _text
 
 FILTER_PUSHDOWN = 0x100   # kaito_rag.h KRAG_FILTER_PUSHDOWN
 RAG_MAX_TOP_K = int(os.getenv("RAG_MAX_TOP_K", 300))  # config.py:127
+# A delete or update compacts the index (Index.compact: dead rows leave the engine, their text leaves the docstore and the
+# snapshots) once the dead rows are at least this share of the rows and at least this many: below that, tombstones cost less
+# than moving every live row behind the first dead one.
+COMPACT_DEAD_FRACTION = 0.25
+COMPACT_MIN_DEAD_ROWS = 65536
 
 
 class HTTPException(Exception):
@@ -116,11 +121,12 @@ class RWLock:
 
 
 class _Node:
-    __slots__ = ("node_id", "ref_doc_id", "text", "metadata", "ordinal", "alive")
+    __slots__ = ("node_id", "ref_doc_id", "text", "metadata", "ordinal", "alive", "key")
 
-    def __init__(self, node_id, ref_doc_id, text, metadata, ordinal):
+    def __init__(self, node_id, ref_doc_id, text, metadata, ordinal, key=None):
         self.node_id, self.ref_doc_id, self.text, self.metadata, self.ordinal, self.alive = \
             node_id, ref_doc_id, text, metadata, ordinal, True
+        self.key = ordinal if key is None else key   # the engine's node id; stays when a compaction changes the ordinal
 
 
 class _IndexState:
@@ -130,6 +136,8 @@ class _IndexState:
         self.nodes: list[_Node] = []             # by ordinal (== insertion order == engine row)
         self.ref_docs: dict[str, dict] = {}      # doc_id -> {"text", "metadata", "nodes": [ordinal]}
         self.committed = False
+        self.next_key = 0                        # engine node id of the next node: len(nodes) until the first compaction
+        self.n_dead = 0                          # tombstoned nodes still in `nodes` (and rows in the engine)
         self._filter_cache: dict[str, tuple[int, np.ndarray]] = {}   # filter json -> (nodes covered, allow bitmap)
         self._frag_cache: dict[int, tuple[bytes, bytes]] = {}        # ordinal -> serialised halves of its NodeWithScore
 
@@ -288,13 +296,14 @@ class VectorStore:
             ords = []
             for i, chunk in enumerate(self.split_document(text, metadata)):
                 ordinal = base + len(new_nodes)
-                new_nodes.append(_Node(f"{doc_id}-{i}", doc_id, chunk, metadata, ordinal))
+                key = st.next_key + len(new_nodes)
+                new_nodes.append(_Node(f"{doc_id}-{i}", doc_id, chunk, metadata, ordinal, key))
                 et = embed_text(chunk, metadata)
                 texts.append(et)
                 t_ids, t_tf, dl = st.vocab.doc_terms(et)     # may grow the vocabulary: unused ids are harmless
                 tids.append(t_ids); tfs.append(t_tf); dls.append(dl)
                 offs.append(offs[-1] + len(t_ids))
-                node_ids.append(ordinal)
+                node_ids.append(key)
                 ords.append(ordinal)
             new_refs[doc_id] = {"text": text, "metadata": metadata, "nodes": ords}
         vecs = np.asarray(self.embed_model.get_text_embedding_batch(texts), np.float32)
@@ -304,6 +313,7 @@ class VectorStore:
         # the rows are in the engine: publish.  (A failing commit below leaves the index "uncommitted": /retrieve takes
         # the reference's vector-only fallback until the next successful commit.)
         st.nodes.extend(new_nodes)
+        st.next_key += len(new_nodes)
         old = {d: st.ref_docs.get(d) for d in new_refs} if replace else {}
         st.ref_docs.update(new_refs)
         st.committed = False
@@ -329,6 +339,25 @@ class VectorStore:
         # the reference rebuilds BM25 on every query (hybrid_retriever.py:104-130); here once per mutation
         st.index.commit(max(1, len(st.vocab)))
         st.committed = True
+
+    def _maybe_compact(self, st: _IndexState):
+        """after a committed delete / update (writer lock held): compact the engine index when enough of it is dead, then
+        drop the dead nodes from the host mirror and renumber the live ones as the engine did (order kept)"""
+        if (st.n_dead < COMPACT_MIN_DEAD_ROWS or st.n_dead < COMPACT_DEAD_FRACTION * len(st.nodes)
+                or not hasattr(st.index, "compact")):      # the sharded engine keeps its tombstones
+            return
+        st.index.compact()
+        live = [n for n in st.nodes if n.alive]
+        remap = {}
+        for i, n in enumerate(live):
+            remap[n.ordinal] = i
+            n.ordinal = i
+        st.nodes = live
+        for rec in st.ref_docs.values():
+            rec["nodes"] = [remap[o] for o in rec["nodes"]]
+        st.n_dead = 0
+        st._frag_cache.clear()           # both caches are keyed by ordinal
+        st._filter_cache.clear()
 
     # --------------------------------------------------------------- /retrieve
     def retrieve(self, index_name: str, query: str, max_node_count: int = 5, metadata_filter: dict | None = None):
@@ -500,10 +529,12 @@ class VectorStore:
                 deleted.append(d)
                 for o in rec["nodes"]:
                     st.nodes[o].alive = False
-                    rows.append(o)
+                    rows.append(st.nodes[o].key)
             if rows:
                 st.index.remove(np.asarray(rows, np.uint64))
+                st.n_dead += len(rows)
                 self._commit(st)
+                self._maybe_compact(st)
             return {"deleted_doc_ids": deleted, "not_found_doc_ids": missing}
 
     def update_documents(self, index_name: str, documents: list[dict]):
@@ -526,9 +557,12 @@ class VectorStore:
                     self._insert(st, [(doc["doc_id"], doc["text"], doc.get("metadata") or {})], replace=True)
                     for o in old_rows:
                         st.nodes[o].alive = False
-                    st.index.remove(np.asarray(old_rows, np.uint64))
+                    st.index.remove(np.asarray([st.nodes[o].key for o in old_rows], np.uint64))
+                    st.n_dead += len(old_rows)
                     self._commit(st)
                     updated.append(doc)
+            if updated:
+                self._maybe_compact(st)
             return {"updated_documents": updated, "unchanged_documents": unchanged, "not_found_documents": missing}
 
     def delete_index(self, index_name: str):
@@ -546,9 +580,12 @@ class VectorStore:
             st = self.index_map[index_name]
             os.makedirs(path, exist_ok=True)
             st.index.persist(path)
+            ds = {"version": 1, "vocab": st.vocab.terms, "ref_docs": st.ref_docs,
+                  "nodes": [[n.node_id, n.ref_doc_id, n.text, n.metadata, n.alive] for n in st.nodes]}
+            if any(n.key != n.ordinal for n in st.nodes):    # engine node ids; absent: key = ordinal (every earlier snapshot)
+                ds["keys"] = [n.key for n in st.nodes]
             with open(os.path.join(path, "docstore.json"), "w") as f:
-                json.dump({"version": 1, "vocab": st.vocab.terms, "ref_docs": st.ref_docs,
-                           "nodes": [[n.node_id, n.ref_doc_id, n.text, n.metadata, n.alive] for n in st.nodes]}, f)
+                json.dump(ds, f)
 
     def load(self, index_name: str, path: str, overwrite: bool = False):
         """base.py:811-868."""
@@ -567,10 +604,13 @@ class VectorStore:
                     for t in ds["vocab"]:
                         fresh.vocab.add(t)
                     fresh.ref_docs = ds["ref_docs"]
+                    keys = ds.get("keys")
                     for i, (nid, rid, text, meta, alive) in enumerate(ds["nodes"]):
-                        n = _Node(nid, rid, text, meta, i)
+                        n = _Node(nid, rid, text, meta, i, keys[i] if keys else i)
                         n.alive = alive
                         fresh.nodes.append(n)
+                    fresh.next_key = max(keys) + 1 if keys else len(fresh.nodes)
+                    fresh.n_dead = sum(1 for n in fresh.nodes if not n.alive)
                     fresh.committed = True
                 except Exception:
                     fresh.index.drop()
