@@ -134,8 +134,8 @@ int32_t krag_index_remove(krag_index* idx, int64_t n, const uint64_t* node_ids, 
 /* Remove tombstoned rows from the index: live rows keep their relative order and move down to rows [0, n_live).
  * Node ids, vectors, term lists, BM25 scores and every search result (ids, scores, tie order) are unchanged; only the
  * ordinals of rows behind a removed row change.  Takes the index's writer lock.  *n_reclaimed_out = rows removed.
- * The rows move in place on the device (a bounded staging buffer, no second copy of the index); a committed index gets
- * its postings rebuilt with the statistics of its last commit, an uncommitted one stays uncommitted.  Buffers that shrank
+ * The rows move in place on the device (a bounded staging buffer, no second copy of the index); the committed postings
+ * are renumbered with the scores of the last commit (an uncommitted index stays uncommitted and keeps them for its next commit).  Buffers that shrank
  * are reallocated at their exact size when that fits beside the old ones.  No dead rows: a no-op, 0 reclaimed.
  * KRAG_E_UNSUPPORTED for an ordinal stride > 1 (round-robin shards, krag_index_set_ordinal_map): the index is unchanged.
  * No counterpart in the reference, whose FAISS IndexIDMap.remove_ids compacts on every delete. */
@@ -143,7 +143,8 @@ int32_t krag_index_compact(krag_index* idx, int64_t* n_reclaimed_out);
 /*
  * (Re)build BM25 postings for the rows added so far.  replaces the per-query
  * BM25Retriever.from_defaults rebuild (hybrid_retriever.py:104-130): same scores,
- * built once.  Single-shard form:
+ * built once.  After the first commit, a commit merges the added and removed rows into the
+ * committed postings on the device (bit-identical to a full build; krag_last_commit).  Single-shard form:
  */
 int32_t krag_index_commit(krag_index* idx, int64_t vocab);
 /* Multi-shard form: each rank reports local stats, the host all-reduces them (sum),
@@ -310,9 +311,15 @@ int64_t krag_host_rows_fetched(void);
  * flops of that launch -- bench.py's roofline line is computed from it. */
 int32_t krag_last_dense_kernel(float* ms, int32_t* kernel_id, int64_t* algorithmic_bytes, int64_t* flops);
 /* Figures of the last krag_index_compact on this process: CUDA-event duration of the row-move phase (device moves and
- * the host-row memmoves they overlap), host-clock duration of the postings rebuild (0 if the index was not committed),
+ * the host-row memmoves they overlap), host-clock duration of the postings remap (0 if the index never committed),
  * live rows that changed position, and the bytes of the moved rows and term lists (each counted once). */
 int32_t krag_last_compact(float* move_ms, float* postings_ms, int64_t* rows_moved, int64_t* bytes_moved);
+/* Figures of the last commit on this process (krag_index_commit, or a commit_local / commit_global pair, reported by the
+ * commit_global): host-clock duration of the whole commit, the part of it spent on the host computing idf, merged = 1
+ * when the committed postings were merged with the changes (0: a full build, the first commit of an index and the one after
+ * krag_index_load or krag_synth_fill), the postings written, and the term-list entries read to build them (those of the
+ * rows added since the last commit when merged, every entry otherwise). */
+int32_t krag_last_commit(float* total_ms, float* host_ms, int32_t* merged, int64_t* postings_written, int64_t* delta_entries);
 /* raw K2 output a[j][r] = |x_r|^2 - 2 x_r.q_j (TF32) for every row, [nq_pad][S] row-major;
  * call with out == NULL to query S and nq_pad.  Test hook for the tensor-core kernel; KRAG_E_UNSUPPORTED for
  * KRAG_ROWS_HOST indexes. */

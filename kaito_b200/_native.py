@@ -37,6 +37,7 @@ SYMBOLS = [
     "krag_debug_linear_ln", "krag_index_set_dense_mode", "krag_text_analyze", "krag_wordpiece_create",
     "krag_wordpiece_encode_batch", "krag_wordpiece_destroy", "krag_p2p_create", "krag_p2p_connect", "krag_dev_exchange_merge", "krag_p2p_destroy",
     "krag_host_pinned_bytes", "krag_host_rows_fetched", "krag_index_compact", "krag_last_compact",
+    "krag_last_commit",
 ]
 
 
@@ -131,6 +132,7 @@ def load() -> C.CDLL:
     L.krag_tc_fallback_queries.restype = i64
     L.krag_last_dense_kernel.argtypes = [C.POINTER(C.c_float), C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]
     L.krag_last_compact.argtypes = [C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(i64), C.POINTER(i64)]
+    L.krag_last_commit.argtypes = [C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]
     L.krag_debug_tc_dump.argtypes = [vp, i32, vp, vp, i64, C.POINTER(i64), C.POINTER(i32)]
     for name in SYMBOLS:
         fn = getattr(L, name)
@@ -167,6 +169,15 @@ def last_compact() -> dict:
     mv, po, rows, by = C.c_float(0), C.c_float(0), C.c_int64(0), C.c_int64(0)
     check(load().krag_last_compact(C.byref(mv), C.byref(po), C.byref(rows), C.byref(by)))
     return {"move_ms": mv.value, "postings_ms": po.value, "rows_moved": rows.value, "bytes_moved": by.value}
+
+
+def last_commit() -> dict:
+    """figures of the last commit of this process: total_ms (host clock), host_ms (idf on the host), merged (1: the committed
+    postings were merged with the changes, 0: a full build), postings_written, delta_entries (term-list entries read)"""
+    tot, host, mg, pw, de = C.c_float(0), C.c_float(0), C.c_int32(0), C.c_int64(0), C.c_int64(0)
+    check(load().krag_last_commit(C.byref(tot), C.byref(host), C.byref(mg), C.byref(pw), C.byref(de)))
+    return {"total_ms": tot.value, "host_ms": host.value, "merged": mg.value, "postings_written": pw.value,
+            "delta_entries": de.value}
 
 
 def device_bytes() -> int:

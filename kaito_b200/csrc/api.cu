@@ -5,6 +5,7 @@
 #include <string.h>
 #include <sys/stat.h>
 
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -12,6 +13,7 @@
 #include <mutex>
 #include <shared_mutex>
 #include <string>
+#include <thread>
 #include <unordered_map>
 #include <vector>
 
@@ -138,6 +140,17 @@ struct krag_ctx {
     ~krag_ctx() { if (admin) cudaStreamDestroy(admin); }
 };
 
+// what krag_index_commit_local leaves for krag_index_commit_global: valid for one index state (epoch) and vocab
+struct CommitPrep {
+    bool valid = false, merge = false;
+    int64_t vocab = 0, epoch = 0;
+    DevArray<uint32_t> entry_doc;   // row of each entry read: every entry (full build) or those of rows >= committed_rows (merge)
+    int64_t e0 = 0;                 // first entry read
+    SurvivorCounts sc;              // merge: live base postings per term
+    DevArray<uint32_t> delta_df;    // merge: live entries of rows >= committed_rows per term
+    double ms = 0.0;                // host-clock time spent preparing
+};
+
 struct krag_index {
     krag_ctx* ctx = nullptr;
     std::string name;
@@ -165,11 +178,13 @@ struct krag_index {
     DevArray<uint32_t> dlen;
     int64_t nnz = 0;
     uint32_t max_term_id = 0;       // largest term id ever added (commit requires vocab > max_term_id)
-    // committed postings
+    // committed postings; after later adds, removes or a compaction they stay the base of the next commit (has_base), exact
+    // for rows [0, committed_rows)
     Postings post;
-    DevArray<uint32_t> entry_doc;  // scratch kept between commit_local and commit_global
-    bool committed = false;
+    bool committed = false, has_base = false;
     int64_t committed_rows = 0;
+    int64_t epoch = 0;              // bumped by every change of the rows (add, remove, compact, synth fill)
+    CommitPrep prep;                // made by commit_local, used by the commit_global that follows it
     int64_t vocab = 0, n_docs_global = 0, total_len_global = 0;
     std::vector<float> idf;         // [vocab] and avgdl of the last commit: compaction rebuilds the postings with them
     double avgdl = 1.0;
@@ -363,34 +378,127 @@ void derive_host_rows(krag_index* ix, int64_t row0, int64_t n, cudaStream_t st, 
     KRAG_CUDA(cudaStreamSynchronize(st));
 }
 
+// figures of the last commit (krag_last_commit): process-wide, last writer wins
+struct CommitReport { float total_ms = 0.f, host_ms = 0.f; int32_t merged = 0; int64_t postings_written = 0, delta_entries = 0; bool valid = false; };
+std::mutex g_commit_mu;
+CommitReport g_commit;
+
+double ms_since(std::chrono::steady_clock::time_point t0)
+{
+    return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+}
+
+// device work both halves of a commit need: the entries to read and, with a base, its survivor counts and the delta's df
+void commit_prepare(krag_index* ix, int64_t vocab)
+{
+    const auto t0 = std::chrono::steady_clock::now();
+    cudaStream_t st = ix->ctx->admin;
+    CommitPrep& pr = ix->prep;
+    pr = CommitPrep{};
+    pr.merge = ix->has_base;
+    const int64_t row0 = pr.merge ? ix->committed_rows : 0;
+    if (row0 > 0) KRAG_CUDA(cudaMemcpyAsync(&pr.e0, ix->toff.p + row0, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    KRAG_CUDA(cudaStreamSynchronize(st));
+    const int64_t n_entries = ix->nnz - pr.e0;
+    pr.entry_doc.alloc(n_entries > 0 ? n_entries : 1);
+    if (ix->n_rows > row0) launch_expand_entry_doc(ix->toff.p, ix->n_rows - row0, pr.entry_doc.p, st, row0);
+    if (pr.merge) {
+        count_survivors(ix->post, alive_ptr(ix), vocab, pr.sc, st);
+        pr.delta_df.alloc(vocab);
+        KRAG_CUDA(cudaMemsetAsync(pr.delta_df.p, 0, sizeof(uint32_t) * (size_t)vocab, st));
+        if (n_entries > 0) launch_df_histogram(ix->tid.p + pr.e0, pr.entry_doc.p, alive_ptr(ix), n_entries, pr.delta_df.p, st);
+    }
+    KRAG_CUDA(cudaStreamSynchronize(st));
+    pr.vocab = vocab;
+    pr.epoch = ix->epoch;
+    pr.valid = true;
+    pr.ms = ms_since(t0);
+}
+
 void commit_local_impl(krag_index* ix, int64_t vocab, uint32_t* df_out, int64_t* n_live_out, int64_t* total_len_out)
 {
     cudaStream_t st = ix->ctx->admin;
     KRAG_REQUIRE(ix->has_sparse || ix->n_rows == 0, KRAG_E_STATE, "index holds no term lists (dense-only)");
     KRAG_REQUIRE(vocab > 0 && vocab < 0x7fffffffll, KRAG_E_INVALID, "vocab out of range");
-    ix->entry_doc.reserve(ix->nnz > 0 ? ix->nnz : 1, 0, st);
-    if (ix->n_rows > 0) launch_expand_entry_doc(ix->toff.p, ix->n_rows, ix->entry_doc.p, st);
-    DevArray<uint32_t> df;
-    df.alloc(vocab);
-    KRAG_CUDA(cudaMemsetAsync(df.p, 0, sizeof(uint32_t) * (size_t)vocab, st));
     // term ids >= vocab would make the df kernel write out of bounds: the largest id is tracked on the host at add time
     KRAG_REQUIRE(ix->nnz == 0 || vocab > (int64_t)ix->max_term_id, KRAG_E_INVALID,
                  "vocab must exceed the largest term id added to the index");
-    if (ix->nnz > 0) {
-        launch_df_histogram(ix->tid.p, ix->entry_doc.p, alive_ptr(ix), ix->nnz, df.p, st);
+    const auto t0 = std::chrono::steady_clock::now();
+    commit_prepare(ix, vocab);
+    DevArray<uint32_t> df;
+    df.alloc(vocab);
+    if (ix->prep.merge) {
+        launch_add_u32(ix->prep.sc.per_term.p, ix->prep.delta_df.p, vocab, df.p, st);
+    } else {
+        KRAG_CUDA(cudaMemsetAsync(df.p, 0, sizeof(uint32_t) * (size_t)vocab, st));
+        if (ix->nnz > 0) launch_df_histogram(ix->tid.p, ix->prep.entry_doc.p, alive_ptr(ix), ix->nnz, df.p, st);
     }
     KRAG_CUDA(cudaMemcpyAsync(df_out, df.p, sizeof(uint32_t) * (size_t)vocab, cudaMemcpyDeviceToHost, st));
-    // total length over live docs (host side: doc_len is small)
-    std::vector<uint32_t> dl((size_t)ix->n_rows);
-    if (ix->n_rows > 0)
-        KRAG_CUDA(cudaMemcpyAsync(dl.data(), ix->dlen.p, sizeof(uint32_t) * (size_t)ix->n_rows, cudaMemcpyDeviceToHost, st));
+    live_doc_stats(ix->dlen.p, alive_ptr(ix), ix->n_rows, n_live_out, total_len_out, st);
+    ix->prep.ms = ms_since(t0);
+}
+
+// idf on the host with glibc log(): the same libm call chain as the reference's math.log.  Split across threads for large
+// vocabularies; every value is computed alone, so the bits do not depend on the split.
+std::vector<float> host_idf(const uint32_t* df_global, int64_t vocab, int64_t n_docs_global)
+{
+    std::vector<float> idf((size_t)vocab);
+    auto run = [&](int64_t lo, int64_t hi) {
+        for (int64_t t = lo; t < hi; ++t) {
+            double dfd = (double)df_global[t];
+            idf[(size_t)t] = (float)log(1.0 + ((double)n_docs_global - dfd + 0.5) / (dfd + 0.5));
+        }
+    };
+    const int64_t per_thread = (int64_t)1 << 16;
+    int64_t n_threads = (vocab + per_thread - 1) / per_thread;
+    const int64_t hw = (int64_t)std::thread::hardware_concurrency();
+    n_threads = std::min<int64_t>(n_threads, std::min<int64_t>(hw > 0 ? hw : 1, 16));
+    if (n_threads <= 1) {
+        run(0, vocab);
+        return idf;
+    }
+    std::vector<std::thread> th;
+    const int64_t step = (vocab + n_threads - 1) / n_threads;
+    for (int64_t i = 0; i < n_threads; ++i) th.emplace_back(run, i * step, std::min(vocab, (i + 1) * step));
+    for (auto& t : th) t.join();
+    return idf;
+}
+
+// the base merged with the rows added since: survivors in base order, then the live new rows, every posting rescored
+Postings merge_postings(krag_index* ix, int64_t vocab, const float* idf, double avgdl)
+{
+    cudaStream_t st = ix->ctx->admin;
+    const CommitPrep& pr = ix->prep;
+    const int64_t n_entries = ix->nnz - pr.e0;
+    DevArray<int64_t> delta_off;
+    std::vector<int64_t> h_delta_off;
+    df_offsets(pr.delta_df.p, vocab, delta_off, &h_delta_off, st);
+    Postings out;
+    {
+        DevArray<uint32_t> df;
+        df.alloc(vocab);
+        launch_add_u32(pr.sc.per_term.p, pr.delta_df.p, vocab, df.p, st);
+        df_offsets(df.p, vocab, out.off, nullptr, st);
+    }
+    int64_t nnz = 0;
+    KRAG_CUDA(cudaMemcpyAsync(&nnz, out.off.p + vocab, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     KRAG_CUDA(cudaStreamSynchronize(st));
-    df.release();
-    int64_t total = 0, live = 0;
-    for (int64_t r = 0; r < ix->n_rows; ++r)
-        if ((ix->alive_h[(size_t)(r >> 5)] >> (r & 31)) & 1u) { total += dl[(size_t)r]; ++live; }
-    *n_live_out = live;
-    *total_len_out = total;
+    out.vocab = vocab;
+    out.nnz = nnz;
+    out.doc.alloc(nnz > 0 ? nnz : 1);
+    out.tf.alloc(nnz > 0 ? nnz : 1);
+    out.score.alloc(nnz > 0 ? nnz : 1);
+    if (nnz > 0) prepare_tile_index(out.off.p, vocab, ix->n_rows, out, st);
+    else empty_tile_index(vocab, ix->n_rows, out);
+    write_survivors(ix->post, alive_ptr(ix), pr.sc, out.off.p, nullptr, ix->dlen.p, idf, avgdl, out, st);
+    if (n_entries > 0)
+        sort_entries_by_term(ix->tid.p + pr.e0, ix->ttf.p + pr.e0, pr.entry_doc.p, alive_ptr(ix), n_entries, vocab, h_delta_off,
+                             [&](int64_t q_base, int64_t m, const uint32_t* keys, const uint64_t* vals) {
+                                 write_delta(keys, vals, q_base, m, delta_off.p, pr.sc, out.off.p, ix->dlen.p, idf, avgdl, out, st);
+                             }, st);
+    fill_tile_index(out, st);
+    KRAG_CUDA(cudaStreamSynchronize(st));
+    return out;
 }
 
 void commit_global_impl(krag_index* ix, int64_t vocab, const uint32_t* df_global, int64_t n_docs_global,
@@ -403,25 +511,33 @@ void commit_global_impl(krag_index* ix, int64_t vocab, const uint32_t* df_global
     KRAG_REQUIRE(n_docs_global >= 0 && total_len_global >= 0, KRAG_E_INVALID, "n_docs_global / total_len_global must be >= 0");
     KRAG_REQUIRE(ix->nnz == 0 || vocab > (int64_t)ix->max_term_id, KRAG_E_INVALID,
                  "vocab must exceed the largest term id added to the index");
-    // idf on the host with glibc log(): the same libm call chain as the reference's math.log
-    std::vector<float> idf((size_t)vocab);
-    for (int64_t t = 0; t < vocab; ++t) {
-        double dfd = (double)df_global[t];
-        idf[(size_t)t] = (float)log(1.0 + ((double)n_docs_global - dfd + 0.5) / (dfd + 0.5));
+    const auto t0 = std::chrono::steady_clock::now();
+    double local_ms = ix->prep.ms;      // commit_local's time; a preparation made here is inside this call's own time
+    if (!ix->prep.valid || ix->prep.vocab != vocab || ix->prep.epoch != ix->epoch) {
+        commit_prepare(ix, vocab);
+        local_ms = 0.0;
     }
+    const auto th = std::chrono::steady_clock::now();
+    std::vector<float> idf = host_idf(df_global, vocab, n_docs_global);
+    const double host_ms = ms_since(th);
     DevArray<float> d_idf;
     d_idf.alloc(vocab);
     KRAG_CUDA(cudaMemcpyAsync(d_idf.p, idf.data(), sizeof(float) * (size_t)vocab, cudaMemcpyHostToDevice, st));
     const double avgdl = n_docs_global > 0 ? (double)total_len_global / (double)n_docs_global : 1.0;
-    if (ix->entry_doc.cap < (ix->nnz > 0 ? ix->nnz : 1)) {
-        ix->entry_doc.reserve(ix->nnz > 0 ? ix->nnz : 1, 0, st);
-        if (ix->n_rows > 0) launch_expand_entry_doc(ix->toff.p, ix->n_rows, ix->entry_doc.p, st);
+    const bool merged = ix->prep.merge;
+    const int64_t delta_entries = ix->nnz - ix->prep.e0;
+    if (merged) {
+        Postings out = merge_postings(ix, vocab, d_idf.p, avgdl);   // the base stays intact until this has succeeded
+        ix->post = std::move(out);
+    } else {
+        ix->has_base = false;                                         // build_postings writes into ix->post
+        ix->committed = false;
+        build_postings(ix->tid.p, ix->ttf.p, ix->prep.entry_doc.p, ix->dlen.p, alive_ptr(ix), ix->nnz, vocab, d_idf.p, avgdl,
+                       ix->n_rows, ix->post, st);
     }
-    build_postings(ix->tid.p, ix->ttf.p, ix->entry_doc.p, ix->dlen.p, alive_ptr(ix), ix->nnz, vocab, d_idf.p, avgdl,
-                   ix->n_rows, ix->post, st);
     KRAG_CUDA(cudaStreamSynchronize(st));
     d_idf.release();
-    ix->entry_doc.release();
+    ix->prep = CommitPrep{};
     ix->idf = std::move(idf);
     ix->avgdl = avgdl;
     ix->vocab = vocab;
@@ -429,7 +545,17 @@ void commit_global_impl(krag_index* ix, int64_t vocab, const uint32_t* df_global
     ix->total_len_global = total_len_global;
     ix->ord_base = ord_base;
     ix->committed = true;
+    ix->has_base = true;
     ix->committed_rows = ix->n_rows;
+    CommitReport rep;
+    rep.total_ms = (float)(local_ms + ms_since(t0));
+    rep.host_ms = (float)host_ms;
+    rep.merged = merged ? 1 : 0;
+    rep.postings_written = ix->post.nnz;
+    rep.delta_entries = delta_entries;
+    rep.valid = true;
+    std::lock_guard<std::mutex> lk(g_commit_mu);
+    g_commit = rep;
 }
 
 // figures of the last compaction (krag_last_compact): process-wide, last writer wins
@@ -446,11 +572,42 @@ void compact_impl(krag_index* ix)
     compact_plan(ix->alive_d.p, ix->n_rows, ix->has_sparse ? ix->toff.p : nullptr, plan, st);
     const int64_t n = plan.n_live;
     const int64_t nnz = ix->has_sparse ? plan.h_toff_new[(size_t)n] : 0;
+    CompactReport rep;
+
+    // postings first, while the old row numbers and alive bits are still in place: the base's survivors renumbered to their
+    // ranks, scores and tf unchanged (the statistics they were computed with do not change), into new arrays -- an
+    // allocation failure leaves the index as it was
+    Postings remapped;
+    const bool keep_base = ix->has_base;
+    int64_t base_rows = 0;
+    if (keep_base) {
+        const auto t0 = std::chrono::steady_clock::now();
+        DevArray<uint32_t> rank;
+        rank.alloc(ix->n_rows);
+        launch_rank_of_rows(plan.src.p, n, rank.p, st);
+        SurvivorCounts sc;
+        count_survivors(ix->post, alive_ptr(ix), ix->post.vocab, sc, st);
+        int64_t pn = 0;
+        KRAG_CUDA(cudaMemcpyAsync(&pn, sc.before.p + ix->post.vocab, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+        KRAG_CUDA(cudaStreamSynchronize(st));
+        remapped.vocab = ix->post.vocab;
+        remapped.nnz = pn;
+        remapped.doc.alloc(pn > 0 ? pn : 1);
+        remapped.tf.alloc(pn > 0 ? pn : 1);
+        remapped.score.alloc(pn > 0 ? pn : 1);
+        write_survivors(ix->post, alive_ptr(ix), sc, sc.before.p, rank.p, nullptr, nullptr, 0.0, remapped, st);
+        remapped.off = std::move(sc.before);                        // the remapped offsets are the survivors' exclusive scan
+        if (pn > 0) prepare_tile_index(remapped.off.p, remapped.vocab, n, remapped, st);
+        else empty_tile_index(remapped.vocab, n, remapped);
+        fill_tile_index(remapped, st);
+        KRAG_CUDA(cudaStreamSynchronize(st));
+        base_rows = (int64_t)(std::lower_bound(plan.h_src.begin(), plan.h_src.end(), (uint32_t)ix->committed_rows) - plan.h_src.begin());
+        rep.postings_ms = (float)ms_since(t0);
+    }
 
     cudaEvent_t e0, e1;
     KRAG_CUDA(cudaEventCreate(&e0));
     KRAG_CUDA(cudaEventCreate(&e1));
-    CompactReport rep;
     KRAG_CUDA(cudaEventRecord(e0, st));
     // device arrays first (asynchronous); the pinned host rows move on the CPU meanwhile
     if (!ix->host_rows) rep.bytes_moved += compact_rows(ix->X.p, dp * (int64_t)sizeof(float), plan, st);
@@ -499,8 +656,10 @@ void compact_impl(krag_index* ix)
     ix->n_live = n;
     ix->has_dead = false;
     ix->nnz = nnz;
-    ix->entry_doc.release();
-    ix->post = Postings{};
+    ix->epoch++;
+    ix->prep = CommitPrep{};
+    ix->post = std::move(remapped);      // empty without a base
+    ix->committed_rows = base_rows;
 
     // exact-size buffers where they fit (never empty: a null Xh means "no bf16 shadow")
     const int64_t rows1 = n > 0 ? n : 1;
@@ -517,24 +676,6 @@ void compact_impl(krag_index* ix)
         ix->ttf.shrink(nnz > 0 ? nnz : 1, st);
     }
 
-    // postings of a committed index: rebuilt over the compacted term lists with the statistics of the last commit, so every
-    // score is the one the index returned before (including after a commit_global with multi-shard statistics)
-    const bool rebuild = ix->committed;
-    ix->committed = false;            // until the rebuild below has succeeded
-    if (rebuild) {
-        const auto t0 = std::chrono::steady_clock::now();
-        DevArray<float> d_idf;
-        d_idf.alloc(ix->vocab);
-        KRAG_CUDA(cudaMemcpyAsync(d_idf.p, ix->idf.data(), sizeof(float) * (size_t)ix->vocab, cudaMemcpyHostToDevice, st));
-        ix->entry_doc.alloc(nnz > 0 ? nnz : 1);
-        if (n > 0) launch_expand_entry_doc(ix->toff.p, n, ix->entry_doc.p, st);
-        build_postings(ix->tid.p, ix->ttf.p, ix->entry_doc.p, ix->dlen.p, nullptr, nnz, ix->vocab, d_idf.p, ix->avgdl, n, ix->post, st);
-        KRAG_CUDA(cudaStreamSynchronize(st));
-        ix->entry_doc.release();
-        ix->committed = true;
-        ix->committed_rows = n;
-        rep.postings_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    }
     rep.valid = true;
     std::lock_guard<std::mutex> lk(g_compact_mu);
     g_compact = rep;
@@ -714,6 +855,7 @@ int32_t krag_index_add(krag_index* ix, int64_t n, const uint64_t* node_ids, cons
         ix->n_live += n;
         ix->nnz += add_nnz;
         ix->has_sparse = sparse;
+        ix->epoch++;
         ix->committed = false;  // postings are stale until the next commit (reference rebuilds per query)
     });
 }
@@ -736,7 +878,7 @@ int32_t krag_index_remove(krag_index* ix, int64_t n, const uint64_t* node_ids, i
             ++removed;
         }
         KRAG_CUDA(cudaStreamSynchronize(ix->ctx->admin));
-        if (removed) { ix->has_dead = true; ix->n_live -= removed; }
+        if (removed) { ix->has_dead = true; ix->n_live -= removed; ix->epoch++; }
         if (n_removed) *n_removed = removed;
     });
 }
@@ -765,6 +907,17 @@ int32_t krag_last_compact(float* move_ms, float* postings_ms, int64_t* rows_move
         KRAG_REQUIRE(g_compact.valid, KRAG_E_STATE, "no compaction has run yet");
         *move_ms = g_compact.move_ms; *postings_ms = g_compact.postings_ms;
         *rows_moved = g_compact.rows_moved; *bytes_moved = g_compact.bytes_moved;
+    });
+}
+
+int32_t krag_last_commit(float* total_ms, float* host_ms, int32_t* merged, int64_t* postings_written, int64_t* delta_entries)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(total_ms && host_ms && merged && postings_written && delta_entries, KRAG_E_INVALID, "null argument");
+        std::lock_guard<std::mutex> lk(g_commit_mu);
+        KRAG_REQUIRE(g_commit.valid, KRAG_E_STATE, "no commit has run yet");
+        *total_ms = g_commit.total_ms; *host_ms = g_commit.host_ms; *merged = g_commit.merged;
+        *postings_written = g_commit.postings_written; *delta_entries = g_commit.delta_entries;
     });
 }
 
@@ -824,7 +977,7 @@ int32_t krag_index_stats(krag_index* ix, krag_stats_t* out)
         out->ordinal_base = ix->ord_base; out->dim = ix->dim; out->dim_padded = ix->dpad;
         out->committed = ix->committed && ix->committed_rows == ix->n_rows;
         out->device_bytes = ix->X.bytes() + ix->Xh.bytes() + ix->xres.bytes() + ix->xnorm.bytes() + ix->alive_d.bytes() + ix->toff.bytes() + ix->tid.bytes() + ix->ttf.bytes() +
-                            ix->dlen.bytes() + (ix->committed ? (int64_t)(ix->post.nnz * 8 + (ix->post.vocab + 1) * 8) : 0);
+                            ix->dlen.bytes() + (ix->committed ? (int64_t)(ix->post.nnz * 10 + (ix->post.vocab + 1) * 8) : 0);
     });
 }
 
@@ -1042,6 +1195,7 @@ int32_t krag_synth_fill(krag_index* ix, int64_t n, int64_t row_base, uint64_t se
         ix->node_ids.resize((size_t)n);
         for (int64_t i = 0; i < n; ++i) { ix->node_ids[(size_t)i] = (uint64_t)(row_base + i); ix->id2row[(uint64_t)(row_base + i)] = i; }
         ix->n_rows = n; ix->n_live = n; ix->ord_base = row_base; ix->ord_stride = 1; ix->committed = false;
+        ix->has_base = false; ix->post = Postings{}; ix->epoch++;
     });
 }
 

@@ -31,19 +31,21 @@
 namespace krag {
 
 // -------------------------------------------------------------------------- index time
-__global__ void expand_entry_doc_kernel(const int64_t* __restrict__ off, int64_t n_docs, uint32_t* __restrict__ entry_doc)
+__global__ void expand_entry_doc_kernel(const int64_t* __restrict__ off, int64_t row0, int64_t n_docs, uint32_t* __restrict__ entry_doc)
 {
     // one warp per document
     int64_t d = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     int lane = threadIdx.x & 31;
     if (d >= n_docs) return;
-    for (int64_t i = off[d] + lane; i < off[d + 1]; i += 32) entry_doc[i] = (uint32_t)d;
+    d += row0;
+    const int64_t e0 = off[row0];
+    for (int64_t i = off[d] + lane; i < off[d + 1]; i += 32) entry_doc[i - e0] = (uint32_t)d;
 }
-void launch_expand_entry_doc(const int64_t* term_offsets, int64_t n_docs, uint32_t* entry_doc, cudaStream_t st)
+void launch_expand_entry_doc(const int64_t* term_offsets, int64_t n_docs, uint32_t* entry_doc, cudaStream_t st, int64_t row0)
 {
     if (n_docs == 0) return;
     int64_t threads = n_docs * 32;
-    expand_entry_doc_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(term_offsets, n_docs, entry_doc);
+    expand_entry_doc_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(term_offsets, row0, n_docs, entry_doc);
     KRAG_CUDA(cudaGetLastError());
     count_launch();
 }
@@ -121,22 +123,16 @@ chunk_scatter_kernel(const uint32_t* __restrict__ term_ids, const uint16_t* __re
 
 __global__ void score_postings_kernel(const uint32_t* __restrict__ sorted_terms, const uint64_t* __restrict__ sorted_vals,
                                       const uint32_t* __restrict__ doc_len, const float* __restrict__ idf, double avgdl,
-                                      int64_t nnz_live, uint32_t* __restrict__ post_doc, float* __restrict__ post_score)
+                                      int64_t nnz_live, uint32_t* __restrict__ post_doc, uint16_t* __restrict__ post_tf,
+                                      float* __restrict__ post_score)
 {
-    const double k1 = 1.5, b = 0.75;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nnz_live; i += (int64_t)gridDim.x * blockDim.x) {
         uint64_t v = sorted_vals[i];
         uint32_t d = (uint32_t)(v >> 16);
-        double tf = (double)(uint32_t)(v & 0xffffu);
-        // tf / (k1 * ((1 - b) + b * dl / avgdl) + tf), left-to-right as Python evaluates it
-        double t1 = __dmul_rn(b, (double)doc_len[d]);
-        double t2 = __ddiv_rn(t1, avgdl);
-        double t3 = __dadd_rn(__dsub_rn(1.0, b), t2);
-        double t4 = __dmul_rn(k1, t3);
-        double t5 = __dadd_rn(t4, tf);
-        double tfc = __ddiv_rn(tf, t5);
+        const uint32_t tf = (uint32_t)(v & 0xffffu);
         post_doc[i] = d;
-        post_score[i] = __double2float_rn(__dmul_rn((double)idf[sorted_terms[i]], tfc));
+        post_tf[i] = (uint16_t)tf;
+        post_score[i] = bm25_posting_score(idf[sorted_terms[i]], tf, doc_len[d], avgdl);
     }
 }
 
@@ -180,8 +176,8 @@ __global__ void tile_index_kernel(const uint32_t* __restrict__ sorted_terms, con
 // cub temporary storage: never a null pointer, which cub would take for a size query
 static size_t cub_tmp_bytes(size_t bytes) { return bytes ? bytes : 1; }
 
-// slots of the frequent terms (df > BM25_RARE_MAX) and the (still empty) boundary table; filled range by range below
-static void prepare_tile_index(const int64_t* off, int64_t vocab, int64_t n_rows, Postings& out, cudaStream_t st)
+// slots of the frequent terms (df > BM25_RARE_MAX) and the (still empty) boundary table
+void prepare_tile_index(const int64_t* off, int64_t vocab, int64_t n_rows, Postings& out, cudaStream_t st)
 {
     DevArray<int32_t> flag, scan, slot;
     flag.alloc(vocab + 1);
@@ -208,6 +204,26 @@ static void prepare_tile_index(const int64_t* off, int64_t vocab, int64_t n_rows
     out.tile_slot = std::move(slot); out.tile_off = std::move(tile_off); out.n_slots = n_slots; out.n_tiles = n_tiles;
 }
 
+void df_offsets(const uint32_t* df, int64_t vocab, DevArray<int64_t>& off, std::vector<int64_t>* h_off, cudaStream_t st)
+{
+    DevArray<int64_t> tmp64;
+    off.alloc(vocab + 1);
+    tmp64.alloc(vocab + 1);
+    df_to_i64_kernel<<<256, 256, 0, st>>>(df, vocab, tmp64.p);
+    count_launch();
+    size_t scan_bytes = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, tmp64.p, off.p, (int)(vocab + 1), st);
+    DevArray<unsigned char> scan_tmp;
+    scan_tmp.alloc(cub_tmp_bytes(scan_bytes));
+    cub::DeviceScan::ExclusiveSum(scan_tmp.p, scan_bytes, tmp64.p, off.p, (int)(vocab + 1), st);
+    count_launch();
+    if (h_off) {
+        h_off->resize((size_t)(vocab + 1));
+        KRAG_CUDA(cudaMemcpyAsync(h_off->data(), off.p, sizeof(int64_t) * (size_t)(vocab + 1), cudaMemcpyDeviceToHost, st));
+    }
+    KRAG_CUDA(cudaStreamSynchronize(st));
+}
+
 // postings per term range of the build: KRAG_BM25_BUILD_CHUNK, else what fits in 70 % of the free device memory at 24 bytes
 // of sort buffers per posting + 12 for the alternate key/value buffers the radix sort keeps in its temporary storage
 static int64_t build_chunk_cap(int64_t nnz_live)
@@ -225,6 +241,93 @@ static int64_t build_chunk_cap(int64_t nnz_live)
     return cap < nnz_live ? cap : nnz_live;
 }
 
+void empty_tile_index(int64_t vocab, int64_t n_rows, Postings& out)
+{
+    DevArray<int32_t> slot;
+    slot.alloc(vocab);
+    KRAG_CUDA(cudaMemset(slot.p, 0xFF, sizeof(int32_t) * (size_t)vocab));
+    DevArray<uint32_t> toff;
+    toff.alloc(4);
+    out.tile_slot = std::move(slot); out.tile_off = std::move(toff); out.n_slots = 0;
+    out.n_tiles = (n_rows + BM25_SUB_DOCS - 1) / BM25_SUB_DOCS < 1 ? 1 : (n_rows + BM25_SUB_DOCS - 1) / BM25_SUB_DOCS;
+}
+
+void sort_entries_by_term(const uint32_t* term_ids, const uint16_t* term_tf, const uint32_t* entry_doc, const uint32_t* alive,
+                          int64_t nnz, int64_t vocab, const std::vector<int64_t>& h_off, const TermRangeFn& per_range,
+                          cudaStream_t st)
+{
+    const int64_t nnz_live = h_off[(size_t)vocab];
+    if (nnz == 0 || nnz_live == 0) return;
+    // term ranges [t_lo, t_hi) of at most `cap` postings each (a single term longer than that is a range of its own).  The
+    // sort buffers are sized for the widest range; if they do not fit after all (fragmentation, another context on the
+    // device), the ranges are halved until they do
+    int64_t cap = build_chunk_cap(nnz_live);
+    const int64_t n_blocks = (nnz + (int64_t)CC_THREADS * CC_ITEMS - 1) / ((int64_t)CC_THREADS * CC_ITEMS);
+    if (n_blocks >= ((int64_t)1 << 31)) throw std::runtime_error("bm25 build: too many index entries on one shard");
+    DevArray<uint32_t> block_cnt, block_off;
+    block_cnt.alloc(n_blocks);
+    block_off.alloc(n_blocks);
+    size_t bscan_bytes = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, bscan_bytes, block_cnt.p, block_off.p, (int)n_blocks, st);
+    DevArray<unsigned char> bscan_tmp;
+    bscan_tmp.alloc(cub_tmp_bytes(bscan_bytes));
+    int end_bit = 1;
+    while (((int64_t)1 << end_bit) < vocab) ++end_bit;  // keys range over [0, vocab)
+    std::vector<int64_t> cuts;
+    DevArray<uint32_t> k_in, k_out;
+    DevArray<uint64_t> v_in, v_out;
+    DevArray<unsigned char> sort_tmp;
+    size_t sort_bytes = 0;
+    for (;;) {
+        cuts.assign(1, 0);
+        int64_t widest = 0;
+        while (cuts.back() < vocab) {
+            const int64_t t_lo = cuts.back();
+            int64_t t_hi = (int64_t)(std::upper_bound(h_off.begin() + t_lo, h_off.end(), h_off[(size_t)t_lo] + cap) - h_off.begin()) - 1;
+            if (t_hi <= t_lo) t_hi = t_lo + 1;
+            if (t_hi > vocab) t_hi = vocab;
+            cuts.push_back(t_hi);
+            widest = std::max(widest, h_off[(size_t)t_hi] - h_off[(size_t)t_lo]);
+        }
+        if (widest >= ((int64_t)1 << 31)) throw std::runtime_error("bm25 build: a single term has too many postings for one build range");
+        try {
+            // stable LSD radix sort by term id keeps documents ascending inside every term
+            k_in.alloc(widest);
+            k_out.alloc(widest);
+            v_in.alloc(widest);
+            v_out.alloc(widest);
+            sort_bytes = 0;
+            cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, k_in.p, k_out.p, v_in.p, v_out.p, widest, 0, end_bit, st);
+            sort_tmp.alloc(cub_tmp_bytes(sort_bytes));
+            break;
+        } catch (const DevOom&) {
+            k_in.release(); k_out.release(); v_in.release(); v_out.release();
+            if (cap <= ((int64_t)1 << 22) || widest > cap) throw;      // cannot get smaller: the widest range is one term
+            cap /= 2;
+        }
+    }
+    for (size_t c = 0; c + 1 < cuts.size(); ++c) {
+        const int64_t t_lo = cuts[c], t_hi = cuts[c + 1];
+        const int64_t p_base = h_off[(size_t)t_lo], m = h_off[(size_t)t_hi] - p_base;
+        if (m == 0) continue;
+        chunk_count_kernel<<<(unsigned)n_blocks, CC_THREADS, 0, st>>>(term_ids, entry_doc, alive, nnz, (uint32_t)t_lo, (uint32_t)t_hi,
+                                                                     block_cnt.p);
+        KRAG_CUDA(cudaGetLastError());
+        count_launch();
+        cub::DeviceScan::ExclusiveSum(bscan_tmp.p, bscan_bytes, block_cnt.p, block_off.p, (int)n_blocks, st);
+        count_launch();
+        chunk_scatter_kernel<<<(unsigned)n_blocks, CC_THREADS, 0, st>>>(term_ids, term_tf, entry_doc, alive, nnz, (uint32_t)t_lo,
+                                                                       (uint32_t)t_hi, block_off.p, k_in.p, v_in.p);
+        KRAG_CUDA(cudaGetLastError());
+        count_launch();
+        size_t sb = sort_bytes;
+        cub::DeviceRadixSort::SortPairs(sort_tmp.p, sb, k_in.p, k_out.p, v_in.p, v_out.p, m, 0, end_bit, st);
+        count_launch();
+        per_range(p_base, m, k_out.p, v_out.p);
+    }
+    KRAG_CUDA(cudaStreamSynchronize(st));
+}
+
 void build_postings(const uint32_t* term_ids, const uint16_t* term_tf, const uint32_t* entry_doc,
                     const uint32_t* doc_len, const uint32_t* alive, int64_t nnz, int64_t vocab, const float* idf,
                     double avgdl, int64_t n_docs_rows, Postings& out, cudaStream_t st)
@@ -234,115 +337,37 @@ void build_postings(const uint32_t* term_ids, const uint16_t* term_tf, const uin
     df_local.alloc(vocab + 1);
     KRAG_CUDA(cudaMemsetAsync(df_local.p, 0, sizeof(uint32_t) * (size_t)(vocab + 1), st));
     launch_df_histogram(term_ids, entry_doc, alive, nnz, df_local.p, st);
-    DevArray<int64_t> off, tmp64;
-    off.alloc(vocab + 1);
-    tmp64.alloc(vocab + 1);
-    df_to_i64_kernel<<<256, 256, 0, st>>>(df_local.p, vocab, tmp64.p);
-    count_launch();
-    size_t scan_bytes = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, tmp64.p, off.p, (int)(vocab + 1), st);
-    DevArray<unsigned char> scan_tmp;
-    scan_tmp.alloc(cub_tmp_bytes(scan_bytes));
-    cub::DeviceScan::ExclusiveSum(scan_tmp.p, scan_bytes, tmp64.p, off.p, (int)(vocab + 1), st);
-    count_launch();
-    std::vector<int64_t> h_off((size_t)(vocab + 1));
-    KRAG_CUDA(cudaMemcpyAsync(h_off.data(), off.p, sizeof(int64_t) * (size_t)(vocab + 1), cudaMemcpyDeviceToHost, st));
-    KRAG_CUDA(cudaStreamSynchronize(st));
+    DevArray<int64_t> off;
+    std::vector<int64_t> h_off;
+    df_offsets(df_local.p, vocab, off, &h_off, st);
     const int64_t nnz_live = h_off[(size_t)vocab];
-    scan_tmp.release(); tmp64.release(); df_local.release();
+    df_local.release();
 
     DevArray<uint32_t> post_doc;
+    DevArray<uint16_t> post_tf;
     DevArray<float> post_score;
     post_doc.alloc(nnz_live > 0 ? nnz_live : 1);
+    post_tf.alloc(nnz_live > 0 ? nnz_live : 1);
     post_score.alloc(nnz_live > 0 ? nnz_live : 1);
 
     if (nnz > 0 && nnz_live > 0) {
         prepare_tile_index(off.p, vocab, n_docs_rows, out, st);
-        // term ranges [t_lo, t_hi) of at most `cap` postings each (a single term longer than that is a range of its own).  The
-        // sort buffers are sized for the widest range; if they do not fit after all (fragmentation, another context on the
-        // device), the ranges are halved until they do
-        int64_t cap = build_chunk_cap(nnz_live);
-        const int64_t n_blocks = (nnz + (int64_t)CC_THREADS * CC_ITEMS - 1) / ((int64_t)CC_THREADS * CC_ITEMS);
-        if (n_blocks >= ((int64_t)1 << 31)) throw std::runtime_error("bm25 build: too many index entries on one shard");
-        DevArray<uint32_t> block_cnt, block_off;
-        block_cnt.alloc(n_blocks);
-        block_off.alloc(n_blocks);
-        size_t bscan_bytes = 0;
-        cub::DeviceScan::ExclusiveSum(nullptr, bscan_bytes, block_cnt.p, block_off.p, (int)n_blocks, st);
-        DevArray<unsigned char> bscan_tmp;
-        bscan_tmp.alloc(cub_tmp_bytes(bscan_bytes));
-        int end_bit = 1;
-        while (((int64_t)1 << end_bit) < vocab) ++end_bit;  // keys range over [0, vocab)
-        std::vector<int64_t> cuts;
-        DevArray<uint32_t> k_in, k_out;
-        DevArray<uint64_t> v_in, v_out;
-        DevArray<unsigned char> sort_tmp;
-        size_t sort_bytes = 0;
-        for (;;) {
-            cuts.assign(1, 0);
-            int64_t widest = 0;
-            while (cuts.back() < vocab) {
-                const int64_t t_lo = cuts.back();
-                int64_t t_hi = (int64_t)(std::upper_bound(h_off.begin() + t_lo, h_off.end(), h_off[(size_t)t_lo] + cap) - h_off.begin()) - 1;
-                if (t_hi <= t_lo) t_hi = t_lo + 1;
-                if (t_hi > vocab) t_hi = vocab;
-                cuts.push_back(t_hi);
-                widest = std::max(widest, h_off[(size_t)t_hi] - h_off[(size_t)t_lo]);
-            }
-            if (widest >= ((int64_t)1 << 31)) throw std::runtime_error("bm25 build: a single term has too many postings for one build range");
-            try {
-                // stable LSD radix sort by term id keeps documents ascending inside every term
-                k_in.alloc(widest);
-                k_out.alloc(widest);
-                v_in.alloc(widest);
-                v_out.alloc(widest);
-                sort_bytes = 0;
-                cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, k_in.p, k_out.p, v_in.p, v_out.p, widest, 0, end_bit, st);
-                sort_tmp.alloc(cub_tmp_bytes(sort_bytes));
-                break;
-            } catch (const DevOom&) {
-                k_in.release(); k_out.release(); v_in.release(); v_out.release();
-                if (cap <= ((int64_t)1 << 22) || widest > cap) throw;      // cannot get smaller: the widest range is one term
-                cap /= 2;
-            }
-        }
-        for (size_t c = 0; c + 1 < cuts.size(); ++c) {
-            const int64_t t_lo = cuts[c], t_hi = cuts[c + 1];
-            const int64_t p_base = h_off[(size_t)t_lo], m = h_off[(size_t)t_hi] - p_base;
-            if (m == 0) continue;
-            chunk_count_kernel<<<(unsigned)n_blocks, CC_THREADS, 0, st>>>(term_ids, entry_doc, alive, nnz, (uint32_t)t_lo, (uint32_t)t_hi,
-                                                                         block_cnt.p);
-            KRAG_CUDA(cudaGetLastError());
-            count_launch();
-            cub::DeviceScan::ExclusiveSum(bscan_tmp.p, bscan_bytes, block_cnt.p, block_off.p, (int)n_blocks, st);
-            count_launch();
-            chunk_scatter_kernel<<<(unsigned)n_blocks, CC_THREADS, 0, st>>>(term_ids, term_tf, entry_doc, alive, nnz, (uint32_t)t_lo,
-                                                                           (uint32_t)t_hi, block_off.p, k_in.p, v_in.p);
-            KRAG_CUDA(cudaGetLastError());
-            count_launch();
-            size_t sb = sort_bytes;
-            cub::DeviceRadixSort::SortPairs(sort_tmp.p, sb, k_in.p, k_out.p, v_in.p, v_out.p, m, 0, end_bit, st);
-            count_launch();
-            score_postings_kernel<<<132 * 8, 256, 0, st>>>(k_out.p, v_out.p, doc_len, idf, avgdl, m, post_doc.p + p_base, post_score.p + p_base);
+        sort_entries_by_term(term_ids, term_tf, entry_doc, alive, nnz, vocab, h_off,
+                             [&](int64_t p_base, int64_t m, const uint32_t* keys, const uint64_t* vals) {
+            score_postings_kernel<<<132 * 8, 256, 0, st>>>(keys, vals, doc_len, idf, avgdl, m, post_doc.p + p_base, post_tf.p + p_base,
+                                                           post_score.p + p_base);
             count_launch();
             if (out.n_slots > 0) {
-                tile_index_kernel<<<132 * 8, 256, 0, st>>>(k_out.p, post_doc.p, off.p, out.tile_slot.p, p_base, m, out.n_tiles, out.tile_off.p);
+                tile_index_kernel<<<132 * 8, 256, 0, st>>>(keys, post_doc.p, off.p, out.tile_slot.p, p_base, m, out.n_tiles, out.tile_off.p);
                 KRAG_CUDA(cudaGetLastError());
                 count_launch();
             }
-        }
-        KRAG_CUDA(cudaStreamSynchronize(st));
+        }, st);
+    } else {   // no postings: every term is "rare" with an empty list
+        empty_tile_index(vocab, n_docs_rows, out);
     }
-    if (nnz_live == 0 || nnz == 0) {   // no postings: every term is "rare" with an empty list
-        DevArray<int32_t> slot;
-        slot.alloc(vocab);
-        KRAG_CUDA(cudaMemset(slot.p, 0xFF, sizeof(int32_t) * (size_t)vocab));
-        DevArray<uint32_t> toff;
-        toff.alloc(4);
-        out.tile_slot = std::move(slot); out.tile_off = std::move(toff); out.n_slots = 0;
-        out.n_tiles = (n_docs_rows + BM25_SUB_DOCS - 1) / BM25_SUB_DOCS < 1 ? 1 : (n_docs_rows + BM25_SUB_DOCS - 1) / BM25_SUB_DOCS;
-    }
-    out.off = std::move(off); out.doc = std::move(post_doc); out.score = std::move(post_score); out.vocab = vocab; out.nnz = nnz_live;
+    out.off = std::move(off); out.doc = std::move(post_doc); out.tf = std::move(post_tf); out.score = std::move(post_score);
+    out.vocab = vocab; out.nnz = nnz_live;
 }
 
 // -------------------------------------------------------------------------- query time

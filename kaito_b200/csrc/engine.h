@@ -5,6 +5,7 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <functional>
 #include <stdexcept>
 #include <utility>
 #include <vector>
@@ -293,6 +294,7 @@ constexpr int BM25_TILE_DOCS = BM25_SUB_DOCS * BM25_SUBS_PER_TILE;   // doc rang
 struct Postings {
     DevArray<int64_t> off;     // [vocab+1]
     DevArray<uint32_t> doc;    // [nnz] local rows ascending inside a term
+    DevArray<uint16_t> tf;     // [nnz] term frequency of the posting: an incremental commit rescores from it (K3 never reads it)
     DevArray<float> score;     // [nnz]
     int64_t vocab = 0, nnz = 0;
     // tile index: for terms with more than BM25_RARE_MAX postings, the offset (relative to off[t]) of the
@@ -306,7 +308,35 @@ struct Postings {
 constexpr int BM25_RARE_MAX = 2048;
 void launch_df_histogram(const uint32_t* term_ids, const uint32_t* entry_doc, const uint32_t* alive, int64_t nnz,
                          uint32_t* df, cudaStream_t st);
-void launch_expand_entry_doc(const int64_t* term_offsets, int64_t n_docs, uint32_t* entry_doc, cudaStream_t st);
+// entry_doc[i - term_offsets[row0]] = d for the entries i of rows d in [row0, row0 + n_docs)
+void launch_expand_entry_doc(const int64_t* term_offsets, int64_t n_docs, uint32_t* entry_doc, cudaStream_t st, int64_t row0 = 0);
+// score(t, d) = f32(f64(idf[t]) * tf / (k1 * ((1 - b) + b * dl / avgdl) + tf)), k1 = 1.5, b = 0.75, left to right as Python
+// evaluates it, every operation correctly rounded and none contracted: the full build and the incremental merge both use it
+__device__ __forceinline__ float bm25_posting_score(float idf, uint32_t tf, uint32_t dl, double avgdl)
+{
+    const double k1 = 1.5, b = 0.75;
+    const double tfd = (double)tf;
+    double t1 = __dmul_rn(b, (double)dl);
+    double t2 = __ddiv_rn(t1, avgdl);
+    double t3 = __dadd_rn(__dsub_rn(1.0, b), t2);
+    double t4 = __dmul_rn(k1, t3);
+    double t5 = __dadd_rn(t4, tfd);
+    double tfc = __ddiv_rn(tfd, t5);
+    return __double2float_rn(__dmul_rn((double)idf, tfc));
+}
+// df [vocab] (device) -> off [vocab + 1] = exclusive scan (int64), with a host copy when h_off != null; synchronises st
+void df_offsets(const uint32_t* df, int64_t vocab, DevArray<int64_t>& off, std::vector<int64_t>* h_off, cudaStream_t st);
+// tile index of postings with offsets off: slots of the frequent terms and the boundary table, to be filled; or, for
+// postings without entries, no slot at all
+void prepare_tile_index(const int64_t* off, int64_t vocab, int64_t n_rows, Postings& out, cudaStream_t st);
+void empty_tile_index(int64_t vocab, int64_t n_rows, Postings& out);
+// The live entries of CSR-by-doc arrays sorted by term, documents ascending inside a term, one term range at a time:
+// per_range(p_base, m, keys, vals) gets postings [p_base, p_base + m) of the offsets h_off (host copy of the live df's
+// exclusive scan) as term ids and (doc << 16 | tf), valid until it returns.  Synchronises st at the end.
+using TermRangeFn = std::function<void(int64_t p_base, int64_t m, const uint32_t* keys, const uint64_t* vals)>;
+void sort_entries_by_term(const uint32_t* term_ids, const uint16_t* term_tf, const uint32_t* entry_doc, const uint32_t* alive,
+                          int64_t nnz, int64_t vocab, const std::vector<int64_t>& h_off, const TermRangeFn& per_range,
+                          cudaStream_t st);
 // builds postings from CSR-by-doc arrays; idf is a device array [vocab] computed on the host (glibc log)
 void build_postings(const uint32_t* term_ids, const uint16_t* term_tf, const uint32_t* entry_doc,
                     const uint32_t* doc_len, const uint32_t* alive, int64_t nnz, int64_t vocab, const float* idf,
@@ -316,6 +346,33 @@ size_t bm25_resolve_bytes(int64_t n_rows, int n_terms_total);   // size of launc
 void launch_bm25(const DeviceInfo& di, const Postings& post, int64_t n_rows, const uint32_t* alive,
                  const uint32_t* q_terms, const int32_t* q_term_offsets, int n_terms_total, void* resolve_ws, int batch, int P,
                  OrdMap ord_base, uint64_t* part, uint64_t* keys_out, cudaStream_t st);
+
+// ---- incremental postings (postings_merge.cu).  The postings of a commit stay the *base* of the next one: for each term,
+// the rows below base_rows that were alive then, ascending.  Rows never come back to life and rows added since have higher
+// numbers, so a term's new list is its base list without the rows dead now, followed by its live new rows.
+struct SurvivorCounts {
+    DevArray<uint32_t> per_term;    // [vocab] live postings of each term's base list
+    DevArray<int64_t> before;       // [vocab + 1] exclusive scan of per_term
+    DevArray<int64_t> block_off;    // [blocks of the base postings] live base postings before each block
+};
+// survivors of base postings `base` (alive == null: all live) counted per term, for the new vocab (>= every base term + 1)
+void count_survivors(const Postings& base, const uint32_t* alive, int64_t vocab, SurvivorCounts& sc, cudaStream_t st);
+// writes the survivors of `base` into out (allocated): survivor k of term t (base order) lands at out_off[t] + k.
+// Rescored (doc_len, idf, avgdl) when rank == null; otherwise doc -> rank[doc] with tf and score copied.
+void write_survivors(const Postings& base, const uint32_t* alive, const SurvivorCounts& sc, const int64_t* out_off,
+                     const uint32_t* rank, const uint32_t* doc_len, const float* idf, double avgdl, Postings& out, cudaStream_t st);
+// delta postings (term ids keys, (doc << 16 | tf) vals) [q_base, q_base + m) of the delta offsets delta_off: delta posting q of
+// term t lands at out_off[t] + survivors(t) + (q - delta_off[t]), rescored
+void write_delta(const uint32_t* keys, const uint64_t* vals, int64_t q_base, int64_t m, const int64_t* delta_off,
+                 const SurvivorCounts& sc, const int64_t* out_off, const uint32_t* doc_len, const float* idf, double avgdl,
+                 Postings& out, cudaStream_t st);
+// fills the tile index prepared by prepare_tile_index from out.off / out.doc
+void fill_tile_index(Postings& out, cudaStream_t st);
+// (live rows, sum of their doc_len) over rows [0, n_rows)
+void live_doc_stats(const uint32_t* doc_len, const uint32_t* alive, int64_t n_rows, int64_t* n_live, int64_t* total_len,
+                    cudaStream_t st);
+void launch_add_u32(const uint32_t* a, const uint32_t* b, int64_t n, uint32_t* out, cudaStream_t st);
+void launch_rank_of_rows(const uint32_t* src, int64_t n_live, uint32_t* rank, cudaStream_t st);
 
 // ---- compaction (compact.cu): tombstoned rows removed in place, live rows keep their order
 constexpr int64_t COMPACT_STAGE_BYTES = (int64_t)32 << 20;   // staging of windows whose source and destination overlap
