@@ -140,6 +140,43 @@ int32_t krag_index_remove(krag_index* idx, int64_t n, const uint64_t* node_ids, 
  * KRAG_E_UNSUPPORTED for an ordinal stride > 1 (round-robin shards, krag_index_set_ordinal_map): the index is unchanged.
  * No counterpart in the reference, whose FAISS IndexIDMap.remove_ids compacts on every delete. */
 int32_t krag_index_compact(krag_index* idx, int64_t* n_reclaimed_out);
+/* Copy of the alive bitmap (bit r of word r / 32 = local row r is live; bits past the rows are 0).  *words_out =
+ * (n_rows + 31) / 32; out == NULL only reports it.  The input of krag_redeal_begin. */
+int32_t krag_index_alive_bitmap(krag_index* idx, uint32_t* out, int64_t cap_words, int64_t* words_out);
+/*
+ * Redeal: compaction of the G round-robin shards of one index together (shard s = ordinal map (s, G), one per rank; no
+ * counterpart in the reference).  Afterwards shard s, row j holds the live row whose new global ordinal is j * G + s: the
+ * layout a fresh service builds by inserting only the live nodes, in their old order.  Node ids become the new ordinals
+ * (every node id must equal its ordinal before).  Vectors, the bf16 copy, norms, doc lengths and term lists move; the
+ * postings are dropped, so the session ends with the collective commit (commit_local -> all-reduce -> commit_global), a
+ * full build under the last commit's statistics.  Rows move between ranks in windows of new ordinals over a transport the
+ * host provides (kaito_b200/sharded.py: all_to_all_single).  Every rank, in the same order:
+ *   1. krag_index_alive_bitmap; the host gathers every shard's bitmap, padded to the longest: alive_all [G][words].
+ *   2. krag_redeal_begin: the plan.  KRAG_E_STATE when rows were added or removed since the last commit, or a node id
+ *      differs from its ordinal.  n_windows, n_live (over all shards) and row_bytes (payload of one row) come back.
+ *   3. krag_redeal_tables: [n_windows][G] rows and term entries this shard sends to each shard, rows it receives from each.
+ *      The host exchanges the entry tables: recv_entries[k][t] = send_entries of shard t for window k, this shard.
+ *   4. krag_redeal_prepare(recv_entries): allocates the new term arrays.  Until here nothing has changed: on any failure
+ *      krag_redeal_abort on every rank leaves every shard as it was.
+ *   5. per window k = 0 .. n_windows-1: krag_dev_redeal_pack (this shard's rows of the window into d_rows, row_bytes
+ *      each, and their entries into d_entries, 8 B each, grouped by destination shard), the exchange of both buffers
+ *      (split sizes from the tables), krag_dev_redeal_unpack (the received buffers, grouped by source shard).  Device
+ *      pointers, ordered on `stream` (cudaStream_t).
+ *   6. krag_redeal_finish: *n_rows_out = this shard's rows; then the collective commit.
+ * While a session is open every other call on the index returns KRAG_E_STATE.  After the first unpack the rows are in
+ * flight: a failure (or krag_redeal_abort) from there on leaves the index unusable and only krag_index_drop is allowed.
+ * krag_last_compact reports the session: move_ms from the first pack to the finish, postings_ms 0, rows_moved and
+ * bytes_moved = what this shard sent.  window_rows bounds the rows of one window (staging: up to window_rows rows sent and
+ * window_rows / G + 1 received per window).
+ */
+int32_t krag_redeal_begin(krag_index* idx, const uint32_t* alive_all /*[G][words] host*/, int64_t words, int64_t window_rows,
+                          int64_t* n_windows_out, int64_t* n_live_out, int64_t* row_bytes_out);
+int32_t krag_redeal_tables(krag_index* idx, int64_t* send_rows, int64_t* send_entries, int64_t* recv_rows /*[n_windows][G] each*/);
+int32_t krag_redeal_prepare(krag_index* idx, const int64_t* recv_entries /*[n_windows][G]*/);
+int32_t krag_dev_redeal_pack(krag_index* idx, int64_t window, void* d_rows, void* d_entries, void* stream);
+int32_t krag_dev_redeal_unpack(krag_index* idx, int64_t window, const void* d_rows, const void* d_entries, void* stream);
+int32_t krag_redeal_finish(krag_index* idx, void* stream, int64_t* n_rows_out);
+int32_t krag_redeal_abort(krag_index* idx);
 /*
  * (Re)build BM25 postings for the rows added so far.  replaces the per-query
  * BM25Retriever.from_defaults rebuild (hybrid_retriever.py:104-130): same scores,
@@ -310,7 +347,7 @@ int64_t krag_host_rows_fetched(void);
  * 6 = device bf16 rows of a KRAG_ROWS_HOST index), with the algorithmic bytes and
  * flops of that launch -- bench.py's roofline line is computed from it. */
 int32_t krag_last_dense_kernel(float* ms, int32_t* kernel_id, int64_t* algorithmic_bytes, int64_t* flops);
-/* Figures of the last krag_index_compact on this process: CUDA-event duration of the row-move phase (device moves and
+/* Figures of the last krag_index_compact (or redeal, see krag_redeal_begin) on this process: CUDA-event duration of the row-move phase (device moves and
  * the host-row memmoves they overlap), host-clock duration of the postings remap (0 if the index never committed),
  * live rows that changed position, and the bytes of the moved rows and term lists (each counted once). */
 int32_t krag_last_compact(float* move_ms, float* postings_ms, int64_t* rows_moved, int64_t* bytes_moved);

@@ -37,7 +37,8 @@ SYMBOLS = [
     "krag_debug_linear_ln", "krag_index_set_dense_mode", "krag_text_analyze", "krag_wordpiece_create",
     "krag_wordpiece_encode_batch", "krag_wordpiece_destroy", "krag_p2p_create", "krag_p2p_connect", "krag_dev_exchange_merge", "krag_p2p_destroy",
     "krag_host_pinned_bytes", "krag_host_rows_fetched", "krag_index_compact", "krag_last_compact",
-    "krag_last_commit",
+    "krag_last_commit", "krag_index_alive_bitmap", "krag_redeal_begin", "krag_redeal_tables", "krag_redeal_prepare",
+    "krag_dev_redeal_pack", "krag_dev_redeal_unpack", "krag_redeal_finish", "krag_redeal_abort",
 ]
 
 
@@ -94,6 +95,14 @@ def load() -> C.CDLL:
     L.krag_index_add.argtypes = [vp, i64, vp, vp, vp, vp, vp, vp]
     L.krag_index_remove.argtypes = [vp, i64, vp, C.POINTER(i64)]
     L.krag_index_compact.argtypes = [vp, C.POINTER(i64)]
+    L.krag_index_alive_bitmap.argtypes = [vp, vp, i64, C.POINTER(i64)]
+    L.krag_redeal_begin.argtypes = [vp, vp, i64, i64, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64)]
+    L.krag_redeal_tables.argtypes = [vp, vp, vp, vp]
+    L.krag_redeal_prepare.argtypes = [vp, vp]
+    L.krag_dev_redeal_pack.argtypes = [vp, i64, vp, vp, vp]
+    L.krag_dev_redeal_unpack.argtypes = [vp, i64, vp, vp, vp]
+    L.krag_redeal_finish.argtypes = [vp, vp, C.POINTER(i64)]
+    L.krag_redeal_abort.argtypes = [vp]
     L.krag_index_commit.argtypes = [vp, i64]
     L.krag_index_commit_local.argtypes = [vp, i64, vp, C.POINTER(i64), C.POINTER(i64)]
     L.krag_index_commit_global.argtypes = [vp, i64, vp, i64, i64, i64]
@@ -387,6 +396,44 @@ class Index:
         n = C.c_int64(0)
         check(self._L.krag_index_compact(self._h, C.byref(n)))
         return n.value
+
+    def alive_bitmap(self) -> np.ndarray:
+        """the alive bits of the rows (uint32 words, bits past the rows 0)"""
+        words = C.c_int64(0)
+        check(self._L.krag_index_alive_bitmap(self._h, None, 0, C.byref(words)))
+        out = np.zeros(words.value, np.uint32)
+        check(self._L.krag_index_alive_bitmap(self._h, ptr(out), out.size, C.byref(words)))
+        return out
+
+    # ---- redeal session (kaito_rag.h, krag_redeal_begin): compaction of round-robin shards together, one call per step
+    def redeal_begin(self, alive_all: np.ndarray, window_rows: int):
+        """alive_all [G, words] uint32 -> (n_windows, n_live, row_bytes, send_rows, send_entries, recv_rows), tables
+        [n_windows, G] int64"""
+        alive_all = np.ascontiguousarray(alive_all, np.uint32)
+        nw, nl, rb = C.c_int64(0), C.c_int64(0), C.c_int64(0)
+        check(self._L.krag_redeal_begin(self._h, ptr(alive_all), alive_all.shape[1], window_rows, C.byref(nw), C.byref(nl), C.byref(rb)))
+        G = alive_all.shape[0]
+        tabs = [np.zeros((nw.value, G), np.int64) for _ in range(3)]
+        check(self._L.krag_redeal_tables(self._h, *(ptr(t) for t in tabs)))
+        return (nw.value, nl.value, rb.value, *tabs)
+
+    def redeal_prepare(self, recv_entries: np.ndarray):
+        recv_entries = np.ascontiguousarray(recv_entries, np.int64)
+        check(self._L.krag_redeal_prepare(self._h, ptr(recv_entries)))
+
+    def dev_redeal_pack(self, window: int, d_rows, d_entries, stream=0):
+        check(self._L.krag_dev_redeal_pack(self._h, window, ptr(d_rows), ptr(d_entries), ptr(stream)))
+
+    def dev_redeal_unpack(self, window: int, d_rows, d_entries, stream=0):
+        check(self._L.krag_dev_redeal_unpack(self._h, window, ptr(d_rows), ptr(d_entries), ptr(stream)))
+
+    def redeal_finish(self, stream=0) -> int:
+        n = C.c_int64(0)
+        check(self._L.krag_redeal_finish(self._h, ptr(stream), C.byref(n)))
+        return n.value
+
+    def redeal_abort(self):
+        check(self._L.krag_redeal_abort(self._h))
 
     def commit(self, vocab: int):
         check(self._L.krag_index_commit(self._h, vocab))

@@ -189,7 +189,25 @@ struct krag_index {
     std::vector<float> idf;         // [vocab] and avgdl of the last commit: compaction rebuilds the postings with them
     double avgdl = 1.0;
     int64_t ord_base = 0, ord_stride = 1;   // global ordinal of local row r = ord_base + r * ord_stride
+    int64_t commit_epoch = -1;      // epoch of the last commit (a redeal needs an index unchanged since then)
+    struct RedealSession* redeal = nullptr;   // open krag_redeal_* session: every other call is refused
+    bool broken = false;            // a redeal failed after rows had moved: only krag_index_drop is allowed
+    ~krag_index();
 };
+
+// an open krag_redeal_* session: the plan and the figures krag_last_compact reports
+struct RedealSession {
+    RedealPlan plan;
+    bool prepared = false, moved = false;
+    int64_t packed = 0, unpacked = 0, bytes_moved = 0;
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    ~RedealSession()
+    {
+        if (e0) cudaEventDestroy(e0);
+        if (e1) cudaEventDestroy(e1);
+    }
+};
+krag_index::~krag_index() { delete redeal; }
 
 namespace {
 
@@ -216,6 +234,13 @@ struct SlotLease {
 const uint32_t* alive_ptr(const krag_index* ix) { return ix->has_dead ? ix->alive_d.p : nullptr; }
 OrdMap ord_map(const krag_index* ix) { return OrdMap{(uint32_t)ix->ord_base, (uint32_t)ix->ord_stride}; }
 int64_t ord_last(const krag_index* ix) { return ix->ord_base + (ix->n_rows > 0 ? (ix->n_rows - 1) * ix->ord_stride : 0); }
+
+// every call on an index except the redeal session's own and drop: refused while a session is open or after a failed one
+void require_idle(const krag_index* ix)
+{
+    KRAG_REQUIRE(!ix->broken, KRAG_E_STATE, "index is unusable: a redeal failed after rows had moved (drop it)");
+    KRAG_REQUIRE(!ix->redeal, KRAG_E_STATE, "a redeal session is open on this index");
+}
 
 void check_P(int P) { KRAG_REQUIRE(P >= 1 && P <= KRAG_MAX_POOL, KRAG_E_INVALID, "candidate pool must be in [1, 1024]"); }
 
@@ -547,6 +572,7 @@ void commit_global_impl(krag_index* ix, int64_t vocab, const uint32_t* df_global
     ix->committed = true;
     ix->has_base = true;
     ix->committed_rows = ix->n_rows;
+    ix->commit_epoch = ix->epoch;
     CommitReport rep;
     rep.total_ms = (float)(local_ms + ms_since(t0));
     rep.host_ms = (float)host_ms;
@@ -773,6 +799,7 @@ int32_t krag_index_reserve(krag_index* ix, int64_t rows, int64_t nnz)
     return guarded([&] {
         KRAG_REQUIRE(ix && rows >= 0, KRAG_E_INVALID, "bad argument");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         ensure_capacity(ix, rows, nnz > 0 ? nnz : -1, ix->ctx->admin);
     });
@@ -789,6 +816,7 @@ int32_t krag_index_add(krag_index* ix, int64_t n, const uint64_t* node_ids, cons
         const bool sparse = term_offsets != nullptr;
         KRAG_REQUIRE(!sparse || (term_ids && term_tf && doc_len), KRAG_E_INVALID, "term_ids/term_tf/doc_len required with term_offsets");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         cudaStream_t st = ix->ctx->admin;
         KRAG_REQUIRE(ix->n_rows == 0 || sparse == ix->has_sparse, KRAG_E_STATE,
@@ -865,6 +893,7 @@ int32_t krag_index_remove(krag_index* ix, int64_t n, const uint64_t* node_ids, i
     return guarded([&] {
         KRAG_REQUIRE(ix && (n == 0 || node_ids), KRAG_E_INVALID, "bad argument");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         int64_t removed = 0;
         for (int64_t i = 0; i < n; ++i) {
@@ -888,6 +917,7 @@ int32_t krag_index_compact(krag_index* ix, int64_t* n_reclaimed_out)
     return guarded([&] {
         KRAG_REQUIRE(ix, KRAG_E_INVALID, "null index");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         KRAG_REQUIRE(ix->ord_stride == 1, KRAG_E_UNSUPPORTED,
                      "compaction needs ordinal stride 1: rows of a round-robin shard cannot move down without leaving it");
@@ -910,6 +940,220 @@ int32_t krag_last_compact(float* move_ms, float* postings_ms, int64_t* rows_move
     });
 }
 
+// ------------------------------------------------------------- redeal: compaction of round-robin shards together
+int32_t krag_index_alive_bitmap(krag_index* ix, uint32_t* out, int64_t cap_words, int64_t* words_out)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(ix && words_out, KRAG_E_INVALID, "null argument");
+        std::unique_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
+        const int64_t words = (ix->n_rows + 31) / 32;
+        *words_out = words;
+        if (!out) return;
+        KRAG_REQUIRE(cap_words >= words, KRAG_E_INVALID, "bitmap buffer holds fewer words than the index has rows / 32");
+        if (words > 0) memcpy(out, ix->alive_h.data(), sizeof(uint32_t) * (size_t)words);
+    });
+}
+
+static RedealSession* open_session(krag_index* ix)
+{
+    KRAG_REQUIRE(!ix->broken, KRAG_E_STATE, "index is unusable: a redeal failed after rows had moved (drop it)");
+    KRAG_REQUIRE(ix->redeal, KRAG_E_STATE, "no redeal session is open on this index");
+    return ix->redeal;
+}
+
+static RedealRows redeal_rows(krag_index* ix)
+{
+    const bool sp = ix->has_sparse;
+    return RedealRows{ix->host_rows ? ix->Xp.d : ix->X.p, ix->Xh.p, ix->xres.p, ix->xnorm.p, sp ? ix->dlen.p : nullptr,
+                      sp ? ix->toff.p : nullptr, sp ? ix->tid.p : nullptr, sp ? ix->ttf.p : nullptr, ix->dpad};
+}
+
+int32_t krag_redeal_begin(krag_index* ix, const uint32_t* alive_all, int64_t words, int64_t window_rows, int64_t* n_windows_out,
+                          int64_t* n_live_out, int64_t* row_bytes_out)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(ix && alive_all && n_windows_out && n_live_out && row_bytes_out && words >= 0 && window_rows >= 1,
+                     KRAG_E_INVALID, "bad argument");
+        std::unique_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
+        KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
+        const int G = (int)ix->ord_stride, s = (int)ix->ord_base;
+        KRAG_REQUIRE(s < G, KRAG_E_STATE, "not a round-robin shard: the ordinal base must be below the stride");
+        KRAG_REQUIRE(words >= (ix->n_rows + 31) / 32, KRAG_E_INVALID, "the bitmaps hold fewer words than this shard has rows / 32");
+        KRAG_REQUIRE(ix->committed && ix->commit_epoch == ix->epoch, KRAG_E_STATE,
+                     "rows were added or removed since the last commit: commit before the redeal");
+        for (int64_t r = 0; r < ix->n_rows; ++r)
+            KRAG_REQUIRE(ix->node_ids[(size_t)r] == (uint64_t)(s + r * G), KRAG_E_STATE,
+                         "a node id differs from its global ordinal: the redeal renumbers node ids to the new ordinals");
+        const uint32_t* own = alive_all + (size_t)s * (size_t)words;
+        const int64_t own_words = (ix->n_rows + 31) / 32;
+        bool same = own_words == 0 || memcmp(own, ix->alive_h.data(), sizeof(uint32_t) * (size_t)own_words) == 0;
+        for (int64_t w = own_words; w < words; ++w) same = same && own[w] == 0;
+        KRAG_REQUIRE(same, KRAG_E_INVALID, "this shard's bitmap in alive_all differs from its alive rows");
+        const bool has_xh = ix->Xh.p != nullptr ||
+                            (ix->n_rows == 0 && (ix->host_rows || ix->ctx->cfg.dense_mode == KRAG_DENSE_TC_BF16));
+        auto sess = std::make_unique<RedealSession>();
+        redeal_plan(alive_all, G, s, words, ix->n_rows, ix->has_sparse ? ix->toff.p : nullptr, has_xh, ix->dpad, window_rows, sess->plan,
+                    ix->ctx->admin);
+        *n_windows_out = sess->plan.n_windows;
+        *n_live_out = sess->plan.n_live;
+        *row_bytes_out = sess->plan.row_bytes;
+        ix->redeal = sess.release();
+    });
+}
+
+int32_t krag_redeal_tables(krag_index* ix, int64_t* send_rows, int64_t* send_entries, int64_t* recv_rows)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(ix && send_rows && send_entries && recv_rows, KRAG_E_INVALID, "null argument");
+        std::unique_lock<std::shared_mutex> lk(ix->mu);
+        const RedealPlan& p = open_session(ix)->plan;
+        const size_t n = p.send_rows.size();
+        std::copy(p.send_rows.begin(), p.send_rows.end(), send_rows);
+        std::copy(p.send_ents.begin(), p.send_ents.begin() + n, send_entries);
+        std::copy(p.recv_rows.begin(), p.recv_rows.begin() + n, recv_rows);
+    });
+}
+
+int32_t krag_redeal_prepare(krag_index* ix, const int64_t* recv_entries)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(ix, KRAG_E_INVALID, "null index");
+        std::unique_lock<std::shared_mutex> lk(ix->mu);
+        RedealSession* ss = open_session(ix);
+        KRAG_REQUIRE(!ss->prepared, KRAG_E_STATE, "the redeal session is already prepared");
+        KRAG_REQUIRE(recv_entries || ss->plan.n_windows == 0, KRAG_E_INVALID, "null argument");
+        for (int64_t i = 0; i < ss->plan.n_windows * ss->plan.G; ++i)
+            KRAG_REQUIRE(recv_entries[i] >= 0 && (ix->has_sparse || recv_entries[i] == 0), KRAG_E_INVALID, "bad entry count");
+        KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
+        const bool sp = ix->has_sparse;
+        redeal_prepare(recv_entries, sp ? ix->toff.p : nullptr, sp ? ix->tid.p : nullptr, sp ? ix->ttf.p : nullptr, ss->plan,
+                       ix->ctx->admin);
+        ss->prepared = true;
+    });
+}
+
+int32_t krag_dev_redeal_pack(krag_index* ix, int64_t window, void* d_rows, void* d_entries, void* stream)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(ix && d_rows && d_entries, KRAG_E_INVALID, "null argument");
+        std::unique_lock<std::shared_mutex> lk(ix->mu);
+        RedealSession* ss = open_session(ix);
+        const RedealPlan& p = ss->plan;
+        KRAG_REQUIRE(ss->prepared && window == ss->packed && ss->packed == ss->unpacked && window < p.n_windows, KRAG_E_STATE,
+                     "windows are packed in ascending order, each after the previous one was unpacked");
+        KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
+        cudaStream_t st = (cudaStream_t)stream;
+        if (!ss->e0) {
+            KRAG_CUDA(cudaEventCreate(&ss->e0));
+            KRAG_CUDA(cudaEventCreate(&ss->e1));
+            KRAG_CUDA(cudaEventRecord(ss->e0, st));
+        }
+        redeal_pack(redeal_rows(ix), p, window, d_rows, d_entries, st);
+        const size_t a = (size_t)(window * p.G), b = (size_t)((window + 1) * p.G);
+        ss->bytes_moved += (p.seg_row[b] - p.seg_row[a]) * p.row_bytes;
+        for (size_t i = a; i < b; ++i) ss->bytes_moved += p.send_ents[i] * REDEAL_ENTRY_BYTES;
+        ++ss->packed;
+    });
+}
+
+int32_t krag_dev_redeal_unpack(krag_index* ix, int64_t window, const void* d_rows, const void* d_entries, void* stream)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(ix && d_rows && d_entries, KRAG_E_INVALID, "null argument");
+        std::unique_lock<std::shared_mutex> lk(ix->mu);
+        RedealSession* ss = open_session(ix);
+        KRAG_REQUIRE(window == ss->unpacked && ss->packed == window + 1, KRAG_E_STATE, "unpack the window that was packed last");
+        KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
+        ss->moved = true;
+        redeal_unpack(redeal_rows(ix), ss->plan, window, d_rows, d_entries, (cudaStream_t)stream);
+        ++ss->unpacked;
+    });
+}
+
+int32_t krag_redeal_finish(krag_index* ix, void* stream, int64_t* n_rows_out)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(ix && n_rows_out, KRAG_E_INVALID, "null argument");
+        std::unique_lock<std::shared_mutex> lk(ix->mu);
+        RedealSession* ss = open_session(ix);
+        RedealPlan& p = ss->plan;
+        KRAG_REQUIRE(ss->prepared && ss->unpacked == p.n_windows, KRAG_E_STATE, "windows remain to be moved");
+        KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
+        ss->moved = true;
+        cudaStream_t st = (cudaStream_t)stream, ad = ix->ctx->admin;
+        CompactReport rep;
+        if (ss->e0) {
+            KRAG_CUDA(cudaEventRecord(ss->e1, st));
+            KRAG_CUDA(cudaEventSynchronize(ss->e1));
+            KRAG_CUDA(cudaEventElapsedTime(&rep.move_ms, ss->e0, ss->e1));
+        }
+        KRAG_CUDA(cudaStreamSynchronize(st));
+        const int64_t n = p.n_new, G = p.G, s = p.s, dp = ix->dpad;
+        if (ix->has_sparse) {
+            ix->toff = std::move(p.toff_new);
+            ix->tid = std::move(p.tid_new);
+            ix->ttf = std::move(p.ttf_new);
+            ix->nnz = p.ent_base.back();
+            if (ix->nnz > 0) ix->max_term_id = std::max<uint32_t>(ix->max_term_id, (uint32_t)(ix->vocab - 1));   // every shard's terms are below the committed vocab
+        }
+        launch_max_bits(ix->xnorm.p, n, ix->xn_max.p, ad);
+        ix->node_ids.resize((size_t)n);
+        ix->id2row.clear();
+        ix->id2row.reserve((size_t)n);
+        for (int64_t j = 0; j < n; ++j) {
+            ix->node_ids[(size_t)j] = (uint64_t)(s + j * G);
+            ix->id2row[(uint64_t)(s + j * G)] = j;
+        }
+        const int64_t words = (n + 31) / 32;
+        ix->alive_h.assign((size_t)words, 0xFFFFFFFFu);
+        if (n & 31) ix->alive_h.back() = (1u << (n & 31)) - 1u;
+        if (words > 0)
+            KRAG_CUDA(cudaMemcpyAsync(ix->alive_d.p, ix->alive_h.data(), sizeof(uint32_t) * (size_t)words, cudaMemcpyHostToDevice, ad));
+        KRAG_CUDA(cudaStreamSynchronize(ad));
+        ix->n_rows = n;
+        ix->n_live = n;
+        ix->has_dead = false;
+        ix->epoch++;
+        ix->prep = CommitPrep{};
+        ix->post = Postings{};          // no base: the collective commit that follows is a full build under the same statistics
+        ix->committed = false;
+        ix->has_base = false;
+        ix->committed_rows = 0;
+        const int64_t rows1 = n > 0 ? n : 1;
+        if (ix->host_rows) ix->Xp.shrink(rows1 * dp);
+        else ix->X.shrink(rows1 * dp, ad);
+        ix->Xh.shrink(rows1 * dp, ad);
+        ix->xres.shrink(rows1, ad);
+        ix->xnorm.shrink(rows1, ad);
+        ix->alive_d.shrink(words > 0 ? words : 1, ad);
+        if (ix->has_sparse) ix->dlen.shrink(rows1, ad);
+        rep.rows_moved = p.n_send;
+        rep.bytes_moved = ss->bytes_moved;
+        rep.valid = true;
+        delete ss;
+        ix->redeal = nullptr;
+        *n_rows_out = n;
+        std::lock_guard<std::mutex> g(g_compact_mu);
+        g_compact = rep;
+    });
+}
+
+int32_t krag_redeal_abort(krag_index* ix)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(ix, KRAG_E_INVALID, "null index");
+        std::unique_lock<std::shared_mutex> lk(ix->mu);
+        KRAG_REQUIRE(ix->redeal, KRAG_E_STATE, "no redeal session is open on this index");
+        cudaSetDevice(ix->ctx->di.device);
+        cudaDeviceSynchronize();
+        if (ix->redeal->moved) ix->broken = true;
+        delete ix->redeal;
+        ix->redeal = nullptr;
+    });
+}
+
 int32_t krag_last_commit(float* total_ms, float* host_ms, int32_t* merged, int64_t* postings_written, int64_t* delta_entries)
 {
     return guarded([&] {
@@ -926,6 +1170,7 @@ int32_t krag_index_commit_local(krag_index* ix, int64_t vocab, uint32_t* df_out,
     return guarded([&] {
         KRAG_REQUIRE(ix && df_out && n_live_out && total_len_out, KRAG_E_INVALID, "null argument");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         commit_local_impl(ix, vocab, df_out, n_live_out, total_len_out);
     });
@@ -937,6 +1182,7 @@ int32_t krag_index_commit_global(krag_index* ix, int64_t vocab, const uint32_t* 
     return guarded([&] {
         KRAG_REQUIRE(ix && df_global, KRAG_E_INVALID, "null argument");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         commit_global_impl(ix, vocab, df_global, n_docs_global, total_len_global, ordinal_base);
     });
@@ -948,6 +1194,7 @@ int32_t krag_index_commit(krag_index* ix, int64_t vocab)
         KRAG_REQUIRE(ix, KRAG_E_INVALID, "null index");
         KRAG_REQUIRE(vocab >= 1 && vocab <= (int64_t)1 << 31, KRAG_E_INVALID, "vocab must be in [1, 2^31]");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         std::vector<uint32_t> df((size_t)vocab);
         int64_t live = 0, total = 0;
@@ -961,6 +1208,7 @@ int32_t krag_index_set_ordinal_map(krag_index* ix, int64_t ordinal_base, int64_t
     return guarded([&] {
         KRAG_REQUIRE(ix && ordinal_base >= 0 && ordinal_stride >= 1 && ordinal_stride <= 64, KRAG_E_INVALID, "bad argument");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         KRAG_REQUIRE(ordinal_base + ix->n_rows * ordinal_stride <= 0xFFFFFFFFll, KRAG_E_UNSUPPORTED, "global ordinal exceeds 32 bits");
         ix->ord_base = ordinal_base; ix->ord_stride = ordinal_stride;
     });
@@ -971,6 +1219,7 @@ int32_t krag_index_stats(krag_index* ix, krag_stats_t* out)
     return guarded([&] {
         KRAG_REQUIRE(ix && out, KRAG_E_INVALID, "null argument");
         std::shared_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         memset(out, 0, sizeof *out);
         out->n_rows = ix->n_rows; out->n_live = ix->n_live; out->nnz = ix->committed ? ix->post.nnz : ix->nnz;
         out->n_docs_global = ix->n_docs_global; out->total_len_global = ix->total_len_global; out->vocab = ix->vocab;
@@ -986,6 +1235,7 @@ int32_t krag_index_node_ids(krag_index* ix, int64_t n, const int64_t* ordinals, 
     return guarded([&] {
         KRAG_REQUIRE(ix && (n == 0 || (ordinals && out)), KRAG_E_INVALID, "null argument");
         std::shared_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         for (int64_t i = 0; i < n; ++i) {
             const int64_t off = ordinals[i] - ix->ord_base;
             KRAG_REQUIRE(off >= 0 && off % ix->ord_stride == 0, KRAG_E_NOT_FOUND, "ordinal is not held by this shard");
@@ -1003,6 +1253,7 @@ int32_t krag_search_dense(krag_index* ix, int32_t batch, const float* q, int32_t
         KRAG_REQUIRE(ix && q && out_l2sq && out_ord && batch >= 1, KRAG_E_INVALID, "bad argument");
         check_P(k);
         std::shared_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         SlotLease lease(ix->ctx);
         Slot* s = lease.s;
@@ -1026,6 +1277,7 @@ int32_t krag_search_bm25(krag_index* ix, int32_t batch, const uint32_t* q_terms,
         KRAG_REQUIRE(ix && q_toff && out_score && out_ord && batch >= 1, KRAG_E_INVALID, "bad argument");
         check_P(k);
         std::shared_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         SlotLease lease(ix->ctx);
         Slot* s = lease.s;
@@ -1059,6 +1311,7 @@ int32_t krag_retrieve(krag_index* ix, int32_t batch, const float* q, const uint3
         const int P = (int)((double)k * mult);
         check_P(P);
         std::shared_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         // the bitmap is read (n_rows + 31) / 32 words deep: the caller states how many it holds, so a bitmap built
         // before a concurrent krag_index_add is refused instead of over-read
         KRAG_REQUIRE(keyword_allow_bitmap == nullptr || keyword_allow_words >= (ix->n_rows + 31) / 32, KRAG_E_INVALID,
@@ -1118,6 +1371,7 @@ int32_t krag_dev_dense_candidates(krag_index* ix, int32_t batch, const float* d_
         KRAG_REQUIRE(ix && d_q && d_keys && batch >= 1, KRAG_E_INVALID, "bad argument");
         check_P(P);
         std::shared_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         SlotLease lease(ix->ctx);
         dense_candidates_dev(ix, lease.s, d_q, batch, P, d_keys, (cudaStream_t)stream);
@@ -1131,6 +1385,7 @@ int32_t krag_dev_bm25_candidates(krag_index* ix, int32_t batch, const uint32_t* 
         KRAG_REQUIRE(ix && d_toff && d_keys && batch >= 1, KRAG_E_INVALID, "bad argument");
         check_P(P);
         std::shared_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         SlotLease lease(ix->ctx);
         bm25_candidates_dev(ix, lease.s, d_terms, d_toff, h_toff ? h_toff[batch] : -1, batch, P, d_keys, (cudaStream_t)stream);
@@ -1171,6 +1426,7 @@ int32_t krag_synth_fill(krag_index* ix, int64_t n, int64_t row_base, uint64_t se
     return guarded([&] {
         KRAG_REQUIRE(ix && n >= 0, KRAG_E_INVALID, "bad argument");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         cudaStream_t st = ix->ctx->admin;
         KRAG_REQUIRE(ix->n_rows == 0, KRAG_E_STATE, "synthetic fill needs an empty index");
@@ -1204,6 +1460,7 @@ int32_t krag_index_read_rows(krag_index* ix, int64_t row0, int64_t n, float* out
     return guarded([&] {
         KRAG_REQUIRE(ix && out && row0 >= 0 && n >= 0 && row0 + n <= ix->n_rows, KRAG_E_INVALID, "row range out of bounds");
         std::shared_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         if (n == 0) return;
         if (ix->host_rows) {
@@ -1220,6 +1477,7 @@ int32_t krag_index_read_postings(krag_index* ix, uint32_t term, int64_t cap, uin
     return guarded([&] {
         KRAG_REQUIRE(ix && n_out, KRAG_E_INVALID, "null argument");
         std::shared_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         KRAG_REQUIRE(ix->committed, KRAG_E_STATE, "index not committed");
         KRAG_REQUIRE((int64_t)term < ix->post.vocab, KRAG_E_INVALID, "term id out of range");
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
@@ -1238,6 +1496,7 @@ int32_t krag_index_set_dense_mode(krag_index* ix, int32_t dense_mode, int32_t re
     return guarded([&] {
         KRAG_REQUIRE(ix && dense_mode >= KRAG_DENSE_AUTO && dense_mode <= KRAG_DENSE_TC_TF32, KRAG_E_INVALID, "bad argument");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         cudaStream_t st = ix->ctx->admin;
         if (dense_mode == KRAG_DENSE_TC_BF16 && ix->Xh.p == nullptr && ix->X.p != nullptr) {
@@ -1268,6 +1527,7 @@ int32_t krag_debug_tc_dump(krag_index* ix, int32_t nq, const float* q, float* ou
     return guarded([&] {
         KRAG_REQUIRE(ix && q && S_out && nq_pad_out && nq >= 1 && nq <= 256, KRAG_E_INVALID, "bad argument");
         std::shared_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         KRAG_REQUIRE(!ix->host_rows, KRAG_E_UNSUPPORTED, "the fp32 tensor-core dump needs device-resident rows");
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         SlotLease lease(ix->ctx);
@@ -1460,6 +1720,7 @@ int32_t krag_index_persist(krag_index* ix, const char* dir)
     return guarded([&] {
         KRAG_REQUIRE(ix && dir, KRAG_E_INVALID, "null argument");
         std::shared_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         mkdir(dir, 0755);
         std::string path = std::string(dir) + "/krag_index.bin";

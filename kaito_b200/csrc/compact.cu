@@ -114,6 +114,140 @@ void exclusive_sum(const T* in, T* out, int64_t n, cudaStream_t st)
     count_launch();
 }
 
+// ---- redeal kernels
+constexpr uint32_t REDEAL_STAY = 0xFFFFFFFFu;   // sort key of rows that do not move (dead, or below the first dead ordinal)
+
+// *first = lowest ordinal m * G + t of a zero bit over all shards' words (dead row, or padding: ordinal >= the row count)
+__global__ void first_dead_kernel(const uint32_t* __restrict__ alive, int G, int64_t words, unsigned long long* first)
+{
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < G * words; i += (int64_t)gridDim.x * blockDim.x) {
+        const uint32_t z = ~alive[i];
+        if (!z) continue;
+        const int64_t t = i / words, m = (i % words) * 32 + (__ffs(z) - 1);
+        atomicMin(first, (unsigned long long)(m * G + t));
+    }
+}
+
+// live rows among shard t's first m rows; wscan = exclusive scan of the per-word popcounts of all shards' words
+__device__ __forceinline__ int64_t live_below(const uint32_t* __restrict__ alive, const int64_t* __restrict__ wscan, int64_t words,
+                                              int64_t t, int64_t m)
+{
+    const int64_t w = m >> 5;
+    int64_t c = wscan[t * words + w] - wscan[t * words];
+    if (m & 31) c += __popc(alive[t * words + w] & ((1u << (m & 31)) - 1u));
+    return c;
+}
+
+// every live row (t, m) of every shard: its new ordinal, window and destination.  This shard's rows get their sort key and
+// rank and fill the send tables; rows bound for this shard fill the receive table.
+__global__ void redeal_rank_kernel(const uint32_t* __restrict__ alive, const int64_t* __restrict__ wscan, int G, int s, int64_t words,
+                                   int64_t first, int64_t window_rows, const int64_t* __restrict__ toff, uint32_t* __restrict__ key,
+                                   uint32_t* __restrict__ rank_out, uint32_t* __restrict__ iota, int64_t n_rows,
+                                   unsigned long long* send_rows, unsigned long long* send_ents, unsigned long long* recv_rows)
+{
+    const int64_t bits = (int64_t)G * words * 32;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < bits; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t t = i / (words * 32), m = i % (words * 32);
+        if (t == s && m < n_rows) { key[m] = REDEAL_STAY; iota[m] = (uint32_t)m; }
+        if (!((alive[t * words + (m >> 5)] >> (m & 31)) & 1u)) continue;
+        int64_t rank = 0;
+        for (int u = 0; u < G; ++u) rank += live_below(alive, wscan, words, u, u < t ? m + 1 : m);
+        if (t == s) rank_out[m] = (uint32_t)rank;
+        if (rank < first) continue;
+        const int64_t k = (rank - first) / window_rows, d = rank % G;
+        if (t == s) {
+            key[m] = (uint32_t)(k * G + d);
+            atomicAdd(send_rows + k * G + d, 1ull);
+            if (toff) atomicAdd(send_ents + k * G + d, (unsigned long long)(toff[m + 1] - toff[m]));
+        }
+        if (d == s) atomicAdd(recv_rows + k * G + t, 1ull);
+    }
+}
+
+// one warp per row of the window's send segment: payload header, scalars and rows; the term entries into ents
+__global__ void __launch_bounds__(256)
+redeal_pack_kernel(RedealRows v, const uint32_t* __restrict__ send_row, const uint32_t* __restrict__ send_key,
+                   const uint32_t* __restrict__ rank, const int64_t* __restrict__ send_ent, const int64_t* __restrict__ seg_ent, int G,
+                   int64_t p0, int64_t n, int64_t row_vecs, uint4* __restrict__ out, uint2* __restrict__ ents)
+{
+    const int lane = threadIdx.x & 31;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    const int64_t e0 = send_ent[p0];
+    for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += nwarps) {
+        const int64_t p = p0 + i;
+        const uint32_t r = send_row[p];
+        const int64_t b = v.toff ? v.toff[r] : 0, len = v.toff ? v.toff[r + 1] - b : 0;
+        uint4* o = out + i * row_vecs;
+        if (lane == 0) {
+            const int64_t in_chunk = send_ent[p] - seg_ent[send_key[p]];
+            o[0] = make_uint4(rank[r] / (uint32_t)G, (uint32_t)len, (uint32_t)in_chunk, (uint32_t)((uint64_t)in_chunk >> 32));
+            o[1] = make_uint4(v.dlen ? v.dlen[r] : 0u, __float_as_uint(v.xnorm[r]), v.xres ? __float_as_uint(v.xres[r]) : 0u, 0u);
+        }
+        const int64_t xv = v.dpad / 4, hv = v.dpad / 8;
+        const uint4* xs = reinterpret_cast<const uint4*>(v.x + (int64_t)r * v.dpad);
+        for (int64_t j = lane; j < xv; j += 32) o[2 + j] = xs[j];
+        if (v.xh) {
+            const uint4* hs = reinterpret_cast<const uint4*>(v.xh + (int64_t)r * v.dpad);
+            for (int64_t j = lane; j < hv; j += 32) o[2 + xv + j] = hs[j];
+        }
+        uint2* e = ents + (send_ent[p] - e0);
+        for (int64_t j = lane; j < len; j += 32) e[j] = make_uint2(v.tid[b + j], (uint32_t)v.ttf[b + j]);
+    }
+}
+
+// one warp per received row: scalars and rows to the destination row, its term count to lens[row - j0]
+__global__ void __launch_bounds__(256)
+redeal_unpack_rows_kernel(RedealRows v, const uint4* __restrict__ in, int64_t n, int64_t row_vecs, int64_t j0, int64_t* __restrict__ lens)
+{
+    const int lane = threadIdx.x & 31;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += nwarps) {
+        const uint4* h = in + i * row_vecs;
+        const uint4 hd = h[0];
+        const int64_t j = hd.x;
+        if (lane == 0) {
+            const uint4 sc = h[1];
+            lens[j - j0] = hd.y;
+            if (v.dlen) v.dlen[j] = sc.x;
+            v.xnorm[j] = __uint_as_float(sc.y);
+            if (v.xres) v.xres[j] = __uint_as_float(sc.z);
+        }
+        const int64_t xv = v.dpad / 4, hv = v.dpad / 8;
+        uint4* xd = reinterpret_cast<uint4*>(v.x + j * v.dpad);
+        for (int64_t c = lane; c < xv; c += 32) xd[c] = h[2 + c];
+        if (v.xh) {
+            uint4* hdst = reinterpret_cast<uint4*>(v.xh + j * v.dpad);
+            for (int64_t c = lane; c < hv; c += 32) hdst[c] = h[2 + xv + c];
+        }
+    }
+}
+
+// one warp per received row: its entries (sender t's chunk starts at ent_disp[t]) to the new term arrays at toff_new[row]
+__global__ void __launch_bounds__(256)
+redeal_unpack_terms_kernel(const uint4* __restrict__ in, int64_t n, int64_t row_vecs, const uint2* __restrict__ ents,
+                           const int64_t* __restrict__ row_disp, const int64_t* __restrict__ ent_disp, int G,
+                           const int64_t* __restrict__ toff_new, uint32_t* __restrict__ tid, uint16_t* __restrict__ ttf)
+{
+    const int lane = threadIdx.x & 31;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += nwarps) {
+        const uint4 hd = in[i * row_vecs];
+        const int64_t len = hd.y;
+        if (len == 0) continue;
+        int t = 0;
+        while (t + 1 < G && row_disp[t + 1] <= i) ++t;       // the sender: received rows are grouped by sender
+        const uint2* e = ents + ent_disp[t] + (int64_t)(((uint64_t)hd.w << 32) | hd.z);
+        const int64_t o = toff_new[hd.x];
+        for (int64_t j = lane; j < len; j += 32) {
+            const uint2 x = e[j];
+            tid[o + j] = x.x;
+            ttf[o + j] = (uint16_t)x.y;
+        }
+    }
+}
+
+int64_t ceil_rows(int64_t R, int s, int G) { return R > s ? (R - s + G - 1) / G : 0; }   // rows j of shard s with j*G+s < R
+
 }  // namespace
 
 void compact_plan(const uint32_t* alive, int64_t n_rows, const int64_t* toff, CompactPlan& plan, cudaStream_t st)
@@ -223,6 +357,181 @@ void launch_max_bits(const float* x, int64_t n, uint32_t* max_bits, cudaStream_t
     KRAG_CUDA(cudaMemsetAsync(max_bits, 0, sizeof(uint32_t), st));
     if (n == 0) return;
     max_bits_kernel<<<grid_for(n), 256, 0, st>>>(x, n, max_bits);
+    KRAG_CUDA(cudaGetLastError());
+    count_launch();
+}
+
+// ------------------------------------------------------------------------------------------------------------ redeal
+int64_t RedealPlan::j0(int64_t k) const { return ceil_rows(std::min(n_live, first + k * window_rows), s, G); }
+
+void redeal_plan(const uint32_t* h_alive, int G, int s, int64_t words, int64_t n_rows, const int64_t* toff, bool has_xh, int dpad,
+                 int64_t window_rows, RedealPlan& p, cudaStream_t st)
+{
+    p.G = G; p.s = s; p.words = words; p.n_rows = n_rows; p.window_rows = window_rows;
+    p.row_bytes = REDEAL_HEAD_BYTES + (int64_t)dpad * (int64_t)sizeof(float) + (has_xh ? (int64_t)dpad * (int64_t)sizeof(uint16_t) : 0);
+    const int64_t all_words = (int64_t)G * words;
+    DevArray<uint32_t> alive;
+    DevArray<int64_t> cnt, wscan;
+    DevArray<unsigned long long> first;
+    alive.alloc(all_words > 0 ? all_words : 1);
+    cnt.alloc(all_words + 1);
+    wscan.alloc(all_words + 1);
+    first.alloc(1);
+    if (all_words > 0) KRAG_CUDA(cudaMemcpyAsync(alive.p, h_alive, sizeof(uint32_t) * (size_t)all_words, cudaMemcpyHostToDevice, st));
+    word_popc_kernel<<<grid_for(all_words + 1), 256, 0, st>>>(alive.p, all_words, all_words * 32, cnt.p);
+    KRAG_CUDA(cudaGetLastError());
+    count_launch();
+    exclusive_sum(cnt.p, wscan.p, all_words + 1, st);
+    const unsigned long long none = (unsigned long long)(all_words * 32);
+    KRAG_CUDA(cudaMemcpyAsync(first.p, &none, sizeof none, cudaMemcpyHostToDevice, st));
+    first_dead_kernel<<<grid_for(all_words), 256, 0, st>>>(alive.p, G, words, first.p);
+    KRAG_CUDA(cudaGetLastError());
+    count_launch();
+    unsigned long long h_first = 0;
+    KRAG_CUDA(cudaMemcpyAsync(&h_first, first.p, sizeof h_first, cudaMemcpyDeviceToHost, st));
+    KRAG_CUDA(cudaMemcpyAsync(&p.n_live, wscan.p + all_words, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    KRAG_CUDA(cudaStreamSynchronize(st));
+    p.first = std::min<int64_t>((int64_t)h_first, p.n_live);
+    p.n_windows = p.n_live > p.first ? (p.n_live - p.first + window_rows - 1) / window_rows : 0;
+    p.n_new = ceil_rows(p.n_live, s, G);
+    p.j_first = ceil_rows(p.first, s, G);
+    const int64_t WG = p.n_windows * G;
+    if (WG >= (int64_t)REDEAL_STAY) throw std::invalid_argument("too many redeal windows: raise the window width");
+
+    DevArray<unsigned long long> tab;
+    tab.alloc(3 * WG + 1);
+    KRAG_CUDA(cudaMemsetAsync(tab.p, 0, sizeof(unsigned long long) * (size_t)(3 * WG + 1), st));
+    DevArray<uint32_t> key, iota;
+    const int64_t nr1 = n_rows > 0 ? n_rows : 1;
+    key.alloc(nr1);
+    iota.alloc(nr1);
+    p.rank.alloc(nr1);
+    redeal_rank_kernel<<<grid_for(all_words * 32), 256, 0, st>>>(alive.p, wscan.p, G, s, words, p.first, window_rows, toff, key.p, p.rank.p,
+                                                                 iota.p, n_rows, tab.p, tab.p + WG, tab.p + 2 * WG);
+    KRAG_CUDA(cudaGetLastError());
+    count_launch();
+    std::vector<unsigned long long> h_tab((size_t)(3 * WG));
+    if (WG > 0) KRAG_CUDA(cudaMemcpyAsync(h_tab.data(), tab.p, sizeof(unsigned long long) * (size_t)(3 * WG), cudaMemcpyDeviceToHost, st));
+    KRAG_CUDA(cudaStreamSynchronize(st));
+    p.send_rows.assign(h_tab.begin(), h_tab.begin() + WG);
+    p.send_ents.assign(h_tab.begin() + WG, h_tab.begin() + 2 * WG);
+    p.recv_rows.assign(h_tab.begin() + 2 * WG, h_tab.end());
+    p.seg_row.assign((size_t)WG + 1, 0);
+    std::vector<int64_t> seg_ent((size_t)WG + 1, 0);
+    for (int64_t i = 0; i < WG; ++i) {
+        p.seg_row[(size_t)i + 1] = p.seg_row[(size_t)i] + p.send_rows[(size_t)i];
+        seg_ent[(size_t)i + 1] = seg_ent[(size_t)i] + p.send_ents[(size_t)i];
+    }
+    p.n_send = p.seg_row[(size_t)WG];
+
+    // send order: a stable sort by (window, destination) keeps ascending rank inside each segment; the moving rows come first
+    p.send_key.alloc(nr1);
+    p.send_row.alloc(nr1);
+    if (n_rows > 0) {
+        size_t bytes = 0;
+        KRAG_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, key.p, p.send_key.p, iota.p, p.send_row.p, n_rows, 0, 32, st));
+        DevArray<unsigned char> tmp;
+        tmp.alloc(bytes ? (int64_t)bytes : 1);
+        KRAG_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, bytes, key.p, p.send_key.p, iota.p, p.send_row.p, n_rows, 0, 32, st));
+        count_launch();
+    }
+    p.send_ent.alloc(p.n_send + 1);
+    if (toff) {
+        DevArray<int64_t> len;
+        len.alloc(p.n_send + 1);
+        new_len_kernel<<<grid_for(p.n_send + 1), 256, 0, st>>>(toff, p.send_row.p, p.n_send, len.p);
+        KRAG_CUDA(cudaGetLastError());
+        count_launch();
+        exclusive_sum(len.p, p.send_ent.p, p.n_send + 1, st);
+    } else {
+        KRAG_CUDA(cudaMemsetAsync(p.send_ent.p, 0, sizeof(int64_t) * (size_t)(p.n_send + 1), st));
+    }
+    p.seg_ent.alloc(WG + 1);
+    KRAG_CUDA(cudaMemcpyAsync(p.seg_ent.p, seg_ent.data(), sizeof(int64_t) * (size_t)(WG + 1), cudaMemcpyHostToDevice, st));
+    KRAG_CUDA(cudaStreamSynchronize(st));
+    for (int64_t k = 0; k < p.n_windows; ++k) {   // each window's new ordinals of this shard arrive exactly once
+        int64_t got = 0;
+        for (int t = 0; t < G; ++t) got += p.recv_rows[(size_t)(k * G + t)];
+        if (got != p.j0(k + 1) - p.j0(k)) throw std::logic_error("redeal plan: the received rows do not cover the window");
+    }
+}
+
+void redeal_prepare(const int64_t* recv_ents, const int64_t* toff, const uint32_t* tid, const uint16_t* ttf, RedealPlan& p,
+                    cudaStream_t st)
+{
+    const int G = p.G;
+    const int64_t W = p.n_windows;
+    p.recv_ents.assign(recv_ents, recv_ents + W * G);
+    std::vector<int64_t> row_disp((size_t)(W * (G + 1))), ent_disp((size_t)(W * G));
+    p.ent_base.assign((size_t)W + 1, 0);
+    if (toff && p.j_first > 0) KRAG_CUDA(cudaMemcpyAsync(&p.ent_base[0], toff + p.j_first, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    KRAG_CUDA(cudaStreamSynchronize(st));
+    int64_t max_rows = 1;
+    for (int64_t k = 0; k < W; ++k) {
+        int64_t r = 0, e = 0;
+        for (int t = 0; t < G; ++t) {
+            row_disp[(size_t)(k * (G + 1) + t)] = r;
+            ent_disp[(size_t)(k * G + t)] = e;
+            r += p.recv_rows[(size_t)(k * G + t)];
+            e += p.recv_ents[(size_t)(k * G + t)];
+        }
+        row_disp[(size_t)(k * (G + 1) + G)] = r;
+        p.ent_base[(size_t)k + 1] = p.ent_base[(size_t)k] + e;
+        max_rows = std::max(max_rows, r);
+    }
+    const int64_t nnz = p.ent_base[(size_t)W];
+    p.recv_row_disp.alloc(W * (G + 1) + 1);
+    p.recv_ent_disp.alloc(W * G + 1);
+    p.lens.alloc(max_rows);
+    p.toff_new.alloc(p.n_new + 1);
+    p.tid_new.alloc(nnz > 0 ? nnz : 1);
+    p.ttf_new.alloc(nnz > 0 ? nnz : 1);
+    p.scan_bytes = 0;
+    KRAG_CUDA(cub::DeviceScan::ExclusiveScan(nullptr, p.scan_bytes, p.lens.p, p.toff_new.p, ::cuda::std::plus<int64_t>{}, (int64_t)0, max_rows, st));
+    p.scan_tmp.alloc(p.scan_bytes ? (int64_t)p.scan_bytes : 1);
+    if (W > 0) {
+        KRAG_CUDA(cudaMemcpyAsync(p.recv_row_disp.p, row_disp.data(), sizeof(int64_t) * row_disp.size(), cudaMemcpyHostToDevice, st));
+        KRAG_CUDA(cudaMemcpyAsync(p.recv_ent_disp.p, ent_disp.data(), sizeof(int64_t) * ent_disp.size(), cudaMemcpyHostToDevice, st));
+    }
+    // rows [0, j_first) keep their place and their term lists: copied to the new arrays as they are
+    if (toff) {
+        KRAG_CUDA(cudaMemcpyAsync(p.toff_new.p, toff, sizeof(int64_t) * (size_t)(p.j_first + 1), cudaMemcpyDeviceToDevice, st));
+        if (p.ent_base[0] > 0) {
+            KRAG_CUDA(cudaMemcpyAsync(p.tid_new.p, tid, sizeof(uint32_t) * (size_t)p.ent_base[0], cudaMemcpyDeviceToDevice, st));
+            KRAG_CUDA(cudaMemcpyAsync(p.ttf_new.p, ttf, sizeof(uint16_t) * (size_t)p.ent_base[0], cudaMemcpyDeviceToDevice, st));
+        }
+    } else {
+        KRAG_CUDA(cudaMemsetAsync(p.toff_new.p, 0, sizeof(int64_t) * (size_t)(p.j_first + 1), st));
+    }
+    KRAG_CUDA(cudaMemcpyAsync(p.toff_new.p + p.n_new, &p.ent_base[(size_t)W], sizeof(int64_t), cudaMemcpyHostToDevice, st));
+    KRAG_CUDA(cudaStreamSynchronize(st));
+}
+
+void redeal_pack(const RedealRows& v, const RedealPlan& p, int64_t k, void* rows, void* ents, cudaStream_t st)
+{
+    const int64_t p0 = p.seg_row[(size_t)(k * p.G)], n = p.seg_row[(size_t)((k + 1) * p.G)] - p0;
+    if (n == 0) return;
+    redeal_pack_kernel<<<grid_for(n * 32), 256, 0, st>>>(v, p.send_row.p, p.send_key.p, p.rank.p, p.send_ent.p, p.seg_ent.p, p.G, p0, n,
+                                                         p.row_bytes / 16, static_cast<uint4*>(rows), static_cast<uint2*>(ents));
+    KRAG_CUDA(cudaGetLastError());
+    count_launch();
+}
+
+void redeal_unpack(const RedealRows& v, RedealPlan& p, int64_t k, const void* rows, const void* ents, cudaStream_t st)
+{
+    const int64_t j0 = p.j0(k), n = p.j0(k + 1) - j0;
+    if (n == 0) return;
+    const uint4* in = static_cast<const uint4*>(rows);
+    redeal_unpack_rows_kernel<<<grid_for(n * 32), 256, 0, st>>>(v, in, n, p.row_bytes / 16, j0, p.lens.p);
+    KRAG_CUDA(cudaGetLastError());
+    count_launch();
+    if (!v.dlen) return;
+    size_t bytes = p.scan_bytes;
+    KRAG_CUDA(cub::DeviceScan::ExclusiveScan(p.scan_tmp.p, bytes, p.lens.p, p.toff_new.p + j0, ::cuda::std::plus<int64_t>{}, p.ent_base[(size_t)k], n, st));
+    count_launch();
+    redeal_unpack_terms_kernel<<<grid_for(n * 32), 256, 0, st>>>(in, n, p.row_bytes / 16, static_cast<const uint2*>(ents),
+                                                                 p.recv_row_disp.p + k * (p.G + 1), p.recv_ent_disp.p + k * p.G, p.G,
+                                                                 p.toff_new.p, p.tid_new.p, p.ttf_new.p);
     KRAG_CUDA(cudaGetLastError());
     count_launch();
 }

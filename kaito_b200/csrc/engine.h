@@ -396,6 +396,62 @@ int64_t compact_terms(uint32_t* tid, uint16_t* ttf, const int64_t* toff_old, con
 // *max_bits = bits of max x[i] over [0, n), x >= 0 (the K2 certificate's max |x|^2, as row_norms_kernel keeps it)
 void launch_max_bits(const float* x, int64_t n, uint32_t* max_bits, cudaStream_t st);
 
+// ---- redeal (compact.cu): G round-robin shards (shard s holds global ordinals s, s + G, ...) compacted together.  Live row
+// with old ordinal o gets the new ordinal rank(o) (live ordinals below o) and moves to shard rank % G, row rank / G.  Moves
+// run in windows [R0, R1) of new ordinals, ascending from the first dead ordinal; rank(o) <= o, so every row a shard reads
+// in a window or later lies at or above R0 and every row it wrote before lies below: packing a window before unpacking it
+// overwrites no row that is still to be read.  Term lists go to new arrays of their exact size.
+// Row payload: 16 B header (u32 destination row, u32 term count, i64 entry offset inside the sender's chunk for this
+// destination), 16 B scalars (u32 doc_len, f32 |x|^2, f32 xres, 0), the fp32 row [dpad], the bf16 row [dpad] if present.
+// Entry payload: 8 B (u32 term id, u32 tf).
+constexpr int64_t REDEAL_HEAD_BYTES = 32;
+constexpr int64_t REDEAL_ENTRY_BYTES = 8;
+struct RedealRows {
+    float* x;            // fp32 rows (device, or the mapped address of pinned host rows)
+    uint16_t* xh;        // bf16 rows or null
+    float* xres;         // or null
+    float* xnorm;
+    uint32_t* dlen;      // or null (no term lists)
+    const int64_t* toff; // or null
+    const uint32_t* tid;
+    const uint16_t* ttf;
+    int dpad;
+};
+struct RedealPlan {
+    int G = 1, s = 0;
+    int64_t words = 0, n_rows = 0, window_rows = 1;
+    int64_t n_live = 0;          // live rows over all shards
+    int64_t first = 0;           // first dead ordinal (new ordinals below it do not move)
+    int64_t n_windows = 0, row_bytes = 0;
+    int64_t n_send = 0;          // this shard's rows that move
+    int64_t n_new = 0, j_first = 0;   // rows of this shard afterwards; rows [0, j_first) stay where they are
+    DevArray<uint32_t> rank;     // [n_rows] new ordinal of each live local row
+    DevArray<uint32_t> send_key, send_row;   // [n_send] window * G + destination, local row: in send order
+    DevArray<int64_t> send_ent;  // [n_send + 1] entry offsets in send order
+    DevArray<int64_t> seg_ent;   // [n_windows * G + 1] send_ent at the start of each (window, destination) segment
+    std::vector<int64_t> send_rows, send_ents, recv_rows;   // [n_windows][G]
+    std::vector<int64_t> seg_row;                            // [n_windows * G + 1]
+    // receiving side (redeal_prepare)
+    std::vector<int64_t> recv_ents, ent_base;                // [n_windows][G], [n_windows + 1]
+    DevArray<int64_t> recv_row_disp, recv_ent_disp;          // [n_windows][G + 1], [n_windows][G]
+    DevArray<int64_t> lens, toff_new;                        // [max window rows], [n_new + 1]
+    DevArray<uint32_t> tid_new;
+    DevArray<uint16_t> ttf_new;
+    DevArray<unsigned char> scan_tmp;
+    size_t scan_bytes = 0;
+    int64_t j0(int64_t k) const;      // first destination row of window k on this shard
+};
+// the plan from every shard's alive bitmap (host [G][words]; bits past a shard's rows are 0), this shard's term offsets (or
+// null) and the window width; synchronises st
+void redeal_plan(const uint32_t* h_alive, int G, int s, int64_t words, int64_t n_rows, const int64_t* toff, bool has_xh, int dpad,
+                 int64_t window_rows, RedealPlan& p, cudaStream_t st);
+// the receiving side: the senders' entry counts [n_windows][G], the new term arrays (rows that stay copied over); synchronises st
+void redeal_prepare(const int64_t* recv_ents, const int64_t* toff, const uint32_t* tid, const uint16_t* ttf, RedealPlan& p,
+                    cudaStream_t st);
+// window k: this shard's rows into rows / ents (send order), and the received rows / ents into place
+void redeal_pack(const RedealRows& v, const RedealPlan& p, int64_t k, void* rows, void* ents, cudaStream_t st);
+void redeal_unpack(const RedealRows& v, RedealPlan& p, int64_t k, const void* rows, const void* ents, cudaStream_t st);
+
 // ---- K5: BERT encoder forward (embed.cu)
 struct BertConfig;
 struct Embedder;

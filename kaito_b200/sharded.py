@@ -67,6 +67,28 @@ class NativeStages:
     def commit_local(self, vocab):
         return self.index.commit_local(vocab)
 
+    # redeal: compaction of the round-robin shards together (ShardedRetriever.compact)
+    def alive_bitmap(self) -> np.ndarray:
+        return self.index.alive_bitmap()
+
+    def redeal_begin(self, alive_all: np.ndarray, window_rows: int):
+        return self.index.redeal_begin(alive_all, window_rows)
+
+    def redeal_prepare(self, recv_entries: np.ndarray):
+        self.index.redeal_prepare(recv_entries)
+
+    def redeal_pack(self, window: int, rows: torch.Tensor, entries: torch.Tensor):
+        self.index.dev_redeal_pack(window, rows.data_ptr(), entries.data_ptr(), self.stream())
+
+    def redeal_unpack(self, window: int, rows: torch.Tensor, entries: torch.Tensor):
+        self.index.dev_redeal_unpack(window, rows.data_ptr(), entries.data_ptr(), self.stream())
+
+    def redeal_finish(self) -> int:
+        return self.index.redeal_finish(self.stream())
+
+    def redeal_abort(self):
+        self.index.redeal_abort()
+
     def commit_global(self, vocab, df, n_docs, total_len, ordinal_base):
         self.index.commit_global(vocab, df, n_docs, total_len, ordinal_base)
 
@@ -134,6 +156,105 @@ class ShardedRetriever:
         self.stages.commit_global(vocab, df_t.cpu().numpy().astype(np.uint32), n_docs, total, base)
         self.hybrid = True
         return n_docs, total, base
+
+    # ------------------------------------------------------------------ compaction
+    COMPACT_WINDOW_ROWS = 1 << 15     # new ordinals per window: at 768 dims about 150 MB of send staging per rank at most
+    REDEAL_ENTRY_BYTES = 8
+
+    def compact(self, vocab: int, window_rows: int | None = None) -> tuple[int, int]:
+        """Remove the dead rows of round-robin shards (base = rank, stride = world) together, every rank in lock step: the live
+        rows are renumbered in their old order and re-dealt across the shards as a fresh service would have dealt them
+        (kaito_rag.h, krag_redeal_begin), then committed again.  The index must be unchanged since its last commit.
+        Returns (rows reclaimed over all shards, this shard's rows afterwards).  A refusal or an allocation failure on any
+        rank leaves every shard unchanged; a failure once rows have moved leaves the index unusable (drop it)."""
+        st, dev, G = self.stages, self.device, self.world
+        window_rows = window_rows or self.COMPACT_WINDOW_ROWS
+        n_rows = st.n_rows()
+        bm = st.alive_bitmap()
+        meta = torch.zeros((G, 2), dtype=torch.int64, device=dev)
+        meta[self.rank, 0], meta[self.rank, 1] = len(bm), n_rows
+        if G > 1:
+            dist.all_reduce(meta, group=self.group)
+        words, n_total = int(meta[:, 0].max().item()), int(meta[:, 1].sum().item())
+        loc = torch.zeros(max(words, 1), dtype=torch.int32, device=dev)
+        if len(bm):
+            loc[: len(bm)] = torch.from_numpy(bm.view(np.int32)).to(dev)
+        gathered = torch.empty(G * loc.numel(), dtype=torch.int32, device=dev)
+        if G > 1:
+            dist.all_gather_into_tensor(gathered, loc, group=self.group)
+        else:
+            gathered.copy_(loc)
+        alive_all = np.ascontiguousarray(gathered.cpu().numpy().view(np.uint32).reshape(G, -1)[:, :words])
+
+        plan, err = None, None
+        try:
+            plan = st.redeal_begin(alive_all, window_rows)
+        except Exception as e:
+            err = e
+        row_bytes = plan[2] if plan is not None else 0
+        flag = self._sum(torch.tensor([0 if err is None else 1, row_bytes], dtype=torch.int64, device=dev))
+        if flag[0] or flag[1] != G * row_bytes:
+            if plan is not None:
+                st.redeal_abort()
+            raise err or RuntimeError("compaction refused on another rank (or the shards disagree on the row layout); "
+                                      "every shard is unchanged")
+        n_windows, n_live, row_bytes, send_rows, send_ents, recv_rows = plan
+        if n_live == n_total:              # nothing dead: every rank sees the same bitmaps
+            st.redeal_abort()
+            return 0, n_rows
+
+        recv_ents = np.zeros((n_windows, G), np.int64)
+        if n_windows > 0:                  # recv_ents[k][t] = what shard t sends this shard in window k
+            se = torch.from_numpy(send_ents).to(dev)
+            g = torch.empty((G * n_windows, G), dtype=torch.int64, device=dev)
+            if G > 1:
+                dist.all_gather_into_tensor(g, se, group=self.group)
+            else:
+                g.copy_(se)
+            recv_ents = np.ascontiguousarray(g.view(G, n_windows, G)[:, :, self.rank].T.cpu().numpy())
+        err, bufs = None, None
+        try:
+            st.redeal_prepare(recv_ents)
+            peak = lambda tab, per: max(1, int(tab.sum(axis=1).max(initial=0)) * per)
+            bufs = [torch.empty(peak(send_rows, row_bytes), dtype=torch.uint8, device=dev),
+                    torch.empty(peak(recv_rows, row_bytes), dtype=torch.uint8, device=dev),
+                    torch.empty(peak(send_ents, self.REDEAL_ENTRY_BYTES), dtype=torch.uint8, device=dev),
+                    torch.empty(peak(recv_ents, self.REDEAL_ENTRY_BYTES), dtype=torch.uint8, device=dev)]
+        except Exception as e:
+            err = e
+        if self._sum(torch.tensor([0 if err is None else 1], dtype=torch.int64, device=dev))[0]:
+            st.redeal_abort()
+            raise err or RuntimeError("compaction failed on another rank before any row moved; every shard is unchanged")
+        s_rows, r_rows, s_ents, r_ents = bufs
+        try:
+            for k in range(n_windows):
+                st.redeal_pack(k, s_rows, s_ents)
+                self._all_to_all(r_rows, s_rows, recv_rows[k] * row_bytes, send_rows[k] * row_bytes)
+                self._all_to_all(r_ents, s_ents, recv_ents[k] * self.REDEAL_ENTRY_BYTES, send_ents[k] * self.REDEAL_ENTRY_BYTES)
+                st.redeal_unpack(k, r_rows, r_ents)
+            n_new = st.redeal_finish()
+        except Exception:
+            try:
+                st.redeal_abort()        # rows were in flight: the shard is now unusable (drop it)
+            except Exception:
+                pass
+            raise
+        del bufs, s_rows, r_rows, s_ents, r_ents
+        self.commit(vocab, n_new, ordinal_base=self.rank)
+        return n_total - n_live, n_new
+
+    def _sum(self, t: torch.Tensor) -> list[int]:
+        if self.world > 1:
+            dist.all_reduce(t, group=self.group)
+        return [int(v) for v in t.cpu().tolist()]
+
+    def _all_to_all(self, out: torch.Tensor, inp: torch.Tensor, out_splits, in_splits):
+        o, i = int(np.sum(out_splits)), int(np.sum(in_splits))
+        if self.world == 1:
+            out[:o].copy_(inp[:i])
+            return
+        dist.all_to_all_single(out[:o], inp[:i], output_split_sizes=[int(x) for x in out_splits],
+                               input_split_sizes=[int(x) for x in in_splits], group=self.group)
 
     # ------------------------------------------------------------------ query time
     def _use_p2p(self, nl: int, B: int, P: int) -> bool:

@@ -167,6 +167,10 @@ class ShardedEngine:
             if len(mine):
                 sh.stages.remove(mine.astype(np.uint64))
             return None
+        if op == "compact":
+            kw = {"window_rows": cmd["window_rows"]} if cmd.get("window_rows") else {}
+            reclaimed, sh.rows = sh.sr.compact(sh.vocab, **kw)
+            return reclaimed
         if op == "commit":
             sh.vocab = cmd["vocab"]
             sh.sr.commit(sh.vocab, sh.rows, ordinal_base=self.rank)
@@ -233,6 +237,16 @@ class ShardedIndex:
         ords = np.asarray(node_ids, np.int64)
         self.eng._run({"op": "remove", "name": self.name, "ordinals": ords})
         return len(ords)
+
+    # node ids are the global ordinals, so a compaction renumbers them with the ordinals (VectorStore follows)
+    compact_renumbers_keys = True
+
+    def compact(self, window_rows: int | None = None) -> int:
+        """remove the dead rows of every shard (ShardedRetriever.compact on every rank); the live nodes keep their order and
+        get the ordinals 0 .. n_live-1.  Returns the rows reclaimed."""
+        reclaimed = int(self.eng._run({"op": "compact", "name": self.name, "window_rows": window_rows}))
+        self.n -= reclaimed
+        return reclaimed
 
     def commit(self, vocab: int):
         self.vocab = vocab

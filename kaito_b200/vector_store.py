@@ -344,14 +344,20 @@ class VectorStore:
         """after a committed delete / update (writer lock held): compact the engine index when enough of it is dead, then
         drop the dead nodes from the host mirror and renumber the live ones as the engine did (order kept)"""
         if (st.n_dead < COMPACT_MIN_DEAD_ROWS or st.n_dead < COMPACT_DEAD_FRACTION * len(st.nodes)
-                or not hasattr(st.index, "compact")):      # the sharded engine keeps its tombstones
+                or not hasattr(st.index, "compact")):      # an engine without compaction keeps its tombstones
             return
         st.index.compact()
         live = [n for n in st.nodes if n.alive]
+        # the sharded engine's node ids are the ordinals: its compaction renumbers them too, and the next node gets n_live
+        renumber = getattr(st.index, "compact_renumbers_keys", False)
         remap = {}
         for i, n in enumerate(live):
             remap[n.ordinal] = i
             n.ordinal = i
+            if renumber:
+                n.key = i
+        if renumber:
+            st.next_key = len(live)
         st.nodes = live
         for rec in st.ref_docs.values():
             rec["nodes"] = [remap[o] for o in rec["nodes"]]
