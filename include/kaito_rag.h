@@ -287,7 +287,7 @@ int32_t krag_p2p_destroy(krag_p2p* p);
 
 /* ------------------------------------------------------------- embedding forward (K5) */
 /* replaces: LocalHuggingFaceEmbedding (embedding/huggingface_local_embedding.py:34-53) -> sentence-
- * transformers BertModel forward, CLS pooling, L2 normalisation.  Tokenisation (WordPiece) stays in
+ * transformers BertModel forward, CLS or mean pooling, L2 normalisation.  Tokenisation (WordPiece) stays in
  * the host.  Weights are loaded by their Hugging Face BertModel names ("embeddings.word_embeddings.weight",
  * "encoder.layer.0.attention.self.query.weight", ...), fp32, row-major as torch stores them. */
 typedef struct krag_embedder krag_embedder;
@@ -304,6 +304,13 @@ int32_t krag_embed(krag_embedder* e, int32_t batch, const int32_t* tok_ids, cons
  * krag_dev_dense_candidates takes); `stream` (cudaStream_t) is made to wait for the embeddings. tok_* are HOST. */
 int32_t krag_embed_dev(krag_embedder* e, int32_t batch, const int32_t* tok_ids, const int32_t* tok_offsets, float* d_out,
                        int32_t ld_out, void* stream);
+/* Pooling of the last hidden state before the L2 normalisation (sentence-transformers' Pooling module, read from the
+ * snapshot's modules.json and <pooling dir>/config.json by the host): the [CLS] row (default), or the mean over every token
+ * of the sequence, [CLS] and [SEP] included.  May be called before or after finalize and between forwards; any other
+ * mode is KRAG_E_INVALID. */
+#define KRAG_POOL_CLS 0
+#define KRAG_POOL_MEAN 1
+int32_t krag_embedder_set_pooling(krag_embedder* e, int32_t mode);
 int32_t krag_embedder_destroy(krag_embedder* e);
 
 /* ------------------------------------------------- host-side text analysis (no GPU involved; ASCII input) */

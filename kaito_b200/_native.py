@@ -23,6 +23,7 @@ FUSION_REFERENCE, FUSION_SIMILARITY = 0, 1
 FILTER_PUSHDOWN = 0x100   # OR into fusion_mode: the allow bitmap restricts the dense and BM25 scans themselves
 DENSE_AUTO, DENSE_SCAN, DENSE_TC, DENSE_TC_BF16, DENSE_TC_TF32 = 0, 1, 2, 3, 4
 ROWS_DEVICE, ROWS_HOST = 0, 1   # krag_config.row_storage: fp32 rows in HBM, or in pinned host memory with a bf16 device copy
+POOL_CLS, POOL_MEAN = 0, 1      # krag_embedder_set_pooling: the [CLS] row, or the mean over every token of the sequence
 
 # every symbol include/kaito_rag.h declares (tests check the export table against this)
 SYMBOLS = [
@@ -38,7 +39,7 @@ SYMBOLS = [
     "krag_wordpiece_encode_batch", "krag_wordpiece_destroy", "krag_p2p_create", "krag_p2p_connect", "krag_dev_exchange_merge", "krag_p2p_destroy",
     "krag_host_pinned_bytes", "krag_host_rows_fetched", "krag_index_compact", "krag_last_compact",
     "krag_last_commit", "krag_index_alive_bitmap", "krag_redeal_begin", "krag_redeal_tables", "krag_redeal_prepare",
-    "krag_dev_redeal_pack", "krag_dev_redeal_unpack", "krag_redeal_finish", "krag_redeal_abort",
+    "krag_dev_redeal_pack", "krag_dev_redeal_unpack", "krag_redeal_finish", "krag_redeal_abort", "krag_embedder_set_pooling",
 ]
 
 
@@ -126,6 +127,7 @@ def load() -> C.CDLL:
     L.krag_embedder_finalize.argtypes = [vp]
     L.krag_embed.argtypes = [vp, i32, vp, vp, vp]
     L.krag_embed_dev.argtypes = [vp, i32, vp, vp, vp, i32, vp]
+    L.krag_embedder_set_pooling.argtypes = [vp, i32]
     L.krag_embedder_destroy.argtypes = [vp]
     L.krag_debug_gemm_tf32.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp, i32, vp]
     L.krag_debug_linear_ln.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, C.c_float, vp]
@@ -328,6 +330,10 @@ class Embedder:
     def embed_dev(self, flat_tokens: np.ndarray, offsets: np.ndarray, d_out: int, ld_out: int, stream: int = 0):
         """embeddings written to device memory (row stride ld_out floats); `stream` waits for them"""
         check(self._L.krag_embed_dev(self._h, len(offsets) - 1, ptr(flat_tokens), ptr(offsets), ptr(d_out), ld_out, ptr(stream)))
+
+    def set_pooling(self, mode: int):
+        """POOL_CLS (default) or POOL_MEAN for the following forwards"""
+        check(self._L.krag_embedder_set_pooling(self._h, mode))
 
     def destroy(self):
         if self._h:

@@ -1668,6 +1668,15 @@ int32_t krag_embed_dev(krag_embedder* h, int32_t batch, const int32_t* tok_ids, 
         embedder_forward(h->e, batch, tok_ids, tok_offsets, nullptr, d_out, ld_out, (cudaStream_t)stream);
     });
 }
+static_assert(KRAG_POOL_CLS == EMB_POOL_CLS && KRAG_POOL_MEAN == EMB_POOL_MEAN, "pooling modes");
+int32_t krag_embedder_set_pooling(krag_embedder* h, int32_t mode)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(h, KRAG_E_INVALID, "null embedder");
+        KRAG_REQUIRE(mode == KRAG_POOL_CLS || mode == KRAG_POOL_MEAN, KRAG_E_INVALID, "pooling mode must be KRAG_POOL_CLS or KRAG_POOL_MEAN");
+        embedder_set_pooling(h->e, mode);
+    });
+}
 int32_t krag_embedder_destroy(krag_embedder* h)
 {
     return guarded([&] {

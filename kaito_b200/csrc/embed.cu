@@ -7,7 +7,7 @@
 //
 //   tokens (packed, variable length: no padding rows)  ->  word+position+type embeddings -> LayerNorm
 //   L x [ QKV GEMM -> attention -> O GEMM (+bias +residual) -> LayerNorm -> FFN1 GEMM (+bias, erf-GELU)
-//         -> FFN2 GEMM (+bias +residual) -> LayerNorm ]  ->  CLS row  ->  L2 normalise
+//         -> FFN2 GEMM (+bias +residual) -> LayerNorm ]  ->  CLS row or token mean (krag_embedder_set_pooling)  ->  L2 normalise
 //
 // The four GEMMs per layer (24 S d^2 of the 24 S d^2 + 4 S^2 d flops) run on fp16 wgmma over split operands (see
 // gemm_f16s_kernel) with fp32 accumulation in registers, operands staged by TMA; bias / GELU / residual are fused into
@@ -617,6 +617,73 @@ cls_normalize_kernel(const float* __restrict__ x, const int32_t* __restrict__ se
     for (int i = lane; i < d; i += 32) out[(size_t)b * ld_out + i] = row[i] / n;
 }
 
+// mean pooling + L2 normalisation (sentence-transformers Pooling(pooling_mode_mean_tokens) over every token of the
+// sequence, [CLS] and [SEP] included, then F.normalize, eps 1e-12).  One CTA per sequence; a lane owns G = d / 128 float4
+// column groups of every row, warp w sums rows w * U + k + j * MP_WARPS * U (k < U: U rows loaded before they are added).
+// The warps' partial sums meet in shared memory and are added in warp order: the bits depend on the tokens alone.
+constexpr int MP_WARPS = 8;
+template <int G>
+__global__ void __launch_bounds__(MP_WARPS * 32)
+mean_normalize_kernel(const float* __restrict__ x, const int32_t* __restrict__ seq_off, float* __restrict__ out, int ld_out)
+{
+    constexpr int D = G * 128, U = 16 / G < 4 ? 16 / G : 4;
+    __shared__ __align__(16) float part[MP_WARPS][D];
+    __shared__ float s_sq[MP_WARPS];
+    pdl_launch_dependents();
+    pdl_wait();
+    const int b = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int t0 = seq_off[b], len = seq_off[b + 1] - t0;
+    const float4* rows = reinterpret_cast<const float4*>(x + (size_t)t0 * D);
+    float4 acc[G];
+#pragma unroll
+    for (int g = 0; g < G; ++g) acc[g] = make_float4(0.f, 0.f, 0.f, 0.f);
+    auto add = [&](const float4& v, int g) { acc[g].x += v.x; acc[g].y += v.y; acc[g].z += v.z; acc[g].w += v.w; };
+    int r0 = warp * U;
+    for (; r0 + U <= len; r0 += MP_WARPS * U) {      // U whole rows: all U * G loads in flight before the adds
+        float4 v[U][G];
+#pragma unroll
+        for (int k = 0; k < U; ++k)
+#pragma unroll
+            for (int g = 0; g < G; ++g) v[k][g] = rows[(size_t)(r0 + k) * (D / 4) + lane + 32 * g];
+#pragma unroll
+        for (int k = 0; k < U; ++k)
+#pragma unroll
+            for (int g = 0; g < G; ++g) add(v[k][g], g);
+    }
+#pragma unroll
+    for (int k = 0; k < U; ++k)                      // the warp's last, partial step
+        if (r0 + k < len)
+#pragma unroll
+            for (int g = 0; g < G; ++g) add(rows[(size_t)(r0 + k) * (D / 4) + lane + 32 * g], g);
+#pragma unroll
+    for (int g = 0; g < G; ++g) reinterpret_cast<float4*>(part[warp])[lane + 32 * g] = acc[g];
+    __syncthreads();
+    // thread i: float4 column group i (D / 4 <= 256 = the block size)
+    const int c = threadIdx.x;
+    const bool on = c < D / 4;
+    float4 m = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (on) {
+#pragma unroll
+        for (int w = 0; w < MP_WARPS; ++w) {
+            const float4 p = reinterpret_cast<const float4*>(part[w])[c];
+            m.x += p.x; m.y += p.y; m.z += p.z; m.w += p.w;
+        }
+        const float fl = (float)len;
+        m.x /= fl; m.y /= fl; m.z /= fl; m.w /= fl;
+    }
+    const float sq = warp_sum((m.x * m.x + m.y * m.y) + (m.z * m.z + m.w * m.w));
+    if (lane == 0) s_sq[warp] = sq;
+    __syncthreads();
+    float s = 0.f;
+#pragma unroll
+    for (int w = 0; w < MP_WARPS; ++w) s += s_sq[w];
+    const float n = fmaxf(sqrtf(s), 1e-12f);
+    if (on) {
+        float* o = out + (size_t)b * ld_out + 4 * c;
+        o[0] = m.x / n; o[1] = m.y / n; o[2] = m.z / n; o[3] = m.w / n;
+    }
+}
+
 // ------------------------------------------------------------------------------------ host
 // launch with programmatic stream serialization (see pdl_wait in tc_ptx.cuh); only for kernels that call pdl_wait()
 template <typename... KArgs, typename... Args>
@@ -773,6 +840,7 @@ struct Embedder {
     cudaEvent_t done = nullptr, in_ev = nullptr;
     std::map<std::tuple<int, int, int>, cudaGraphExec_t> graphs;   // captured forward per (n_tok, batch, max_len)
     std::map<std::tuple<int, int, int>, int> seen;
+    int pooling = EMB_POOL_CLS;           // read by the final writer, which runs outside the captured graphs
     // workspaces, grown on demand
     int cap_tok = 0, cap_batch = 0;
     DevArray<int32_t> d_tok, d_pos, d_off;
@@ -879,6 +947,39 @@ void embedder_destroy(Embedder* e) { delete e; }
 
 int embedder_hidden(const Embedder* e) { return e->cfg.hidden; }
 
+void embedder_set_pooling(Embedder* e, int mode)
+{
+    if (mode != EMB_POOL_CLS && mode != EMB_POOL_MEAN) throw std::runtime_error("embedder: pooling mode must be CLS or MEAN");
+    e->pooling = mode;
+}
+
+template <int G>
+static void launch_mean_normalize(const float* x, const int32_t* seq_off, float* out, int batch, int ld_out, cudaStream_t st)
+{
+    mean_normalize_kernel<G><<<(unsigned)batch, MP_WARPS * 32, 0, st>>>(x, seq_off, out, ld_out);
+}
+// the final writer: pooled, L2-normalised embeddings of the residual stream x into rows of stride ld_out
+static void launch_pool(const Embedder* e, int batch, float* out, int ld_out, cudaStream_t st)
+{
+    const int d = e->cfg.hidden;
+    if (e->pooling == EMB_POOL_MEAN) {
+        switch (d / 128) {             // embedder_create: d % 128 == 0, d <= 1024
+        case 1: launch_mean_normalize<1>(e->x.p, e->d_off.p, out, batch, ld_out, st); break;
+        case 2: launch_mean_normalize<2>(e->x.p, e->d_off.p, out, batch, ld_out, st); break;
+        case 3: launch_mean_normalize<3>(e->x.p, e->d_off.p, out, batch, ld_out, st); break;
+        case 4: launch_mean_normalize<4>(e->x.p, e->d_off.p, out, batch, ld_out, st); break;
+        case 5: launch_mean_normalize<5>(e->x.p, e->d_off.p, out, batch, ld_out, st); break;
+        case 6: launch_mean_normalize<6>(e->x.p, e->d_off.p, out, batch, ld_out, st); break;
+        case 7: launch_mean_normalize<7>(e->x.p, e->d_off.p, out, batch, ld_out, st); break;
+        default: launch_mean_normalize<8>(e->x.p, e->d_off.p, out, batch, ld_out, st); break;
+        }
+    } else {
+        cls_normalize_kernel<<<(batch * 32 + 255) / 256, 256, 0, st>>>(e->x.p, e->d_off.p, out, batch, d, ld_out);
+    }
+    KRAG_CUDA(cudaGetLastError());
+    count_launch();
+}
+
 // tok_ids: packed tokens of all sequences; tok_offsets [batch+1]; out_host [batch, hidden]
 // out_host != nullptr: embeddings are copied to the host and the call returns synchronised.
 // out_dev  != nullptr: embeddings are written to device rows of stride ld_out floats and `consumer` (a stream of
@@ -975,17 +1076,13 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
         if (!e->in_ev) KRAG_CUDA(cudaEventCreateWithFlags(&e->in_ev, cudaEventDisableTiming));
         KRAG_CUDA(cudaEventRecord(e->in_ev, consumer));
         KRAG_CUDA(cudaStreamWaitEvent(st, e->in_ev, 0));
-        cls_normalize_kernel<<<(batch * 32 + 255) / 256, 256, 0, st>>>(e->x.p, e->d_off.p, out_dev, batch, d, ld_out);
-        KRAG_CUDA(cudaGetLastError());
-        count_launch();
+        launch_pool(e, batch, out_dev, ld_out, st);
         if (!e->done) KRAG_CUDA(cudaEventCreateWithFlags(&e->done, cudaEventDisableTiming));
         KRAG_CUDA(cudaEventRecord(e->done, st));
         KRAG_CUDA(cudaStreamWaitEvent(consumer, e->done, 0));
     }
     if (out_host) {
-        cls_normalize_kernel<<<(batch * 32 + 255) / 256, 256, 0, st>>>(e->x.p, e->d_off.p, e->out.p, batch, d, d);
-        KRAG_CUDA(cudaGetLastError());
-        count_launch();
+        launch_pool(e, batch, e->out.p, d, st);
         KRAG_CUDA(cudaMemcpyAsync(out_host, e->out.p, 4 * (size_t)batch * d, cudaMemcpyDeviceToHost, st));
         KRAG_CUDA(cudaStreamSynchronize(st));
     }

@@ -460,6 +460,8 @@ void embedder_load(Embedder* e, const char* name, const float* data, int64_t n);
 void embedder_finalize(Embedder* e);
 void embedder_destroy(Embedder* e);
 int embedder_hidden(const Embedder* e);
+enum { EMB_POOL_CLS = 0, EMB_POOL_MEAN = 1 };   // = KRAG_POOL_CLS / KRAG_POOL_MEAN
+void embedder_set_pooling(Embedder* e, int mode);
 void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int32_t* tok_offsets, float* out_host,
                       float* out_dev = nullptr, int ld_out = 0, cudaStream_t consumer = nullptr);
 // A fp32 matrix carried as two fp16 planes: v = hi + lo * 2^-11 (see embed.cu: split operands of the K5 GEMMs)

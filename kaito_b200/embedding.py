@@ -5,6 +5,8 @@ tests (no checkpoints are available offline) and never the default of the servic
 from __future__ import annotations
 
 import hashlib
+import json
+import os
 import re
 
 import numpy as np
@@ -53,41 +55,138 @@ class HashingEmbedding(BaseEmbeddingModel):
 
 BGE_QUERY_INSTRUCTION = "Represent this question for searching relevant passages: "
 
+_ST_MODULE = "sentence_transformers.models."
+_POOLING_FLAGS = ("pooling_mode_cls_token", "pooling_mode_mean_tokens", "pooling_mode_max_tokens",
+                  "pooling_mode_mean_sqrt_len_tokens", "pooling_mode_weightedmean_tokens", "pooling_mode_lasttoken")
+
+
+def _json(path: str, required: bool = True):
+    if not os.path.isfile(path):
+        if required:
+            raise ValueError(f"{path}: file missing")
+        return None
+    try:
+        with open(path, encoding="utf-8") as f:
+            return json.load(f)
+    except (OSError, ValueError) as e:
+        raise ValueError(f"{path}: unreadable ({e})") from None
+
+
+def read_snapshot_spec(model_dir: str) -> dict:
+    """What sentence-transformers would compute from a model snapshot, or a ValueError naming the file and field that asks for
+    something K5 does not compute.  Reads JSON only (no weights, no GPU).  Returns
+      pooling            "cls" | "mean"   (modules.json + <Pooling path>/config.json; no modules.json: "cls")
+      max_length         tokens per sequence incl. [CLS] / [SEP] (sentence_bert_config.json max_seq_length, else
+                         min(tokenizer_config.json model_max_length, config.json max_position_embeddings), else 512)
+      do_lower_case      tokenizer_config.json do_lower_case (default true)
+      query_instruction  the bge prefix for CLS-pooled snapshots, None for mean-pooled ones [3P-unverified]"""
+    join = os.path.join
+    pooling = "cls"
+    mpath = join(model_dir, "modules.json")
+    modules = _json(mpath, required=False)
+    if modules is not None:
+        types = [m.get("type", "") if isinstance(m, dict) else "" for m in modules] if isinstance(modules, list) else []
+        names = [t[len(_ST_MODULE):] if t.startswith(_ST_MODULE) else t for t in types]
+        if names[:2] != ["Transformer", "Pooling"] or names[2:] not in ([], ["Normalize"]):
+            raise ValueError(f"{mpath}: modules {types}: supported are a Transformer, then a Pooling, then an optional "
+                             "Normalize (a Dense head or any other module is not)")
+        if modules[0].get("path", "") != "":
+            raise ValueError(f"{mpath}: the Transformer's path is {modules[0]['path']!r}: the model must be at the snapshot root")
+        ppath = join(model_dir, modules[1].get("path", ""), "config.json")
+        pc = _json(ppath)
+        on = [k for k in _POOLING_FLAGS if pc.get(k)]
+        if on not in (["pooling_mode_cls_token"], ["pooling_mode_mean_tokens"]):
+            raise ValueError(f"{ppath}: pooling modes {on}: exactly one of pooling_mode_cls_token or pooling_mode_mean_tokens "
+                             "must be true (max, mean_sqrt_len, weightedmean, lasttoken and combinations are not supported)")
+        if pc.get("include_prompt", True) is not True:
+            raise ValueError(f"{ppath}: include_prompt {pc['include_prompt']!r}: only true (pool over every token) is supported")
+        pooling = "cls" if on[0] == "pooling_mode_cls_token" else "mean"
+
+    cpath = join(model_dir, "config.json")
+    cfg = _json(cpath)
+    for field, want, default in (("model_type", "bert", None), ("position_embedding_type", "absolute", "absolute"),
+                                 ("hidden_act", "gelu", "gelu"), ("is_decoder", False, False)):
+        if cfg.get(field, default) != want:
+            raise ValueError(f"{cpath}: {field} {cfg.get(field, default)!r}: K5 runs {field} {want!r} only")
+    d, heads, inter = cfg.get("hidden_size"), cfg.get("num_attention_heads"), cfg.get("intermediate_size")
+    if not all(isinstance(v, int) and v > 0 for v in (d, heads, inter)):
+        raise ValueError(f"{cpath}: hidden_size, num_attention_heads and intermediate_size must be positive integers")
+    if d % heads or d // heads not in (32, 64):
+        raise ValueError(f"{cpath}: hidden_size {d} / num_attention_heads {heads}: K5 runs attention heads of 32 or 64 dims")
+    if d % 128 or d > 1024:
+        raise ValueError(f"{cpath}: hidden_size {d}: K5 runs multiples of 128 up to 1024")
+    if inter % 128:
+        raise ValueError(f"{cpath}: intermediate_size {inter}: K5 runs multiples of 128")
+    if modules is not None and pc.get("word_embedding_dimension", d) != d:
+        raise ValueError(f"{ppath}: word_embedding_dimension {pc['word_embedding_dimension']} differs from config.json "
+                         f"hidden_size {d}")
+    max_pos = cfg.get("max_position_embeddings", 512)
+
+    tpath = join(model_dir, "tokenizer_config.json")
+    tc = _json(tpath, required=False) or {}
+    do_lower_case = tc.get("do_lower_case", True)
+    spath = join(model_dir, "sentence_bert_config.json")
+    sbc = _json(spath, required=False) or {}
+    if sbc.get("do_lower_case") and not do_lower_case:
+        raise ValueError(f"{spath}: do_lower_case true with a cased tokenizer ({tpath} do_lower_case false) is not supported")
+    if sbc.get("max_seq_length") is not None:
+        max_length, where = sbc["max_seq_length"], f"{spath}: max_seq_length"
+    else:
+        max_length, where = min(tc.get("model_max_length", max_pos), max_pos), f"{tpath}: model_max_length"
+    if not isinstance(max_length, int) or not 2 <= max_length <= max_pos:
+        raise ValueError(f"{where} {max_length!r}: must be an integer in [2, config.json max_position_embeddings {max_pos}]")
+    if not os.path.isfile(join(model_dir, "vocab.txt")):
+        raise ValueError(f"{join(model_dir, 'vocab.txt')}: file missing (K5 takes WordPiece vocabularies)")
+    return {"pooling": pooling, "max_length": max_length, "do_lower_case": bool(do_lower_case),
+            "query_instruction": BGE_QUERY_INSTRUCTION if pooling == "cls" else None}
+
 
 class GpuBertEmbedding(BaseEmbeddingModel):
-    """bge-small / bge-base / bge-large on the GPU (K5, kaito_b200/csrc/embed.cu): WordPiece on the host,
-    BERT encoder forward + CLS pooling + L2 normalisation in libkaito_rag.  Mirrors
-    LocalHuggingFaceEmbedding (embedding/huggingface_local_embedding.py:31-61); queries get the bge
-    instruction prefix LlamaIndex adds for BAAI/bge-* models [3P-unverified]."""
+    """BERT sentence embedders (bge, all-MiniLM, e5, gte, ...) on the GPU (K5, kaito_b200/csrc/embed.cu): WordPiece on the
+    host, BERT encoder forward + CLS or mean pooling + L2 normalisation in libkaito_rag.  Mirrors
+    LocalHuggingFaceEmbedding (embedding/huggingface_local_embedding.py:31-61); from_pretrained reads the pooling, casing
+    and length from the snapshot (read_snapshot_spec).  CLS-pooled snapshots' queries get the bge instruction prefix
+    LlamaIndex adds for BAAI/bge-* models [3P-unverified]."""
 
     def __init__(self, engine, tokenizer, config: dict, state_dict: dict, query_instruction: str | None = BGE_QUERY_INSTRUCTION,
-                 max_batch_tokens: int = 65536):
+                 max_batch_tokens: int = 65536, pooling: str = "cls"):
         from . import _native
+        if pooling not in ("cls", "mean"):
+            raise ValueError(f"pooling {pooling!r}: expected 'cls' or 'mean'")
         self.tokenizer, self.query_instruction, self.max_batch_tokens = tokenizer, query_instruction, max_batch_tokens
-        self.dim = config["hidden_size"]
+        self.dim, self.pooling = config["hidden_size"], pooling
         self._emb = _native.Embedder(engine, config["num_hidden_layers"], config["hidden_size"], config["num_attention_heads"],
                                      config["intermediate_size"], config["vocab_size"], config.get("max_position_embeddings", 512),
                                      config.get("type_vocab_size", 2), config.get("layer_norm_eps", 1e-12))
+        if pooling == "mean":
+            self._emb.set_pooling(_native.POOL_MEAN)
         self._emb.load_state_dict(state_dict)
         import threading
         self._mu = threading.Lock()          # one forward at a time: the embedder owns one set of activation buffers
 
     @classmethod
     def from_pretrained(cls, engine, model_dir: str, **kw):
-        """model_dir: a Hugging Face snapshot (config.json, vocab.txt, model.safetensors or pytorch_model.bin)."""
-        import json
-        import os
+        """model_dir: a Hugging Face / sentence-transformers snapshot (config.json, vocab.txt, model.safetensors or
+        pytorch_model.bin; modules.json, the Pooling config, sentence_bert_config.json and tokenizer_config.json when
+        present).  Raises ValueError before any weight is read when the snapshot asks for what K5 does not compute."""
         from .text import WordPieceTokenizer
-        cfg = json.load(open(os.path.join(model_dir, "config.json")))
-        st_path = os.path.join(model_dir, "model.safetensors")
+        spec = read_snapshot_spec(model_dir)
+        cfg = _json(os.path.join(model_dir, "config.json"))
+        st_path, bin_path = os.path.join(model_dir, "model.safetensors"), os.path.join(model_dir, "pytorch_model.bin")
         if os.path.exists(st_path):
             from safetensors.numpy import load_file
             state = load_file(st_path)
-        else:
+        elif os.path.exists(bin_path):
             import torch
-            state = {k: v.float().numpy() for k, v in torch.load(os.path.join(model_dir, "pytorch_model.bin"), map_location="cpu").items()}
+            state = {k: v.float().numpy() for k, v in torch.load(bin_path, map_location="cpu").items()}
+        else:
+            raise ValueError(f"{model_dir}: neither model.safetensors nor pytorch_model.bin")
         state = {k[5:] if k.startswith("bert.") else k: v for k, v in state.items()}
-        return cls(engine, WordPieceTokenizer.from_file(os.path.join(model_dir, "vocab.txt")), cfg, state, **kw)
+        kw.setdefault("query_instruction", spec["query_instruction"])
+        kw.setdefault("pooling", spec["pooling"])
+        tok = WordPieceTokenizer.from_file(os.path.join(model_dir, "vocab.txt"), do_lower_case=spec["do_lower_case"],
+                                           max_length=spec["max_length"])
+        return cls(engine, tok, cfg, state, **kw)
 
     def get_embedding_dimension(self) -> int:
         return self.dim

@@ -414,7 +414,7 @@ def main():
     import sys
     import uvicorn
     from . import _native
-    from .embedding import GpuBertEmbedding, HashingEmbedding
+    from .embedding import GpuBertEmbedding, HashingEmbedding, read_snapshot_spec
     # the event loop thread and the coalescer's dispatcher thread share the GIL; the dispatcher re-acquires it after every
     # engine (ctypes) call, and with the default 5 ms switch interval each re-acquisition can wait that long behind a busy loop
     sys.setswitchinterval(float(os.getenv("KRAG_GIL_SWITCH_S", "0.0002")))
@@ -424,6 +424,12 @@ def main():
     source = cfg["embedding_source"].lower()
     if source not in ("local", "remote"):
         raise SystemExit("Invalid Embedding Type Specified (Must be Local or Remote)")          # main.py:133-141
+    model_dir = resolve_model_dir(cfg["embedding_model"]) if source == "local" else None
+    if model_dir:
+        try:
+            read_snapshot_spec(model_dir)            # refuse a snapshot K5 cannot run before any GPU work starts
+        except ValueError as e:
+            raise SystemExit(f"embedding model '{cfg['embedding_model']}' is not supported by this image: {e}")
     n_gpus = int(os.getenv("KRAG_NUM_GPUS", "0")) or _gpu_count()
     ctx = _native.Context(device_id=cfg["device_id"], rank=0, world_size=max(1, n_gpus),
                           row_storage=_native.row_storage_from_env())
@@ -440,12 +446,11 @@ def main():
         workers = se.spawn_workers(n_gpus, port)
         ctl = se.init_distributed(0, n_gpus, cfg["device_id"], port)
         engine = se.ShardedEngine(se.native_stages_factory(ctx), torch.device("cuda", cfg["device_id"]), None, ctl)
-    model_dir = resolve_model_dir(cfg["embedding_model"]) if source == "local" else None
     if source == "remote":
         from .embedding import RemoteEmbeddingModel
         embed = RemoteEmbeddingModel(cfg["remote_embedding_url"], cfg["remote_embedding_access_secret"])
     elif model_dir:
-        embed = GpuBertEmbedding.from_pretrained(ctx, model_dir)             # K5: bge forward on the GPU
+        embed = GpuBertEmbedding.from_pretrained(ctx, model_dir)             # K5: BERT forward on the GPU
     elif os.getenv("KRAG_ALLOW_HASHING_EMBEDDING") == "1":
         embed = HashingEmbedding(384)                                        # functional tests only, not a language model
     else:
