@@ -311,6 +311,9 @@ int32_t krag_embed_dev(krag_embedder* e, int32_t batch, const int32_t* tok_ids, 
 #define KRAG_POOL_CLS 0
 #define KRAG_POOL_MEAN 1
 int32_t krag_embedder_set_pooling(krag_embedder* e, int32_t mode);
+/* Under CLS pooling the last layer's O projection, FFN and LayerNorms run on the [CLS] rows only (on = 1, the default).
+ * on = 0 runs them over every token; the embeddings are the same bits either way.  Test hook. */
+int32_t krag_debug_embedder_cls_rows(krag_embedder* e, int32_t on);
 int32_t krag_embedder_destroy(krag_embedder* e);
 
 /* ------------------------------------------------- host-side text analysis (no GPU involved; ASCII input) */
@@ -331,9 +334,12 @@ int32_t krag_wordpiece_destroy(krag_wordpiece* w);
 
 /* ------------------------------------------------------------------- diagnostics */
 /* C[M,N] = A[M,K] . B[N,K]^T + bias (+erf-GELU) (+residual) through K5's split-fp16 wgmma GEMM; host buffers.
- * N % 128 == 0, K % 32 == 0.  Test hook. */
+ * N % 128 == 0, K % 64 == 0.  tile_n = 0: the tiles the forward would pick; 32, 64 or 128: 128 x tile_n tiles over the
+ * whole K range.  reps > 0: the GEMM runs reps more times on the device operands and *ms_out gets the mean
+ * time of one launch (CUDA events).  Test and probe hook. */
 int32_t krag_debug_gemm_tf32(krag_ctx* ctx, int32_t M, int32_t N, int32_t K, const float* A, const float* B,
-                             const float* bias, const float* residual, int32_t gelu, float* C_out);
+                             const float* bias, const float* residual, int32_t gelu, float* C_out, int32_t tile_n,
+                             int32_t reps, float* ms_out);
 /* Y = LayerNorm(A . B^T + bias (+residual)) * gamma + beta through K5's linear-layer dispatcher (for a handful of rows:
  * 128 x 32 split-K tiles + the reduce/LayerNorm kernel).  Test hook. */
 int32_t krag_debug_linear_ln(krag_ctx* ctx, int32_t M, int32_t N, int32_t K, const float* A, const float* B,

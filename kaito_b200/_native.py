@@ -40,6 +40,7 @@ SYMBOLS = [
     "krag_host_pinned_bytes", "krag_host_rows_fetched", "krag_index_compact", "krag_last_compact",
     "krag_last_commit", "krag_index_alive_bitmap", "krag_redeal_begin", "krag_redeal_tables", "krag_redeal_prepare",
     "krag_dev_redeal_pack", "krag_dev_redeal_unpack", "krag_redeal_finish", "krag_redeal_abort", "krag_embedder_set_pooling",
+    "krag_debug_embedder_cls_rows",
 ]
 
 
@@ -128,8 +129,9 @@ def load() -> C.CDLL:
     L.krag_embed.argtypes = [vp, i32, vp, vp, vp]
     L.krag_embed_dev.argtypes = [vp, i32, vp, vp, vp, i32, vp]
     L.krag_embedder_set_pooling.argtypes = [vp, i32]
+    L.krag_debug_embedder_cls_rows.argtypes = [vp, i32]
     L.krag_embedder_destroy.argtypes = [vp]
-    L.krag_debug_gemm_tf32.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp, i32, vp]
+    L.krag_debug_gemm_tf32.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp, i32, vp, i32, i32, C.POINTER(C.c_float)]
     L.krag_debug_linear_ln.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, C.c_float, vp]
     L.krag_index_set_dense_mode.argtypes = [vp, i32, i32]
     L.krag_text_analyze.argtypes = [C.c_char_p, i64, vp, i64, C.POINTER(i64), C.POINTER(i32)]
@@ -335,21 +337,36 @@ class Embedder:
         """POOL_CLS (default) or POOL_MEAN for the following forwards"""
         check(self._L.krag_embedder_set_pooling(self._h, mode))
 
+    def debug_cls_rows(self, on: bool):
+        """test hook: False runs the last layer over every token under CLS pooling too (same embeddings)"""
+        check(self._L.krag_debug_embedder_cls_rows(self._h, 1 if on else 0))
+
     def destroy(self):
         if self._h:
             check(self._L.krag_embedder_destroy(self._h))
             self._h = None
 
 
-def debug_gemm_tf32(ctx: "Context", A, B, bias, residual=None, gelu=False) -> np.ndarray:
+def debug_gemm_tf32(ctx: "Context", A, B, bias, residual=None, gelu=False, tile_n=0) -> np.ndarray:
+    """tile_n = 0: the tiles the forward picks for this shape; 32 / 64 / 128: 128 x tile_n tiles, whole K range"""
+    return _debug_gemm(ctx, A, B, bias, residual, gelu, tile_n, 0)[0]
+
+
+def debug_gemm_time(ctx: "Context", A, B, bias, residual=None, gelu=False, tile_n=0, reps=50):
+    """(C, mean ms of one GEMM launch over `reps` launches on the device operands)"""
+    return _debug_gemm(ctx, A, B, bias, residual, gelu, tile_n, reps)
+
+
+def _debug_gemm(ctx, A, B, bias, residual, gelu, tile_n, reps):
     A = np.ascontiguousarray(A, np.float32); B = np.ascontiguousarray(B, np.float32)
     bias = np.ascontiguousarray(bias, np.float32)
     if residual is not None:
         residual = np.ascontiguousarray(residual, np.float32)
     out = np.empty((A.shape[0], B.shape[0]), np.float32)
+    ms = C.c_float(0.0)
     check(load().krag_debug_gemm_tf32(ctx._h, A.shape[0], B.shape[0], A.shape[1], ptr(A), ptr(B), ptr(bias), ptr(residual),
-                                      1 if gelu else 0, ptr(out)))
-    return out
+                                      1 if gelu else 0, ptr(out), int(tile_n), int(reps), C.byref(ms)))
+    return out, float(ms.value)
 
 
 def debug_linear_ln(ctx: "Context", A, B, bias, residual, gamma, beta, eps=1e-12) -> np.ndarray:

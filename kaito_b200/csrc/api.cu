@@ -1677,6 +1677,13 @@ int32_t krag_embedder_set_pooling(krag_embedder* h, int32_t mode)
         embedder_set_pooling(h->e, mode);
     });
 }
+int32_t krag_debug_embedder_cls_rows(krag_embedder* h, int32_t on)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(h, KRAG_E_INVALID, "null embedder");
+        embedder_set_cls_rows_only(h->e, on != 0);
+    });
+}
 int32_t krag_embedder_destroy(krag_embedder* h)
 {
     return guarded([&] {
@@ -1687,9 +1694,12 @@ int32_t krag_embedder_destroy(krag_embedder* h)
     });
 }
 static void debug_linear(krag_ctx* c, int32_t M, int32_t N, int32_t K, const float* A, const float* B, const float* bias,
-                         const float* residual, int32_t gelu, const float* ln_g, const float* ln_b, float eps, float* out)
+                         const float* residual, int32_t gelu, const float* ln_g, const float* ln_b, float eps, float* out,
+                         int32_t tile_n = 0, int32_t reps = 0, float* ms = nullptr)
 {
     KRAG_REQUIRE(c && A && B && bias && out && M >= 1 && N % 128 == 0 && K % 64 == 0, KRAG_E_INVALID, "bad argument (N % 128, K % 64)");
+    KRAG_REQUIRE((tile_n == 0 || tile_n == 32 || tile_n == 64 || tile_n == 128) && reps >= 0 && (reps == 0 || ms), KRAG_E_INVALID,
+                 "bad tile width (0, 32, 64 or 128) or repeat count");
     KRAG_CUDA(cudaSetDevice(c->di.device));
     DevArray<float> dA, dB, db, dr, dC, dY, dg, dlb, ws;
     const size_t ws_floats = (size_t)4 << 20;
@@ -1701,15 +1711,15 @@ static void debug_linear(krag_ctx* c, int32_t M, int32_t N, int32_t K, const flo
         dg.alloc(N); dlb.alloc(N); dY.alloc((int64_t)M * N);
         KRAG_CUDA(cudaMemcpy(dg.p, ln_g, 4 * (size_t)N, cudaMemcpyHostToDevice)); KRAG_CUDA(cudaMemcpy(dlb.p, ln_b, 4 * (size_t)N, cudaMemcpyHostToDevice));
     }
-    launch_linear_f32(c->di, dA.p, dB.p, M, N, K, db.p, dr.p, gelu != 0, dC.p, dg.p, dlb.p, eps, dY.p, ws.p, ws_floats, c->admin);
+    launch_linear_f32(c->di, dA.p, dB.p, M, N, K, db.p, dr.p, gelu != 0, dC.p, dg.p, dlb.p, eps, dY.p, ws.p, ws_floats, c->admin, tile_n, reps, ms);
     KRAG_CUDA(cudaStreamSynchronize(c->admin));
     KRAG_CUDA(cudaMemcpy(out, ln_g ? dY.p : dC.p, 4 * (size_t)M * N, cudaMemcpyDeviceToHost));
 }
 
 int32_t krag_debug_gemm_tf32(krag_ctx* c, int32_t M, int32_t N, int32_t K, const float* A, const float* B, const float* bias,
-                             const float* residual, int32_t gelu, float* C_out)
+                             const float* residual, int32_t gelu, float* C_out, int32_t tile_n, int32_t reps, float* ms_out)
 {
-    return guarded([&] { debug_linear(c, M, N, K, A, B, bias, residual, gelu, nullptr, nullptr, 0.f, C_out); });
+    return guarded([&] { debug_linear(c, M, N, K, A, B, bias, residual, gelu, nullptr, nullptr, 0.f, C_out, tile_n, reps, ms_out); });
 }
 
 int32_t krag_debug_linear_ln(krag_ctx* c, int32_t M, int32_t N, int32_t K, const float* A, const float* B, const float* bias,

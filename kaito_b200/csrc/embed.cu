@@ -199,34 +199,50 @@ gemm_f16s_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant
                 if (++stage == n_stages) { stage = 0; phase ^= 1; }
             }
             if (!rows_here) continue;
-            // ===== epilogue straight from the registers: acc[4j + 2h + c] is (row r_lo + 8h, column n0 + 8j + 2q + c)
+            // ===== epilogue straight from the registers: acc[4j + 2h + c] is (row r_lo + 8h, column n0 + 8j + 2q + c).
+            // The bias and residual loads of EP_J column groups are issued together before any of them is used: one at a
+            // time, each load's latency (the residual row comes from L2 or HBM) was paid in turn while the tensor cores idled.
+            constexpr int EP_J = R / 4 < 8 ? R / 4 : 8;   // column groups per batch: all of a 128 x 32 tile's 4, else 8
+            static_assert((R / 4) % EP_J == 0, "the batches cover the tile's column groups exactly");
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int row = m0 + r_lo + 8 * h;
                 if (row >= M) continue;
                 const size_t roff = (size_t)row * N;
+                if (splits > 1) {
 #pragma unroll
-                for (int j = 0; j < R / 4; ++j) {
-                    const int col = n0 + 8 * j + 2 * q;
-                    float o0 = fmaf(acc_c[4 * j + 2 * h], GH_LO_INV, acc_m[4 * j + 2 * h]);
-                    float o1 = fmaf(acc_c[4 * j + 2 * h + 1], GH_LO_INV, acc_m[4 * j + 2 * h + 1]);
-                    if (splits > 1) {
+                    for (int j = 0; j < R / 4; ++j) {
+                        const int col = n0 + 8 * j + 2 * q;
+                        const float o0 = fmaf(acc_c[4 * j + 2 * h], GH_LO_INV, acc_m[4 * j + 2 * h]);
+                        const float o1 = fmaf(acc_c[4 * j + 2 * h + 1], GH_LO_INV, acc_m[4 * j + 2 * h + 1]);
                         *reinterpret_cast<float2*>(ws + (size_t)split * M * N + roff + col) = make_float2(o0, o1);
-                        continue;
                     }
-                    const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + col));
-                    o0 += b2.x; o1 += b2.y;
-                    if (act_gelu) { o0 = gelu_erf(o0); o1 = gelu_erf(o1); }
-                    if (residual) {
-                        const float2 r2 = *reinterpret_cast<const float2*>(residual + roff + col);
-                        o0 += r2.x; o1 += r2.y;
+                    continue;
+                }
+#pragma unroll
+                for (int j0 = 0; j0 < R / 4; j0 += EP_J) {
+                    float2 b2[EP_J], r2[EP_J];
+#pragma unroll
+                    for (int u = 0; u < EP_J; ++u) {
+                        const int col = n0 + 8 * (j0 + u) + 2 * q;
+                        b2[u] = __ldg(reinterpret_cast<const float2*>(bias + col));
+                        r2[u] = residual ? *reinterpret_cast<const float2*>(residual + roff + col) : make_float2(0.f, 0.f);
                     }
-                    if (out.c) *reinterpret_cast<float2*>(out.c + roff + col) = make_float2(o0, o1);
-                    if (out.hi) {
-                        uint16_t h0, l0, h1, l1;
-                        split_f16(o0, h0, l0); split_f16(o1, h1, l1);
-                        *reinterpret_cast<uint32_t*>(out.hi + roff + col) = (uint32_t)h0 | ((uint32_t)h1 << 16);
-                        *reinterpret_cast<uint32_t*>(out.lo + roff + col) = (uint32_t)l0 | ((uint32_t)l1 << 16);
+#pragma unroll
+                    for (int u = 0; u < EP_J; ++u) {
+                        const int j = j0 + u, col = n0 + 8 * j + 2 * q;
+                        float o0 = fmaf(acc_c[4 * j + 2 * h], GH_LO_INV, acc_m[4 * j + 2 * h]);
+                        float o1 = fmaf(acc_c[4 * j + 2 * h + 1], GH_LO_INV, acc_m[4 * j + 2 * h + 1]);
+                        o0 += b2[u].x; o1 += b2[u].y;
+                        if (act_gelu) { o0 = gelu_erf(o0); o1 = gelu_erf(o1); }
+                        if (residual) { o0 += r2[u].x; o1 += r2[u].y; }
+                        if (out.c) *reinterpret_cast<float2*>(out.c + roff + col) = make_float2(o0, o1);
+                        if (out.hi) {
+                            uint16_t h0, l0, h1, l1;
+                            split_f16(o0, h0, l0); split_f16(o1, h1, l1);
+                            *reinterpret_cast<uint32_t*>(out.hi + roff + col) = (uint32_t)h0 | ((uint32_t)h1 << 16);
+                            *reinterpret_cast<uint32_t*>(out.lo + roff + col) = (uint32_t)l0 | ((uint32_t)l1 << 16);
+                        }
                     }
                 }
             }
@@ -601,7 +617,27 @@ attention_mma_kernel(const uint16_t* __restrict__ qkv_hi, const uint16_t* __rest
     }
 }
 
-// CLS pooling + L2 normalisation (F.normalize, eps 1e-12): one warp per sequence
+// the [CLS] rows of the residual stream x and of the attention context planes into row b of compact buffers: one warp per
+// sequence, d % 128 == 0
+__global__ void __launch_bounds__(256)
+gather_cls_kernel(const float* __restrict__ x, const uint16_t* __restrict__ c_hi, const uint16_t* __restrict__ c_lo,
+                  const int32_t* __restrict__ seq_off, float* __restrict__ gx, uint16_t* __restrict__ g_hi, uint16_t* __restrict__ g_lo,
+                  int batch, int d)
+{
+    pdl_launch_dependents();
+    pdl_wait();
+    const int b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (b >= batch) return;
+    const size_t src = (size_t)seq_off[b] * d, dst = (size_t)b * d;
+    for (int i = 4 * lane; i < d; i += 128) *reinterpret_cast<float4*>(gx + dst + i) = *reinterpret_cast<const float4*>(x + src + i);
+    for (int i = 8 * lane; i < d; i += 256) {
+        *reinterpret_cast<uint4*>(g_hi + dst + i) = *reinterpret_cast<const uint4*>(c_hi + src + i);
+        *reinterpret_cast<uint4*>(g_lo + dst + i) = *reinterpret_cast<const uint4*>(c_lo + src + i);
+    }
+}
+
+// CLS pooling + L2 normalisation (F.normalize, eps 1e-12): one warp per sequence.  seq_off null: x holds the [CLS] rows
+// only, row b for sequence b.
 __global__ void __launch_bounds__(256)
 cls_normalize_kernel(const float* __restrict__ x, const int32_t* __restrict__ seq_off, float* __restrict__ out, int batch, int d,
                      int ld_out)
@@ -610,7 +646,7 @@ cls_normalize_kernel(const float* __restrict__ x, const int32_t* __restrict__ se
     pdl_wait();
     const int b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (b >= batch) return;
-    const float* row = x + (size_t)seq_off[b] * d;
+    const float* row = x + (size_t)(seq_off ? seq_off[b] : b) * d;
     float s = 0.f;
     for (int i = lane; i < d; i += 32) s = fmaf(row[i], row[i], s);
     const float n = fmaxf(sqrtf(warp_sum(s)), 1e-12f);
@@ -702,7 +738,7 @@ static void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
 
 template <int DH, int WARPS, int KB, int STAGES>
 static void launch_attention_mma(const uint16_t* q_hi, const uint16_t* q_lo, const int32_t* seq_off, uint16_t* out_hi, uint16_t* out_lo, int d,
-                                 int heads, int batch, int max_len, cudaStream_t st)
+                                 int heads, int batch, int max_len, bool first_rows, cudaStream_t st)
 {
     using Cfg = AmCfg<DH, WARPS, KB, STAGES>;
     static bool attr_set = false;
@@ -710,17 +746,20 @@ static void launch_attention_mma(const uint16_t* q_hi, const uint16_t* q_lo, con
         KRAG_CUDA(cudaFuncSetAttribute(attention_mma_kernel<DH, WARPS, KB, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM));
         attr_set = true;
     }
-    launch_pdl(attention_mma_kernel<DH, WARPS, KB, STAGES>, dim3((unsigned)((max_len + 16 * WARPS - 1) / (16 * WARPS)), (unsigned)heads, (unsigned)batch),
+    const unsigned q_blocks = first_rows ? 1u : (unsigned)((max_len + 16 * WARPS - 1) / (16 * WARPS));
+    launch_pdl(attention_mma_kernel<DH, WARPS, KB, STAGES>, dim3(q_blocks, (unsigned)heads, (unsigned)batch),
                dim3(WARPS * 32), Cfg::SMEM, st, q_hi, q_lo, seq_off, out_hi, out_lo, d, heads);
 }
-// queries (<= 32 tokens): 2 warps, one key block; <= 64: 4 warps, one block; chunks: 4 warps, 64-key blocks, double-buffered
+// queries (<= 32 tokens): 2 warps, one key block; <= 64: 4 warps, one block; chunks: 4 warps, 64-key blocks, double-buffered.
+// first_rows: only the first block of query rows of every sequence (the [CLS] row among them); a query row's result does
+// not depend on which other rows run, and the key blocking follows max_len either way
 template <int DH>
 static void attention_mma(const uint16_t* q_hi, const uint16_t* q_lo, const int32_t* seq_off, uint16_t* out_hi, uint16_t* out_lo, int d, int heads,
-                          int batch, int max_len, cudaStream_t st)
+                          int batch, int max_len, bool first_rows, cudaStream_t st)
 {
-    if (max_len <= 32) launch_attention_mma<DH, 2, 32, 1>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, st);
-    else if (max_len <= 64) launch_attention_mma<DH, 4, 64, 1>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, st);
-    else launch_attention_mma<DH, 4, 64, 2>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, st);
+    if (max_len <= 32) launch_attention_mma<DH, 2, 32, 1>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, st);
+    else if (max_len <= 64) launch_attention_mma<DH, 4, 64, 1>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, st);
+    else launch_attention_mma<DH, 4, 64, 2>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, st);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -772,16 +811,13 @@ static void launch_gemm(const DeviceInfo& di, const SplitMat& A, const SplitMat&
                K / GH_KB / splits, n_stages, m_tiles == 1 ? 1 : 0, bias, residual, gelu ? 1 : 0, out, ws);
 }
 
-// Linear layer on split operands: C = A . B^T + bias (+GELU) (+residual) -> fp32 C and / or split planes of C; with ln_g the
-// row LayerNorm of that goes to Y (fp32) and its split planes (C is then scratch).
-void launch_linear(const DeviceInfo& di, const SplitMat& A, const SplitMat& B, int M, int N, int K, const float* bias, const float* residual,
-                   bool gelu, float* C, uint16_t* C_hi, uint16_t* C_lo, const float* ln_g, const float* ln_b, float eps, float* Y,
-                   uint16_t* Y_hi, uint16_t* Y_lo, float* ws, size_t ws_floats, cudaStream_t st)
+// Tile width and K split of a linear layer of M rows.  Every output element is summed in an order fixed by (bn, splits)
+// alone, so a plan made for M rows computes the same bits on any subset of those rows.
+GemmPlan linear_plan(const DeviceInfo& di, int M, int N, int K, bool ln, bool have_ws, size_t ws_floats)
 {
-    if (ln_g && N > 32 * LN_MAX_GROUPS * 8) throw std::runtime_error("launch_linear: fused LayerNorm rows hold at most 1024 elements");
     const int m_tiles = (M + GM_TILE - 1) / GM_TILE;
     const int tiles128 = m_tiles * (N / GM_TILE);
-    if (ws && tiles128 < di.sm_count / 2 && N % 64 == 0 && K % GH_KB == 0 && (!ln_g || N <= 1024)) {
+    if (have_ws && tiles128 < di.sm_count / 2 && N % 64 == 0 && K % GH_KB == 0 && (!ln || N <= 1024)) {
         // long-K layers over several activation tiles (FFN2 for tens of queries): 128 x 128 tiles halve the operand
         // re-reads through L2 (the binding resource); split-K restores the CTA count
         const int BN = m_tiles == 1 ? 32 : ((K >= 2048 && N % 128 == 0) ? 128 : 64);
@@ -792,14 +828,30 @@ void launch_linear(const DeviceInfo& di, const SplitMat& A, const SplitMat& B, i
             for (int sp = want; sp >= 2; --sp)
                 if (kblocks % sp == 0 && kblocks / sp >= 2 && (size_t)sp * M * N <= ws_floats) { splits = sp; break; }
         }
+        return GemmPlan{BN, splits, true};
+    }
+    return GemmPlan{128, 1, false};
+}
+
+// Linear layer on split operands: C = A . B^T + bias (+GELU) (+residual) -> fp32 C and / or split planes of C; with ln_g the
+// row LayerNorm of that goes to Y (fp32) and its split planes (C is then scratch).  plan: null = linear_plan(M, ...).
+void launch_linear(const DeviceInfo& di, const SplitMat& A, const SplitMat& B, int M, int N, int K, const float* bias, const float* residual,
+                   bool gelu, float* C, uint16_t* C_hi, uint16_t* C_lo, const float* ln_g, const float* ln_b, float eps, float* Y,
+                   uint16_t* Y_hi, uint16_t* Y_lo, float* ws, size_t ws_floats, cudaStream_t st, const GemmPlan* plan)
+{
+    if (ln_g && N > 32 * LN_MAX_GROUPS * 8) throw std::runtime_error("launch_linear: fused LayerNorm rows hold at most 1024 elements");
+    const GemmPlan p = plan ? *plan : linear_plan(di, M, N, K, ln_g != nullptr, ws != nullptr, ws_floats);
+    if (N % p.bn || K % GH_KB || (K / GH_KB) % p.splits || (p.splits > 1 && (!ws || (size_t)p.splits * M * N > ws_floats)))
+        throw std::runtime_error("launch_linear: plan does not fit the problem");
+    if (p.small_m) {
         // splits == 1 and a LayerNorm to follow: the GEMM writes fp32 C (scratch), the LayerNorm kernel writes Y + planes
         const GemmOut direct = ln_g ? GemmOut{C, nullptr, nullptr} : GemmOut{C, C_hi, C_lo};
-        if (BN == 32) launch_gemm<32>(di, A, B, M, N, K, splits, bias, residual, gelu, direct, ws, st);
-        else if (BN == 128) launch_gemm<128>(di, A, B, M, N, K, splits, bias, residual, gelu, direct, ws, st);
-        else launch_gemm<64>(di, A, B, M, N, K, splits, bias, residual, gelu, direct, ws, st);
-        if (splits > 1) {
-            launch_pdl(splitk_reduce_kernel, dim3((unsigned)M), dim3(256), 0, st, ws, splits, M, N, bias, residual, gelu ? 1 : 0, ln_g, ln_b, eps,
-                       ln_g ? Y : C, ln_g ? Y_hi : C_hi, ln_g ? Y_lo : C_lo);
+        if (p.bn == 32) launch_gemm<32>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
+        else if (p.bn == 128) launch_gemm<128>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
+        else launch_gemm<64>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
+        if (p.splits > 1) {
+            launch_pdl(splitk_reduce_kernel, dim3((unsigned)M), dim3(256), 0, st, ws, p.splits, M, N, bias, residual, gelu ? 1 : 0, ln_g, ln_b,
+                       eps, ln_g ? Y : C, ln_g ? Y_hi : C_hi, ln_g ? Y_lo : C_lo);
             return;
         }
     } else {
@@ -814,15 +866,36 @@ void launch_linear(const DeviceInfo& di, const SplitMat& A, const SplitMat& B, i
 // test hook (krag_debug_gemm_tf32 / krag_debug_linear_ln): fp32 device operands are split here, then take the product path
 void launch_linear_f32(const DeviceInfo& di, const float* A, const float* B, int M, int N, int K, const float* bias, const float* residual,
                        bool gelu, float* C, const float* ln_g, const float* ln_b, float eps, float* Y, float* ws, size_t ws_floats,
-                       cudaStream_t st)
+                       cudaStream_t st, int tile_n, int reps, float* ms)
 {
+    if (tile_n != 0 && tile_n != 32 && tile_n != 64 && tile_n != 128)
+        throw std::runtime_error("launch_linear_f32: tile width must be 0, 32, 64 or 128");
+    const GemmPlan forced{tile_n, 1, true};
+    const GemmPlan* plan = tile_n ? &forced : nullptr;
     const size_t na = (size_t)M * K, nb = (size_t)N * K;
     DevArray<uint16_t> planes;
     planes.alloc((int64_t)(2 * na + 2 * nb));
     SplitMat As{planes.p, planes.p + na}, Bs{planes.p + 2 * na, planes.p + 2 * na + nb};
     launch_split_f16(A, As.hi, As.lo, (int64_t)na, st);
     launch_split_f16(B, Bs.hi, Bs.lo, (int64_t)nb, st);
-    launch_linear(di, As, Bs, M, N, K, bias, residual, gelu, C, nullptr, nullptr, ln_g, ln_b, eps, Y, nullptr, nullptr, ws, ws_floats, st);
+    auto run = [&] {
+        launch_linear(di, As, Bs, M, N, K, bias, residual, gelu, C, nullptr, nullptr, ln_g, ln_b, eps, Y, nullptr, nullptr, ws, ws_floats, st, plan);
+    };
+    run();
+    if (reps > 0) {
+        // C = A.B^T + bias (+residual) does not read C: repeating the launch leaves the result as it was
+        cudaEvent_t e0, e1;
+        KRAG_CUDA(cudaEventCreate(&e0));
+        KRAG_CUDA(cudaEventCreate(&e1));
+        KRAG_CUDA(cudaEventRecord(e0, st));
+        for (int r = 0; r < reps; ++r) run();
+        KRAG_CUDA(cudaEventRecord(e1, st));
+        KRAG_CUDA(cudaEventSynchronize(e1));
+        float t = 0.f;
+        KRAG_CUDA(cudaEventElapsedTime(&t, e0, e1));
+        cudaEventDestroy(e0); cudaEventDestroy(e1);
+        if (ms) *ms = t / (float)reps;
+    }
     KRAG_CUDA(cudaStreamSynchronize(st));
 }
 
@@ -838,9 +911,10 @@ struct Embedder {
     bool finalized = false;
     cudaStream_t st = nullptr;
     cudaEvent_t done = nullptr, in_ev = nullptr;
-    std::map<std::tuple<int, int, int>, cudaGraphExec_t> graphs;   // captured forward per (n_tok, batch, max_len)
-    std::map<std::tuple<int, int, int>, int> seen;
+    std::map<std::tuple<int, int, int, int>, cudaGraphExec_t> graphs;   // captured forward per (n_tok, batch, max_len, cls_rows)
+    std::map<std::tuple<int, int, int, int>, int> seen;
     int pooling = EMB_POOL_CLS;           // read by the final writer, which runs outside the captured graphs
+    bool cls_rows_only = true;            // CLS pooling: the last layer after QKV + attention runs on the [CLS] rows only
     // workspaces, grown on demand
     int cap_tok = 0, cap_batch = 0;
     DevArray<int32_t> d_tok, d_pos, d_off;
@@ -848,6 +922,10 @@ struct Embedder {
     DevArray<uint16_t> xs, cs, fs;        // split planes [2][T][*] of x (LayerNorm outputs), attention context, FFN1 output
     DevArray<uint16_t> qkv;               // split planes [2][n_tok][3d] of the QKV projection (the lo plane starts at n_tok rows)
     DevArray<float> ws;                   // split-K partials (small token counts)
+    // the last layer on the [CLS] rows only: residual stream, GEMM scratch, split planes of the attention context, of the
+    // LayerNorm output and of FFN1's output, [cap_batch] rows each
+    DevArray<float> cx, cx2;
+    DevArray<uint16_t> ccs, cxs, cfs;
     static constexpr size_t WS_FLOATS = (size_t)4 << 20;
 
     void drop_graphs()
@@ -953,13 +1031,16 @@ void embedder_set_pooling(Embedder* e, int mode)
     e->pooling = mode;
 }
 
+void embedder_set_cls_rows_only(Embedder* e, bool on) { e->cls_rows_only = on; }
+
 template <int G>
 static void launch_mean_normalize(const float* x, const int32_t* seq_off, float* out, int batch, int ld_out, cudaStream_t st)
 {
     mean_normalize_kernel<G><<<(unsigned)batch, MP_WARPS * 32, 0, st>>>(x, seq_off, out, ld_out);
 }
-// the final writer: pooled, L2-normalised embeddings of the residual stream x into rows of stride ld_out
-static void launch_pool(const Embedder* e, int batch, float* out, int ld_out, cudaStream_t st)
+// the final writer: pooled, L2-normalised embeddings of the residual stream x (cls_rows: of the [CLS] rows in cx) into rows
+// of stride ld_out
+static void launch_pool(const Embedder* e, int batch, bool cls_rows, float* out, int ld_out, cudaStream_t st)
 {
     const int d = e->cfg.hidden;
     if (e->pooling == EMB_POOL_MEAN) {
@@ -974,7 +1055,8 @@ static void launch_pool(const Embedder* e, int batch, float* out, int ld_out, cu
         default: launch_mean_normalize<8>(e->x.p, e->d_off.p, out, batch, ld_out, st); break;
         }
     } else {
-        cls_normalize_kernel<<<(batch * 32 + 255) / 256, 256, 0, st>>>(e->x.p, e->d_off.p, out, batch, d, ld_out);
+        cls_normalize_kernel<<<(batch * 32 + 255) / 256, 256, 0, st>>>(cls_rows ? e->cx.p : e->x.p, cls_rows ? nullptr : e->d_off.p, out, batch,
+                                                                        d, ld_out);
     }
     KRAG_CUDA(cudaGetLastError());
     count_launch();
@@ -1008,10 +1090,12 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
         e->cap_tok = e->cap_batch = 0;
         e->d_tok.release(); e->d_pos.release(); e->d_off.release(); e->x.release(); e->x2.release(); e->qkv.release();
         e->xs.release(); e->cs.release(); e->fs.release(); e->out.release();
+        e->cx.release(); e->cx2.release(); e->ccs.release(); e->cxs.release(); e->cfs.release();
         e->d_tok.alloc(T); e->d_pos.alloc(T); e->d_off.alloc(Bc + 1);
         e->x.alloc(T * d); e->x2.alloc(T * d); e->qkv.alloc(2 * T * 3 * d);
         e->xs.alloc(2 * T * d); e->cs.alloc(2 * T * d); e->fs.alloc(2 * T * c.inter);
         e->out.alloc(Bc * d);
+        e->cx.alloc(Bc * d); e->cx2.alloc(Bc * d); e->ccs.alloc(2 * Bc * d); e->cxs.alloc(2 * Bc * d); e->cfs.alloc(2 * Bc * c.inter);
         e->cap_tok = (int)T; e->cap_batch = (int)Bc;
     }
     // split planes: [hi plane | lo plane], each cap_tok rows
@@ -1021,8 +1105,13 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
     KRAG_CUDA(cudaMemcpyAsync(e->d_pos.p, pos.data(), 4 * (size_t)n_tok, cudaMemcpyHostToDevice, st));
     KRAG_CUDA(cudaMemcpyAsync(e->d_off.p, tok_offsets, 4 * (size_t)(batch + 1), cudaMemcpyHostToDevice, st));
 
+    // CLS pooling reads one row per sequence of the last layer's output.  K and V of every token are still needed, so the
+    // last QKV projection runs over all tokens; attention then runs for the first query rows only, and the O projection,
+    // FFN and LayerNorms run on the gathered [CLS] rows.  Those GEMMs keep the plan (tile width, K split) of the full
+    // token count, so every [CLS] row gets the same bits as in the full layer.  Taken when it saves a 128-row tile.
+    const bool cls_rows = e->pooling == EMB_POOL_CLS && e->cls_rows_only && (n_tok + GM_TILE - 1) / GM_TILE > (batch + GM_TILE - 1) / GM_TILE;
     // The forward is ~7 kernels per layer; for a handful of query tokens it is bound by launch gaps and kernel
-    // prologues, so each (n_tok, batch, max_len) shape is captured into a CUDA graph the second time it is seen.
+    // prologues, so each (n_tok, batch, max_len, cls_rows) shape is captured into a CUDA graph the second time it is seen.
     auto run_layers = [&]() {
     launch_pdl(embed_ln_kernel, dim3((unsigned)((n_tok + 7) / 8)), dim3(256), (size_t)8 * d * 4, st, e->d_tok.p, e->d_pos.p,
                e->t["embeddings.word_embeddings.weight"].p, e->t["embeddings.position_embeddings.weight"].p,
@@ -1034,10 +1123,29 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
     uint16_t* q_lo = q_hi + (size_t)n_tok * 3 * d;
     for (int l = 0; l < c.layers; ++l) {
         const size_t L = (size_t)l;
+        const bool last_cls = cls_rows && l == c.layers - 1;
         launch_linear(e->di, xs, e->s_qkv[L], n_tok, 3 * d, d, e->bqkv[L].p, nullptr, false, nullptr, q_hi, q_lo, nullptr, nullptr, 0.f,
                       nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st);
-        if (dh == 64) attention_mma<64>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, st);
-        else attention_mma<32>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, st);
+        if (dh == 64) attention_mma<64>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, st);
+        else attention_mma<32>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, st);
+        if (last_cls) {
+            const SplitMat ccs{e->ccs.p, e->ccs.p + (size_t)batch * d}, cxs{e->cxs.p, e->cxs.p + (size_t)batch * d},
+                           cfs{e->cfs.p, e->cfs.p + (size_t)batch * c.inter};
+            const GemmPlan po = linear_plan(e->di, n_tok, d, d, true, true, Embedder::WS_FLOATS);
+            const GemmPlan p1 = linear_plan(e->di, n_tok, c.inter, d, false, true, Embedder::WS_FLOATS);
+            const GemmPlan p2 = linear_plan(e->di, n_tok, d, c.inter, true, true, Embedder::WS_FLOATS);
+            launch_pdl(gather_cls_kernel, dim3((unsigned)((batch * 32 + 255) / 256)), dim3(256), 0, st, e->x.p, cs.hi, cs.lo, e->d_off.p, e->cx.p,
+                       ccs.hi, ccs.lo, batch, d);
+            launch_linear(e->di, ccs, e->s_o[L], batch, d, d, e->t[lname(l, "attention.output.dense.bias")].p, e->cx.p, false, e->cx2.p, nullptr,
+                          nullptr, e->t[lname(l, "attention.output.LayerNorm.weight")].p, e->t[lname(l, "attention.output.LayerNorm.bias")].p, c.eps,
+                          e->cx.p, cxs.hi, cxs.lo, e->ws.p, Embedder::WS_FLOATS, st, &po);
+            launch_linear(e->di, cxs, e->s_f1[L], batch, c.inter, d, e->t[lname(l, "intermediate.dense.bias")].p, nullptr, true, nullptr, cfs.hi,
+                          cfs.lo, nullptr, nullptr, 0.f, nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st, &p1);
+            launch_linear(e->di, cfs, e->s_f2[L], batch, d, c.inter, e->t[lname(l, "output.dense.bias")].p, e->cx.p, false, e->cx2.p, nullptr,
+                          nullptr, e->t[lname(l, "output.LayerNorm.weight")].p, e->t[lname(l, "output.LayerNorm.bias")].p, c.eps, e->cx.p, cxs.hi,
+                          cxs.lo, e->ws.p, Embedder::WS_FLOATS, st, &p2);
+            break;
+        }
         // O projection (+bias +residual) -> LayerNorm -> x (fp32 residual stream) + its split planes
         launch_linear(e->di, cs, e->s_o[L], n_tok, d, d, e->t[lname(l, "attention.output.dense.bias")].p, e->x.p, false, e->x2.p, nullptr, nullptr,
                       e->t[lname(l, "attention.output.LayerNorm.weight")].p, e->t[lname(l, "attention.output.LayerNorm.bias")].p, c.eps, e->x.p, xs.hi, xs.lo,
@@ -1051,11 +1159,11 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
                       Embedder::WS_FLOATS, st);
     }
     };   // run_layers
-    const std::tuple<int, int, int> key(n_tok, batch, max_len);
+    const std::tuple<int, int, int, int> key(n_tok, batch, max_len, cls_rows ? 1 : 0);
     auto git = e->graphs.find(key);
     if (git != e->graphs.end()) {
         KRAG_CUDA(cudaGraphLaunch(git->second, st));
-        count_launch(1 + 7 * c.layers);
+        count_launch(1 + 7 * c.layers + (cls_rows ? 1 : 0));
     } else if (e->seen.size() > 4096 ? (e->seen.clear(), false) : e->seen[key]++ >= 1) {
         if (e->graphs.size() >= 64) e->drop_graphs();
         cudaGraph_t g = nullptr;
@@ -1076,13 +1184,13 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
         if (!e->in_ev) KRAG_CUDA(cudaEventCreateWithFlags(&e->in_ev, cudaEventDisableTiming));
         KRAG_CUDA(cudaEventRecord(e->in_ev, consumer));
         KRAG_CUDA(cudaStreamWaitEvent(st, e->in_ev, 0));
-        launch_pool(e, batch, out_dev, ld_out, st);
+        launch_pool(e, batch, cls_rows, out_dev, ld_out, st);
         if (!e->done) KRAG_CUDA(cudaEventCreateWithFlags(&e->done, cudaEventDisableTiming));
         KRAG_CUDA(cudaEventRecord(e->done, st));
         KRAG_CUDA(cudaStreamWaitEvent(consumer, e->done, 0));
     }
     if (out_host) {
-        launch_pool(e, batch, e->out.p, d, st);
+        launch_pool(e, batch, cls_rows, e->out.p, d, st);
         KRAG_CUDA(cudaMemcpyAsync(out_host, e->out.p, 4 * (size_t)batch * d, cudaMemcpyDeviceToHost, st));
         KRAG_CUDA(cudaStreamSynchronize(st));
     }
