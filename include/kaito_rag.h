@@ -314,6 +314,20 @@ int32_t krag_embedder_set_pooling(krag_embedder* e, int32_t mode);
 /* Under CLS pooling the last layer's O projection, FFN and LayerNorms run on the [CLS] rows only (on = 1, the default).
  * on = 0 runs them over every token; the embeddings are the same bits either way.  Test hook. */
 int32_t krag_debug_embedder_cls_rows(krag_embedder* e, int32_t on);
+/* Cross-encoder reranking (BertForSequenceClassification with one label).  The embedder must have been loaded with the
+ * head as well: "pooler.dense.weight" [hidden, hidden], "pooler.dense.bias", "classifier.weight" [1, hidden] and
+ * "classifier.bias" [1].  Query i owns pairs pair_offsets[i] .. pair_offsets[i+1] (0 to 300 of them); pair p is the packed
+ * sequence tok_ids[tok_offsets[p] .. tok_offsets[p+1]) = [CLS] query [SEP] passage [SEP] (at most max_position tokens), whose
+ * tokens from seg_b[p] on (the first passage token, in [1, length]) take token type 1.  score = activation(classifier .
+ * tanh(pooler([CLS] row))).  out_pos / out_score [n_queries, top_k]: per query its best top_k pairs (position within the
+ * query's pairs), scores descending, equal scores by position ascending; -1 / NaN past the query's pair count.  All
+ * arguments are HOST memory; the call returns synchronised.  KRAG_E_INVALID: head missing, top_k outside [1, 300],
+ * unknown activation, a pair too long or seg_b out of range. */
+#define KRAG_RERANK_SIGMOID 0
+#define KRAG_RERANK_IDENTITY 1
+int32_t krag_rerank(krag_embedder* e, int32_t n_queries, const int32_t* pair_offsets, const int32_t* tok_ids,
+                    const int32_t* tok_offsets, const int32_t* seg_b, int32_t activation, int32_t top_k, int32_t* out_pos,
+                    float* out_score);
 int32_t krag_embedder_destroy(krag_embedder* e);
 
 /* ------------------------------------------------- host-side text analysis (no GPU involved; ASCII input) */

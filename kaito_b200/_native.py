@@ -40,8 +40,9 @@ SYMBOLS = [
     "krag_host_pinned_bytes", "krag_host_rows_fetched", "krag_index_compact", "krag_last_compact",
     "krag_last_commit", "krag_index_alive_bitmap", "krag_redeal_begin", "krag_redeal_tables", "krag_redeal_prepare",
     "krag_dev_redeal_pack", "krag_dev_redeal_unpack", "krag_redeal_finish", "krag_redeal_abort", "krag_embedder_set_pooling",
-    "krag_debug_embedder_cls_rows",
+    "krag_debug_embedder_cls_rows", "krag_rerank",
 ]
+RERANK_SIGMOID, RERANK_IDENTITY = 0, 1   # krag_rerank: activation of the classifier logit
 
 
 class KragError(RuntimeError):
@@ -130,6 +131,7 @@ def load() -> C.CDLL:
     L.krag_embed_dev.argtypes = [vp, i32, vp, vp, vp, i32, vp]
     L.krag_embedder_set_pooling.argtypes = [vp, i32]
     L.krag_debug_embedder_cls_rows.argtypes = [vp, i32]
+    L.krag_rerank.argtypes = [vp, i32, vp, vp, vp, vp, i32, i32, vp, vp]
     L.krag_embedder_destroy.argtypes = [vp]
     L.krag_debug_gemm_tf32.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp, i32, vp, i32, i32, C.POINTER(C.c_float)]
     L.krag_debug_linear_ln.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, C.c_float, vp]
@@ -297,10 +299,11 @@ class Embedder:
         check(self._L.krag_embedder_create(ctx._h, C.byref(cfg), C.byref(h)))
         self._h = h
 
-    def load_state_dict(self, state: dict):
-        """state: Hugging Face BertModel names -> numpy fp32 arrays (pooler / position_ids entries are ignored)"""
+    def load_state_dict(self, state: dict, head: bool = False):
+        """state: Hugging Face BertModel names -> numpy fp32 arrays (position_ids entries are ignored).  head=False: pooler
+        and classifier entries are ignored too; head=True: they are loaded, and rerank() may be called"""
         for name, arr in state.items():
-            if name.startswith("pooler.") or name.endswith("position_ids"):
+            if name.endswith("position_ids") or (not head and name.startswith(("pooler.", "classifier."))):
                 continue
             a = np.ascontiguousarray(arr, np.float32)
             check(self._L.krag_embedder_load_tensor(self._h, name.encode(), ptr(a), a.size))
@@ -336,6 +339,19 @@ class Embedder:
     def set_pooling(self, mode: int):
         """POOL_CLS (default) or POOL_MEAN for the following forwards"""
         check(self._L.krag_embedder_set_pooling(self._h, mode))
+
+    def rerank(self, pair_offsets, flat_tokens, tok_offsets, seg_b, top_k: int, activation: int = RERANK_SIGMOID):
+        """krag_rerank: (positions int32 [n_queries, top_k], scores float32 [n_queries, top_k]); -1 / NaN past a query's
+        pair count"""
+        pair_offsets = np.ascontiguousarray(pair_offsets, np.int32)
+        flat_tokens = np.ascontiguousarray(flat_tokens, np.int32); tok_offsets = np.ascontiguousarray(tok_offsets, np.int32)
+        seg_b = np.ascontiguousarray(seg_b, np.int32)
+        nq = len(pair_offsets) - 1
+        pos = np.empty((nq, top_k), np.int32)
+        sc = np.empty((nq, top_k), np.float32)
+        check(self._L.krag_rerank(self._h, nq, ptr(pair_offsets), ptr(flat_tokens), ptr(tok_offsets), ptr(seg_b), activation, top_k,
+                                  ptr(pos), ptr(sc)))
+        return pos, sc
 
     def debug_cls_rows(self, on: bool):
         """test hook: False runs the last layer over every token under CLS pooling too (same embeddings)"""

@@ -1684,6 +1684,17 @@ int32_t krag_debug_embedder_cls_rows(krag_embedder* h, int32_t on)
         embedder_set_cls_rows_only(h->e, on != 0);
     });
 }
+static_assert(KRAG_RERANK_SIGMOID == EMB_ACT_SIGMOID && KRAG_RERANK_IDENTITY == EMB_ACT_IDENTITY, "head activations");
+int32_t krag_rerank(krag_embedder* h, int32_t n_queries, const int32_t* pair_offsets, const int32_t* tok_ids, const int32_t* tok_offsets,
+                    const int32_t* seg_b, int32_t activation, int32_t top_k, int32_t* out_pos, float* out_score)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(h && pair_offsets && out_pos && out_score && n_queries >= 1, KRAG_E_INVALID, "bad argument");
+        KRAG_REQUIRE(pair_offsets[n_queries] == 0 || (tok_ids && tok_offsets && seg_b), KRAG_E_INVALID, "bad argument");
+        KRAG_CUDA(cudaSetDevice(h->ctx->di.device));
+        embedder_rerank(h->e, n_queries, pair_offsets, tok_ids, tok_offsets, seg_b, activation, top_k, out_pos, out_score);
+    });
+}
 int32_t krag_embedder_destroy(krag_embedder* h)
 {
     return guarded([&] {

@@ -16,6 +16,7 @@
 #include <cuda_fp16.h>
 #include <math_constants.h>
 
+#include <cstring>
 #include <map>
 #include <memory>
 #include <stdexcept>
@@ -320,10 +321,11 @@ layernorm_kernel(const float* __restrict__ x, float* __restrict__ y, uint16_t* _
                        y_lo ? y_lo + (size_t)r * d : nullptr, g, b, d, eps, lane);
 }
 
-// embeddings: x[t] = LN(word[id] + pos[p] + type[0]); one warp per token; scratch row in shared memory
+// embeddings: x[t] = LN(word[id] + pos[p] + type[typ[t]]); one warp per token; scratch row in shared memory.  typ null (single
+// sequences): type row 0 for every token; a cross-encoder pair has type 0 through its first [SEP] and type 1 after it.
 __global__ void __launch_bounds__(256)
-embed_ln_kernel(const int32_t* __restrict__ tok, const int32_t* __restrict__ pos, const float* __restrict__ word,
-                const float* __restrict__ pemb, const float* __restrict__ temb, const float* __restrict__ g,
+embed_ln_kernel(const int32_t* __restrict__ tok, const int32_t* __restrict__ pos, const int32_t* __restrict__ typ,
+                const float* __restrict__ word, const float* __restrict__ pemb, const float* __restrict__ temb, const float* __restrict__ g,
                 const float* __restrict__ b, float* __restrict__ x, uint16_t* __restrict__ x_hi, uint16_t* __restrict__ x_lo,
                 int n_tok, int d, int vocab, float eps)
 {
@@ -338,7 +340,8 @@ embed_ln_kernel(const int32_t* __restrict__ tok, const int32_t* __restrict__ pos
     id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
     const float* wr = word + (size_t)id * d;
     const float* pr = pemb + (size_t)pos[t] * d;
-    for (int i = lane; i < d; i += 32) row[i] = (wr[i] + temb[i]) + pr[i];   // torch: inputs_embeds + token_type + position
+    const float* tr = typ ? temb + (size_t)typ[t] * d : temb;
+    for (int i = lane; i < d; i += 32) row[i] = (wr[i] + tr[i]) + pr[i];   // torch: inputs_embeds + token_type + position
     __syncwarp();
     warp_layernorm_row(row, x + (size_t)t * d, x_hi + (size_t)t * d, x_lo + (size_t)t * d, g, b, d, eps, lane);
 }
@@ -720,6 +723,56 @@ mean_normalize_kernel(const float* __restrict__ x, const int32_t* __restrict__ s
     }
 }
 
+// ------------------------------------------------------------------------ cross-encoder head
+// BertForSequenceClassification with one label: score = act(w_c . tanh(W_p h + b_p) + b_c) over the [CLS] row h.  p holds
+// W_p h + b_p (the pooler GEMM's output); one warp per pair, lane l adds elements l, l + 32, ... in order, then the butterfly
+// of warp_sum: a fixed fp32 order, so a pair's score does not depend on the other pairs of the batch.
+__global__ void __launch_bounds__(256)
+classifier_head_kernel(const float* __restrict__ p, const float* __restrict__ w, const float* __restrict__ bias, int batch, int d,
+                       int act, float* __restrict__ out)
+{
+    const int b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (b >= batch) return;
+    const float* row = p + (size_t)b * d;
+    float s = 0.f;
+    for (int i = lane; i < d; i += 32) s = fmaf(tanhf(row[i]), w[i], s);
+    const float z = warp_sum(s) + bias[0];
+    if (lane == 0) out[b] = act == EMB_ACT_SIGMOID ? 1.f / (1.f + expf(-z)) : z;
+}
+
+// Per query (one CTA): the top_k of its candidates' scores, descending, ties by fused position ascending.  Keys are
+// (~ordered_bits(score)) << 32 | position: unique, so the ascending bitonic sort in shared memory gives one order whatever
+// the sort does with equal keys.  Positions past the query's candidates are -1 with a NaN score.
+constexpr int RS_MAX = 512;   // >= RERANK_MAX_CANDIDATES, a power of two
+__global__ void __launch_bounds__(256)
+rerank_select_kernel(const float* __restrict__ scores, const int32_t* __restrict__ pair_off, int top_k, int32_t* __restrict__ out_pos,
+                     float* __restrict__ out_score)
+{
+    __shared__ uint64_t keys[RS_MAX];
+    const int q = blockIdx.x;
+    const int p0 = pair_off[q], n = pair_off[q + 1] - p0;
+    int n2 = 1;
+    while (n2 < n) n2 <<= 1;
+    for (int i = threadIdx.x; i < n2; i += blockDim.x) keys[i] = i < n ? make_key_desc(scores[p0 + i], (uint32_t)i) : KEY_PAD;
+    __syncthreads();
+    for (int k = 2; k <= n2; k <<= 1)
+        for (int j = k >> 1; j > 0; j >>= 1) {
+            for (int i = threadIdx.x; i < n2; i += blockDim.x) {
+                const int l = i ^ j;
+                if (l > i) {
+                    const uint64_t a = keys[i], c = keys[l];
+                    if ((a > c) == ((i & k) == 0)) { keys[i] = c; keys[l] = a; }
+                }
+            }
+            __syncthreads();
+        }
+    for (int i = threadIdx.x; i < top_k; i += blockDim.x) {
+        const bool on = i < n;
+        out_pos[(size_t)q * top_k + i] = on ? (int32_t)key_ordinal(keys[i]) : -1;
+        out_score[(size_t)q * top_k + i] = on ? key_value_desc(keys[i]) : CUDART_NAN_F;
+    }
+}
+
 // ------------------------------------------------------------------------------------ host
 // launch with programmatic stream serialization (see pdl_wait in tc_ptx.cuh); only for kernels that call pdl_wait()
 template <typename... KArgs, typename... Args>
@@ -908,16 +961,23 @@ struct Embedder {
     // split fp16 planes of the GEMM weights (finalize): per layer QKV (fused), attention output, FFN1, FFN2
     std::vector<SplitMat> s_qkv, s_o, s_f1, s_f2;
     std::vector<DevArray<uint16_t>> planes;     // the buffers all weight planes live in
+    SplitMat s_pool{nullptr, nullptr};          // pooler.dense.weight (cross-encoders: finalize found the classifier head)
+    bool has_head = false;
     bool finalized = false;
     cudaStream_t st = nullptr;
     cudaEvent_t done = nullptr, in_ev = nullptr;
-    std::map<std::tuple<int, int, int, int>, cudaGraphExec_t> graphs;   // captured forward per (n_tok, batch, max_len, cls_rows)
-    std::map<std::tuple<int, int, int, int>, int> seen;
+    // captured forward per (n_tok, batch, max_len, cls_rows, head): head = 1 for cross-encoder pairs (token types uploaded)
+    using GraphKey = std::tuple<int, int, int, int, int>;
+    std::map<GraphKey, cudaGraphExec_t> graphs;
+    std::map<GraphKey, int> seen;
     int pooling = EMB_POOL_CLS;           // read by the final writer, which runs outside the captured graphs
     bool cls_rows_only = true;            // CLS pooling: the last layer after QKV + attention runs on the [CLS] rows only
     // workspaces, grown on demand
     int cap_tok = 0, cap_batch = 0;
-    DevArray<int32_t> d_tok, d_pos, d_off;
+    DevArray<int32_t> d_tok, d_pos, d_off, d_typ;
+    // reranking: one score per pair of a call, the per-query pair offsets, the selected positions | scores
+    DevArray<float> scores;
+    DevArray<int32_t> d_poff, sel;
     DevArray<float> x, x2, out;
     DevArray<uint16_t> xs, cs, fs;        // split planes [2][T][*] of x (LayerNorm outputs), attention context, FFN1 output
     DevArray<uint16_t> qkv;               // split planes [2][n_tok][3d] of the QKV projection (the lo plane starts at n_tok rows)
@@ -985,6 +1045,7 @@ void embedder_finalize(Embedder* e)
     const int d = e->cfg.hidden, inter = e->cfg.inter;
     e->finalized = false;
     e->bqkv.clear(); e->planes.clear(); e->s_qkv.clear(); e->s_o.clear(); e->s_f1.clear(); e->s_f2.clear();
+    e->s_pool = SplitMat{nullptr, nullptr}; e->has_head = false;
     e->drop_graphs(); e->seen.clear();   // captured weight pointers are about to change
     emb_get(e, "embeddings.word_embeddings.weight", 0); emb_get(e, "embeddings.position_embeddings.weight", 0);
     emb_get(e, "embeddings.token_type_embeddings.weight", 0); emb_get(e, "embeddings.LayerNorm.weight", 0);
@@ -1007,6 +1068,22 @@ void embedder_finalize(Embedder* e)
         e->s_o.push_back(emb_split_weight(e, emb_get(e, lname(l, "attention.output.dense.weight"), 0), (size_t)d * d));
         e->s_f1.push_back(emb_split_weight(e, emb_get(e, lname(l, "intermediate.dense.weight"), 0), (size_t)inter * d));
         e->s_f2.push_back(emb_split_weight(e, emb_get(e, lname(l, "output.dense.weight"), 0), (size_t)d * inter));
+    }
+    // the classifier head of a cross-encoder (BertForSequenceClassification, one label): all four tensors or none
+    const char* head[4] = {"pooler.dense.weight", "pooler.dense.bias", "classifier.weight", "classifier.bias"};
+    const int64_t head_n[4] = {(int64_t)d * d, d, d, 1};
+    int n_head = 0;
+    for (int j = 0; j < 4; ++j) {
+        auto it = e->t.find(head[j]);
+        if (it == e->t.end() || !it->second.p) continue;
+        if (it->second.cap != head_n[j])
+            throw std::runtime_error(std::string("embedder: ") + head[j] + " must hold " + std::to_string(head_n[j]) + " elements");
+        ++n_head;
+    }
+    if (n_head != 0 && n_head != 4) throw std::runtime_error("embedder: the classifier head needs pooler.dense.{weight,bias} and classifier.{weight,bias}");
+    if (n_head == 4) {
+        e->s_pool = emb_split_weight(e, emb_get(e, "pooler.dense.weight", 0), (size_t)d * d);
+        e->has_head = true;
     }
     KRAG_CUDA(cudaStreamSynchronize(e->st));
     wtmp.release();
@@ -1062,24 +1139,29 @@ static void launch_pool(const Embedder* e, int batch, bool cls_rows, float* out,
     count_launch();
 }
 
-// tok_ids: packed tokens of all sequences; tok_offsets [batch+1]; out_host [batch, hidden]
-// out_host != nullptr: embeddings are copied to the host and the call returns synchronised.
-// out_dev  != nullptr: embeddings are written to device rows of stride ld_out floats and `consumer` (a stream of
-//                      the caller) is made to wait for them -- no host round trip.
-void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int32_t* tok_offsets, float* out_host,
-                      float* out_dev, int ld_out, cudaStream_t consumer)
+// The encoder over packed sequences (tok_ids, tok_offsets [batch+1], host) up to the last hidden state, enqueued on e->st.
+// seg_b (host, [batch] or null): index of the first token of segment B of each sequence; tokens from there on add token
+// type row 1, the others row 0 (null: row 0 everywhere, the single-sequence embedding).  cls_ok: only the [CLS] rows of the
+// last layer are read.  Returns whether the last layer ran on the [CLS] rows only (then in cx / cxs, else x / xs).
+static bool encoder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int32_t* tok_offsets, const int32_t* seg_b, bool cls_ok)
 {
     if (!e->finalized) throw std::runtime_error("embedder: call finalize after loading the weights");
     const BertConfig& c = e->cfg;
     const int d = c.hidden, n_tok = tok_offsets[batch];
     cudaStream_t st = e->st;
     int max_len = 0;
-    std::vector<int32_t> pos((size_t)n_tok);
+    std::vector<int32_t> pos((size_t)n_tok), typ(seg_b ? (size_t)n_tok : 0);
+    if (seg_b && (c.type_vocab < 2 || e->t["embeddings.token_type_embeddings.weight"].cap < 2 * (int64_t)d))
+        throw std::runtime_error("embedder: sentence pairs need token type row 1 (type_vocab_size >= 2)");
     for (int b = 0; b < batch; ++b) {
         const int len = tok_offsets[b + 1] - tok_offsets[b];
         if (len < 1 || len > c.max_pos) throw std::runtime_error("embedder: sequence length must be in [1, max_position]");
         max_len = len > max_len ? len : max_len;
         for (int i = 0; i < len; ++i) pos[(size_t)tok_offsets[b] + i] = i;
+        if (seg_b) {
+            if (seg_b[b] < 1 || seg_b[b] > len) throw std::runtime_error("embedder: segment B must start in [1, sequence length]");
+            for (int i = 0; i < len; ++i) typ[(size_t)tok_offsets[b] + i] = i >= seg_b[b] ? 1 : 0;
+        }
     }
     if (n_tok > e->cap_tok || batch > e->cap_batch) {
         const int64_t T = n_tok > e->cap_tok ? n_tok : e->cap_tok, Bc = batch > e->cap_batch ? batch : e->cap_batch;
@@ -1088,10 +1170,10 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
         // all old buffers go before the first new one is allocated (the peak is the new set only); a grow that fails
         // half-way leaves no workspace and capacity 0, so the next call grows again
         e->cap_tok = e->cap_batch = 0;
-        e->d_tok.release(); e->d_pos.release(); e->d_off.release(); e->x.release(); e->x2.release(); e->qkv.release();
+        e->d_tok.release(); e->d_pos.release(); e->d_off.release(); e->d_typ.release(); e->x.release(); e->x2.release(); e->qkv.release();
         e->xs.release(); e->cs.release(); e->fs.release(); e->out.release();
         e->cx.release(); e->cx2.release(); e->ccs.release(); e->cxs.release(); e->cfs.release();
-        e->d_tok.alloc(T); e->d_pos.alloc(T); e->d_off.alloc(Bc + 1);
+        e->d_tok.alloc(T); e->d_pos.alloc(T); e->d_off.alloc(Bc + 1); e->d_typ.alloc(T);
         e->x.alloc(T * d); e->x2.alloc(T * d); e->qkv.alloc(2 * T * 3 * d);
         e->xs.alloc(2 * T * d); e->cs.alloc(2 * T * d); e->fs.alloc(2 * T * c.inter);
         e->out.alloc(Bc * d);
@@ -1104,17 +1186,18 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
     KRAG_CUDA(cudaMemcpyAsync(e->d_tok.p, tok_ids, 4 * (size_t)n_tok, cudaMemcpyHostToDevice, st));
     KRAG_CUDA(cudaMemcpyAsync(e->d_pos.p, pos.data(), 4 * (size_t)n_tok, cudaMemcpyHostToDevice, st));
     KRAG_CUDA(cudaMemcpyAsync(e->d_off.p, tok_offsets, 4 * (size_t)(batch + 1), cudaMemcpyHostToDevice, st));
+    if (seg_b) KRAG_CUDA(cudaMemcpyAsync(e->d_typ.p, typ.data(), 4 * (size_t)n_tok, cudaMemcpyHostToDevice, st));
 
     // CLS pooling reads one row per sequence of the last layer's output.  K and V of every token are still needed, so the
     // last QKV projection runs over all tokens; attention then runs for the first query rows only, and the O projection,
     // FFN and LayerNorms run on the gathered [CLS] rows.  Those GEMMs keep the plan (tile width, K split) of the full
     // token count, so every [CLS] row gets the same bits as in the full layer.  Taken when it saves a 128-row tile.
-    const bool cls_rows = e->pooling == EMB_POOL_CLS && e->cls_rows_only && (n_tok + GM_TILE - 1) / GM_TILE > (batch + GM_TILE - 1) / GM_TILE;
+    const bool cls_rows = cls_ok && e->cls_rows_only && (n_tok + GM_TILE - 1) / GM_TILE > (batch + GM_TILE - 1) / GM_TILE;
     // The forward is ~7 kernels per layer; for a handful of query tokens it is bound by launch gaps and kernel
-    // prologues, so each (n_tok, batch, max_len, cls_rows) shape is captured into a CUDA graph the second time it is seen.
+    // prologues, so each (n_tok, batch, max_len, cls_rows, head) shape is captured into a CUDA graph the second time it is seen.
     auto run_layers = [&]() {
     launch_pdl(embed_ln_kernel, dim3((unsigned)((n_tok + 7) / 8)), dim3(256), (size_t)8 * d * 4, st, e->d_tok.p, e->d_pos.p,
-               e->t["embeddings.word_embeddings.weight"].p, e->t["embeddings.position_embeddings.weight"].p,
+               seg_b ? e->d_typ.p : nullptr, e->t["embeddings.word_embeddings.weight"].p, e->t["embeddings.position_embeddings.weight"].p,
                e->t["embeddings.token_type_embeddings.weight"].p, e->t["embeddings.LayerNorm.weight"].p, e->t["embeddings.LayerNorm.bias"].p, e->x.p,
                xs.hi, xs.lo, n_tok, d, c.vocab, c.eps);
     const int dh = d / c.heads;
@@ -1159,7 +1242,7 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
                       Embedder::WS_FLOATS, st);
     }
     };   // run_layers
-    const std::tuple<int, int, int, int> key(n_tok, batch, max_len, cls_rows ? 1 : 0);
+    const Embedder::GraphKey key(n_tok, batch, max_len, cls_rows ? 1 : 0, seg_b ? 1 : 0);
     auto git = e->graphs.find(key);
     if (git != e->graphs.end()) {
         KRAG_CUDA(cudaGraphLaunch(git->second, st));
@@ -1178,6 +1261,19 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
     } else {
         run_layers();
     }
+    return cls_rows;
+}
+
+// tok_ids: packed tokens of all sequences; tok_offsets [batch+1]; out_host [batch, hidden]
+// out_host != nullptr: embeddings are copied to the host and the call returns synchronised.
+// out_dev  != nullptr: embeddings are written to device rows of stride ld_out floats and `consumer` (a stream of
+//                      the caller) is made to wait for them -- no host round trip.
+void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int32_t* tok_offsets, float* out_host,
+                      float* out_dev, int ld_out, cudaStream_t consumer)
+{
+    const bool cls_rows = encoder_forward(e, batch, tok_ids, tok_offsets, nullptr, e->pooling == EMB_POOL_CLS);
+    const int d = e->cfg.hidden;
+    cudaStream_t st = e->st;
     if (out_dev) {
         // the caller's buffer may still be read by work it enqueued earlier on `consumer` (the previous batch's scan): only
         // the final writer waits for that; the forward itself overlaps with it
@@ -1194,6 +1290,70 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
         KRAG_CUDA(cudaMemcpyAsync(out_host, e->out.p, 4 * (size_t)batch * d, cudaMemcpyDeviceToHost, st));
         KRAG_CUDA(cudaStreamSynchronize(st));
     }
+}
+
+// Cross-encoder reranking.  Pairs [CLS] q [SEP] d [SEP] of n_queries queries, packed: query i owns pairs
+// pair_off[i] .. pair_off[i + 1] (at most RERANK_MAX_CANDIDATES), pair p is tok_ids[tok_off[p] .. tok_off[p + 1]) with
+// segment B from seg_b[p].  The pairs go through forwards of at most RERANK_MAX_TOKENS tokens (whole pairs), each followed by
+// the pooler GEMM and the classifier head, which write the pair's score at its offset in one buffer; one select kernel then
+// orders every query's scores and one copy brings back [n_queries, top_k] positions (within the query's pairs, -1 past its
+// count) and scores.
+void embedder_rerank(Embedder* e, int n_queries, const int32_t* pair_off, const int32_t* tok_ids, const int32_t* tok_off,
+                     const int32_t* seg_b, int act, int top_k, int32_t* out_pos, float* out_score)
+{
+    if (!e->finalized) throw std::runtime_error("embedder: call finalize after loading the weights");
+    if (!e->has_head) throw std::runtime_error("embedder: reranking needs the classifier head (pooler.dense.*, classifier.*)");
+    if (act != EMB_ACT_SIGMOID && act != EMB_ACT_IDENTITY) throw std::runtime_error("embedder: unknown head activation");
+    if (top_k < 1 || top_k > RERANK_MAX_CANDIDATES) throw std::runtime_error("embedder: top_k must be in [1, 300]");
+    if (n_queries < 1 || pair_off[0] != 0) throw std::runtime_error("embedder: pair offsets must start at 0");
+    for (int q = 0; q < n_queries; ++q) {
+        const int n = pair_off[q + 1] - pair_off[q];
+        if (n < 0 || n > RERANK_MAX_CANDIDATES) throw std::runtime_error("embedder: a query has 0 to 300 candidate pairs");
+    }
+    const int n_pairs = pair_off[n_queries], d = e->cfg.hidden;
+    if (n_pairs > 0 && tok_off[0] != 0) throw std::runtime_error("embedder: token offsets must start at 0");
+    for (int p = 0; p < n_pairs; ++p) {
+        const int len = tok_off[p + 1] - tok_off[p];
+        if (len < 1 || len > e->cfg.max_pos) throw std::runtime_error("embedder: a pair's length must be in [1, max_position]");
+    }
+    cudaStream_t st = e->st;
+    if (e->scores.cap < (n_pairs > 0 ? n_pairs : 1)) e->scores.alloc(n_pairs > 0 ? n_pairs : 1);
+    if (e->d_poff.cap < n_queries + 1) e->d_poff.alloc(n_queries + 1);
+    if (e->sel.cap < 2 * (int64_t)n_queries * top_k) e->sel.alloc(2 * (int64_t)n_queries * top_k);
+    std::vector<int32_t> offs;
+    for (int p0 = 0; p0 < n_pairs;) {
+        int p1 = p0 + 1;
+        while (p1 < n_pairs && tok_off[p1 + 1] - tok_off[p0] <= RERANK_MAX_TOKENS) ++p1;
+        const int batch = p1 - p0;
+        offs.assign((size_t)batch + 1, 0);
+        for (int j = 0; j <= batch; ++j) offs[(size_t)j] = tok_off[p0 + j] - tok_off[p0];
+        const bool cls_rows = encoder_forward(e, batch, tok_ids + tok_off[p0], offs.data(), seg_b + p0, true);
+        // the [CLS] rows' split planes: where the shortened last layer left them, else gathered from the full stream
+        const SplitMat cxs{e->cxs.p, e->cxs.p + (size_t)batch * d};
+        if (!cls_rows) {
+            const SplitMat xs{e->xs.p, e->xs.p + (size_t)e->cap_tok * d};
+            launch_pdl(gather_cls_kernel, dim3((unsigned)((batch * 32 + 255) / 256)), dim3(256), 0, st, e->x.p, xs.hi, xs.lo, e->d_off.p,
+                       e->cx.p, cxs.hi, cxs.lo, batch, d);
+        }
+        launch_linear(e->di, cxs, e->s_pool, batch, d, d, e->t["pooler.dense.bias"].p, nullptr, false, e->cx2.p, nullptr, nullptr, nullptr,
+                      nullptr, 0.f, nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st);
+        classifier_head_kernel<<<(unsigned)((batch * 32 + 255) / 256), 256, 0, st>>>(e->cx2.p, e->t["classifier.weight"].p,
+                                                                                   e->t["classifier.bias"].p, batch, d, act, e->scores.p + p0);
+        KRAG_CUDA(cudaGetLastError());
+        count_launch();
+        p0 = p1;
+    }
+    KRAG_CUDA(cudaMemcpyAsync(e->d_poff.p, pair_off, 4 * (size_t)(n_queries + 1), cudaMemcpyHostToDevice, st));
+    const size_t nk = (size_t)n_queries * top_k;
+    rerank_select_kernel<<<(unsigned)n_queries, 256, 0, st>>>(e->scores.p, e->d_poff.p, top_k, e->sel.p,
+                                                             reinterpret_cast<float*>(e->sel.p + nk));
+    KRAG_CUDA(cudaGetLastError());
+    count_launch();
+    std::vector<int32_t> h(2 * nk);
+    KRAG_CUDA(cudaMemcpyAsync(h.data(), e->sel.p, 4 * 2 * nk, cudaMemcpyDeviceToHost, st));
+    KRAG_CUDA(cudaStreamSynchronize(st));
+    std::memcpy(out_pos, h.data(), 4 * nk);
+    std::memcpy(out_score, h.data() + nk, 4 * nk);
 }
 
 }  // namespace krag

@@ -466,6 +466,12 @@ void embedder_set_pooling(Embedder* e, int mode);
 void embedder_set_cls_rows_only(Embedder* e, bool on);
 void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int32_t* tok_offsets, float* out_host,
                       float* out_dev = nullptr, int ld_out = 0, cudaStream_t consumer = nullptr);
+// cross-encoder reranking (classifier head loaded): scores of sentence pairs, top_k per query (see embed.cu)
+enum { EMB_ACT_SIGMOID = 0, EMB_ACT_IDENTITY = 1 };   // = KRAG_RERANK_SIGMOID / KRAG_RERANK_IDENTITY
+constexpr int RERANK_MAX_CANDIDATES = 300;           // pairs per query (= KRAG_MAX_TOP_K)
+constexpr int RERANK_MAX_TOKENS = 65536;             // tokens per forward of a rerank call
+void embedder_rerank(Embedder* e, int n_queries, const int32_t* pair_off, const int32_t* tok_ids, const int32_t* tok_off,
+                     const int32_t* seg_b, int act, int top_k, int32_t* out_pos, float* out_score);
 // A fp32 matrix carried as two fp16 planes: v = hi + lo * 2^-11 (see embed.cu: split operands of the K5 GEMMs)
 struct SplitMat { uint16_t* hi; uint16_t* lo; };
 void launch_split_f16(const float* in, uint16_t* hi, uint16_t* lo, int64_t n /* % 8 == 0 */, cudaStream_t st);

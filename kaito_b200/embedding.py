@@ -72,6 +72,39 @@ def _json(path: str, required: bool = True):
         raise ValueError(f"{path}: unreadable ({e})") from None
 
 
+def check_bert_config(cpath: str, cfg: dict) -> int:
+    """the encoder shapes K5 runs (config.json at cpath, parsed as cfg); returns hidden_size or raises a ValueError naming the
+    file and field (shared by the embedder and cross-encoder snapshot readers)"""
+    for field, want, default in (("model_type", "bert", None), ("position_embedding_type", "absolute", "absolute"),
+                                 ("hidden_act", "gelu", "gelu"), ("is_decoder", False, False)):
+        if cfg.get(field, default) != want:
+            raise ValueError(f"{cpath}: {field} {cfg.get(field, default)!r}: K5 runs {field} {want!r} only")
+    d, heads, inter = cfg.get("hidden_size"), cfg.get("num_attention_heads"), cfg.get("intermediate_size")
+    if not all(isinstance(v, int) and v > 0 for v in (d, heads, inter)):
+        raise ValueError(f"{cpath}: hidden_size, num_attention_heads and intermediate_size must be positive integers")
+    if d % heads or d // heads not in (32, 64):
+        raise ValueError(f"{cpath}: hidden_size {d} / num_attention_heads {heads}: K5 runs attention heads of 32 or 64 dims")
+    if d % 128 or d > 1024:
+        raise ValueError(f"{cpath}: hidden_size {d}: K5 runs multiples of 128 up to 1024")
+    if inter % 128:
+        raise ValueError(f"{cpath}: intermediate_size {inter}: K5 runs multiples of 128")
+    return d
+
+
+def load_state(model_dir: str) -> dict:
+    """model.safetensors or pytorch_model.bin of a snapshot as numpy fp32 arrays, names without the "bert." prefix"""
+    st_path, bin_path = os.path.join(model_dir, "model.safetensors"), os.path.join(model_dir, "pytorch_model.bin")
+    if os.path.exists(st_path):
+        from safetensors.numpy import load_file
+        state = load_file(st_path)
+    elif os.path.exists(bin_path):
+        import torch
+        state = {k: v.float().numpy() for k, v in torch.load(bin_path, map_location="cpu").items()}
+    else:
+        raise ValueError(f"{model_dir}: neither model.safetensors nor pytorch_model.bin")
+    return {k[5:] if k.startswith("bert.") else k: v for k, v in state.items()}
+
+
 def read_snapshot_spec(model_dir: str) -> dict:
     """What sentence-transformers would compute from a model snapshot, or a ValueError naming the file and field that asks for
     something K5 does not compute.  Reads JSON only (no weights, no GPU).  Returns
@@ -104,19 +137,7 @@ def read_snapshot_spec(model_dir: str) -> dict:
 
     cpath = join(model_dir, "config.json")
     cfg = _json(cpath)
-    for field, want, default in (("model_type", "bert", None), ("position_embedding_type", "absolute", "absolute"),
-                                 ("hidden_act", "gelu", "gelu"), ("is_decoder", False, False)):
-        if cfg.get(field, default) != want:
-            raise ValueError(f"{cpath}: {field} {cfg.get(field, default)!r}: K5 runs {field} {want!r} only")
-    d, heads, inter = cfg.get("hidden_size"), cfg.get("num_attention_heads"), cfg.get("intermediate_size")
-    if not all(isinstance(v, int) and v > 0 for v in (d, heads, inter)):
-        raise ValueError(f"{cpath}: hidden_size, num_attention_heads and intermediate_size must be positive integers")
-    if d % heads or d // heads not in (32, 64):
-        raise ValueError(f"{cpath}: hidden_size {d} / num_attention_heads {heads}: K5 runs attention heads of 32 or 64 dims")
-    if d % 128 or d > 1024:
-        raise ValueError(f"{cpath}: hidden_size {d}: K5 runs multiples of 128 up to 1024")
-    if inter % 128:
-        raise ValueError(f"{cpath}: intermediate_size {inter}: K5 runs multiples of 128")
+    d = check_bert_config(cpath, cfg)
     if modules is not None and pc.get("word_embedding_dimension", d) != d:
         raise ValueError(f"{ppath}: word_embedding_dimension {pc['word_embedding_dimension']} differs from config.json "
                          f"hidden_size {d}")
@@ -172,16 +193,7 @@ class GpuBertEmbedding(BaseEmbeddingModel):
         from .text import WordPieceTokenizer
         spec = read_snapshot_spec(model_dir)
         cfg = _json(os.path.join(model_dir, "config.json"))
-        st_path, bin_path = os.path.join(model_dir, "model.safetensors"), os.path.join(model_dir, "pytorch_model.bin")
-        if os.path.exists(st_path):
-            from safetensors.numpy import load_file
-            state = load_file(st_path)
-        elif os.path.exists(bin_path):
-            import torch
-            state = {k: v.float().numpy() for k, v in torch.load(bin_path, map_location="cpu").items()}
-        else:
-            raise ValueError(f"{model_dir}: neither model.safetensors nor pytorch_model.bin")
-        state = {k[5:] if k.startswith("bert.") else k: v for k, v in state.items()}
+        state = load_state(model_dir)
         kw.setdefault("query_instruction", spec["query_instruction"])
         kw.setdefault("pooling", spec["pooling"])
         tok = WordPieceTokenizer.from_file(os.path.join(model_dir, "vocab.txt"), do_lower_case=spec["do_lower_case"],

@@ -430,6 +430,15 @@ def main():
             read_snapshot_spec(model_dir)            # refuse a snapshot K5 cannot run before any GPU work starts
         except ValueError as e:
             raise SystemExit(f"embedding model '{cfg['embedding_model']}' is not supported by this image: {e}")
+    rerank_dir = os.getenv("KRAG_RERANK_MODEL_DIR") or None
+    if rerank_dir:
+        from .rerank import read_cross_encoder_spec
+        try:
+            read_cross_encoder_spec(rerank_dir)      # refuse a cross-encoder K5 cannot run before any GPU work starts
+            if int(os.getenv("KRAG_RERANK_CANDIDATES", "30")) < 1:
+                raise ValueError("KRAG_RERANK_CANDIDATES must be >= 1")
+        except ValueError as e:
+            raise SystemExit(f"reranker '{rerank_dir}' is not supported by this image: {e}")
     n_gpus = int(os.getenv("KRAG_NUM_GPUS", "0")) or _gpu_count()
     ctx = _native.Context(device_id=cfg["device_id"], rank=0, world_size=max(1, n_gpus),
                           row_storage=_native.row_storage_from_env())
@@ -456,7 +465,14 @@ def main():
     else:
         raise SystemExit(f"embedding model '{cfg['embedding_model']}' not found locally (no network in the pod): mount a "
                          "Hugging Face snapshot and set KRAG_MODEL_DIR, or KRAG_ALLOW_HASHING_EMBEDDING=1 for functional tests")
-    app = create_app(vs.VectorStore(embed, engine), cfg)
+    reranker = None
+    if rerank_dir:
+        from .rerank import GpuCrossEncoder
+        try:
+            reranker = GpuCrossEncoder.from_pretrained(ctx, rerank_dir)      # K5 + classifier head, on rank 0 after the exchange
+        except ValueError as e:
+            raise SystemExit(f"reranker '{rerank_dir}' is not supported by this image: {e}")
+    app = create_app(vs.VectorStore(embed, engine, reranker=reranker), cfg)
     fronts, rpc = [], None
     try:
         n_front = int(os.getenv("KRAG_HTTP_WORKERS", "0"))

@@ -385,6 +385,30 @@ class WordPieceTokenizer:
         flat = np.fromiter((i for t in lists for i in t), np.int32, int(toff[-1]))
         return flat, toff
 
+    def encode_batch_plain(self, texts: list[str]) -> list[np.ndarray]:
+        """int32 ids of every text without [CLS] / [SEP] and without truncation (the halves of a sentence pair).  ASCII
+        texts go through the native encoder in one call: a WordPiece token covers at least one character, so a budget of
+        the longest text's length + 2 never truncates."""
+        out: list = [None] * len(texts)
+        idx = [i for i, t in enumerate(texts) if self._nat is not None and t.isascii()]
+        if idx:
+            import ctypes as C
+            raws = [texts[i].encode("ascii") for i in idx]
+            offs = np.zeros(len(raws) + 1, np.int64)
+            np.cumsum([len(r) for r in raws], out=offs[1:])
+            width = max(len(r) for r in raws) + 2
+            ids = np.empty((len(raws), width), np.int32)
+            cnt = np.empty(len(raws), np.int32)
+            rc = _native_lib().krag_wordpiece_encode_batch(self._nat, len(raws), b"".join(raws), offs.ctypes.data_as(C.c_void_p),
+                                                           width, ids.ctypes.data_as(C.c_void_p), cnt.ctypes.data_as(C.c_void_p))
+            if rc == 0:
+                for j, i in enumerate(idx):
+                    out[i] = ids[j, 1: cnt[j] - 1].copy()
+        for i, t in enumerate(texts):
+            if out[i] is None:
+                out[i] = np.asarray([k for w in self._basic(t) for k in self._wordpiece(w)], np.int32)
+        return out
+
     def encode_batch(self, texts: list[str]) -> list[list[int]]:
         """ids of every text; ASCII texts go through the native, multi-threaded encoder in one call, the rest through encode_py"""
         out: list = [None] * len(texts)

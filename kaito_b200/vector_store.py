@@ -140,6 +140,24 @@ class _IndexState:
         self.n_dead = 0                          # tombstoned nodes still in `nodes` (and rows in the engine)
         self._filter_cache: dict[str, tuple[int, np.ndarray]] = {}   # filter json -> (nodes covered, allow bitmap)
         self._frag_cache: dict[int, tuple[bytes, bytes]] = {}        # ordinal -> serialised halves of its NodeWithScore
+        self._pair_cache: dict[int, tuple] = {}                      # ordinal -> its cross-encoder tokens (ids, full length)
+
+    def pair_passages(self, ordinals, encode) -> list[tuple]:
+        """the cross-encoder tokens of nodes `ordinals` (embed_text of each, as the embedder saw it): cached per ordinal,
+        misses tokenised in one `encode` call.  Two dispatcher threads may fill the cache at once under the store's reader
+        lock: nodes are immutable and the tokeniser deterministic, so both compute the same entry, and a dict item assignment
+        is atomic under the GIL -- the worst case is a node tokenised twice.  Compaction renumbers ordinals under the writer
+        lock and clears the cache there."""
+        cache = self._pair_cache
+        got = [cache.get(int(o)) for o in ordinals]
+        miss = [j for j, g in enumerate(got) if g is None]
+        if miss:
+            if len(cache) >= 1 << 20:
+                cache.clear()
+            fresh = encode([embed_text(self.nodes[int(ordinals[j])].text, self.nodes[int(ordinals[j])].metadata) for j in miss])
+            for j, f in zip(miss, fresh):
+                got[j] = cache[int(ordinals[j])] = f
+        return got
 
     def node_fragments(self, o: int) -> tuple[bytes, bytes]:
         """the JSON of node `o` as a /retrieve result, minus the score: (b'{"doc_id":..,"node_id":..,"text":..,"score":',
@@ -185,7 +203,7 @@ class HybridRetriever:
 
     def __init__(self, state: _IndexState, embed_model, max_results: int = 10, candidate_multiplier: float = 3.0,
                  vector_weight: float = 0.7, text_weight: float = 0.3, metadata_filter: dict | None = None,
-                 filter_pushdown: bool = False):
+                 filter_pushdown: bool = False, reranker=None, rerank_top_k: int | None = None):
         total = vector_weight + text_weight
         self._vector_weight = vector_weight / total
         self._text_weight = text_weight / total
@@ -199,6 +217,9 @@ class HybridRetriever:
         self._filter_pushdown = filter_pushdown
         self.want_components = True          # VectorStore turns this off unless KRAG_COMPONENT_SCORES=1 (saves 10 dicts per query)
         self.last_components: list[dict] = []
+        # cross-encoder (kaito_b200.rerank.GpuCrossEncoder or None): the fused max_results candidates are rescored and the
+        # rerank_top_k best kept
+        self._reranker, self._rerank_top_k = reranker, rerank_top_k
 
     def _allow_bitmap(self):
         if not self._metadata_filter:
@@ -242,15 +263,40 @@ class HybridRetriever:
                                 vector_weight=self._vector_weight, text_weight=self._text_weight,
                                 fusion_mode=FILTER_PUSHDOWN if (self._filter_pushdown and allow is not None) else 0,
                                 keyword_allow_bitmap=allow)
+        if self._reranker is not None:
+            out = self._rerank(queries, out)
         return out
+
+    def _rerank(self, queries: list[str], out: dict) -> dict:
+        """the engine's arrays cut to the rerank_top_k fused candidates the cross-encoder scores highest, in that order
+        (equal scores: fused position ascending); "final" becomes the cross-encoder score, "dense" / "sparse" follow their
+        candidates (they describe the fusion stage)"""
+        counts = np.asarray(out["count"])
+        cands = [np.asarray(out["ordinal"][b, :int(counts[b])]) for b in range(len(queries))]
+        k = self._rerank_top_k
+        pos, score = self._reranker.rerank(queries, cands, k, self._state.pair_passages)
+        pos = np.asarray(pos, np.int64)
+        valid = pos >= 0
+        take = np.where(valid, pos, 0)
+        res = {"count": np.minimum(counts, k).astype(counts.dtype),
+               "ordinal": np.where(valid, np.take_along_axis(np.asarray(out["ordinal"]), take, 1), -1),
+               "final": np.where(valid, np.asarray(score, np.float64), 0.0)}
+        for key in ("dense", "sparse"):
+            if key in out:
+                res[key] = np.where(valid, np.take_along_axis(np.asarray(out[key]), take, 1), np.nan)
+        return res
 
 
 class VectorStore:
     """BaseVectorStore + FaissVectorStoreHandler over the CUDA engine."""
 
-    def __init__(self, embed_model, engine):
+    def __init__(self, embed_model, engine, reranker=None):
         self.embed_model = embed_model
         self.engine = engine
+        # optional cross-encoder (KRAG_RERANK_MODEL_DIR): /retrieve fuses N = min(max(top_k, KRAG_RERANK_CANDIDATES),
+        # RAG_MAX_TOP_K) candidates and returns the top_k the cross-encoder scores highest
+        self.reranker = reranker
+        self.rerank_candidates = int(os.getenv("KRAG_RERANK_CANDIDATES", "30"))
         self.dimension = embed_model.get_embedding_dimension()   # faiss_store.py:28
         self.index_map: dict[str, _IndexState] = {}
         self.splitter = SentenceSplitter()
@@ -362,10 +408,20 @@ class VectorStore:
         for rec in st.ref_docs.values():
             rec["nodes"] = [remap[o] for o in rec["nodes"]]
         st.n_dead = 0
-        st._frag_cache.clear()           # both caches are keyed by ordinal
+        st._frag_cache.clear()           # these caches are keyed by ordinal
+        st._pair_cache.clear()
         st._filter_cache.clear()
 
     # --------------------------------------------------------------- /retrieve
+    def _retriever(self, st: _IndexState, top_k: int, metadata_filter: dict | None) -> HybridRetriever:
+        """the retriever every /retrieve path uses: top_k fused results, or with a reranker N fused candidates cut to top_k"""
+        if self.reranker is None:
+            return HybridRetriever(st, self.embed_model, max_results=top_k, metadata_filter=metadata_filter,
+                                   filter_pushdown=self.filter_pushdown)
+        n = min(max(top_k, self.rerank_candidates), RAG_MAX_TOP_K)
+        return HybridRetriever(st, self.embed_model, max_results=n, metadata_filter=metadata_filter,
+                               filter_pushdown=self.filter_pushdown, reranker=self.reranker, rerank_top_k=top_k)
+
     def retrieve(self, index_name: str, query: str, max_node_count: int = 5, metadata_filter: dict | None = None):
         """base.py:870-978."""
         if index_name not in self.index_map:
@@ -375,8 +431,7 @@ class VectorStore:
                 raise HTTPException(400, "Query string cannot be empty.")
             top_k = min(max_node_count, RAG_MAX_TOP_K)
             st = self.index_map[index_name]
-            retriever = HybridRetriever(st, self.embed_model, max_results=top_k, metadata_filter=metadata_filter,
-                                        filter_pushdown=self.filter_pushdown)
+            retriever = self._retriever(st, top_k, metadata_filter)
             t0 = time.time()
             with self._rw.reader():         # base.py:917-919: reader lock around the retrieval
                 nodes = retriever.retrieve(query)
@@ -408,8 +463,7 @@ class VectorStore:
             t0 = time.time()
             with self._rw.reader():
                 st = self.index_map[index_name]
-                retriever = HybridRetriever(st, self.embed_model, max_results=top_k, metadata_filter=metadata_filter,
-                                            filter_pushdown=self.filter_pushdown)
+                retriever = self._retriever(st, top_k, metadata_filter)
                 retriever.want_components = self.component_scores
                 nodes, comps = retriever.retrieve_batch([queries[i] for i in live])
                 for j, i in enumerate(live):
@@ -454,8 +508,7 @@ class VectorStore:
             t0 = time.time()
             with self._rw.reader():
                 st = self.index_map[index_name]
-                retriever = HybridRetriever(st, self.embed_model, max_results=top_k, metadata_filter=metadata_filter,
-                                            filter_pushdown=self.filter_pushdown)
+                retriever = self._retriever(st, top_k, metadata_filter)
                 out = retriever.retrieve_batch_raw([queries[i] for i in live])
                 counts, ords, finals = out["count"].tolist(), out["ordinal"].tolist(), out["final"].tolist()
                 frag = st.node_fragments
