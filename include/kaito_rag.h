@@ -297,6 +297,8 @@ typedef struct krag_bert_config {
 } krag_bert_config;
 int32_t krag_embedder_create(krag_ctx* ctx, const krag_bert_config* cfg, krag_embedder** out);
 int32_t krag_embedder_load_tensor(krag_embedder* e, const char* name, const float* data, int64_t n_elems);
+/* KRAG_E_INVALID, naming the tensor, when one is missing or its element count is not the config's (word table
+ * vocab * hidden, position table max_position * hidden, token-type table type_vocab * hidden, ...) */
 int32_t krag_embedder_finalize(krag_embedder* e);
 /* tok_ids: packed token ids of all sequences ([CLS] ... [SEP] each); tok_offsets [batch+1]; out [batch, hidden] */
 int32_t krag_embed(krag_embedder* e, int32_t batch, const int32_t* tok_ids, const int32_t* tok_offsets, float* out);

@@ -1002,11 +1002,15 @@ struct Embedder {
     }
 };
 
+// the device copy of a loaded tensor, which must hold exactly n elements: the kernels index it by the config's sizes
+// (embed_ln_kernel clamps token ids to cfg.vocab, not to the rows uploaded)
 static float* emb_get(Embedder* e, const std::string& name, int64_t n)
 {
     auto it = e->t.find(name);
     if (it == e->t.end() || it->second.p == nullptr) throw std::runtime_error("embedder: tensor not loaded: " + name);
-    (void)n;
+    if (it->second.cap != n)
+        throw std::runtime_error("embedder: " + name + " must hold " + std::to_string(n) + " elements (the config's shape), not " +
+                                 std::to_string(it->second.cap));
     return it->second.p;
 }
 static std::string lname(int l, const char* s) { return "encoder.layer." + std::to_string(l) + "." + s; }
@@ -1047,9 +1051,22 @@ void embedder_finalize(Embedder* e)
     e->bqkv.clear(); e->planes.clear(); e->s_qkv.clear(); e->s_o.clear(); e->s_f1.clear(); e->s_f2.clear();
     e->s_pool = SplitMat{nullptr, nullptr}; e->has_head = false;
     e->drop_graphs(); e->seen.clear();   // captured weight pointers are about to change
-    emb_get(e, "embeddings.word_embeddings.weight", 0); emb_get(e, "embeddings.position_embeddings.weight", 0);
-    emb_get(e, "embeddings.token_type_embeddings.weight", 0); emb_get(e, "embeddings.LayerNorm.weight", 0);
-    emb_get(e, "embeddings.LayerNorm.bias", 0);
+    const BertConfig& c = e->cfg;
+    // every size first: a refused state leaves no half-built planes behind
+    emb_get(e, "embeddings.word_embeddings.weight", (int64_t)c.vocab * d);
+    emb_get(e, "embeddings.position_embeddings.weight", (int64_t)c.max_pos * d);
+    emb_get(e, "embeddings.token_type_embeddings.weight", (int64_t)c.type_vocab * d);
+    emb_get(e, "embeddings.LayerNorm.weight", d); emb_get(e, "embeddings.LayerNorm.bias", d);
+    for (int l = 0; l < c.layers; ++l) {
+        for (const char* nm : {"attention.self.query", "attention.self.key", "attention.self.value", "attention.output.dense"}) {
+            emb_get(e, lname(l, nm) + ".weight", (int64_t)d * d); emb_get(e, lname(l, nm) + ".bias", d);
+        }
+        for (const char* nm : {"attention.output.LayerNorm.weight", "attention.output.LayerNorm.bias", "output.dense.bias",
+                               "output.LayerNorm.weight", "output.LayerNorm.bias"})
+            emb_get(e, lname(l, nm), d);
+        emb_get(e, lname(l, "intermediate.dense.weight"), (int64_t)inter * d); emb_get(e, lname(l, "intermediate.dense.bias"), inter);
+        emb_get(e, lname(l, "output.dense.weight"), (int64_t)d * inter);
+    }
     DevArray<float> wtmp;
     wtmp.alloc((int64_t)3 * d * d);
     for (int l = 0; l < e->cfg.layers; ++l) {
@@ -1057,17 +1074,14 @@ void embedder_finalize(Embedder* e)
         b.alloc((int64_t)3 * d);
         const char* names[3] = {"attention.self.query", "attention.self.key", "attention.self.value"};
         for (int j = 0; j < 3; ++j) {
-            KRAG_CUDA(cudaMemcpyAsync(wtmp.p + (size_t)j * d * d, emb_get(e, lname(l, names[j]) + ".weight", 0), sizeof(float) * (size_t)d * d, cudaMemcpyDeviceToDevice, e->st));
-            KRAG_CUDA(cudaMemcpyAsync(b.p + (size_t)j * d, emb_get(e, lname(l, names[j]) + ".bias", 0), sizeof(float) * (size_t)d, cudaMemcpyDeviceToDevice, e->st));
+            KRAG_CUDA(cudaMemcpyAsync(wtmp.p + (size_t)j * d * d, emb_get(e, lname(l, names[j]) + ".weight", (int64_t)d * d), sizeof(float) * (size_t)d * d, cudaMemcpyDeviceToDevice, e->st));
+            KRAG_CUDA(cudaMemcpyAsync(b.p + (size_t)j * d, emb_get(e, lname(l, names[j]) + ".bias", d), sizeof(float) * (size_t)d, cudaMemcpyDeviceToDevice, e->st));
         }
         e->bqkv.push_back(std::move(b));
         e->s_qkv.push_back(emb_split_weight(e, wtmp.p, (size_t)3 * d * d));       // stream order: the split reads wtmp before the next layer overwrites it
-        for (const char* nm : {"attention.output.dense.bias", "attention.output.LayerNorm.weight", "attention.output.LayerNorm.bias",
-                               "intermediate.dense.bias", "output.dense.bias", "output.LayerNorm.weight", "output.LayerNorm.bias"})
-            emb_get(e, lname(l, nm), 0);
-        e->s_o.push_back(emb_split_weight(e, emb_get(e, lname(l, "attention.output.dense.weight"), 0), (size_t)d * d));
-        e->s_f1.push_back(emb_split_weight(e, emb_get(e, lname(l, "intermediate.dense.weight"), 0), (size_t)inter * d));
-        e->s_f2.push_back(emb_split_weight(e, emb_get(e, lname(l, "output.dense.weight"), 0), (size_t)d * inter));
+        e->s_o.push_back(emb_split_weight(e, emb_get(e, lname(l, "attention.output.dense.weight"), (int64_t)d * d), (size_t)d * d));
+        e->s_f1.push_back(emb_split_weight(e, emb_get(e, lname(l, "intermediate.dense.weight"), (int64_t)inter * d), (size_t)inter * d));
+        e->s_f2.push_back(emb_split_weight(e, emb_get(e, lname(l, "output.dense.weight"), (int64_t)d * inter), (size_t)d * inter));
     }
     // the classifier head of a cross-encoder (BertForSequenceClassification, one label): all four tensors or none
     const char* head[4] = {"pooler.dense.weight", "pooler.dense.bias", "classifier.weight", "classifier.bias"};
@@ -1082,7 +1096,7 @@ void embedder_finalize(Embedder* e)
     }
     if (n_head != 0 && n_head != 4) throw std::runtime_error("embedder: the classifier head needs pooler.dense.{weight,bias} and classifier.{weight,bias}");
     if (n_head == 4) {
-        e->s_pool = emb_split_weight(e, emb_get(e, "pooler.dense.weight", 0), (size_t)d * d);
+        e->s_pool = emb_split_weight(e, emb_get(e, "pooler.dense.weight", (int64_t)d * d), (size_t)d * d);
         e->has_head = true;
     }
     KRAG_CUDA(cudaStreamSynchronize(e->st));
@@ -1151,7 +1165,7 @@ static bool encoder_forward(Embedder* e, int batch, const int32_t* tok_ids, cons
     cudaStream_t st = e->st;
     int max_len = 0;
     std::vector<int32_t> pos((size_t)n_tok), typ(seg_b ? (size_t)n_tok : 0);
-    if (seg_b && (c.type_vocab < 2 || e->t["embeddings.token_type_embeddings.weight"].cap < 2 * (int64_t)d))
+    if (seg_b && c.type_vocab < 2)          // finalize: the token type table holds type_vocab rows
         throw std::runtime_error("embedder: sentence pairs need token type row 1 (type_vocab_size >= 2)");
     for (int b = 0; b < batch; ++b) {
         const int len = tok_offsets[b + 1] - tok_offsets[b];

@@ -1,5 +1,5 @@
-"""fp64 reference of the K5 forward (BERT encoder, CLS pooling, L2 normalisation) and the yardstick its error is judged by.
-Test infrastructure only.
+"""fp64 reference of the K5 forward (BERT encoder, CLS or mean pooling, L2 normalisation; the cross-encoder's pooler and
+classifier head) and the yardstick its error is judged by.  Test infrastructure only.
 
 K5 packs sequences without padding, so the reference runs transformers.BertModel in fp64 (eager attention) on each
 sequence alone.  Sequences are independent, so a test checks a sample of a batch: `sample()` keeps the first and last
@@ -120,9 +120,20 @@ class Fp64Bert:
         return self._embed(self.m64, token_lists)
 
     def embed_fp32(self, token_lists):
+        return self._embed(self._fp32(), token_lists)
+
+    def _fp32(self):
         if self._m32 is None:
             self._m32 = copy.deepcopy(self.m64).float()
-        return self._embed(self._m32, token_lists)
+        return self._m32
+
+    def pooled(self, token_lists):
+        """(CLS fp64, mean fp64, CLS fp32, mean fp32, largest Linear operand of the fp64 forwards) of each sequence run
+        alone: one forward per sequence and precision gives both poolings"""
+        self.range_max = 0.0
+        c64, m64 = _pools(self.m64, token_lists)
+        c32, m32 = _pools(self._fp32(), token_lists)
+        return c64, m64, c32, m32, self.range_max
 
     def embed_padded(self, token_lists):
         """fp64, all sequences in one zero-padded batch with an attention mask (checks that running them alone is the same)"""
@@ -157,6 +168,69 @@ class Fp64Bert:
             enc.layer = layers
             hq.remove(); hk.remove()
         return float(torch.cat(scores).std())
+
+
+def _pools(model, token_lists):
+    """(CLS rows, token means) of last_hidden_state, each x / max(|x|, 1e-12) in the model's precision"""
+    import torch
+    cls, mean = [], []
+    with torch.no_grad():
+        for t in token_lists:
+            h = model(input_ids=torch.tensor(np.asarray(t, np.int64)[None])).last_hidden_state[0].numpy()
+            m = h.mean(axis=0)
+            cls.append(h[0] / max(np.linalg.norm(h[0]), 1e-12))
+            mean.append(m / max(np.linalg.norm(m), 1e-12))
+    return np.stack(cls).astype(np.float64), np.stack(mean).astype(np.float64)
+
+
+def mean_pool(model, token_lists):
+    """mean of last_hidden_state over every token ([CLS] and [SEP] included), then x / max(|x|, 1e-12), in the model's
+    precision: sentence-transformers' mean pooling and Normalize"""
+    return _pools(model, token_lists)[1]
+
+
+def head_state(cfg, state, seed):
+    """state + the head of a one-label BertForSequenceClassification: pooler N(0, 0.06) / N(0, 0.05), classifier
+    N(0, 0.06) / N(0, 0.05)"""
+    g = np.random.default_rng(seed + 77)
+    d = cfg["hidden_size"]
+    st = dict(state)
+    st["pooler.dense.weight"] = (0.06 * g.standard_normal((d, d))).astype(np.float32)
+    st["pooler.dense.bias"] = (0.05 * g.standard_normal(d)).astype(np.float32)
+    st["classifier.weight"] = (0.06 * g.standard_normal((1, d))).astype(np.float32)
+    st["classifier.bias"] = (0.05 * g.standard_normal(1)).astype(np.float32)
+    return st
+
+
+class Fp64CrossEncoder:
+    """transformers.BertForSequenceClassification (one label, eager attention) in fp64 and its fp32 twin"""
+
+    def __init__(self, cfg, state):
+        import torch
+        from transformers import BertConfig, BertForSequenceClassification
+        from transformers.initialization import no_init_weights
+        with no_init_weights():
+            m = BertForSequenceClassification(BertConfig(**cfg, num_labels=1, attn_implementation="eager"))
+        m = m.double().eval()
+        sd = {(k if k.startswith("classifier.") else "bert." + k): torch.from_numpy(np.asarray(v, np.float64)) for k, v in state.items()}
+        missing, _ = m.load_state_dict(sd, strict=False)
+        assert not [k for k in missing if not k.endswith("position_ids")], missing
+        self.m64, self.m32 = m, copy.deepcopy(m).float()
+
+    @staticmethod
+    def _logits(m, pairs):
+        import torch
+        out = []
+        with torch.no_grad():
+            for ids, seg in pairs:
+                tt = (np.arange(len(ids)) >= seg).astype(np.int64)
+                out.append(float(m(input_ids=torch.tensor(np.asarray(ids, np.int64)[None]),
+                                   token_type_ids=torch.tensor(tt[None])).logits[0, 0]))
+        return np.asarray(out, np.float64)
+
+    def logits(self, pairs):
+        """(fp64 logits, fp32 logits) of (token ids, index of the first segment-B token) pairs, each run alone"""
+        return self._logits(self.m64, pairs), self._logits(self.m32, pairs)
 
 
 def check_range(range_max):

@@ -25,18 +25,6 @@ MODELS = {   # BertConfig of the sentence-transformers checkpoints (random weigh
 REGIMES = ["bench", "stressed"]
 
 
-def _mean_pool(model, toks):
-    """mean of last_hidden_state over every token, then x / max(|x|, 1e-12), in the model's precision"""
-    import torch
-    out = []
-    with torch.no_grad():
-        for t in toks:
-            h = model(input_ids=torch.tensor(np.asarray(t, np.int64)[None])).last_hidden_state[0].numpy()
-            m = h.mean(axis=0)
-            out.append(m / max(np.linalg.norm(m), 1e-12))
-    return np.stack(out).astype(np.float64)
-
-
 class MeanRef:
     """the fp64 BertModel of bert_reference (its Linear range hooks included) and its fp32 twin, mean-pooled"""
 
@@ -48,7 +36,7 @@ class MeanRef:
         if self._m32 is None:
             self._m32 = br.Fp64Bert(self.cfg, self.state).m64.float()
         self.ref.range_max = 0.0
-        return _mean_pool(self.ref.m64, toks), _mean_pool(self._m32, toks), self.ref.range_max
+        return br.mean_pool(self.ref.m64, toks), br.mean_pool(self._m32, toks), self.ref.range_max
 
 
 def _setup(ctx, model, regime, seed=0):
@@ -256,16 +244,16 @@ def test_vector_store_retrieve_on_minilm_snapshot(ctx, tmp_path, monkeypatch):
         store.index_documents("pooling_e2e", docs)
         enc = ge.tokenizer.encode_batch
         for q in queries:
-            q64 = _mean_pool(ref.m64, enc([q]))[0]
+            q64 = br.mean_pool(ref.m64, enc([q]))[0]
             res = store.retrieve("pooling_e2e", q, max_node_count=10)["results"]
             dense = [r for r in res if r["dense_score"] is not None]
             assert dense, q
-            d64 = _mean_pool(ref.m64, enc([r["text"] for r in dense]))
+            d64 = br.mean_pool(ref.m64, enc([r["text"] for r in dense]))
             l2 = ((d64 - q64) ** 2).sum(1)
             assert np.abs(np.array([r["dense_score"] for r in dense]) - l2).max() < 1e-4, q
             ranked = store.dense_candidates("pooling_e2e", q, len(docs))
             assert len(ranked) == len(docs)
-            r64 = ((_mean_pool(ref.m64, enc([n.text for n, _ in ranked])) - q64) ** 2).sum(1)
+            r64 = ((br.mean_pool(ref.m64, enc([n.text for n, _ in ranked])) - q64) ** 2).sum(1)
             assert np.abs(np.array([s for _, s in ranked]) - r64).max() < 1e-4, q
             assert (np.diff(r64) > -1e-4).all(), (q, np.diff(r64).min())
     finally:

@@ -2,8 +2,6 @@
 Logits are held to an fp64 transformers.BertForSequenceClassification run on each pair alone, by the rule of
 test_gpu_embed.py: the error is at most F = 40 times torch fp32's own error against fp64, and the sigmoid score moves by at
 most 1e-4.  Random weights (no checkpoints offline): bert_reference's generators plus a pooler and a one-label classifier."""
-import copy
-
 import numpy as np
 import pytest
 
@@ -23,52 +21,10 @@ CE_MODELS = {   # BertConfig of the cross-encoder checkpoints
 }
 
 
-def _head(cfg, state, seed):
-    """state + pooler N(0, 0.06) / N(0, 0.05) and a one-label classifier N(0, 0.06) / N(0, 0.05)"""
-    g = np.random.default_rng(seed + 77)
-    d = cfg["hidden_size"]
-    st = dict(state)
-    st["pooler.dense.weight"] = (0.06 * g.standard_normal((d, d))).astype(np.float32)
-    st["pooler.dense.bias"] = (0.05 * g.standard_normal(d)).astype(np.float32)
-    st["classifier.weight"] = (0.06 * g.standard_normal((1, d))).astype(np.float32)
-    st["classifier.bias"] = (0.05 * g.standard_normal(1)).astype(np.float32)
-    return st
-
-
 def _state(cfg, regime, seed=0):
     import bench
     st = br.stressed_state(cfg, seed)[0] if regime == "stressed" else bench.random_bert_state(cfg, seed)
-    return _head(cfg, st, seed)
-
-
-class Fp64CrossEncoder:
-    """transformers.BertForSequenceClassification (one label, eager attention) in fp64 and its fp32 twin"""
-
-    def __init__(self, cfg, state):
-        import torch
-        from transformers import BertConfig, BertForSequenceClassification
-        from transformers.initialization import no_init_weights
-        with no_init_weights():
-            m = BertForSequenceClassification(BertConfig(**cfg, num_labels=1, attn_implementation="eager"))
-        m = m.double().eval()
-        sd = {(k if k.startswith("classifier.") else "bert." + k): torch.from_numpy(np.asarray(v, np.float64)) for k, v in state.items()}
-        missing, _ = m.load_state_dict(sd, strict=False)
-        assert not [k for k in missing if not k.endswith("position_ids")], missing
-        self.m64, self.m32 = m, copy.deepcopy(m).float()
-
-    @staticmethod
-    def _logits(m, pairs):
-        import torch
-        out = []
-        with torch.no_grad():
-            for ids, seg in pairs:
-                tt = (np.arange(len(ids)) >= seg).astype(np.int64)
-                out.append(float(m(input_ids=torch.tensor(np.asarray(ids, np.int64)[None]),
-                                   token_type_ids=torch.tensor(tt[None])).logits[0, 0]))
-        return np.asarray(out, np.float64)
-
-    def logits(self, pairs):
-        return self._logits(self.m64, pairs), self._logits(self.m32, pairs)
+    return br.head_state(cfg, st, seed)
 
 
 def _encoder(ctx, cfg, state):
@@ -132,7 +88,7 @@ def test_logits_match_fp64(ctx, model, regime):
     n = len(lens)
     idx = sorted(set(br.sample(lens.tolist(), 12 if model == "base" else 20).tolist()) | {n - 1, n - 2, n - 6}
                  | set(np.flatnonzero(lens == 512)[:2].tolist()))
-    ref = Fp64CrossEncoder(cfg, state)
+    ref = br.Fp64CrossEncoder(cfg, state)
     l64, l32 = ref.logits(_pairs_of(flat, toff, seg, idx))
     got = logit[idx].astype(np.float64)
     k5, t32 = float(np.abs(got - l64).max()), float(np.abs(l32 - l64).max())
@@ -226,7 +182,7 @@ def test_from_pretrained_and_store_retrieve(ctx, tmp_path):
     plain = VectorStore(HashingEmbedding(384), ctx)
     rr = VectorStore(HashingEmbedding(384), ctx, reranker=ce)
     plain.index_documents("ce_plain", docs); rr.index_documents("ce_rr", docs)
-    ref = Fp64CrossEncoder(cfg, state)
+    ref = br.Fp64CrossEncoder(cfg, state)
     for query in ("quick brown fox", "gpu token search passage"):
         got = rr.retrieve("ce_rr", query, max_node_count=10)
         fused = plain.retrieve("ce_plain", query, max_node_count=30)["results"]
