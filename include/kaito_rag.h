@@ -313,6 +313,17 @@ int32_t krag_embed_dev(krag_embedder* e, int32_t batch, const int32_t* tok_ids, 
 #define KRAG_POOL_CLS 0
 #define KRAG_POOL_MEAN 1
 int32_t krag_embedder_set_pooling(krag_embedder* e, int32_t mode);
+/* Arithmetic of the encoder's GEMM and attention products, for every forward of this embedder (krag_embed, krag_embed_dev,
+ * krag_rerank).  KRAG_PRECISION_FP32 (default): split-fp16 operands, three tensor-core products per step, results held to
+ * fp32 arithmetic.  KRAG_PRECISION_FP16: operands rounded to fp16 (round to nearest even, saturating at the largest finite
+ * value), one tensor-core product per step with fp32 accumulation; bias, GELU, the residual stream, LayerNorm, softmax and the
+ * classifier head stay fp32.  Meant for cross-encoder scores, which are only compared with each other.  Embeddings computed in
+ * fp16 mode are OUTSIDE the 1e-4 score contract of the dense search: a host that stores or queries with them does so
+ * knowingly.  The weights are shared by both modes (no second copy).  May be called before or after finalize and between
+ * forwards; any other mode is KRAG_E_INVALID. */
+#define KRAG_PRECISION_FP32 0
+#define KRAG_PRECISION_FP16 1
+int32_t krag_embedder_set_precision(krag_embedder* e, int32_t mode);
 /* Under CLS pooling the last layer's O projection, FFN and LayerNorms run on the [CLS] rows only (on = 1, the default).
  * on = 0 runs them over every token; the embeddings are the same bits either way.  Test hook. */
 int32_t krag_debug_embedder_cls_rows(krag_embedder* e, int32_t on);
@@ -356,6 +367,11 @@ int32_t krag_wordpiece_destroy(krag_wordpiece* w);
 int32_t krag_debug_gemm_tf32(krag_ctx* ctx, int32_t M, int32_t N, int32_t K, const float* A, const float* B,
                              const float* bias, const float* residual, int32_t gelu, float* C_out, int32_t tile_n,
                              int32_t reps, float* ms_out);
+/* The same through the single-plane fp16 GEMM of KRAG_PRECISION_FP16: A and B are rounded to fp16, one wgmma per step, fp32
+ * accumulation and epilogue.  tile_n may also be 256 (N % 256 == 0).  Test and probe hook. */
+int32_t krag_debug_gemm_f16(krag_ctx* ctx, int32_t M, int32_t N, int32_t K, const float* A, const float* B,
+                            const float* bias, const float* residual, int32_t gelu, float* C_out, int32_t tile_n,
+                            int32_t reps, float* ms_out);
 /* Y = LayerNorm(A . B^T + bias (+residual)) * gamma + beta through K5's linear-layer dispatcher (for a handful of rows:
  * 128 x 32 split-K tiles + the reduce/LayerNorm kernel).  Test hook. */
 int32_t krag_debug_linear_ln(krag_ctx* ctx, int32_t M, int32_t N, int32_t K, const float* A, const float* B,

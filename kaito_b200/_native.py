@@ -40,8 +40,10 @@ SYMBOLS = [
     "krag_host_pinned_bytes", "krag_host_rows_fetched", "krag_index_compact", "krag_last_compact",
     "krag_last_commit", "krag_index_alive_bitmap", "krag_redeal_begin", "krag_redeal_tables", "krag_redeal_prepare",
     "krag_dev_redeal_pack", "krag_dev_redeal_unpack", "krag_redeal_finish", "krag_redeal_abort", "krag_embedder_set_pooling",
-    "krag_debug_embedder_cls_rows", "krag_rerank",
+    "krag_debug_embedder_cls_rows", "krag_rerank", "krag_embedder_set_precision", "krag_debug_gemm_f16",
 ]
+# krag_embedder_set_precision: split-fp16 products held to fp32 arithmetic, or fp16 operands with fp32 accumulation
+PRECISIONS = {"fp32": 0, "fp16": 1}
 RERANK_SIGMOID, RERANK_IDENTITY = 0, 1   # krag_rerank: activation of the classifier logit
 
 
@@ -131,9 +133,11 @@ def load() -> C.CDLL:
     L.krag_embed_dev.argtypes = [vp, i32, vp, vp, vp, i32, vp]
     L.krag_embedder_set_pooling.argtypes = [vp, i32]
     L.krag_debug_embedder_cls_rows.argtypes = [vp, i32]
+    L.krag_embedder_set_precision.argtypes = [vp, i32]
     L.krag_rerank.argtypes = [vp, i32, vp, vp, vp, vp, i32, i32, vp, vp]
     L.krag_embedder_destroy.argtypes = [vp]
     L.krag_debug_gemm_tf32.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp, i32, vp, i32, i32, C.POINTER(C.c_float)]
+    L.krag_debug_gemm_f16.argtypes = L.krag_debug_gemm_tf32.argtypes
     L.krag_debug_linear_ln.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, C.c_float, vp]
     L.krag_index_set_dense_mode.argtypes = [vp, i32, i32]
     L.krag_text_analyze.argtypes = [C.c_char_p, i64, vp, i64, C.POINTER(i64), C.POINTER(i32)]
@@ -340,6 +344,12 @@ class Embedder:
         """POOL_CLS (default) or POOL_MEAN for the following forwards"""
         check(self._L.krag_embedder_set_pooling(self._h, mode))
 
+    def set_precision(self, precision: str):
+        """"fp32" (default) or "fp16" for the following forwards (krag_embedder_set_precision)"""
+        if precision not in PRECISIONS:
+            raise ValueError(f"precision {precision!r}: expected 'fp32' or 'fp16'")
+        check(self._L.krag_embedder_set_precision(self._h, PRECISIONS[precision]))
+
     def rerank(self, pair_offsets, flat_tokens, tok_offsets, seg_b, top_k: int, activation: int = RERANK_SIGMOID):
         """krag_rerank: (positions int32 [n_queries, top_k], scores float32 [n_queries, top_k]); -1 / NaN past a query's
         pair count"""
@@ -368,20 +378,25 @@ def debug_gemm_tf32(ctx: "Context", A, B, bias, residual=None, gelu=False, tile_
     return _debug_gemm(ctx, A, B, bias, residual, gelu, tile_n, 0)[0]
 
 
-def debug_gemm_time(ctx: "Context", A, B, bias, residual=None, gelu=False, tile_n=0, reps=50):
-    """(C, mean ms of one GEMM launch over `reps` launches on the device operands)"""
-    return _debug_gemm(ctx, A, B, bias, residual, gelu, tile_n, reps)
+def debug_gemm_f16(ctx: "Context", A, B, bias, residual=None, gelu=False, tile_n=0) -> np.ndarray:
+    """the single-plane fp16 GEMM of the fp16 precision mode (A and B rounded to fp16, fp32 accumulation); tile_n as above, or 256"""
+    return _debug_gemm(ctx, A, B, bias, residual, gelu, tile_n, 0, "krag_debug_gemm_f16")[0]
 
 
-def _debug_gemm(ctx, A, B, bias, residual, gelu, tile_n, reps):
+def debug_gemm_time(ctx: "Context", A, B, bias, residual=None, gelu=False, tile_n=0, reps=50, f16=False):
+    """(C, mean ms of one GEMM launch over `reps` launches on the device operands); f16: the single-plane fp16 GEMM"""
+    return _debug_gemm(ctx, A, B, bias, residual, gelu, tile_n, reps, "krag_debug_gemm_f16" if f16 else "krag_debug_gemm_tf32")
+
+
+def _debug_gemm(ctx, A, B, bias, residual, gelu, tile_n, reps, fn="krag_debug_gemm_tf32"):
     A = np.ascontiguousarray(A, np.float32); B = np.ascontiguousarray(B, np.float32)
     bias = np.ascontiguousarray(bias, np.float32)
     if residual is not None:
         residual = np.ascontiguousarray(residual, np.float32)
     out = np.empty((A.shape[0], B.shape[0]), np.float32)
     ms = C.c_float(0.0)
-    check(load().krag_debug_gemm_tf32(ctx._h, A.shape[0], B.shape[0], A.shape[1], ptr(A), ptr(B), ptr(bias), ptr(residual),
-                                      1 if gelu else 0, ptr(out), int(tile_n), int(reps), C.byref(ms)))
+    check(getattr(load(), fn)(ctx._h, A.shape[0], B.shape[0], A.shape[1], ptr(A), ptr(B), ptr(bias), ptr(residual),
+                              1 if gelu else 0, ptr(out), int(tile_n), int(reps), C.byref(ms)))
     return out, float(ms.value)
 
 

@@ -1677,6 +1677,16 @@ int32_t krag_embedder_set_pooling(krag_embedder* h, int32_t mode)
         embedder_set_pooling(h->e, mode);
     });
 }
+static_assert(KRAG_PRECISION_FP32 == EMB_PREC_FP32 && KRAG_PRECISION_FP16 == EMB_PREC_FP16, "precision modes");
+int32_t krag_embedder_set_precision(krag_embedder* h, int32_t mode)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(h, KRAG_E_INVALID, "null embedder");
+        KRAG_REQUIRE(mode == KRAG_PRECISION_FP32 || mode == KRAG_PRECISION_FP16, KRAG_E_INVALID,
+                     "precision must be KRAG_PRECISION_FP32 or KRAG_PRECISION_FP16");
+        embedder_set_precision(h->e, mode);
+    });
+}
 int32_t krag_debug_embedder_cls_rows(krag_embedder* h, int32_t on)
 {
     return guarded([&] {
@@ -1706,11 +1716,12 @@ int32_t krag_embedder_destroy(krag_embedder* h)
 }
 static void debug_linear(krag_ctx* c, int32_t M, int32_t N, int32_t K, const float* A, const float* B, const float* bias,
                          const float* residual, int32_t gelu, const float* ln_g, const float* ln_b, float eps, float* out,
-                         int32_t tile_n = 0, int32_t reps = 0, float* ms = nullptr)
+                         int32_t tile_n = 0, int32_t reps = 0, float* ms = nullptr, int planes = 2)
 {
     KRAG_REQUIRE(c && A && B && bias && out && M >= 1 && N % 128 == 0 && K % 64 == 0, KRAG_E_INVALID, "bad argument (N % 128, K % 64)");
-    KRAG_REQUIRE((tile_n == 0 || tile_n == 32 || tile_n == 64 || tile_n == 128) && reps >= 0 && (reps == 0 || ms), KRAG_E_INVALID,
-                 "bad tile width (0, 32, 64 or 128) or repeat count");
+    KRAG_REQUIRE((tile_n == 0 || tile_n == 32 || tile_n == 64 || tile_n == 128 || (tile_n == 256 && planes == 1 && N % 256 == 0)) &&
+                     reps >= 0 && (reps == 0 || ms),
+                 KRAG_E_INVALID, "bad tile width (0, 32, 64 or 128; 256 for the fp16 GEMM with N % 256 == 0) or repeat count");
     KRAG_CUDA(cudaSetDevice(c->di.device));
     DevArray<float> dA, dB, db, dr, dC, dY, dg, dlb, ws;
     const size_t ws_floats = (size_t)4 << 20;
@@ -1722,7 +1733,7 @@ static void debug_linear(krag_ctx* c, int32_t M, int32_t N, int32_t K, const flo
         dg.alloc(N); dlb.alloc(N); dY.alloc((int64_t)M * N);
         KRAG_CUDA(cudaMemcpy(dg.p, ln_g, 4 * (size_t)N, cudaMemcpyHostToDevice)); KRAG_CUDA(cudaMemcpy(dlb.p, ln_b, 4 * (size_t)N, cudaMemcpyHostToDevice));
     }
-    launch_linear_f32(c->di, dA.p, dB.p, M, N, K, db.p, dr.p, gelu != 0, dC.p, dg.p, dlb.p, eps, dY.p, ws.p, ws_floats, c->admin, tile_n, reps, ms);
+    launch_linear_f32(c->di, dA.p, dB.p, M, N, K, db.p, dr.p, gelu != 0, dC.p, dg.p, dlb.p, eps, dY.p, ws.p, ws_floats, c->admin, tile_n, reps, ms, planes);
     KRAG_CUDA(cudaStreamSynchronize(c->admin));
     KRAG_CUDA(cudaMemcpy(out, ln_g ? dY.p : dC.p, 4 * (size_t)M * N, cudaMemcpyDeviceToHost));
 }
@@ -1731,6 +1742,12 @@ int32_t krag_debug_gemm_tf32(krag_ctx* c, int32_t M, int32_t N, int32_t K, const
                              const float* residual, int32_t gelu, float* C_out, int32_t tile_n, int32_t reps, float* ms_out)
 {
     return guarded([&] { debug_linear(c, M, N, K, A, B, bias, residual, gelu, nullptr, nullptr, 0.f, C_out, tile_n, reps, ms_out); });
+}
+
+int32_t krag_debug_gemm_f16(krag_ctx* c, int32_t M, int32_t N, int32_t K, const float* A, const float* B, const float* bias,
+                            const float* residual, int32_t gelu, float* C_out, int32_t tile_n, int32_t reps, float* ms_out)
+{
+    return guarded([&] { debug_linear(c, M, N, K, A, B, bias, residual, gelu, nullptr, nullptr, 0.f, C_out, tile_n, reps, ms_out, 1); });
 }
 
 int32_t krag_debug_linear_ln(krag_ctx* c, int32_t M, int32_t N, int32_t K, const float* A, const float* B, const float* bias,

@@ -90,6 +90,12 @@ __device__ __forceinline__ void split_store8(const float* o, uint16_t* p_hi, uin
     *reinterpret_cast<uint4*>(p_hi) = make_uint4(a[0], a[1], a[2], a[3]);
     *reinterpret_cast<uint4*>(p_lo) = make_uint4(b[0], b[1], b[2], b[3]);
 }
+// the hi plane alone: the fp16 operand of the single-plane (KRAG_PRECISION_FP16) products
+__device__ __forceinline__ uint32_t hi_pack2(float a, float b) { return (uint32_t)f2h_sat(a) | ((uint32_t)f2h_sat(b) << 16); }
+__device__ __forceinline__ void hi_store8(const float* o, uint16_t* p_hi)
+{
+    *reinterpret_cast<uint4*>(p_hi) = make_uint4(hi_pack2(o[0], o[1]), hi_pack2(o[2], o[3]), hi_pack2(o[4], o[5]), hi_pack2(o[6], o[7]));
+}
 __global__ void __launch_bounds__(256)
 split_f16_kernel(const float* __restrict__ in, uint16_t* __restrict__ hi, uint16_t* __restrict__ lo, int64_t n8)
 {
@@ -113,10 +119,13 @@ void launch_split_f16(const float* in, uint16_t* hi, uint16_t* lo, int64_t n, cu
 struct GemmOut {
     float* c;            // [M, N] fp32 or null
     uint16_t* hi;        // [M, N] split planes or null
-    uint16_t* lo;
+    uint16_t* lo;        // PLANES == 1: not written
 };
 
-template <int BN>
+// PLANES == 2: the split product above.  PLANES == 1 (KRAG_PRECISION_FP16): the operands are the hi planes alone, fp16(v); a
+// stage holds hi_A and hi_B (half the bytes: the ring is twice as deep), every K = 16 step is ONE wgmma into ONE
+// accumulator (which leaves the registers for 128 x 256 tiles), and the epilogue writes fp32 C and / or the hi plane.
+template <int BN, int PLANES>
 __global__ void __launch_bounds__(GM_THREADS, 1)
 gemm_f16s_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmA2,
                  const __grid_constant__ CUtensorMap tmB1, const __grid_constant__ CUtensorMap tmB2, int M, int N, int splits,
@@ -124,8 +133,9 @@ gemm_f16s_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant
                  int act_gelu, GemmOut out, float* __restrict__ ws)
 {
     constexpr int B_BYTES = BN * 128;                      // one plane of one weight k-block
-    constexpr int STAGE_BYTES = 2 * GM_SLAB + 2 * B_BYTES;
+    constexpr int STAGE_BYTES = PLANES * (GM_SLAB + B_BYTES);
     constexpr int R = BN / 2;                              // accumulators per thread and term
+    constexpr int B_OFF = PLANES * GM_SLAB;                // hi_A (lo_A) hi_B (lo_B)
     extern __shared__ unsigned char gm_smem_raw[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(gm_smem_raw) + 1023) & ~(uintptr_t)1023);
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)n_stages * STAGE_BYTES);
@@ -136,7 +146,8 @@ gemm_f16s_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant
     const int total = m_tiles * n_tiles * splits;
 
     if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tmA1); tma_prefetch_desc(&tmA2); tma_prefetch_desc(&tmB1); tma_prefetch_desc(&tmB2);
+        tma_prefetch_desc(&tmA1); tma_prefetch_desc(&tmB1);
+        if (PLANES == 2) { tma_prefetch_desc(&tmA2); tma_prefetch_desc(&tmB2); }
         for (int s = 0; s < n_stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
         fence_barrier_init();
     }
@@ -158,9 +169,9 @@ gemm_f16s_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant
                     mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
                     const int k0 = (kb0 + i) * GH_KB;
                     tma_load_2d(s0, &tmA1, &full_bar[stage], k0, m0, TMA_EVICT_LAST);
-                    tma_load_2d(s0 + GM_SLAB, &tmA2, &full_bar[stage], k0, m0, TMA_EVICT_LAST);
-                    tma_load_2d(s0 + 2 * GM_SLAB, &tmB1, &full_bar[stage], k0, n0, pol_b);
-                    tma_load_2d(s0 + 2 * GM_SLAB + B_BYTES, &tmB2, &full_bar[stage], k0, n0, pol_b);
+                    if (PLANES == 2) tma_load_2d(s0 + GM_SLAB, &tmA2, &full_bar[stage], k0, m0, TMA_EVICT_LAST);
+                    tma_load_2d(s0 + B_OFF, &tmB1, &full_bar[stage], k0, n0, pol_b);
+                    if (PLANES == 2) tma_load_2d(s0 + B_OFF + B_BYTES, &tmB2, &full_bar[stage], k0, n0, pol_b);
                     if (++stage == n_stages) { stage = 0; phase ^= 1; }
                 }
             }
@@ -170,7 +181,7 @@ gemm_f16s_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant
         const int wg = (warp >> 2) - 1, w = warp & 3;
         const int g = lane >> 2, q = lane & 3;
         const int r_lo = 64 * wg + 16 * w + g;             // this thread's accumulator rows: r_lo and r_lo + 8
-        float acc_m[R], acc_c[R];
+        float acc_m[R], acc_c[PLANES == 2 ? R : 1];        // PLANES == 1: acc_c is never touched
         int stage = 0; uint32_t phase = 0;
         for (int t = blockIdx.x; t < total; t += gridDim.x) {
             const int n0 = (t % n_tiles) * BN, m0 = ((t / n_tiles) % m_tiles) * GM_TILE;
@@ -181,19 +192,22 @@ gemm_f16s_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant
                 if (rows_here) {
                     const uint32_t s0 = smem_u32(smem + (size_t)stage * STAGE_BYTES);
                     const uint64_t a1 = wgmma_desc_sw128(s0 + wg * 64 * 128), a2 = wgmma_desc_sw128(s0 + GM_SLAB + wg * 64 * 128);
-                    const uint64_t b1 = wgmma_desc_sw128(s0 + 2 * GM_SLAB), b2 = wgmma_desc_sw128(s0 + 2 * GM_SLAB + B_BYTES);
+                    const uint64_t b1 = wgmma_desc_sw128(s0 + B_OFF), b2 = wgmma_desc_sw128(s0 + B_OFF + B_BYTES);
+                    (void)a2; (void)b2;
                     wgmma_fence();
 #pragma unroll
                     for (int k = 0; k < GH_KB / 16; ++k) {   // K steps of 16 halfs = 32 bytes = 2 descriptor units
                         const uint32_t first = (uint32_t)((i | k) != 0);
                         wgmma_f16_ss<BN>(acc_m, a1 + 2 * k, b1 + 2 * k, first);
-                        wgmma_f16_ss<BN>(acc_c, a1 + 2 * k, b2 + 2 * k, first);
-                        wgmma_f16_ss<BN>(acc_c, a2 + 2 * k, b1 + 2 * k, 1u);
+                        if constexpr (PLANES == 2) {
+                            wgmma_f16_ss<BN>(acc_c, a1 + 2 * k, b2 + 2 * k, first);
+                            wgmma_f16_ss<BN>(acc_c, a2 + 2 * k, b1 + 2 * k, 1u);
+                        }
                     }
                     wgmma_commit();
                     wgmma_wait<0>();
                     wgmma_fence_operands<R>(acc_m);
-                    wgmma_fence_operands<R>(acc_c);
+                    if constexpr (PLANES == 2) wgmma_fence_operands<R>(acc_c);
                 }
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&empty_bar[stage]);
@@ -205,6 +219,11 @@ gemm_f16s_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant
             // time, each load's latency (the residual row comes from L2 or HBM) was paid in turn while the tensor cores idled.
             constexpr int EP_J = R / 4 < 8 ? R / 4 : 8;   // column groups per batch: all of a 128 x 32 tile's 4, else 8
             static_assert((R / 4) % EP_J == 0, "the batches cover the tile's column groups exactly");
+            // element e of the tile's result: main + 2^-11 correction, or the one accumulator
+            auto acc = [&](int e) {
+                if constexpr (PLANES == 2) return fmaf(acc_c[e], GH_LO_INV, acc_m[e]);
+                else return acc_m[e];
+            };
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int row = m0 + r_lo + 8 * h;
@@ -214,8 +233,7 @@ gemm_f16s_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant
 #pragma unroll
                     for (int j = 0; j < R / 4; ++j) {
                         const int col = n0 + 8 * j + 2 * q;
-                        const float o0 = fmaf(acc_c[4 * j + 2 * h], GH_LO_INV, acc_m[4 * j + 2 * h]);
-                        const float o1 = fmaf(acc_c[4 * j + 2 * h + 1], GH_LO_INV, acc_m[4 * j + 2 * h + 1]);
+                        const float o0 = acc(4 * j + 2 * h), o1 = acc(4 * j + 2 * h + 1);
                         *reinterpret_cast<float2*>(ws + (size_t)split * M * N + roff + col) = make_float2(o0, o1);
                     }
                     continue;
@@ -232,17 +250,20 @@ gemm_f16s_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant
 #pragma unroll
                     for (int u = 0; u < EP_J; ++u) {
                         const int j = j0 + u, col = n0 + 8 * j + 2 * q;
-                        float o0 = fmaf(acc_c[4 * j + 2 * h], GH_LO_INV, acc_m[4 * j + 2 * h]);
-                        float o1 = fmaf(acc_c[4 * j + 2 * h + 1], GH_LO_INV, acc_m[4 * j + 2 * h + 1]);
+                        float o0 = acc(4 * j + 2 * h), o1 = acc(4 * j + 2 * h + 1);
                         o0 += b2[u].x; o1 += b2[u].y;
                         if (act_gelu) { o0 = gelu_erf(o0); o1 = gelu_erf(o1); }
                         if (residual) { o0 += r2[u].x; o1 += r2[u].y; }
                         if (out.c) *reinterpret_cast<float2*>(out.c + roff + col) = make_float2(o0, o1);
-                        if (out.hi) {
-                            uint16_t h0, l0, h1, l1;
-                            split_f16(o0, h0, l0); split_f16(o1, h1, l1);
-                            *reinterpret_cast<uint32_t*>(out.hi + roff + col) = (uint32_t)h0 | ((uint32_t)h1 << 16);
-                            *reinterpret_cast<uint32_t*>(out.lo + roff + col) = (uint32_t)l0 | ((uint32_t)l1 << 16);
+                        if constexpr (PLANES == 2) {
+                            if (out.hi) {
+                                uint16_t h0, l0, h1, l1;
+                                split_f16(o0, h0, l0); split_f16(o1, h1, l1);
+                                *reinterpret_cast<uint32_t*>(out.hi + roff + col) = (uint32_t)h0 | ((uint32_t)h1 << 16);
+                                *reinterpret_cast<uint32_t*>(out.lo + roff + col) = (uint32_t)l0 | ((uint32_t)l1 << 16);
+                            }
+                        } else {
+                            if (out.hi) *reinterpret_cast<uint32_t*>(out.hi + roff + col) = hi_pack2(o0, o1);
                         }
                     }
                 }
@@ -304,7 +325,8 @@ __device__ __forceinline__ void warp_layernorm_row(const float* __restrict__ x, 
                 *reinterpret_cast<float4*>(y + gi * 8) = make_float4(o[0], o[1], o[2], o[3]);
                 *reinterpret_cast<float4*>(y + gi * 8 + 4) = make_float4(o[4], o[5], o[6], o[7]);
             }
-            if (y_hi) split_store8(o, y_hi + gi * 8, y_lo + gi * 8);
+            if (y_lo) split_store8(o, y_hi + gi * 8, y_lo + gi * 8);
+            else if (y_hi) hi_store8(o, y_hi + gi * 8);
         }
     }
 }
@@ -343,7 +365,7 @@ embed_ln_kernel(const int32_t* __restrict__ tok, const int32_t* __restrict__ pos
     const float* tr = typ ? temb + (size_t)typ[t] * d : temb;
     for (int i = lane; i < d; i += 32) row[i] = (wr[i] + tr[i]) + pr[i];   // torch: inputs_embeds + token_type + position
     __syncwarp();
-    warp_layernorm_row(row, x + (size_t)t * d, x_hi + (size_t)t * d, x_lo + (size_t)t * d, g, b, d, eps, lane);
+    warp_layernorm_row(row, x + (size_t)t * d, x_hi + (size_t)t * d, x_lo ? x_lo + (size_t)t * d : nullptr, g, b, d, eps, lane);
 }
 
 // split-K epilogue: out[row] = f(sum_s ws[s][row] + bias) (+GELU) (+residual), optionally followed by LayerNorm over
@@ -382,7 +404,9 @@ splitk_reduce_kernel(const float* __restrict__ ws, int splits, int M, int N, con
     };
     auto store4 = [&](int c, const float4& o) {
         if (out) *reinterpret_cast<float4*>(out + (size_t)row * N + c) = o;
-        if (out_hi) {
+        if (out_hi && !out_lo) {
+            *reinterpret_cast<uint2*>(out_hi + (size_t)row * N + c) = make_uint2(hi_pack2(o.x, o.y), hi_pack2(o.z, o.w));
+        } else if (out_hi) {
             uint16_t h0, l0, h1, l1, h2, l2, h3, l3;
             split_f16(o.x, h0, l0); split_f16(o.y, h1, l1); split_f16(o.z, h2, l2); split_f16(o.w, h3, l3);
             *reinterpret_cast<uint2*>(out_hi + (size_t)row * N + c) = make_uint2((uint32_t)h0 | ((uint32_t)h1 << 16), (uint32_t)h2 | ((uint32_t)h3 << 16));
@@ -455,18 +479,20 @@ __device__ __forceinline__ void split_pack2(float a, float b, uint32_t& hi, uint
 }
 __device__ __forceinline__ void am_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void am_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-template <int DH, int WARPS, int KB, int STAGES> struct AmCfg {
+// PLANES == 1 (KRAG_PRECISION_FP16): only the hi planes are staged and every product is one MMA on them; same key blocking,
+// same fp32 softmax.
+template <int DH, int WARPS, int KB, int STAGES, int PLANES> struct AmCfg {
     static constexpr int LDH = DH + 8;                                   // row stride in halfs (16 bytes of padding)
-    static constexpr int Q_HALFS = 2 * 16 * WARPS * LDH;                 // hi | lo
-    static constexpr int KV_HALFS = 2 * KB * LDH;                        // hi | lo of one operand of one stage
+    static constexpr int Q_HALFS = PLANES * 16 * WARPS * LDH;            // hi | lo
+    static constexpr int KV_HALFS = PLANES * KB * LDH;                   // hi | lo of one operand of one stage
     static constexpr size_t SMEM = 2 * (size_t)(Q_HALFS + 2 * STAGES * KV_HALFS);
 };
-template <int DH, int WARPS, int KB, int STAGES>
+template <int DH, int WARPS, int KB, int STAGES, int PLANES>
 __global__ void __launch_bounds__(WARPS * 32)
 attention_mma_kernel(const uint16_t* __restrict__ qkv_hi, const uint16_t* __restrict__ qkv_lo, const int32_t* __restrict__ seq_off,
                      uint16_t* __restrict__ out_hi, uint16_t* __restrict__ out_lo, int d, int heads)
 {
-    using Cfg = AmCfg<DH, WARPS, KB, STAGES>;
+    using Cfg = AmCfg<DH, WARPS, KB, STAGES, PLANES>;
     constexpr int LDH = Cfg::LDH, QROWS = 16 * WARPS, THREADS = WARPS * 32, CH = DH / 8 /* 16-byte chunks per row */;
     extern __shared__ __align__(16) uint16_t am_sm[];
     uint16_t* sQ = am_sm;                                  // [2][QROWS][LDH]
@@ -482,7 +508,7 @@ attention_mma_kernel(const uint16_t* __restrict__ qkv_hi, const uint16_t* __rest
     const size_t ld = (size_t)3 * d;
     // rows [row0, row0 + nrows) of one of Q | K | V (column offset `col`) of this head, both planes -> dst[2][nrows][LDH]
     auto stage_rows = [&](uint16_t* dst, int nrows, int row0, int col) {
-        for (int i = tid; i < 2 * nrows * CH; i += THREADS) {
+        for (int i = tid; i < PLANES * nrows * CH; i += THREADS) {
             const int pl = i / (nrows * CH), rem = i % (nrows * CH), r = rem / CH, ch = rem % CH;
             const bool valid = row0 + r < len;
             const uint16_t* src = (pl ? qkv_lo : qkv_hi) + (valid ? (size_t)(t0 + row0 + r) * ld + col + h * DH + ch * 8 : 0);
@@ -498,11 +524,14 @@ attention_mma_kernel(const uint16_t* __restrict__ qkv_hi, const uint16_t* __rest
     stage_kv(0, 0);
     const int nkb = (len + KB - 1) / KB;
     uint32_t qh[DH / 16][4], ql[DH / 16][4];
-    float om[DH / 8][4], oc[DH / 8][4];                    // output accumulators: main and correction products
+    float om[DH / 8][4], oc[PLANES == 2 ? DH / 8 : 1][4];  // output accumulators: main and correction products
 #pragma unroll
     for (int j = 0; j < DH / 8; ++j)
 #pragma unroll
-        for (int e = 0; e < 4; ++e) { om[j][e] = 0.f; oc[j][e] = 0.f; }
+        for (int e = 0; e < 4; ++e) {
+            om[j][e] = 0.f;
+            if constexpr (PLANES == 2) oc[j][e] = 0.f;
+        }
     float m_run[2] = {-CUDART_INF_F, -CUDART_INF_F}, l_run[2] = {0.f, 0.f};     // rows g and g + 8 of the warp's 16
     const float scale = rsqrtf((float)DH);
     for (int kb = 0; kb < nkb; ++kb) {
@@ -514,7 +543,7 @@ attention_mma_kernel(const uint16_t* __restrict__ qkv_hi, const uint16_t* __rest
             for (int kk = 0; kk < DH / 16; ++kk) {
                 const uint32_t a = smem_u32(sQ + (size_t)(warp * 16 + (lane & 15)) * LDH + kk * 16 + (lane >> 4) * 8);
                 ldsm_x4(a, qh[kk][0], qh[kk][1], qh[kk][2], qh[kk][3]);
-                ldsm_x4(a + 2 * QROWS * LDH, ql[kk][0], ql[kk][1], ql[kk][2], ql[kk][3]);
+                if constexpr (PLANES == 2) ldsm_x4(a + 2 * QROWS * LDH, ql[kk][0], ql[kk][1], ql[kk][2], ql[kk][3]);
             }
         }
         const uint16_t* kH = sK + stage * Cfg::KV_HALFS;
@@ -524,16 +553,18 @@ attention_mma_kernel(const uint16_t* __restrict__ qkv_hi, const uint16_t* __rest
 #pragma unroll
         for (int j = 0; j < KB / 8; ++j) {
             s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
+            if constexpr (PLANES == 2) {
 #pragma unroll
-            for (int k2 = 0; k2 < DH / 32; ++k2) {
-                const uint32_t a = smem_u32(kH + (size_t)(j * 8 + (lane & 7)) * LDH + k2 * 32 + (lane >> 3) * 8);
-                uint32_t h0, h1, h2, h3, l0, l1, l2, l3;
-                ldsm_x4(a, h0, h1, h2, h3);
-                ldsm_x4(a + 2 * KB * LDH, l0, l1, l2, l3);
-                mma_f16(s[j], qh[2 * k2], l0, l1); mma_f16(s[j], ql[2 * k2], h0, h1);
-                mma_f16(s[j], qh[2 * k2 + 1], l2, l3); mma_f16(s[j], ql[2 * k2 + 1], h2, h3);
+                for (int k2 = 0; k2 < DH / 32; ++k2) {
+                    const uint32_t a = smem_u32(kH + (size_t)(j * 8 + (lane & 7)) * LDH + k2 * 32 + (lane >> 3) * 8);
+                    uint32_t h0, h1, h2, h3, l0, l1, l2, l3;
+                    ldsm_x4(a, h0, h1, h2, h3);
+                    ldsm_x4(a + 2 * KB * LDH, l0, l1, l2, l3);
+                    mma_f16(s[j], qh[2 * k2], l0, l1); mma_f16(s[j], ql[2 * k2], h0, h1);
+                    mma_f16(s[j], qh[2 * k2 + 1], l2, l3); mma_f16(s[j], ql[2 * k2 + 1], h2, h3);
+                }
+                s[j][0] *= GH_LO_INV; s[j][1] *= GH_LO_INV; s[j][2] *= GH_LO_INV; s[j][3] *= GH_LO_INV;
             }
-            s[j][0] *= GH_LO_INV; s[j][1] *= GH_LO_INV; s[j][2] *= GH_LO_INV; s[j][3] *= GH_LO_INV;
 #pragma unroll
             for (int k2 = 0; k2 < DH / 32; ++k2) {
                 const uint32_t a = smem_u32(kH + (size_t)(j * 8 + (lane & 7)) * LDH + k2 * 32 + (lane >> 3) * 8);
@@ -576,24 +607,35 @@ attention_mma_kernel(const uint16_t* __restrict__ qkv_hi, const uint16_t* __rest
 #pragma unroll
         for (int j = 0; j < DH / 8; ++j) {
             om[j][0] *= corr[0]; om[j][1] *= corr[0]; om[j][2] *= corr[1]; om[j][3] *= corr[1];
-            oc[j][0] *= corr[0]; oc[j][1] *= corr[0]; oc[j][2] *= corr[1]; oc[j][3] *= corr[1];
+            if constexpr (PLANES == 2) { oc[j][0] *= corr[0]; oc[j][1] *= corr[0]; oc[j][2] *= corr[1]; oc[j][3] *= corr[1]; }
         }
         // ---- out += P . V : the score accumulators of key tiles 2u, 2u+1 ARE the A fragment of 16-key step u
 #pragma unroll
         for (int u = 0; u < KB / 16; ++u) {
             uint32_t ph[4], pl[4];
-            split_pack2(s[2 * u][0], s[2 * u][1], ph[0], pl[0]);
-            split_pack2(s[2 * u][2], s[2 * u][3], ph[1], pl[1]);
-            split_pack2(s[2 * u + 1][0], s[2 * u + 1][1], ph[2], pl[2]);
-            split_pack2(s[2 * u + 1][2], s[2 * u + 1][3], ph[3], pl[3]);
+            if constexpr (PLANES == 2) {
+                split_pack2(s[2 * u][0], s[2 * u][1], ph[0], pl[0]);
+                split_pack2(s[2 * u][2], s[2 * u][3], ph[1], pl[1]);
+                split_pack2(s[2 * u + 1][0], s[2 * u + 1][1], ph[2], pl[2]);
+                split_pack2(s[2 * u + 1][2], s[2 * u + 1][3], ph[3], pl[3]);
+            } else {
+                ph[0] = hi_pack2(s[2 * u][0], s[2 * u][1]); ph[1] = hi_pack2(s[2 * u][2], s[2 * u][3]);
+                ph[2] = hi_pack2(s[2 * u + 1][0], s[2 * u + 1][1]); ph[3] = hi_pack2(s[2 * u + 1][2], s[2 * u + 1][3]);
+            }
 #pragma unroll
             for (int jp = 0; jp < DH / 16; ++jp) {
                 const uint32_t a = smem_u32(vH + (size_t)(u * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * LDH + jp * 16 + (lane >> 4) * 8);
-                uint32_t h0, h1, h2, h3, l0, l1, l2, l3;
+                uint32_t h0, h1, h2, h3;
                 ldsm_x4_trans(a, h0, h1, h2, h3);
-                ldsm_x4_trans(a + 2 * KB * LDH, l0, l1, l2, l3);
-                mma_f16(om[2 * jp], ph, h0, h1); mma_f16(oc[2 * jp], ph, l0, l1); mma_f16(oc[2 * jp], pl, h0, h1);
-                mma_f16(om[2 * jp + 1], ph, h2, h3); mma_f16(oc[2 * jp + 1], ph, l2, l3); mma_f16(oc[2 * jp + 1], pl, h2, h3);
+                if constexpr (PLANES == 2) {
+                    uint32_t l0, l1, l2, l3;
+                    ldsm_x4_trans(a + 2 * KB * LDH, l0, l1, l2, l3);
+                    mma_f16(om[2 * jp], ph, h0, h1); mma_f16(oc[2 * jp], ph, l0, l1); mma_f16(oc[2 * jp], pl, h0, h1);
+                    mma_f16(om[2 * jp + 1], ph, h2, h3); mma_f16(oc[2 * jp + 1], ph, l2, l3); mma_f16(oc[2 * jp + 1], pl, h2, h3);
+                } else {
+                    mma_f16(om[2 * jp], ph, h0, h1);
+                    mma_f16(om[2 * jp + 1], ph, h2, h3);
+                }
             }
         }
         __syncthreads();                                           // the stage is free again
@@ -612,10 +654,14 @@ attention_mma_kernel(const uint16_t* __restrict__ qkv_hi, const uint16_t* __rest
         const size_t ob = (size_t)(t0 + row) * d + h * DH + 2 * t;
 #pragma unroll
         for (int j = 0; j < DH / 8; ++j) {
-            uint32_t hi, lo;
-            split_pack2(fmaf(oc[j][2 * r], GH_LO_INV, om[j][2 * r]) * inv[r], fmaf(oc[j][2 * r + 1], GH_LO_INV, om[j][2 * r + 1]) * inv[r], hi, lo);
-            *reinterpret_cast<uint32_t*>(out_hi + ob + j * 8) = hi;
-            *reinterpret_cast<uint32_t*>(out_lo + ob + j * 8) = lo;
+            if constexpr (PLANES == 2) {
+                uint32_t hi, lo;
+                split_pack2(fmaf(oc[j][2 * r], GH_LO_INV, om[j][2 * r]) * inv[r], fmaf(oc[j][2 * r + 1], GH_LO_INV, om[j][2 * r + 1]) * inv[r], hi, lo);
+                *reinterpret_cast<uint32_t*>(out_hi + ob + j * 8) = hi;
+                *reinterpret_cast<uint32_t*>(out_lo + ob + j * 8) = lo;
+            } else {
+                *reinterpret_cast<uint32_t*>(out_hi + ob + j * 8) = hi_pack2(om[j][2 * r] * inv[r], om[j][2 * r + 1] * inv[r]);
+            }
         }
     }
 }
@@ -635,7 +681,7 @@ gather_cls_kernel(const float* __restrict__ x, const uint16_t* __restrict__ c_hi
     for (int i = 4 * lane; i < d; i += 128) *reinterpret_cast<float4*>(gx + dst + i) = *reinterpret_cast<const float4*>(x + src + i);
     for (int i = 8 * lane; i < d; i += 256) {
         *reinterpret_cast<uint4*>(g_hi + dst + i) = *reinterpret_cast<const uint4*>(c_hi + src + i);
-        *reinterpret_cast<uint4*>(g_lo + dst + i) = *reinterpret_cast<const uint4*>(c_lo + src + i);
+        if (g_lo) *reinterpret_cast<uint4*>(g_lo + dst + i) = *reinterpret_cast<const uint4*>(c_lo + src + i);
     }
 }
 
@@ -789,30 +835,30 @@ static void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
     count_launch();
 }
 
-template <int DH, int WARPS, int KB, int STAGES>
+template <int DH, int WARPS, int KB, int STAGES, int PLANES>
 static void launch_attention_mma(const uint16_t* q_hi, const uint16_t* q_lo, const int32_t* seq_off, uint16_t* out_hi, uint16_t* out_lo, int d,
                                  int heads, int batch, int max_len, bool first_rows, cudaStream_t st)
 {
-    using Cfg = AmCfg<DH, WARPS, KB, STAGES>;
+    using Cfg = AmCfg<DH, WARPS, KB, STAGES, PLANES>;
     static bool attr_set = false;
     if (!attr_set) {
-        KRAG_CUDA(cudaFuncSetAttribute(attention_mma_kernel<DH, WARPS, KB, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM));
+        KRAG_CUDA(cudaFuncSetAttribute(attention_mma_kernel<DH, WARPS, KB, STAGES, PLANES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM));
         attr_set = true;
     }
     const unsigned q_blocks = first_rows ? 1u : (unsigned)((max_len + 16 * WARPS - 1) / (16 * WARPS));
-    launch_pdl(attention_mma_kernel<DH, WARPS, KB, STAGES>, dim3(q_blocks, (unsigned)heads, (unsigned)batch),
+    launch_pdl(attention_mma_kernel<DH, WARPS, KB, STAGES, PLANES>, dim3(q_blocks, (unsigned)heads, (unsigned)batch),
                dim3(WARPS * 32), Cfg::SMEM, st, q_hi, q_lo, seq_off, out_hi, out_lo, d, heads);
 }
 // queries (<= 32 tokens): 2 warps, one key block; <= 64: 4 warps, one block; chunks: 4 warps, 64-key blocks, double-buffered.
 // first_rows: only the first block of query rows of every sequence (the [CLS] row among them); a query row's result does
-// not depend on which other rows run, and the key blocking follows max_len either way
-template <int DH>
+// not depend on which other rows run, and the key blocking follows max_len either way.  PLANES == 1: q_lo / out_lo are not used
+template <int DH, int PLANES>
 static void attention_mma(const uint16_t* q_hi, const uint16_t* q_lo, const int32_t* seq_off, uint16_t* out_hi, uint16_t* out_lo, int d, int heads,
                           int batch, int max_len, bool first_rows, cudaStream_t st)
 {
-    if (max_len <= 32) launch_attention_mma<DH, 2, 32, 1>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, st);
-    else if (max_len <= 64) launch_attention_mma<DH, 4, 64, 1>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, st);
-    else launch_attention_mma<DH, 4, 64, 2>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, st);
+    if (max_len <= 32) launch_attention_mma<DH, 2, 32, 1, PLANES>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, st);
+    else if (max_len <= 64) launch_attention_mma<DH, 4, 64, 1, PLANES>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, st);
+    else launch_attention_mma<DH, 4, 64, 2, PLANES>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, st);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -844,29 +890,29 @@ static void emb_map(CUtensorMap* tm, const uint16_t* base, int rows, int cols, i
 }
 
 // gemm_f16s_kernel over the 128 x BN tiles of C and `splits` K slices, min(work items, SMs) persistent CTAs
-template <int BN>
+template <int BN, int PLANES>
 static void launch_gemm(const DeviceInfo& di, const SplitMat& A, const SplitMat& B, int M, int N, int K, int splits, const float* bias,
                         const float* residual, bool gelu, const GemmOut& out, float* ws, cudaStream_t st)
 {
-    constexpr int stage_bytes = 2 * GM_SLAB + 2 * BN * 128;
+    constexpr int stage_bytes = PLANES * (GM_SLAB + BN * 128);
     constexpr int n_stages = GM_SMEM_BUDGET / stage_bytes < GM_MAX_STAGES ? GM_SMEM_BUDGET / stage_bytes : GM_MAX_STAGES;
     constexpr size_t smem = 1024 + (size_t)n_stages * stage_bytes + 2 * GM_MAX_STAGES * 8;
     static bool attr = false;
-    if (!attr) { KRAG_CUDA(cudaFuncSetAttribute(gemm_f16s_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = true; }
+    if (!attr) { KRAG_CUDA(cudaFuncSetAttribute(gemm_f16s_kernel<BN, PLANES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = true; }
     CUtensorMap tmA1, tmA2, tmB1, tmB2;
-    emb_map(&tmA1, A.hi, M, K); emb_map(&tmA2, A.lo, M, K);
-    emb_map(&tmB1, B.hi, N, K, BN); emb_map(&tmB2, B.lo, N, K, BN);
+    emb_map(&tmA1, A.hi, M, K); emb_map(&tmA2, PLANES == 2 ? A.lo : A.hi, M, K);     // PLANES == 1: the second maps are not read
+    emb_map(&tmB1, B.hi, N, K, BN); emb_map(&tmB2, PLANES == 2 ? B.lo : B.hi, N, K, BN);
     const int m_tiles = (M + GM_TILE - 1) / GM_TILE;
     const int total = m_tiles * (N / BN) * splits;
     const int grid = total < di.sm_count ? total : di.sm_count;
     // one activation tile: every weight byte is read once, keep it out of the way of the activations in L2
-    launch_pdl(gemm_f16s_kernel<BN>, dim3((unsigned)grid), dim3(GM_THREADS), smem, st, tmA1, tmA2, tmB1, tmB2, M, N, splits,
+    launch_pdl(gemm_f16s_kernel<BN, PLANES>, dim3((unsigned)grid), dim3(GM_THREADS), smem, st, tmA1, tmA2, tmB1, tmB2, M, N, splits,
                K / GH_KB / splits, n_stages, m_tiles == 1 ? 1 : 0, bias, residual, gelu ? 1 : 0, out, ws);
 }
 
 // Tile width and K split of a linear layer of M rows.  Every output element is summed in an order fixed by (bn, splits)
 // alone, so a plan made for M rows computes the same bits on any subset of those rows.
-GemmPlan linear_plan(const DeviceInfo& di, int M, int N, int K, bool ln, bool have_ws, size_t ws_floats)
+GemmPlan linear_plan(const DeviceInfo& di, int M, int N, int K, bool ln, bool have_ws, size_t ws_floats, int planes)
 {
     const int m_tiles = (M + GM_TILE - 1) / GM_TILE;
     const int tiles128 = m_tiles * (N / GM_TILE);
@@ -883,6 +929,10 @@ GemmPlan linear_plan(const DeviceInfo& di, int M, int N, int K, bool ln, bool ha
         }
         return GemmPlan{BN, splits, true};
     }
+    // single-plane product: one accumulator per thread leaves room for 128 x 256 tiles.  Taken from two waves of them on:
+    // at 8192 rows they measured 2-13% faster than 128 x 128 for N = 1536 ... 3072 and 7-9% slower for N = 768, where 192
+    // tiles leave half of the second wave's SMs idle (DESIGN.md section 4, "Cross-encoder head")
+    if (planes == 1 && N % 256 == 0 && m_tiles * (N / 256) >= 2 * di.sm_count) return GemmPlan{256, 1, false};
     return GemmPlan{128, 1, false};
 }
 
@@ -890,26 +940,35 @@ GemmPlan linear_plan(const DeviceInfo& di, int M, int N, int K, bool ln, bool ha
 // row LayerNorm of that goes to Y (fp32) and its split planes (C is then scratch).  plan: null = linear_plan(M, ...).
 void launch_linear(const DeviceInfo& di, const SplitMat& A, const SplitMat& B, int M, int N, int K, const float* bias, const float* residual,
                    bool gelu, float* C, uint16_t* C_hi, uint16_t* C_lo, const float* ln_g, const float* ln_b, float eps, float* Y,
-                   uint16_t* Y_hi, uint16_t* Y_lo, float* ws, size_t ws_floats, cudaStream_t st, const GemmPlan* plan)
+                   uint16_t* Y_hi, uint16_t* Y_lo, float* ws, size_t ws_floats, cudaStream_t st, const GemmPlan* plan, int planes)
 {
     if (ln_g && N > 32 * LN_MAX_GROUPS * 8) throw std::runtime_error("launch_linear: fused LayerNorm rows hold at most 1024 elements");
-    const GemmPlan p = plan ? *plan : linear_plan(di, M, N, K, ln_g != nullptr, ws != nullptr, ws_floats);
-    if (N % p.bn || K % GH_KB || (K / GH_KB) % p.splits || (p.splits > 1 && (!ws || (size_t)p.splits * M * N > ws_floats)))
+    const GemmPlan p = plan ? *plan : linear_plan(di, M, N, K, ln_g != nullptr, ws != nullptr, ws_floats, planes);
+    if (planes == 1) { C_lo = nullptr; Y_lo = nullptr; }
+    if (planes != 1 && planes != 2) throw std::runtime_error("launch_linear: one or two operand planes");
+    if (N % p.bn || (p.bn == 256 && planes != 1) || K % GH_KB || (K / GH_KB) % p.splits || (p.splits > 1 && (!ws || (size_t)p.splits * M * N > ws_floats)))
         throw std::runtime_error("launch_linear: plan does not fit the problem");
     if (p.small_m) {
         // splits == 1 and a LayerNorm to follow: the GEMM writes fp32 C (scratch), the LayerNorm kernel writes Y + planes
         const GemmOut direct = ln_g ? GemmOut{C, nullptr, nullptr} : GemmOut{C, C_hi, C_lo};
-        if (p.bn == 32) launch_gemm<32>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
-        else if (p.bn == 128) launch_gemm<128>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
-        else launch_gemm<64>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
+        if (planes == 1) {
+            if (p.bn == 32) launch_gemm<32, 1>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
+            else if (p.bn == 256) launch_gemm<256, 1>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
+            else if (p.bn == 128) launch_gemm<128, 1>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
+            else launch_gemm<64, 1>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
+        } else if (p.bn == 32) launch_gemm<32, 2>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
+        else if (p.bn == 128) launch_gemm<128, 2>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
+        else launch_gemm<64, 2>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
         if (p.splits > 1) {
             launch_pdl(splitk_reduce_kernel, dim3((unsigned)M), dim3(256), 0, st, ws, p.splits, M, N, bias, residual, gelu ? 1 : 0, ln_g, ln_b,
                        eps, ln_g ? Y : C, ln_g ? Y_hi : C_hi, ln_g ? Y_lo : C_lo);
             return;
         }
     } else {
-        launch_gemm<128>(di, A, B, M, N, K, 1, bias, residual, gelu, ln_g ? GemmOut{C, nullptr, nullptr} : GemmOut{C, C_hi, C_lo},
-                         nullptr, st);
+        const GemmOut direct = ln_g ? GemmOut{C, nullptr, nullptr} : GemmOut{C, C_hi, C_lo};
+        if (planes == 1 && p.bn == 256) launch_gemm<256, 1>(di, A, B, M, N, K, 1, bias, residual, gelu, direct, nullptr, st);
+        else if (planes == 1) launch_gemm<128, 1>(di, A, B, M, N, K, 1, bias, residual, gelu, direct, nullptr, st);
+        else launch_gemm<128, 2>(di, A, B, M, N, K, 1, bias, residual, gelu, direct, nullptr, st);
     }
     if (ln_g) {
         launch_pdl(layernorm_kernel, dim3((unsigned)((M * 32 + 255) / 256)), dim3(256), 0, st, C, Y, Y_hi, Y_lo, ln_g, ln_b, M, N, eps);
@@ -919,20 +978,20 @@ void launch_linear(const DeviceInfo& di, const SplitMat& A, const SplitMat& B, i
 // test hook (krag_debug_gemm_tf32 / krag_debug_linear_ln): fp32 device operands are split here, then take the product path
 void launch_linear_f32(const DeviceInfo& di, const float* A, const float* B, int M, int N, int K, const float* bias, const float* residual,
                        bool gelu, float* C, const float* ln_g, const float* ln_b, float eps, float* Y, float* ws, size_t ws_floats,
-                       cudaStream_t st, int tile_n, int reps, float* ms)
+                       cudaStream_t st, int tile_n, int reps, float* ms, int planes)
 {
-    if (tile_n != 0 && tile_n != 32 && tile_n != 64 && tile_n != 128)
-        throw std::runtime_error("launch_linear_f32: tile width must be 0, 32, 64 or 128");
+    if (tile_n != 0 && tile_n != 32 && tile_n != 64 && tile_n != 128 && !(tile_n == 256 && planes == 1))
+        throw std::runtime_error("launch_linear_f32: tile width must be 0, 32, 64 or 128 (256: single-plane product only)");
     const GemmPlan forced{tile_n, 1, true};
     const GemmPlan* plan = tile_n ? &forced : nullptr;
     const size_t na = (size_t)M * K, nb = (size_t)N * K;
-    DevArray<uint16_t> planes;
-    planes.alloc((int64_t)(2 * na + 2 * nb));
-    SplitMat As{planes.p, planes.p + na}, Bs{planes.p + 2 * na, planes.p + 2 * na + nb};
+    DevArray<uint16_t> buf;
+    buf.alloc((int64_t)(2 * na + 2 * nb));
+    SplitMat As{buf.p, buf.p + na}, Bs{buf.p + 2 * na, buf.p + 2 * na + nb};
     launch_split_f16(A, As.hi, As.lo, (int64_t)na, st);
     launch_split_f16(B, Bs.hi, Bs.lo, (int64_t)nb, st);
     auto run = [&] {
-        launch_linear(di, As, Bs, M, N, K, bias, residual, gelu, C, nullptr, nullptr, ln_g, ln_b, eps, Y, nullptr, nullptr, ws, ws_floats, st, plan);
+        launch_linear(di, As, Bs, M, N, K, bias, residual, gelu, C, nullptr, nullptr, ln_g, ln_b, eps, Y, nullptr, nullptr, ws, ws_floats, st, plan, planes);
     };
     run();
     if (reps > 0) {
@@ -966,10 +1025,12 @@ struct Embedder {
     bool finalized = false;
     cudaStream_t st = nullptr;
     cudaEvent_t done = nullptr, in_ev = nullptr;
-    // captured forward per (n_tok, batch, max_len, cls_rows, head): head = 1 for cross-encoder pairs (token types uploaded)
-    using GraphKey = std::tuple<int, int, int, int, int>;
+    // captured forward per (n_tok, batch, max_len, cls_rows, head, precision): head = 1 for cross-encoder pairs (token types
+    // uploaded); the two precisions run different kernels
+    using GraphKey = std::tuple<int, int, int, int, int, int>;
     std::map<GraphKey, cudaGraphExec_t> graphs;
     std::map<GraphKey, int> seen;
+    int precision = EMB_PREC_FP32;        // EMB_PREC_FP16: single-plane products (the hi planes of weights and activations)
     int pooling = EMB_POOL_CLS;           // read by the final writer, which runs outside the captured graphs
     bool cls_rows_only = true;            // CLS pooling: the last layer after QKV + attention runs on the [CLS] rows only
     // workspaces, grown on demand
@@ -1124,6 +1185,13 @@ void embedder_set_pooling(Embedder* e, int mode)
 
 void embedder_set_cls_rows_only(Embedder* e, bool on) { e->cls_rows_only = on; }
 
+// The weights' hi planes ARE their fp16 values, so the two modes share one copy and the mode can change between forwards.
+void embedder_set_precision(Embedder* e, int mode)
+{
+    if (mode != EMB_PREC_FP32 && mode != EMB_PREC_FP16) throw std::runtime_error("embedder: precision must be FP32 or FP16");
+    e->precision = mode;
+}
+
 template <int G>
 static void launch_mean_normalize(const float* x, const int32_t* seq_off, float* out, int batch, int ld_out, cudaStream_t st)
 {
@@ -1194,9 +1262,12 @@ static bool encoder_forward(Embedder* e, int batch, const int32_t* tok_ids, cons
         e->cx.alloc(Bc * d); e->cx2.alloc(Bc * d); e->ccs.alloc(2 * Bc * d); e->cxs.alloc(2 * Bc * d); e->cfs.alloc(2 * Bc * c.inter);
         e->cap_tok = (int)T; e->cap_batch = (int)Bc;
     }
-    // split planes: [hi plane | lo plane], each cap_tok rows
-    const SplitMat xs{e->xs.p, e->xs.p + (size_t)e->cap_tok * d}, cs{e->cs.p, e->cs.p + (size_t)e->cap_tok * d},
-                   fs{e->fs.p, e->fs.p + (size_t)e->cap_tok * c.inter};
+    // split planes: [hi plane | lo plane], each cap_tok rows.  planes == 1 (fp16 precision): no producer writes a lo plane and
+    // no product reads one
+    const int planes = e->precision == EMB_PREC_FP16 ? 1 : 2;
+    auto lo_of = [&](uint16_t* hi, size_t n) -> uint16_t* { return planes == 2 ? hi + n : nullptr; };
+    const SplitMat xs{e->xs.p, lo_of(e->xs.p, (size_t)e->cap_tok * d)}, cs{e->cs.p, lo_of(e->cs.p, (size_t)e->cap_tok * d)},
+                   fs{e->fs.p, lo_of(e->fs.p, (size_t)e->cap_tok * c.inter)};
     KRAG_CUDA(cudaMemcpyAsync(e->d_tok.p, tok_ids, 4 * (size_t)n_tok, cudaMemcpyHostToDevice, st));
     KRAG_CUDA(cudaMemcpyAsync(e->d_pos.p, pos.data(), 4 * (size_t)n_tok, cudaMemcpyHostToDevice, st));
     KRAG_CUDA(cudaMemcpyAsync(e->d_off.p, tok_offsets, 4 * (size_t)(batch + 1), cudaMemcpyHostToDevice, st));
@@ -1217,46 +1288,49 @@ static bool encoder_forward(Embedder* e, int batch, const int32_t* tok_ids, cons
     const int dh = d / c.heads;
     // the QKV projection writes the split planes only (same bytes as an fp32 matrix); attention reads them on the tensor cores
     uint16_t* q_hi = e->qkv.p;
-    uint16_t* q_lo = q_hi + (size_t)n_tok * 3 * d;
+    uint16_t* q_lo = lo_of(q_hi, (size_t)n_tok * 3 * d);
     for (int l = 0; l < c.layers; ++l) {
         const size_t L = (size_t)l;
         const bool last_cls = cls_rows && l == c.layers - 1;
         launch_linear(e->di, xs, e->s_qkv[L], n_tok, 3 * d, d, e->bqkv[L].p, nullptr, false, nullptr, q_hi, q_lo, nullptr, nullptr, 0.f,
-                      nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st);
-        if (dh == 64) attention_mma<64>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, st);
-        else attention_mma<32>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, st);
+                      nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st, nullptr, planes);
+        if (planes == 1) {
+            if (dh == 64) attention_mma<64, 1>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, st);
+            else attention_mma<32, 1>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, st);
+        } else if (dh == 64) attention_mma<64, 2>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, st);
+        else attention_mma<32, 2>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, st);
         if (last_cls) {
-            const SplitMat ccs{e->ccs.p, e->ccs.p + (size_t)batch * d}, cxs{e->cxs.p, e->cxs.p + (size_t)batch * d},
-                           cfs{e->cfs.p, e->cfs.p + (size_t)batch * c.inter};
-            const GemmPlan po = linear_plan(e->di, n_tok, d, d, true, true, Embedder::WS_FLOATS);
-            const GemmPlan p1 = linear_plan(e->di, n_tok, c.inter, d, false, true, Embedder::WS_FLOATS);
-            const GemmPlan p2 = linear_plan(e->di, n_tok, d, c.inter, true, true, Embedder::WS_FLOATS);
+            const SplitMat ccs{e->ccs.p, lo_of(e->ccs.p, (size_t)batch * d)}, cxs{e->cxs.p, lo_of(e->cxs.p, (size_t)batch * d)},
+                           cfs{e->cfs.p, lo_of(e->cfs.p, (size_t)batch * c.inter)};
+            const GemmPlan po = linear_plan(e->di, n_tok, d, d, true, true, Embedder::WS_FLOATS, planes);
+            const GemmPlan p1 = linear_plan(e->di, n_tok, c.inter, d, false, true, Embedder::WS_FLOATS, planes);
+            const GemmPlan p2 = linear_plan(e->di, n_tok, d, c.inter, true, true, Embedder::WS_FLOATS, planes);
             launch_pdl(gather_cls_kernel, dim3((unsigned)((batch * 32 + 255) / 256)), dim3(256), 0, st, e->x.p, cs.hi, cs.lo, e->d_off.p, e->cx.p,
                        ccs.hi, ccs.lo, batch, d);
             launch_linear(e->di, ccs, e->s_o[L], batch, d, d, e->t[lname(l, "attention.output.dense.bias")].p, e->cx.p, false, e->cx2.p, nullptr,
                           nullptr, e->t[lname(l, "attention.output.LayerNorm.weight")].p, e->t[lname(l, "attention.output.LayerNorm.bias")].p, c.eps,
-                          e->cx.p, cxs.hi, cxs.lo, e->ws.p, Embedder::WS_FLOATS, st, &po);
+                          e->cx.p, cxs.hi, cxs.lo, e->ws.p, Embedder::WS_FLOATS, st, &po, planes);
             launch_linear(e->di, cxs, e->s_f1[L], batch, c.inter, d, e->t[lname(l, "intermediate.dense.bias")].p, nullptr, true, nullptr, cfs.hi,
-                          cfs.lo, nullptr, nullptr, 0.f, nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st, &p1);
+                          cfs.lo, nullptr, nullptr, 0.f, nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st, &p1, planes);
             launch_linear(e->di, cfs, e->s_f2[L], batch, d, c.inter, e->t[lname(l, "output.dense.bias")].p, e->cx.p, false, e->cx2.p, nullptr,
                           nullptr, e->t[lname(l, "output.LayerNorm.weight")].p, e->t[lname(l, "output.LayerNorm.bias")].p, c.eps, e->cx.p, cxs.hi,
-                          cxs.lo, e->ws.p, Embedder::WS_FLOATS, st, &p2);
+                          cxs.lo, e->ws.p, Embedder::WS_FLOATS, st, &p2, planes);
             break;
         }
         // O projection (+bias +residual) -> LayerNorm -> x (fp32 residual stream) + its split planes
         launch_linear(e->di, cs, e->s_o[L], n_tok, d, d, e->t[lname(l, "attention.output.dense.bias")].p, e->x.p, false, e->x2.p, nullptr, nullptr,
                       e->t[lname(l, "attention.output.LayerNorm.weight")].p, e->t[lname(l, "attention.output.LayerNorm.bias")].p, c.eps, e->x.p, xs.hi, xs.lo,
-                      e->ws.p, Embedder::WS_FLOATS, st);
+                      e->ws.p, Embedder::WS_FLOATS, st, nullptr, planes);
         // FFN1 (+bias, GELU): only the split planes are written (FFN2 is the sole consumer)
         launch_linear(e->di, xs, e->s_f1[L], n_tok, c.inter, d, e->t[lname(l, "intermediate.dense.bias")].p, nullptr, true, nullptr, fs.hi, fs.lo,
-                      nullptr, nullptr, 0.f, nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st);
+                      nullptr, nullptr, 0.f, nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st, nullptr, planes);
         // FFN2 (+bias +residual) -> LayerNorm -> x + split planes
         launch_linear(e->di, fs, e->s_f2[L], n_tok, d, c.inter, e->t[lname(l, "output.dense.bias")].p, e->x.p, false, e->x2.p, nullptr, nullptr,
                       e->t[lname(l, "output.LayerNorm.weight")].p, e->t[lname(l, "output.LayerNorm.bias")].p, c.eps, e->x.p, xs.hi, xs.lo, e->ws.p,
-                      Embedder::WS_FLOATS, st);
+                      Embedder::WS_FLOATS, st, nullptr, planes);
     }
     };   // run_layers
-    const Embedder::GraphKey key(n_tok, batch, max_len, cls_rows ? 1 : 0, seg_b ? 1 : 0);
+    const Embedder::GraphKey key(n_tok, batch, max_len, cls_rows ? 1 : 0, seg_b ? 1 : 0, e->precision);
     auto git = e->graphs.find(key);
     if (git != e->graphs.end()) {
         KRAG_CUDA(cudaGraphLaunch(git->second, st));
@@ -1343,14 +1417,15 @@ void embedder_rerank(Embedder* e, int n_queries, const int32_t* pair_off, const 
         for (int j = 0; j <= batch; ++j) offs[(size_t)j] = tok_off[p0 + j] - tok_off[p0];
         const bool cls_rows = encoder_forward(e, batch, tok_ids + tok_off[p0], offs.data(), seg_b + p0, true);
         // the [CLS] rows' split planes: where the shortened last layer left them, else gathered from the full stream
-        const SplitMat cxs{e->cxs.p, e->cxs.p + (size_t)batch * d};
+        const int planes = e->precision == EMB_PREC_FP16 ? 1 : 2;
+        const SplitMat cxs{e->cxs.p, planes == 2 ? e->cxs.p + (size_t)batch * d : nullptr};
         if (!cls_rows) {
-            const SplitMat xs{e->xs.p, e->xs.p + (size_t)e->cap_tok * d};
+            const SplitMat xs{e->xs.p, planes == 2 ? e->xs.p + (size_t)e->cap_tok * d : nullptr};
             launch_pdl(gather_cls_kernel, dim3((unsigned)((batch * 32 + 255) / 256)), dim3(256), 0, st, e->x.p, xs.hi, xs.lo, e->d_off.p,
                        e->cx.p, cxs.hi, cxs.lo, batch, d);
         }
         launch_linear(e->di, cxs, e->s_pool, batch, d, d, e->t["pooler.dense.bias"].p, nullptr, false, e->cx2.p, nullptr, nullptr, nullptr,
-                      nullptr, 0.f, nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st);
+                      nullptr, 0.f, nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st, nullptr, planes);
         classifier_head_kernel<<<(unsigned)((batch * 32 + 255) / 256), 256, 0, st>>>(e->cx2.p, e->t["classifier.weight"].p,
                                                                                    e->t["classifier.bias"].p, batch, d, act, e->scores.p + p0);
         KRAG_CUDA(cudaGetLastError());

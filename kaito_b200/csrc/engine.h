@@ -464,6 +464,10 @@ enum { EMB_POOL_CLS = 0, EMB_POOL_MEAN = 1 };   // = KRAG_POOL_CLS / KRAG_POOL_M
 void embedder_set_pooling(Embedder* e, int mode);
 // test hook: false runs the last layer over every token under CLS pooling too (same results)
 void embedder_set_cls_rows_only(Embedder* e, bool on);
+// arithmetic of every GEMM / attention product of the forward: split fp16 operands, three MMAs (fp32-accurate), or the hi
+// planes alone, one MMA; accumulation, residual stream, LayerNorm, softmax and the head are fp32 in both
+enum { EMB_PREC_FP32 = 0, EMB_PREC_FP16 = 1 };   // = KRAG_PRECISION_FP32 / KRAG_PRECISION_FP16
+void embedder_set_precision(Embedder* e, int mode);
 void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int32_t* tok_offsets, float* out_host,
                       float* out_dev = nullptr, int ld_out = 0, cudaStream_t consumer = nullptr);
 // cross-encoder reranking (classifier head loaded): scores of sentence pairs, top_k per query (see embed.cu)
@@ -479,19 +483,22 @@ void launch_split_f16(const float* in, uint16_t* hi, uint16_t* lo, int64_t n /* 
 // outputs: fp32 C and / or the split planes of C; with ln_g the row LayerNorm of that goes to Y / Y planes (C is scratch).
 // Tile width bn of the 128 x bn output tiles, K slices (splits > 1: fp32 partials in ws + a reduce kernel), and whether the
 // small-M path (bn 32 / 64 / 128, split-K, workspace) or the large-M one (128 x 128, whole K) runs.
+// planes = 1: the single-plane product (A.lo, B.lo and the lo outputs are not touched; one fp16 wgmma per step, fp32
+// accumulation), whose large-M path also has 128 x 256 tiles.
 struct GemmPlan { int bn; int splits; bool small_m; };
 // the plan launch_linear picks for M rows: 128 x 128 tiles, or 128 x BN split-K tiles for few activation tiles
-GemmPlan linear_plan(const DeviceInfo& di, int M, int N, int K, bool ln, bool have_ws, size_t ws_floats);
+GemmPlan linear_plan(const DeviceInfo& di, int M, int N, int K, bool ln, bool have_ws, size_t ws_floats, int planes = 2);
 // plan = null: linear_plan(M, ...); ws = split-K workspace (may be null)
 void launch_linear(const DeviceInfo& di, const SplitMat& A, const SplitMat& B, int M, int N, int K, const float* bias, const float* residual,
                    bool gelu, float* C, uint16_t* C_hi, uint16_t* C_lo, const float* ln_g, const float* ln_b, float eps, float* Y,
-                   uint16_t* Y_hi, uint16_t* Y_lo, float* ws, size_t ws_floats, cudaStream_t st, const GemmPlan* plan = nullptr);
+                   uint16_t* Y_hi, uint16_t* Y_lo, float* ws, size_t ws_floats, cudaStream_t st, const GemmPlan* plan = nullptr,
+                   int planes = 2);
 // test hook: fp32 device operands, split on the fly, then the path above.  tile_n = 0: launch_linear's own plan; 32, 64 or
-// 128: that tile width over the whole K range.  reps > 0: the GEMM is launched reps more times between two CUDA
+// 128 (256 with planes = 1): that tile width over the whole K range.  reps > 0: the GEMM is launched reps more times between two CUDA
 // events and *ms gets the mean time of one launch.
 void launch_linear_f32(const DeviceInfo& di, const float* A, const float* B, int M, int N, int K, const float* bias, const float* residual,
                        bool gelu, float* C, const float* ln_g, const float* ln_b, float eps, float* Y, float* ws, size_t ws_floats,
-                       cudaStream_t st, int tile_n = 0, int reps = 0, float* ms = nullptr);
+                       cudaStream_t st, int tile_n = 0, int reps = 0, float* ms = nullptr, int planes = 2);
 
 // ---- synthetic data (synth.cu)
 void launch_synth_dense(float* X, int64_t n, int d, int dpad, int64_t row_base, uint64_t seed, cudaStream_t st);

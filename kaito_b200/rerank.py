@@ -14,6 +14,15 @@ from .embedding import _json, check_bert_config, load_state
 
 RERANK_CANDIDATES = 30           # KRAG_RERANK_CANDIDATES default
 _ACTIVATIONS = {"Sigmoid": "sigmoid", "Identity": "identity"}
+PRECISIONS = ("fp32", "fp16")    # KRAG_RERANK_PRECISION; the default is the fp32-accurate forward
+
+
+def precision_from_env() -> str:
+    """KRAG_RERANK_PRECISION: "fp32" (default) or "fp16"; a ValueError for anything else"""
+    p = os.getenv("KRAG_RERANK_PRECISION") or "fp32"
+    if p not in PRECISIONS:
+        raise ValueError(f"KRAG_RERANK_PRECISION {p!r}: expected 'fp32' or 'fp16'")
+    return p
 
 
 def read_cross_encoder_spec(model_dir: str) -> dict:
@@ -113,16 +122,22 @@ class GpuCrossEncoder:
     every (query, passage) pair and returns the positions and scores of each query's top_k; `passages(ordinals, encode)` is the
     store's per-ordinal token cache (_IndexState.pair_passages), filled through `encode_passages` on a miss."""
 
-    def __init__(self, engine, tokenizer, config: dict, state_dict: dict, max_length: int = 512, activation: str = "sigmoid"):
+    def __init__(self, engine, tokenizer, config: dict, state_dict: dict, max_length: int = 512, activation: str = "sigmoid",
+                 precision: str = "fp32"):
         from . import _native
         if activation not in ("sigmoid", "identity"):
             raise ValueError(f"activation {activation!r}: expected 'sigmoid' or 'identity'")
-        self.tokenizer, self.max_length, self.activation = tokenizer, max_length, activation
+        if precision not in PRECISIONS:
+            raise ValueError(f"precision {precision!r}: expected 'fp32' or 'fp16'")
+        self.tokenizer, self.max_length, self.activation, self.precision = tokenizer, max_length, activation, precision
         self._act = _native.RERANK_SIGMOID if activation == "sigmoid" else _native.RERANK_IDENTITY
         self._emb = _native.Embedder(engine, config["num_hidden_layers"], config["hidden_size"], config["num_attention_heads"],
                                      config["intermediate_size"], config["vocab_size"], config.get("max_position_embeddings", 512),
                                      config.get("type_vocab_size", 2), config.get("layer_norm_eps", 1e-12))
         self._emb.load_state_dict(state_dict, head=True)
+        # "fp16": fp16 GEMM / attention operands, one tensor-core product per step, fp32 accumulation and everything else.  The
+        # scores of a query's candidates are only compared with each other, so they need not be held to fp32 arithmetic.
+        self._emb.set_precision(precision)
         self._mu = threading.Lock()          # one call at a time: the cross-encoder owns one set of activation buffers
 
     @classmethod

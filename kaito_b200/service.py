@@ -432,9 +432,10 @@ def main():
             raise SystemExit(f"embedding model '{cfg['embedding_model']}' is not supported by this image: {e}")
     rerank_dir = os.getenv("KRAG_RERANK_MODEL_DIR") or None
     if rerank_dir:
-        from .rerank import read_cross_encoder_spec
+        from .rerank import precision_from_env, read_cross_encoder_spec
         try:
             read_cross_encoder_spec(rerank_dir)      # refuse a cross-encoder K5 cannot run before any GPU work starts
+            rerank_precision = precision_from_env()
             if int(os.getenv("KRAG_RERANK_CANDIDATES", "30")) < 1:
                 raise ValueError("KRAG_RERANK_CANDIDATES must be >= 1")
         except ValueError as e:
@@ -469,7 +470,7 @@ def main():
     if rerank_dir:
         from .rerank import GpuCrossEncoder
         try:
-            reranker = GpuCrossEncoder.from_pretrained(ctx, rerank_dir)      # K5 + classifier head, on rank 0 after the exchange
+            reranker = GpuCrossEncoder.from_pretrained(ctx, rerank_dir, precision=rerank_precision)      # K5 + classifier head, on rank 0 after the exchange
         except ValueError as e:
             raise SystemExit(f"reranker '{rerank_dir}' is not supported by this image: {e}")
     app = create_app(vs.VectorStore(embed, engine, reranker=reranker), cfg)

@@ -6,7 +6,11 @@ wgmma per product) and the operand bytes the CTAs pull from L2 (tiles x k-blocks
 128-row activation block and a BN-row weight block, 4 (128 + BN) bytes per K element) per second.  If time per flop
 tracks bytes per flop across tile widths the GEMM is bound by the operand feed from L2; if not, by issue or latency.
 
-    python scripts/k5_gemm_probe.py [--tiles 64,128] [--reps 50]
+--f16 adds the single-plane fp16 GEMM of the fp16 precision mode (one wgmma per product, hi planes only: 2 (128 + BN) operand
+bytes per K element) at the bge-base and MiniLM shapes, M = 8192, 128 x 128 against 128 x 256 tiles: ms per launch, TFLOP/s
+from the shapes and their share of the data sheet's 989 dense fp16 TFLOP/s (H100 SXM, 700 W).
+
+    python scripts/k5_gemm_probe.py [--tiles 64,128] [--reps 50] [--f16] [--no-split]
 """
 import argparse
 import os
@@ -23,6 +27,9 @@ from kaito_b200 import _native  # noqa: E402
 M = 256 * 32
 SHAPES = [("QKV", 2304, 768, False, False), ("O", 768, 768, False, True), ("FFN1", 3072, 768, True, False),
           ("FFN2", 768, 3072, False, True)]
+MINILM_SHAPES = [("QKV", 1152, 384, False, False), ("O", 384, 384, False, True), ("FFN1", 1536, 384, True, False),
+                 ("FFN2", 384, 1536, False, True)]
+PEAK_FP16_TFLOPS = 989.0    # NVIDIA H100 SXM data sheet, dense, card allowed 700 W
 
 
 def card():
@@ -45,11 +52,17 @@ def main():
     ap.add_argument("--tiles", default="64,128")
     ap.add_argument("--reps", type=int, default=50)
     ap.add_argument("--forward-reps", type=int, default=20)
+    ap.add_argument("--f16", action="store_true", help="also the single-plane fp16 GEMM, tiles 128 and 256")
+    ap.add_argument("--no-split", action="store_true", help="skip the split-fp16 GEMMs and the forward")
     args = ap.parse_args()
     tiles = [int(t) for t in args.tiles.split(",")]
     print(f"card: {card()}")
     ctx = _native.Context(device_id=0)
     try:
+        if args.f16:
+            probe_f16(ctx, args.reps)
+        if args.no_split:
+            return
         g = np.random.default_rng(0)
         print(f"{'GEMM':5} {'M x N x K':>17} {'BN':>4} {'ms':>8} {'TFLOP/s':>8} {'pipe':>7} {'L2 GB/s':>8} {'FLOP/B':>7}")
         for name, N, K, gelu, res in SHAPES:
@@ -67,6 +80,23 @@ def main():
         forward(ctx, args.forward_reps)
     finally:
         ctx.close()
+
+
+def probe_f16(ctx, reps):
+    g = np.random.default_rng(1)
+    print(f"{'model':8} {'GEMM':5} {'M x N x K':>17} {'BN':>4} {'ms':>8} {'TFLOP/s':>8} {'of 989':>7}")
+    for model, shapes in (("bge-base", SHAPES), ("MiniLM", MINILM_SHAPES)):
+        for name, N, K, gelu, res in shapes:
+            A = g.standard_normal((M, K)).astype(np.float32)
+            B = (g.standard_normal((N, K)) / np.sqrt(K)).astype(np.float32)
+            bias = g.standard_normal(N).astype(np.float32)
+            R = g.standard_normal((M, N)).astype(np.float32) if res else None
+            for bn in (128, 256):
+                if N % bn:
+                    continue
+                _, ms = _native.debug_gemm_time(ctx, A, B, bias, R, gelu, tile_n=bn, reps=reps, f16=True)
+                tf = 2.0 * M * N * K / ms / 1e9
+                print(f"{model:8} {name:5} {f'{M}x{N}x{K}':>17} {bn:>4} {ms:8.4f} {tf:8.1f} {tf / PEAK_FP16_TFLOPS:7.1%}")
 
 
 def forward(ctx, reps):

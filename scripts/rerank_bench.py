@@ -1,9 +1,13 @@
 """Cross-encoder reranking throughput on the GPU: krag_rerank (K5 + classifier head + top-k) at the MiniLM-L6 / L12
 cross-encoder shapes, random weights, 256 queries x N candidates, passages of fixed length; and the same pairs through torch
-BertForSequenceClassification (padded batches, SDPA) in fp32 and bf16 as the bar.  Prints one JSON line per point (--out:
-also the list of them as a JSON file).
+BertForSequenceClassification (padded batches, SDPA) in fp32 and bf16 as the bar.  The precision modes of K5 (--precision) are
+timed in the same call on the same inputs, alternating, after a warm-up of each; with both, the row also carries the mean
+top-10 overlap of their results.  Prints one JSON line per point (--out: also the list of them as a JSON file), each with the
+card name and power limit read in this call.  --profile DIR: instead of timing, one call per mode and point under
+torch.profiler, per-kernel CUDA times written to DIR/rerank_profile_<mode>.txt.
 
-  python scripts/rerank_bench.py [--models L6,L12] [--n 10,30,100] [--lens 128,256,480] [--reps 3] [--out file]"""
+  python scripts/rerank_bench.py [--models L6,L12] [--n 10,30,100] [--lens 128,256,480] [--precision fp32,fp16] [--reps 3]
+                                 [--out file] [--profile dir]"""
 import argparse
 import json
 import os
@@ -33,9 +37,14 @@ def main():
     ap.add_argument("--lens", default="128,256,480")
     ap.add_argument("--queries", type=int, default=256)
     ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--precision", default="fp32,fp16")
+    ap.add_argument("--profile", default=None)
     ap.add_argument("--no-torch", action="store_true")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
+    modes = a.precision.split(",")
+    if not modes or any(m not in ("fp32", "fp16") for m in modes) or a.reps < 1:
+        ap.error("--precision takes fp32, fp16 or both; --reps >= 1")
     import torch
     from kaito_b200 import _native
     from kaito_b200.rerank import build_pairs
@@ -50,7 +59,7 @@ def main():
         state = _state(cfg, "bench")
         enc = _encoder(ctx, cfg, state)
         tm = {}
-        if not a.no_torch:
+        if not a.no_torch and not a.profile:
             from transformers import BertConfig, BertForSequenceClassification
             m = BertForSequenceClassification(BertConfig(**cfg, num_labels=1, attn_implementation="sdpa"))
             sd = {(k if k.startswith("classifier.") else "bert." + k): torch.from_numpy(v) for k, v in state.items()}
@@ -64,17 +73,30 @@ def main():
                 flat, toff, seg, poff = build_pairs(2, 3, qs, ds, 512)
                 n_pairs, n_tok = int(poff[-1]), int(toff[-1])
                 fl = flops(cfg, np.diff(toff).tolist())
-                enc.rerank(poff, flat, toff, seg, 10)                  # warm-up (graphs are captured on the second sight)
-                enc.rerank(poff, flat, toff, seg, 10)
-                t = []
+                for mode in modes:                                     # warm-up (graphs are captured on the second sight)
+                    enc.set_precision(mode)
+                    enc.rerank(poff, flat, toff, seg, 10)
+                    enc.rerank(poff, flat, toff, seg, 10)
+                if a.profile:
+                    profile(enc, modes, (poff, flat, toff, seg, 10), a.profile, f"MiniLM-{mk} N={n} passage={plen}")
+                    continue
+                t, top = {mode: [] for mode in modes}, {}
                 for _ in range(a.reps):
-                    t0 = time.perf_counter()
-                    enc.rerank(poff, flat, toff, seg, 10)              # returns synchronised
-                    t.append(time.perf_counter() - t0)
-                s = float(np.median(t))
-                row = {"model": f"MiniLM-{mk}", "queries": a.queries, "N": n, "passage_tokens": plen, "pairs": n_pairs, "tokens": n_tok,
-                       "krag_ms": s * 1e3, "pairs_per_s": n_pairs / s, "tokens_per_s": n_tok / s, "tflops_fp32_equiv": fl / s / 1e12,
-                       "gpu": gpu}
+                    for mode in modes:                                 # alternating: both modes see the same minutes of the card
+                        enc.set_precision(mode)
+                        t0 = time.perf_counter()
+                        top[mode] = enc.rerank(poff, flat, toff, seg, 10)[0]      # returns synchronised
+                        t[mode].append(time.perf_counter() - t0)
+                row = {"model": f"MiniLM-{mk}", "queries": a.queries, "N": n, "passage_tokens": plen, "pairs": n_pairs, "tokens": n_tok}
+                for mode in modes:
+                    s = float(np.median(t[mode]))
+                    sfx = "" if mode == "fp32" else "_fp16"
+                    row.update({f"krag{sfx}_ms": s * 1e3, f"pairs_per_s{sfx}": n_pairs / s, f"tokens_per_s{sfx}": n_tok / s,
+                                f"tflops_fp32_equiv{sfx}": fl / s / 1e12})
+                if len(modes) == 2:
+                    row["top10_overlap"] = float(np.mean([len(set(x.tolist()) & set(y.tolist())) / 10.0
+                                                          for x, y in zip(top["fp32"], top["fp16"])]))
+                row["gpu"] = gpu
                 for name, m in tm.items():
                     L = int(np.diff(toff).max())
                     ids = torch.zeros((n_pairs, L), dtype=torch.int64)
@@ -100,9 +122,21 @@ def main():
                 print(json.dumps(row), flush=True)
                 rows.append(row)
         enc.destroy()
-    if a.out:
+    if a.out and not a.profile:
         with open(a.out, "w") as f:
             json.dump(rows, f, indent=1)
+
+
+def profile(enc, modes, call, out_dir, label):
+    """per-kernel CUDA time of one krag_rerank call per mode (tracing slows the host: no end-to-end time is taken here)"""
+    from torch.profiler import ProfilerActivity, profile as torch_profile
+    os.makedirs(out_dir, exist_ok=True)
+    for mode in modes:
+        enc.set_precision(mode)
+        with torch_profile(activities=[ProfilerActivity.CUDA]) as prof:
+            enc.rerank(*call)
+        with open(os.path.join(out_dir, f"rerank_profile_{mode}.txt"), "a") as f:
+            f.write(f"== {label} {mode}\n{prof.key_averages().table(sort_by='cuda_time_total', row_limit=12, max_name_column_width=60)}\n")
 
 
 if __name__ == "__main__":
