@@ -324,15 +324,21 @@ int32_t krag_embedder_set_pooling(krag_embedder* e, int32_t mode);
 #define KRAG_PRECISION_FP32 0
 #define KRAG_PRECISION_FP16 1
 int32_t krag_embedder_set_precision(krag_embedder* e, int32_t mode);
+/* Position row of a sequence's first token (default 0): token i of every sequence takes position row off + i, so a
+ * sequence may hold at most max_position - off tokens (else the forward is KRAG_E_INVALID).  RoBERTa / XLM-RoBERTa models
+ * number positions from pad_token_id + 1 (= 2).  off >= 0; may be called before or after finalize and between forwards. */
+int32_t krag_embedder_set_position_offset(krag_embedder* e, int32_t off);
 /* Under CLS pooling the last layer's O projection, FFN and LayerNorms run on the [CLS] rows only (on = 1, the default).
  * on = 0 runs them over every token; the embeddings are the same bits either way.  Test hook. */
 int32_t krag_debug_embedder_cls_rows(krag_embedder* e, int32_t on);
 /* Cross-encoder reranking (BertForSequenceClassification with one label).  The embedder must have been loaded with the
  * head as well: "pooler.dense.weight" [hidden, hidden], "pooler.dense.bias", "classifier.weight" [1, hidden] and
  * "classifier.bias" [1].  Query i owns pairs pair_offsets[i] .. pair_offsets[i+1] (0 to 300 of them); pair p is the packed
- * sequence tok_ids[tok_offsets[p] .. tok_offsets[p+1]) = [CLS] query [SEP] passage [SEP] (at most max_position tokens), whose
- * tokens from seg_b[p] on (the first passage token, in [1, length]) take token type 1.  score = activation(classifier .
- * tanh(pooler([CLS] row))).  out_pos / out_score [n_queries, top_k]: per query its best top_k pairs (position within the
+ * sequence tok_ids[tok_offsets[p] .. tok_offsets[p+1]) = [CLS] query [SEP] passage [SEP] (at most max_position - the
+ * position offset tokens), whose tokens from seg_b[p] on (the first passage token, in [1, length]) take token type 1.
+ * seg_b = NULL: unsegmented pairs, every token takes token type 0 (XLM-RoBERTa's <s> query </s></s> passage </s>; any
+ * type_vocab >= 1).  score = activation(classifier . tanh(pooler([CLS] row))); an XLM-RoBERTa head (classifier.dense,
+ * classifier.out_proj) is the same arithmetic, loaded under the pooler / classifier names.  out_pos / out_score [n_queries, top_k]: per query its best top_k pairs (position within the
  * query's pairs), scores descending, equal scores by position ascending; -1 / NaN past the query's pair count.  All
  * arguments are HOST memory; the call returns synchronised.  KRAG_E_INVALID: head missing, top_k outside [1, 300],
  * unknown activation, a pair too long or seg_b out of range. */
@@ -358,6 +364,22 @@ int32_t krag_wordpiece_create(const char* vocab, int64_t len, int32_t lower_case
 int32_t krag_wordpiece_encode_batch(const krag_wordpiece* w, int64_t n, const char* texts, const int64_t* offsets /*[n+1]*/,
                                     int32_t max_len, int32_t* out_ids /*[n * max_len]*/, int32_t* out_n /*[n]*/);
 int32_t krag_wordpiece_destroy(krag_wordpiece* w);
+/* krag_text_unigram_*: the SentencePiece Unigram tokeniser of XLM-RoBERTa models (bge-reranker-*) as the Rust `tokenizers`
+ *   library runs a tokenizer.json, over tables the host parsed from it (kaito_b200/text.py, read_unigram_json):
+ *   pieces = the model's pieces concatenated, piece i = pieces[piece_off[i] .. piece_off[i+1]) with log-probability
+ *   scores[i]; unk_id; charsmap = the decoded normalizer precompiled_charsmap (charsmap_len 0: no normaliser); flags =
+ *   1 (Replace " {2,}" -> " " after it) | 2 (WhitespaceSplit before Metaspace) | 4 (Metaspace prepend_scheme "first",
+ *   else "always"); the added tokens likewise packed, with their ids and added_strip = 1 (lstrip) | 2 (rstrip).
+ *   encode_batch writes the ids of text i without <s> / </s>, untruncated, into out_ids[i * cap ...] (at most cap of them)
+ *   and their count into out_n[i] (which may exceed cap: call again with a larger cap). */
+typedef struct krag_unigram krag_unigram;
+int32_t krag_text_unigram_create(const char* pieces, const int64_t* piece_off /*[n_pieces+1]*/, const double* scores,
+                                 int64_t n_pieces, int32_t unk_id, const char* charsmap, int64_t charsmap_len, int32_t flags,
+                                 const char* added, const int64_t* added_off /*[n_added+1]*/, const int32_t* added_ids,
+                                 const int32_t* added_strip, int32_t n_added, krag_unigram** out);
+int32_t krag_text_unigram_encode_batch(const krag_unigram* u, int64_t n, const char* texts, const int64_t* offsets /*[n+1]*/,
+                                       int32_t cap, int32_t* out_ids /*[n * cap]*/, int32_t* out_n /*[n]*/);
+int32_t krag_text_unigram_destroy(krag_unigram* u);
 
 /* ------------------------------------------------------------------- diagnostics */
 /* C[M,N] = A[M,K] . B[N,K]^T + bias (+erf-GELU) (+residual) through K5's split-fp16 wgmma GEMM; host buffers.

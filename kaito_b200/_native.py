@@ -41,6 +41,8 @@ SYMBOLS = [
     "krag_last_commit", "krag_index_alive_bitmap", "krag_redeal_begin", "krag_redeal_tables", "krag_redeal_prepare",
     "krag_dev_redeal_pack", "krag_dev_redeal_unpack", "krag_redeal_finish", "krag_redeal_abort", "krag_embedder_set_pooling",
     "krag_debug_embedder_cls_rows", "krag_rerank", "krag_embedder_set_precision", "krag_debug_gemm_f16",
+    "krag_embedder_set_position_offset", "krag_text_unigram_create", "krag_text_unigram_encode_batch",
+    "krag_text_unigram_destroy",
 ]
 # krag_embedder_set_precision: split-fp16 products held to fp32 arithmetic, or fp16 operands with fp32 accumulation
 PRECISIONS = {"fp32": 0, "fp16": 1}
@@ -134,6 +136,7 @@ def load() -> C.CDLL:
     L.krag_embedder_set_pooling.argtypes = [vp, i32]
     L.krag_debug_embedder_cls_rows.argtypes = [vp, i32]
     L.krag_embedder_set_precision.argtypes = [vp, i32]
+    L.krag_embedder_set_position_offset.argtypes = [vp, i32]
     L.krag_rerank.argtypes = [vp, i32, vp, vp, vp, vp, i32, i32, vp, vp]
     L.krag_embedder_destroy.argtypes = [vp]
     L.krag_debug_gemm_tf32.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp, i32, vp, i32, i32, C.POINTER(C.c_float)]
@@ -144,6 +147,10 @@ def load() -> C.CDLL:
     L.krag_wordpiece_create.argtypes = [C.c_char_p, i64, i32, C.POINTER(vp)]
     L.krag_wordpiece_encode_batch.argtypes = [vp, i64, C.c_char_p, vp, i32, vp, vp]
     L.krag_wordpiece_destroy.argtypes = [vp]
+    L.krag_text_unigram_create.argtypes = [C.c_char_p, vp, vp, i64, i32, C.c_char_p, i64, i32, C.c_char_p, vp, vp, vp, i32,
+                                           C.POINTER(vp)]
+    L.krag_text_unigram_encode_batch.argtypes = [vp, i64, C.c_char_p, vp, i32, vp, vp]
+    L.krag_text_unigram_destroy.argtypes = [vp]
     L.krag_p2p_create.argtypes = [vp, i32, i32, i32, i32, C.POINTER(vp), vp]
     L.krag_p2p_connect.argtypes = [vp, vp]
     L.krag_dev_exchange_merge.argtypes = [vp, i32, i32, i32, vp, vp, vp]
@@ -350,12 +357,16 @@ class Embedder:
             raise ValueError(f"precision {precision!r}: expected 'fp32' or 'fp16'")
         check(self._L.krag_embedder_set_precision(self._h, PRECISIONS[precision]))
 
+    def set_position_offset(self, off: int):
+        """position row of every sequence's first token (krag_embedder_set_position_offset; XLM-R: pad_token_id + 1)"""
+        check(self._L.krag_embedder_set_position_offset(self._h, off))
+
     def rerank(self, pair_offsets, flat_tokens, tok_offsets, seg_b, top_k: int, activation: int = RERANK_SIGMOID):
         """krag_rerank: (positions int32 [n_queries, top_k], scores float32 [n_queries, top_k]); -1 / NaN past a query's
-        pair count"""
+        pair count.  seg_b None: unsegmented pairs (token type 0 throughout)"""
         pair_offsets = np.ascontiguousarray(pair_offsets, np.int32)
         flat_tokens = np.ascontiguousarray(flat_tokens, np.int32); tok_offsets = np.ascontiguousarray(tok_offsets, np.int32)
-        seg_b = np.ascontiguousarray(seg_b, np.int32)
+        seg_b = None if seg_b is None else np.ascontiguousarray(seg_b, np.int32)
         nq = len(pair_offsets) - 1
         pos = np.empty((nq, top_k), np.int32)
         sc = np.empty((nq, top_k), np.float32)

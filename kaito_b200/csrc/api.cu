@@ -1687,6 +1687,14 @@ int32_t krag_embedder_set_precision(krag_embedder* h, int32_t mode)
         embedder_set_precision(h->e, mode);
     });
 }
+int32_t krag_embedder_set_position_offset(krag_embedder* h, int32_t off)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(h, KRAG_E_INVALID, "null embedder");
+        KRAG_REQUIRE(off >= 0, KRAG_E_INVALID, "position offset must be >= 0");
+        embedder_set_position_offset(h->e, off);
+    });
+}
 int32_t krag_debug_embedder_cls_rows(krag_embedder* h, int32_t on)
 {
     return guarded([&] {
@@ -1700,7 +1708,7 @@ int32_t krag_rerank(krag_embedder* h, int32_t n_queries, const int32_t* pair_off
 {
     return guarded([&] {
         KRAG_REQUIRE(h && pair_offsets && out_pos && out_score && n_queries >= 1, KRAG_E_INVALID, "bad argument");
-        KRAG_REQUIRE(pair_offsets[n_queries] == 0 || (tok_ids && tok_offsets && seg_b), KRAG_E_INVALID, "bad argument");
+        KRAG_REQUIRE(pair_offsets[n_queries] == 0 || (tok_ids && tok_offsets), KRAG_E_INVALID, "bad argument");
         KRAG_CUDA(cudaSetDevice(h->ctx->di.device));
         embedder_rerank(h->e, n_queries, pair_offsets, tok_ids, tok_offsets, seg_b, activation, top_k, out_pos, out_score);
     });

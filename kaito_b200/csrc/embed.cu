@@ -1032,6 +1032,8 @@ struct Embedder {
     std::map<GraphKey, int> seen;
     int precision = EMB_PREC_FP32;        // EMB_PREC_FP16: single-plane products (the hi planes of weights and activations)
     int pooling = EMB_POOL_CLS;           // read by the final writer, which runs outside the captured graphs
+    int pos_off = 0;                      // position row of a sequence's first token: built into the host's position array,
+                                          // which is uploaded before a graph launches, so no captured pointer or shape depends on it
     bool cls_rows_only = true;            // CLS pooling: the last layer after QKV + attention runs on the [CLS] rows only
     // workspaces, grown on demand
     int cap_tok = 0, cap_batch = 0;
@@ -1192,6 +1194,12 @@ void embedder_set_precision(Embedder* e, int mode)
     e->precision = mode;
 }
 
+void embedder_set_position_offset(Embedder* e, int off)
+{
+    if (off < 0) throw std::runtime_error("embedder: the position offset must be >= 0");
+    e->pos_off = off;
+}
+
 template <int G>
 static void launch_mean_normalize(const float* x, const int32_t* seq_off, float* out, int batch, int ld_out, cudaStream_t st)
 {
@@ -1235,11 +1243,13 @@ static bool encoder_forward(Embedder* e, int batch, const int32_t* tok_ids, cons
     std::vector<int32_t> pos((size_t)n_tok), typ(seg_b ? (size_t)n_tok : 0);
     if (seg_b && c.type_vocab < 2)          // finalize: the token type table holds type_vocab rows
         throw std::runtime_error("embedder: sentence pairs need token type row 1 (type_vocab_size >= 2)");
+    const int off = e->pos_off;
     for (int b = 0; b < batch; ++b) {
         const int len = tok_offsets[b + 1] - tok_offsets[b];
-        if (len < 1 || len > c.max_pos) throw std::runtime_error("embedder: sequence length must be in [1, max_position]");
+        if (len < 1 || len > c.max_pos - off)
+            throw std::runtime_error("embedder: sequence length must be in [1, max_position - position offset]");
         max_len = len > max_len ? len : max_len;
-        for (int i = 0; i < len; ++i) pos[(size_t)tok_offsets[b] + i] = i;
+        for (int i = 0; i < len; ++i) pos[(size_t)tok_offsets[b] + i] = off + i;
         if (seg_b) {
             if (seg_b[b] < 1 || seg_b[b] > len) throw std::runtime_error("embedder: segment B must start in [1, sequence length]");
             for (int i = 0; i < len; ++i) typ[(size_t)tok_offsets[b] + i] = i >= seg_b[b] ? 1 : 0;
@@ -1382,7 +1392,7 @@ void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int3
 
 // Cross-encoder reranking.  Pairs [CLS] q [SEP] d [SEP] of n_queries queries, packed: query i owns pairs
 // pair_off[i] .. pair_off[i + 1] (at most RERANK_MAX_CANDIDATES), pair p is tok_ids[tok_off[p] .. tok_off[p + 1]) with
-// segment B from seg_b[p].  The pairs go through forwards of at most RERANK_MAX_TOKENS tokens (whole pairs), each followed by
+// segment B from seg_b[p]; seg_b null (XLM-R's <s> q </s></s> d </s>): type row 0 for every token.  The pairs go through forwards of at most RERANK_MAX_TOKENS tokens (whole pairs), each followed by
 // the pooler GEMM and the classifier head, which write the pair's score at its offset in one buffer; one select kernel then
 // orders every query's scores and one copy brings back [n_queries, top_k] positions (within the query's pairs, -1 past its
 // count) and scores.
@@ -1402,7 +1412,8 @@ void embedder_rerank(Embedder* e, int n_queries, const int32_t* pair_off, const 
     if (n_pairs > 0 && tok_off[0] != 0) throw std::runtime_error("embedder: token offsets must start at 0");
     for (int p = 0; p < n_pairs; ++p) {
         const int len = tok_off[p + 1] - tok_off[p];
-        if (len < 1 || len > e->cfg.max_pos) throw std::runtime_error("embedder: a pair's length must be in [1, max_position]");
+        if (len < 1 || len > e->cfg.max_pos - e->pos_off)
+            throw std::runtime_error("embedder: a pair's length must be in [1, max_position - position offset]");
     }
     cudaStream_t st = e->st;
     if (e->scores.cap < (n_pairs > 0 ? n_pairs : 1)) e->scores.alloc(n_pairs > 0 ? n_pairs : 1);
@@ -1415,7 +1426,7 @@ void embedder_rerank(Embedder* e, int n_queries, const int32_t* pair_off, const 
         const int batch = p1 - p0;
         offs.assign((size_t)batch + 1, 0);
         for (int j = 0; j <= batch; ++j) offs[(size_t)j] = tok_off[p0 + j] - tok_off[p0];
-        const bool cls_rows = encoder_forward(e, batch, tok_ids + tok_off[p0], offs.data(), seg_b + p0, true);
+        const bool cls_rows = encoder_forward(e, batch, tok_ids + tok_off[p0], offs.data(), seg_b ? seg_b + p0 : nullptr, true);
         // the [CLS] rows' split planes: where the shortened last layer left them, else gathered from the full stream
         const int planes = e->precision == EMB_PREC_FP16 ? 1 : 2;
         const SplitMat cxs{e->cxs.p, planes == 2 ? e->cxs.p + (size_t)batch * d : nullptr};

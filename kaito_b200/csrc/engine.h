@@ -468,6 +468,8 @@ void embedder_set_cls_rows_only(Embedder* e, bool on);
 // planes alone, one MMA; accumulation, residual stream, LayerNorm, softmax and the head are fp32 in both
 enum { EMB_PREC_FP32 = 0, EMB_PREC_FP16 = 1 };   // = KRAG_PRECISION_FP32 / KRAG_PRECISION_FP16
 void embedder_set_precision(Embedder* e, int mode);
+// first position row of every sequence (RoBERTa / XLM-R: pad_token_id + 1); token i of a sequence takes row off + i
+void embedder_set_position_offset(Embedder* e, int off);
 void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int32_t* tok_offsets, float* out_host,
                       float* out_dev = nullptr, int ld_out = 0, cudaStream_t consumer = nullptr);
 // cross-encoder reranking (classifier head loaded): scores of sentence pairs, top_k per query (see embed.cu)

@@ -8,8 +8,11 @@
 // these functions are tested against (tests/test_text_native.py); the host calls the native path for ASCII text only.
 // No CUDA in this file; it is part of libkaito_rag.so so that a cgo host gets the same analysis as the Python host.
 #include <stdint.h>
+#include <stddef.h>
 #include <string.h>
 
+#include <algorithm>
+#include <memory>
 #include <stdexcept>
 #include <string>
 #include <thread>
@@ -263,6 +266,191 @@ struct krag_wordpiece {
     }
 };
 
+// ------------------------------------------------------------------------------------------ Unigram (XLM-R)
+// The tokenizer.json of an XLM-R snapshot as the Rust `tokenizers` library runs it, over the tables kaito_b200/text.py
+// (UnigramTokenizer, the spec) parsed: added tokens split out of the raw text, the Precompiled normaliser per grapheme
+// cluster (for ASCII input every character is a cluster of its own except "\r\n"), Replace " {2,}" -> " ", Metaspace
+// (after WhitespaceSplit when configured) and the Unigram Viterbi.
+namespace {
+inline int utf8_len(unsigned char c) { return c < 0x80 ? 1 : c < 0xE0 ? 2 : c < 0xF0 ? 3 : 4; }
+uint32_t utf8_cp(const std::string& s, size_t i, int n)
+{
+    const unsigned char* p = (const unsigned char*)s.data() + i;
+    if (n == 1) return p[0];
+    if (n == 2) return ((p[0] & 0x1Fu) << 6) | (p[1] & 0x3Fu);
+    if (n == 3) return ((p[0] & 0x0Fu) << 12) | ((p[1] & 0x3Fu) << 6) | (p[2] & 0x3Fu);
+    return ((p[0] & 0x07u) << 18) | ((p[1] & 0x3Fu) << 12) | ((p[2] & 0x3Fu) << 6) | (p[3] & 0x3Fu);
+}
+// Rust char::is_whitespace: the Unicode White_Space property
+inline bool white_space(uint32_t c)
+{
+    return (c >= 0x09 && c <= 0x0D) || c == 0x20 || c == 0x85 || c == 0xA0 || c == 0x1680 || (c >= 0x2000 && c <= 0x200A) ||
+           c == 0x2028 || c == 0x2029 || c == 0x202F || c == 0x205F || c == 0x3000;
+}
+const char kMeta[] = "\xE2\x96\x81";   // U+2581, Metaspace's replacement
+constexpr double kUnkPenalty = 10.0;
+}  // namespace
+
+struct krag_unigram {
+    enum { COLLAPSE_SPACES = 1, WS_SPLIT = 2, PREPEND_FIRST = 4 };
+    // pieces: a byte trie with one hash table of edges (node << 8 | byte) -> child; node_id[node] = piece id or -1
+    std::unordered_map<uint64_t, int32_t> edge;
+    std::vector<int32_t> node_id{-1};
+    std::unordered_map<std::string, int32_t> ids;   // for a fused run of unknowns, looked up as a whole
+    std::vector<double> score;
+    int32_t unk = 0;
+    double min_score = 0.0;
+    // darts-clone double array of the precompiled charsmap and the NUL-terminated replacements after it
+    std::vector<uint32_t> units;
+    std::string repl;
+    int flags = 0;
+    struct Added { std::string s; int32_t id; bool lstrip, rstrip; };
+    std::vector<Added> added;       // longest first: the first that matches at a position is the leftmost-longest match
+
+    // replacement of the shortest charsmap key that prefixes key[0, n) (the Rust normaliser's results[0]), or null
+    const char* charsmap(const char* key, size_t n) const
+    {
+        if (units.empty()) return nullptr;
+        auto offset = [](uint32_t u) { return (size_t)((u >> 10) << ((u & (1u << 9)) >> 6)); };
+        size_t node = offset(units[0]);
+        for (size_t i = 0; i < n; ++i) {
+            const unsigned char c = (unsigned char)key[i];
+            if (c == 0) break;
+            node ^= c;
+            if (node >= units.size()) return nullptr;
+            const uint32_t u = units[node];
+            if ((u & ((1u << 31) | 0xFFu)) != c) return nullptr;
+            node ^= offset(u);
+            if ((u >> 8) & 1) {
+                if (node >= units.size()) return nullptr;
+                const size_t v = units[node] & ((1u << 31) - 1);
+                return v < repl.size() ? repl.c_str() + v : nullptr;
+            }
+        }
+        return nullptr;
+    }
+    void normalize(const char* s, size_t n, std::string& out) const
+    {
+        out.clear();
+        for (size_t i = 0; i < n;) {
+            const size_t g = (s[i] == '\r' && i + 1 < n && s[i + 1] == '\n') ? 2 : 1;   // ASCII grapheme clusters
+            const char* r = charsmap(s + i, g);
+            if (r) { out += r; i += g; continue; }
+            for (size_t k = 0; k < g; ++k, ++i) {
+                const char* rc = g > 1 ? charsmap(s + i, 1) : nullptr;
+                if (rc) out += rc; else out += s[i];
+            }
+        }
+        if (flags & COLLAPSE_SPACES) {
+            size_t w = 0;
+            for (size_t i = 0; i < out.size(); ++i)
+                if (!(out[i] == ' ' && i > 0 && out[i - 1] == ' ')) out[w++] = out[i];   // out[i - 1] is still the input byte
+            out.resize(w);
+        }
+    }
+    void viterbi(const std::string& w, std::vector<int32_t>& ids_out) const
+    {
+        const size_t n = w.size();
+        if (n == 0) return;
+        struct Node { double best; int64_t start; int32_t id; };
+        std::vector<Node> nodes(n + 1, Node{0.0, -1, 0});
+        nodes[0].start = 0;
+        const double unk_score = min_score - kUnkPenalty;
+        for (size_t i = 0; i < n;) {
+            const size_t mb = (size_t)utf8_len((unsigned char)w[i]);
+            const double base = nodes[i].best;
+            bool single = false;
+            int32_t node = 0;
+            for (size_t j = i; j < n; ++j) {
+                auto it = edge.find(((uint64_t)node << 8) | (unsigned char)w[j]);
+                if (it == edge.end()) break;
+                node = it->second;
+                const int32_t id = node_id[(size_t)node];
+                if (id < 0) continue;
+                Node& t = nodes[j + 1];
+                const double c = score[(size_t)id] + base;
+                if (t.start < 0 || c > t.best) { t.best = c; t.start = (int64_t)i; t.id = id; }
+                if (j + 1 - i == mb) single = true;
+            }
+            if (!single) {
+                Node& t = nodes[i + mb];
+                const double c = unk_score + base;
+                if (t.start < 0 || c > t.best) { t.best = c; t.start = (int64_t)i; t.id = unk; }
+            }
+            i += mb;
+        }
+        const size_t mark = ids_out.size();
+        int64_t end = (int64_t)n, run_end = -1;
+        auto flush_run = [&](int64_t from) {
+            auto it = ids.find(w.substr((size_t)from, (size_t)(run_end - from)));
+            ids_out.push_back(it == ids.end() ? unk : it->second);
+            run_end = -1;
+        };
+        while (end > 0) {
+            const Node& t = nodes[(size_t)end];
+            if (t.id == unk) { if (run_end < 0) run_end = end; }
+            else {
+                if (run_end >= 0) flush_run(end);
+                ids_out.push_back(t.id);
+            }
+            end = t.start;
+        }
+        if (run_end >= 0) flush_run(0);
+        std::reverse(ids_out.begin() + (ptrdiff_t)mark, ids_out.end());
+    }
+    // Metaspace over one normalised segment (after WhitespaceSplit when configured), then the Viterbi of every piece
+    void pre_tokenize(const std::string& s, bool at_origin, std::vector<int32_t>& out) const
+    {
+        std::string word, piece;
+        auto emit = [&](size_t from, size_t to) {
+            word.clear();
+            for (size_t i = from; i < to; ++i) { if (s[i] == ' ') word += kMeta; else word += s[i]; }
+            if (word.empty()) return;
+            const bool prepend = word.compare(0, 3, kMeta) != 0 && (!(flags & PREPEND_FIRST) || (at_origin && from == 0));
+            if (prepend) word.insert(0, kMeta);
+            size_t p0 = 0;
+            for (size_t i = 3; i + 3 <= word.size(); ++i)
+                if (word.compare(i, 3, kMeta) == 0) { viterbi(word.substr(p0, i - p0), out); p0 = i; i += 2; }
+            viterbi(word.substr(p0), out);
+        };
+        if (!(flags & WS_SPLIT)) { emit(0, s.size()); return; }
+        size_t start = SIZE_MAX;
+        for (size_t i = 0; i < s.size();) {
+            const int m = utf8_len((unsigned char)s[i]);
+            const bool ws = white_space(utf8_cp(s, i, m));
+            if (ws && start != SIZE_MAX) { emit(start, i); start = SIZE_MAX; }
+            else if (!ws && start == SIZE_MAX) start = i;
+            i += (size_t)m;
+        }
+        if (start != SIZE_MAX) emit(start, s.size());
+    }
+    // ids of one ASCII text without <s> / </s>
+    void encode(const char* t, size_t n, std::vector<int32_t>& out) const
+    {
+        out.clear();
+        std::string norm;
+        auto segment = [&](size_t a, size_t b) {
+            normalize(t + a, b - a, norm);
+            pre_tokenize(norm, a == 0, out);
+        };
+        auto ws = [&](char c) { return c == ' ' || (c >= 0x09 && c <= 0x0D); };
+        size_t pos = 0;
+        for (size_t i = 0; i < n;) {
+            const Added* m = nullptr;
+            for (const Added& a : added)
+                if (a.s.size() <= n - i && memcmp(t + i, a.s.data(), a.s.size()) == 0) { m = &a; break; }
+            if (!m) { ++i; continue; }
+            size_t start = i, stop = i + m->s.size();
+            if (m->lstrip) { while (start > pos && ws(t[start - 1])) --start; }
+            if (m->rstrip) { while (stop < n && ws(t[stop])) ++stop; }
+            if (pos < start) segment(pos, start);
+            out.push_back(m->id);
+            pos = i = stop;
+        }
+        if (pos < n) segment(pos, n);
+    }
+};
+
 namespace {
 thread_local std::string g_text_err;
 template <class F>
@@ -341,6 +529,73 @@ int32_t krag_wordpiece_encode_batch(const krag_wordpiece* w, int64_t n, const ch
 int32_t krag_wordpiece_destroy(krag_wordpiece* w)
 {
     delete w;
+    return KRAG_OK;
+}
+
+int32_t krag_text_unigram_create(const char* pieces, const int64_t* piece_off, const double* scores, int64_t n_pieces, int32_t unk_id,
+                                 const char* charsmap, int64_t charsmap_len, int32_t flags, const char* added, const int64_t* added_off,
+                                 const int32_t* added_ids, const int32_t* added_strip, int32_t n_added, krag_unigram** out)
+{
+    return text_guard([&] {
+        if (!pieces || !piece_off || !scores || !out || n_pieces < 1 || unk_id < 0 || unk_id >= n_pieces || charsmap_len < 0 ||
+            n_added < 0 || (n_added && (!added || !added_off || !added_ids || !added_strip)) || (charsmap_len && !charsmap))
+            throw std::invalid_argument("bad argument");
+        auto u = std::make_unique<krag_unigram>();
+        u->unk = unk_id;
+        u->flags = flags;
+        u->score.assign(scores, scores + n_pieces);
+        u->min_score = *std::min_element(u->score.begin(), u->score.end());
+        for (int64_t p = 0; p < n_pieces; ++p) {
+            const std::string s(pieces + piece_off[p], (size_t)(piece_off[p + 1] - piece_off[p]));
+            u->ids[s] = (int32_t)p;                     // a repeated piece keeps its last id
+            int32_t node = 0;
+            for (unsigned char c : s) {
+                auto it = u->edge.find(((uint64_t)node << 8) | c);
+                if (it == u->edge.end()) {
+                    it = u->edge.emplace(((uint64_t)node << 8) | c, (int32_t)u->node_id.size()).first;
+                    u->node_id.push_back(-1);
+                }
+                node = it->second;
+            }
+            if (node) u->node_id[(size_t)node] = (int32_t)p;
+        }
+        if (charsmap_len) {
+            uint32_t n = 0;
+            memcpy(&n, charsmap, 4);                    // little-endian hosts only (x86-64, aarch64)
+            if (charsmap_len < 4 || n % 4 || 4 + (int64_t)n > charsmap_len) throw std::invalid_argument("charsmap");
+            u->units.resize(n / 4);
+            memcpy(u->units.data(), charsmap + 4, n);
+            u->repl.assign(charsmap + 4 + n, (size_t)(charsmap_len - 4 - n));
+        }
+        for (int32_t a = 0; a < n_added; ++a)
+            u->added.push_back({std::string(added + added_off[a], (size_t)(added_off[a + 1] - added_off[a])), added_ids[a],
+                                (added_strip[a] & 1) != 0, (added_strip[a] & 2) != 0});
+        std::stable_sort(u->added.begin(), u->added.end(), [](const krag_unigram::Added& x, const krag_unigram::Added& y) {
+            return x.s.size() > y.s.size();
+        });
+        u->added.erase(std::remove_if(u->added.begin(), u->added.end(), [](const krag_unigram::Added& x) { return x.s.empty(); }),
+                       u->added.end());
+        *out = u.release();
+    });
+}
+
+int32_t krag_text_unigram_encode_batch(const krag_unigram* u, int64_t n, const char* texts, const int64_t* offsets /*[n+1]*/,
+                                       int32_t cap, int32_t* out_ids /*[n * cap]*/, int32_t* out_n /*[n]*/)
+{
+    return text_guard([&] {
+        if (!u || !texts || !offsets || !out_ids || !out_n || n < 0 || cap < 1) throw std::invalid_argument("bad argument");
+        parallel_for(n, offsets[n] - offsets[0], [&](int64_t i) {
+            std::vector<int32_t> ids;
+            u->encode(texts + offsets[i], (size_t)(offsets[i + 1] - offsets[i]), ids);
+            out_n[i] = (int32_t)ids.size();
+            memcpy(out_ids + i * (int64_t)cap, ids.data(), std::min(ids.size(), (size_t)cap) * sizeof(int32_t));
+        });
+    });
+}
+
+int32_t krag_text_unigram_destroy(krag_unigram* u)
+{
+    delete u;
     return KRAG_OK;
 }
 

@@ -429,3 +429,330 @@ class WordPieceTokenizer:
             if out[i] is None:
                 out[i] = self.encode_py(t)
         return out
+
+
+# ------------------------------------------------------ Unigram (XLM-RoBERTa / bge-reranker tokeniser)
+# What the Rust `tokenizers` library does with the tokenizer.json of an XLM-R snapshot, restated: added tokens matched in the
+# raw text, the SentencePiece `Precompiled` normaliser (optionally followed by Replace " {2,}" -> " "), the `Metaspace`
+# pre-tokeniser (alone or after `WhitespaceSplit`) and the `Unigram` model's Viterbi.  The native path
+# (krag_text_unigram_*, csrc/text_native.cpp) runs the same tables for ASCII text.
+import base64  # noqa: E402
+import json  # noqa: E402
+
+_METASPACE = "▁"
+# Rust char::is_whitespace (the Unicode White_Space property), which WhitespaceSplit and an added token's lstrip / rstrip use
+_WHITE_SPACE = frozenset(chr(c) for c in (*range(0x09, 0x0E), 0x20, 0x85, 0xA0, 0x1680, *range(0x2000, 0x200B), 0x2028,
+                                          0x2029, 0x202F, 0x205F, 0x3000))
+_UNK_PENALTY = 10.0                       # an uncovered character scores min_score - 10 (sentencepiece's kUnkPenalty)
+
+
+class _Charsmap:
+    """The `precompiled_charsmap` of a SentencePiece normaliser: a little-endian u32 trie size, a darts-clone double-array
+    trie of that many bytes whose values index the NUL-terminated replacement strings that follow it."""
+
+    def __init__(self, blob: bytes, where: str):
+        if len(blob) < 4:
+            raise ValueError(f"{where}: normalizer.precompiled_charsmap: {len(blob)} bytes, too short for its trie size")
+        n = int.from_bytes(blob[:4], "little")
+        if n % 4 or 4 + n > len(blob):
+            raise ValueError(f"{where}: normalizer.precompiled_charsmap: trie size {n} does not fit its {len(blob)} bytes")
+        self.blob = blob
+        self.units = np.frombuffer(blob, "<u4", n // 4, 4).tolist()
+        self.strings = blob[4 + n:]
+        self._memo: dict[str, str | None] = {}
+
+    def lookup(self, key: str):
+        """the replacement of the shortest key that prefixes `key` (what the Rust normaliser takes: results[0] of the
+        common-prefix search), or None"""
+        r = self._memo.get(key, 0)
+        if r != 0:
+            return r
+        r, units, node = None, self.units, 0
+        try:
+            unit = units[0]
+            node ^= (unit >> 10) << ((unit & (1 << 9)) >> 6)
+            for c in key.encode("utf-8"):
+                if c == 0:
+                    break
+                node ^= c
+                unit = units[node]
+                if unit & ((1 << 31) | 0xFF) != c:
+                    break
+                node ^= (unit >> 10) << ((unit & (1 << 9)) >> 6)
+                if (unit >> 8) & 1:
+                    v = units[node] & ((1 << 31) - 1)
+                    end = self.strings.find(b"\0", v)
+                    r = self.strings[v: end if end >= 0 else len(self.strings)].decode("utf-8")
+                    break
+        except IndexError:
+            r = None
+        self._memo[key] = r
+        return r
+
+
+def _ws_split(s: str) -> list[tuple[str, int]]:
+    """WhitespaceSplit: (word, its index in s) of every maximal run of non-White_Space characters"""
+    out, start = [], None
+    for i, ch in enumerate(s):
+        if ch in _WHITE_SPACE:
+            if start is not None:
+                out.append((s[start:i], start)); start = None
+        elif start is None:
+            start = i
+    if start is not None:
+        out.append((s[start:], start))
+    return out
+
+
+def read_unigram_json(path: str) -> dict:
+    """the tables of an XLM-R tokenizer.json, or a ValueError naming the file and the field that asks for something this
+    restatement does not do.  Returns pieces, scores, unk_id, charsmap (bytes or None), collapse_spaces, ws_split,
+    prepend ("always" | "first") and added [(content, id, lstrip, rstrip)]"""
+    try:
+        with open(path, encoding="utf-8") as f:
+            tj = json.load(f)
+    except OSError as ex:
+        raise ValueError(f"{path}: cannot be read ({ex.strerror})") from None
+    except ValueError as ex:
+        raise ValueError(f"{path}: not JSON ({ex})") from None
+    model = tj.get("model") or {}
+    if model.get("type") != "Unigram":
+        raise ValueError(f"{path}: model.type {model.get('type')!r}: the XLM-R reranker path reads Unigram models only")
+    if model.get("byte_fallback"):
+        raise ValueError(f"{path}: model.byte_fallback true: byte-fallback pieces are not restated")
+    vocab = model.get("vocab")
+    if not isinstance(vocab, list) or not vocab or not all(isinstance(v, list) and len(v) == 2 for v in vocab):
+        raise ValueError(f"{path}: model.vocab: expected a non-empty list of [piece, score]")
+    unk = model.get("unk_id")
+    if not isinstance(unk, int) or not 0 <= unk < len(vocab):
+        raise ValueError(f"{path}: model.unk_id {unk!r}: must index model.vocab")
+    # normaliser: null, Precompiled, Replace(" {2,}" -> " "), or a Sequence of those
+    norm = tj.get("normalizer")
+    steps = [] if norm is None else (norm.get("normalizers") if norm.get("type") == "Sequence" else [norm])
+    charsmap, collapse = None, False
+    for i, st in enumerate(steps or []):
+        kind = st.get("type") if isinstance(st, dict) else None
+        if kind == "Precompiled" and charsmap is None and not collapse:
+            raw = st.get("precompiled_charsmap") or ""
+            charsmap = _Charsmap(base64.b64decode(raw), path) if raw else None
+        elif (kind == "Replace" and st.get("pattern") == {"Regex": " {2,}"} and st.get("content") == " " and not collapse):
+            collapse = True
+        else:
+            raise ValueError(f"{path}: normalizer {kind!r} (step {i}): only Precompiled, optionally followed by Replace "
+                             f"' {{2,}}' -> ' ', is restated")
+    # pre-tokeniser: Metaspace, alone or after WhitespaceSplit
+    pre = tj.get("pre_tokenizer") or {}
+    seq = pre.get("pretokenizers") if pre.get("type") == "Sequence" else [pre]
+    ws = len(seq or []) == 2 and isinstance(seq[0], dict) and seq[0].get("type") == "WhitespaceSplit"
+    meta = seq[-1] if seq and isinstance(seq[-1], dict) else {}
+    if len(seq or []) != (2 if ws else 1) or meta.get("type") != "Metaspace":
+        raise ValueError(f"{path}: pre_tokenizer {pre.get('type')!r}: expected Metaspace, alone or after WhitespaceSplit")
+    scheme = meta.get("prepend_scheme") or ("always" if meta.get("add_prefix_space", True) else "never")
+    if meta.get("replacement", _METASPACE) != _METASPACE or scheme not in ("always", "first") or meta.get("split", True) is not True:
+        raise ValueError(f"{path}: pre_tokenizer Metaspace (replacement {meta.get('replacement')!r}, prepend_scheme {scheme!r}, "
+                         f"split {meta.get('split', True)!r}): expected '▁', 'always' or 'first', split true")
+    added = []
+    for t in tj.get("added_tokens") or []:
+        if t.get("normalized") or t.get("single_word"):
+            raise ValueError(f"{path}: added_tokens {t.get('content')!r}: normalized / single_word tokens are not restated")
+        added.append((t["content"], int(t["id"]), bool(t.get("lstrip")), bool(t.get("rstrip"))))
+    return {"pieces": [str(v[0]) for v in vocab], "scores": [float(v[1]) for v in vocab], "unk_id": unk, "charsmap": charsmap,
+            "collapse_spaces": collapse, "ws_split": ws, "prepend": scheme, "added": added}
+
+
+class UnigramTokenizer:
+    """XLM-RoBERTa's SentencePiece Unigram tokeniser (bge-reranker-*), read from tokenizer.json.  encode_batch_plain gives
+    what `tokenizers.Tokenizer.encode(text, add_special_tokens=False).ids` gives; `cls` / `sep` are <s> / </s>.  All-ASCII
+    batches go through the native encoder; other text through this restatement."""
+
+    def __init__(self, tables: dict, max_length: int = 512):
+        self.max_length = max_length
+        self.pieces, self.scores, self.unk = tables["pieces"], tables["scores"], tables["unk_id"]
+        self.charsmap, self.collapse, self.ws_split = tables["charsmap"], tables["collapse_spaces"], tables["ws_split"]
+        self.prepend_first = tables["prepend"] == "first"
+        self.added = tables["added"]
+        self.ids = {p: i for i, p in enumerate(self.pieces)}          # a repeated piece keeps its last id, as in Rust
+        self.min_score = min(self.scores)
+        self.max_piece = max(len(p) for p in self.pieces)
+        amap = {c: i for c, i, _, _ in self.added}
+        try:
+            self.cls, self.sep = amap.get("<s>", self.ids["<s>"]), amap.get("</s>", self.ids["</s>"])
+        except KeyError:
+            raise ValueError("tokenizer.json: <s> / </s> missing from added_tokens and model.vocab") from None
+        self._added_re = (re.compile("|".join(re.escape(c) for c, *_ in sorted(self.added, key=lambda a: -len(a[0]))))
+                          if self.added else None)
+        self._added = {c: (i, l, r) for c, i, l, r in self.added}
+        self._nat = None
+        L = _native_lib()
+        if L:
+            import ctypes as C
+            enc = [p.encode("utf-8") for p in self.pieces]
+            poff = np.zeros(len(enc) + 1, np.int64)
+            np.cumsum([len(b) for b in enc], out=poff[1:])
+            sc = np.asarray(self.scores, np.float64)
+            cm = self.charsmap.blob if self.charsmap else b""
+            aenc = [c.encode("utf-8") for c, *_ in self.added]
+            aoff = np.zeros(len(aenc) + 1, np.int64)
+            np.cumsum([len(b) for b in aenc], out=aoff[1:])
+            aid = np.asarray([i for _, i, _, _ in self.added] or [0], np.int32)
+            afl = np.asarray([int(l) | 2 * int(r) for _, _, l, r in self.added] or [0], np.int32)
+            flags = int(self.collapse) | 2 * int(self.ws_split) | 4 * int(self.prepend_first)
+            h = C.c_void_p()
+            if L.krag_text_unigram_create(b"".join(enc), poff.ctypes.data_as(C.c_void_p), sc.ctypes.data_as(C.c_void_p), len(enc),
+                                          self.unk, cm, len(cm), flags, b"".join(aenc), aoff.ctypes.data_as(C.c_void_p),
+                                          aid.ctypes.data_as(C.c_void_p), afl.ctypes.data_as(C.c_void_p), len(aenc),
+                                          C.byref(h)) == 0:
+                self._nat = h
+
+    def __del__(self):
+        if getattr(self, "_nat", None):
+            try:
+                _native_lib().krag_text_unigram_destroy(self._nat)
+            except Exception:
+                pass
+            self._nat = None
+
+    @classmethod
+    def from_file(cls, path: str, max_length: int = 512):
+        """tokenizer.json of an XLM-R snapshot; a ValueError naming the file and field it refuses"""
+        return cls(read_unigram_json(path), max_length=max_length)
+
+    # ---- the restatement (any text)
+    def _split_added(self, text: str) -> list[tuple[str, int | None, int]]:
+        """(segment, added-token id or None, segment's start in text): the added tokens' leftmost-longest matches, an lstrip
+        token taking the White_Space before it (not past the previous match), an rstrip one the White_Space after it"""
+        if self._added_re is None or not text:
+            return [(text, None, 0)]
+        out, pos = [], 0
+        for m in self._added_re.finditer(text):
+            start, stop = m.start(), m.end()
+            tid, lstrip, rstrip = self._added[m.group()]
+            if lstrip:
+                j = start
+                while j > 0 and text[j - 1] in _WHITE_SPACE:
+                    j -= 1
+                start = max(j, pos)
+            if rstrip:
+                while stop < len(text) and text[stop] in _WHITE_SPACE:
+                    stop += 1
+            if pos < start:
+                out.append((text[pos:start], None, pos))
+            out.append((text[start:stop], tid, start))
+            pos = stop
+        if pos < len(text):
+            out.append((text[pos:], None, pos))
+        return out
+
+    def _normalize(self, s: str) -> str:
+        if self.charsmap is not None:
+            import regex
+            look, out = self.charsmap.lookup, []
+            for g in regex.findall(r"\X", s):
+                if len(g.encode("utf-8")) < 6:
+                    r = look(g)
+                    if r is not None:
+                        out.append(r)
+                        continue
+                for ch in g:
+                    r = look(ch)
+                    out.append(ch if r is None else r)
+            s = "".join(out)
+        if self.collapse:
+            s = re.sub(" {2,}", " ", s)
+        return s
+
+    def _pre_tokenize(self, s: str, at_origin: bool) -> list[str]:
+        """Metaspace (after WhitespaceSplit when configured): ' ' -> U+2581, prepended to every word ("always") or to the one
+        that starts the input ("first"), then split before every U+2581"""
+        words = _ws_split(s) if self.ws_split else [(s, 0)]
+        out = []
+        for w, at in words:
+            w = w.replace(" ", _METASPACE)
+            if w and not w.startswith(_METASPACE) and (not self.prepend_first or (at_origin and at == 0)):
+                w = _METASPACE + w
+            out += [p for p in re.split(f"(?={_METASPACE})", w) if p]
+        return out
+
+    def _viterbi(self, w: str) -> list[int]:
+        """the Unigram model's best segmentation of one pre-token (Rust encode_optimized): a later path replaces an earlier
+        one only with a strictly higher score; an uncovered character is unk at min_score - 10; adjacent unks fuse"""
+        n, ids, scores, maxp = len(w), self.ids, self.scores, self.max_piece
+        if n == 0:
+            return []
+        unk_score = self.min_score - _UNK_PENALTY
+        best = [0.0] * (n + 1)
+        start = [-1] * (n + 1)
+        tok = [0] * (n + 1)
+        start[0] = 0
+        for i in range(n):
+            base = best[i]
+            single = False
+            for j in range(i + 1, min(n, i + maxp) + 1):
+                t = ids.get(w[i:j])
+                if t is None:
+                    continue
+                c = scores[t] + base
+                if start[j] < 0 or c > best[j]:
+                    best[j], start[j], tok[j] = c, i, t
+                if j == i + 1:
+                    single = True
+            if not single:
+                c = unk_score + base
+                if start[i + 1] < 0 or c > best[i + 1]:
+                    best[i + 1], start[i + 1], tok[i + 1] = c, i, self.unk
+        # back from the end; a run of unk nodes becomes one piece, looked up as a whole (not found: unk)
+        out, end, run_end = [], n, -1
+        while end > 0:
+            b = start[end]
+            if tok[end] == self.unk:
+                if run_end < 0:
+                    run_end = end
+            else:
+                if run_end >= 0:
+                    out.append(self.ids.get(w[end:run_end], self.unk)); run_end = -1
+                out.append(tok[end])
+            end = b
+        if run_end >= 0:
+            out.append(self.ids.get(w[0:run_end], self.unk))
+        out.reverse()
+        return out
+
+    def encode_py(self, text: str) -> list[int]:
+        """ids of one text without <s> / </s>, untruncated"""
+        ids = []
+        for seg, tid, at in self._split_added(text):
+            if tid is not None:
+                ids.append(tid)
+                continue
+            for w in self._pre_tokenize(self._normalize(seg), at == 0):
+                ids += self._viterbi(w)
+        return ids
+
+    # ---- batch entry points
+    def encode_batch_plain(self, texts: list[str]) -> list[np.ndarray]:
+        """int32 ids of every text without <s> / </s> and without truncation (the halves of a sentence pair); all-ASCII
+        texts in one native call"""
+        out: list = [None] * len(texts)
+        idx = [i for i, t in enumerate(texts) if self._nat is not None and t.isascii()]
+        if idx:
+            import ctypes as C
+            raws = [texts[i].encode("ascii") for i in idx]
+            offs = np.zeros(len(raws) + 1, np.int64)
+            np.cumsum([len(r) for r in raws], out=offs[1:])
+            blob = b"".join(raws)
+            cap = max(len(r) for r in raws) + 8
+            for _ in range(2):                 # the count of a text longer than cap is reported; grow once and redo
+                ids = np.empty((len(raws), cap), np.int32)
+                cnt = np.empty(len(raws), np.int32)
+                rc = _native_lib().krag_text_unigram_encode_batch(self._nat, len(raws), blob, offs.ctypes.data_as(C.c_void_p), cap,
+                                                                  ids.ctypes.data_as(C.c_void_p), cnt.ctypes.data_as(C.c_void_p))
+                if rc != 0 or int(cnt.max()) <= cap:
+                    break
+                cap = int(cnt.max())
+            if rc == 0 and int(cnt.max()) <= cap:
+                for j, i in enumerate(idx):
+                    out[i] = ids[j, : cnt[j]].copy()
+        for i, t in enumerate(texts):
+            if out[i] is None:
+                out[i] = np.asarray(self.encode_py(t), np.int32)
+        return out
