@@ -241,7 +241,12 @@ int32_t krag_retrieve(krag_index* idx, int32_t batch, const float* q,
 /* ------------------------------- stage API, DEVICE pointers (one process per GPU) */
 /* All pointers are device pointers valid on ctx's device; `stream` is a cudaStream_t
  * (NULL = legacy default stream).  These let the host place one NCCL all-gather
- * between the local candidate stage and the merge/fuse stage (SURVEY.md section 8e). */
+ * between the local candidate stage and the merge/fuse stage (SURVEY.md section 8e).
+ * The candidate stages return with their work still queued on `stream`.  That work is
+ * ordered before every later search that reuses its workspace (search_slots of them per
+ * context) and before every later mutation of the index: a mutation first waits for it
+ * (the host blocks until it has finished), so queued kernels never see rows, tombstones
+ * or postings change under them. */
 int32_t krag_dev_dense_candidates(krag_index* idx, int32_t batch, const float* d_q, int32_t P,
                                   uint64_t* d_keys_out /*[batch,P]*/, void* stream);
 int32_t krag_dev_bm25_candidates(krag_index* idx, int32_t batch, const uint32_t* d_q_terms,

@@ -117,9 +117,11 @@ struct Slot {
     DevArray<float> q_sel;
     cudaStream_t copy_st = nullptr;
     cudaEvent_t copied[2] = {nullptr, nullptr}, freed[2] = {nullptr, nullptr};
+    // recorded after the work of each call that used the slot, on the stream that work went to (SlotLease)
+    cudaEvent_t done = nullptr;
     ~Slot()
     {
-        for (cudaEvent_t e : {copied[0], copied[1], freed[0], freed[1]}) if (e) cudaEventDestroy(e);
+        for (cudaEvent_t e : {copied[0], copied[1], freed[0], freed[1], done}) if (e) cudaEventDestroy(e);
         if (copy_st) cudaStreamDestroy(copy_st);
         if (st) cudaStreamDestroy(st);
     }
@@ -211,17 +213,40 @@ krag_index::~krag_index() { delete redeal; }
 
 namespace {
 
+// A search slot for one call.  `st` is the stream the call enqueues its work with the slot's buffers on: the slot's own
+// stream (host-buffer searches, which synchronise it before they return) or the caller's (stage API, which returns with
+// the work queued).  The lease orders `st` after the slot's previous user and records the slot's `done` event on `st` when
+// it ends, so a slot passes to the next call only once the GPU has finished with it.  Buffers that grow (DevArray::reserve)
+// synchronise `st` before freeing the old allocation, which therefore also waits for the previous user.
 struct SlotLease {
     krag_ctx* c;
     Slot* s;
-    explicit SlotLease(krag_ctx* ctx) : c(ctx)
-    {
-        std::unique_lock<std::mutex> lk(c->mu);
-        c->cv.wait(lk, [&] { return !c->free_slots.empty(); });
-        s = c->free_slots.back();
-        c->free_slots.pop_back();
-    }
+    cudaStream_t st;
+    explicit SlotLease(krag_ctx* ctx) : SlotLease(ctx, nullptr, true) {}
+    SlotLease(krag_ctx* ctx, cudaStream_t caller) : SlotLease(ctx, caller, false) {}
     ~SlotLease()
+    {
+        cudaEventRecord(s->done, st);
+        give_back();
+    }
+
+private:
+    SlotLease(krag_ctx* ctx, cudaStream_t caller, bool own) : c(ctx)
+    {
+        {
+            std::unique_lock<std::mutex> lk(c->mu);
+            c->cv.wait(lk, [&] { return !c->free_slots.empty(); });
+            s = c->free_slots.back();
+            c->free_slots.pop_back();
+        }
+        st = own ? s->st : caller;
+        const cudaError_t e = cudaStreamWaitEvent(st, s->done, 0);
+        if (e != cudaSuccess) {
+            give_back();
+            KRAG_CUDA(e);
+        }
+    }
+    void give_back()
     {
         {
             std::lock_guard<std::mutex> lk(c->mu);
@@ -230,6 +255,15 @@ struct SlotLease {
         c->cv.notify_one();
     }
 };
+
+// Called by every mutation under the index's unique lock, before it changes anything: blocks until the search work already
+// issued has finished.  Stage calls return with their kernels queued on the caller's stream; each recorded its slot's
+// `done` event after them, and every later user of a slot is ordered after that event, so the last record of each slot's
+// event covers all the work ever issued with the slot.  Work on other indexes of the context is waited for as well.
+void wait_issued_searches(const krag_index* ix)
+{
+    for (const auto& s : ix->ctx->all_slots) KRAG_CUDA(cudaEventSynchronize(s->done));
+}
 
 const uint32_t* alive_ptr(const krag_index* ix) { return ix->has_dead ? ix->alive_d.p : nullptr; }
 OrdMap ord_map(const krag_index* ix) { return OrdMap{(uint32_t)ix->ord_base, (uint32_t)ix->ord_stride}; }
@@ -244,8 +278,10 @@ void require_idle(const krag_index* ix)
 
 void check_P(int P) { KRAG_REQUIRE(P >= 1 && P <= KRAG_MAX_POOL, KRAG_E_INVALID, "candidate pool must be in [1, 1024]"); }
 
-// the slot's staging for the streamed scan of a host-rows index, grown to this call's shape
-ScanStaging scan_staging(const krag_index* ix, Slot* s, int batch, int P)
+// the slot's staging for the streamed scan of a host-rows index, grown to this call's shape on st, the stream the lease
+// ordered after the slot's previous user.  copy_st needs no wait of its own: every copy into a staging buffer waits for a
+// `freed` event recorded on st (launch_dense_scan_streamed).
+ScanStaging scan_staging(const krag_index* ix, Slot* s, int batch, int P, cudaStream_t st)
 {
     if (!s->copy_st) {
         KRAG_CUDA(cudaStreamCreateWithFlags(&s->copy_st, cudaStreamNonBlocking));
@@ -254,10 +290,10 @@ ScanStaging scan_staging(const krag_index* ix, Slot* s, int batch, int P)
     }
     const int64_t R = stream_scan_chunk_rows(ix->dpad);
     const int64_t half = (R < ix->n_rows ? R : ix->n_rows) * ix->dpad;
-    s->stage.reserve(2 * half, 0, s->st);
-    s->fold.reserve(2 * (int64_t)(batch > 256 ? batch : 256) * P, 0, s->st);
-    s->q_sel.reserve((int64_t)256 * ix->dpad, 0, s->st);
-    s->k_sel.reserve((int64_t)256 * P, 0, s->st);
+    s->stage.reserve(2 * half, 0, st);
+    s->fold.reserve(2 * (int64_t)(batch > 256 ? batch : 256) * P, 0, st);
+    s->q_sel.reserve((int64_t)256 * ix->dpad, 0, st);
+    s->k_sel.reserve((int64_t)256 * P, 0, st);
     return ScanStaging{{s->stage.p, s->stage.p + half}, R, s->copy_st, {s->copied[0], s->copied[1]}, {s->freed[0], s->freed[1]},
                        s->fold.p, s->q_sel.p, s->k_sel.p};
 }
@@ -277,7 +313,7 @@ void dense_candidates_dev(krag_index* ix, Slot* s, const float* d_q, int batch, 
     int mode = c->cfg.dense_mode;
     if (ix->host_rows) {
         const HostRowsView hr{ix->Xp.h, ix->Xp.d, ix->Xh.p, ix->xres.p};
-        const ScanStaging sg = scan_staging(ix, s, batch, P);
+        const ScanStaging sg = scan_staging(ix, s, batch, P, st);
         if (mode != KRAG_DENSE_SCAN && dense_tc_host_rows_supported(c->di, ix->n_rows, ix->dpad)) {
             const size_t ws = dense_tc_workspace_bytes(c->di, ix->n_rows, P, true);
             s->tc_ws.reserve((int64_t)ws, 0, st);
@@ -744,6 +780,7 @@ int32_t krag_init(const krag_config* cfg, krag_ctx** out)
         for (int i = 0; i < ns; ++i) {
             c->all_slots.push_back(std::make_unique<Slot>());
             KRAG_CUDA(cudaStreamCreateWithFlags(&c->all_slots.back()->st, cudaStreamNonBlocking));
+            KRAG_CUDA(cudaEventCreateWithFlags(&c->all_slots.back()->done, cudaEventDisableTiming));
             c->free_slots.push_back(c->all_slots.back().get());
         }
         *out = c.release();
@@ -800,6 +837,7 @@ int32_t krag_index_reserve(krag_index* ix, int64_t rows, int64_t nnz)
         KRAG_REQUIRE(ix && rows >= 0, KRAG_E_INVALID, "bad argument");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
+        wait_issued_searches(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         ensure_capacity(ix, rows, nnz > 0 ? nnz : -1, ix->ctx->admin);
     });
@@ -817,6 +855,7 @@ int32_t krag_index_add(krag_index* ix, int64_t n, const uint64_t* node_ids, cons
         KRAG_REQUIRE(!sparse || (term_ids && term_tf && doc_len), KRAG_E_INVALID, "term_ids/term_tf/doc_len required with term_offsets");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
+        wait_issued_searches(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         cudaStream_t st = ix->ctx->admin;
         KRAG_REQUIRE(ix->n_rows == 0 || sparse == ix->has_sparse, KRAG_E_STATE,
@@ -894,6 +933,7 @@ int32_t krag_index_remove(krag_index* ix, int64_t n, const uint64_t* node_ids, i
         KRAG_REQUIRE(ix && (n == 0 || node_ids), KRAG_E_INVALID, "bad argument");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
+        wait_issued_searches(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         int64_t removed = 0;
         for (int64_t i = 0; i < n; ++i) {
@@ -918,6 +958,7 @@ int32_t krag_index_compact(krag_index* ix, int64_t* n_reclaimed_out)
         KRAG_REQUIRE(ix, KRAG_E_INVALID, "null index");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
+        wait_issued_searches(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         KRAG_REQUIRE(ix->ord_stride == 1, KRAG_E_UNSUPPORTED,
                      "compaction needs ordinal stride 1: rows of a round-robin shard cannot move down without leaving it");
@@ -977,6 +1018,7 @@ int32_t krag_redeal_begin(krag_index* ix, const uint32_t* alive_all, int64_t wor
                      KRAG_E_INVALID, "bad argument");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
+        wait_issued_searches(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         const int G = (int)ix->ord_stride, s = (int)ix->ord_base;
         KRAG_REQUIRE(s < G, KRAG_E_STATE, "not a round-robin shard: the ordinal base must be below the stride");
@@ -1171,6 +1213,7 @@ int32_t krag_index_commit_local(krag_index* ix, int64_t vocab, uint32_t* df_out,
         KRAG_REQUIRE(ix && df_out && n_live_out && total_len_out, KRAG_E_INVALID, "null argument");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
+        wait_issued_searches(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         commit_local_impl(ix, vocab, df_out, n_live_out, total_len_out);
     });
@@ -1183,6 +1226,7 @@ int32_t krag_index_commit_global(krag_index* ix, int64_t vocab, const uint32_t* 
         KRAG_REQUIRE(ix && df_global, KRAG_E_INVALID, "null argument");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
+        wait_issued_searches(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         commit_global_impl(ix, vocab, df_global, n_docs_global, total_len_global, ordinal_base);
     });
@@ -1195,6 +1239,7 @@ int32_t krag_index_commit(krag_index* ix, int64_t vocab)
         KRAG_REQUIRE(vocab >= 1 && vocab <= (int64_t)1 << 31, KRAG_E_INVALID, "vocab must be in [1, 2^31]");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
+        wait_issued_searches(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         std::vector<uint32_t> df((size_t)vocab);
         int64_t live = 0, total = 0;
@@ -1209,6 +1254,7 @@ int32_t krag_index_set_ordinal_map(krag_index* ix, int64_t ordinal_base, int64_t
         KRAG_REQUIRE(ix && ordinal_base >= 0 && ordinal_stride >= 1 && ordinal_stride <= 64, KRAG_E_INVALID, "bad argument");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
+        wait_issued_searches(ix);
         KRAG_REQUIRE(ordinal_base + ix->n_rows * ordinal_stride <= 0xFFFFFFFFll, KRAG_E_UNSUPPORTED, "global ordinal exceeds 32 bits");
         ix->ord_base = ordinal_base; ix->ord_stride = ordinal_stride;
     });
@@ -1373,8 +1419,8 @@ int32_t krag_dev_dense_candidates(krag_index* ix, int32_t batch, const float* d_
         std::shared_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
-        SlotLease lease(ix->ctx);
-        dense_candidates_dev(ix, lease.s, d_q, batch, P, d_keys, (cudaStream_t)stream);
+        SlotLease lease(ix->ctx, (cudaStream_t)stream);
+        dense_candidates_dev(ix, lease.s, d_q, batch, P, d_keys, lease.st);
     });
 }
 
@@ -1387,8 +1433,8 @@ int32_t krag_dev_bm25_candidates(krag_index* ix, int32_t batch, const uint32_t* 
         std::shared_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
-        SlotLease lease(ix->ctx);
-        bm25_candidates_dev(ix, lease.s, d_terms, d_toff, h_toff ? h_toff[batch] : -1, batch, P, d_keys, (cudaStream_t)stream);
+        SlotLease lease(ix->ctx, (cudaStream_t)stream);
+        bm25_candidates_dev(ix, lease.s, d_terms, d_toff, h_toff ? h_toff[batch] : -1, batch, P, d_keys, lease.st);
     });
 }
 
@@ -1427,6 +1473,7 @@ int32_t krag_synth_fill(krag_index* ix, int64_t n, int64_t row_base, uint64_t se
         KRAG_REQUIRE(ix && n >= 0, KRAG_E_INVALID, "bad argument");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
+        wait_issued_searches(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         cudaStream_t st = ix->ctx->admin;
         KRAG_REQUIRE(ix->n_rows == 0, KRAG_E_STATE, "synthetic fill needs an empty index");
@@ -1497,6 +1544,7 @@ int32_t krag_index_set_dense_mode(krag_index* ix, int32_t dense_mode, int32_t re
         KRAG_REQUIRE(ix && dense_mode >= KRAG_DENSE_AUTO && dense_mode <= KRAG_DENSE_TC_TF32, KRAG_E_INVALID, "bad argument");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
+        wait_issued_searches(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         cudaStream_t st = ix->ctx->admin;
         if (dense_mode == KRAG_DENSE_TC_BF16 && ix->Xh.p == nullptr && ix->X.p != nullptr) {
@@ -1776,6 +1824,7 @@ int32_t krag_index_persist(krag_index* ix, const char* dir)
         KRAG_REQUIRE(ix && dir, KRAG_E_INVALID, "null argument");
         std::shared_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
+        wait_issued_searches(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         mkdir(dir, 0755);
         std::string path = std::string(dir) + "/krag_index.bin";
