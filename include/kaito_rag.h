@@ -52,8 +52,8 @@ extern "C" {
 
 #define KRAG_DENSE_AUTO 0   /* exact fp32 scan for small batches, tensor-core path for large */
 #define KRAG_DENSE_SCAN 1   /* K1: exact fp32 CUDA-core scan */
-#define KRAG_DENSE_TC 2     /* K2: wgmma prune pass (fp32 rows rounded to bf16 on chip, bf16 wgmma; TF32 when the
-                               padded dimension is not a multiple of 64) + exact fp32 rescoring */
+#define KRAG_DENSE_TC 2     /* K2: wgmma prune pass (bf16 wgmma on the bf16 high halves the device rows are stored with;
+                               TF32 when the padded dimension is not a multiple of 64) + exact fp32 rescoring */
 #define KRAG_DENSE_TC_BF16 3 /* K2 pruning on a bf16 SHADOW copy of the corpus (+50% memory); the returned distances are
                                still exact fp32 re-scores of the fp32 corpus and carry the same exactness certificate */
 
@@ -415,7 +415,7 @@ int64_t krag_tc_fallback_queries(void);
 /* rows rescored from host memory by KRAG_ROWS_HOST searches (process-wide counter) */
 int64_t krag_host_rows_fetched(void);
 /* CUDA-event duration of the dominant dense kernel of the last search on this process
- * (kernel_id 1 = K1 exact scan; K2 main pass: 3 = TF32, 4 = bf16 shadow, 5 = fp32 rows rounded to bf16 on chip,
+ * (kernel_id 1 = K1 exact scan; K2 main pass: 3 = TF32, 4 = bf16 shadow, 5 = bf16 high halves of the device rows,
  * 6 = device bf16 rows of a KRAG_ROWS_HOST index), with the algorithmic bytes and
  * flops of that launch -- bench.py's roofline line is computed from it. */
 int32_t krag_last_dense_kernel(float* ms, int32_t* kernel_id, int64_t* algorithmic_bytes, int64_t* flops);
@@ -432,6 +432,9 @@ int32_t krag_last_commit(float* total_ms, float* host_ms, int32_t* merged, int64
 /* raw K2 output a[j][r] = |x_r|^2 - 2 x_r.q_j (TF32) for every row, [nq_pad][S] row-major;
  * call with out == NULL to query S and nq_pad.  Test hook for the tensor-core kernel; KRAG_E_UNSUPPORTED for
  * KRAG_ROWS_HOST indexes. */
+/* test hook: rows [row0, row0 + n) of a device-resident index as stored, dim_padded 32-bit words per row (split rows where
+ * dim_padded % 64 == 0, DESIGN.md section 4 K2) */
+int32_t krag_debug_read_stored_rows(krag_index* idx, int64_t row0, int64_t n, float* out);
 int32_t krag_debug_tc_dump(krag_index* idx, int32_t nq, const float* q, float* out, int64_t out_elems,
                            int64_t* S_out, int32_t* nq_pad_out);
 

@@ -33,7 +33,7 @@ SYMBOLS = [
     "krag_index_node_ids", "krag_index_set_ordinal_map", "krag_index_persist", "krag_index_load", "krag_search_dense", "krag_search_bm25",
     "krag_retrieve", "krag_dev_dense_candidates", "krag_dev_bm25_candidates", "krag_dev_merge", "krag_dev_fuse",
     "krag_synth_fill", "krag_index_read_rows", "krag_index_read_postings", "krag_tc_fallback_queries",
-    "krag_debug_tc_dump", "krag_last_dense_kernel", "krag_embedder_create", "krag_embedder_load_tensor",
+    "krag_debug_tc_dump", "krag_debug_read_stored_rows", "krag_last_dense_kernel", "krag_embedder_create", "krag_embedder_load_tensor",
     "krag_embedder_finalize", "krag_embed", "krag_embed_dev", "krag_embedder_destroy", "krag_debug_gemm_tf32",
     "krag_debug_linear_ln", "krag_index_set_dense_mode", "krag_text_analyze", "krag_wordpiece_create",
     "krag_wordpiece_encode_batch", "krag_wordpiece_destroy", "krag_p2p_create", "krag_p2p_connect", "krag_dev_exchange_merge", "krag_p2p_destroy",
@@ -160,6 +160,7 @@ def load() -> C.CDLL:
     L.krag_last_compact.argtypes = [C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(i64), C.POINTER(i64)]
     L.krag_last_commit.argtypes = [C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]
     L.krag_debug_tc_dump.argtypes = [vp, i32, vp, vp, i64, C.POINTER(i64), C.POINTER(i32)]
+    L.krag_debug_read_stored_rows.argtypes = [vp, i64, i64, vp]
     for name in SYMBOLS:
         fn = getattr(L, name)
         if fn.restype is C.c_int:  # default: every remaining call returns an int32 status
@@ -607,6 +608,12 @@ class Index:
         check(self._L.krag_debug_tc_dump(self._h, q.shape[0], ptr(q), None, 0, C.byref(S), C.byref(nqp)))
         out = np.empty((nqp.value, S.value), np.float32)
         check(self._L.krag_debug_tc_dump(self._h, q.shape[0], ptr(q), ptr(out), out.size, C.byref(S), C.byref(nqp)))
+        return out
+
+    def debug_stored_rows(self, row0: int, n: int) -> np.ndarray:
+        """rows [row0, row0 + n) as the device stores them: uint32 [n, dim_padded] (test hook)"""
+        out = np.empty((n, self.stats().dim_padded), np.uint32)
+        check(self._L.krag_debug_read_stored_rows(self._h, row0, n, ptr(out)))
         return out
 
     def read_postings(self, term: int, cap: int = 1 << 22):

@@ -21,6 +21,7 @@
 #include "common.cuh"
 #include "embed_config.h"
 #include "engine.h"
+#include "split_rows.cuh"
 
 namespace krag {
 
@@ -160,7 +161,8 @@ struct krag_index {
     std::shared_mutex mu;
     // dense shard
     bool host_rows = false;         // KRAG_ROWS_HOST: the fp32 rows are Xp (pinned host memory) and X stays empty
-    DevArray<float> X;
+    DevArray<float> X;              // device-resident rows [rows, dpad], zero padded; split rows (split_rows.cuh) when split_rows
+    bool split_rows = false;
     HostArray<float> Xp;            // host-resident fp32 rows [rows, dpad], zero padded
     DevArray<float> xnorm;          // |x|^2 per row (K2 epilogue), from the fp32 rows in either storage
     DevArray<uint16_t> Xh;          // bf16 copy of the rows: optional shadow (KRAG_DENSE_TC_BF16), always present for host rows
@@ -331,12 +333,12 @@ void dense_candidates_dev(krag_index* ix, Slot* s, const float* d_q, int batch, 
         s->tc_ws.reserve((int64_t)ws, 0, st);
         if (launch_dense_tc(c->di, ix->X.p, ix->n_rows, ix->dpad, alive, ix->xnorm.p, ix->xn_max.p, d_q, batch, P,
                             ord_map(ix), s->tc_ws.p, ws, s->part.p, d_keys, st,
-                            mode == KRAG_DENSE_TC_BF16 ? ix->Xh.p : nullptr, mode != KRAG_DENSE_TC_TF32))
+                            mode == KRAG_DENSE_TC_BF16 ? ix->Xh.p : nullptr, mode != KRAG_DENSE_TC_TF32, ix->split_rows))
             return;
     }
     KRAG_REQUIRE((mode != KRAG_DENSE_TC && mode != KRAG_DENSE_TC_TF32) || !dense_tc_wants(ix->n_rows, 16), KRAG_E_UNSUPPORTED, "tensor-core dense path unavailable for this index/device");
     launch_dense_scan(c->di, ix->X.p, ix->n_rows, ix->dpad, alive, d_q, batch, P, ord_map(ix),
-                      s->part.p, d_keys, st);
+                      s->part.p, d_keys, st, ix->split_rows);
 }
 
 void bm25_candidates_dev(krag_index* ix, Slot* s, const uint32_t* d_terms, const int32_t* d_toff, int n_terms_total, int batch,
@@ -814,6 +816,7 @@ int32_t krag_index_create(krag_ctx* c, const char* name, int32_t dim, krag_index
         ix->dpad = (dim + KRAG_LANES - 1) / KRAG_LANES * KRAG_LANES;
         ix->ord_base = 0;
         ix->host_rows = c->cfg.row_storage == KRAG_ROWS_HOST;
+        ix->split_rows = split_rows_layout(ix->dpad, ix->host_rows);
         *out = ix;
     });
 }
@@ -890,9 +893,10 @@ int32_t krag_index_add(krag_index* ix, int64_t n, const uint64_t* node_ids, cons
             KRAG_CUDA(cudaMemcpy2DAsync(dst, sizeof(float) * ix->dpad, vecs, sizeof(float) * ix->dim, sizeof(float) * ix->dim,
                                         (size_t)n, cudaMemcpyHostToDevice, st));
         }
-        if (!ix->host_rows) {
+        if (!ix->host_rows) {   // norms and shadow from the plain rows, then the rows take their stored layout
             launch_row_norms(ix->X.p, ix->n_rows, n, ix->dpad, ix->xnorm.p, ix->xn_max.p, st);
             if (ix->Xh.p) launch_f32_to_bf16(dst, ix->Xh.p + ix->n_rows * ix->dpad, n * ix->dpad, st);
+            if (ix->split_rows) launch_split_encode(dst, n, ix->dpad, st);
         }
         std::vector<int64_t> shifted;
         if (sparse) {
@@ -1484,6 +1488,7 @@ int32_t krag_synth_fill(krag_index* ix, int64_t n, int64_t row_base, uint64_t se
             launch_synth_dense(ix->X.p, n, ix->dim, ix->dpad, row_base, seed, st);
             launch_row_norms(ix->X.p, 0, n, ix->dpad, ix->xnorm.p, ix->xn_max.p, st);
             if (ix->Xh.p) launch_f32_to_bf16(ix->X.p, ix->Xh.p, n * ix->dpad, st);
+            if (ix->split_rows) launch_split_encode(ix->X.p, n, ix->dpad, st);
         }
         if (vocab > 0) {
             DevArray<int64_t> off; DevArray<uint32_t> ids; DevArray<uint16_t> tf; DevArray<uint32_t> dl; int64_t nnz = 0;
@@ -1514,8 +1519,27 @@ int32_t krag_index_read_rows(krag_index* ix, int64_t row0, int64_t n, float* out
             for (int64_t i = 0; i < n; ++i) memcpy(out + i * ix->dim, ix->Xp.h + (row0 + i) * ix->dpad, sizeof(float) * ix->dim);
             return;
         }
+        if (ix->split_rows) {
+            std::vector<float> raw((size_t)n * ix->dpad);
+            KRAG_CUDA(cudaMemcpy(raw.data(), ix->X.p + row0 * ix->dpad, sizeof(float) * raw.size(), cudaMemcpyDeviceToHost));
+            for (int64_t i = 0; i < n; ++i) split_row_decode_host(raw.data() + i * ix->dpad, ix->dim, out + i * ix->dim);
+            return;
+        }
         KRAG_CUDA(cudaMemcpy2D(out, sizeof(float) * ix->dim, ix->X.p + row0 * ix->dpad, sizeof(float) * ix->dpad,
                                sizeof(float) * ix->dim, (size_t)n, cudaMemcpyDeviceToHost));
+    });
+}
+
+int32_t krag_debug_read_stored_rows(krag_index* ix, int64_t row0, int64_t n, float* out)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(ix && out && row0 >= 0 && n >= 0 && row0 + n <= ix->n_rows, KRAG_E_INVALID, "row range out of bounds");
+        std::shared_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
+        KRAG_REQUIRE(!ix->host_rows, KRAG_E_UNSUPPORTED, "the stored layout is that of device-resident rows");
+        KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
+        if (n > 0)
+            KRAG_CUDA(cudaMemcpy(out, ix->X.p + row0 * ix->dpad, sizeof(float) * (size_t)(n * ix->dpad), cudaMemcpyDeviceToHost));
     });
 }
 
@@ -1549,7 +1573,8 @@ int32_t krag_index_set_dense_mode(krag_index* ix, int32_t dense_mode, int32_t re
         cudaStream_t st = ix->ctx->admin;
         if (dense_mode == KRAG_DENSE_TC_BF16 && ix->Xh.p == nullptr && ix->X.p != nullptr) {
             ix->Xh.reserve(ix->X.cap, 0, st);                     // same capacity as the fp32 rows: later appends convert in place
-            launch_f32_to_bf16(ix->X.p, ix->Xh.p, ix->n_rows * ix->dpad, st);
+            if (ix->split_rows) launch_split_to_bf16(ix->X.p, ix->n_rows, ix->dpad, ix->Xh.p, st);
+            else launch_f32_to_bf16(ix->X.p, ix->Xh.p, ix->n_rows * ix->dpad, st);
         }
         if (dense_mode != KRAG_DENSE_TC_BF16 && release_shadow && !ix->host_rows) ix->Xh.release();   // host rows: Xh is the device copy
         KRAG_CUDA(cudaStreamSynchronize(st));
@@ -1581,14 +1606,14 @@ int32_t krag_debug_tc_dump(krag_index* ix, int32_t nq, const float* q, float* ou
         SlotLease lease(ix->ctx);
         Slot* s = lease.s;
         int64_t S = 0; int nqp = 0;
-        KRAG_REQUIRE(dense_tc_debug_dump(ix->ctx->di, ix->X.p, ix->n_rows, ix->dpad, ix->xnorm.p, nullptr, nq, nullptr, &S, &nqp, s->st),
+        KRAG_REQUIRE(dense_tc_debug_dump(ix->ctx->di, ix->X.p, ix->split_rows, ix->n_rows, ix->dpad, ix->xnorm.p, nullptr, nq, nullptr, &S, &nqp, s->st),
                      KRAG_E_UNSUPPORTED, "tensor-core path unavailable");
         *S_out = S; *nq_pad_out = nqp;
         if (!out) return;
         KRAG_REQUIRE(out_elems >= S * nqp, KRAG_E_INVALID, "output buffer too small");
         const float* dq = upload_queries(ix, s, q, nq);
         s->tc_ws.reserve(S * nqp * 4, 0, s->st);
-        KRAG_REQUIRE(dense_tc_debug_dump(ix->ctx->di, ix->X.p, ix->n_rows, ix->dpad, ix->xnorm.p, dq, nq, (float*)s->tc_ws.p, &S, &nqp, s->st),
+        KRAG_REQUIRE(dense_tc_debug_dump(ix->ctx->di, ix->X.p, ix->split_rows, ix->n_rows, ix->dpad, ix->xnorm.p, dq, nq, (float*)s->tc_ws.p, &S, &nqp, s->st),
                      KRAG_E_UNSUPPORTED, "tensor-core dump failed");
         KRAG_CUDA(cudaMemcpyAsync(out, s->tc_ws.p, sizeof(float) * (size_t)(S * nqp), cudaMemcpyDeviceToHost, s->st));
         KRAG_CUDA(cudaStreamSynchronize(s->st));
@@ -1836,12 +1861,15 @@ int32_t krag_index_persist(krag_index* ix, const char* dir)
         W(ix->node_ids.data(), sizeof(uint64_t) * (size_t)ix->n_rows);
         W(ix->alive_h.data(), sizeof(uint32_t) * (size_t)((ix->n_rows + 31) / 32));
         const int64_t chunk = 1 << 16;
-        std::vector<float> rows((size_t)chunk * ix->dim);
+        std::vector<float> rows((size_t)chunk * ix->dim), raw(ix->split_rows ? (size_t)chunk * ix->dpad : 0);
         for (int64_t r = 0; r < ix->n_rows; r += chunk) {
             int64_t m = ix->n_rows - r < chunk ? ix->n_rows - r : chunk;
             if (ix->host_rows) {
                 for (int64_t i = 0; i < m; ++i)
                     memcpy(rows.data() + i * ix->dim, ix->Xp.h + (r + i) * ix->dpad, sizeof(float) * ix->dim);
+            } else if (ix->split_rows) {
+                KRAG_CUDA(cudaMemcpy(raw.data(), ix->X.p + r * ix->dpad, sizeof(float) * (size_t)(m * ix->dpad), cudaMemcpyDeviceToHost));
+                for (int64_t i = 0; i < m; ++i) split_row_decode_host(raw.data() + i * ix->dpad, ix->dim, rows.data() + i * ix->dim);
             } else {
                 KRAG_CUDA(cudaMemcpy2D(rows.data(), sizeof(float) * ix->dim, ix->X.p + r * ix->dpad, sizeof(float) * ix->dpad,
                                        sizeof(float) * ix->dim, (size_t)m, cudaMemcpyDeviceToHost));

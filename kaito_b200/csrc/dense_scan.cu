@@ -11,9 +11,13 @@
 //
 // Layout: X row-major [n_rows, dpad], dpad % 32 == 0, zero padded.  A warp reads 8 rows
 // per iteration as 2 x (4 rows x 128 contiguous bytes) per load instruction -- fully
-// coalesced 128-byte segments, streamed with L1 no-allocate.
+// coalesced 128-byte segments, streamed with L1 no-allocate.  On split rows (split_rows.cuh)
+// a lane reads the 16-byte high-half and low-half words of its 8 elements of a 64-element
+// block (its steps 2 b and 2 b + 1: again 4 rows x 128 contiguous bytes per load) and
+// rebuilds the same fp32 values.
 #include "engine.h"
 #include "select.cuh"
+#include "split_rows.cuh"
 
 namespace krag {
 
@@ -22,7 +26,7 @@ constexpr int DS_WARPS = DS_THREADS / 32;
 constexpr int DS_ROWS_PER_WARP = 8;
 constexpr int DS_TILE_ROWS = DS_WARPS * DS_ROWS_PER_WARP;  // 64 rows per CTA iteration
 
-template <int NQ>
+template <int NQ, bool SPLIT>
 __global__ void __launch_bounds__(DS_THREADS, 2)
 dense_scan_kernel(const float* __restrict__ X, int64_t n_rows, int dpad, const uint32_t* __restrict__ alive,
                   const float* __restrict__ Q, int P, int cap, int epoch_iters, OrdMap ord_base,
@@ -57,17 +61,15 @@ dense_scan_kernel(const float* __restrict__ X, int64_t n_rows, int dpad, const u
         const int64_t rowB = rowA + 4;
         const int64_t ra = rowA < n_rows ? rowA : n_rows - 1;  // clamp the address, discard the value
         const int64_t rb = rowB < n_rows ? rowB : n_rows - 1;
-        const float4* pa = reinterpret_cast<const float4*>(X + ra * dpad) + l8;
-        const float4* pb = reinterpret_cast<const float4*>(X + rb * dpad) + l8;
+        const float* xa = X + ra * dpad;
+        const float* xb = X + rb * dpad;
+        const float4* pa = reinterpret_cast<const float4*>(xa) + l8;
+        const float4* pb = reinterpret_cast<const float4*>(xb) + l8;
 
         float4 accA[NQ], accB[NQ];
 #pragma unroll
         for (int q = 0; q < NQ; ++q) { accA[q] = make_float4(0.f, 0.f, 0.f, 0.f); accB[q] = accA[q]; }
-
-#pragma unroll 4
-        for (int i = 0; i < steps; ++i) {
-            const float4 a = ldg_stream_f4(pa + i * 8);
-            const float4 b = ldg_stream_f4(pb + i * 8);
+        auto step = [&](int i, const float4& a, const float4& b) {
 #pragma unroll
             for (int q = 0; q < NQ; ++q) {
                 const float4 qv = *reinterpret_cast<const float4*>(sq + q * dpad + i * KRAG_LANES + l8 * 4);
@@ -81,6 +83,20 @@ dense_scan_kernel(const float* __restrict__ X, int64_t n_rows, int dpad, const u
                 t = b.z - qv.z; accB[q].z = fmaf(t, t, accB[q].z);
                 t = b.w - qv.w; accB[q].w = fmaf(t, t, accB[q].w);
             }
+        };
+
+        if (SPLIT) {   // steps 2 b and 2 b + 1 from block b, in the same order
+#pragma unroll 2
+            for (int blk = 0; blk < steps / 2; ++blk) {
+                float4 a0, a1, b0, b1;
+                split_ld8<true>(xa, blk, l8, a0, a1);
+                split_ld8<true>(xb, blk, l8, b0, b1);
+                step(2 * blk, a0, b0);
+                step(2 * blk + 1, a1, b1);
+            }
+        } else {
+#pragma unroll 4
+            for (int i = 0; i < steps; ++i) step(i, ldg_stream_f4(pa + i * 8), ldg_stream_f4(pb + i * 8));
         }
         const bool okA = rowA < n_rows && (alive == nullptr || bit_test(alive, (uint32_t)rowA));
         const bool okB = rowB < n_rows && (alive == nullptr || bit_test(alive, (uint32_t)rowB));
@@ -130,7 +146,7 @@ static int ds_grid(const DeviceInfo& di, int64_t n_rows)
 
 size_t dense_scan_part_elems(const DeviceInfo& di, int P) { return (size_t)4 * 2 * di.sm_count * P + 4; }
 
-template <int NQ>
+template <int NQ, bool SPLIT>
 static void ds_launch(const DeviceInfo& di, const float* X, int64_t n_rows, int dpad, const uint32_t* alive,
                       const float* q, int P, OrdMap ord_base, uint64_t* part, unsigned long long* g_thr, cudaStream_t st)
 {
@@ -139,13 +155,13 @@ static void ds_launch(const DeviceInfo& di, const float* X, int64_t n_rows, int 
     const size_t smem = (size_t)NQ * dpad * 4 + (size_t)NQ * cap * 8;
     static bool attr_set = false;
     if (!attr_set) {
-        KRAG_CUDA(cudaFuncSetAttribute(dense_scan_kernel<NQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+        KRAG_CUDA(cudaFuncSetAttribute(dense_scan_kernel<NQ, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
         attr_set = true;
     }
     const int grid = ds_grid(di, n_rows);
     KRAG_CUDA(cudaMemsetAsync(g_thr, 0xFF, sizeof(unsigned long long) * NQ, st));
     dense_timer_begin(st, 1, n_rows * (int64_t)dpad * 4, 3 * (int64_t)NQ * n_rows * dpad);
-    dense_scan_kernel<NQ><<<grid, DS_THREADS, smem, st>>>(X, n_rows, dpad, alive, q, P, cap, epoch, ord_base, part, g_thr);
+    dense_scan_kernel<NQ, SPLIT><<<grid, DS_THREADS, smem, st>>>(X, n_rows, dpad, alive, q, P, cap, epoch, ord_base, part, g_thr);
     dense_timer_end(st);
     KRAG_CUDA(cudaGetLastError());
     count_launch();
@@ -153,7 +169,7 @@ static void ds_launch(const DeviceInfo& di, const float* X, int64_t n_rows, int 
 
 void launch_dense_scan(const DeviceInfo& di, const float* X, int64_t n_rows, int dpad, const uint32_t* alive,
                        const float* q, int batch, int P, OrdMap ord_base, uint64_t* part, uint64_t* keys_out,
-                       cudaStream_t st)
+                       cudaStream_t st, bool split)
 {
     const int grid = ds_grid(di, n_rows);
     unsigned long long* g_thr = reinterpret_cast<unsigned long long*>(part + (size_t)4 * 2 * di.sm_count * P);
@@ -163,9 +179,15 @@ void launch_dense_scan(const DeviceInfo& di, const float* X, int64_t n_rows, int
         // smem budget: NQ * (dpad*4 + cap*8) must stay under 100 KB (2 CTAs per SM)
         while (nq > 1 && (size_t)nq * ((size_t)dpad * 4 + (size_t)ds_cap(P) * 8) > 96 * 1024) nq >>= 1;
         const float* qb = q + (size_t)b * dpad;
-        if (nq == 4) ds_launch<4>(di, X, n_rows, dpad, alive, qb, P, ord_base, part, g_thr, st);
-        else if (nq == 2) ds_launch<2>(di, X, n_rows, dpad, alive, qb, P, ord_base, part, g_thr, st);
-        else ds_launch<1>(di, X, n_rows, dpad, alive, qb, P, ord_base, part, g_thr, st);
+        if (split) {
+            if (nq == 4) ds_launch<4, true>(di, X, n_rows, dpad, alive, qb, P, ord_base, part, g_thr, st);
+            else if (nq == 2) ds_launch<2, true>(di, X, n_rows, dpad, alive, qb, P, ord_base, part, g_thr, st);
+            else ds_launch<1, true>(di, X, n_rows, dpad, alive, qb, P, ord_base, part, g_thr, st);
+        } else {
+            if (nq == 4) ds_launch<4, false>(di, X, n_rows, dpad, alive, qb, P, ord_base, part, g_thr, st);
+            else if (nq == 2) ds_launch<2, false>(di, X, n_rows, dpad, alive, qb, P, ord_base, part, g_thr, st);
+            else ds_launch<1, false>(di, X, n_rows, dpad, alive, qb, P, ord_base, part, g_thr, st);
+        }
         // part is [nq][grid][P]: lists = CTAs
         launch_merge(part, grid, P, nq, P, /*list_stride=*/P, /*batch_stride=*/(int64_t)grid * P,
                      keys_out + (size_t)b * P, st, reinterpret_cast<const uint64_t*>(g_thr));
@@ -201,7 +223,7 @@ void launch_dense_scan_streamed(const DeviceInfo& di, const float* X_host, int64
         KRAG_CUDA(cudaEventRecord(sg.copied[b], sg.copy));
         KRAG_CUDA(cudaStreamWaitEvent(st, sg.copied[b], 0));
         const OrdMap om{ord_base + (uint32_t)r0, ord_base.stride};
-        launch_dense_scan(di, sg.buf[b], m, dpad, alive ? alive + r0 / 32 : nullptr, q, batch, P, om, part, i == 0 ? run : chk, st);
+        launch_dense_scan(di, sg.buf[b], m, dpad, alive ? alive + r0 / 32 : nullptr, q, batch, P, om, part, i == 0 ? run : chk, st, false);
         KRAG_CUDA(cudaEventRecord(sg.freed[b], st));
         if (i > 0) {
             launch_merge(run, 2, P, batch, P, list, P, keys_out, st);

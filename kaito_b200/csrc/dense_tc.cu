@@ -5,10 +5,12 @@
 //
 //   1. dense_tc_kernel<NQ, MODE, DUMP>  (wgmma, TMA-staged, accumulators in registers)
 //        D[128 corpus rows x NQ queries] = X_tile . Q^T.  The prune pass has three operand modes:
-//          TC_CVT  (default) fp32 corpus rows staged by TMA, rounded to bf16 while they are loaded into the
-//                  A-operand registers, bf16 queries from shared memory: 4 bytes/element from HBM, bf16 tensor rate
-//          TC_TF32 fp32 corpus and queries consumed as TF32 straight from shared memory
-//          TC_BF16 (opt-in) a bf16 shadow of the corpus: half the HBM bytes
+//          TC_BF16  bf16 corpus and queries from shared memory: 2 bytes/element from HBM.  The corpus operand is the high
+//                   halves of split rows (split_rows.cuh: the default on rows with dpad % 64 == 0), the opt-in bf16 shadow
+//                   (KRAG_DENSE_TC_BF16) or the device copy of host-resident rows
+//          TC_TF32  plain fp32 corpus rows and queries consumed as TF32 straight from shared memory
+//          TC_TF32S TC_TF32 on split rows: both halves staged by TMA, rebuilt to fp32 in the A registers (tf32 wgmma with A
+//                   from registers); the same products as TC_TF32 on the plain rows, bit for bit
 //        epilogue: a = |x|^2 - 2 x.q  per (row, query), compared with a per-query threshold;
 //        rows below it are appended to that query's candidate list (rare: ~C of N rows).
 //        DUMP mode writes `a` (TF32) for a strided 1/64 sample of the tiles instead.
@@ -23,7 +25,7 @@
 //
 // So the tensor cores only PRUNE; every returned score is an exact fp32 distance.
 //
-// Roofline: bytes = n_rows*dpad*4 per pass (HBM; 2 with the bf16 shadow), flops = 2*NQ*n_rows*dpad.
+// Roofline: bytes = n_rows*dpad*2 per bf16 pass, n_rows*dpad*4 per tf32 pass (HBM), flops = 2*NQ*n_rows*dpad.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <math_constants.h>
@@ -34,6 +36,7 @@
 
 #include "engine.h"
 #include "select.cuh"
+#include "split_rows.cuh"
 #include "tc_ptx.cuh"
 
 namespace krag {
@@ -43,16 +46,17 @@ constexpr int TC_TILE_M = 128;          // corpus rows per tile: two consumer wa
 constexpr int TC_KBLOCK = 32;           // fp32 elements per k-block = one 128-byte swizzle row
 constexpr int TC_THREADS = 384;         // warpgroup 0: TMA producer, warpgroups 1-2: wgmma + epilogue
 constexpr int TC_SAMPLE_STRIDE = 64;    // DUMP mode visits every 64th tile
-constexpr int TC_A_BYTES = TC_TILE_M * 128;  // 16 KB: 128 rows x one 128-byte swizzle row
+constexpr int TC_A_BYTES = TC_TILE_M * 128;  // 16 KB: 128 rows x one 128-byte swizzle row (32 fp32 or 64 halves)
 constexpr int TC_DUMP_GROUP = 16;       // rows per minimum in the threshold-sampling dump (one warp's wgmma rows)
 
-enum { TC_TF32 = 0, TC_BF16 = 1, TC_CVT = 2 };
+enum { TC_TF32 = 0, TC_BF16 = 1, TC_TF32S = 2 };
 
-// One ring; a stage holds the corpus rows of the tile and all NQ query rows for 32 (TF32) or 64 (bf16) elements of
-// the dimension: 4 wgmma K steps either way.  In TC_CVT mode the corpus part is two fp32 k-blocks.
+// One ring; a stage holds the corpus rows of the tile and all NQ query rows for 32 (TF32) or 64 (bf16, TF32S) elements of
+// the dimension: 4 wgmma K steps (8 in TF32S mode, whose stage holds one 64-element block of split rows: its high-half and
+// low-half boxes, and two fp32 query boxes).
 template <int NQ, int MODE> struct TcCfg {
-    static constexpr int A_BYTES = (MODE == TC_CVT ? 2 : 1) * TC_A_BYTES;
-    static constexpr int Q_BYTES = NQ * 128;
+    static constexpr int A_BYTES = (MODE == TC_TF32S ? 2 : 1) * TC_A_BYTES;
+    static constexpr int Q_BYTES = (MODE == TC_TF32S ? 2 : 1) * NQ * 128;
     static constexpr int STAGE_BYTES = A_BYTES + Q_BYTES;
     static constexpr int STAGES = (200 * 1024) / STAGE_BYTES > 8 ? 8 : (200 * 1024) / STAGE_BYTES;
     static constexpr int ELEMS = MODE == TC_TF32 ? TC_KBLOCK : 2 * TC_KBLOCK;   // dimension elements per stage
@@ -60,27 +64,26 @@ template <int NQ, int MODE> struct TcCfg {
     static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + 1024 /*align*/ + BAR_BYTES + NQ * 4;
 };
 
-// bf16 A fragment (mma.sync / wgmma register layout) of K step s from a TMA-swizzled fp32 staging stage: this thread's
-// rows r and r + 8 (r & 7 == g), elements 16 s + 2 q (+1) and 16 s + 8 + 2 q (+1), rounded to nearest even
-__device__ __forceinline__ void cvt_a_fragment(const unsigned char* stage_a, int r, int g, int q, int s, uint32_t* a)
+// tf32 A fragment (mma.sync m16n8k8 / wgmma register layout) of K step s (0..7) from a TF32S stage: the high-half box at
+// `hi`, the low-half box TC_A_BYTES later, each 128 rows x 64 halves (a block's half in split_pos order), 128B-swizzled.
+// This thread's rows r and r + 8 (r & 7 == g), elements e = 8 s + q and e + 4, gathered in element order and rebuilt to
+// their fp32 bits:  a0 (r, e), a1 (r + 8, e), a2 (r, e + 4), a3 (r + 8, e + 4).
+__device__ __forceinline__ void tf32s_a_fragment(const unsigned char* hi, int r, int g, int q, int s, uint32_t* a)
 {
-    const unsigned char* box = stage_a + (s >> 1) * TC_A_BYTES;
+    const unsigned char* lo = hi + TC_A_BYTES;
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {              // h = 0: elements e, e + 1; h = 1: e + 8, e + 9
-        const int e = 16 * (s & 1) + 8 * h + 2 * q;
-        const int off = (((e >> 2) ^ g) << 4) + ((e & 3) << 2);
-        const float2 v0 = *reinterpret_cast<const float2*>(box + r * 128 + off);
-        const float2 v1 = *reinterpret_cast<const float2*>(box + (r + 8) * 128 + off);
-        const __nv_bfloat162 b0 = __floats2bfloat162_rn(v0.x, v0.y), b1 = __floats2bfloat162_rn(v1.x, v1.y);
-        a[2 * h + 0] = *reinterpret_cast<const uint32_t*>(&b0);
-        a[2 * h + 1] = *reinterpret_cast<const uint32_t*>(&b1);
+    for (int k = 0; k < 4; ++k) {
+        const int p = split_pos(8 * s + q + 4 * (k >> 1));
+        const int o = (r + 8 * (k & 1)) * 128 + (((p >> 3) ^ g) << 4) + 2 * (p & 7);
+        a[k] = split_join(*reinterpret_cast<const uint16_t*>(hi + o), *reinterpret_cast<const uint16_t*>(lo + o));
     }
 }
 
 template <int NQ, int MODE, bool DUMP>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 dense_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmQ, int64_t n_rows,
-                int kblocks /*stages per tile*/, int64_t n_ltiles, int tile_stride, const float* __restrict__ xnorm,
+                int kblocks /*stages per tile*/, int piece_step /*TC_BF16: 128-byte pieces per k-block*/, int64_t n_ltiles,
+                int tile_stride, const float* __restrict__ xnorm,
                 const uint32_t* __restrict__ alive, const float* __restrict__ thr_g, uint32_t* __restrict__ cand_count,
                 uint32_t* __restrict__ cand_rows, int cap, float* __restrict__ dump, int64_t S, int dump_min)
 {
@@ -117,9 +120,12 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
                     mbar_wait(&empty_bar[stage], phase ^ 1);
                     unsigned char* sa = smem + (size_t)stage * Cfg::STAGE_BYTES;
                     mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-                    if (MODE == TC_CVT) {
-                        tma_load_2d(sa, &tmX, &full_bar[stage], (2 * kb) * TC_KBLOCK, row0, TMA_EVICT_FIRST);
-                        tma_load_2d(sa + TC_A_BYTES, &tmX, &full_bar[stage], (2 * kb + 1) * TC_KBLOCK, row0, TMA_EVICT_FIRST);
+                    if (MODE == TC_TF32S) {   // split rows: the high and the low halves of block kb, two query boxes
+                        tma_load_3d(sa, &tmX, &full_bar[stage], 0, 2 * kb, row0, TMA_EVICT_FIRST);
+                        tma_load_3d(sa + TC_A_BYTES, &tmX, &full_bar[stage], 0, 2 * kb + 1, row0, TMA_EVICT_FIRST);
+                        tma_load_2d(sa + Cfg::A_BYTES + NQ * 128, &tmQ, &full_bar[stage], kb * Cfg::ELEMS + TC_KBLOCK, 0, TMA_EVICT_LAST);
+                    } else if (MODE == TC_BF16) {
+                        tma_load_3d(sa, &tmX, &full_bar[stage], 0, kb * piece_step, row0, TMA_EVICT_FIRST);
                     } else {
                         tma_load_2d(sa, &tmX, &full_bar[stage], kb * Cfg::ELEMS, row0, TMA_EVICT_FIRST);
                     }
@@ -141,15 +147,19 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
                 mbar_wait(&full_bar[stage], phase);
                 unsigned char* sa = smem + (size_t)stage * Cfg::STAGE_BYTES;
                 const uint64_t bdesc = wgmma_desc_sw128(smem_u32(sa + Cfg::A_BYTES));
-                if (MODE == TC_CVT) {
-                    uint32_t af[4][4];
+                if (MODE == TC_TF32S) {
 #pragma unroll
-                    for (int s = 0; s < 4; ++s) cvt_a_fragment(sa, r_lo, g, q, s, af[s]);
-                    wgmma_fence();
+                    for (int h = 0; h < 2; ++h) {              // query box h: elements 32 h .. 32 h + 31 of the block
+                        uint32_t af[4][4];
 #pragma unroll
-                    for (int s = 0; s < 4; ++s) wgmma_bf16_rs<NQ>(acc, af[s], bdesc + 2 * s, (uint32_t)((kb | s) != 0));
-                    wgmma_commit();
-                    wgmma_wait<0>();                           // the A registers are reused by the next stage
+                        for (int s = 0; s < 4; ++s) tf32s_a_fragment(sa, r_lo, g, q, 4 * h + s, af[s]);
+                        wgmma_fence();
+#pragma unroll
+                        for (int s = 0; s < 4; ++s)
+                            wgmma_tf32_rs<NQ>(acc, af[s], bdesc + h * (NQ * 128 / 16) + 2 * s, (uint32_t)((kb | h | s) != 0));
+                        wgmma_commit();
+                        wgmma_wait<0>();                       // the A registers are reused by the next K steps
+                    }
                 } else {
                     const uint64_t adesc = wgmma_desc_sw128(smem_u32(sa + wg * 64 * 128));
                     wgmma_fence();
@@ -360,7 +370,8 @@ sample_threshold_kernel(const float* __restrict__ dump, int64_t S, int m, int nq
 }
 
 // ------------------------------------------------------------------ exact rescoring
-// one 8-lane group per candidate; same arithmetic as dense_scan_kernel / oracle l2sq_row
+// one 8-lane group per candidate; same arithmetic as dense_scan_kernel / oracle l2sq_row, on plain or split rows
+template <bool SPLIT>
 __global__ void __launch_bounds__(256)
 rescore_kernel(const float* __restrict__ X, int dpad, const float* __restrict__ Q, const uint32_t* __restrict__ cand_count,
                const uint32_t* __restrict__ cand_rows, int cap, OrdMap ord_base, uint64_t* __restrict__ exact_keys)
@@ -377,18 +388,29 @@ rescore_kernel(const float* __restrict__ X, int dpad, const float* __restrict__ 
     __syncthreads();
     const bool valid = c < cnt;
     const uint32_t row = valid ? cand_rows[(size_t)j * cap + c] : 0u;
-    const float4* p = reinterpret_cast<const float4*>(X + (size_t)row * dpad) + l8;
+    const float* xr = X + (size_t)row * dpad;
+    const float4* p = reinterpret_cast<const float4*>(xr) + l8;
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
     const int steps = dpad / KRAG_LANES;
-#pragma unroll 4
-    for (int i = 0; i < steps; ++i) {
-        const float4 a = __ldg(p + i * 8);
+    auto step = [&](int i, const float4& a) {
         const float4 qv = *reinterpret_cast<const float4*>(rs_q + i * KRAG_LANES + l8 * 4);
         float t;
         t = a.x - qv.x; acc.x = fmaf(t, t, acc.x);
         t = a.y - qv.y; acc.y = fmaf(t, t, acc.y);
         t = a.z - qv.z; acc.z = fmaf(t, t, acc.z);
         t = a.w - qv.w; acc.w = fmaf(t, t, acc.w);
+    };
+    if (SPLIT) {   // steps 2 b and 2 b + 1 from block b, in the same order
+#pragma unroll 2
+        for (int b = 0; b < steps / 2; ++b) {
+            float4 a0, a1;
+            split_ld8<false>(xr, b, l8, a0, a1);
+            step(2 * b, a0);
+            step(2 * b + 1, a1);
+        }
+    } else {
+#pragma unroll 4
+        for (int i = 0; i < steps; ++i) step(i, __ldg(p + i * 8));
     }
     float s = (acc.x + acc.y) + (acc.z + acc.w);
     s += __shfl_xor_sync(0xffffffffu, s, 4);
@@ -563,6 +585,7 @@ static EncodeTiledFn get_encode()
     });
     return fn;
 }
+// 2-D map over [rows, dpad] fp32 (box 32 x box_rows) or bf16 (box 64 x box_rows) rows, 128B swizzle
 static bool make_map(CUtensorMap* tm, const void* base, int64_t rows, int dpad, int box_rows, bool bf16 = false)
 {
     EncodeTiledFn enc = get_encode();
@@ -577,11 +600,30 @@ static bool make_map(CUtensorMap* tm, const void* base, int64_t rows, int dpad, 
     return r == CUDA_SUCCESS;
 }
 
+// 3-D map over 128-byte pieces of 64 halves: piece p of row r at base + r * row_bytes + 128 p; box = one piece of
+// TC_TILE_M rows, 128B swizzle (the shared-memory image of a bf16 box of make_map).  bf16 rows: dpad / 64 pieces of 2 dpad
+// bytes; split rows: split_pieces(dpad) pieces of 4 dpad bytes.
+// Split rows promote L2 fills to 128 B only: a 256-byte promotion would fetch the low halves beside every high-half piece.
+static bool make_map_pieces(CUtensorMap* tm, const void* base, int64_t rows, int dpad, bool split)
+{
+    EncodeTiledFn enc = get_encode();
+    if (!enc) return false;
+    cuuint64_t gdim[3] = {(cuuint64_t)SPLIT_BLOCK, (cuuint64_t)(split ? split_pieces(dpad) : dpad / 64), (cuuint64_t)rows};
+    cuuint64_t gstride[2] = {128, (cuuint64_t)dpad * (split ? 4 : 2)};
+    cuuint32_t box[3] = {(cuuint32_t)SPLIT_BLOCK, 1, (cuuint32_t)TC_TILE_M};
+    cuuint32_t estr[3] = {1, 1, 1};
+    CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), gdim, gstride, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                     split ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B : CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    return r == CUDA_SUCCESS;
+}
+
 constexpr int64_t TC_MIN_ROWS = 262144;   // below this the exact scan is cheaper than sample + prune + rescore
 
 bool dense_tc_supported(const DeviceInfo& di, int dpad)
 {
-    return di.cc_major == 9 && dpad % TC_KBLOCK == 0 && di.smem_optin >= TcCfg<256, TC_CVT>::SMEM && get_encode() != nullptr;
+    return di.cc_major == 9 && dpad % TC_KBLOCK == 0 && di.smem_optin >= TcCfg<256, TC_TF32S>::SMEM && get_encode() != nullptr;
 }
 
 static int tc_target(int P, bool bf16 = false)
@@ -648,9 +690,10 @@ static void fetch_rule_constants(int dpad, float* scale, float* eta2)
 static std::atomic<int64_t> g_host_rows_fetched{0};
 int64_t host_rows_fetched() { return g_host_rows_fetched.load(); }
 
-// one launch of the prune kernel (sample pass: MODE = TC_TF32, DUMP) over n_ltiles tiles of 128 rows, tile_stride apart
+// one launch of the prune kernel (sample pass: DUMP) over n_ltiles tiles of 128 rows, tile_stride apart; TC_BF16 reads
+// tmX = make_map_pieces, piece_step 2 on split rows (their high halves), 1 on bf16 rows
 template <int NQ, int MODE, bool DUMP>
-static void tc_launch(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensorMap& tmQ, int64_t n_rows, int dpad,
+static void tc_launch(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensorMap& tmQ, int64_t n_rows, int dpad, int piece_step,
                       int64_t n_ltiles, int tile_stride, const float* xnorm, const uint32_t* alive, const float* thr,
                       uint32_t* cand_count, uint32_t* cand_rows, int cap, float* dump, int64_t S, int dump_min, cudaStream_t st)
 {
@@ -661,7 +704,7 @@ static void tc_launch(const DeviceInfo& di, const CUtensorMap& tmX, const CUtens
         attr_set = true;
     }
     const int grid = (int)(n_ltiles < di.sm_count ? n_ltiles : di.sm_count);
-    dense_tc_kernel<NQ, MODE, DUMP><<<grid, TC_THREADS, Cfg::SMEM, st>>>(tmX, tmQ, n_rows, dpad / Cfg::ELEMS, n_ltiles, tile_stride,
+    dense_tc_kernel<NQ, MODE, DUMP><<<grid, TC_THREADS, Cfg::SMEM, st>>>(tmX, tmQ, n_rows, dpad / Cfg::ELEMS, piece_step, n_ltiles, tile_stride,
                                                                          xnorm, alive, thr, cand_count, cand_rows, cap, dump, S, dump_min);
 }
 
@@ -669,10 +712,11 @@ template <int NQ>
 static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensorMap& tmQ, const float* X, int64_t n_rows,
                     int dpad, const float* xnorm, const uint32_t* xn_max_bits, const uint32_t* alive, const float* q,
                     int nq, int P, OrdMap ord_base, const TcWorkspace& w, int cap, int64_t S, uint64_t* keys_out,
-                    const uint16_t* Xh, bool cvt, const HostRowsView* hr, cudaStream_t st)
+                    const uint16_t* Xh, bool split, bool allow_bf16, const HostRowsView* hr, cudaStream_t st)
 {
     const bool host = hr != nullptr;             // fp32 rows in pinned host memory: both passes read the bf16 copy Xh
-    const bool bf16 = Xh != nullptr || cvt;      // bf16 operands in the prune pass (shadow copy, or converted on chip)
+    // bf16 operands in the prune pass: a bf16 copy Xh (shadow, host rows) or the high halves of split rows (tmX)
+    const bool bf16 = Xh != nullptr || (split && allow_bf16);
     const int64_t n_tiles = (n_rows + TC_TILE_M - 1) / TC_TILE_M;
     const int64_t s_tiles = tc_sample_tiles(n_rows);
     // 1. sample pass (1/64 of the tiles), dump a = |x|^2 - 2 x.q
@@ -682,12 +726,15 @@ static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensor
     if (host) {   // the sample pass only chooses thr: bf16 operands do not enter soundness
         CUtensorMap tmQh, tmXh;
         launch_f32_to_bf16(q, w.q_bf16, (int64_t)nq * dpad, st);
-        if (!make_map(&tmQh, (const void*)w.q_bf16, nq, dpad, NQ, true) || !make_map(&tmXh, Xh, n_rows, dpad, TC_TILE_M, true))
+        if (!make_map(&tmQh, (const void*)w.q_bf16, nq, dpad, NQ, true) || !make_map_pieces(&tmXh, Xh, n_rows, dpad, false))
             throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled(bf16 rows)", __FILE__, __LINE__};
-        tc_launch<NQ, TC_BF16, true>(di, tmXh, tmQh, n_rows, dpad, s_tiles, TC_SAMPLE_STRIDE, xnorm, alive, nullptr, nullptr, nullptr, 0,
+        tc_launch<NQ, TC_BF16, true>(di, tmXh, tmQh, n_rows, dpad, 1, s_tiles, TC_SAMPLE_STRIDE, xnorm, alive, nullptr, nullptr, nullptr, 0,
                                      w.dump, S_min, 1, st);
+    } else if (split) {
+        tc_launch<NQ, TC_TF32S, true>(di, tmX, tmQ, n_rows, dpad, 2, s_tiles, TC_SAMPLE_STRIDE, xnorm, alive, nullptr, nullptr, nullptr, 0,
+                                      w.dump, S_min, 1, st);
     } else {
-        tc_launch<NQ, TC_TF32, true>(di, tmX, tmQ, n_rows, dpad, s_tiles, TC_SAMPLE_STRIDE, xnorm, alive, nullptr, nullptr, nullptr, 0,
+        tc_launch<NQ, TC_TF32, true>(di, tmX, tmQ, n_rows, dpad, 1, s_tiles, TC_SAMPLE_STRIDE, xnorm, alive, nullptr, nullptr, nullptr, 0,
                                      w.dump, S_min, 1, st);
     }
     KRAG_CUDA(cudaGetLastError());
@@ -709,24 +756,29 @@ static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensor
     count_launch();
     KRAG_CUDA(cudaMemsetAsync(w.cand_count, 0, 256 * 4, st));
     // 3. main pass: stream the corpus once, prune on the tensor cores
-    if (bf16 && !host) launch_f32_to_bf16(q, w.q_bf16, (int64_t)nq * dpad, st);
-    dense_timer_begin(st, host ? 6 : (cvt ? 5 : (bf16 ? 4 : 3)), n_rows * (int64_t)dpad * ((bf16 && !cvt) ? 2 : 4),
-                      2 * (int64_t)NQ * n_rows * dpad);
+    // split rows: queries in the rows' lane order inside each 64-element block
+    if (Xh && !host) launch_f32_to_bf16(q, w.q_bf16, (int64_t)nq * dpad, st);
+    else if (bf16 && !host) launch_bf16_split_order(q, w.q_bf16, (int64_t)nq * dpad, st);
+    // kernel ids: 6 host rows' bf16 copy, 4 bf16 shadow, 5 high halves of split rows, 3 tf32
+    dense_timer_begin(st, host ? 6 : (Xh ? 4 : (bf16 ? 5 : 3)), n_rows * (int64_t)dpad * (bf16 ? 2 : 4), 2 * (int64_t)NQ * n_rows * dpad);
     if (bf16) {
         CUtensorMap tmQh, tmXh;
         if (!make_map(&tmQh, (const void*)w.q_bf16, nq, dpad, NQ, true))
             throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled(Q, bf16)", __FILE__, __LINE__};
-        if (cvt) {
-            tc_launch<NQ, TC_CVT, false>(di, tmX, tmQh, n_rows, dpad, n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap,
-                                         nullptr, 0, 0, st);
+        if (Xh) {
+            if (!make_map_pieces(&tmXh, Xh, n_rows, dpad, false))
+                throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled(bf16 rows)", __FILE__, __LINE__};
+            tc_launch<NQ, TC_BF16, false>(di, tmXh, tmQh, n_rows, dpad, 1, n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap,
+                                          nullptr, 0, 0, st);
         } else {
-            if (!make_map(&tmXh, Xh, n_rows, dpad, TC_TILE_M, true))
-                throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled(bf16 shadow)", __FILE__, __LINE__};
-            tc_launch<NQ, TC_BF16, false>(di, tmXh, tmQh, n_rows, dpad, n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap,
+            tc_launch<NQ, TC_BF16, false>(di, tmX, tmQh, n_rows, dpad, 2, n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap,
                                           nullptr, 0, 0, st);
         }
+    } else if (split) {
+        tc_launch<NQ, TC_TF32S, false>(di, tmX, tmQ, n_rows, dpad, 2, n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap,
+                                       nullptr, 0, 0, st);
     } else {
-        tc_launch<NQ, TC_TF32, false>(di, tmX, tmQ, n_rows, dpad, n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap,
+        tc_launch<NQ, TC_TF32, false>(di, tmX, tmQ, n_rows, dpad, 1, n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap,
                                       nullptr, 0, 0, st);
     }
     dense_timer_end(st);
@@ -735,7 +787,8 @@ static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensor
     // 4. exact fp32 rescoring of the survivors + top-P
     static bool rs_attr_set = false;
     if (!rs_attr_set) {   // the query row sits in shared memory: up to 64 KB at dim 16384, past the default 48 KB limit
-        KRAG_CUDA(cudaFuncSetAttribute(rescore_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 4));
+        KRAG_CUDA(cudaFuncSetAttribute(rescore_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 4));
+        KRAG_CUDA(cudaFuncSetAttribute(rescore_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 4));
         rs_attr_set = true;
     }
     dim3 rg((unsigned)((cap + 31) / 32), (unsigned)nq);
@@ -762,7 +815,8 @@ static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensor
         rescore_mapped_kernel<<<rg, 256, (size_t)dpad * 4, st>>>(hr->d, dpad, q, w.fetch_count, w.fetch_rows, cap, ord_base,
                                                                  w.exact_keys);
     } else {
-        rescore_kernel<<<rg, 256, (size_t)dpad * 4, st>>>(X, dpad, q, w.cand_count, w.cand_rows, cap, ord_base, w.exact_keys);
+        if (split) rescore_kernel<true><<<rg, 256, (size_t)dpad * 4, st>>>(X, dpad, q, w.cand_count, w.cand_rows, cap, ord_base, w.exact_keys);
+        else rescore_kernel<false><<<rg, 256, (size_t)dpad * 4, st>>>(X, dpad, q, w.cand_count, w.cand_rows, cap, ord_base, w.exact_keys);
     }
     KRAG_CUDA(cudaGetLastError());
     count_launch();
@@ -780,19 +834,17 @@ int64_t dense_tc_fallback_queries() { return g_tc_fallback_queries.load(); }
 bool launch_dense_tc(const DeviceInfo& di, const float* X, int64_t n_rows, int dpad, const uint32_t* alive,
                      const float* xnorm, const uint32_t* xn_max_bits, const float* q, int batch, int P, OrdMap ord_base,
                      void* workspace, size_t workspace_bytes, uint64_t* part, uint64_t* keys_out, cudaStream_t st,
-                     const uint16_t* Xh, bool allow_cvt)
+                     const uint16_t* Xh, bool allow_bf16, bool split)
 {
     if (Xh != nullptr && dpad % (2 * TC_KBLOCK) != 0) Xh = nullptr;   // bf16 k-blocks are 64 elements wide
-    // default prune pass: fp32 rows rounded to bf16 on their way into the wgmma A registers (no shadow); allow_cvt = false
-    // keeps the TF32 pass
-    const bool cvt = Xh == nullptr && allow_cvt && dpad % (2 * TC_KBLOCK) == 0;
+    // default prune pass on split rows: bf16 wgmma on their high halves; allow_bf16 = false keeps the TF32 pass
     if (n_rows < TC_MIN_ROWS || n_rows >= (1ll << 31) || xnorm == nullptr) return false;
     const int cap = tc_cap(P);
     const int64_t S = tc_sample_tiles(n_rows) * TC_TILE_M;
     TcWorkspace w;
     if (tc_carve(&w, (unsigned char*)workspace, cap, S) > workspace_bytes) return false;
     CUtensorMap tmX;
-    if (!make_map(&tmX, X, n_rows, dpad, TC_TILE_M)) return false;
+    if (!(split ? make_map_pieces(&tmX, X, n_rows, dpad, true) : make_map(&tmX, X, n_rows, dpad, TC_TILE_M))) return false;
     std::vector<int32_t> flags(256);
     for (int b0 = 0; b0 < batch; b0 += 256) {
         const int nq = batch - b0 < 256 ? batch - b0 : 256;
@@ -801,16 +853,16 @@ bool launch_dense_tc(const DeviceInfo& di, const float* X, int64_t n_rows, int d
         CUtensorMap tmQ;
         if (!make_map(&tmQ, qb, nq, dpad, NQ)) return false;
         uint64_t* ko = keys_out + (size_t)b0 * P;
-        if (NQ == 64) tc_pass<64>(di, tmX, tmQ, X, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, Xh, cvt, nullptr, st);
-        else if (NQ == 128) tc_pass<128>(di, tmX, tmQ, X, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, Xh, cvt, nullptr, st);
-        else tc_pass<256>(di, tmX, tmQ, X, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, Xh, cvt, nullptr, st);
+        if (NQ == 64) tc_pass<64>(di, tmX, tmQ, X, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, Xh, split, allow_bf16, nullptr, st);
+        else if (NQ == 128) tc_pass<128>(di, tmX, tmQ, X, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, Xh, split, allow_bf16, nullptr, st);
+        else tc_pass<256>(di, tmX, tmQ, X, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, Xh, split, allow_bf16, nullptr, st);
         // uncertified queries (rare) are re-run on the exact scan kernel -- still on the GPU
         KRAG_CUDA(cudaMemcpyAsync(flags.data(), w.flags, sizeof(int32_t) * (size_t)nq, cudaMemcpyDeviceToHost, st));
         KRAG_CUDA(cudaStreamSynchronize(st));
         for (int j = 0; j < nq; ++j) {
             if (flags[(size_t)j]) continue;
             ++g_tc_fallback_queries;
-            launch_dense_scan(di, X, n_rows, dpad, alive, qb + (size_t)j * dpad, 1, P, ord_base, part, ko + (size_t)j * P, st);
+            launch_dense_scan(di, X, n_rows, dpad, alive, qb + (size_t)j * dpad, 1, P, ord_base, part, ko + (size_t)j * P, st, split);
         }
     }
     return true;
@@ -836,9 +888,9 @@ bool launch_dense_tc_host(const DeviceInfo& di, const HostRowsView& hr, int64_t 
         const int NQ = nq <= 64 ? 64 : (nq <= 128 ? 128 : 256);
         const float* qb = q + (size_t)b0 * dpad;
         uint64_t* ko = keys_out + (size_t)b0 * P;
-        if (NQ == 64) tc_pass<64>(di, unused, unused, nullptr, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, hr.bf16, false, &hr, st);
-        else if (NQ == 128) tc_pass<128>(di, unused, unused, nullptr, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, hr.bf16, false, &hr, st);
-        else tc_pass<256>(di, unused, unused, nullptr, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, hr.bf16, false, &hr, st);
+        if (NQ == 64) tc_pass<64>(di, unused, unused, nullptr, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, hr.bf16, false, false, &hr, st);
+        else if (NQ == 128) tc_pass<128>(di, unused, unused, nullptr, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, hr.bf16, false, false, &hr, st);
+        else tc_pass<256>(di, unused, unused, nullptr, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, hr.bf16, false, false, &hr, st);
         KRAG_CUDA(cudaMemcpyAsync(flags.data(), w.flags, sizeof(int32_t) * (size_t)nq, cudaMemcpyDeviceToHost, st));
         KRAG_CUDA(cudaMemcpyAsync(fetched.data(), w.fetch_count, sizeof(uint32_t) * (size_t)nq, cudaMemcpyDeviceToHost, st));
         KRAG_CUDA(cudaStreamSynchronize(st));
@@ -862,7 +914,7 @@ bool launch_dense_tc_host(const DeviceInfo& di, const HostRowsView& hr, int64_t 
     return true;
 }
 
-bool dense_tc_debug_dump(const DeviceInfo& di, const float* X, int64_t n_rows, int dpad, const float* xnorm,
+bool dense_tc_debug_dump(const DeviceInfo& di, const float* X, bool split, int64_t n_rows, int dpad, const float* xnorm,
                          const float* q, int nq, float* dump_out, int64_t* S_out, int* nq_pad_out, cudaStream_t st)
 {
     if (!dense_tc_supported(di, dpad) || nq > 256) return false;
@@ -873,10 +925,12 @@ bool dense_tc_debug_dump(const DeviceInfo& di, const float* X, int64_t n_rows, i
     *nq_pad_out = NQ;
     if (dump_out == nullptr) return true;   // size query
     CUtensorMap tmX, tmQ;
-    if (!make_map(&tmX, X, n_rows, dpad, TC_TILE_M) || !make_map(&tmQ, q, nq, dpad, NQ)) return false;
-#define KRAG_TC_DUMP(N)                                                                                                    \
-    tc_launch<N, TC_TF32, true>(di, tmX, tmQ, n_rows, dpad, n_tiles, 1, xnorm, nullptr, nullptr, nullptr, nullptr, 0, dump_out, S, 0, st)
-    if (NQ == 64) KRAG_TC_DUMP(64); else if (NQ == 128) KRAG_TC_DUMP(128); else KRAG_TC_DUMP(256);
+    if (!(split ? make_map_pieces(&tmX, X, n_rows, dpad, true) : make_map(&tmX, X, n_rows, dpad, TC_TILE_M)) || !make_map(&tmQ, q, nq, dpad, NQ))
+        return false;
+#define KRAG_TC_DUMP(N, MODE)                                                                                              \
+    tc_launch<N, MODE, true>(di, tmX, tmQ, n_rows, dpad, 2, n_tiles, 1, xnorm, nullptr, nullptr, nullptr, nullptr, 0, dump_out, S, 0, st)
+    if (split) { if (NQ == 64) KRAG_TC_DUMP(64, TC_TF32S); else if (NQ == 128) KRAG_TC_DUMP(128, TC_TF32S); else KRAG_TC_DUMP(256, TC_TF32S); }
+    else { if (NQ == 64) KRAG_TC_DUMP(64, TC_TF32); else if (NQ == 128) KRAG_TC_DUMP(128, TC_TF32); else KRAG_TC_DUMP(256, TC_TF32); }
 #undef KRAG_TC_DUMP
     KRAG_CUDA(cudaGetLastError());
     count_launch();

@@ -211,11 +211,11 @@ int64_t launch_count();
 
 // ---- K1: exact fp32 L2^2 scan + fused top-P (dense_scan.cu)
 // q: device [batch, dpad] zero-padded.  part: workspace >= dense_scan_part_elems() u64.
-// keys_out: device [batch, P], ascending, KEY_PAD padded, ordinals already global.
+// keys_out: device [batch, P], ascending, KEY_PAD padded, ordinals already global.  split: X holds split rows (split_rows.cuh).
 size_t dense_scan_part_elems(const DeviceInfo& di, int P);
 void launch_dense_scan(const DeviceInfo& di, const float* X, int64_t n_rows, int dpad, const uint32_t* alive,
                        const float* q, int batch, int P, OrdMap ord_base, uint64_t* part, uint64_t* keys_out,
-                       cudaStream_t st);
+                       cudaStream_t st, bool split);
 
 // ---- host-resident rows (KRAG_ROWS_HOST): fp32 rows in pinned host memory, bf16 copy + residual norms on the device
 struct HostRowsView {
@@ -259,12 +259,13 @@ void launch_row_norms(const float* X, int64_t row0, int64_t n, int dpad, float* 
 bool launch_dense_tc(const DeviceInfo& di, const float* X, int64_t n_rows, int dpad, const uint32_t* alive,
                      const float* xnorm, const uint32_t* xn_max_bits, const float* q, int batch, int P,
                      OrdMap ord_base, void* workspace, size_t workspace_bytes, uint64_t* part, uint64_t* keys_out,
-                     cudaStream_t st, const uint16_t* Xh = nullptr /* optional bf16 shadow of X for the prune pass */,
-                     bool allow_cvt = true /* fp32 rows rounded to bf16 on chip (bf16 wgmma) instead of tf32 wgmma */);
+                     cudaStream_t st, const uint16_t* Xh /* optional bf16 shadow of X for the prune pass */,
+                     bool allow_bf16 /* split rows: bf16 wgmma on their high halves instead of tf32 wgmma */,
+                     bool split /* X holds split rows (split_rows.cuh) */);
 void launch_f32_to_bf16(const float* in, uint16_t* out, int64_t n_elems, cudaStream_t st);
 int64_t dense_tc_fallback_queries();   // queries re-run on K1 because the exactness certificate failed
 // diagnostics: a[j][r] = |x_r|^2 - 2 x_r.q_j for ALL rows through the tensor-core kernel (tests only)
-bool dense_tc_debug_dump(const DeviceInfo& di, const float* X, int64_t n_rows, int dpad, const float* xnorm,
+bool dense_tc_debug_dump(const DeviceInfo& di, const float* X, bool split, int64_t n_rows, int dpad, const float* xnorm,
                          const float* q, int nq, float* dump_out /*[NQ_pad][S]*/, int64_t* S_out, int* nq_pad_out,
                          cudaStream_t st);
 
