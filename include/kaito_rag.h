@@ -429,14 +429,30 @@ int32_t krag_last_compact(float* move_ms, float* postings_ms, int64_t* rows_move
  * krag_index_load or krag_synth_fill), the postings written, and the term-list entries read to build them (those of the
  * rows added since the last commit when merged, every entry otherwise). */
 int32_t krag_last_commit(float* total_ms, float* host_ms, int32_t* merged, int64_t* postings_written, int64_t* delta_entries);
-/* raw K2 output a[j][r] = |x_r|^2 - 2 x_r.q_j (TF32) for every row, [nq_pad][S] row-major;
- * call with out == NULL to query S and nq_pad.  Test hook for the tensor-core kernel; KRAG_E_UNSUPPORTED for
- * KRAG_ROWS_HOST indexes. */
 /* test hook: rows [row0, row0 + n) of a device-resident index as stored, dim_padded 32-bit words per row (split rows where
  * dim_padded % 64 == 0, DESIGN.md section 4 K2) */
 int32_t krag_debug_read_stored_rows(krag_index* idx, int64_t row0, int64_t n, float* out);
+/* raw K2 output a[j][r] = |x_r|^2 - 2 x_r.q_j (TF32) for every row, [nq_pad][S] row-major;
+ * call with out == NULL to query S and nq_pad.  Test hook for the tensor-core kernel; KRAG_E_UNSUPPORTED for
+ * KRAG_ROWS_HOST indexes.  The same as krag_debug_tc_dump_pass(idx, KRAG_TC_PASS_TF32, ...). */
 int32_t krag_debug_tc_dump(krag_index* idx, int32_t nq, const float* q, float* out, int64_t out_elems,
                            int64_t* S_out, int32_t* nq_pad_out);
+/* the prune passes of K2 the test hooks below run (each the kernel instantiation the search itself uses) */
+#define KRAG_TC_PASS_TF32 0        /* tf32 wgmma: on split rows their rebuilt fp32 values, else the plain fp32 rows */
+#define KRAG_TC_PASS_BF16_SPLIT 1  /* bf16 wgmma on the high halves of split rows (kernel id 5) */
+#define KRAG_TC_PASS_BF16_SHADOW 2 /* bf16 wgmma on the bf16 shadow (kernel id 4); KRAG_E_STATE when there is none */
+#define KRAG_TC_PASS_BF16_HOST 3   /* bf16 wgmma on the device copy of a KRAG_ROWS_HOST index (kernel id 6) */
+/* krag_debug_tc_dump for any prune pass: a[j][r] = |x_r|^2 - 2 x_r.q_j as that pass computes it, for every row (rows past
+ * the end and tombstones included; the padding rows up to S are +inf) and every query column up to nq_pad (the NQ bucket
+ * of nq: 64, 128 or 256; padded columns hold zero queries, so they return |x_r|^2).  Test hook. */
+int32_t krag_debug_tc_dump_pass(krag_index* idx, int32_t pass, int32_t nq, const float* q, float* out, int64_t out_elems,
+                                int64_t* S_out, int32_t* nq_pad_out);
+/* one main prune pass of K2 over every row with caller-chosen thresholds: thr [nq_pad] (nq_pad = 64, 128 or 256, the NQ
+ * bucket of nq; padded columns run zero queries with the thresholds given for them), the index's tombstones honoured.
+ * counts_out [nq_pad] = rows with a < thr[j] (as the epilogue decides it), rows_out [nq_pad][cap] = the first
+ * min(count, cap) of them in no particular order (entries past that undefined).  Test hook. */
+int32_t krag_debug_tc_prune(krag_index* idx, int32_t pass, int32_t nq, const float* q, const float* thr, int32_t cap,
+                            uint32_t* counts_out, uint32_t* rows_out);
 
 #ifdef __cplusplus
 }

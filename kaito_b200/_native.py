@@ -42,8 +42,10 @@ SYMBOLS = [
     "krag_dev_redeal_pack", "krag_dev_redeal_unpack", "krag_redeal_finish", "krag_redeal_abort", "krag_embedder_set_pooling",
     "krag_debug_embedder_cls_rows", "krag_rerank", "krag_embedder_set_precision", "krag_debug_gemm_f16",
     "krag_embedder_set_position_offset", "krag_text_unigram_create", "krag_text_unigram_encode_batch",
-    "krag_text_unigram_destroy",
+    "krag_text_unigram_destroy", "krag_debug_tc_dump_pass", "krag_debug_tc_prune",
 ]
+# krag_debug_tc_dump_pass / krag_debug_tc_prune: the prune pass to run (KRAG_TC_PASS_*)
+TC_PASS_TF32, TC_PASS_BF16_SPLIT, TC_PASS_BF16_SHADOW, TC_PASS_BF16_HOST = 0, 1, 2, 3
 # krag_embedder_set_precision: split-fp16 products held to fp32 arithmetic, or fp16 operands with fp32 accumulation
 PRECISIONS = {"fp32": 0, "fp16": 1}
 RERANK_SIGMOID, RERANK_IDENTITY = 0, 1   # krag_rerank: activation of the classifier logit
@@ -160,6 +162,8 @@ def load() -> C.CDLL:
     L.krag_last_compact.argtypes = [C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(i64), C.POINTER(i64)]
     L.krag_last_commit.argtypes = [C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]
     L.krag_debug_tc_dump.argtypes = [vp, i32, vp, vp, i64, C.POINTER(i64), C.POINTER(i32)]
+    L.krag_debug_tc_dump_pass.argtypes = [vp, i32, i32, vp, vp, i64, C.POINTER(i64), C.POINTER(i32)]
+    L.krag_debug_tc_prune.argtypes = [vp, i32, i32, vp, vp, i32, vp, vp]
     L.krag_debug_read_stored_rows.argtypes = [vp, i64, i64, vp]
     for name in SYMBOLS:
         fn = getattr(L, name)
@@ -609,6 +613,28 @@ class Index:
         out = np.empty((nqp.value, S.value), np.float32)
         check(self._L.krag_debug_tc_dump(self._h, q.shape[0], ptr(q), ptr(out), out.size, C.byref(S), C.byref(nqp)))
         return out
+
+    def debug_tc_dump_pass(self, q, tc_pass: int) -> np.ndarray:
+        """a[j, r] = |x_r|^2 - 2 x_r.q_j from one prune pass (TC_PASS_*) over every row: [nq_pad, S] (test hook)"""
+        q = np.ascontiguousarray(q, np.float32).reshape(-1, self.dim)
+        S, nqp = C.c_int64(0), C.c_int32(0)
+        check(self._L.krag_debug_tc_dump_pass(self._h, tc_pass, q.shape[0], ptr(q), None, 0, C.byref(S), C.byref(nqp)))
+        out = np.empty((nqp.value, S.value), np.float32)
+        check(self._L.krag_debug_tc_dump_pass(self._h, tc_pass, q.shape[0], ptr(q), ptr(out), out.size, C.byref(S), C.byref(nqp)))
+        return out
+
+    def debug_tc_prune(self, q, thr, cap: int, tc_pass: int):
+        """one main prune pass (TC_PASS_*) with thresholds thr [nq_pad] (nq_pad = 64, 128 or 256, the NQ bucket of the
+        batch): (counts uint32 [nq_pad], rows uint32 [nq_pad, cap], valid in each row up to min(count, cap)) (test hook)"""
+        q = np.ascontiguousarray(q, np.float32).reshape(-1, self.dim)
+        nqp = 64 if q.shape[0] <= 64 else (128 if q.shape[0] <= 128 else 256)
+        thr = np.ascontiguousarray(thr, np.float32)
+        if thr.shape != (nqp,):
+            raise ValueError(f"thr must hold {nqp} thresholds, one per query column of the NQ bucket")
+        counts = np.zeros(nqp, np.uint32)
+        rows = np.zeros((nqp, cap), np.uint32)
+        check(self._L.krag_debug_tc_prune(self._h, tc_pass, q.shape[0], ptr(q), ptr(thr), cap, ptr(counts), ptr(rows)))
+        return counts, rows
 
     def debug_stored_rows(self, row0: int, n: int) -> np.ndarray:
         """rows [row0, row0 + n) as the device stores them: uint32 [n, dim_padded] (test hook)"""

@@ -1595,27 +1595,80 @@ int32_t krag_last_dense_kernel(float* ms, int32_t* kernel_id, int64_t* algorithm
     });
 }
 
-int32_t krag_debug_tc_dump(krag_index* ix, int32_t nq, const float* q, float* out, int64_t out_elems, int64_t* S_out, int32_t* nq_pad_out)
+namespace {
+// the index's rows for one prune pass of the test hooks (krag_debug_tc_dump_pass, krag_debug_tc_prune)
+void require_tc_pass(const krag_index* ix, int32_t pass)
+{
+    KRAG_REQUIRE(pass >= KRAG_TC_PASS_TF32 && pass <= KRAG_TC_PASS_BF16_HOST, KRAG_E_INVALID, "unknown prune pass");
+    KRAG_REQUIRE(ix->n_rows > 0, KRAG_E_STATE, "index has no rows");
+    if (pass == KRAG_TC_PASS_BF16_HOST) {
+        KRAG_REQUIRE(ix->host_rows, KRAG_E_UNSUPPORTED, "the host-rows pass needs a KRAG_ROWS_HOST index");
+        return;
+    }
+    KRAG_REQUIRE(!ix->host_rows, KRAG_E_UNSUPPORTED, "this prune pass needs device-resident rows");
+    KRAG_REQUIRE(pass != KRAG_TC_PASS_BF16_SPLIT || ix->split_rows, KRAG_E_UNSUPPORTED, "the index does not keep split rows");
+    KRAG_REQUIRE(pass != KRAG_TC_PASS_BF16_SHADOW || ix->Xh.p, KRAG_E_STATE, "the index has no bf16 shadow");
+}
+}  // namespace
+
+int32_t krag_debug_tc_dump_pass(krag_index* ix, int32_t pass, int32_t nq, const float* q, float* out, int64_t out_elems,
+                                int64_t* S_out, int32_t* nq_pad_out)
 {
     return guarded([&] {
         KRAG_REQUIRE(ix && q && S_out && nq_pad_out && nq >= 1 && nq <= 256, KRAG_E_INVALID, "bad argument");
         std::shared_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
-        KRAG_REQUIRE(!ix->host_rows, KRAG_E_UNSUPPORTED, "the fp32 tensor-core dump needs device-resident rows");
+        require_tc_pass(ix, pass);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
+        KRAG_REQUIRE(dense_tc_supported(ix->ctx->di, ix->dpad), KRAG_E_UNSUPPORTED, "tensor-core path unavailable");
         SlotLease lease(ix->ctx);
         Slot* s = lease.s;
         int64_t S = 0; int nqp = 0;
-        KRAG_REQUIRE(dense_tc_debug_dump(ix->ctx->di, ix->X.p, ix->split_rows, ix->n_rows, ix->dpad, ix->xnorm.p, nullptr, nq, nullptr, &S, &nqp, s->st),
-                     KRAG_E_UNSUPPORTED, "tensor-core path unavailable");
+        const size_t ws = dense_tc_debug_carve(nullptr, nullptr, ix->n_rows, ix->dpad, nq, 0, &S, &nqp);
         *S_out = S; *nq_pad_out = nqp;
         if (!out) return;
         KRAG_REQUIRE(out_elems >= S * nqp, KRAG_E_INVALID, "output buffer too small");
         const float* dq = upload_queries(ix, s, q, nq);
-        s->tc_ws.reserve(S * nqp * 4, 0, s->st);
-        KRAG_REQUIRE(dense_tc_debug_dump(ix->ctx->di, ix->X.p, ix->split_rows, ix->n_rows, ix->dpad, ix->xnorm.p, dq, nq, (float*)s->tc_ws.p, &S, &nqp, s->st),
+        s->tc_ws.reserve((int64_t)ws, 0, s->st);
+        TcDebugWs w;
+        dense_tc_debug_carve(&w, s->tc_ws.p, ix->n_rows, ix->dpad, nq, 0, &S, &nqp);
+        KRAG_REQUIRE(dense_tc_debug_pass(ix->ctx->di, pass, ix->X.p, ix->Xh.p, ix->split_rows, ix->n_rows, ix->dpad, ix->xnorm.p,
+                                         nullptr, dq, nq, w, 0, s->st),
                      KRAG_E_UNSUPPORTED, "tensor-core dump failed");
-        KRAG_CUDA(cudaMemcpyAsync(out, s->tc_ws.p, sizeof(float) * (size_t)(S * nqp), cudaMemcpyDeviceToHost, s->st));
+        KRAG_CUDA(cudaMemcpyAsync(out, w.dump, sizeof(float) * (size_t)(S * nqp), cudaMemcpyDeviceToHost, s->st));
+        KRAG_CUDA(cudaStreamSynchronize(s->st));
+    });
+}
+
+int32_t krag_debug_tc_dump(krag_index* ix, int32_t nq, const float* q, float* out, int64_t out_elems, int64_t* S_out, int32_t* nq_pad_out)
+{
+    return krag_debug_tc_dump_pass(ix, KRAG_TC_PASS_TF32, nq, q, out, out_elems, S_out, nq_pad_out);
+}
+
+int32_t krag_debug_tc_prune(krag_index* ix, int32_t pass, int32_t nq, const float* q, const float* thr, int32_t cap,
+                            uint32_t* counts_out, uint32_t* rows_out)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(ix && q && thr && counts_out && rows_out && nq >= 1 && nq <= 256 && cap >= 1, KRAG_E_INVALID, "bad argument");
+        std::shared_lock<std::shared_mutex> lk(ix->mu);
+        require_idle(ix);
+        require_tc_pass(ix, pass);
+        KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
+        KRAG_REQUIRE(dense_tc_supported(ix->ctx->di, ix->dpad), KRAG_E_UNSUPPORTED, "tensor-core path unavailable");
+        SlotLease lease(ix->ctx);
+        Slot* s = lease.s;
+        int64_t S = 0; int nqp = 0;
+        const size_t ws = dense_tc_debug_carve(nullptr, nullptr, ix->n_rows, ix->dpad, nq, cap, &S, &nqp);
+        const float* dq = upload_queries(ix, s, q, nq);
+        s->tc_ws.reserve((int64_t)ws, 0, s->st);
+        TcDebugWs w;
+        dense_tc_debug_carve(&w, s->tc_ws.p, ix->n_rows, ix->dpad, nq, cap, &S, &nqp);
+        KRAG_CUDA(cudaMemcpyAsync(w.thr, thr, sizeof(float) * (size_t)nqp, cudaMemcpyHostToDevice, s->st));
+        KRAG_REQUIRE(dense_tc_debug_pass(ix->ctx->di, pass, ix->X.p, ix->Xh.p, ix->split_rows, ix->n_rows, ix->dpad, ix->xnorm.p,
+                                         alive_ptr(ix), dq, nq, w, cap, s->st),
+                     KRAG_E_UNSUPPORTED, "tensor-core prune pass failed");
+        KRAG_CUDA(cudaMemcpyAsync(counts_out, w.cand_count, sizeof(uint32_t) * (size_t)nqp, cudaMemcpyDeviceToHost, s->st));
+        KRAG_CUDA(cudaMemcpyAsync(rows_out, w.cand_rows, sizeof(uint32_t) * (size_t)nqp * cap, cudaMemcpyDeviceToHost, s->st));
         KRAG_CUDA(cudaStreamSynchronize(s->st));
     });
 }

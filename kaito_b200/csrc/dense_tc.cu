@@ -542,7 +542,7 @@ fetch_compact_kernel(const uint32_t* __restrict__ cand_count, const uint32_t* __
 // ------------------------------------------------------------------------ certificate
 __global__ void certify_kernel(const float* __restrict__ Q, int dpad, int nq, int P, const float* __restrict__ thr,
                                const uint32_t* __restrict__ cand_count, int cap, const uint64_t* __restrict__ keys_out,
-                               const uint32_t* __restrict__ xn_max_bits, float eps_rel, int32_t* __restrict__ flags)
+                               const uint32_t* __restrict__ xn_max_bits, float eps_rel, float slack_rel, int32_t* __restrict__ flags)
 {
     const int j = blockIdx.x * blockDim.x / 32 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (j >= nq) return;
@@ -561,7 +561,7 @@ __global__ void certify_kernel(const float* __restrict__ Q, int dpad, int nq, in
             //   bf16 (both operands rounded to nearest, 2^-8 each): 2^-7 + 2^-12
             // a pruned row has main-pass a >= thr, so its exact a >= thr - 2 eps; the sample pass only picks thr
             const float eps = eps_rel * sqrtf(xmax) * sqrtf(qn);
-            const float slack = 4e-6f * (1.f + qn + xmax);   // fp32 rounding of |x|^2, |q|^2 and the epilogue fma
+            const float slack = slack_rel * (1.f + qn + xmax);   // fp32 rounding elsewhere (certify_slack_rel)
             ok = dP <= thr[j] + qn - 2.f * eps - slack;
         }
         flags[j] = ok ? 1 : 0;
@@ -687,8 +687,29 @@ static void fetch_rule_constants(int dpad, float* scale, float* eta2)
     *eta2 = nextafterf((float)(2.0 * eta / (1.0 - gamma)), INFINITY);
 }
 
+// Slack of the certificate (certify_kernel): what fp32 rounding outside the main pass's dot product can move a pruned row's
+// distance by, as a multiple of (1 + |q|^2 + |x|^2max).  A term passes through at most
+//   mx = dpad / 128 + 9 roundings in |x|^2 (row_norms_kernel: its square and the 3 adds of its float4, the lane's dpad / 128
+//        float4 adds, the 5-step butterfly),
+//   mq = dpad / 32 + 5 in |q|^2 (certify_kernel: the lane's FFMA chain of dpad / 32 steps, the butterfly),
+//   mk = dpad / 32 + 7 in K1's distance of the pruned row (fetch_rule_constants), whose D <= 2 (|x|^2 + |q|^2),
+// and the epilogue's add (|2 acc + thr| <= 3 (|x|^2max + |q|^2)) and the certificate's three adds (operands below
+// 2 (|x|^2max + |q|^2)) round 9 more times.  With u = 2^-24 that is (max(mx, mq) + 2 mk + 9) gamma-factors of u, rounded up;
+// never below 4e-6, the constant it replaces, which rows from dpad 448 on outgrow (6.0e-6 at 768, 9.3e-5 at 16384).
+static float certify_slack_rel(int dpad)
+{
+    const double u = ldexp(1.0, -24);
+    const double mx = dpad / 128 + 9, mq = dpad / KRAG_LANES + 5, mk = dpad / KRAG_LANES + 7;
+    const double m = (mx > mq ? mx : mq) + 2.0 * mk + 9.0;
+    const double c = m * u / (1.0 - m * u);
+    return c > 4e-6 ? nextafterf((float)c, INFINITY) : 4e-6f;
+}
+
 static std::atomic<int64_t> g_host_rows_fetched{0};
 int64_t host_rows_fetched() { return g_host_rows_fetched.load(); }
+
+// TC_BF16 k-block step in 128-byte pieces: split rows interleave high- and low-half pieces, a bf16 copy holds only bf16 pieces
+static int tc_bf16_piece_step(bool split) { return split ? 2 : 1; }
 
 // one launch of the prune kernel (sample pass: DUMP) over n_ltiles tiles of 128 rows, tile_stride apart; TC_BF16 reads
 // tmX = make_map_pieces, piece_step 2 on split rows (their high halves), 1 on bf16 rows
@@ -768,10 +789,10 @@ static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensor
         if (Xh) {
             if (!make_map_pieces(&tmXh, Xh, n_rows, dpad, false))
                 throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled(bf16 rows)", __FILE__, __LINE__};
-            tc_launch<NQ, TC_BF16, false>(di, tmXh, tmQh, n_rows, dpad, 1, n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap,
+            tc_launch<NQ, TC_BF16, false>(di, tmXh, tmQh, n_rows, dpad, tc_bf16_piece_step(false), n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap,
                                           nullptr, 0, 0, st);
         } else {
-            tc_launch<NQ, TC_BF16, false>(di, tmX, tmQh, n_rows, dpad, 2, n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap,
+            tc_launch<NQ, TC_BF16, false>(di, tmX, tmQh, n_rows, dpad, tc_bf16_piece_step(true), n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap,
                                           nullptr, 0, 0, st);
         }
     } else if (split) {
@@ -823,7 +844,8 @@ static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensor
     launch_merge(w.exact_keys, 1, cap, nq, P, cap, cap, keys_out, st);
     // 5. certificate: the error bound of the main pass's operands (the sample pass only chooses thr, whatever its value)
     const float eps_rel = bf16 ? (0.0078125f + 0.000244140625f) : (0.001953125f + 0.000244140625f);
-    certify_kernel<<<(nq * 32 + 255) / 256, 256, 0, st>>>(q, dpad, nq, P, w.thr, w.cand_count, cap, keys_out, xn_max_bits, eps_rel, w.flags);
+    certify_kernel<<<(nq * 32 + 255) / 256, 256, 0, st>>>(q, dpad, nq, P, w.thr, w.cand_count, cap, keys_out, xn_max_bits, eps_rel,
+                                                          certify_slack_rel(dpad), w.flags);
     KRAG_CUDA(cudaGetLastError());
     count_launch();
 }
@@ -914,24 +936,76 @@ bool launch_dense_tc_host(const DeviceInfo& di, const HostRowsView& hr, int64_t 
     return true;
 }
 
-bool dense_tc_debug_dump(const DeviceInfo& di, const float* X, bool split, int64_t n_rows, int dpad, const float* xnorm,
-                         const float* q, int nq, float* dump_out, int64_t* S_out, int* nq_pad_out, cudaStream_t st)
+size_t dense_tc_debug_carve(TcDebugWs* w, unsigned char* base, int64_t n_rows, int dpad, int nq, int cap, int64_t* S_out,
+                            int* nq_pad_out)
 {
-    if (!dense_tc_supported(di, dpad) || nq > 256) return false;
     const int NQ = nq <= 64 ? 64 : (nq <= 128 ? 128 : 256);
-    const int64_t n_tiles = (n_rows + TC_TILE_M - 1) / TC_TILE_M;
-    const int64_t S = n_tiles * TC_TILE_M;
+    const int64_t S = (n_rows + TC_TILE_M - 1) / TC_TILE_M * TC_TILE_M;
     *S_out = S;
     *nq_pad_out = NQ;
-    if (dump_out == nullptr) return true;   // size query
+    size_t o = 0;
+    auto take = [&](size_t bytes) { size_t at = o; o = (o + bytes + 255) & ~(size_t)255; return base ? base + at : nullptr; };
+    TcDebugWs t{};
+    t.q_bf16 = (uint16_t*)take((size_t)NQ * dpad * 2);
+    if (cap == 0) {
+        t.dump = (float*)take((size_t)NQ * S * 4);
+    } else {
+        t.thr = (float*)take((size_t)NQ * 4);
+        t.cand_count = (uint32_t*)take((size_t)NQ * 4);
+        t.cand_rows = (uint32_t*)take((size_t)NQ * cap * 4);
+    }
+    if (w) *w = t;
+    return o;
+}
+
+template <int NQ, int MODE>
+static void tc_debug_launch(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensorMap& tmQ, int64_t n_rows, int dpad,
+                            int piece_step, const float* xnorm, const uint32_t* alive, const TcDebugWs& w, int cap, cudaStream_t st)
+{
+    const int64_t n_tiles = (n_rows + TC_TILE_M - 1) / TC_TILE_M;
+    if (cap == 0)   // as the host-rows sample pass, but over every tile and every row (dump_min = 0)
+        tc_launch<NQ, MODE, true>(di, tmX, tmQ, n_rows, dpad, piece_step, n_tiles, 1, xnorm, nullptr, nullptr, nullptr, nullptr, 0,
+                                  w.dump, n_tiles * TC_TILE_M, 0, st);
+    else            // the main pass of tc_pass
+        tc_launch<NQ, MODE, false>(di, tmX, tmQ, n_rows, dpad, piece_step, n_tiles, 1, xnorm, alive, w.thr, w.cand_count,
+                                   w.cand_rows, cap, nullptr, 0, 0, st);
+}
+
+template <int NQ>
+static bool tc_debug_pass(const DeviceInfo& di, int pass, const float* X, const uint16_t* Xh, bool split, int64_t n_rows, int dpad,
+                          const float* xnorm, const uint32_t* alive, const float* q, int nq, const TcDebugWs& w, int cap, cudaStream_t st)
+{
     CUtensorMap tmX, tmQ;
-    if (!(split ? make_map_pieces(&tmX, X, n_rows, dpad, true) : make_map(&tmX, X, n_rows, dpad, TC_TILE_M)) || !make_map(&tmQ, q, nq, dpad, NQ))
-        return false;
-#define KRAG_TC_DUMP(N, MODE)                                                                                              \
-    tc_launch<N, MODE, true>(di, tmX, tmQ, n_rows, dpad, 2, n_tiles, 1, xnorm, nullptr, nullptr, nullptr, nullptr, 0, dump_out, S, 0, st)
-    if (split) { if (NQ == 64) KRAG_TC_DUMP(64, TC_TF32S); else if (NQ == 128) KRAG_TC_DUMP(128, TC_TF32S); else KRAG_TC_DUMP(256, TC_TF32S); }
-    else { if (NQ == 64) KRAG_TC_DUMP(64, TC_TF32); else if (NQ == 128) KRAG_TC_DUMP(128, TC_TF32); else KRAG_TC_DUMP(256, TC_TF32); }
-#undef KRAG_TC_DUMP
+    if (pass == 0) {   // TF32: fp32 queries straight from the caller's rows
+        if (!(split ? make_map_pieces(&tmX, X, n_rows, dpad, true) : make_map(&tmX, X, n_rows, dpad, TC_TILE_M)) ||
+            !make_map(&tmQ, q, nq, dpad, NQ))
+            return false;
+        if (split) tc_debug_launch<NQ, TC_TF32S>(di, tmX, tmQ, n_rows, dpad, 2, xnorm, alive, w, cap, st);
+        else tc_debug_launch<NQ, TC_TF32>(di, tmX, tmQ, n_rows, dpad, 1, xnorm, alive, w, cap, st);
+        return true;
+    }
+    // bf16: the queries converted as tc_pass converts them for the same rows
+    if (pass == 1) launch_bf16_split_order(q, w.q_bf16, (int64_t)nq * dpad, st);
+    else launch_f32_to_bf16(q, w.q_bf16, (int64_t)nq * dpad, st);
+    if (!make_map(&tmQ, (const void*)w.q_bf16, nq, dpad, NQ, true)) return false;
+    if (!(pass == 1 ? make_map_pieces(&tmX, X, n_rows, dpad, true) : make_map_pieces(&tmX, Xh, n_rows, dpad, false))) return false;
+    tc_debug_launch<NQ, TC_BF16>(di, tmX, tmQ, n_rows, dpad, tc_bf16_piece_step(pass == 1), xnorm, alive, w, cap, st);
+    return true;
+}
+
+bool dense_tc_debug_pass(const DeviceInfo& di, int pass, const float* X, const uint16_t* Xh, bool split, int64_t n_rows, int dpad,
+                         const float* xnorm, const uint32_t* alive, const float* q, int nq, const TcDebugWs& w, int cap,
+                         cudaStream_t st)
+{
+    if (!dense_tc_supported(di, dpad) || nq < 1 || nq > 256 || n_rows < 1 || n_rows >= (1ll << 31)) return false;
+    if (pass < 0 || pass > 3 || (pass == 1 && !split) || (pass >= 2 && (Xh == nullptr || dpad % (2 * TC_KBLOCK) != 0))) return false;
+    const int NQ = nq <= 64 ? 64 : (nq <= 128 ? 128 : 256);
+    if (cap > 0) KRAG_CUDA(cudaMemsetAsync(w.cand_count, 0, (size_t)NQ * 4, st));
+    bool ok;
+    if (NQ == 64) ok = tc_debug_pass<64>(di, pass, X, Xh, split, n_rows, dpad, xnorm, alive, q, nq, w, cap, st);
+    else if (NQ == 128) ok = tc_debug_pass<128>(di, pass, X, Xh, split, n_rows, dpad, xnorm, alive, q, nq, w, cap, st);
+    else ok = tc_debug_pass<256>(di, pass, X, Xh, split, n_rows, dpad, xnorm, alive, q, nq, w, cap, st);
+    if (!ok) return false;
     KRAG_CUDA(cudaGetLastError());
     count_launch();
     return true;

@@ -264,9 +264,17 @@ bool launch_dense_tc(const DeviceInfo& di, const float* X, int64_t n_rows, int d
                      bool split /* X holds split rows (split_rows.cuh) */);
 void launch_f32_to_bf16(const float* in, uint16_t* out, int64_t n_elems, cudaStream_t st);
 int64_t dense_tc_fallback_queries();   // queries re-run on K1 because the exactness certificate failed
-// diagnostics: a[j][r] = |x_r|^2 - 2 x_r.q_j for ALL rows through the tensor-core kernel (tests only)
-bool dense_tc_debug_dump(const DeviceInfo& di, const float* X, bool split, int64_t n_rows, int dpad, const float* xnorm,
-                         const float* q, int nq, float* dump_out /*[NQ_pad][S]*/, int64_t* S_out, int* nq_pad_out,
+// diagnostics (tests only): one prune pass of K2 over every tile of the rows, in the production instantiation.
+// pass (KRAG_TC_PASS_*): 0 the TF32 pass (TC_TF32S on split rows, TC_TF32 on plain rows), 1 the bf16 pass on the high halves
+// of split rows, 2 the bf16 pass on the shadow Xh, 3 the bf16 pass on a host-rows index's device copy Xh.
+// cap == 0: the DUMP instantiation writes a[j][r] = |x_r|^2 - 2 x_r.q_j for ALL rows and NQ_pad query columns to w.dump
+// [NQ_pad][S] (rows past n_rows: +inf); cap > 0: the main pass appends the alive rows with a < w.thr[j] to w.cand_rows
+// [NQ_pad][cap] and counts them in w.cand_count [NQ_pad].  w is carved by dense_tc_debug_carve (base == nullptr: size only).
+struct TcDebugWs { uint16_t* q_bf16; float* dump; float* thr; uint32_t* cand_count; uint32_t* cand_rows; };
+size_t dense_tc_debug_carve(TcDebugWs* w, unsigned char* base, int64_t n_rows, int dpad, int nq, int cap, int64_t* S_out,
+                            int* nq_pad_out);
+bool dense_tc_debug_pass(const DeviceInfo& di, int pass, const float* X, const uint16_t* Xh, bool split, int64_t n_rows, int dpad,
+                         const float* xnorm, const uint32_t* alive, const float* q, int nq, const TcDebugWs& w, int cap,
                          cudaStream_t st);
 
 // ---- merge / fuse (merge_fuse.cu)

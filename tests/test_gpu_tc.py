@@ -10,8 +10,8 @@ pytestmark = pytest.mark.gpu
 
 @pytest.fixture(scope="module", params=["cvt", "tf32"])
 def ctx_tc(request):
-    """K2 forced for every batch size: the default prune pass (fp32 rows rounded to bf16 on chip, bf16 wgmma) and
-    the direct TF32 pass (tf32 wgmma)"""
+    """K2 forced for every batch size: the default prune pass ("cvt": bf16 wgmma on the high halves of split rows, TF32
+    on rows with dpad % 64 == 32) and the TF32 pass (tf32 wgmma)"""
     from kaito_b200 import _native
     c = _native.Context(device_id=0, dense_mode=_native.DENSE_TC if request.param == "cvt" else _native.DENSE_TC_TF32)
     yield c
@@ -19,20 +19,30 @@ def ctx_tc(request):
 
 
 @pytest.mark.parametrize("n,d,nq", [(128, 32, 3), (1000, 64, 5), (777, 768, 100), (4096, 384, 256), (130, 1024, 64)])
-def test_tc_raw_output_matches_numpy(ctx_tc, oracle, n, d, nq):
+def test_tc_raw_output_matches_numpy(ctx_tc, oracle, request, n, d, nq):
+    from kaito_b200 import _native
+    from tests import test_gpu_tc_passes as passes
     x = oracle.synth_dense(n, d, seed=n + d)
     q = oracle.synth_queries(x, nq, seed=n)
     ix = ctx_tc.create_index(f"tcraw_{n}_{d}", d)
     try:
         ix.add(np.arange(n, dtype=np.uint64), x)
-        a = ix.debug_tc_dump(q)                       # [nq_pad, S]
-        ref = (x.astype(np.float64) ** 2).sum(1)[None, :] - 2.0 * (q.astype(np.float64) @ x.astype(np.float64).T)
+        # the pass the search runs: the default one dumps the bf16 pass on split rows, the TF32 mode the TF32 pass
+        split = ix.stats().dim_padded % 64 == 0
+        tc_pass = _native.TC_PASS_BF16_SPLIT if request.node.callspec.params["ctx_tc"] == "cvt" and split else _native.TC_PASS_TF32
+        a = ix.debug_tc_dump_pass(q, tc_pass)         # [nq_pad, S]
+        xo, qo = passes.operands(x, q, tc_pass, split)
+        xn = (x.astype(np.float64) ** 2).sum(1)
+        ref = xn[None, :] - 2.0 * (qo.astype(np.float64) @ xo.astype(np.float64).T)
         got = a[:nq, :n].astype(np.float64)
         err = np.abs(got - ref)
-        assert err.max() < 5e-3, err.max()            # worst-case TF32 bound is 2 * 2^-9 for unit vectors
-        assert err.mean() < 3e-4, err.mean()
-        assert np.isinf(a[:nq, n:]).all()             # rows past the end never qualify
-        assert np.allclose(a[nq:, :n], (x.astype(np.float64) ** 2).sum(1)[None, :], atol=1e-5)  # zero-filled queries
+        # fp32 accumulation over k K steps (one ulp of the running magnitude each), |x|^2 and the epilogue's rounding
+        absref = np.abs(qo.astype(np.float64)) @ np.abs(xo.astype(np.float64)).T
+        k = passes.k_steps(d, tc_pass)
+        bound = 2.0 * k * 2.0 ** -23 * absref + (d // 128 + 10) * 2.0 ** -24 * xn[None, :] + 2.0 ** -24 * np.abs(got)
+        assert (err <= bound).all(), (err / bound).max()
+        assert np.isposinf(a[:nq, n:]).all()          # rows past the end never qualify
+        assert np.allclose(a[nq:, :n], xn[None, :], rtol=(d // 128 + 10) * 2.0 ** -24, atol=0)   # zero-filled queries
     finally:
         ix.drop()
 
