@@ -294,7 +294,14 @@ int32_t krag_p2p_destroy(krag_p2p* p);
 /* replaces: LocalHuggingFaceEmbedding (embedding/huggingface_local_embedding.py:34-53) -> sentence-
  * transformers BertModel forward, CLS or mean pooling, L2 normalisation.  Tokenisation (WordPiece) stays in
  * the host.  Weights are loaded by their Hugging Face BertModel names ("embeddings.word_embeddings.weight",
- * "encoder.layer.0.attention.self.query.weight", ...), fp32, row-major as torch stores them. */
+ * "encoder.layer.0.attention.self.query.weight", ...), fp32, row-major as torch stores them.
+ * MPNet (all-mpnet-base-v2, multi-qa-mpnet-*): an embedder loaded with "encoder.relative_attention_bias.weight"
+ * [32 buckets, heads] (transformers MPNetModel's name) is an MPNet encoder: every attention score of head h gets
+ * weight[bucket][h], bucket = MPNetEncoder.relative_position_bucket(key - query, 32 buckets, max distance 128) (see
+ * krag_debug_relative_bucket).  The host loads the other MPNet tensors under the BERT names (attention.attn.q -> .self.query,
+ * .k -> .self.key, .v -> .self.value, .o -> .output.dense, attention.LayerNorm -> attention.output.LayerNorm), a zero
+ * token-type table with type_vocab = 1, and sets the position offset to 2.  finalize: KRAG_E_INVALID, naming the tensor,
+ * when it does not hold 32 * heads elements. */
 typedef struct krag_embedder krag_embedder;
 typedef struct krag_bert_config {
     int32_t layers, hidden, heads, intermediate, vocab, max_position, type_vocab;
@@ -336,6 +343,10 @@ int32_t krag_embedder_set_position_offset(krag_embedder* e, int32_t off);
 /* Under CLS pooling the last layer's O projection, FFN and LayerNorms run on the [CLS] rows only (on = 1, the default).
  * on = 0 runs them over every token; the embeddings are the same bits either way.  Test hook. */
 int32_t krag_debug_embedder_cls_rows(krag_embedder* e, int32_t on);
+/* The relative-position bucket an MPNet embedder's attention applies at rel = key position - query position: transformers'
+ * MPNetEncoder.relative_position_bucket with 32 buckets and max distance 128 (the distance is clamped to [-128, 128] first,
+ * which changes no bucket).  Host-only: needs no device.  Test hook. */
+int32_t krag_debug_relative_bucket(int32_t rel);
 /* Cross-encoder reranking (BertForSequenceClassification with one label).  The embedder must have been loaded with the
  * head as well: "pooler.dense.weight" [hidden, hidden], "pooler.dense.bias", "classifier.weight" [1, hidden] and
  * "classifier.bias" [1].  Query i owns pairs pair_offsets[i] .. pair_offsets[i+1] (0 to 300 of them); pair p is the packed
@@ -362,10 +373,14 @@ int32_t krag_embedder_destroy(krag_embedder* e);
  *   Writes the stems separated by '\n' into out (if *out_len <= cap) and always reports the needed length and the token count.
  * krag_wordpiece_*: BertTokenizer (uncased) of the bge models (huggingface_local_embedding.py:34-53): BasicTokenizer +
  *   greedy longest-match WordPiece; vocab = the lines of vocab.txt joined by '\n'; encode_batch writes, per text,
- *   [CLS] ids[: max_len - 2] [SEP] into out_ids[i * max_len ...] and its length into out_n[i] (texts are threaded). */
+ *   [CLS] ids[: max_len - 2] [SEP] (or the create_specials tokens) into out_ids[i * max_len ...] and its length into out_n[i] (texts are threaded). */
 typedef struct krag_wordpiece krag_wordpiece;
 int32_t krag_text_analyze(const char* text, int64_t len, char* out, int64_t cap, int64_t* out_len, int32_t* n_terms);
 int32_t krag_wordpiece_create(const char* vocab, int64_t len, int32_t lower_case, krag_wordpiece** out);
+/* the same with the unknown / first / last special tokens named (krag_wordpiece_create: "[UNK]", "[CLS]", "[SEP]"; MPNet:
+ * "[UNK]", "<s>", "</s>"); each must be a line of vocab, else KRAG_E_INVALID.  Specials typed in a text are text. */
+int32_t krag_wordpiece_create_specials(const char* vocab, int64_t len, int32_t lower_case, const char* unk_token,
+                                       const char* cls_token, const char* sep_token, krag_wordpiece** out);
 int32_t krag_wordpiece_encode_batch(const krag_wordpiece* w, int64_t n, const char* texts, const int64_t* offsets /*[n+1]*/,
                                     int32_t max_len, int32_t* out_ids /*[n * max_len]*/, int32_t* out_n /*[n]*/);
 int32_t krag_wordpiece_destroy(krag_wordpiece* w);

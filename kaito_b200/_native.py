@@ -42,7 +42,8 @@ SYMBOLS = [
     "krag_dev_redeal_pack", "krag_dev_redeal_unpack", "krag_redeal_finish", "krag_redeal_abort", "krag_embedder_set_pooling",
     "krag_debug_embedder_cls_rows", "krag_rerank", "krag_embedder_set_precision", "krag_debug_gemm_f16",
     "krag_embedder_set_position_offset", "krag_text_unigram_create", "krag_text_unigram_encode_batch",
-    "krag_text_unigram_destroy", "krag_debug_tc_dump_pass", "krag_debug_tc_prune",
+    "krag_text_unigram_destroy", "krag_debug_tc_dump_pass", "krag_debug_tc_prune", "krag_debug_relative_bucket",
+    "krag_wordpiece_create_specials",
 ]
 # krag_debug_tc_dump_pass / krag_debug_tc_prune: the prune pass to run (KRAG_TC_PASS_*)
 TC_PASS_TF32, TC_PASS_BF16_SPLIT, TC_PASS_BF16_SHADOW, TC_PASS_BF16_HOST = 0, 1, 2, 3
@@ -147,6 +148,8 @@ def load() -> C.CDLL:
     L.krag_index_set_dense_mode.argtypes = [vp, i32, i32]
     L.krag_text_analyze.argtypes = [C.c_char_p, i64, vp, i64, C.POINTER(i64), C.POINTER(i32)]
     L.krag_wordpiece_create.argtypes = [C.c_char_p, i64, i32, C.POINTER(vp)]
+    L.krag_wordpiece_create_specials.argtypes = [C.c_char_p, i64, i32, C.c_char_p, C.c_char_p, C.c_char_p, C.POINTER(vp)]
+    L.krag_debug_relative_bucket.argtypes = [i32]
     L.krag_wordpiece_encode_batch.argtypes = [vp, i64, C.c_char_p, vp, i32, vp, vp]
     L.krag_wordpiece_destroy.argtypes = [vp]
     L.krag_text_unigram_create.argtypes = [C.c_char_p, vp, vp, i64, i32, C.c_char_p, i64, i32, C.c_char_p, vp, vp, vp, i32,
@@ -387,6 +390,11 @@ class Embedder:
         if self._h:
             check(self._L.krag_embedder_destroy(self._h))
             self._h = None
+
+
+def debug_relative_bucket(rel: int) -> int:
+    """the MPNet relative-position bucket K5's attention applies at rel = key - query (krag_debug_relative_bucket; no GPU)"""
+    return int(load().krag_debug_relative_bucket(rel))
 
 
 def debug_gemm_tf32(ctx: "Context", A, B, bias, residual=None, gelu=False, tile_n=0) -> np.ndarray:

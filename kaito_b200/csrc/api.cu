@@ -1821,6 +1821,7 @@ int32_t krag_embedder_set_position_offset(krag_embedder* h, int32_t off)
         embedder_set_position_offset(h->e, off);
     });
 }
+int32_t krag_debug_relative_bucket(int32_t rel) { return relative_bucket(rel); }
 int32_t krag_debug_embedder_cls_rows(krag_embedder* h, int32_t on)
 {
     return guarded([&] {

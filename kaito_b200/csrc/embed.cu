@@ -1,4 +1,5 @@
-// embed.cu -- K5: BERT-family (bge-small / bge-base / bge-large) encoder forward on the GPU.
+// embed.cu -- K5: BERT-family (bge-small / bge-base / bge-large, all-MiniLM, e5, gte; MPNet with its relative-position attention
+// bias: all-mpnet-base-v2) encoder forward on the GPU.
 //
 // Replaces the torch / sentence-transformers forward behind
 // presets/ragengine/embedding/huggingface_local_embedding.py:34-53 (LlamaIndex HuggingFaceEmbedding ->
@@ -16,6 +17,7 @@
 #include <cuda_fp16.h>
 #include <math_constants.h>
 
+#include <cmath>
 #include <cstring>
 #include <map>
 #include <memory>
@@ -481,16 +483,21 @@ __device__ __forceinline__ void am_commit() { asm volatile("cp.async.commit_grou
 template <int N> __device__ __forceinline__ void am_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 // PLANES == 1 (KRAG_PRECISION_FP16): only the hi planes are staged and every product is one MMA on them; same key blocking,
 // same fp32 softmax.
+//
+// REL (MPNet): every score gets its head's learned bias at the key - query distance, clamped to [-REL_MAX, REL_MAX]:
+// rel_tab [heads][REL_TAB] holds it at index distance + REL_MAX (embedder_finalize builds it from the 32-bucket table).  The
+// head's row is staged after the K / V stages in shared memory.  REL = false ignores rel_tab and is the BERT kernel.
+constexpr int REL_MAX = 128, REL_TAB = 2 * REL_MAX + 1;
 template <int DH, int WARPS, int KB, int STAGES, int PLANES> struct AmCfg {
     static constexpr int LDH = DH + 8;                                   // row stride in halfs (16 bytes of padding)
     static constexpr int Q_HALFS = PLANES * 16 * WARPS * LDH;            // hi | lo
     static constexpr int KV_HALFS = PLANES * KB * LDH;                   // hi | lo of one operand of one stage
     static constexpr size_t SMEM = 2 * (size_t)(Q_HALFS + 2 * STAGES * KV_HALFS);
 };
-template <int DH, int WARPS, int KB, int STAGES, int PLANES>
+template <int DH, int WARPS, int KB, int STAGES, int PLANES, bool REL>
 __global__ void __launch_bounds__(WARPS * 32)
 attention_mma_kernel(const uint16_t* __restrict__ qkv_hi, const uint16_t* __restrict__ qkv_lo, const int32_t* __restrict__ seq_off,
-                     uint16_t* __restrict__ out_hi, uint16_t* __restrict__ out_lo, int d, int heads)
+                     uint16_t* __restrict__ out_hi, uint16_t* __restrict__ out_lo, int d, int heads, const float* __restrict__ rel_tab)
 {
     using Cfg = AmCfg<DH, WARPS, KB, STAGES, PLANES>;
     constexpr int LDH = Cfg::LDH, QROWS = 16 * WARPS, THREADS = WARPS * 32, CH = DH / 8 /* 16-byte chunks per row */;
@@ -498,6 +505,7 @@ attention_mma_kernel(const uint16_t* __restrict__ qkv_hi, const uint16_t* __rest
     uint16_t* sQ = am_sm;                                  // [2][QROWS][LDH]
     uint16_t* sK = sQ + Cfg::Q_HALFS;                      // [STAGES][2][KB][LDH]
     uint16_t* sV = sK + STAGES * Cfg::KV_HALFS;            // [STAGES][2][KB][LDH]
+    float* sRel = reinterpret_cast<float*>(sV + STAGES * Cfg::KV_HALFS);   // REL: [REL_TAB]
     pdl_launch_dependents();
     pdl_wait();
     const int b = blockIdx.z, h = blockIdx.y;
@@ -522,6 +530,9 @@ attention_mma_kernel(const uint16_t* __restrict__ qkv_hi, const uint16_t* __rest
     };
     stage_rows(sQ, QROWS, r0, 0);
     stage_kv(0, 0);
+    if constexpr (REL) {                                   // read after the first key block's __syncthreads
+        for (int i = tid; i < REL_TAB; i += THREADS) sRel[i] = rel_tab[(size_t)h * REL_TAB + i];
+    }
     const int nkb = (len + KB - 1) / KB;
     uint32_t qh[DH / 16][4], ql[DH / 16][4];
     float om[DH / 8][4], oc[PLANES == 2 ? DH / 8 : 1][4];  // output accumulators: main and correction products
@@ -575,13 +586,20 @@ attention_mma_kernel(const uint16_t* __restrict__ qkv_hi, const uint16_t* __rest
         }
         // ---- online softmax (fp32): thread (g, t) holds columns 2t, 2t+1 of every 8-key tile for rows g (e = 0, 1) and g + 8 (e = 2, 3)
         const int k0 = kb * KB;
+        const int dist0 = k0 + 2 * t - (r0 + warp * 16 + g);     // REL: key - query of element (j, e) is dist0 + 8j + (e & 1) - 8(e >> 1)
         float mx[2] = {-CUDART_INF_F, -CUDART_INF_F};
 #pragma unroll
         for (int j = 0; j < KB / 8; ++j)
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
                 const bool in = k0 + j * 8 + 2 * t + (e & 1) < len;
-                s[j][e] = in ? s[j][e] * scale : -CUDART_INF_F;
+                if constexpr (REL) {                       // transformers' order: scale, then + position bias, then the mask
+                    const int c = dist0 + j * 8 + (e & 1) - 8 * (e >> 1);
+                    const float bias = sRel[min(max(c, -REL_MAX), REL_MAX) + REL_MAX];
+                    s[j][e] = in ? fmaf(s[j][e], scale, bias) : -CUDART_INF_F;
+                } else {
+                    s[j][e] = in ? s[j][e] * scale : -CUDART_INF_F;
+                }
                 mx[e >> 1] = fmaxf(mx[e >> 1], s[j][e]);
             }
         float corr[2];
@@ -835,30 +853,39 @@ static void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
     count_launch();
 }
 
-template <int DH, int WARPS, int KB, int STAGES, int PLANES>
+template <int DH, int WARPS, int KB, int STAGES, int PLANES, bool REL>
 static void launch_attention_mma(const uint16_t* q_hi, const uint16_t* q_lo, const int32_t* seq_off, uint16_t* out_hi, uint16_t* out_lo, int d,
-                                 int heads, int batch, int max_len, bool first_rows, cudaStream_t st)
+                                 int heads, int batch, int max_len, bool first_rows, const float* rel_tab, cudaStream_t st)
 {
     using Cfg = AmCfg<DH, WARPS, KB, STAGES, PLANES>;
+    constexpr size_t smem = Cfg::SMEM + (REL ? sizeof(float) * REL_TAB : 0);
     static bool attr_set = false;
     if (!attr_set) {
-        KRAG_CUDA(cudaFuncSetAttribute(attention_mma_kernel<DH, WARPS, KB, STAGES, PLANES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM));
+        KRAG_CUDA(cudaFuncSetAttribute(attention_mma_kernel<DH, WARPS, KB, STAGES, PLANES, REL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set = true;
     }
     const unsigned q_blocks = first_rows ? 1u : (unsigned)((max_len + 16 * WARPS - 1) / (16 * WARPS));
-    launch_pdl(attention_mma_kernel<DH, WARPS, KB, STAGES, PLANES>, dim3(q_blocks, (unsigned)heads, (unsigned)batch),
-               dim3(WARPS * 32), Cfg::SMEM, st, q_hi, q_lo, seq_off, out_hi, out_lo, d, heads);
+    launch_pdl(attention_mma_kernel<DH, WARPS, KB, STAGES, PLANES, REL>, dim3(q_blocks, (unsigned)heads, (unsigned)batch),
+               dim3(WARPS * 32), smem, st, q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, rel_tab);
+}
+template <int DH, int PLANES, bool REL>
+static void attention_mma_blocks(const uint16_t* q_hi, const uint16_t* q_lo, const int32_t* seq_off, uint16_t* out_hi, uint16_t* out_lo, int d,
+                                 int heads, int batch, int max_len, bool first_rows, const float* rel_tab, cudaStream_t st)
+{
+    if (max_len <= 32) launch_attention_mma<DH, 2, 32, 1, PLANES, REL>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, rel_tab, st);
+    else if (max_len <= 64) launch_attention_mma<DH, 4, 64, 1, PLANES, REL>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, rel_tab, st);
+    else launch_attention_mma<DH, 4, 64, 2, PLANES, REL>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, rel_tab, st);
 }
 // queries (<= 32 tokens): 2 warps, one key block; <= 64: 4 warps, one block; chunks: 4 warps, 64-key blocks, double-buffered.
 // first_rows: only the first block of query rows of every sequence (the [CLS] row among them); a query row's result does
-// not depend on which other rows run, and the key blocking follows max_len either way.  PLANES == 1: q_lo / out_lo are not used
+// not depend on which other rows run, and the key blocking follows max_len either way.  PLANES == 1: q_lo / out_lo are not used.
+// rel_tab: the MPNet relative-position bias table (REL instantiations), null for BERT.
 template <int DH, int PLANES>
 static void attention_mma(const uint16_t* q_hi, const uint16_t* q_lo, const int32_t* seq_off, uint16_t* out_hi, uint16_t* out_lo, int d, int heads,
-                          int batch, int max_len, bool first_rows, cudaStream_t st)
+                          int batch, int max_len, bool first_rows, const float* rel_tab, cudaStream_t st)
 {
-    if (max_len <= 32) launch_attention_mma<DH, 2, 32, 1, PLANES>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, st);
-    else if (max_len <= 64) launch_attention_mma<DH, 4, 64, 1, PLANES>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, st);
-    else launch_attention_mma<DH, 4, 64, 2, PLANES>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, st);
+    if (rel_tab) attention_mma_blocks<DH, PLANES, true>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, rel_tab, st);
+    else attention_mma_blocks<DH, PLANES, false>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, nullptr, st);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -1021,6 +1048,7 @@ struct Embedder {
     std::vector<SplitMat> s_qkv, s_o, s_f1, s_f2;
     std::vector<DevArray<uint16_t>> planes;     // the buffers all weight planes live in
     SplitMat s_pool{nullptr, nullptr};          // pooler.dense.weight (cross-encoders: finalize found the classifier head)
+    DevArray<float> rel_tab;                    // MPNet: [heads][REL_TAB] relative-position bias by distance (finalize); else null
     bool has_head = false;
     bool finalized = false;
     cudaStream_t st = nullptr;
@@ -1107,15 +1135,33 @@ static SplitMat emb_split_weight(Embedder* e, const float* w, size_t n)
     return m;
 }
 
+// MPNetEncoder.relative_position_bucket(rel, num_buckets = 32, max_distance = 128): future keys (rel > 0) take 16 + b(rel),
+// the others b(-rel); b(n) = n below 8, else min(15, 8 + floor(ln(n / 8) / ln 16 * 8)).  b saturates from n = 91 on, so the
+// kernel's clamp of the distance to +-REL_MAX changes no bucket at any sequence length.
+int relative_bucket(int rel)
+{
+    rel = rel < -REL_MAX ? -REL_MAX : (rel > REL_MAX ? REL_MAX : rel);
+    const int base = rel > 0 ? 16 : 0, n = rel > 0 ? rel : -rel;
+    if (n < 8) return base + n;
+    const int v = 8 + (int)(std::log(n / 8.0) / std::log(16.0) * 8.0);
+    return base + (v < 15 ? v : 15);
+}
+static const char* const REL_BIAS = "encoder.relative_attention_bias.weight";   // MPNet: [32 buckets][heads]
+constexpr int REL_BUCKETS = 32;
+
 void embedder_finalize(Embedder* e)
 {
     const int d = e->cfg.hidden, inter = e->cfg.inter;
     e->finalized = false;
     e->bqkv.clear(); e->planes.clear(); e->s_qkv.clear(); e->s_o.clear(); e->s_f1.clear(); e->s_f2.clear();
     e->s_pool = SplitMat{nullptr, nullptr}; e->has_head = false;
+    e->rel_tab.release();
     e->drop_graphs(); e->seen.clear();   // captured weight pointers are about to change
     const BertConfig& c = e->cfg;
     // every size first: a refused state leaves no half-built planes behind
+    const auto rit = e->t.find(REL_BIAS);
+    const bool rel = rit != e->t.end() && rit->second.p;   // an MPNet encoder: loaded with the relative-position bias
+    if (rel) emb_get(e, REL_BIAS, (int64_t)REL_BUCKETS * c.heads);
     emb_get(e, "embeddings.word_embeddings.weight", (int64_t)c.vocab * d);
     emb_get(e, "embeddings.position_embeddings.weight", (int64_t)c.max_pos * d);
     emb_get(e, "embeddings.token_type_embeddings.weight", (int64_t)c.type_vocab * d);
@@ -1161,6 +1207,16 @@ void embedder_finalize(Embedder* e)
     if (n_head == 4) {
         e->s_pool = emb_split_weight(e, emb_get(e, "pooler.dense.weight", (int64_t)d * d), (size_t)d * d);
         e->has_head = true;
+    }
+    if (rel) {
+        // the bias by distance, [heads][REL_TAB]: the kernel looks a score's bias up without computing its bucket
+        std::vector<float> w((size_t)REL_BUCKETS * c.heads), tab((size_t)c.heads * REL_TAB);
+        KRAG_CUDA(cudaMemcpy(w.data(), emb_get(e, REL_BIAS, (int64_t)w.size()), sizeof(float) * w.size(), cudaMemcpyDeviceToHost));
+        for (int h = 0; h < c.heads; ++h)
+            for (int dist = -REL_MAX; dist <= REL_MAX; ++dist)
+                tab[(size_t)h * REL_TAB + dist + REL_MAX] = w[(size_t)relative_bucket(dist) * c.heads + h];
+        e->rel_tab.alloc((int64_t)tab.size());
+        KRAG_CUDA(cudaMemcpy(e->rel_tab.p, tab.data(), sizeof(float) * tab.size(), cudaMemcpyHostToDevice));
     }
     KRAG_CUDA(cudaStreamSynchronize(e->st));
     wtmp.release();
@@ -1304,11 +1360,12 @@ static bool encoder_forward(Embedder* e, int batch, const int32_t* tok_ids, cons
         const bool last_cls = cls_rows && l == c.layers - 1;
         launch_linear(e->di, xs, e->s_qkv[L], n_tok, 3 * d, d, e->bqkv[L].p, nullptr, false, nullptr, q_hi, q_lo, nullptr, nullptr, 0.f,
                       nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st, nullptr, planes);
+        const float* rel = e->rel_tab.p;                  // null: BERT
         if (planes == 1) {
-            if (dh == 64) attention_mma<64, 1>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, st);
-            else attention_mma<32, 1>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, st);
-        } else if (dh == 64) attention_mma<64, 2>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, st);
-        else attention_mma<32, 2>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, st);
+            if (dh == 64) attention_mma<64, 1>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, rel, st);
+            else attention_mma<32, 1>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, rel, st);
+        } else if (dh == 64) attention_mma<64, 2>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, rel, st);
+        else attention_mma<32, 2>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, rel, st);
         if (last_cls) {
             const SplitMat ccs{e->ccs.p, lo_of(e->ccs.p, (size_t)batch * d)}, cxs{e->cxs.p, lo_of(e->cxs.p, (size_t)batch * d)},
                            cfs{e->cfs.p, lo_of(e->cfs.p, (size_t)batch * c.inter)};

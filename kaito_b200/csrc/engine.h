@@ -479,6 +479,9 @@ enum { EMB_PREC_FP32 = 0, EMB_PREC_FP16 = 1 };   // = KRAG_PRECISION_FP32 / KRAG
 void embedder_set_precision(Embedder* e, int mode);
 // first position row of every sequence (RoBERTa / XLM-R: pad_token_id + 1); token i of a sequence takes row off + i
 void embedder_set_position_offset(Embedder* e, int off);
+// MPNet: the bucket of MPNetEncoder.relative_position_bucket (32 buckets, max distance 128) the attention kernel applies at
+// rel = key - query (the distance clamped to +-128 first); host-only
+int relative_bucket(int rel);
 void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int32_t* tok_offsets, float* out_host,
                       float* out_dev = nullptr, int ld_out = 0, cudaStream_t consumer = nullptr);
 // cross-encoder reranking (classifier head loaded): scores of sentence pairs, top_k per query (see embed.cu)

@@ -492,8 +492,14 @@ int32_t krag_text_analyze(const char* text, int64_t len, char* out, int64_t cap,
 
 int32_t krag_wordpiece_create(const char* vocab, int64_t len, int32_t lower_case, krag_wordpiece** out)
 {
+    return krag_wordpiece_create_specials(vocab, len, lower_case, "[UNK]", "[CLS]", "[SEP]", out);
+}
+
+int32_t krag_wordpiece_create_specials(const char* vocab, int64_t len, int32_t lower_case, const char* unk_token,
+                                       const char* cls_token, const char* sep_token, krag_wordpiece** out)
+{
     return text_guard([&] {
-        if (!vocab || !out || len < 0) throw std::invalid_argument("null argument");
+        if (!vocab || !out || len < 0 || !unk_token || !cls_token || !sep_token) throw std::invalid_argument("null argument");
         krag_wordpiece* w = new krag_wordpiece();
         w->lower_case = lower_case != 0;
         // one token per line, exactly like "\n".join(tokens).split("\n"); a repeated token keeps its LAST id (dict semantics)
@@ -507,7 +513,7 @@ int32_t krag_wordpiece_create(const char* vocab, int64_t len, int32_t lower_case
             p = nl + 1;
         }
         auto need = [&](const char* t) { auto it = w->vocab.find(t); if (it == w->vocab.end()) { delete w; throw std::invalid_argument(t); } return it->second; };
-        w->unk = need("[UNK]"); w->cls = need("[CLS]"); w->sep = need("[SEP]");
+        w->unk = need(unk_token); w->cls = need(cls_token); w->sep = need(sep_token);
         *out = w;
     });
 }

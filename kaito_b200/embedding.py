@@ -72,10 +72,11 @@ def _json(path: str, required: bool = True):
         raise ValueError(f"{path}: unreadable ({e})") from None
 
 
-def check_bert_config(cpath: str, cfg: dict) -> int:
-    """the encoder shapes K5 runs (config.json at cpath, parsed as cfg); returns hidden_size or raises a ValueError naming the
-    file and field (shared by the embedder and cross-encoder snapshot readers)"""
-    for field, want, default in (("model_type", "bert", None), ("position_embedding_type", "absolute", "absolute"),
+def check_bert_config(cpath: str, cfg: dict, model_type: str = "bert") -> int:
+    """the encoder shapes K5 runs (config.json at cpath, parsed as cfg, of a `model_type` encoder: "bert" or "mpnet");
+    returns hidden_size or raises a ValueError naming the file and field (shared by the embedder and cross-encoder snapshot
+    readers)"""
+    for field, want, default in (("model_type", model_type, None), ("position_embedding_type", "absolute", "absolute"),
                                  ("hidden_act", "gelu", "gelu"), ("is_decoder", False, False)):
         if cfg.get(field, default) != want:
             raise ValueError(f"{cpath}: {field} {cfg.get(field, default)!r}: K5 runs {field} {want!r} only")
@@ -91,8 +92,29 @@ def check_bert_config(cpath: str, cfg: dict) -> int:
     return d
 
 
+# transformers MPNetModel names -> the BertModel names K5 loads (encoder.relative_attention_bias.weight keeps its name)
+_MPNET_NAMES = ((".attention.attn.q.", ".attention.self.query."), (".attention.attn.k.", ".attention.self.key."),
+                (".attention.attn.v.", ".attention.self.value."), (".attention.attn.o.", ".attention.output.dense."),
+                (".attention.LayerNorm.", ".attention.output.LayerNorm."))
+MPNET_REL_BIAS = "encoder.relative_attention_bias.weight"
+MPNET_BUCKETS = 32            # transformers' MPNetEncoder computes 32 relative-position buckets whatever the config says
+MPNET_POSITION_OFFSET = 2     # MPNet numbers positions from padding_idx + 1, padding_idx = 1
+
+
+def _k5_name(k: str) -> str:
+    """a checkpoint tensor name without its "bert." / "mpnet." prefix, MPNet names mapped onto BERT's"""
+    for prefix in ("bert.", "mpnet."):
+        if k.startswith(prefix):
+            k = k[len(prefix):]
+            break
+    for a, b in _MPNET_NAMES:
+        k = k.replace(a, b)
+    return k
+
+
 def load_state(model_dir: str) -> dict:
-    """model.safetensors or pytorch_model.bin of a snapshot as numpy fp32 arrays, names without the "bert." prefix"""
+    """model.safetensors or pytorch_model.bin of a snapshot as numpy fp32 arrays, names without the "bert." / "mpnet."
+    prefix; MPNet's attention names are mapped onto BERT's (attention.attn.q -> attention.self.query, ...)"""
     st_path, bin_path = os.path.join(model_dir, "model.safetensors"), os.path.join(model_dir, "pytorch_model.bin")
     if os.path.exists(st_path):
         from safetensors.numpy import load_file
@@ -102,7 +124,21 @@ def load_state(model_dir: str) -> dict:
         state = {k: v.float().numpy() for k, v in torch.load(bin_path, map_location="cpu").items()}
     else:
         raise ValueError(f"{model_dir}: neither model.safetensors nor pytorch_model.bin")
-    return {k[5:] if k.startswith("bert.") else k: v for k, v in state.items()}
+    return {_k5_name(k): v for k, v in state.items()}
+
+
+def _check_mpnet_config(cpath: str, cfg: dict):
+    """what an MPNet config.json must state before anything else of the snapshot is read"""
+    nb = cfg.get("relative_attention_num_buckets")
+    if nb != MPNET_BUCKETS:
+        raise ValueError(f"{cpath}: model_type 'mpnet' with relative_attention_num_buckets {nb!r}: K5 runs MPNet encoders that "
+                         f"state {MPNET_BUCKETS} buckets (transformers always computes {MPNET_BUCKETS})")
+
+
+def _special(tc: dict, field: str, default: str) -> str:
+    """a special token of tokenizer_config.json: a string or an AddedToken dict {"content": ...}"""
+    v = tc.get(field, default)
+    return v.get("content", default) if isinstance(v, dict) else v
 
 
 def read_snapshot_spec(model_dir: str) -> dict:
@@ -112,8 +148,20 @@ def read_snapshot_spec(model_dir: str) -> dict:
       max_length         tokens per sequence incl. [CLS] / [SEP] (sentence_bert_config.json max_seq_length, else
                          min(tokenizer_config.json model_max_length, config.json max_position_embeddings), else 512)
       do_lower_case      tokenizer_config.json do_lower_case (default true)
-      query_instruction  the bge prefix for CLS-pooled snapshots, None for mean-pooled ones [3P-unverified]"""
+      query_instruction  the bge prefix for CLS-pooled BERT snapshots, None for mean-pooled and MPNet ones [3P-unverified]
+    and for config.json model_type "mpnet" (all-mpnet-base-v2, multi-qa-mpnet-*) also
+      model_type         "mpnet"
+      position_offset    2 (MPNet's first position row)
+      cls_token, sep_token, unk_token   tokenizer_config.json's specials (default <s>, </s>, [UNK]), each in vocab.txt"""
     join = os.path.join
+    cpath = join(model_dir, "config.json")
+    try:
+        peek = _json(cpath, required=False)
+    except ValueError:
+        peek = None
+    mpnet = isinstance(peek, dict) and peek.get("model_type") == "mpnet"
+    if mpnet:
+        _check_mpnet_config(cpath, peek)
     pooling = "cls"
     mpath = join(model_dir, "modules.json")
     modules = _json(mpath, required=False)
@@ -135,13 +183,14 @@ def read_snapshot_spec(model_dir: str) -> dict:
             raise ValueError(f"{ppath}: include_prompt {pc['include_prompt']!r}: only true (pool over every token) is supported")
         pooling = "cls" if on[0] == "pooling_mode_cls_token" else "mean"
 
-    cpath = join(model_dir, "config.json")
     cfg = _json(cpath)
-    d = check_bert_config(cpath, cfg)
+    d = check_bert_config(cpath, cfg, "mpnet" if mpnet else "bert")
     if modules is not None and pc.get("word_embedding_dimension", d) != d:
         raise ValueError(f"{ppath}: word_embedding_dimension {pc['word_embedding_dimension']} differs from config.json "
                          f"hidden_size {d}")
     max_pos = cfg.get("max_position_embeddings", 512)
+    off = MPNET_POSITION_OFFSET if mpnet else 0
+    max_tok = max_pos - off                  # positions off .. max_pos - 1
 
     tpath = join(model_dir, "tokenizer_config.json")
     tc = _json(tpath, required=False) or {}
@@ -153,24 +202,36 @@ def read_snapshot_spec(model_dir: str) -> dict:
     if sbc.get("max_seq_length") is not None:
         max_length, where = sbc["max_seq_length"], f"{spath}: max_seq_length"
     else:
-        max_length, where = min(tc.get("model_max_length", max_pos), max_pos), f"{tpath}: model_max_length"
-    if not isinstance(max_length, int) or not 2 <= max_length <= max_pos:
-        raise ValueError(f"{where} {max_length!r}: must be an integer in [2, config.json max_position_embeddings {max_pos}]")
-    if not os.path.isfile(join(model_dir, "vocab.txt")):
-        raise ValueError(f"{join(model_dir, 'vocab.txt')}: file missing (K5 takes WordPiece vocabularies)")
-    return {"pooling": pooling, "max_length": max_length, "do_lower_case": bool(do_lower_case),
-            "query_instruction": BGE_QUERY_INSTRUCTION if pooling == "cls" else None}
+        max_length, where = min(tc.get("model_max_length", max_tok), max_tok), f"{tpath}: model_max_length"
+    if not isinstance(max_length, int) or not 2 <= max_length <= max_tok:
+        bound = f"config.json max_position_embeddings {max_pos} - {off}" if off else f"config.json max_position_embeddings {max_pos}"
+        raise ValueError(f"{where} {max_length!r}: must be an integer in [2, {bound}]")
+    vpath = join(model_dir, "vocab.txt")
+    if not os.path.isfile(vpath):
+        raise ValueError(f"{vpath}: file missing (K5 takes WordPiece vocabularies)")
+    if not mpnet:
+        return {"pooling": pooling, "max_length": max_length, "do_lower_case": bool(do_lower_case),
+                "query_instruction": BGE_QUERY_INSTRUCTION if pooling == "cls" else None}
+    specials = {f: _special(tc, f, dv) for f, dv in (("cls_token", "<s>"), ("sep_token", "</s>"), ("unk_token", "[UNK]"))}
+    with open(vpath, encoding="utf-8") as f:
+        vocab = {line.rstrip("\n") for line in f}
+    for field, tok in specials.items():
+        if not isinstance(tok, str) or tok not in vocab:
+            raise ValueError(f"{vpath}: {tpath} {field} {tok!r} is not a token of the vocabulary")
+    return dict({"pooling": pooling, "max_length": max_length, "do_lower_case": bool(do_lower_case), "query_instruction": None,
+                 "model_type": "mpnet", "position_offset": MPNET_POSITION_OFFSET}, **specials)
 
 
 class GpuBertEmbedding(BaseEmbeddingModel):
-    """BERT sentence embedders (bge, all-MiniLM, e5, gte, ...) on the GPU (K5, kaito_b200/csrc/embed.cu): WordPiece on the
+    """BERT and MPNet sentence embedders (bge, all-MiniLM, e5, gte, all-mpnet, ...) on the GPU (K5, kaito_b200/csrc/embed.cu): WordPiece on the
     host, BERT encoder forward + CLS or mean pooling + L2 normalisation in libkaito_rag.  Mirrors
     LocalHuggingFaceEmbedding (embedding/huggingface_local_embedding.py:31-61); from_pretrained reads the pooling, casing
     and length from the snapshot (read_snapshot_spec).  CLS-pooled snapshots' queries get the bge instruction prefix
     LlamaIndex adds for BAAI/bge-* models [3P-unverified]."""
 
     def __init__(self, engine, tokenizer, config: dict, state_dict: dict, query_instruction: str | None = BGE_QUERY_INSTRUCTION,
-                 max_batch_tokens: int = 65536, pooling: str = "cls"):
+                 max_batch_tokens: int = 65536, pooling: str = "cls", position_offset: int = 0):
+        """position_offset: the position row of a sequence's first token (MPNet: 2)"""
         from . import _native
         if pooling not in ("cls", "mean"):
             raise ValueError(f"pooling {pooling!r}: expected 'cls' or 'mean'")
@@ -181,6 +242,8 @@ class GpuBertEmbedding(BaseEmbeddingModel):
                                      config.get("type_vocab_size", 2), config.get("layer_norm_eps", 1e-12))
         if pooling == "mean":
             self._emb.set_pooling(_native.POOL_MEAN)
+        if position_offset:
+            self._emb.set_position_offset(position_offset)
         self._emb.load_state_dict(state_dict)
         import threading
         self._mu = threading.Lock()          # one forward at a time: the embedder owns one set of activation buffers
@@ -189,15 +252,25 @@ class GpuBertEmbedding(BaseEmbeddingModel):
     def from_pretrained(cls, engine, model_dir: str, **kw):
         """model_dir: a Hugging Face / sentence-transformers snapshot (config.json, vocab.txt, model.safetensors or
         pytorch_model.bin; modules.json, the Pooling config, sentence_bert_config.json and tokenizer_config.json when
-        present).  Raises ValueError before any weight is read when the snapshot asks for what K5 does not compute."""
+        present).  Raises ValueError before any weight is read when the snapshot asks for what K5 does not compute.
+        MPNet snapshots: the weights are loaded under K5's BERT names with a zero token-type row (adding +0.0 changes no
+        bit), positions start at row 2 and the tokenizer takes the snapshot's <s> / </s> / [UNK]."""
         from .text import WordPieceTokenizer
         spec = read_snapshot_spec(model_dir)
         cfg = _json(os.path.join(model_dir, "config.json"))
         state = load_state(model_dir)
         kw.setdefault("query_instruction", spec["query_instruction"])
         kw.setdefault("pooling", spec["pooling"])
+        specials = {}
+        if spec.get("model_type") == "mpnet":
+            if MPNET_REL_BIAS not in state:
+                raise ValueError(f"{model_dir}: model_type 'mpnet' without the tensor {MPNET_REL_BIAS}")
+            cfg = dict(cfg, type_vocab_size=1)
+            state = dict(state, **{"embeddings.token_type_embeddings.weight": np.zeros((1, cfg["hidden_size"]), np.float32)})
+            kw.setdefault("position_offset", spec["position_offset"])
+            specials = {k: spec[k] for k in ("cls_token", "sep_token", "unk_token")}
         tok = WordPieceTokenizer.from_file(os.path.join(model_dir, "vocab.txt"), do_lower_case=spec["do_lower_case"],
-                                           max_length=spec["max_length"])
+                                           max_length=spec["max_length"], **specials)
         return cls(engine, tok, cfg, state, **kw)
 
     def get_embedding_dimension(self) -> int:

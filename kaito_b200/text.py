@@ -277,13 +277,15 @@ class WordPieceTokenizer:
     embedder takes: [CLS] tokens [SEP], truncated to max_length.  The reference reaches the same
     tokenizer through sentence-transformers (embedding/huggingface_local_embedding.py:34-53)."""
 
-    def __init__(self, vocab: dict[str, int] | list[str], do_lower_case: bool = True, max_length: int = 512):
+    def __init__(self, vocab: dict[str, int] | list[str], do_lower_case: bool = True, max_length: int = 512,
+                 cls_token: str = "[CLS]", sep_token: str = "[SEP]", unk_token: str = "[UNK]"):
+        """cls_token / sep_token / unk_token: the specials (MPNet: <s>, </s>, [UNK]); a special typed in a text is text"""
         tokens = None
         if not isinstance(vocab, dict):
             tokens = list(vocab)
             vocab = {t: i for i, t in enumerate(tokens)}
         self.vocab, self.lower, self.max_length = vocab, do_lower_case, max_length
-        self.unk, self.cls, self.sep = vocab["[UNK]"], vocab["[CLS]"], vocab["[SEP]"]
+        self.unk, self.cls, self.sep = vocab[unk_token], vocab[cls_token], vocab[sep_token]
         # native encoder (csrc/text_native.cpp) for ASCII text; needs the ordered token list and tokens without newlines
         self._nat = None
         L = _native_lib()
@@ -291,7 +293,8 @@ class WordPieceTokenizer:
             import ctypes as C
             blob = "\n".join(tokens).encode("utf-8")
             h = C.c_void_p()
-            if L.krag_wordpiece_create(blob, len(blob), 1 if do_lower_case else 0, C.byref(h)) == 0:
+            if L.krag_wordpiece_create_specials(blob, len(blob), 1 if do_lower_case else 0, unk_token.encode("utf-8"),
+                                                cls_token.encode("utf-8"), sep_token.encode("utf-8"), C.byref(h)) == 0:
                 self._nat = h
 
     def __del__(self):
