@@ -301,7 +301,19 @@ int32_t krag_p2p_destroy(krag_p2p* p);
  * krag_debug_relative_bucket).  The host loads the other MPNet tensors under the BERT names (attention.attn.q -> .self.query,
  * .k -> .self.key, .v -> .self.value, .o -> .output.dense, attention.LayerNorm -> attention.output.LayerNorm), a zero
  * token-type table with type_vocab = 1, and sets the position offset to 2.  finalize: KRAG_E_INVALID, naming the tensor,
- * when it does not hold 32 * heads elements. */
+ * when it does not hold 32 * heads elements.
+ * nomic-bert (nomic-embed-text-v1 / -v1.5) is a post-LN BERT with two variants, each selectable alone:
+ *  - rotary positions (krag_embedder_set_rotary with base > 0, before finalize): no position table is read (none need be
+ *    loaded); Q and K of token i of a sequence (position off + i) are rotated as transformers' default RoPE does,
+ *    q' = q cos + rotate_half(q) sin, pairing element j < dh/2 of a head with j + dh/2, at the fp32 angle fp32(pos) *
+ *    (1 / base^(2j / dh)) (see krag_debug_rotary_cos_sin).  Sequences may hold max_position - off tokens.
+ *  - a gated FFN (SwiGLU): an embedder loaded with "encoder.layer.{l}.intermediate.gate.weight" [intermediate, hidden] and
+ *    "encoder.layer.{l}.intermediate.gate.bias" [intermediate] computes output.dense(silu(gate . h) * (intermediate.dense . h))
+ *    in place of output.dense(gelu(intermediate.dense . h)); intermediate.dense is the up projection.
+ * nomic has no Linear biases: the host loads zero biases under every BERT bias name (and the gate's), a zero token-type row
+ * if the checkpoint has none, and maps the names (see INTEGRATION.md).  finalize: KRAG_E_INVALID, naming the tensor, when a
+ * gate tensor has the wrong size or is loaded on some layers but not others, or when rotary is off and the position table
+ * is missing. */
 typedef struct krag_embedder krag_embedder;
 typedef struct krag_bert_config {
     int32_t layers, hidden, heads, intermediate, vocab, max_position, type_vocab;
@@ -347,6 +359,13 @@ int32_t krag_debug_embedder_cls_rows(krag_embedder* e, int32_t on);
  * MPNetEncoder.relative_position_bucket with 32 buckets and max distance 128 (the distance is clamped to [-128, 128] first,
  * which changes no bucket).  Host-only: needs no device.  Test hook. */
 int32_t krag_debug_relative_bucket(int32_t rel);
+/* Rotary positions (nomic-bert): base = the model's rotary base (rotary_emb_base / rope_theta; nomic: 1000), 0 = off (the
+ * default: the position table).  Takes effect at the next krag_embedder_finalize.  base < 0 or infinite: KRAG_E_INVALID. */
+int32_t krag_embedder_set_rotary(krag_embedder* e, float base);
+/* The fp32 cos and sin a rotary embedder applies at position pos to pairs j = 0 .. dh/2 - 1 of a head (cos_out, sin_out:
+ * dh/2 floats each): the angle fp32(pos) * inv_freq[j], inv_freq[j] = 1 / base^(2j / dh), both fp32 as torch computes
+ * them.  Host-only: needs no device.  Test hook. */
+int32_t krag_debug_rotary_cos_sin(float base, int32_t dh, int32_t pos, float* cos_out, float* sin_out);
 /* Cross-encoder reranking (BertForSequenceClassification with one label).  The embedder must have been loaded with the
  * head as well: "pooler.dense.weight" [hidden, hidden], "pooler.dense.bias", "classifier.weight" [1, hidden] and
  * "classifier.bias" [1].  Query i owns pairs pair_offsets[i] .. pair_offsets[i+1] (0 to 300 of them); pair p is the packed

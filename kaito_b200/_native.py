@@ -43,7 +43,7 @@ SYMBOLS = [
     "krag_debug_embedder_cls_rows", "krag_rerank", "krag_embedder_set_precision", "krag_debug_gemm_f16",
     "krag_embedder_set_position_offset", "krag_text_unigram_create", "krag_text_unigram_encode_batch",
     "krag_text_unigram_destroy", "krag_debug_tc_dump_pass", "krag_debug_tc_prune", "krag_debug_relative_bucket",
-    "krag_wordpiece_create_specials",
+    "krag_wordpiece_create_specials", "krag_embedder_set_rotary", "krag_debug_rotary_cos_sin",
 ]
 # krag_debug_tc_dump_pass / krag_debug_tc_prune: the prune pass to run (KRAG_TC_PASS_*)
 TC_PASS_TF32, TC_PASS_BF16_SPLIT, TC_PASS_BF16_SHADOW, TC_PASS_BF16_HOST = 0, 1, 2, 3
@@ -150,6 +150,8 @@ def load() -> C.CDLL:
     L.krag_wordpiece_create.argtypes = [C.c_char_p, i64, i32, C.POINTER(vp)]
     L.krag_wordpiece_create_specials.argtypes = [C.c_char_p, i64, i32, C.c_char_p, C.c_char_p, C.c_char_p, C.POINTER(vp)]
     L.krag_debug_relative_bucket.argtypes = [i32]
+    L.krag_embedder_set_rotary.argtypes = [vp, C.c_float]
+    L.krag_debug_rotary_cos_sin.argtypes = [C.c_float, i32, i32, vp, vp]
     L.krag_wordpiece_encode_batch.argtypes = [vp, i64, C.c_char_p, vp, i32, vp, vp]
     L.krag_wordpiece_destroy.argtypes = [vp]
     L.krag_text_unigram_create.argtypes = [C.c_char_p, vp, vp, i64, i32, C.c_char_p, i64, i32, C.c_char_p, vp, vp, vp, i32,
@@ -308,7 +310,9 @@ class P2PExchange:
 
 
 class Embedder:
-    """krag_embedder: BERT-family encoder forward on the GPU (K5)."""
+    """krag_embedder: BERT-family encoder forward on the GPU (K5).  Variants (kaito_rag.h): MPNet when loaded with
+    encoder.relative_attention_bias.weight; nomic-bert's rotary positions with set_rotary(base) before load_state_dict; a
+    gated (SwiGLU) FFN when loaded with encoder.layer.{l}.intermediate.gate.weight / .bias on every layer."""
 
     def __init__(self, ctx: "Context", layers, hidden, heads, intermediate, vocab, max_position=512, type_vocab=2,
                  ln_eps=1e-12):
@@ -369,6 +373,11 @@ class Embedder:
         """position row of every sequence's first token (krag_embedder_set_position_offset; XLM-R: pad_token_id + 1)"""
         check(self._L.krag_embedder_set_position_offset(self._h, off))
 
+    def set_rotary(self, base: float):
+        """rotary positions with this base (nomic-bert: rotary_emb_base 1000) instead of a position table, 0 = off
+        (krag_embedder_set_rotary); before load_state_dict, which finalizes"""
+        check(self._L.krag_embedder_set_rotary(self._h, float(base)))
+
     def rerank(self, pair_offsets, flat_tokens, tok_offsets, seg_b, top_k: int, activation: int = RERANK_SIGMOID):
         """krag_rerank: (positions int32 [n_queries, top_k], scores float32 [n_queries, top_k]); -1 / NaN past a query's
         pair count.  seg_b None: unsegmented pairs (token type 0 throughout)"""
@@ -395,6 +404,13 @@ class Embedder:
 def debug_relative_bucket(rel: int) -> int:
     """the MPNet relative-position bucket K5's attention applies at rel = key - query (krag_debug_relative_bucket; no GPU)"""
     return int(load().krag_debug_relative_bucket(rel))
+
+
+def debug_rotary_cos_sin(base: float, dh: int, pos: int) -> tuple[np.ndarray, np.ndarray]:
+    """the fp32 (cos [dh / 2], sin [dh / 2]) a rotary embedder applies at position pos (krag_debug_rotary_cos_sin; no GPU)"""
+    cos, sin = np.empty(dh // 2, np.float32), np.empty(dh // 2, np.float32)
+    check(load().krag_debug_rotary_cos_sin(float(base), dh, pos, ptr(cos), ptr(sin)))
+    return cos, sin
 
 
 def debug_gemm_tf32(ctx: "Context", A, B, bias, residual=None, gelu=False, tile_n=0) -> np.ndarray:

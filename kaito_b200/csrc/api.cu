@@ -1822,6 +1822,20 @@ int32_t krag_embedder_set_position_offset(krag_embedder* h, int32_t off)
     });
 }
 int32_t krag_debug_relative_bucket(int32_t rel) { return relative_bucket(rel); }
+int32_t krag_embedder_set_rotary(krag_embedder* h, float base)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(h, KRAG_E_INVALID, "null embedder");
+        embedder_set_rotary(h->e, base);
+    });
+}
+int32_t krag_debug_rotary_cos_sin(float base, int32_t dh, int32_t pos, float* cos_out, float* sin_out)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(cos_out && sin_out && base > 0.f && dh >= 2 && dh % 2 == 0 && pos >= 0, KRAG_E_INVALID, "bad argument");
+        rotary_cos_sin(base, dh, pos, cos_out, sin_out);
+    });
+}
 int32_t krag_debug_embedder_cls_rows(krag_embedder* h, int32_t on)
 {
     return guarded([&] {

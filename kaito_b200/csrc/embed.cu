@@ -124,15 +124,32 @@ struct GemmOut {
     uint16_t* lo;        // PLANES == 1: not written
 };
 
+__device__ __forceinline__ float silu(float g) { return g / (1.f + expf(-g)); }
+// EP_ROPE: (o0, o1) = elements i and i + dh/2 of a query or key head (the weight rows were permuted at finalize so that
+// they are adjacent columns), rotated by the angle of (row position, pair i): q * cos + rotate_half(q) * sin in fp32
+__device__ __forceinline__ void rope_rotate(float& o0, float& o1, float2 cs)
+{
+    const float a = o0 * cs.x - o1 * cs.y, b = o1 * cs.x + o0 * cs.y;
+    o0 = a; o1 = b;
+}
+
 // PLANES == 2: the split product above.  PLANES == 1 (KRAG_PRECISION_FP16): the operands are the hi planes alone, fp16(v); a
 // stage holds hi_A and hi_B (half the bytes: the ring is twice as deep), every K = 16 step is ONE wgmma into ONE
 // accumulator (which leaves the registers for 128 x 256 tiles), and the epilogue writes fp32 C and / or the hi plane.
-template <int BN, int PLANES>
+//
+// EP (compile time) selects what the epilogue does after the bias (EpiArgs, engine.h):
+//   EP_PLAIN   the BERT epilogue (+GELU) (+residual);
+//   EP_ROPE    the QKV projection of a rotary encoder: columns below ep.rope_cols (Q and K) are rotated pairwise, a thread's
+//              (c = 0, 1) pair being one (i, i + dh/2) pair of a head;
+//   EP_SWIGLU  the gated FFN1: the weight rows are interleaved in blocks of 16 (8 up rows, then the 8 gate rows of the same
+//              outputs), so column group j (even) holds up and group j + 1 the matching gate values; the epilogue writes
+//              silu(gate) * up to [M][N / 2] outputs.
+template <int BN, int PLANES, int EP = EP_PLAIN>
 __global__ void __launch_bounds__(GM_THREADS, 1)
 gemm_f16s_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmA2,
                  const __grid_constant__ CUtensorMap tmB1, const __grid_constant__ CUtensorMap tmB2, int M, int N, int splits,
                  int kb_per_split, int n_stages, int b_evict_first, const float* __restrict__ bias, const float* residual,
-                 int act_gelu, GemmOut out, float* __restrict__ ws)
+                 int act_gelu, GemmOut out, float* __restrict__ ws, EpiArgs ep)
 {
     constexpr int B_BYTES = BN * 128;                      // one plane of one weight k-block
     constexpr int STAGE_BYTES = PLANES * (GM_SLAB + B_BYTES);
@@ -240,32 +257,46 @@ gemm_f16s_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant
                     }
                     continue;
                 }
+                // EP_SWIGLU writes rows of N / 2 outputs; EP_ROPE: this row's (cos, sin) pairs
+                const size_t ooff = EP == EP_SWIGLU ? (size_t)row * (N / 2) : roff;
+                const float2* rope_row = nullptr;
+                if constexpr (EP == EP_ROPE) rope_row = reinterpret_cast<const float2*>(ep.rope) + (size_t)__ldg(ep.pos + row) * ep.half;
 #pragma unroll
                 for (int j0 = 0; j0 < R / 4; j0 += EP_J) {
-                    float2 b2[EP_J], r2[EP_J];
+                    float2 b2[EP_J], r2[EP_J], cs[EP == EP_ROPE ? EP_J : 1];
 #pragma unroll
                     for (int u = 0; u < EP_J; ++u) {
                         const int col = n0 + 8 * (j0 + u) + 2 * q;
                         b2[u] = __ldg(reinterpret_cast<const float2*>(bias + col));
                         r2[u] = residual ? *reinterpret_cast<const float2*>(residual + roff + col) : make_float2(0.f, 0.f);
+                        if constexpr (EP == EP_ROPE)
+                            cs[u] = col < ep.rope_cols ? __ldg(rope_row + ((col & (2 * ep.half - 1)) >> 1)) : make_float2(1.f, 0.f);
                     }
 #pragma unroll
                     for (int u = 0; u < EP_J; ++u) {
-                        const int j = j0 + u, col = n0 + 8 * j + 2 * q;
+                        const int j = j0 + u;
+                        int col = n0 + 8 * j + 2 * q;
                         float o0 = acc(4 * j + 2 * h), o1 = acc(4 * j + 2 * h + 1);
                         o0 += b2[u].x; o1 += b2[u].y;
+                        if constexpr (EP == EP_SWIGLU) {
+                            if (u & 1) continue;                     // the gate group: consumed with its up group
+                            const float g0 = acc(4 * j + 4 + 2 * h) + b2[u + 1].x, g1 = acc(4 * j + 4 + 2 * h + 1) + b2[u + 1].y;
+                            o0 = silu(g0) * o0; o1 = silu(g1) * o1;
+                            col = n0 / 2 + 4 * j + 2 * q;              // output column of the 16-column block's 8 outputs
+                        }
                         if (act_gelu) { o0 = gelu_erf(o0); o1 = gelu_erf(o1); }
+                        if constexpr (EP == EP_ROPE) rope_rotate(o0, o1, cs[u]);
                         if (residual) { o0 += r2[u].x; o1 += r2[u].y; }
-                        if (out.c) *reinterpret_cast<float2*>(out.c + roff + col) = make_float2(o0, o1);
+                        if (out.c) *reinterpret_cast<float2*>(out.c + ooff + col) = make_float2(o0, o1);
                         if constexpr (PLANES == 2) {
                             if (out.hi) {
                                 uint16_t h0, l0, h1, l1;
                                 split_f16(o0, h0, l0); split_f16(o1, h1, l1);
-                                *reinterpret_cast<uint32_t*>(out.hi + roff + col) = (uint32_t)h0 | ((uint32_t)h1 << 16);
-                                *reinterpret_cast<uint32_t*>(out.lo + roff + col) = (uint32_t)l0 | ((uint32_t)l1 << 16);
+                                *reinterpret_cast<uint32_t*>(out.hi + ooff + col) = (uint32_t)h0 | ((uint32_t)h1 << 16);
+                                *reinterpret_cast<uint32_t*>(out.lo + ooff + col) = (uint32_t)l0 | ((uint32_t)l1 << 16);
                             }
                         } else {
-                            if (out.hi) *reinterpret_cast<uint32_t*>(out.hi + roff + col) = hi_pack2(o0, o1);
+                            if (out.hi) *reinterpret_cast<uint32_t*>(out.hi + ooff + col) = hi_pack2(o0, o1);
                         }
                     }
                 }
@@ -347,6 +378,8 @@ layernorm_kernel(const float* __restrict__ x, float* __restrict__ y, uint16_t* _
 
 // embeddings: x[t] = LN(word[id] + pos[p] + type[typ[t]]); one warp per token; scratch row in shared memory.  typ null (single
 // sequences): type row 0 for every token; a cross-encoder pair has type 0 through its first [SEP] and type 1 after it.
+// POS = false (rotary encoders): no position row, x[t] = LN(word[id] + type[typ[t]]); pos and pemb are not read.
+template <bool POS>
 __global__ void __launch_bounds__(256)
 embed_ln_kernel(const int32_t* __restrict__ tok, const int32_t* __restrict__ pos, const int32_t* __restrict__ typ,
                 const float* __restrict__ word, const float* __restrict__ pemb, const float* __restrict__ temb, const float* __restrict__ g,
@@ -363,9 +396,13 @@ embed_ln_kernel(const int32_t* __restrict__ tok, const int32_t* __restrict__ pos
     int id = tok[t];
     id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
     const float* wr = word + (size_t)id * d;
-    const float* pr = pemb + (size_t)pos[t] * d;
+    const float* pr = POS ? pemb + (size_t)pos[t] * d : nullptr;
     const float* tr = typ ? temb + (size_t)typ[t] * d : temb;
-    for (int i = lane; i < d; i += 32) row[i] = (wr[i] + tr[i]) + pr[i];   // torch: inputs_embeds + token_type + position
+    if constexpr (POS) {
+        for (int i = lane; i < d; i += 32) row[i] = (wr[i] + tr[i]) + pr[i];   // torch: inputs_embeds + token_type + position
+    } else {
+        for (int i = lane; i < d; i += 32) row[i] = wr[i] + tr[i];
+    }
     __syncwarp();
     warp_layernorm_row(row, x + (size_t)t * d, x_hi + (size_t)t * d, x_lo ? x_lo + (size_t)t * d : nullptr, g, b, d, eps, lane);
 }
@@ -374,17 +411,22 @@ embed_ln_kernel(const int32_t* __restrict__ tok, const int32_t* __restrict__ pos
 // the row (N <= 1024).  One 256-thread block per row, one float4 column group per thread: the `splits` partial loads
 // of a thread are independent (all in flight at once) -- with a few rows this kernel is pure load latency.
 // `residual` and `out` may alias (a thread reads its residual elements before it writes them).
+// EP as in gemm_f16s_kernel (no LayerNorm with EP_ROPE / EP_SWIGLU): EP_ROPE rotates the float4's two (i, i + dh/2) pairs
+// below ep.rope_cols; EP_SWIGLU reads output group c's up columns and the gate columns 8 to their right and writes
+// silu(gate) * up to rows of N / 2.
 constexpr int SK_MAX_SPLITS = 8;
+template <int EP = EP_PLAIN>
 __global__ void __launch_bounds__(256)
 splitk_reduce_kernel(const float* __restrict__ ws, int splits, int M, int N, const float* __restrict__ bias, const float* residual,
                      int act_gelu, const float* __restrict__ ln_g, const float* __restrict__ ln_b, float eps, float* out,
-                     uint16_t* __restrict__ out_hi, uint16_t* __restrict__ out_lo)
+                     uint16_t* __restrict__ out_hi, uint16_t* __restrict__ out_lo, EpiArgs ep)
 {
     __shared__ float s_red[2][8];
     pdl_launch_dependents();
     pdl_wait();
     const int row = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const size_t plane = (size_t)M * N;
+    const int ldo = EP == EP_SWIGLU ? N / 2 : N;              // output row stride
     const float* w0 = ws + (size_t)row * N;
     auto element = [&](int c) {
         float4 p[SK_MAX_SPLITS];
@@ -405,16 +447,36 @@ splitk_reduce_kernel(const float* __restrict__ ws, int splits, int M, int N, con
         return s;
     };
     auto store4 = [&](int c, const float4& o) {
-        if (out) *reinterpret_cast<float4*>(out + (size_t)row * N + c) = o;
+        if (out) *reinterpret_cast<float4*>(out + (size_t)row * ldo + c) = o;
         if (out_hi && !out_lo) {
-            *reinterpret_cast<uint2*>(out_hi + (size_t)row * N + c) = make_uint2(hi_pack2(o.x, o.y), hi_pack2(o.z, o.w));
+            *reinterpret_cast<uint2*>(out_hi + (size_t)row * ldo + c) = make_uint2(hi_pack2(o.x, o.y), hi_pack2(o.z, o.w));
         } else if (out_hi) {
             uint16_t h0, l0, h1, l1, h2, l2, h3, l3;
             split_f16(o.x, h0, l0); split_f16(o.y, h1, l1); split_f16(o.z, h2, l2); split_f16(o.w, h3, l3);
-            *reinterpret_cast<uint2*>(out_hi + (size_t)row * N + c) = make_uint2((uint32_t)h0 | ((uint32_t)h1 << 16), (uint32_t)h2 | ((uint32_t)h3 << 16));
-            *reinterpret_cast<uint2*>(out_lo + (size_t)row * N + c) = make_uint2((uint32_t)l0 | ((uint32_t)l1 << 16), (uint32_t)l2 | ((uint32_t)l3 << 16));
+            *reinterpret_cast<uint2*>(out_hi + (size_t)row * ldo + c) = make_uint2((uint32_t)h0 | ((uint32_t)h1 << 16), (uint32_t)h2 | ((uint32_t)h3 << 16));
+            *reinterpret_cast<uint2*>(out_lo + (size_t)row * ldo + c) = make_uint2((uint32_t)l0 | ((uint32_t)l1 << 16), (uint32_t)l2 | ((uint32_t)l3 << 16));
         }
     };
+    if constexpr (EP == EP_SWIGLU) {
+        for (int c = tid * 4; c < ldo; c += 1024) {
+            const int cu = (c >> 3) * 16 + (c & 7);                // up columns of outputs c .. c + 3; the gate's are cu + 8
+            const float4 u = element(cu), g = element(cu + 8);
+            store4(c, make_float4(silu(g.x) * u.x, silu(g.y) * u.y, silu(g.z) * u.z, silu(g.w) * u.w));
+        }
+        return;
+    } else if constexpr (EP == EP_ROPE) {
+        const float2* rope_row = reinterpret_cast<const float2*>(ep.rope) + (size_t)__ldg(ep.pos + row) * ep.half;
+        for (int c = tid * 4; c < N; c += 1024) {
+            float4 o = element(c);
+            if (c < ep.rope_cols) {
+                const int i = (c & (2 * ep.half - 1)) >> 1;       // pairs (c, c + 1) and (c + 2, c + 3): i and i + 1
+                rope_rotate(o.x, o.y, __ldg(rope_row + i));
+                rope_rotate(o.z, o.w, __ldg(rope_row + i + 1));
+            }
+            store4(c, o);
+        }
+        return;
+    }
     if (ln_g == nullptr) {
         for (int c = tid * 4; c < N; c += 1024) store4(c, element(c));
         return;
@@ -916,16 +978,24 @@ static void emb_map(CUtensorMap* tm, const uint16_t* base, int rows, int cols, i
         throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled failed", __FILE__, __LINE__};
 }
 
+template <int BN, int PLANES, int EP>
+static void launch_gemm_ep(dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap& tmA1, const CUtensorMap& tmA2, const CUtensorMap& tmB1,
+                           const CUtensorMap& tmB2, int M, int N, int splits, int kb_per_split, int n_stages, int b_evict_first,
+                           const float* bias, const float* residual, bool gelu, const GemmOut& out, float* ws, const EpiArgs& ep)
+{
+    static bool attr = false;
+    if (!attr) { KRAG_CUDA(cudaFuncSetAttribute(gemm_f16s_kernel<BN, PLANES, EP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = true; }
+    launch_pdl(gemm_f16s_kernel<BN, PLANES, EP>, grid, dim3(GM_THREADS), smem, st, tmA1, tmA2, tmB1, tmB2, M, N, splits, kb_per_split,
+               n_stages, b_evict_first, bias, residual, gelu ? 1 : 0, out, ws, ep);
+}
 // gemm_f16s_kernel over the 128 x BN tiles of C and `splits` K slices, min(work items, SMs) persistent CTAs
 template <int BN, int PLANES>
 static void launch_gemm(const DeviceInfo& di, const SplitMat& A, const SplitMat& B, int M, int N, int K, int splits, const float* bias,
-                        const float* residual, bool gelu, const GemmOut& out, float* ws, cudaStream_t st)
+                        const float* residual, bool gelu, const GemmOut& out, float* ws, cudaStream_t st, const EpiArgs& ep)
 {
     constexpr int stage_bytes = PLANES * (GM_SLAB + BN * 128);
     constexpr int n_stages = GM_SMEM_BUDGET / stage_bytes < GM_MAX_STAGES ? GM_SMEM_BUDGET / stage_bytes : GM_MAX_STAGES;
     constexpr size_t smem = 1024 + (size_t)n_stages * stage_bytes + 2 * GM_MAX_STAGES * 8;
-    static bool attr = false;
-    if (!attr) { KRAG_CUDA(cudaFuncSetAttribute(gemm_f16s_kernel<BN, PLANES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = true; }
     CUtensorMap tmA1, tmA2, tmB1, tmB2;
     emb_map(&tmA1, A.hi, M, K); emb_map(&tmA2, PLANES == 2 ? A.lo : A.hi, M, K);     // PLANES == 1: the second maps are not read
     emb_map(&tmB1, B.hi, N, K, BN); emb_map(&tmB2, PLANES == 2 ? B.lo : B.hi, N, K, BN);
@@ -933,8 +1003,16 @@ static void launch_gemm(const DeviceInfo& di, const SplitMat& A, const SplitMat&
     const int total = m_tiles * (N / BN) * splits;
     const int grid = total < di.sm_count ? total : di.sm_count;
     // one activation tile: every weight byte is read once, keep it out of the way of the activations in L2
-    launch_pdl(gemm_f16s_kernel<BN, PLANES>, dim3((unsigned)grid), dim3(GM_THREADS), smem, st, tmA1, tmA2, tmB1, tmB2, M, N, splits,
-               K / GH_KB / splits, n_stages, m_tiles == 1 ? 1 : 0, bias, residual, gelu ? 1 : 0, out, ws);
+    const int kbs = K / GH_KB / splits, evict_b = m_tiles == 1 ? 1 : 0;
+    if (ep.mode == EP_ROPE)
+        launch_gemm_ep<BN, PLANES, EP_ROPE>(dim3((unsigned)grid), smem, st, tmA1, tmA2, tmB1, tmB2, M, N, splits, kbs, n_stages, evict_b, bias,
+                                            residual, gelu, out, ws, ep);
+    else if (ep.mode == EP_SWIGLU)
+        launch_gemm_ep<BN, PLANES, EP_SWIGLU>(dim3((unsigned)grid), smem, st, tmA1, tmA2, tmB1, tmB2, M, N, splits, kbs, n_stages, evict_b, bias,
+                                              residual, gelu, out, ws, ep);
+    else
+        launch_gemm_ep<BN, PLANES, EP_PLAIN>(dim3((unsigned)grid), smem, st, tmA1, tmA2, tmB1, tmB2, M, N, splits, kbs, n_stages, evict_b, bias,
+                                             residual, gelu, out, ws, ep);
 }
 
 // Tile width and K split of a linear layer of M rows.  Every output element is summed in an order fixed by (bn, splits)
@@ -967,9 +1045,13 @@ GemmPlan linear_plan(const DeviceInfo& di, int M, int N, int K, bool ln, bool ha
 // row LayerNorm of that goes to Y (fp32) and its split planes (C is then scratch).  plan: null = linear_plan(M, ...).
 void launch_linear(const DeviceInfo& di, const SplitMat& A, const SplitMat& B, int M, int N, int K, const float* bias, const float* residual,
                    bool gelu, float* C, uint16_t* C_hi, uint16_t* C_lo, const float* ln_g, const float* ln_b, float eps, float* Y,
-                   uint16_t* Y_hi, uint16_t* Y_lo, float* ws, size_t ws_floats, cudaStream_t st, const GemmPlan* plan, int planes)
+                   uint16_t* Y_hi, uint16_t* Y_lo, float* ws, size_t ws_floats, cudaStream_t st, const GemmPlan* plan, int planes,
+                   const EpiArgs* epi)
 {
     if (ln_g && N > 32 * LN_MAX_GROUPS * 8) throw std::runtime_error("launch_linear: fused LayerNorm rows hold at most 1024 elements");
+    const EpiArgs ep = epi ? *epi : EpiArgs{EP_PLAIN, nullptr, nullptr, 0, 0};
+    if (ep.mode != EP_PLAIN && (ln_g || residual || gelu))
+        throw std::runtime_error("launch_linear: the rotary and gated epilogues take no LayerNorm, residual or GELU");
     const GemmPlan p = plan ? *plan : linear_plan(di, M, N, K, ln_g != nullptr, ws != nullptr, ws_floats, planes);
     if (planes == 1) { C_lo = nullptr; Y_lo = nullptr; }
     if (planes != 1 && planes != 2) throw std::runtime_error("launch_linear: one or two operand planes");
@@ -979,23 +1061,25 @@ void launch_linear(const DeviceInfo& di, const SplitMat& A, const SplitMat& B, i
         // splits == 1 and a LayerNorm to follow: the GEMM writes fp32 C (scratch), the LayerNorm kernel writes Y + planes
         const GemmOut direct = ln_g ? GemmOut{C, nullptr, nullptr} : GemmOut{C, C_hi, C_lo};
         if (planes == 1) {
-            if (p.bn == 32) launch_gemm<32, 1>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
-            else if (p.bn == 256) launch_gemm<256, 1>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
-            else if (p.bn == 128) launch_gemm<128, 1>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
-            else launch_gemm<64, 1>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
-        } else if (p.bn == 32) launch_gemm<32, 2>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
-        else if (p.bn == 128) launch_gemm<128, 2>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
-        else launch_gemm<64, 2>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st);
+            if (p.bn == 32) launch_gemm<32, 1>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st, ep);
+            else if (p.bn == 256) launch_gemm<256, 1>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st, ep);
+            else if (p.bn == 128) launch_gemm<128, 1>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st, ep);
+            else launch_gemm<64, 1>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st, ep);
+        } else if (p.bn == 32) launch_gemm<32, 2>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st, ep);
+        else if (p.bn == 128) launch_gemm<128, 2>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st, ep);
+        else launch_gemm<64, 2>(di, A, B, M, N, K, p.splits, bias, residual, gelu, direct, ws, st, ep);
         if (p.splits > 1) {
-            launch_pdl(splitk_reduce_kernel, dim3((unsigned)M), dim3(256), 0, st, ws, p.splits, M, N, bias, residual, gelu ? 1 : 0, ln_g, ln_b,
-                       eps, ln_g ? Y : C, ln_g ? Y_hi : C_hi, ln_g ? Y_lo : C_lo);
+            auto reduce = ep.mode == EP_ROPE ? splitk_reduce_kernel<EP_ROPE>
+                          : ep.mode == EP_SWIGLU ? splitk_reduce_kernel<EP_SWIGLU> : splitk_reduce_kernel<EP_PLAIN>;
+            launch_pdl(reduce, dim3((unsigned)M), dim3(256), 0, st, ws, p.splits, M, N, bias, residual, gelu ? 1 : 0, ln_g, ln_b,
+                       eps, ln_g ? Y : C, ln_g ? Y_hi : C_hi, ln_g ? Y_lo : C_lo, ep);
             return;
         }
     } else {
         const GemmOut direct = ln_g ? GemmOut{C, nullptr, nullptr} : GemmOut{C, C_hi, C_lo};
-        if (planes == 1 && p.bn == 256) launch_gemm<256, 1>(di, A, B, M, N, K, 1, bias, residual, gelu, direct, nullptr, st);
-        else if (planes == 1) launch_gemm<128, 1>(di, A, B, M, N, K, 1, bias, residual, gelu, direct, nullptr, st);
-        else launch_gemm<128, 2>(di, A, B, M, N, K, 1, bias, residual, gelu, direct, nullptr, st);
+        if (planes == 1 && p.bn == 256) launch_gemm<256, 1>(di, A, B, M, N, K, 1, bias, residual, gelu, direct, nullptr, st, ep);
+        else if (planes == 1) launch_gemm<128, 1>(di, A, B, M, N, K, 1, bias, residual, gelu, direct, nullptr, st, ep);
+        else launch_gemm<128, 2>(di, A, B, M, N, K, 1, bias, residual, gelu, direct, nullptr, st, ep);
     }
     if (ln_g) {
         launch_pdl(layernorm_kernel, dim3((unsigned)((M * 32 + 255) / 256)), dim3(256), 0, st, C, Y, Y_hi, Y_lo, ln_g, ln_b, M, N, eps);
@@ -1049,6 +1133,13 @@ struct Embedder {
     std::vector<DevArray<uint16_t>> planes;     // the buffers all weight planes live in
     SplitMat s_pool{nullptr, nullptr};          // pooler.dense.weight (cross-encoders: finalize found the classifier head)
     DevArray<float> rel_tab;                    // MPNet: [heads][REL_TAB] relative-position bias by distance (finalize); else null
+    // rotary encoders (nomic-bert): rope_base > 0 (krag_embedder_set_rotary); finalize permutes each head's Q and K weight rows
+    // so that elements i and i + dh/2 are adjacent and builds rope [max_pos][dh/2] (cos, sin)
+    float rope_base = 0.f;
+    DevArray<float> rope;
+    // gated FFN (SwiGLU): loaded with intermediate.gate.*; finalize interleaves up / gate rows into s_f1 and their biases into bf1
+    bool gated = false;
+    std::vector<DevArray<float>> bf1;
     bool has_head = false;
     bool finalized = false;
     cudaStream_t st = nullptr;
@@ -1149,21 +1240,77 @@ int relative_bucket(int rel)
 static const char* const REL_BIAS = "encoder.relative_attention_bias.weight";   // MPNet: [32 buckets][heads]
 constexpr int REL_BUCKETS = 32;
 
+// transformers' default RoPE (NomicBertRotaryEmbedding): inv_freq[i] = 1 / base^(2i / dh) and the angle fp32(pos) *
+// inv_freq[i], both fp32 as torch computes them; cos and sin of that fp32 angle rounded to fp32.  (Angles computed in fp64
+// would differ by up to half an fp32 ulp of the angle: 2.4e-4 rad at position 8000.)
+void rotary_cos_sin(float base, int dh, int pos, float* cos_out, float* sin_out)
+{
+    for (int i = 0; i < dh / 2; ++i) {
+        const float ex = (float)(2 * i) / (float)dh;
+        const float inv = 1.f / (float)std::pow((double)base, (double)ex);
+        const float theta = (float)pos * inv;
+        cos_out[i] = (float)std::cos((double)theta);
+        sin_out[i] = (float)std::sin((double)theta);
+    }
+}
+
+void embedder_set_rotary(Embedder* e, float base)
+{
+    if (!(base >= 0.f) || std::isinf(base)) throw std::runtime_error("embedder: the rotary base must be finite and >= 0 (0: off)");
+    e->rope_base = base;
+    e->finalized = false;
+}
+
+static bool emb_has(const Embedder* e, const std::string& name)
+{
+    const auto it = e->t.find(name);
+    return it != e->t.end() && it->second.p;
+}
+// rows [heads * dh][cols] copied to dst with each head's rows i and i + dh/2 made adjacent (rows 2i, 2i + 1): the pair the
+// rotary epilogue rotates is then one thread's two columns (q . k is unchanged when Q and K are permuted alike)
+static void rope_permute_rows(float* dst, const float* src, int heads, int dh, int cols, cudaStream_t st)
+{
+    const int half = dh / 2;
+    const size_t row = sizeof(float) * (size_t)cols;
+    for (int h = 0; h < heads; ++h)
+        for (int s = 0; s < 2; ++s)
+            KRAG_CUDA(cudaMemcpy2DAsync(dst + ((size_t)h * dh + s) * cols, 2 * row, src + ((size_t)h * dh + (size_t)s * half) * cols, row, row,
+                                        (size_t)half, cudaMemcpyDeviceToDevice, st));
+}
+// up rows 8b .. 8b + 7 -> rows 16b .. 16b + 7 and gate rows 8b .. 8b + 7 -> rows 16b + 8 .. 16b + 15 of dst [2 * inter][cols]
+static void swiglu_interleave_rows(float* dst, const float* up, const float* gate, int inter, int cols, cudaStream_t st)
+{
+    const size_t blk = sizeof(float) * 8 * (size_t)cols;
+    KRAG_CUDA(cudaMemcpy2DAsync(dst, 2 * blk, up, blk, blk, (size_t)inter / 8, cudaMemcpyDeviceToDevice, st));
+    KRAG_CUDA(cudaMemcpy2DAsync(dst + 8 * (size_t)cols, 2 * blk, gate, blk, blk, (size_t)inter / 8, cudaMemcpyDeviceToDevice, st));
+}
+
 void embedder_finalize(Embedder* e)
 {
     const int d = e->cfg.hidden, inter = e->cfg.inter;
     e->finalized = false;
     e->bqkv.clear(); e->planes.clear(); e->s_qkv.clear(); e->s_o.clear(); e->s_f1.clear(); e->s_f2.clear();
     e->s_pool = SplitMat{nullptr, nullptr}; e->has_head = false;
-    e->rel_tab.release();
+    e->rel_tab.release(); e->rope.release(); e->bf1.clear(); e->gated = false;
     e->drop_graphs(); e->seen.clear();   // captured weight pointers are about to change
     const BertConfig& c = e->cfg;
+    const int dh = d / c.heads;
     // every size first: a refused state leaves no half-built planes behind
     const auto rit = e->t.find(REL_BIAS);
     const bool rel = rit != e->t.end() && rit->second.p;   // an MPNet encoder: loaded with the relative-position bias
     if (rel) emb_get(e, REL_BIAS, (int64_t)REL_BUCKETS * c.heads);
+    const bool rotary = e->rope_base > 0.f;
+    // a gated FFN: every layer loaded with intermediate.gate.weight [inter][hidden] (and its bias), or none
+    const bool gated = emb_has(e, lname(0, "intermediate.gate.weight"));
+    for (int l = 0; l < c.layers; ++l) {
+        if (emb_has(e, lname(l, "intermediate.gate.weight")) != gated)
+            throw std::runtime_error("embedder: " + lname(l, "intermediate.gate.weight") + (gated ? " missing" : " loaded") +
+                                     ": a gated FFN needs the gate tensors on every layer (" + lname(0, "intermediate.gate.weight") +
+                                     (gated ? " is loaded)" : " is not)"));
+        if (gated) { emb_get(e, lname(l, "intermediate.gate.weight"), (int64_t)inter * d); emb_get(e, lname(l, "intermediate.gate.bias"), inter); }
+    }
     emb_get(e, "embeddings.word_embeddings.weight", (int64_t)c.vocab * d);
-    emb_get(e, "embeddings.position_embeddings.weight", (int64_t)c.max_pos * d);
+    if (!rotary) emb_get(e, "embeddings.position_embeddings.weight", (int64_t)c.max_pos * d);
     emb_get(e, "embeddings.token_type_embeddings.weight", (int64_t)c.type_vocab * d);
     emb_get(e, "embeddings.LayerNorm.weight", d); emb_get(e, "embeddings.LayerNorm.bias", d);
     for (int l = 0; l < c.layers; ++l) {
@@ -1177,21 +1324,51 @@ void embedder_finalize(Embedder* e)
         emb_get(e, lname(l, "output.dense.weight"), (int64_t)d * inter);
     }
     DevArray<float> wtmp;
-    wtmp.alloc((int64_t)3 * d * d);
+    wtmp.alloc(gated && 2 * inter > 3 * d ? (int64_t)2 * inter * d : (int64_t)3 * d * d);
     for (int l = 0; l < e->cfg.layers; ++l) {
         DevArray<float> b;
         b.alloc((int64_t)3 * d);
         const char* names[3] = {"attention.self.query", "attention.self.key", "attention.self.value"};
         for (int j = 0; j < 3; ++j) {
-            KRAG_CUDA(cudaMemcpyAsync(wtmp.p + (size_t)j * d * d, emb_get(e, lname(l, names[j]) + ".weight", (int64_t)d * d), sizeof(float) * (size_t)d * d, cudaMemcpyDeviceToDevice, e->st));
-            KRAG_CUDA(cudaMemcpyAsync(b.p + (size_t)j * d, emb_get(e, lname(l, names[j]) + ".bias", d), sizeof(float) * (size_t)d, cudaMemcpyDeviceToDevice, e->st));
+            const float* w = emb_get(e, lname(l, names[j]) + ".weight", (int64_t)d * d);
+            const float* bj = emb_get(e, lname(l, names[j]) + ".bias", d);
+            if (rotary && j < 2) {                       // Q and K: each head's (i, i + dh/2) rows adjacent
+                rope_permute_rows(wtmp.p + (size_t)j * d * d, w, c.heads, dh, d, e->st);
+                rope_permute_rows(b.p + (size_t)j * d, bj, c.heads, dh, 1, e->st);
+                continue;
+            }
+            KRAG_CUDA(cudaMemcpyAsync(wtmp.p + (size_t)j * d * d, w, sizeof(float) * (size_t)d * d, cudaMemcpyDeviceToDevice, e->st));
+            KRAG_CUDA(cudaMemcpyAsync(b.p + (size_t)j * d, bj, sizeof(float) * (size_t)d, cudaMemcpyDeviceToDevice, e->st));
         }
         e->bqkv.push_back(std::move(b));
         e->s_qkv.push_back(emb_split_weight(e, wtmp.p, (size_t)3 * d * d));       // stream order: the split reads wtmp before the next layer overwrites it
         e->s_o.push_back(emb_split_weight(e, emb_get(e, lname(l, "attention.output.dense.weight"), (int64_t)d * d), (size_t)d * d));
-        e->s_f1.push_back(emb_split_weight(e, emb_get(e, lname(l, "intermediate.dense.weight"), (int64_t)inter * d), (size_t)inter * d));
+        if (gated) {                                     // FFN1 = [up; gate] rows interleaved in blocks of 8, N = 2 * inter
+            DevArray<float> bf;
+            bf.alloc((int64_t)2 * inter);
+            swiglu_interleave_rows(wtmp.p, emb_get(e, lname(l, "intermediate.dense.weight"), (int64_t)inter * d),
+                                   emb_get(e, lname(l, "intermediate.gate.weight"), (int64_t)inter * d), inter, d, e->st);
+            swiglu_interleave_rows(bf.p, emb_get(e, lname(l, "intermediate.dense.bias"), inter), emb_get(e, lname(l, "intermediate.gate.bias"), inter),
+                                   inter, 1, e->st);
+            e->bf1.push_back(std::move(bf));
+            e->s_f1.push_back(emb_split_weight(e, wtmp.p, (size_t)2 * inter * d));
+        } else {
+            e->s_f1.push_back(emb_split_weight(e, emb_get(e, lname(l, "intermediate.dense.weight"), (int64_t)inter * d), (size_t)inter * d));
+        }
         e->s_f2.push_back(emb_split_weight(e, emb_get(e, lname(l, "output.dense.weight"), (int64_t)d * inter), (size_t)d * inter));
     }
+    if (rotary) {
+        // (cos, sin) by [position][pair]: ~2 MB at 8192 positions x 32 pairs
+        const int half = dh / 2;
+        std::vector<float> tab((size_t)c.max_pos * half * 2), cs((size_t)half), sn((size_t)half);
+        for (int p = 0; p < c.max_pos; ++p) {
+            rotary_cos_sin(e->rope_base, dh, p, cs.data(), sn.data());
+            for (int i = 0; i < half; ++i) { tab[((size_t)p * half + i) * 2] = cs[(size_t)i]; tab[((size_t)p * half + i) * 2 + 1] = sn[(size_t)i]; }
+        }
+        e->rope.alloc((int64_t)tab.size());
+        KRAG_CUDA(cudaMemcpy(e->rope.p, tab.data(), sizeof(float) * tab.size(), cudaMemcpyHostToDevice));
+    }
+    e->gated = gated;
     // the classifier head of a cross-encoder (BertForSequenceClassification, one label): all four tensors or none
     const char* head[4] = {"pooler.dense.weight", "pooler.dense.bias", "classifier.weight", "classifier.bias"};
     const int64_t head_n[4] = {(int64_t)d * d, d, d, 1};
@@ -1223,7 +1400,7 @@ void embedder_finalize(Embedder* e)
     // the fp32 copies of the GEMM weights are not read again: free them (the split planes hold the same bytes per element)
     for (int l = 0; l < e->cfg.layers; ++l)
         for (const char* nm : {"attention.self.query.weight", "attention.self.key.weight", "attention.self.value.weight",
-                               "attention.output.dense.weight", "intermediate.dense.weight", "output.dense.weight"}) {
+                               "attention.output.dense.weight", "intermediate.dense.weight", "intermediate.gate.weight", "output.dense.weight"}) {
             auto it = e->t.find(lname(l, nm));
             if (it != e->t.end()) it->second.release();
         }
@@ -1346,12 +1523,24 @@ static bool encoder_forward(Embedder* e, int batch, const int32_t* tok_ids, cons
     const bool cls_rows = cls_ok && e->cls_rows_only && (n_tok + GM_TILE - 1) / GM_TILE > (batch + GM_TILE - 1) / GM_TILE;
     // The forward is ~7 kernels per layer; for a handful of query tokens it is bound by launch gaps and kernel
     // prologues, so each (n_tok, batch, max_len, cls_rows, head) shape is captured into a CUDA graph the second time it is seen.
-    auto run_layers = [&]() {
-    launch_pdl(embed_ln_kernel, dim3((unsigned)((n_tok + 7) / 8)), dim3(256), (size_t)8 * d * 4, st, e->d_tok.p, e->d_pos.p,
-               seg_b ? e->d_typ.p : nullptr, e->t["embeddings.word_embeddings.weight"].p, e->t["embeddings.position_embeddings.weight"].p,
-               e->t["embeddings.token_type_embeddings.weight"].p, e->t["embeddings.LayerNorm.weight"].p, e->t["embeddings.LayerNorm.bias"].p, e->x.p,
-               xs.hi, xs.lo, n_tok, d, c.vocab, c.eps);
     const int dh = d / c.heads;
+    // rotary encoders: no position row; Q and K are rotated in the QKV epilogue.  Gated FFN: FFN1 has 2 * inter columns
+    const bool rotary = e->rope.p != nullptr;
+    const EpiArgs ep_qkv{rotary ? EP_ROPE : EP_PLAIN, e->rope.p, e->d_pos.p, 2 * d, dh / 2};
+    const EpiArgs ep_f1{e->gated ? EP_SWIGLU : EP_PLAIN, nullptr, nullptr, 0, 0};
+    const int n_f1 = e->gated ? 2 * c.inter : c.inter;
+    auto f1_bias = [&](int l) { return e->gated ? e->bf1[(size_t)l].p : e->t[lname(l, "intermediate.dense.bias")].p; };
+    auto run_layers = [&]() {
+    if (rotary)
+        launch_pdl(embed_ln_kernel<false>, dim3((unsigned)((n_tok + 7) / 8)), dim3(256), (size_t)8 * d * 4, st, e->d_tok.p, nullptr,
+                   seg_b ? e->d_typ.p : nullptr, e->t["embeddings.word_embeddings.weight"].p, nullptr,
+                   e->t["embeddings.token_type_embeddings.weight"].p, e->t["embeddings.LayerNorm.weight"].p, e->t["embeddings.LayerNorm.bias"].p,
+                   e->x.p, xs.hi, xs.lo, n_tok, d, c.vocab, c.eps);
+    else
+        launch_pdl(embed_ln_kernel<true>, dim3((unsigned)((n_tok + 7) / 8)), dim3(256), (size_t)8 * d * 4, st, e->d_tok.p, e->d_pos.p,
+                   seg_b ? e->d_typ.p : nullptr, e->t["embeddings.word_embeddings.weight"].p, e->t["embeddings.position_embeddings.weight"].p,
+                   e->t["embeddings.token_type_embeddings.weight"].p, e->t["embeddings.LayerNorm.weight"].p, e->t["embeddings.LayerNorm.bias"].p, e->x.p,
+                   xs.hi, xs.lo, n_tok, d, c.vocab, c.eps);
     // the QKV projection writes the split planes only (same bytes as an fp32 matrix); attention reads them on the tensor cores
     uint16_t* q_hi = e->qkv.p;
     uint16_t* q_lo = lo_of(q_hi, (size_t)n_tok * 3 * d);
@@ -1359,7 +1548,7 @@ static bool encoder_forward(Embedder* e, int batch, const int32_t* tok_ids, cons
         const size_t L = (size_t)l;
         const bool last_cls = cls_rows && l == c.layers - 1;
         launch_linear(e->di, xs, e->s_qkv[L], n_tok, 3 * d, d, e->bqkv[L].p, nullptr, false, nullptr, q_hi, q_lo, nullptr, nullptr, 0.f,
-                      nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st, nullptr, planes);
+                      nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st, nullptr, planes, &ep_qkv);
         const float* rel = e->rel_tab.p;                  // null: BERT
         if (planes == 1) {
             if (dh == 64) attention_mma<64, 1>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, rel, st);
@@ -1370,15 +1559,15 @@ static bool encoder_forward(Embedder* e, int batch, const int32_t* tok_ids, cons
             const SplitMat ccs{e->ccs.p, lo_of(e->ccs.p, (size_t)batch * d)}, cxs{e->cxs.p, lo_of(e->cxs.p, (size_t)batch * d)},
                            cfs{e->cfs.p, lo_of(e->cfs.p, (size_t)batch * c.inter)};
             const GemmPlan po = linear_plan(e->di, n_tok, d, d, true, true, Embedder::WS_FLOATS, planes);
-            const GemmPlan p1 = linear_plan(e->di, n_tok, c.inter, d, false, true, Embedder::WS_FLOATS, planes);
+            const GemmPlan p1 = linear_plan(e->di, n_tok, n_f1, d, false, true, Embedder::WS_FLOATS, planes);
             const GemmPlan p2 = linear_plan(e->di, n_tok, d, c.inter, true, true, Embedder::WS_FLOATS, planes);
             launch_pdl(gather_cls_kernel, dim3((unsigned)((batch * 32 + 255) / 256)), dim3(256), 0, st, e->x.p, cs.hi, cs.lo, e->d_off.p, e->cx.p,
                        ccs.hi, ccs.lo, batch, d);
             launch_linear(e->di, ccs, e->s_o[L], batch, d, d, e->t[lname(l, "attention.output.dense.bias")].p, e->cx.p, false, e->cx2.p, nullptr,
                           nullptr, e->t[lname(l, "attention.output.LayerNorm.weight")].p, e->t[lname(l, "attention.output.LayerNorm.bias")].p, c.eps,
                           e->cx.p, cxs.hi, cxs.lo, e->ws.p, Embedder::WS_FLOATS, st, &po, planes);
-            launch_linear(e->di, cxs, e->s_f1[L], batch, c.inter, d, e->t[lname(l, "intermediate.dense.bias")].p, nullptr, true, nullptr, cfs.hi,
-                          cfs.lo, nullptr, nullptr, 0.f, nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st, &p1, planes);
+            launch_linear(e->di, cxs, e->s_f1[L], batch, n_f1, d, f1_bias(l), nullptr, !e->gated, nullptr, cfs.hi,
+                          cfs.lo, nullptr, nullptr, 0.f, nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st, &p1, planes, &ep_f1);
             launch_linear(e->di, cfs, e->s_f2[L], batch, d, c.inter, e->t[lname(l, "output.dense.bias")].p, e->cx.p, false, e->cx2.p, nullptr,
                           nullptr, e->t[lname(l, "output.LayerNorm.weight")].p, e->t[lname(l, "output.LayerNorm.bias")].p, c.eps, e->cx.p, cxs.hi,
                           cxs.lo, e->ws.p, Embedder::WS_FLOATS, st, &p2, planes);
@@ -1388,9 +1577,9 @@ static bool encoder_forward(Embedder* e, int batch, const int32_t* tok_ids, cons
         launch_linear(e->di, cs, e->s_o[L], n_tok, d, d, e->t[lname(l, "attention.output.dense.bias")].p, e->x.p, false, e->x2.p, nullptr, nullptr,
                       e->t[lname(l, "attention.output.LayerNorm.weight")].p, e->t[lname(l, "attention.output.LayerNorm.bias")].p, c.eps, e->x.p, xs.hi, xs.lo,
                       e->ws.p, Embedder::WS_FLOATS, st, nullptr, planes);
-        // FFN1 (+bias, GELU): only the split planes are written (FFN2 is the sole consumer)
-        launch_linear(e->di, xs, e->s_f1[L], n_tok, c.inter, d, e->t[lname(l, "intermediate.dense.bias")].p, nullptr, true, nullptr, fs.hi, fs.lo,
-                      nullptr, nullptr, 0.f, nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st, nullptr, planes);
+        // FFN1 (+bias, GELU; gated: silu(gate) * up): only the split planes are written (FFN2 is the sole consumer)
+        launch_linear(e->di, xs, e->s_f1[L], n_tok, n_f1, d, f1_bias(l), nullptr, !e->gated, nullptr, fs.hi, fs.lo,
+                      nullptr, nullptr, 0.f, nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st, nullptr, planes, &ep_f1);
         // FFN2 (+bias +residual) -> LayerNorm -> x + split planes
         launch_linear(e->di, fs, e->s_f2[L], n_tok, d, c.inter, e->t[lname(l, "output.dense.bias")].p, e->x.p, false, e->x2.p, nullptr, nullptr,
                       e->t[lname(l, "output.LayerNorm.weight")].p, e->t[lname(l, "output.LayerNorm.bias")].p, c.eps, e->x.p, xs.hi, xs.lo, e->ws.p,

@@ -482,6 +482,12 @@ void embedder_set_position_offset(Embedder* e, int off);
 // MPNet: the bucket of MPNetEncoder.relative_position_bucket (32 buckets, max distance 128) the attention kernel applies at
 // rel = key - query (the distance clamped to +-128 first); host-only
 int relative_bucket(int rel);
+// rotary encoders (nomic-bert): positions rotate Q and K instead of a position table; base = the rotary base (0: off).
+// Called before finalize.
+void embedder_set_rotary(Embedder* e, float base);
+// the fp32 (cos, sin) of the rotary angle fp32(pos) * inv_freq[i], inv_freq[i] = 1 / base^(2i / dh) in fp32, for i < dh / 2
+// (what the QKV epilogue applies; transformers' default RoPE); host-only
+void rotary_cos_sin(float base, int dh, int pos, float* cos_out, float* sin_out);
 void embedder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int32_t* tok_offsets, float* out_host,
                       float* out_dev = nullptr, int ld_out = 0, cudaStream_t consumer = nullptr);
 // cross-encoder reranking (classifier head loaded): scores of sentence pairs, top_k per query (see embed.cu)
@@ -500,13 +506,25 @@ void launch_split_f16(const float* in, uint16_t* hi, uint16_t* lo, int64_t n /* 
 // planes = 1: the single-plane product (A.lo, B.lo and the lo outputs are not touched; one fp16 wgmma per step, fp32
 // accumulation), whose large-M path also has 128 x 256 tiles.
 struct GemmPlan { int bn; int splits; bool small_m; };
+// Epilogue variants of a linear layer (compile-time kernel variants, see gemm_f16s_kernel): EP_PLAIN (BERT), EP_ROPE (rotary
+// positions on the Q and K columns of a QKV projection whose weight rows were permuted per head), EP_SWIGLU (gated FFN1 on
+// interleaved up / gate rows: N = 2 * inter columns in, inter out).
+enum { EP_PLAIN = 0, EP_ROPE = 1, EP_SWIGLU = 2 };
+struct EpiArgs {
+    int mode;                 // EP_*
+    const float* rope;        // EP_ROPE: [positions][half] (cos, sin) pairs, fp32
+    const int32_t* pos;       // EP_ROPE: position of every row of A
+    int rope_cols;            // EP_ROPE: columns [0, rope_cols) are rotated (2 * hidden: Q and K)
+    int half;                 // EP_ROPE: head_dim / 2
+};
 // the plan launch_linear picks for M rows: 128 x 128 tiles, or 128 x BN split-K tiles for few activation tiles
 GemmPlan linear_plan(const DeviceInfo& di, int M, int N, int K, bool ln, bool have_ws, size_t ws_floats, int planes = 2);
-// plan = null: linear_plan(M, ...); ws = split-K workspace (may be null)
+// plan = null: linear_plan(M, ...); ws = split-K workspace (may be null); ep = null: EP_PLAIN (EP_ROPE / EP_SWIGLU take no
+// LayerNorm, residual or GELU; EP_SWIGLU's C / C planes are [M][N / 2])
 void launch_linear(const DeviceInfo& di, const SplitMat& A, const SplitMat& B, int M, int N, int K, const float* bias, const float* residual,
                    bool gelu, float* C, uint16_t* C_hi, uint16_t* C_lo, const float* ln_g, const float* ln_b, float eps, float* Y,
                    uint16_t* Y_hi, uint16_t* Y_lo, float* ws, size_t ws_floats, cudaStream_t st, const GemmPlan* plan = nullptr,
-                   int planes = 2);
+                   int planes = 2, const EpiArgs* ep = nullptr);
 // test hook: fp32 device operands, split on the fly, then the path above.  tile_n = 0: launch_linear's own plan; 32, 64 or
 // 128 (256 with planes = 1): that tile width over the whole K range.  reps > 0: the GEMM is launched reps more times between two CUDA
 // events and *ms gets the mean time of one launch.
