@@ -3,17 +3,17 @@
 // Replaces faiss IndexFlatL2.search for query batches (its nq >= 20 sgemm path; reference
 // call site presets/ragengine/vector_store/faiss_store.py:44-49 via hybrid_retriever.py:209-213).
 //
-//   1. dense_tc_kernel<NQ, MODE, DUMP>  (wgmma, TMA-staged, accumulators in registers)
-//        D[128 corpus rows x NQ queries] = X_tile . Q^T.  The prune pass has three operand modes:
-//          TC_BF16  bf16 corpus and queries from shared memory: 2 bytes/element from HBM.  The corpus operand is the high
-//                   halves of split rows (split_rows.cuh: the default on rows with dpad % 64 == 0), the opt-in bf16 shadow
-//                   (KRAG_DENSE_TC_BF16) or the device copy of host-resident rows
-//          TC_TF32  plain fp32 corpus rows and queries consumed as TF32 straight from shared memory
+//   1. the prune pass (wgmma, TMA-staged, accumulators in registers): D[corpus rows x NQ queries] = X_tile . Q^T
+//        dense_tc_bf16_kernel<NQ, DUMP>  192-row tiles, bf16 corpus and queries from shared memory: 2 bytes/element from
+//                   HBM.  The corpus operand is the high halves of split rows (split_rows.cuh: the default on rows with
+//                   dpad % 64 == 0), the opt-in bf16 shadow (KRAG_DENSE_TC_BF16) or the device copy of host-resident rows
+//        dense_tc_kernel<NQ, MODE, DUMP>  128-row tiles, fp32 operands consumed as TF32:
+//          TC_TF32  plain fp32 corpus rows and queries straight from shared memory
 //          TC_TF32S TC_TF32 on split rows: both halves staged by TMA, rebuilt to fp32 in the A registers (tf32 wgmma with A
 //                   from registers); the same products as TC_TF32 on the plain rows, bit for bit
 //        epilogue: a = |x|^2 - 2 x.q  per (row, query), compared with a per-query threshold;
 //        rows below it are appended to that query's candidate list (rare: ~C of N rows).
-//        DUMP mode writes `a` (TF32) for a strided 1/64 sample of the tiles instead.
+//        DUMP mode writes `a` for a strided 1/64 sample of the tiles instead.
 //   2. sample_threshold_kernel: per query, the m-th smallest sampled `a` -> threshold that
 //        admits ~C = max(512, 4P) rows of the full corpus.
 //   3. rescore_kernel: EXACT fp32 squared L2 of every candidate in K1's operation order
@@ -25,7 +25,8 @@
 //
 // So the tensor cores only PRUNE; every returned score is an exact fp32 distance.
 //
-// Roofline: bytes = n_rows*dpad*2 per bf16 pass, n_rows*dpad*4 per tf32 pass (HBM), flops = 2*NQ*n_rows*dpad.
+// Roofline: bytes = n_rows*dpad*2 per bf16 pass, n_rows*dpad*4 per tf32 pass (HBM), flops = 2*NQ*n_rows*dpad.  Every
+// tile also stages all NQ query rows from L2 into shared memory: NQ / tile rows query bytes per corpus byte (bf16 pass).
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <math_constants.h>
@@ -42,17 +43,19 @@
 namespace krag {
 
 // ------------------------------------------------------------------------- the kernel
-constexpr int TC_TILE_M = 128;          // corpus rows per tile: two consumer warpgroups x wgmma M = 64
+constexpr int TC_TILE_M = 128;          // corpus rows per TF32 tile: two consumer warpgroups x wgmma M = 64
 constexpr int TC_KBLOCK = 32;           // fp32 elements per k-block = one 128-byte swizzle row
 constexpr int TC_THREADS = 384;         // warpgroup 0: TMA producer, warpgroups 1-2: wgmma + epilogue
 constexpr int TC_SAMPLE_STRIDE = 64;    // DUMP mode visits every 64th tile
 constexpr int TC_A_BYTES = TC_TILE_M * 128;  // 16 KB: 128 rows x one 128-byte swizzle row (32 fp32 or 64 halves)
 constexpr int TC_DUMP_GROUP = 16;       // rows per minimum in the threshold-sampling dump (one warp's wgmma rows)
+constexpr int TC16_TILE_M = 192;        // corpus rows per bf16 tile: three wgmma M = 64 blocks
+constexpr int TC16_THREADS = 256;       // two warpgroups, both wgmma + epilogue; thread 0 also issues the TMA loads
 
-enum { TC_TF32 = 0, TC_BF16 = 1, TC_TF32S = 2 };
+enum { TC_TF32 = 0, TC_TF32S = 2 };
 
-// One ring; a stage holds the corpus rows of the tile and all NQ query rows for 32 (TF32) or 64 (bf16, TF32S) elements of
-// the dimension: 4 wgmma K steps (8 in TF32S mode, whose stage holds one 64-element block of split rows: its high-half and
+// One ring; a stage holds the corpus rows of the tile and all NQ query rows for 32 (TF32) or 64 (TF32S) elements of the
+// dimension: 4 wgmma K steps (8 in TF32S mode, whose stage holds one 64-element block of split rows: its high-half and
 // low-half boxes, and two fp32 query boxes).
 template <int NQ, int MODE> struct TcCfg {
     static constexpr int A_BYTES = (MODE == TC_TF32S ? 2 : 1) * TC_A_BYTES;
@@ -60,6 +63,16 @@ template <int NQ, int MODE> struct TcCfg {
     static constexpr int STAGE_BYTES = A_BYTES + Q_BYTES;
     static constexpr int STAGES = (200 * 1024) / STAGE_BYTES > 8 ? 8 : (200 * 1024) / STAGE_BYTES;
     static constexpr int ELEMS = MODE == TC_TF32 ? TC_KBLOCK : 2 * TC_KBLOCK;   // dimension elements per stage
+    static constexpr int BAR_BYTES = 256;
+    static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + 1024 /*align*/ + BAR_BYTES + NQ * 4;
+};
+// The bf16 ring: a stage holds the 192 corpus rows of the tile and all NQ query rows for 64 elements (4 wgmma K steps).
+// 4 stages of 56 KB at NQ = 256 (224 KB + barriers + thresholds: inside the 227 KB opt-in).
+template <int NQ> struct Tc16Cfg {
+    static constexpr int A_BYTES = TC16_TILE_M * 128;
+    static constexpr int STAGE_BYTES = A_BYTES + NQ * 128;
+    static constexpr int STAGES = (224 * 1024) / STAGE_BYTES > 8 ? 8 : (224 * 1024) / STAGE_BYTES;
+    static constexpr int ELEMS = 2 * TC_KBLOCK;
     static constexpr int BAR_BYTES = 256;
     static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + 1024 /*align*/ + BAR_BYTES + NQ * 4;
 };
@@ -79,11 +92,74 @@ __device__ __forceinline__ void tf32s_a_fragment(const unsigned char* hi, int r,
     }
 }
 
+// Epilogue of one wgmma accumulator block, straight from its registers: acc[4i + 2h + c] is (tile row ra + 8h, query
+// qoff + 8i + 2q + c), i < R / 4, and xn[h] that row's |x|^2 (+inf: past the end or deleted).
+//   main pass: the rows with a = |x|^2 - 2 x.q below the query's threshold go to its candidate list
+//   DUMP, dump_min: threshold sampling, per query only the minimum of a over this warp's 16 rows, as dump group grp
+//   DUMP, !dump_min: a itself, in dump column dcol0 + row (columns from S on are not written)
+template <int R, bool DUMP>
+__device__ __forceinline__ void tc_epilogue(float* acc, const float* xn, int ra, int qoff, int g, int q, int64_t tile_row0,
+                                            const float* s_thr, uint32_t* cand_count, uint32_t* cand_rows, int cap,
+                                            float* dump, int64_t S, int dump_min, int64_t grp, int64_t dcol0)
+{
+    if (DUMP) {
+        if (dump_min) {
+            // the few smallest values of the sample, which is all the threshold needs, survive
+#pragma unroll
+            for (int i = 0; i < R / 4; ++i) {
+#pragma unroll
+                for (int c = 0; c < 2; ++c) {
+                    float v = fminf(fmaf(-2.f, acc[4 * i + c], xn[0]), fmaf(-2.f, acc[4 * i + 2 + c], xn[1]));
+                    v = fminf(v, __shfl_xor_sync(0xffffffffu, v, 4));
+                    v = fminf(v, __shfl_xor_sync(0xffffffffu, v, 8));
+                    v = fminf(v, __shfl_xor_sync(0xffffffffu, v, 16));
+                    if (g == 0) dump[(int64_t)(qoff + 8 * i + 2 * q + c) * S + grp] = v;
+                }
+            }
+        } else {
+#pragma unroll
+            for (int i = 0; i < R / 4; ++i)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int c = 0; c < 2; ++c)
+                        if (dcol0 + ra + 8 * h < S)
+                            dump[(int64_t)(qoff + 8 * i + 2 * q + c) * S + dcol0 + ra + 8 * h] = fmaf(-2.f, acc[4 * i + 2 * h + c], xn[h]);
+        }
+    } else {
+        // s_thr[j] = thr_j / 2 (see the kernels); ~2 instructions per (row, query) pair on the common path: one add and one max; hits are ~1 in 20000
+        const float half0 = 0.5f * xn[0], half1 = 0.5f * xn[1];
+        float mx0 = -CUDART_INF_F, mx1 = -CUDART_INF_F;
+#pragma unroll
+        for (int i = 0; i < R / 4; ++i) {
+            const float2 t = *reinterpret_cast<const float2*>(s_thr + qoff + 8 * i + 2 * q);
+            acc[4 * i + 0] += t.x; acc[4 * i + 1] += t.y; acc[4 * i + 2] += t.x; acc[4 * i + 3] += t.y;
+            mx0 = fmaxf(mx0, fmaxf(acc[4 * i + 0], acc[4 * i + 1]));
+            mx1 = fmaxf(mx1, fmaxf(acc[4 * i + 2], acc[4 * i + 3]));
+        }
+        if (mx0 > half0 || mx1 > half1) {   // rare: some pair passes  x.q + thr/2 > |x|^2/2
+#pragma unroll
+            for (int i = 0; i < R / 4; ++i) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        if (acc[4 * i + 2 * h + c] > (h ? half1 : half0)) {
+                            const int j = qoff + 8 * i + 2 * q + c;
+                            const uint32_t pos = atomicAdd(&cand_count[j], 1u);
+                            if (pos < (uint32_t)cap) cand_rows[(size_t)j * cap + pos] = (uint32_t)(tile_row0 + ra + 8 * h);
+                        }
+                    }
+                }
+            }
+        }
+    }
+}
+
 template <int NQ, int MODE, bool DUMP>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 dense_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmQ, int64_t n_rows,
-                int kblocks /*stages per tile*/, int piece_step /*TC_BF16: 128-byte pieces per k-block*/, int64_t n_ltiles,
-                int tile_stride, const float* __restrict__ xnorm,
+                int kblocks /*stages per tile*/, int64_t n_ltiles, int tile_stride, const float* __restrict__ xnorm,
                 const uint32_t* __restrict__ alive, const float* __restrict__ thr_g, uint32_t* __restrict__ cand_count,
                 uint32_t* __restrict__ cand_rows, int cap, float* __restrict__ dump, int64_t S, int dump_min)
 {
@@ -124,8 +200,6 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
                         tma_load_3d(sa, &tmX, &full_bar[stage], 0, 2 * kb, row0, TMA_EVICT_FIRST);
                         tma_load_3d(sa + TC_A_BYTES, &tmX, &full_bar[stage], 0, 2 * kb + 1, row0, TMA_EVICT_FIRST);
                         tma_load_2d(sa + Cfg::A_BYTES + NQ * 128, &tmQ, &full_bar[stage], kb * Cfg::ELEMS + TC_KBLOCK, 0, TMA_EVICT_LAST);
-                    } else if (MODE == TC_BF16) {
-                        tma_load_3d(sa, &tmX, &full_bar[stage], 0, kb * piece_step, row0, TMA_EVICT_FIRST);
                     } else {
                         tma_load_2d(sa, &tmX, &full_bar[stage], kb * Cfg::ELEMS, row0, TMA_EVICT_FIRST);
                     }
@@ -164,10 +238,8 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
                     const uint64_t adesc = wgmma_desc_sw128(smem_u32(sa + wg * 64 * 128));
                     wgmma_fence();
 #pragma unroll
-                    for (int s = 0; s < 4; ++s) {              // K steps of 32 bytes: 8 tf32 or 16 bf16
-                        if (MODE == TC_TF32) wgmma_tf32_ss<NQ>(acc, adesc + 2 * s, bdesc + 2 * s, (uint32_t)((kb | s) != 0));
-                        else wgmma_bf16_ss<NQ>(acc, adesc + 2 * s, bdesc + 2 * s, (uint32_t)((kb | s) != 0));
-                    }
+                    for (int s = 0; s < 4; ++s)                // K steps of 32 bytes: 8 tf32
+                        wgmma_tf32_ss<NQ>(acc, adesc + 2 * s, bdesc + 2 * s, (uint32_t)((kb | s) != 0));
                     wgmma_commit();
                     wgmma_wait<0>();
                 }
@@ -186,61 +258,126 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
                 xn[h] = CUDART_INF_F;
                 if (row < n_rows && (alive == nullptr || bit_test(alive, (uint32_t)row))) xn[h] = xnorm[row];
             }
-            if (DUMP) {
-                if (dump_min) {
-                    // threshold sampling: per query only the MINIMUM over this warp's 16 rows is kept -- the few smallest
-                    // values of the sample, which is all the threshold needs, survive
-                    const int64_t grp = lt * (TC_TILE_M / TC_DUMP_GROUP) + 4 * wg + w;
+            tc_epilogue<R, DUMP>(acc, xn, r_lo, 0, g, q, tile_row0, s_thr, cand_count, cand_rows, cap, dump, S, dump_min,
+                                 lt * (TC_TILE_M / TC_DUMP_GROUP) + 4 * wg + w, lt * TC_TILE_M);
+        }
+    }
+}
+
+// The bf16 prune pass on 192-row tiles.  A stage's query rows come from L2 once per tile, so a taller tile reads fewer
+// query bytes per corpus byte: NQ / 192 instead of NQ / 128.  The accumulators bound the tile: 192 x NQ fp32 over 256
+// threads is 3 NQ / 4 registers per thread, which leaves no registers for a separate producer warp (ptxas holds every
+// thread of the kernel to 65536 / threads, whatever setmaxnreg says).  So both warpgroups compute:
+//   warpgroup wg: tile rows [64 wg, 64 wg + 64) x all NQ queries                (m64nNQ,     acc0: NQ / 2 per thread)
+//                 tile rows [128, 192)         x queries [wg NQ/2, wg NQ/2 + NQ/2) (m64n(NQ/2), acc1: NQ / 4 per thread)
+// and thread 0 issues the TMA loads, across tile boundaries.  One wgmma group stays in flight: a warp releases the stage of
+// k-block i - 1 once it has issued k-block i's group and group i - 1 has completed, and thread 0 then refills that stage
+// with k-block i - 1 + STAGES.  This cannot deadlock: thread 0 waits on `empty` only for a stage its own warp has already
+// released, and the other warps' releases of k-block i - 1 need only `full` of k-block i, loaded before, never further
+// progress of thread 0.  Every (row, query) product is the same wgmma k16 sequence as a 128-row tile's: the same operands
+// in the same order.
+template <int NQ, bool DUMP>
+__global__ void __launch_bounds__(TC16_THREADS, 1)
+dense_tc_bf16_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmQ, int64_t n_rows,
+                     int kblocks /*stages per tile*/, int piece_step /*128-byte pieces per k-block*/, int64_t n_ltiles,
+                     int row_step /*first rows of consecutive tiles*/, const float* __restrict__ xnorm, const uint32_t* __restrict__ alive,
+                     const float* __restrict__ thr_g, uint32_t* __restrict__ cand_count, uint32_t* __restrict__ cand_rows,
+                     int cap, float* __restrict__ dump, int64_t S, int dump_min)
+{
+    using Cfg = Tc16Cfg<NQ>;
+    constexpr int R0 = NQ / 2, R1 = NQ / 4;    // accumulators per thread: the warpgroup's own 64 rows, the shared 64 rows
+    extern __shared__ unsigned char tc_smem_raw[];
+    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~(uintptr_t)1023);
+    unsigned char* tail = smem + (size_t)Cfg::STAGES * Cfg::STAGE_BYTES;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);            // [STAGES] producer arrival + TMA bytes
+    uint64_t* empty_bar = full_bar + Cfg::STAGES;                       // [STAGES] one arrival per warp
+    float* s_thr = reinterpret_cast<float*>(tail + Cfg::BAR_BYTES);     // [NQ]
+    static_assert(2 * Cfg::STAGES * 8 <= Cfg::BAR_BYTES, "barrier area too small");
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = warp >> 2, w = warp & 3, g = lane >> 2, q = lane & 3;
+    const int r0 = 64 * wg + 16 * w + g;        // acc0 rows r0, r0 + 8
+    const int r1 = 128 + 16 * w + g;            // acc1 rows r1, r1 + 8
+    const int q1 = wg * (NQ / 2);               // acc1's first query
+
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&tmX);
+        tma_prefetch_desc(&tmQ);
+        for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
+        fence_barrier_init();
+    }
+    // s_thr[j] = thr_j / 2:  a = |x|^2 - 2 x.q < thr_j   <=>   x.q + thr_j/2 > |x|^2/2
+    if (!DUMP) for (int j = threadIdx.x; j < NQ; j += TC16_THREADS) s_thr[j] = 0.5f * thr_g[j];
+    __syncthreads();
+
+    // producer state (thread 0): the next k-block to load, flattened over this CTA's tiles
+    int64_t p_lt = blockIdx.x;
+    int p_kb = 0, p_stage = 0;
+    uint32_t p_phase = 0;
+    auto produce = [&]() {
+        if (p_lt >= n_ltiles) return;
+        mbar_wait(&empty_bar[p_stage], p_phase ^ 1);
+        unsigned char* sa = smem + (size_t)p_stage * Cfg::STAGE_BYTES;
+        mbar_expect_tx(&full_bar[p_stage], Cfg::STAGE_BYTES);
+        tma_load_3d(sa, &tmX, &full_bar[p_stage], 0, p_kb * piece_step, (int)(p_lt * row_step), TMA_EVICT_FIRST);
+        tma_load_2d(sa + Cfg::A_BYTES, &tmQ, &full_bar[p_stage], p_kb * Cfg::ELEMS, 0, TMA_EVICT_LAST);
+        if (++p_stage == Cfg::STAGES) { p_stage = 0; p_phase ^= 1; }
+        if (++p_kb == kblocks) { p_kb = 0; p_lt += gridDim.x; }
+    };
+    if (threadIdx.x == 0)
+        for (int i = 0; i < Cfg::STAGES; ++i) produce();
+    // this warp is done with `stage`: release it, and thread 0 refills it
+    auto release = [&](int stage) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);
+        if (threadIdx.x == 0) produce();
+        __syncwarp();
+    };
+
+    float acc0[R0], acc1[R1];
+    int stage = 0, prev = 0; uint32_t phase = 0;
+    for (int64_t lt = blockIdx.x; lt < n_ltiles; lt += gridDim.x) {
+        const int64_t tile_row0 = lt * row_step;
+        float xn0[2], xn1[2];
+        for (int kb = 0; kb < kblocks; ++kb) {
+            if (kb == kblocks - 1) {   // the epilogue's row norms, loaded while the last k-block lands and multiplies
 #pragma unroll
-                    for (int i = 0; i < R / 4; ++i) {
-#pragma unroll
-                        for (int c = 0; c < 2; ++c) {
-                            float v = fminf(fmaf(-2.f, acc[4 * i + c], xn[0]), fmaf(-2.f, acc[4 * i + 2 + c], xn[1]));
-                            v = fminf(v, __shfl_xor_sync(0xffffffffu, v, 4));
-                            v = fminf(v, __shfl_xor_sync(0xffffffffu, v, 8));
-                            v = fminf(v, __shfl_xor_sync(0xffffffffu, v, 16));
-                            if (g == 0) dump[(int64_t)(8 * i + 2 * q + c) * S + grp] = v;
-                        }
-                    }
-                } else {
-#pragma unroll
-                    for (int i = 0; i < R / 4; ++i)
-#pragma unroll
-                        for (int h = 0; h < 2; ++h)
-#pragma unroll
-                            for (int c = 0; c < 2; ++c)
-                                dump[(int64_t)(8 * i + 2 * q + c) * S + lt * TC_TILE_M + r_lo + 8 * h] =
-                                    fmaf(-2.f, acc[4 * i + 2 * h + c], xn[h]);
-                }
-            } else {
-                // ~2 instructions per (row, query) pair on the common path: one add and one max; hits are ~1 in 20000
-                const float half0 = 0.5f * xn[0], half1 = 0.5f * xn[1];
-                float mx0 = -CUDART_INF_F, mx1 = -CUDART_INF_F;
-#pragma unroll
-                for (int i = 0; i < R / 4; ++i) {
-                    const float2 t = *reinterpret_cast<const float2*>(s_thr + 8 * i + 2 * q);
-                    acc[4 * i + 0] += t.x; acc[4 * i + 1] += t.y; acc[4 * i + 2] += t.x; acc[4 * i + 3] += t.y;
-                    mx0 = fmaxf(mx0, fmaxf(acc[4 * i + 0], acc[4 * i + 1]));
-                    mx1 = fmaxf(mx1, fmaxf(acc[4 * i + 2], acc[4 * i + 3]));
-                }
-                if (mx0 > half0 || mx1 > half1) {   // rare: some pair passes  x.q + thr/2 > |x|^2/2
-#pragma unroll
-                    for (int i = 0; i < R / 4; ++i) {
-#pragma unroll
-                        for (int h = 0; h < 2; ++h) {
-#pragma unroll
-                            for (int c = 0; c < 2; ++c) {
-                                if (acc[4 * i + 2 * h + c] > (h ? half1 : half0)) {
-                                    const int j = 8 * i + 2 * q + c;
-                                    const uint32_t pos = atomicAdd(&cand_count[j], 1u);
-                                    if (pos < (uint32_t)cap) cand_rows[(size_t)j * cap + pos] = (uint32_t)(tile_row0 + r_lo + 8 * h);
-                                }
-                            }
-                        }
-                    }
+                for (int h = 0; h < 2; ++h) {
+                    const int64_t ra = tile_row0 + r0 + 8 * h, rb = tile_row0 + r1 + 8 * h;
+                    xn0[h] = (ra < n_rows && (alive == nullptr || bit_test(alive, (uint32_t)ra))) ? xnorm[ra] : CUDART_INF_F;
+                    xn1[h] = (rb < n_rows && (alive == nullptr || bit_test(alive, (uint32_t)rb))) ? xnorm[rb] : CUDART_INF_F;
                 }
             }
+            mbar_wait(&full_bar[stage], phase);
+            unsigned char* sa = smem + (size_t)stage * Cfg::STAGE_BYTES;
+            const uint64_t adesc0 = wgmma_desc_sw128(smem_u32(sa + wg * 64 * 128));
+            const uint64_t adesc1 = wgmma_desc_sw128(smem_u32(sa + 128 * 128));
+            const uint64_t bdesc0 = wgmma_desc_sw128(smem_u32(sa + Cfg::A_BYTES));
+            const uint64_t bdesc1 = wgmma_desc_sw128(smem_u32(sa + Cfg::A_BYTES + q1 * 128));
+            wgmma_fence();
+#pragma unroll
+            for (int s = 0; s < 4; ++s) {              // K steps of 32 bytes: 16 bf16
+                wgmma_bf16_ss<NQ>(acc0, adesc0 + 2 * s, bdesc0 + 2 * s, (uint32_t)((kb | s) != 0));
+                wgmma_bf16_ss<NQ / 2>(acc1, adesc1 + 2 * s, bdesc1 + 2 * s, (uint32_t)((kb | s) != 0));
+            }
+            wgmma_commit();
+            if (kb > 0) {
+                wgmma_wait<1>();                       // k-block kb - 1's group is done with its stage
+                release(prev);
+            }
+            prev = stage;
+            if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
         }
+        wgmma_wait<0>();
+        wgmma_fence_operands<R0>(acc0);
+        wgmma_fence_operands<R1>(acc1);
+        release(prev);
+        // 12 dump groups of 16 rows per tile: 4 wg + w for acc0, 8 + w for acc1 (each warpgroup writes half its queries)
+        const int64_t grp0 = lt * (TC16_TILE_M / TC_DUMP_GROUP);
+        tc_epilogue<R0, DUMP>(acc0, xn0, r0, 0, g, q, tile_row0, s_thr, cand_count, cand_rows, cap, dump, S, dump_min,
+                              grp0 + 4 * wg + w, tile_row0);
+        tc_epilogue<R1, DUMP>(acc1, xn1, r1, q1, g, q, tile_row0, s_thr, cand_count, cand_rows, cap, dump, S, dump_min,
+                              grp0 + 8 + w, tile_row0);
     }
 }
 
@@ -601,16 +738,16 @@ static bool make_map(CUtensorMap* tm, const void* base, int64_t rows, int dpad, 
 }
 
 // 3-D map over 128-byte pieces of 64 halves: piece p of row r at base + r * row_bytes + 128 p; box = one piece of
-// TC_TILE_M rows, 128B swizzle (the shared-memory image of a bf16 box of make_map).  bf16 rows: dpad / 64 pieces of 2 dpad
-// bytes; split rows: split_pieces(dpad) pieces of 4 dpad bytes.
+// box_rows rows (the pass's tile), 128B swizzle (the shared-memory image of a bf16 box of make_map).  bf16 rows: dpad / 64
+// pieces of 2 dpad bytes; split rows: split_pieces(dpad) pieces of 4 dpad bytes.
 // Split rows promote L2 fills to 128 B only: a 256-byte promotion would fetch the low halves beside every high-half piece.
-static bool make_map_pieces(CUtensorMap* tm, const void* base, int64_t rows, int dpad, bool split)
+static bool make_map_pieces(CUtensorMap* tm, const void* base, int64_t rows, int dpad, bool split, int box_rows)
 {
     EncodeTiledFn enc = get_encode();
     if (!enc) return false;
     cuuint64_t gdim[3] = {(cuuint64_t)SPLIT_BLOCK, (cuuint64_t)(split ? split_pieces(dpad) : dpad / 64), (cuuint64_t)rows};
     cuuint64_t gstride[2] = {128, (cuuint64_t)dpad * (split ? 4 : 2)};
-    cuuint32_t box[3] = {(cuuint32_t)SPLIT_BLOCK, 1, (cuuint32_t)TC_TILE_M};
+    cuuint32_t box[3] = {(cuuint32_t)SPLIT_BLOCK, 1, (cuuint32_t)box_rows};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), gdim, gstride, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
@@ -623,7 +760,8 @@ constexpr int64_t TC_MIN_ROWS = 262144;   // below this the exact scan is cheape
 
 bool dense_tc_supported(const DeviceInfo& di, int dpad)
 {
-    return di.cc_major == 9 && dpad % TC_KBLOCK == 0 && di.smem_optin >= TcCfg<256, TC_TF32S>::SMEM && get_encode() != nullptr;
+    const size_t smem = TcCfg<256, TC_TF32S>::SMEM > Tc16Cfg<256>::SMEM ? TcCfg<256, TC_TF32S>::SMEM : Tc16Cfg<256>::SMEM;
+    return di.cc_major == 9 && dpad % TC_KBLOCK == 0 && di.smem_optin >= smem && get_encode() != nullptr;
 }
 
 static int tc_target(int P, bool bf16 = false)
@@ -708,13 +846,9 @@ static float certify_slack_rel(int dpad)
 static std::atomic<int64_t> g_host_rows_fetched{0};
 int64_t host_rows_fetched() { return g_host_rows_fetched.load(); }
 
-// TC_BF16 k-block step in 128-byte pieces: split rows interleave high- and low-half pieces, a bf16 copy holds only bf16 pieces
-static int tc_bf16_piece_step(bool split) { return split ? 2 : 1; }
-
-// one launch of the prune kernel (sample pass: DUMP) over n_ltiles tiles of 128 rows, tile_stride apart; TC_BF16 reads
-// tmX = make_map_pieces, piece_step 2 on split rows (their high halves), 1 on bf16 rows
+// one launch of a prune kernel (sample pass: DUMP) over n_ltiles tiles, tile_stride apart
 template <int NQ, int MODE, bool DUMP>
-static void tc_launch(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensorMap& tmQ, int64_t n_rows, int dpad, int piece_step,
+static void tc_launch(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensorMap& tmQ, int64_t n_rows, int dpad,
                       int64_t n_ltiles, int tile_stride, const float* xnorm, const uint32_t* alive, const float* thr,
                       uint32_t* cand_count, uint32_t* cand_rows, int cap, float* dump, int64_t S, int dump_min, cudaStream_t st)
 {
@@ -725,8 +859,30 @@ static void tc_launch(const DeviceInfo& di, const CUtensorMap& tmX, const CUtens
         attr_set = true;
     }
     const int grid = (int)(n_ltiles < di.sm_count ? n_ltiles : di.sm_count);
-    dense_tc_kernel<NQ, MODE, DUMP><<<grid, TC_THREADS, Cfg::SMEM, st>>>(tmX, tmQ, n_rows, dpad / Cfg::ELEMS, piece_step, n_ltiles, tile_stride,
+    dense_tc_kernel<NQ, MODE, DUMP><<<grid, TC_THREADS, Cfg::SMEM, st>>>(tmX, tmQ, n_rows, dpad / Cfg::ELEMS, n_ltiles, tile_stride,
                                                                          xnorm, alive, thr, cand_count, cand_rows, cap, dump, S, dump_min);
+}
+// one launch of the bf16 kernel over the high halves of split rows (split) or over bf16 rows, with the nq bf16 queries qh:
+// n_ltiles tiles, row_step rows apart.  A k-block steps 2 pieces on split rows (high- and low-half pieces interleave), 1 on
+// bf16 rows
+template <int NQ, bool DUMP>
+static void tc16_launch(const DeviceInfo& di, const void* rows, bool split, const uint16_t* qh, int nq, int64_t n_rows, int dpad,
+                        int64_t n_ltiles, int row_step, const float* xnorm, const uint32_t* alive, const float* thr,
+                        uint32_t* cand_count, uint32_t* cand_rows, int cap, float* dump, int64_t S, int dump_min, cudaStream_t st)
+{
+    using Cfg = Tc16Cfg<NQ>;
+    CUtensorMap tmX, tmQ;
+    if (!make_map(&tmQ, (const void*)qh, nq, dpad, NQ, true) || !make_map_pieces(&tmX, rows, n_rows, dpad, split, TC16_TILE_M))
+        throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled(bf16 pass)", __FILE__, __LINE__};
+    static bool attr_set = false;
+    if (!attr_set) {
+        KRAG_CUDA(cudaFuncSetAttribute(dense_tc_bf16_kernel<NQ, DUMP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM));
+        attr_set = true;
+    }
+    const int grid = (int)(n_ltiles < di.sm_count ? n_ltiles : di.sm_count);
+    dense_tc_bf16_kernel<NQ, DUMP><<<grid, TC16_THREADS, Cfg::SMEM, st>>>(tmX, tmQ, n_rows, dpad / Cfg::ELEMS, split ? 2 : 1, n_ltiles,
+                                                                          row_step, xnorm, alive, thr, cand_count, cand_rows,
+                                                                          cap, dump, S, dump_min);
 }
 
 template <int NQ>
@@ -736,26 +892,24 @@ static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensor
                     const uint16_t* Xh, bool split, bool allow_bf16, const HostRowsView* hr, cudaStream_t st)
 {
     const bool host = hr != nullptr;             // fp32 rows in pinned host memory: both passes read the bf16 copy Xh
-    // bf16 operands in the prune pass: a bf16 copy Xh (shadow, host rows) or the high halves of split rows (tmX)
+    // bf16 operands in the prune pass: a bf16 copy Xh (shadow, host rows) or the high halves of split rows (X)
     const bool bf16 = Xh != nullptr || (split && allow_bf16);
-    const int64_t n_tiles = (n_rows + TC_TILE_M - 1) / TC_TILE_M;
-    const int64_t s_tiles = tc_sample_tiles(n_rows);
-    // 1. sample pass (1/64 of the tiles), dump a = |x|^2 - 2 x.q
+    // 1. sample pass, dump a = |x|^2 - 2 x.q: one tile at the start of every TC_SAMPLE_STRIDE 128-row tiles, so every pass
+    // samples the same rows first; bf16 on host rows (192-row tiles), TF32 otherwise (128-row tiles)
     // the dump holds one value per (16-row group of a sampled tile, query): S_min per query
-    const int64_t S_min = s_tiles * (TC_TILE_M / TC_DUMP_GROUP);
+    const int sample_m = host ? TC16_TILE_M : TC_TILE_M;
+    const int64_t s_tiles = tc_sample_tiles(n_rows);
+    const int64_t S_min = s_tiles * (sample_m / TC_DUMP_GROUP);
     (void)S;
     if (host) {   // the sample pass only chooses thr: bf16 operands do not enter soundness
-        CUtensorMap tmQh, tmXh;
         launch_f32_to_bf16(q, w.q_bf16, (int64_t)nq * dpad, st);
-        if (!make_map(&tmQh, (const void*)w.q_bf16, nq, dpad, NQ, true) || !make_map_pieces(&tmXh, Xh, n_rows, dpad, false))
-            throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled(bf16 rows)", __FILE__, __LINE__};
-        tc_launch<NQ, TC_BF16, true>(di, tmXh, tmQh, n_rows, dpad, 1, s_tiles, TC_SAMPLE_STRIDE, xnorm, alive, nullptr, nullptr, nullptr, 0,
-                                     w.dump, S_min, 1, st);
+        tc16_launch<NQ, true>(di, Xh, false, w.q_bf16, nq, n_rows, dpad, s_tiles, TC_SAMPLE_STRIDE * TC_TILE_M, xnorm, alive,
+                              nullptr, nullptr, nullptr, 0, w.dump, S_min, 1, st);
     } else if (split) {
-        tc_launch<NQ, TC_TF32S, true>(di, tmX, tmQ, n_rows, dpad, 2, s_tiles, TC_SAMPLE_STRIDE, xnorm, alive, nullptr, nullptr, nullptr, 0,
+        tc_launch<NQ, TC_TF32S, true>(di, tmX, tmQ, n_rows, dpad, s_tiles, TC_SAMPLE_STRIDE, xnorm, alive, nullptr, nullptr, nullptr, 0,
                                       w.dump, S_min, 1, st);
     } else {
-        tc_launch<NQ, TC_TF32, true>(di, tmX, tmQ, n_rows, dpad, 1, s_tiles, TC_SAMPLE_STRIDE, xnorm, alive, nullptr, nullptr, nullptr, 0,
+        tc_launch<NQ, TC_TF32, true>(di, tmX, tmQ, n_rows, dpad, s_tiles, TC_SAMPLE_STRIDE, xnorm, alive, nullptr, nullptr, nullptr, 0,
                                      w.dump, S_min, 1, st);
     }
     KRAG_CUDA(cudaGetLastError());
@@ -764,7 +918,7 @@ static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensor
     int64_t sampled_rows = 0;
     for (int64_t t = 0; t < s_tiles; ++t) {
         int64_t r0 = t * TC_SAMPLE_STRIDE * TC_TILE_M;
-        sampled_rows += (r0 + TC_TILE_M <= n_rows) ? TC_TILE_M : (n_rows > r0 ? n_rows - r0 : 0);
+        sampled_rows += (r0 + sample_m <= n_rows) ? sample_m : (n_rows > r0 ? n_rows - r0 : 0);
     }
     int m = (int)((double)tc_target(P, bf16) * (double)sampled_rows / (double)n_rows + 0.5);
     if (m < 4) m = 4;
@@ -783,24 +937,15 @@ static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensor
     // kernel ids: 6 host rows' bf16 copy, 4 bf16 shadow, 5 high halves of split rows, 3 tf32
     dense_timer_begin(st, host ? 6 : (Xh ? 4 : (bf16 ? 5 : 3)), n_rows * (int64_t)dpad * (bf16 ? 2 : 4), 2 * (int64_t)NQ * n_rows * dpad);
     if (bf16) {
-        CUtensorMap tmQh, tmXh;
-        if (!make_map(&tmQh, (const void*)w.q_bf16, nq, dpad, NQ, true))
-            throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled(Q, bf16)", __FILE__, __LINE__};
-        if (Xh) {
-            if (!make_map_pieces(&tmXh, Xh, n_rows, dpad, false))
-                throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled(bf16 rows)", __FILE__, __LINE__};
-            tc_launch<NQ, TC_BF16, false>(di, tmXh, tmQh, n_rows, dpad, tc_bf16_piece_step(false), n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap,
-                                          nullptr, 0, 0, st);
-        } else {
-            tc_launch<NQ, TC_BF16, false>(di, tmX, tmQh, n_rows, dpad, tc_bf16_piece_step(true), n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap,
-                                          nullptr, 0, 0, st);
-        }
-    } else if (split) {
-        tc_launch<NQ, TC_TF32S, false>(di, tmX, tmQ, n_rows, dpad, 2, n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap,
-                                       nullptr, 0, 0, st);
+        const int64_t n_tiles = (n_rows + TC16_TILE_M - 1) / TC16_TILE_M;
+        tc16_launch<NQ, false>(di, Xh ? (const void*)Xh : (const void*)X, Xh == nullptr, w.q_bf16, nq, n_rows, dpad, n_tiles,
+                               TC16_TILE_M, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap, nullptr, 0, 0, st);
     } else {
-        tc_launch<NQ, TC_TF32, false>(di, tmX, tmQ, n_rows, dpad, 1, n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap,
-                                      nullptr, 0, 0, st);
+        const int64_t n_tiles = (n_rows + TC_TILE_M - 1) / TC_TILE_M;
+        if (split) tc_launch<NQ, TC_TF32S, false>(di, tmX, tmQ, n_rows, dpad, n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows,
+                                                  cap, nullptr, 0, 0, st);
+        else tc_launch<NQ, TC_TF32, false>(di, tmX, tmQ, n_rows, dpad, n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows,
+                                           cap, nullptr, 0, 0, st);
     }
     dense_timer_end(st);
     KRAG_CUDA(cudaGetLastError());
@@ -866,7 +1011,7 @@ bool launch_dense_tc(const DeviceInfo& di, const float* X, int64_t n_rows, int d
     TcWorkspace w;
     if (tc_carve(&w, (unsigned char*)workspace, cap, S) > workspace_bytes) return false;
     CUtensorMap tmX;
-    if (!(split ? make_map_pieces(&tmX, X, n_rows, dpad, true) : make_map(&tmX, X, n_rows, dpad, TC_TILE_M))) return false;
+    if (!(split ? make_map_pieces(&tmX, X, n_rows, dpad, true, TC_TILE_M) : make_map(&tmX, X, n_rows, dpad, TC_TILE_M))) return false;
     std::vector<int32_t> flags(256);
     for (int b0 = 0; b0 < batch; b0 += 256) {
         const int nq = batch - b0 < 256 ? batch - b0 : 256;
@@ -936,6 +1081,7 @@ bool launch_dense_tc_host(const DeviceInfo& di, const HostRowsView& hr, int64_t 
     return true;
 }
 
+// the dump's columns: the rows rounded up to 128 for every pass (the bf16 passes' dump covers them with 192-row tiles)
 size_t dense_tc_debug_carve(TcDebugWs* w, unsigned char* base, int64_t n_rows, int dpad, int nq, int cap, int64_t* S_out,
                             int* nq_pad_out)
 {
@@ -960,14 +1106,14 @@ size_t dense_tc_debug_carve(TcDebugWs* w, unsigned char* base, int64_t n_rows, i
 
 template <int NQ, int MODE>
 static void tc_debug_launch(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensorMap& tmQ, int64_t n_rows, int dpad,
-                            int piece_step, const float* xnorm, const uint32_t* alive, const TcDebugWs& w, int cap, cudaStream_t st)
+                            const float* xnorm, const uint32_t* alive, const TcDebugWs& w, int cap, cudaStream_t st)
 {
     const int64_t n_tiles = (n_rows + TC_TILE_M - 1) / TC_TILE_M;
-    if (cap == 0)   // as the host-rows sample pass, but over every tile and every row (dump_min = 0)
-        tc_launch<NQ, MODE, true>(di, tmX, tmQ, n_rows, dpad, piece_step, n_tiles, 1, xnorm, nullptr, nullptr, nullptr, nullptr, 0,
+    if (cap == 0)   // as a sample pass, but over every tile and every row (dump_min = 0)
+        tc_launch<NQ, MODE, true>(di, tmX, tmQ, n_rows, dpad, n_tiles, 1, xnorm, nullptr, nullptr, nullptr, nullptr, 0,
                                   w.dump, n_tiles * TC_TILE_M, 0, st);
     else            // the main pass of tc_pass
-        tc_launch<NQ, MODE, false>(di, tmX, tmQ, n_rows, dpad, piece_step, n_tiles, 1, xnorm, alive, w.thr, w.cand_count,
+        tc_launch<NQ, MODE, false>(di, tmX, tmQ, n_rows, dpad, n_tiles, 1, xnorm, alive, w.thr, w.cand_count,
                                    w.cand_rows, cap, nullptr, 0, 0, st);
 }
 
@@ -975,21 +1121,26 @@ template <int NQ>
 static bool tc_debug_pass(const DeviceInfo& di, int pass, const float* X, const uint16_t* Xh, bool split, int64_t n_rows, int dpad,
                           const float* xnorm, const uint32_t* alive, const float* q, int nq, const TcDebugWs& w, int cap, cudaStream_t st)
 {
-    CUtensorMap tmX, tmQ;
     if (pass == 0) {   // TF32: fp32 queries straight from the caller's rows
-        if (!(split ? make_map_pieces(&tmX, X, n_rows, dpad, true) : make_map(&tmX, X, n_rows, dpad, TC_TILE_M)) ||
+        CUtensorMap tmX, tmQ;
+        if (!(split ? make_map_pieces(&tmX, X, n_rows, dpad, true, TC_TILE_M) : make_map(&tmX, X, n_rows, dpad, TC_TILE_M)) ||
             !make_map(&tmQ, q, nq, dpad, NQ))
             return false;
-        if (split) tc_debug_launch<NQ, TC_TF32S>(di, tmX, tmQ, n_rows, dpad, 2, xnorm, alive, w, cap, st);
-        else tc_debug_launch<NQ, TC_TF32>(di, tmX, tmQ, n_rows, dpad, 1, xnorm, alive, w, cap, st);
+        if (split) tc_debug_launch<NQ, TC_TF32S>(di, tmX, tmQ, n_rows, dpad, xnorm, alive, w, cap, st);
+        else tc_debug_launch<NQ, TC_TF32>(di, tmX, tmQ, n_rows, dpad, xnorm, alive, w, cap, st);
         return true;
     }
     // bf16: the queries converted as tc_pass converts them for the same rows
     if (pass == 1) launch_bf16_split_order(q, w.q_bf16, (int64_t)nq * dpad, st);
     else launch_f32_to_bf16(q, w.q_bf16, (int64_t)nq * dpad, st);
-    if (!make_map(&tmQ, (const void*)w.q_bf16, nq, dpad, NQ, true)) return false;
-    if (!(pass == 1 ? make_map_pieces(&tmX, X, n_rows, dpad, true) : make_map_pieces(&tmX, Xh, n_rows, dpad, false))) return false;
-    tc_debug_launch<NQ, TC_BF16>(di, tmX, tmQ, n_rows, dpad, tc_bf16_piece_step(pass == 1), xnorm, alive, w, cap, st);
+    const void* rows = pass == 1 ? (const void*)X : (const void*)Xh;
+    const int64_t S = (n_rows + TC_TILE_M - 1) / TC_TILE_M * TC_TILE_M;
+    if (cap == 0)   // as the host-rows sample pass, but over every row and the padding columns up to S (dump_min = 0)
+        tc16_launch<NQ, true>(di, rows, pass == 1, w.q_bf16, nq, n_rows, dpad, (S + TC16_TILE_M - 1) / TC16_TILE_M, TC16_TILE_M,
+                              xnorm, nullptr, nullptr, nullptr, nullptr, 0, w.dump, S, 0, st);
+    else
+        tc16_launch<NQ, false>(di, rows, pass == 1, w.q_bf16, nq, n_rows, dpad, (n_rows + TC16_TILE_M - 1) / TC16_TILE_M, TC16_TILE_M, xnorm,
+                               alive, w.thr, w.cand_count, w.cand_rows, cap, nullptr, 0, 0, st);
     return true;
 }
 
