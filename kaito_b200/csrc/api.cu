@@ -21,7 +21,6 @@
 #include "common.cuh"
 #include "embed_config.h"
 #include "engine.h"
-#include "split_rows.cuh"
 
 namespace krag {
 
@@ -157,18 +156,9 @@ struct CommitPrep {
 struct krag_index {
     krag_ctx* ctx = nullptr;
     std::string name;
-    int dim = 0, dpad = 0;
     std::shared_mutex mu;
-    // dense shard
-    bool host_rows = false;         // KRAG_ROWS_HOST: the fp32 rows are Xp (pinned host memory) and X stays empty
-    DevArray<float> X;              // device-resident rows [rows, dpad], zero padded; split rows (split_rows.cuh) when split_rows
-    bool split_rows = false;
-    HostArray<float> Xp;            // host-resident fp32 rows [rows, dpad], zero padded
-    DevArray<float> xnorm;          // |x|^2 per row (K2 epilogue), from the fp32 rows in either storage
-    DevArray<uint16_t> Xh;          // bf16 copy of the rows: optional shadow (KRAG_DENSE_TC_BF16), always present for host rows
-    DevArray<float> xres;           // host rows only: |x - bf16(x)| per row, rounded up (refine bound)
-    DevArray<uint32_t> xn_max;      // [1] bits of max |x|^2 (K2 certificate)
-    int64_t n_rows = 0, n_live = 0;
+    DenseRows rows;                 // the dense shard; rows.n is the index's row count
+    int64_t n_live = 0;
     std::vector<uint32_t> alive_h;
     DevArray<uint32_t> alive_d;
     bool has_dead = false;
@@ -269,7 +259,7 @@ void wait_issued_searches(const krag_index* ix)
 
 const uint32_t* alive_ptr(const krag_index* ix) { return ix->has_dead ? ix->alive_d.p : nullptr; }
 OrdMap ord_map(const krag_index* ix) { return OrdMap{(uint32_t)ix->ord_base, (uint32_t)ix->ord_stride}; }
-int64_t ord_last(const krag_index* ix) { return ix->ord_base + (ix->n_rows > 0 ? (ix->n_rows - 1) * ix->ord_stride : 0); }
+int64_t ord_last(const krag_index* ix) { return ix->ord_base + (ix->rows.n > 0 ? (ix->rows.n - 1) * ix->ord_stride : 0); }
 
 // every call on an index except the redeal session's own and drop: refused while a session is open or after a failed one
 void require_idle(const krag_index* ix)
@@ -282,7 +272,7 @@ void check_P(int P) { KRAG_REQUIRE(P >= 1 && P <= KRAG_MAX_POOL, KRAG_E_INVALID,
 
 // the slot's staging for the streamed scan of a host-rows index, grown to this call's shape on st, the stream the lease
 // ordered after the slot's previous user.  copy_st needs no wait of its own: every copy into a staging buffer waits for a
-// `freed` event recorded on st (launch_dense_scan_streamed).
+// `freed` event recorded on st (launch_dense_scan).
 ScanStaging scan_staging(const krag_index* ix, Slot* s, int batch, int P, cudaStream_t st)
 {
     if (!s->copy_st) {
@@ -290,55 +280,47 @@ ScanStaging scan_staging(const krag_index* ix, Slot* s, int batch, int P, cudaSt
         for (cudaEvent_t* e : {&s->copied[0], &s->copied[1], &s->freed[0], &s->freed[1]})
             KRAG_CUDA(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
     }
-    const int64_t R = stream_scan_chunk_rows(ix->dpad);
-    const int64_t half = (R < ix->n_rows ? R : ix->n_rows) * ix->dpad;
+    const int64_t R = stream_scan_chunk_rows(ix->rows.dpad);
+    const int64_t half = (R < ix->rows.n ? R : ix->rows.n) * ix->rows.dpad;
     s->stage.reserve(2 * half, 0, st);
     s->fold.reserve(2 * (int64_t)(batch > 256 ? batch : 256) * P, 0, st);
-    s->q_sel.reserve((int64_t)256 * ix->dpad, 0, st);
+    s->q_sel.reserve((int64_t)256 * ix->rows.dpad, 0, st);
     s->k_sel.reserve((int64_t)256 * P, 0, st);
     return ScanStaging{{s->stage.p, s->stage.p + half}, R, s->copy_st, {s->copied[0], s->copied[1]}, {s->freed[0], s->freed[1]},
                        s->fold.p, s->q_sel.p, s->k_sel.p};
 }
 
-// dense candidates for device-resident padded queries
+// dense candidates for device-resident padded queries: the dense mode's choice of kernel, then K2 or K1
 void dense_candidates_dev(krag_index* ix, Slot* s, const float* d_q, int batch, int P, uint64_t* d_keys, cudaStream_t st,
                           const uint32_t* eligible = nullptr)
 {
     krag_ctx* c = ix->ctx;
+    const DenseRows& r = ix->rows;
     const uint32_t* alive = eligible ? eligible : alive_ptr(ix);     // rows the scan may return (tombstones [& filter])
-    if (ix->n_rows == 0) {
+    if (r.n == 0) {
         KRAG_CUDA(cudaMemsetAsync(d_keys, 0xFF, sizeof(uint64_t) * (size_t)batch * P, st));
         return;
     }
     KRAG_REQUIRE(ord_last(ix) < 0xFFFFFFFFll, KRAG_E_UNSUPPORTED, "global ordinal exceeds 32 bits");
     s->part.reserve((int64_t)dense_scan_part_elems(c->di, P), 0, st);
-    int mode = c->cfg.dense_mode;
-    if (ix->host_rows) {
-        const HostRowsView hr{ix->Xp.h, ix->Xp.d, ix->Xh.p, ix->xres.p};
-        const ScanStaging sg = scan_staging(ix, s, batch, P, st);
-        if (mode != KRAG_DENSE_SCAN && dense_tc_host_rows_supported(c->di, ix->n_rows, ix->dpad)) {
-            const size_t ws = dense_tc_workspace_bytes(c->di, ix->n_rows, P, true);
-            s->tc_ws.reserve((int64_t)ws, 0, st);
-            if (launch_dense_tc_host(c->di, hr, ix->n_rows, ix->dpad, alive, ix->xnorm.p, ix->xn_max.p, d_q, batch, P, ord_map(ix),
-                                     s->tc_ws.p, ws, s->part.p, sg, d_keys, st))
-                return;
-        }
-        launch_dense_scan_streamed(c->di, ix->Xp.h, ix->n_rows, ix->dpad, alive, d_q, batch, P, ord_map(ix), s->part.p, sg, d_keys, st);
-        return;
-    }
-    bool use_tc = (mode == KRAG_DENSE_TC) || (mode == KRAG_DENSE_TC_TF32) || (mode == KRAG_DENSE_TC_BF16 && dense_tc_wants(ix->n_rows, batch)) ||
-                  (mode == KRAG_DENSE_AUTO && dense_tc_wants(ix->n_rows, batch));
-    if (use_tc && dense_tc_supported(c->di, ix->dpad)) {
-        size_t ws = dense_tc_workspace_bytes(c->di, ix->n_rows, P);
+    const int mode = c->cfg.dense_mode;
+    ScanStaging sg{};
+    if (r.host()) sg = scan_staging(ix, s, batch, P, st);
+    // host rows: K2 whenever it can serve them (K1 streams every row over the host link); device rows: K2 when forced, or
+    // for the batches and indexes it serves faster
+    const TcOp op = tc_operand(r, mode == KRAG_DENSE_TC_BF16, mode == KRAG_DENSE_TC_TF32);
+    const bool use_tc = (r.host() ? mode != KRAG_DENSE_SCAN
+                                  : mode == KRAG_DENSE_TC || mode == KRAG_DENSE_TC_TF32 ||
+                                        ((mode == KRAG_DENSE_AUTO || mode == KRAG_DENSE_TC_BF16) && dense_tc_wants(r.n, batch))) &&
+                        dense_tc_serves(c->di, r, op);
+    if (use_tc) {
+        const size_t ws = dense_tc_workspace_bytes(c->di, r.n, P, r.host());
         s->tc_ws.reserve((int64_t)ws, 0, st);
-        if (launch_dense_tc(c->di, ix->X.p, ix->n_rows, ix->dpad, alive, ix->xnorm.p, ix->xn_max.p, d_q, batch, P,
-                            ord_map(ix), s->tc_ws.p, ws, s->part.p, d_keys, st,
-                            mode == KRAG_DENSE_TC_BF16 ? ix->Xh.p : nullptr, mode != KRAG_DENSE_TC_TF32, ix->split_rows))
-            return;
+        if (launch_dense_tc(c->di, r, op, alive, d_q, batch, P, ord_map(ix), s->tc_ws.p, ws, s->part.p, &sg, d_keys, st)) return;
     }
-    KRAG_REQUIRE((mode != KRAG_DENSE_TC && mode != KRAG_DENSE_TC_TF32) || !dense_tc_wants(ix->n_rows, 16), KRAG_E_UNSUPPORTED, "tensor-core dense path unavailable for this index/device");
-    launch_dense_scan(c->di, ix->X.p, ix->n_rows, ix->dpad, alive, d_q, batch, P, ord_map(ix),
-                      s->part.p, d_keys, st, ix->split_rows);
+    KRAG_REQUIRE(r.host() || (mode != KRAG_DENSE_TC && mode != KRAG_DENSE_TC_TF32) || !dense_tc_wants(r.n, 16), KRAG_E_UNSUPPORTED,
+                 "tensor-core dense path unavailable for this index/device");
+    launch_dense_scan(c->di, r, alive, d_q, batch, P, ord_map(ix), s->part.p, d_keys, st, &sg);
 }
 
 void bm25_candidates_dev(krag_index* ix, Slot* s, const uint32_t* d_terms, const int32_t* d_toff, int n_terms_total, int batch,
@@ -360,7 +342,7 @@ void bm25_candidates_dev(krag_index* ix, Slot* s, const uint32_t* d_terms, const
 // stage padded queries on the device
 const float* upload_queries(krag_index* ix, Slot* s, const float* q, int batch)
 {
-    const int d = ix->dim, dp = ix->dpad;
+    const int d = ix->rows.dim, dp = ix->rows.dpad;
     s->q.reserve((int64_t)batch * dp, 0, s->st);
     if (d == dp) {
         KRAG_CUDA(cudaMemcpyAsync(s->q.p, q, sizeof(float) * (size_t)batch * d, cudaMemcpyHostToDevice, s->st));
@@ -384,7 +366,7 @@ void upload_terms(Slot* s, const uint32_t* q_terms, const int32_t* q_toff, int b
 
 void mark_alive(krag_index* ix, int64_t row0, int64_t n, cudaStream_t st)
 {
-    int64_t words = (ix->n_rows + n + 31) / 32;
+    int64_t words = (ix->rows.n + n + 31) / 32;
     if ((int64_t)ix->alive_h.size() < words) ix->alive_h.resize((size_t)words, 0u);
     for (int64_t r = row0; r < row0 + n; ++r) ix->alive_h[(size_t)(r >> 5)] |= 1u << (r & 31);
     ix->alive_d.reserve(words, (row0 + 31) / 32, st);
@@ -393,52 +375,13 @@ void mark_alive(krag_index* ix, int64_t row0, int64_t n, cudaStream_t st)
                               cudaMemcpyHostToDevice, st));
 }
 
-void ensure_capacity(krag_index* ix, int64_t rows, int64_t nnz, cudaStream_t st)
+// room for the term lists of `rows` rows and nnz entries
+void reserve_terms(krag_index* ix, int64_t rows, int64_t nnz, cudaStream_t st)
 {
-    if (ix->host_rows) {
-        ix->Xp.reserve(rows * ix->dpad, ix->n_rows * ix->dpad);
-        ix->xres.reserve(rows, ix->n_rows, st);
-    } else {
-        ix->X.reserve(rows * ix->dpad, ix->n_rows * ix->dpad, st);
-    }
-    ix->xnorm.reserve(rows, ix->n_rows, st);
-    if (ix->ctx->cfg.dense_mode == KRAG_DENSE_TC_BF16 || ix->Xh.p || ix->host_rows) ix->Xh.reserve(rows * ix->dpad, ix->n_rows * ix->dpad, st);
-    if (ix->xn_max.p == nullptr) {
-        ix->xn_max.reserve(1, 0, st);
-        KRAG_CUDA(cudaMemsetAsync(ix->xn_max.p, 0, sizeof(uint32_t), st));
-    }
-    if (nnz >= 0) {
-        ix->toff.reserve(rows + 1, ix->n_rows + 1, st);
-        ix->dlen.reserve(rows, ix->n_rows, st);
-        ix->tid.reserve(nnz > 0 ? nnz : 1, ix->nnz, st);
-        ix->ttf.reserve(nnz > 0 ? nnz : 1, ix->nnz, st);
-    }
-}
-
-// Host rows [row0, row0 + n) -> xnorm (row_norms_kernel, as for device rows), the bf16 copy and xres, streamed through a
-// device staging buffer that is freed before returning.  gen_seed != nullptr: the rows are first generated on the device
-// (krag_synth_fill, global rows row_base + r) and copied to the pinned rows; otherwise they are already there.
-void derive_host_rows(krag_index* ix, int64_t row0, int64_t n, cudaStream_t st, const uint64_t* gen_seed = nullptr,
-                      int64_t row_base = 0)
-{
-    if (n == 0) return;
-    const int64_t R = stream_scan_chunk_rows(ix->dpad);
-    const int dp = ix->dpad;
-    DevArray<float> stage;
-    stage.alloc((n < R ? n : R) * dp);
-    for (int64_t r = row0; r < row0 + n; r += R) {
-        const int64_t m = row0 + n - r < R ? row0 + n - r : R;
-        float* host = ix->Xp.h + r * dp;
-        if (gen_seed) {
-            launch_synth_dense(stage.p, m, ix->dim, dp, row_base + r, *gen_seed, st);
-            KRAG_CUDA(cudaMemcpyAsync(host, stage.p, sizeof(float) * (size_t)(m * dp), cudaMemcpyDeviceToHost, st));
-        } else {
-            KRAG_CUDA(cudaMemcpyAsync(stage.p, host, sizeof(float) * (size_t)(m * dp), cudaMemcpyHostToDevice, st));
-        }
-        launch_row_norms(stage.p, 0, m, dp, ix->xnorm.p + r, ix->xn_max.p, st);
-        launch_bf16_residual(stage.p, m, dp, ix->Xh.p + r * dp, ix->xres.p + r, st);
-    }
-    KRAG_CUDA(cudaStreamSynchronize(st));
+    ix->toff.reserve(rows + 1, ix->rows.n + 1, st);
+    ix->dlen.reserve(rows, ix->rows.n, st);
+    ix->tid.reserve(nnz > 0 ? nnz : 1, ix->nnz, st);
+    ix->ttf.reserve(nnz > 0 ? nnz : 1, ix->nnz, st);
 }
 
 // figures of the last commit (krag_last_commit): process-wide, last writer wins
@@ -464,7 +407,7 @@ void commit_prepare(krag_index* ix, int64_t vocab)
     KRAG_CUDA(cudaStreamSynchronize(st));
     const int64_t n_entries = ix->nnz - pr.e0;
     pr.entry_doc.alloc(n_entries > 0 ? n_entries : 1);
-    if (ix->n_rows > row0) launch_expand_entry_doc(ix->toff.p, ix->n_rows - row0, pr.entry_doc.p, st, row0);
+    if (ix->rows.n > row0) launch_expand_entry_doc(ix->toff.p, ix->rows.n - row0, pr.entry_doc.p, st, row0);
     if (pr.merge) {
         count_survivors(ix->post, alive_ptr(ix), vocab, pr.sc, st);
         pr.delta_df.alloc(vocab);
@@ -481,7 +424,7 @@ void commit_prepare(krag_index* ix, int64_t vocab)
 void commit_local_impl(krag_index* ix, int64_t vocab, uint32_t* df_out, int64_t* n_live_out, int64_t* total_len_out)
 {
     cudaStream_t st = ix->ctx->admin;
-    KRAG_REQUIRE(ix->has_sparse || ix->n_rows == 0, KRAG_E_STATE, "index holds no term lists (dense-only)");
+    KRAG_REQUIRE(ix->has_sparse || ix->rows.n == 0, KRAG_E_STATE, "index holds no term lists (dense-only)");
     KRAG_REQUIRE(vocab > 0 && vocab < 0x7fffffffll, KRAG_E_INVALID, "vocab out of range");
     // term ids >= vocab would make the df kernel write out of bounds: the largest id is tracked on the host at add time
     KRAG_REQUIRE(ix->nnz == 0 || vocab > (int64_t)ix->max_term_id, KRAG_E_INVALID,
@@ -497,7 +440,7 @@ void commit_local_impl(krag_index* ix, int64_t vocab, uint32_t* df_out, int64_t*
         if (ix->nnz > 0) launch_df_histogram(ix->tid.p, ix->prep.entry_doc.p, alive_ptr(ix), ix->nnz, df.p, st);
     }
     KRAG_CUDA(cudaMemcpyAsync(df_out, df.p, sizeof(uint32_t) * (size_t)vocab, cudaMemcpyDeviceToHost, st));
-    live_doc_stats(ix->dlen.p, alive_ptr(ix), ix->n_rows, n_live_out, total_len_out, st);
+    live_doc_stats(ix->dlen.p, alive_ptr(ix), ix->rows.n, n_live_out, total_len_out, st);
     ix->prep.ms = ms_since(t0);
 }
 
@@ -551,8 +494,8 @@ Postings merge_postings(krag_index* ix, int64_t vocab, const float* idf, double 
     out.doc.alloc(nnz > 0 ? nnz : 1);
     out.tf.alloc(nnz > 0 ? nnz : 1);
     out.score.alloc(nnz > 0 ? nnz : 1);
-    if (nnz > 0) prepare_tile_index(out.off.p, vocab, ix->n_rows, out, st);
-    else empty_tile_index(vocab, ix->n_rows, out);
+    if (nnz > 0) prepare_tile_index(out.off.p, vocab, ix->rows.n, out, st);
+    else empty_tile_index(vocab, ix->rows.n, out);
     write_survivors(ix->post, alive_ptr(ix), pr.sc, out.off.p, nullptr, ix->dlen.p, idf, avgdl, out, st);
     if (n_entries > 0)
         sort_entries_by_term(ix->tid.p + pr.e0, ix->ttf.p + pr.e0, pr.entry_doc.p, alive_ptr(ix), n_entries, vocab, h_delta_off,
@@ -568,7 +511,7 @@ void commit_global_impl(krag_index* ix, int64_t vocab, const uint32_t* df_global
                         int64_t total_len_global, int64_t ord_base)
 {
     cudaStream_t st = ix->ctx->admin;
-    KRAG_REQUIRE(ord_base >= 0 && ord_base + ix->n_rows * ix->ord_stride <= 0xFFFFFFFFll, KRAG_E_UNSUPPORTED, "global ordinal exceeds 32 bits");
+    KRAG_REQUIRE(ord_base >= 0 && ord_base + ix->rows.n * ix->ord_stride <= 0xFFFFFFFFll, KRAG_E_UNSUPPORTED, "global ordinal exceeds 32 bits");
     // n_docs_global == 0 is legal: every document deleted (the reference's docstore is then empty and its retriever
     // falls back to vector-only, hybrid_retriever.py:113-121); the postings come out empty and avgdl is irrelevant
     KRAG_REQUIRE(n_docs_global >= 0 && total_len_global >= 0, KRAG_E_INVALID, "n_docs_global / total_len_global must be >= 0");
@@ -596,7 +539,7 @@ void commit_global_impl(krag_index* ix, int64_t vocab, const uint32_t* df_global
         ix->has_base = false;                                         // build_postings writes into ix->post
         ix->committed = false;
         build_postings(ix->tid.p, ix->ttf.p, ix->prep.entry_doc.p, ix->dlen.p, alive_ptr(ix), ix->nnz, vocab, d_idf.p, avgdl,
-                       ix->n_rows, ix->post, st);
+                       ix->rows.n, ix->post, st);
     }
     KRAG_CUDA(cudaStreamSynchronize(st));
     d_idf.release();
@@ -609,7 +552,7 @@ void commit_global_impl(krag_index* ix, int64_t vocab, const uint32_t* df_global
     ix->ord_base = ord_base;
     ix->committed = true;
     ix->has_base = true;
-    ix->committed_rows = ix->n_rows;
+    ix->committed_rows = ix->rows.n;
     ix->commit_epoch = ix->epoch;
     CommitReport rep;
     rep.total_ms = (float)(local_ms + ms_since(t0));
@@ -627,13 +570,36 @@ struct CompactReport { float move_ms = 0.f, postings_ms = 0.f; int64_t rows_move
 std::mutex g_compact_mu;
 CompactReport g_compact;
 
+// after a compaction or a redeal has moved the rows: row d holds node ids[d] and every row is alive; exact-size buffers
+// where they fit
+void renumber_rows(krag_index* ix, std::vector<uint64_t> ids, cudaStream_t st)
+{
+    const int64_t n = (int64_t)ids.size();
+    ix->id2row.clear();
+    ix->id2row.reserve((size_t)n);
+    for (int64_t d = 0; d < n; ++d) ix->id2row[ids[(size_t)d]] = d;
+    ix->node_ids = std::move(ids);
+    const int64_t words = (n + 31) / 32;
+    ix->alive_h.assign((size_t)words, 0xFFFFFFFFu);
+    if (n & 31) ix->alive_h.back() = (1u << (n & 31)) - 1u;
+    if (words > 0)
+        KRAG_CUDA(cudaMemcpyAsync(ix->alive_d.p, ix->alive_h.data(), sizeof(uint32_t) * (size_t)words, cudaMemcpyHostToDevice, st));
+    KRAG_CUDA(cudaStreamSynchronize(st));
+    ix->n_live = n;
+    ix->has_dead = false;
+    ix->epoch++;
+    ix->prep = CommitPrep{};
+    ix->rows.shrink(n, st);
+    ix->alive_d.shrink(words > 0 ? words : 1, st);
+    if (ix->has_sparse) ix->dlen.shrink(n > 0 ? n : 1, st);
+}
+
 // krag_index_compact on an index with dead rows and ordinal stride 1 (writer lock held)
 void compact_impl(krag_index* ix)
 {
     cudaStream_t st = ix->ctx->admin;
-    const int64_t dp = ix->dpad;
     CompactPlan plan;
-    compact_plan(ix->alive_d.p, ix->n_rows, ix->has_sparse ? ix->toff.p : nullptr, plan, st);
+    compact_plan(ix->alive_d.p, ix->rows.n, ix->has_sparse ? ix->toff.p : nullptr, plan, st);
     const int64_t n = plan.n_live;
     const int64_t nnz = ix->has_sparse ? plan.h_toff_new[(size_t)n] : 0;
     CompactReport rep;
@@ -647,7 +613,7 @@ void compact_impl(krag_index* ix)
     if (keep_base) {
         const auto t0 = std::chrono::steady_clock::now();
         DevArray<uint32_t> rank;
-        rank.alloc(ix->n_rows);
+        rank.alloc(ix->rows.n);
         launch_rank_of_rows(plan.src.p, n, rank.p, st);
         SurvivorCounts sc;
         count_survivors(ix->post, alive_ptr(ix), ix->post.vocab, sc, st);
@@ -673,26 +639,12 @@ void compact_impl(krag_index* ix)
     KRAG_CUDA(cudaEventCreate(&e0));
     KRAG_CUDA(cudaEventCreate(&e1));
     KRAG_CUDA(cudaEventRecord(e0, st));
-    // device arrays first (asynchronous); the pinned host rows move on the CPU meanwhile
-    if (!ix->host_rows) rep.bytes_moved += compact_rows(ix->X.p, dp * (int64_t)sizeof(float), plan, st);
-    if (ix->Xh.p) rep.bytes_moved += compact_rows(ix->Xh.p, dp * (int64_t)sizeof(uint16_t), plan, st);
-    if (ix->xres.p) rep.bytes_moved += compact_rows(ix->xres.p, sizeof(float), plan, st);
-    rep.bytes_moved += compact_rows(ix->xnorm.p, sizeof(float), plan, st);
     if (ix->has_sparse) {
         rep.bytes_moved += compact_rows(ix->dlen.p, sizeof(uint32_t), plan, st);
         rep.bytes_moved += compact_terms(ix->tid.p, ix->ttf.p, ix->toff.p, plan, st);
         KRAG_CUDA(cudaMemcpyAsync(ix->toff.p, plan.toff_new.p, sizeof(int64_t) * (size_t)(n + 1), cudaMemcpyDeviceToDevice, st));
     }
-    launch_max_bits(ix->xnorm.p, n, ix->xn_max.p, st);
-    if (ix->host_rows) {
-        // runs of consecutive live rows, ascending: a destination never lies above its source, so memmove is safe
-        for (int64_t d = plan.first; d < n;) {
-            int64_t e = d + 1;
-            while (e < n && plan.h_src[(size_t)e] == plan.h_src[(size_t)e - 1] + 1) ++e;
-            memmove(ix->Xp.h + d * dp, ix->Xp.h + (int64_t)plan.h_src[(size_t)d] * dp, sizeof(float) * (size_t)((e - d) * dp));
-            d = e;
-        }
-    }
+    rep.bytes_moved += ix->rows.compact(plan, st);
     KRAG_CUDA(cudaEventRecord(e1, st));
     KRAG_CUDA(cudaEventSynchronize(e1));
     KRAG_CUDA(cudaEventElapsedTime(&rep.move_ms, e0, e1));
@@ -702,40 +654,14 @@ void compact_impl(krag_index* ix)
 
     // host-side state
     std::vector<uint64_t> ids((size_t)n);
-    ix->id2row.clear();
-    ix->id2row.reserve((size_t)n);
-    for (int64_t d = 0; d < n; ++d) {
-        ids[(size_t)d] = ix->node_ids[plan.h_src[(size_t)d]];
-        ix->id2row[ids[(size_t)d]] = d;
-    }
-    ix->node_ids = std::move(ids);
-    const int64_t words = (n + 31) / 32;
-    ix->alive_h.assign((size_t)words, 0xFFFFFFFFu);
-    if (n & 31) ix->alive_h.back() = (1u << (n & 31)) - 1u;
-    if (words > 0)
-        KRAG_CUDA(cudaMemcpyAsync(ix->alive_d.p, ix->alive_h.data(), sizeof(uint32_t) * (size_t)words, cudaMemcpyHostToDevice, st));
-    KRAG_CUDA(cudaStreamSynchronize(st));
+    for (int64_t d = 0; d < n; ++d) ids[(size_t)d] = ix->node_ids[plan.h_src[(size_t)d]];
     plan = CompactPlan{};
-    ix->n_rows = n;
-    ix->n_live = n;
-    ix->has_dead = false;
     ix->nnz = nnz;
-    ix->epoch++;
-    ix->prep = CommitPrep{};
     ix->post = std::move(remapped);      // empty without a base
     ix->committed_rows = base_rows;
-
-    // exact-size buffers where they fit (never empty: a null Xh means "no bf16 shadow")
-    const int64_t rows1 = n > 0 ? n : 1;
-    if (ix->host_rows) ix->Xp.shrink(rows1 * dp);
-    else ix->X.shrink(rows1 * dp, st);
-    ix->Xh.shrink(rows1 * dp, st);
-    ix->xres.shrink(rows1, st);
-    ix->xnorm.shrink(rows1, st);
-    ix->alive_d.shrink(words > 0 ? words : 1, st);
+    renumber_rows(ix, std::move(ids), st);
     if (ix->has_sparse) {
         ix->toff.shrink(n + 1, st);
-        ix->dlen.shrink(rows1, st);
         ix->tid.shrink(nnz > 0 ? nnz : 1, st);
         ix->ttf.shrink(nnz > 0 ? nnz : 1, st);
     }
@@ -812,11 +738,8 @@ int32_t krag_index_create(krag_ctx* c, const char* name, int32_t dim, krag_index
         krag_index* ix = new krag_index();
         ix->ctx = c;
         ix->name = name;
-        ix->dim = dim;
-        ix->dpad = (dim + KRAG_LANES - 1) / KRAG_LANES * KRAG_LANES;
+        ix->rows.init(dim, c->cfg.row_storage == KRAG_ROWS_HOST);
         ix->ord_base = 0;
-        ix->host_rows = c->cfg.row_storage == KRAG_ROWS_HOST;
-        ix->split_rows = split_rows_layout(ix->dpad, ix->host_rows);
         *out = ix;
     });
 }
@@ -842,7 +765,8 @@ int32_t krag_index_reserve(krag_index* ix, int64_t rows, int64_t nnz)
         require_idle(ix);
         wait_issued_searches(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
-        ensure_capacity(ix, rows, nnz > 0 ? nnz : -1, ix->ctx->admin);
+        ix->rows.reserve(rows, ix->ctx->cfg.dense_mode, ix->ctx->admin);
+        if (nnz > 0) reserve_terms(ix, rows, nnz, ix->ctx->admin);
     });
 }
 
@@ -861,7 +785,7 @@ int32_t krag_index_add(krag_index* ix, int64_t n, const uint64_t* node_ids, cons
         wait_issued_searches(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         cudaStream_t st = ix->ctx->admin;
-        KRAG_REQUIRE(ix->n_rows == 0 || sparse == ix->has_sparse, KRAG_E_STATE,
+        KRAG_REQUIRE(ix->rows.n == 0 || sparse == ix->has_sparse, KRAG_E_STATE,
                      "an index is either hybrid (term lists for every node) or dense-only");
         {
             std::unordered_map<uint64_t, int64_t> batch;   // ids must be new to the index AND unique inside the call
@@ -873,31 +797,8 @@ int32_t krag_index_add(krag_index* ix, int64_t n, const uint64_t* node_ids, cons
         }
         const int64_t add_nnz = sparse ? term_offsets[n] - term_offsets[0] : 0;
         KRAG_REQUIRE(!sparse || (term_offsets[0] == 0 && add_nnz >= 0), KRAG_E_INVALID, "term_offsets must start at 0");
-        ensure_capacity(ix, ix->n_rows + n, sparse ? ix->nnz + add_nnz : -1, st);
-        float* dst = ix->X.p + ix->n_rows * ix->dpad;
-        if (ix->host_rows) {
-            float* h = ix->Xp.h + ix->n_rows * ix->dpad;
-            if (ix->dim == ix->dpad) {
-                memcpy(h, vecs, sizeof(float) * (size_t)n * ix->dim);
-            } else {
-                for (int64_t i = 0; i < n; ++i) {
-                    memcpy(h + i * ix->dpad, vecs + i * ix->dim, sizeof(float) * ix->dim);
-                    memset(h + i * ix->dpad + ix->dim, 0, sizeof(float) * (ix->dpad - ix->dim));
-                }
-            }
-            derive_host_rows(ix, ix->n_rows, n, st);
-        } else if (ix->dim == ix->dpad) {
-            KRAG_CUDA(cudaMemcpyAsync(dst, vecs, sizeof(float) * (size_t)n * ix->dim, cudaMemcpyHostToDevice, st));
-        } else {
-            KRAG_CUDA(cudaMemsetAsync(dst, 0, sizeof(float) * (size_t)n * ix->dpad, st));
-            KRAG_CUDA(cudaMemcpy2DAsync(dst, sizeof(float) * ix->dpad, vecs, sizeof(float) * ix->dim, sizeof(float) * ix->dim,
-                                        (size_t)n, cudaMemcpyHostToDevice, st));
-        }
-        if (!ix->host_rows) {   // norms and shadow from the plain rows, then the rows take their stored layout
-            launch_row_norms(ix->X.p, ix->n_rows, n, ix->dpad, ix->xnorm.p, ix->xn_max.p, st);
-            if (ix->Xh.p) launch_f32_to_bf16(dst, ix->Xh.p + ix->n_rows * ix->dpad, n * ix->dpad, st);
-            if (ix->split_rows) launch_split_encode(dst, n, ix->dpad, st);
-        }
+        if (sparse) reserve_terms(ix, ix->rows.n + n, ix->nnz + add_nnz, st);
+        ix->rows.append(vecs, n, ix->ctx->cfg.dense_mode, st);   // rows [rows.n, rows.n + n), published below
         std::vector<int64_t> shifted;
         if (sparse) {
             shifted.resize((size_t)n + 1);
@@ -905,9 +806,9 @@ int32_t krag_index_add(krag_index* ix, int64_t n, const uint64_t* node_ids, cons
                 KRAG_REQUIRE(i == 0 || term_offsets[i] >= term_offsets[i - 1], KRAG_E_INVALID, "term_offsets must be non-decreasing");
                 shifted[(size_t)i] = ix->nnz + term_offsets[i];
             }
-            KRAG_CUDA(cudaMemcpyAsync(ix->toff.p + ix->n_rows, shifted.data(), sizeof(int64_t) * (size_t)(n + 1),
+            KRAG_CUDA(cudaMemcpyAsync(ix->toff.p + ix->rows.n, shifted.data(), sizeof(int64_t) * (size_t)(n + 1),
                                       cudaMemcpyHostToDevice, st));
-            KRAG_CUDA(cudaMemcpyAsync(ix->dlen.p + ix->n_rows, doc_len, sizeof(uint32_t) * (size_t)n, cudaMemcpyHostToDevice, st));
+            KRAG_CUDA(cudaMemcpyAsync(ix->dlen.p + ix->rows.n, doc_len, sizeof(uint32_t) * (size_t)n, cudaMemcpyHostToDevice, st));
             if (add_nnz > 0) {
                 uint32_t mx = ix->max_term_id;
                 for (int64_t i = 0; i < add_nnz; ++i) mx = term_ids[i] > mx ? term_ids[i] : mx;
@@ -916,13 +817,13 @@ int32_t krag_index_add(krag_index* ix, int64_t n, const uint64_t* node_ids, cons
                 KRAG_CUDA(cudaMemcpyAsync(ix->ttf.p + ix->nnz, term_tf, sizeof(uint16_t) * (size_t)add_nnz, cudaMemcpyHostToDevice, st));
             }
         }
-        mark_alive(ix, ix->n_rows, n, st);
+        mark_alive(ix, ix->rows.n, n, st);
         KRAG_CUDA(cudaStreamSynchronize(st));
         for (int64_t i = 0; i < n; ++i) {
-            ix->id2row[node_ids[i]] = ix->n_rows + i;
+            ix->id2row[node_ids[i]] = ix->rows.n + i;
             ix->node_ids.push_back(node_ids[i]);
         }
-        ix->n_rows += n;
+        ix->rows.n += n;
         ix->n_live += n;
         ix->nnz += add_nnz;
         ix->has_sparse = sparse;
@@ -967,10 +868,10 @@ int32_t krag_index_compact(krag_index* ix, int64_t* n_reclaimed_out)
         KRAG_REQUIRE(ix->ord_stride == 1, KRAG_E_UNSUPPORTED,
                      "compaction needs ordinal stride 1: rows of a round-robin shard cannot move down without leaving it");
         if (n_reclaimed_out) *n_reclaimed_out = 0;
-        if (!ix->has_dead || ix->n_live == ix->n_rows) return;
-        const int64_t before = ix->n_rows;
+        if (!ix->has_dead || ix->n_live == ix->rows.n) return;
+        const int64_t before = ix->rows.n;
         compact_impl(ix);
-        if (n_reclaimed_out) *n_reclaimed_out = before - ix->n_rows;
+        if (n_reclaimed_out) *n_reclaimed_out = before - ix->rows.n;
     });
 }
 
@@ -992,7 +893,7 @@ int32_t krag_index_alive_bitmap(krag_index* ix, uint32_t* out, int64_t cap_words
         KRAG_REQUIRE(ix && words_out, KRAG_E_INVALID, "null argument");
         std::unique_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
-        const int64_t words = (ix->n_rows + 31) / 32;
+        const int64_t words = (ix->rows.n + 31) / 32;
         *words_out = words;
         if (!out) return;
         KRAG_REQUIRE(cap_words >= words, KRAG_E_INVALID, "bitmap buffer holds fewer words than the index has rows / 32");
@@ -1010,8 +911,7 @@ static RedealSession* open_session(krag_index* ix)
 static RedealRows redeal_rows(krag_index* ix)
 {
     const bool sp = ix->has_sparse;
-    return RedealRows{ix->host_rows ? ix->Xp.d : ix->X.p, ix->Xh.p, ix->xres.p, ix->xnorm.p, sp ? ix->dlen.p : nullptr,
-                      sp ? ix->toff.p : nullptr, sp ? ix->tid.p : nullptr, sp ? ix->ttf.p : nullptr, ix->dpad};
+    return ix->rows.redeal_rows(sp ? ix->dlen.p : nullptr, sp ? ix->toff.p : nullptr, sp ? ix->tid.p : nullptr, sp ? ix->ttf.p : nullptr);
 }
 
 int32_t krag_redeal_begin(krag_index* ix, const uint32_t* alive_all, int64_t words, int64_t window_rows, int64_t* n_windows_out,
@@ -1026,21 +926,23 @@ int32_t krag_redeal_begin(krag_index* ix, const uint32_t* alive_all, int64_t wor
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         const int G = (int)ix->ord_stride, s = (int)ix->ord_base;
         KRAG_REQUIRE(s < G, KRAG_E_STATE, "not a round-robin shard: the ordinal base must be below the stride");
-        KRAG_REQUIRE(words >= (ix->n_rows + 31) / 32, KRAG_E_INVALID, "the bitmaps hold fewer words than this shard has rows / 32");
+        KRAG_REQUIRE(words >= (ix->rows.n + 31) / 32, KRAG_E_INVALID, "the bitmaps hold fewer words than this shard has rows / 32");
         KRAG_REQUIRE(ix->committed && ix->commit_epoch == ix->epoch, KRAG_E_STATE,
                      "rows were added or removed since the last commit: commit before the redeal");
-        for (int64_t r = 0; r < ix->n_rows; ++r)
+        for (int64_t r = 0; r < ix->rows.n; ++r)
             KRAG_REQUIRE(ix->node_ids[(size_t)r] == (uint64_t)(s + r * G), KRAG_E_STATE,
                          "a node id differs from its global ordinal: the redeal renumbers node ids to the new ordinals");
         const uint32_t* own = alive_all + (size_t)s * (size_t)words;
-        const int64_t own_words = (ix->n_rows + 31) / 32;
+        const int64_t own_words = (ix->rows.n + 31) / 32;
         bool same = own_words == 0 || memcmp(own, ix->alive_h.data(), sizeof(uint32_t) * (size_t)own_words) == 0;
         for (int64_t w = own_words; w < words; ++w) same = same && own[w] == 0;
         KRAG_REQUIRE(same, KRAG_E_INVALID, "this shard's bitmap in alive_all differs from its alive rows");
-        const bool has_xh = ix->Xh.p != nullptr ||
-                            (ix->n_rows == 0 && (ix->host_rows || ix->ctx->cfg.dense_mode == KRAG_DENSE_TC_BF16));
+        // every shard's rows carry a bf16 copy or none: a shard whose copy the dense mode asks for but does not exist yet
+        // builds it from its rows here
+        ix->rows.reserve(ix->rows.n, ix->ctx->cfg.dense_mode, ix->ctx->admin);
+        const bool has_xh = ix->rows.keeps_bf16(ix->ctx->cfg.dense_mode);
         auto sess = std::make_unique<RedealSession>();
-        redeal_plan(alive_all, G, s, words, ix->n_rows, ix->has_sparse ? ix->toff.p : nullptr, has_xh, ix->dpad, window_rows, sess->plan,
+        redeal_plan(alive_all, G, s, words, ix->rows.n, ix->has_sparse ? ix->toff.p : nullptr, has_xh, ix->rows.dpad, window_rows, sess->plan,
                     ix->ctx->admin);
         *n_windows_out = sess->plan.n_windows;
         *n_live_out = sess->plan.n_live;
@@ -1136,7 +1038,7 @@ int32_t krag_redeal_finish(krag_index* ix, void* stream, int64_t* n_rows_out)
             KRAG_CUDA(cudaEventElapsedTime(&rep.move_ms, ss->e0, ss->e1));
         }
         KRAG_CUDA(cudaStreamSynchronize(st));
-        const int64_t n = p.n_new, G = p.G, s = p.s, dp = ix->dpad;
+        const int64_t n = p.n_new, G = p.G, s = p.s;
         if (ix->has_sparse) {
             ix->toff = std::move(p.toff_new);
             ix->tid = std::move(p.tid_new);
@@ -1144,37 +1046,13 @@ int32_t krag_redeal_finish(krag_index* ix, void* stream, int64_t* n_rows_out)
             ix->nnz = p.ent_base.back();
             if (ix->nnz > 0) ix->max_term_id = std::max<uint32_t>(ix->max_term_id, (uint32_t)(ix->vocab - 1));   // every shard's terms are below the committed vocab
         }
-        launch_max_bits(ix->xnorm.p, n, ix->xn_max.p, ad);
-        ix->node_ids.resize((size_t)n);
-        ix->id2row.clear();
-        ix->id2row.reserve((size_t)n);
-        for (int64_t j = 0; j < n; ++j) {
-            ix->node_ids[(size_t)j] = (uint64_t)(s + j * G);
-            ix->id2row[(uint64_t)(s + j * G)] = j;
-        }
-        const int64_t words = (n + 31) / 32;
-        ix->alive_h.assign((size_t)words, 0xFFFFFFFFu);
-        if (n & 31) ix->alive_h.back() = (1u << (n & 31)) - 1u;
-        if (words > 0)
-            KRAG_CUDA(cudaMemcpyAsync(ix->alive_d.p, ix->alive_h.data(), sizeof(uint32_t) * (size_t)words, cudaMemcpyHostToDevice, ad));
-        KRAG_CUDA(cudaStreamSynchronize(ad));
-        ix->n_rows = n;
-        ix->n_live = n;
-        ix->has_dead = false;
-        ix->epoch++;
-        ix->prep = CommitPrep{};
+        std::vector<uint64_t> ids((size_t)n);
+        for (int64_t j = 0; j < n; ++j) ids[(size_t)j] = (uint64_t)(s + j * G);
         ix->post = Postings{};          // no base: the collective commit that follows is a full build under the same statistics
         ix->committed = false;
         ix->has_base = false;
         ix->committed_rows = 0;
-        const int64_t rows1 = n > 0 ? n : 1;
-        if (ix->host_rows) ix->Xp.shrink(rows1 * dp);
-        else ix->X.shrink(rows1 * dp, ad);
-        ix->Xh.shrink(rows1 * dp, ad);
-        ix->xres.shrink(rows1, ad);
-        ix->xnorm.shrink(rows1, ad);
-        ix->alive_d.shrink(words > 0 ? words : 1, ad);
-        if (ix->has_sparse) ix->dlen.shrink(rows1, ad);
+        renumber_rows(ix, std::move(ids), ad);
         rep.rows_moved = p.n_send;
         rep.bytes_moved = ss->bytes_moved;
         rep.valid = true;
@@ -1259,7 +1137,7 @@ int32_t krag_index_set_ordinal_map(krag_index* ix, int64_t ordinal_base, int64_t
         std::unique_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
         wait_issued_searches(ix);
-        KRAG_REQUIRE(ordinal_base + ix->n_rows * ordinal_stride <= 0xFFFFFFFFll, KRAG_E_UNSUPPORTED, "global ordinal exceeds 32 bits");
+        KRAG_REQUIRE(ordinal_base + ix->rows.n * ordinal_stride <= 0xFFFFFFFFll, KRAG_E_UNSUPPORTED, "global ordinal exceeds 32 bits");
         ix->ord_base = ordinal_base; ix->ord_stride = ordinal_stride;
     });
 }
@@ -1271,11 +1149,11 @@ int32_t krag_index_stats(krag_index* ix, krag_stats_t* out)
         std::shared_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
         memset(out, 0, sizeof *out);
-        out->n_rows = ix->n_rows; out->n_live = ix->n_live; out->nnz = ix->committed ? ix->post.nnz : ix->nnz;
+        out->n_rows = ix->rows.n; out->n_live = ix->n_live; out->nnz = ix->committed ? ix->post.nnz : ix->nnz;
         out->n_docs_global = ix->n_docs_global; out->total_len_global = ix->total_len_global; out->vocab = ix->vocab;
-        out->ordinal_base = ix->ord_base; out->dim = ix->dim; out->dim_padded = ix->dpad;
-        out->committed = ix->committed && ix->committed_rows == ix->n_rows;
-        out->device_bytes = ix->X.bytes() + ix->Xh.bytes() + ix->xres.bytes() + ix->xnorm.bytes() + ix->alive_d.bytes() + ix->toff.bytes() + ix->tid.bytes() + ix->ttf.bytes() +
+        out->ordinal_base = ix->ord_base; out->dim = ix->rows.dim; out->dim_padded = ix->rows.dpad;
+        out->committed = ix->committed && ix->committed_rows == ix->rows.n;
+        out->device_bytes = ix->rows.device_bytes() + ix->alive_d.bytes() + ix->toff.bytes() + ix->tid.bytes() + ix->ttf.bytes() +
                             ix->dlen.bytes() + (ix->committed ? (int64_t)(ix->post.nnz * 10 + (ix->post.vocab + 1) * 8) : 0);
     });
 }
@@ -1290,7 +1168,7 @@ int32_t krag_index_node_ids(krag_index* ix, int64_t n, const int64_t* ordinals, 
             const int64_t off = ordinals[i] - ix->ord_base;
             KRAG_REQUIRE(off >= 0 && off % ix->ord_stride == 0, KRAG_E_NOT_FOUND, "ordinal is not held by this shard");
             const int64_t r = off / ix->ord_stride;
-            KRAG_REQUIRE(r < ix->n_rows, KRAG_E_NOT_FOUND, "ordinal is not held by this shard");
+            KRAG_REQUIRE(r < ix->rows.n, KRAG_E_NOT_FOUND, "ordinal is not held by this shard");
             out[i] = ix->node_ids[(size_t)r];
         }
     });
@@ -1364,7 +1242,7 @@ int32_t krag_retrieve(krag_index* ix, int32_t batch, const float* q, const uint3
         require_idle(ix);
         // the bitmap is read (n_rows + 31) / 32 words deep: the caller states how many it holds, so a bitmap built
         // before a concurrent krag_index_add is refused instead of over-read
-        KRAG_REQUIRE(keyword_allow_bitmap == nullptr || keyword_allow_words >= (ix->n_rows + 31) / 32, KRAG_E_INVALID,
+        KRAG_REQUIRE(keyword_allow_bitmap == nullptr || keyword_allow_words >= (ix->rows.n + 31) / 32, KRAG_E_INVALID,
                      "keyword_allow_bitmap holds fewer words than the index has rows / 32");
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         SlotLease lease(ix->ctx);
@@ -1375,7 +1253,7 @@ int32_t krag_retrieve(krag_index* ix, int32_t batch, const float* q, const uint3
         fusion_mode &= 0xFF;
         const uint32_t* eligible = nullptr;
         if (pushdown) {   // eligible = allow & alive, consumed by K1/K2/K3 in place of the tombstone bitmap
-            const int64_t words = (ix->n_rows + 31) / 32;
+            const int64_t words = (ix->rows.n + 31) / 32;
             s->allow.reserve(words > 0 ? words : 1, 0, st);
             KRAG_CUDA(cudaMemcpyAsync(s->allow.p, keyword_allow_bitmap, sizeof(uint32_t) * (size_t)words, cudaMemcpyHostToDevice, st));
             if (ix->has_dead && words > 0) launch_bitmap_and(s->allow.p, ix->alive_d.p, words, st);
@@ -1393,7 +1271,7 @@ int32_t krag_retrieve(krag_index* ix, int32_t batch, const float* q, const uint3
                 // bitmap is over local rows; fuse tests global ordinals -> shift by ord_base words is only
                 // valid when ord_base % 32 == 0; the host path is single-shard (ord_base == 0)
                 KRAG_REQUIRE(ix->ord_base == 0 && ix->ord_stride == 1, KRAG_E_UNSUPPORTED, "keyword filter on host path requires ordinal_base 0, stride 1");
-                int64_t words = (ix->n_rows + 31) / 32;
+                int64_t words = (ix->rows.n + 31) / 32;
                 s->allow.reserve(words, 0, st);
                 KRAG_CUDA(cudaMemcpyAsync(s->allow.p, keyword_allow_bitmap, sizeof(uint32_t) * (size_t)words, cudaMemcpyHostToDevice, st));
                 d_allow = s->allow.p;
@@ -1480,16 +1358,8 @@ int32_t krag_synth_fill(krag_index* ix, int64_t n, int64_t row_base, uint64_t se
         wait_issued_searches(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         cudaStream_t st = ix->ctx->admin;
-        KRAG_REQUIRE(ix->n_rows == 0, KRAG_E_STATE, "synthetic fill needs an empty index");
-        ensure_capacity(ix, n, -1, st);
-        if (ix->host_rows) {
-            derive_host_rows(ix, 0, n, st, &seed, row_base);
-        } else {
-            launch_synth_dense(ix->X.p, n, ix->dim, ix->dpad, row_base, seed, st);
-            launch_row_norms(ix->X.p, 0, n, ix->dpad, ix->xnorm.p, ix->xn_max.p, st);
-            if (ix->Xh.p) launch_f32_to_bf16(ix->X.p, ix->Xh.p, n * ix->dpad, st);
-            if (ix->split_rows) launch_split_encode(ix->X.p, n, ix->dpad, st);
-        }
+        KRAG_REQUIRE(ix->rows.n == 0, KRAG_E_STATE, "synthetic fill needs an empty index");
+        ix->rows.synth(n, row_base, seed, ix->ctx->cfg.dense_mode, st);
         if (vocab > 0) {
             DevArray<int64_t> off; DevArray<uint32_t> ids; DevArray<uint16_t> tf; DevArray<uint32_t> dl; int64_t nnz = 0;
             synth_sparse(n, row_base, seed, vocab, off, ids, tf, dl, &nnz, st);
@@ -1502,7 +1372,7 @@ int32_t krag_synth_fill(krag_index* ix, int64_t n, int64_t row_base, uint64_t se
         KRAG_CUDA(cudaStreamSynchronize(st));
         ix->node_ids.resize((size_t)n);
         for (int64_t i = 0; i < n; ++i) { ix->node_ids[(size_t)i] = (uint64_t)(row_base + i); ix->id2row[(uint64_t)(row_base + i)] = i; }
-        ix->n_rows = n; ix->n_live = n; ix->ord_base = row_base; ix->ord_stride = 1; ix->committed = false;
+        ix->rows.n = n; ix->n_live = n; ix->ord_base = row_base; ix->ord_stride = 1; ix->committed = false;
         ix->has_base = false; ix->post = Postings{}; ix->epoch++;
     });
 }
@@ -1510,36 +1380,23 @@ int32_t krag_synth_fill(krag_index* ix, int64_t n, int64_t row_base, uint64_t se
 int32_t krag_index_read_rows(krag_index* ix, int64_t row0, int64_t n, float* out)
 {
     return guarded([&] {
-        KRAG_REQUIRE(ix && out && row0 >= 0 && n >= 0 && row0 + n <= ix->n_rows, KRAG_E_INVALID, "row range out of bounds");
+        KRAG_REQUIRE(ix && out && row0 >= 0 && n >= 0 && row0 + n <= ix->rows.n, KRAG_E_INVALID, "row range out of bounds");
         std::shared_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
-        if (n == 0) return;
-        if (ix->host_rows) {
-            for (int64_t i = 0; i < n; ++i) memcpy(out + i * ix->dim, ix->Xp.h + (row0 + i) * ix->dpad, sizeof(float) * ix->dim);
-            return;
-        }
-        if (ix->split_rows) {
-            std::vector<float> raw((size_t)n * ix->dpad);
-            KRAG_CUDA(cudaMemcpy(raw.data(), ix->X.p + row0 * ix->dpad, sizeof(float) * raw.size(), cudaMemcpyDeviceToHost));
-            for (int64_t i = 0; i < n; ++i) split_row_decode_host(raw.data() + i * ix->dpad, ix->dim, out + i * ix->dim);
-            return;
-        }
-        KRAG_CUDA(cudaMemcpy2D(out, sizeof(float) * ix->dim, ix->X.p + row0 * ix->dpad, sizeof(float) * ix->dpad,
-                               sizeof(float) * ix->dim, (size_t)n, cudaMemcpyDeviceToHost));
+        ix->rows.read(row0, n, out);
     });
 }
 
 int32_t krag_debug_read_stored_rows(krag_index* ix, int64_t row0, int64_t n, float* out)
 {
     return guarded([&] {
-        KRAG_REQUIRE(ix && out && row0 >= 0 && n >= 0 && row0 + n <= ix->n_rows, KRAG_E_INVALID, "row range out of bounds");
+        KRAG_REQUIRE(ix && out && row0 >= 0 && n >= 0 && row0 + n <= ix->rows.n, KRAG_E_INVALID, "row range out of bounds");
         std::shared_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
-        KRAG_REQUIRE(!ix->host_rows, KRAG_E_UNSUPPORTED, "the stored layout is that of device-resident rows");
+        KRAG_REQUIRE(!ix->rows.host(), KRAG_E_UNSUPPORTED, "the stored layout is that of device-resident rows");
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
-        if (n > 0)
-            KRAG_CUDA(cudaMemcpy(out, ix->X.p + row0 * ix->dpad, sizeof(float) * (size_t)(n * ix->dpad), cudaMemcpyDeviceToHost));
+        ix->rows.read_stored(row0, n, out);
     });
 }
 
@@ -1571,12 +1428,7 @@ int32_t krag_index_set_dense_mode(krag_index* ix, int32_t dense_mode, int32_t re
         wait_issued_searches(ix);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
         cudaStream_t st = ix->ctx->admin;
-        if (dense_mode == KRAG_DENSE_TC_BF16 && ix->Xh.p == nullptr && ix->X.p != nullptr) {
-            ix->Xh.reserve(ix->X.cap, 0, st);                     // same capacity as the fp32 rows: later appends convert in place
-            if (ix->split_rows) launch_split_to_bf16(ix->X.p, ix->n_rows, ix->dpad, ix->Xh.p, st);
-            else launch_f32_to_bf16(ix->X.p, ix->Xh.p, ix->n_rows * ix->dpad, st);
-        }
-        if (dense_mode != KRAG_DENSE_TC_BF16 && release_shadow && !ix->host_rows) ix->Xh.release();   // host rows: Xh is the device copy
+        ix->rows.set_shadow(ix->rows.keeps_bf16(dense_mode, release_shadow != 0), st);
         KRAG_CUDA(cudaStreamSynchronize(st));
         ix->ctx->cfg.dense_mode = dense_mode;
     });
@@ -1596,18 +1448,21 @@ int32_t krag_last_dense_kernel(float* ms, int32_t* kernel_id, int64_t* algorithm
 }
 
 namespace {
-// the index's rows for one prune pass of the test hooks (krag_debug_tc_dump_pass, krag_debug_tc_prune)
-void require_tc_pass(const krag_index* ix, int32_t pass)
+// the prune operand of pass KRAG_TC_PASS_* on the index's rows, for the test hooks (krag_debug_tc_dump_pass, krag_debug_tc_prune)
+static_assert(TC_OP_BF16_SPLIT == KRAG_TC_PASS_BF16_SPLIT + 1 && TC_OP_BF16_SHADOW == KRAG_TC_PASS_BF16_SHADOW + 1 &&
+                  TC_OP_BF16_HOST == KRAG_TC_PASS_BF16_HOST + 1, "prune passes");
+TcOp require_tc_pass(const krag_index* ix, int32_t pass)
 {
+    const DenseRows& r = ix->rows;
     KRAG_REQUIRE(pass >= KRAG_TC_PASS_TF32 && pass <= KRAG_TC_PASS_BF16_HOST, KRAG_E_INVALID, "unknown prune pass");
-    KRAG_REQUIRE(ix->n_rows > 0, KRAG_E_STATE, "index has no rows");
-    if (pass == KRAG_TC_PASS_BF16_HOST) {
-        KRAG_REQUIRE(ix->host_rows, KRAG_E_UNSUPPORTED, "the host-rows pass needs a KRAG_ROWS_HOST index");
-        return;
-    }
-    KRAG_REQUIRE(!ix->host_rows, KRAG_E_UNSUPPORTED, "this prune pass needs device-resident rows");
-    KRAG_REQUIRE(pass != KRAG_TC_PASS_BF16_SPLIT || ix->split_rows, KRAG_E_UNSUPPORTED, "the index does not keep split rows");
-    KRAG_REQUIRE(pass != KRAG_TC_PASS_BF16_SHADOW || ix->Xh.p, KRAG_E_STATE, "the index has no bf16 shadow");
+    KRAG_REQUIRE(r.n > 0, KRAG_E_STATE, "index has no rows");
+    const TcOp op = pass == KRAG_TC_PASS_TF32 ? (r.split() ? TC_OP_TF32S : TC_OP_TF32) : (TcOp)(pass + 1);
+    KRAG_REQUIRE(r.host() == (op == TC_OP_BF16_HOST), KRAG_E_UNSUPPORTED,
+                 r.host() ? "this prune pass needs device-resident rows" : "the host-rows pass needs a KRAG_ROWS_HOST index");
+    KRAG_REQUIRE(op != TC_OP_BF16_SPLIT || r.split(), KRAG_E_UNSUPPORTED, "the index does not keep split rows");
+    KRAG_REQUIRE(op != TC_OP_BF16_SHADOW || r.bf16(), KRAG_E_STATE, "the index has no bf16 shadow");
+    KRAG_REQUIRE(dense_tc_supported(ix->ctx->di, r.dpad), KRAG_E_UNSUPPORTED, "tensor-core path unavailable");
+    return op;
 }
 }  // namespace
 
@@ -1618,22 +1473,20 @@ int32_t krag_debug_tc_dump_pass(krag_index* ix, int32_t pass, int32_t nq, const 
         KRAG_REQUIRE(ix && q && S_out && nq_pad_out && nq >= 1 && nq <= 256, KRAG_E_INVALID, "bad argument");
         std::shared_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
-        require_tc_pass(ix, pass);
+        const TcOp op = require_tc_pass(ix, pass);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
-        KRAG_REQUIRE(dense_tc_supported(ix->ctx->di, ix->dpad), KRAG_E_UNSUPPORTED, "tensor-core path unavailable");
         SlotLease lease(ix->ctx);
         Slot* s = lease.s;
         int64_t S = 0; int nqp = 0;
-        const size_t ws = dense_tc_debug_carve(nullptr, nullptr, ix->n_rows, ix->dpad, nq, 0, &S, &nqp);
+        const size_t ws = dense_tc_debug_carve(nullptr, nullptr, ix->rows.n, ix->rows.dpad, nq, 0, &S, &nqp);
         *S_out = S; *nq_pad_out = nqp;
         if (!out) return;
         KRAG_REQUIRE(out_elems >= S * nqp, KRAG_E_INVALID, "output buffer too small");
         const float* dq = upload_queries(ix, s, q, nq);
         s->tc_ws.reserve((int64_t)ws, 0, s->st);
         TcDebugWs w;
-        dense_tc_debug_carve(&w, s->tc_ws.p, ix->n_rows, ix->dpad, nq, 0, &S, &nqp);
-        KRAG_REQUIRE(dense_tc_debug_pass(ix->ctx->di, pass, ix->X.p, ix->Xh.p, ix->split_rows, ix->n_rows, ix->dpad, ix->xnorm.p,
-                                         nullptr, dq, nq, w, 0, s->st),
+        dense_tc_debug_carve(&w, s->tc_ws.p, ix->rows.n, ix->rows.dpad, nq, 0, &S, &nqp);
+        KRAG_REQUIRE(dense_tc_debug_pass(ix->ctx->di, ix->rows, op, nullptr, dq, nq, w, 0, s->st),
                      KRAG_E_UNSUPPORTED, "tensor-core dump failed");
         KRAG_CUDA(cudaMemcpyAsync(out, w.dump, sizeof(float) * (size_t)(S * nqp), cudaMemcpyDeviceToHost, s->st));
         KRAG_CUDA(cudaStreamSynchronize(s->st));
@@ -1652,20 +1505,18 @@ int32_t krag_debug_tc_prune(krag_index* ix, int32_t pass, int32_t nq, const floa
         KRAG_REQUIRE(ix && q && thr && counts_out && rows_out && nq >= 1 && nq <= 256 && cap >= 1, KRAG_E_INVALID, "bad argument");
         std::shared_lock<std::shared_mutex> lk(ix->mu);
         require_idle(ix);
-        require_tc_pass(ix, pass);
+        const TcOp op = require_tc_pass(ix, pass);
         KRAG_CUDA(cudaSetDevice(ix->ctx->di.device));
-        KRAG_REQUIRE(dense_tc_supported(ix->ctx->di, ix->dpad), KRAG_E_UNSUPPORTED, "tensor-core path unavailable");
         SlotLease lease(ix->ctx);
         Slot* s = lease.s;
         int64_t S = 0; int nqp = 0;
-        const size_t ws = dense_tc_debug_carve(nullptr, nullptr, ix->n_rows, ix->dpad, nq, cap, &S, &nqp);
+        const size_t ws = dense_tc_debug_carve(nullptr, nullptr, ix->rows.n, ix->rows.dpad, nq, cap, &S, &nqp);
         const float* dq = upload_queries(ix, s, q, nq);
         s->tc_ws.reserve((int64_t)ws, 0, s->st);
         TcDebugWs w;
-        dense_tc_debug_carve(&w, s->tc_ws.p, ix->n_rows, ix->dpad, nq, cap, &S, &nqp);
+        dense_tc_debug_carve(&w, s->tc_ws.p, ix->rows.n, ix->rows.dpad, nq, cap, &S, &nqp);
         KRAG_CUDA(cudaMemcpyAsync(w.thr, thr, sizeof(float) * (size_t)nqp, cudaMemcpyHostToDevice, s->st));
-        KRAG_REQUIRE(dense_tc_debug_pass(ix->ctx->di, pass, ix->X.p, ix->Xh.p, ix->split_rows, ix->n_rows, ix->dpad, ix->xnorm.p,
-                                         alive_ptr(ix), dq, nq, w, cap, s->st),
+        KRAG_REQUIRE(dense_tc_debug_pass(ix->ctx->di, ix->rows, op, alive_ptr(ix), dq, nq, w, cap, s->st),
                      KRAG_E_UNSUPPORTED, "tensor-core prune pass failed");
         KRAG_CUDA(cudaMemcpyAsync(counts_out, w.cand_count, sizeof(uint32_t) * (size_t)nqp, cudaMemcpyDeviceToHost, s->st));
         KRAG_CUDA(cudaMemcpyAsync(rows_out, w.cand_rows, sizeof(uint32_t) * (size_t)nqp * cap, cudaMemcpyDeviceToHost, s->st));
@@ -1924,32 +1775,23 @@ int32_t krag_index_persist(krag_index* ix, const char* dir)
         FILE* f = fopen((path + ".tmp").c_str(), "wb");
         KRAG_REQUIRE(f, KRAG_E_IO, "cannot open " + path + ".tmp for writing");
         auto W = [&](const void* p, size_t n) { if (n && fwrite(p, 1, n, f) != n) { fclose(f); throw ApiError{KRAG_E_IO, "short write to " + path}; } };
-        int64_t hdr[8] = {ix->dim, ix->n_rows, ix->nnz, ix->has_sparse ? 1 : 0, ix->committed ? ix->vocab : 0, 0, 0, 0};
+        int64_t hdr[8] = {ix->rows.dim, ix->rows.n, ix->nnz, ix->has_sparse ? 1 : 0, ix->committed ? ix->vocab : 0, 0, 0, 0};
         W(kMagic, 8); W(hdr, sizeof hdr);
-        W(ix->node_ids.data(), sizeof(uint64_t) * (size_t)ix->n_rows);
-        W(ix->alive_h.data(), sizeof(uint32_t) * (size_t)((ix->n_rows + 31) / 32));
+        W(ix->node_ids.data(), sizeof(uint64_t) * (size_t)ix->rows.n);
+        W(ix->alive_h.data(), sizeof(uint32_t) * (size_t)((ix->rows.n + 31) / 32));
         const int64_t chunk = 1 << 16;
-        std::vector<float> rows((size_t)chunk * ix->dim), raw(ix->split_rows ? (size_t)chunk * ix->dpad : 0);
-        for (int64_t r = 0; r < ix->n_rows; r += chunk) {
-            int64_t m = ix->n_rows - r < chunk ? ix->n_rows - r : chunk;
-            if (ix->host_rows) {
-                for (int64_t i = 0; i < m; ++i)
-                    memcpy(rows.data() + i * ix->dim, ix->Xp.h + (r + i) * ix->dpad, sizeof(float) * ix->dim);
-            } else if (ix->split_rows) {
-                KRAG_CUDA(cudaMemcpy(raw.data(), ix->X.p + r * ix->dpad, sizeof(float) * (size_t)(m * ix->dpad), cudaMemcpyDeviceToHost));
-                for (int64_t i = 0; i < m; ++i) split_row_decode_host(raw.data() + i * ix->dpad, ix->dim, rows.data() + i * ix->dim);
-            } else {
-                KRAG_CUDA(cudaMemcpy2D(rows.data(), sizeof(float) * ix->dim, ix->X.p + r * ix->dpad, sizeof(float) * ix->dpad,
-                                       sizeof(float) * ix->dim, (size_t)m, cudaMemcpyDeviceToHost));
-            }
-            W(rows.data(), sizeof(float) * (size_t)m * ix->dim);
+        std::vector<float> rows((size_t)chunk * ix->rows.dim);
+        for (int64_t r = 0; r < ix->rows.n; r += chunk) {
+            int64_t m = ix->rows.n - r < chunk ? ix->rows.n - r : chunk;
+            ix->rows.read(r, m, rows.data());
+            W(rows.data(), sizeof(float) * (size_t)m * ix->rows.dim);
         }
         if (ix->has_sparse) {
-            std::vector<int64_t> off((size_t)ix->n_rows + 1);
-            std::vector<uint32_t> dl((size_t)ix->n_rows), ids((size_t)ix->nnz);
+            std::vector<int64_t> off((size_t)ix->rows.n + 1);
+            std::vector<uint32_t> dl((size_t)ix->rows.n), ids((size_t)ix->nnz);
             std::vector<uint16_t> tf((size_t)ix->nnz);
             KRAG_CUDA(cudaMemcpy(off.data(), ix->toff.p, sizeof(int64_t) * off.size(), cudaMemcpyDeviceToHost));
-            if (ix->n_rows) KRAG_CUDA(cudaMemcpy(dl.data(), ix->dlen.p, sizeof(uint32_t) * dl.size(), cudaMemcpyDeviceToHost));
+            if (ix->rows.n) KRAG_CUDA(cudaMemcpy(dl.data(), ix->dlen.p, sizeof(uint32_t) * dl.size(), cudaMemcpyDeviceToHost));
             if (ix->nnz) {
                 KRAG_CUDA(cudaMemcpy(ids.data(), ix->tid.p, sizeof(uint32_t) * ids.size(), cudaMemcpyDeviceToHost));
                 KRAG_CUDA(cudaMemcpy(tf.data(), ix->ttf.p, sizeof(uint16_t) * tf.size(), cudaMemcpyDeviceToHost));

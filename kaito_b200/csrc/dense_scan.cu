@@ -167,9 +167,9 @@ static void ds_launch(const DeviceInfo& di, const float* X, int64_t n_rows, int 
     count_launch();
 }
 
-void launch_dense_scan(const DeviceInfo& di, const float* X, int64_t n_rows, int dpad, const uint32_t* alive,
-                       const float* q, int batch, int P, OrdMap ord_base, uint64_t* part, uint64_t* keys_out,
-                       cudaStream_t st, bool split)
+// device rows X (split rows when split), or one staged chunk of host rows
+static void scan_rows(const DeviceInfo& di, const float* X, int64_t n_rows, int dpad, const uint32_t* alive, const float* q,
+                      int batch, int P, OrdMap ord_base, uint64_t* part, uint64_t* keys_out, cudaStream_t st, bool split)
 {
     const int grid = ds_grid(di, n_rows);
     unsigned long long* g_thr = reinterpret_cast<unsigned long long*>(part + (size_t)4 * 2 * di.sm_count * P);
@@ -179,15 +179,9 @@ void launch_dense_scan(const DeviceInfo& di, const float* X, int64_t n_rows, int
         // smem budget: NQ * (dpad*4 + cap*8) must stay under 100 KB (2 CTAs per SM)
         while (nq > 1 && (size_t)nq * ((size_t)dpad * 4 + (size_t)ds_cap(P) * 8) > 96 * 1024) nq >>= 1;
         const float* qb = q + (size_t)b * dpad;
-        if (split) {
-            if (nq == 4) ds_launch<4, true>(di, X, n_rows, dpad, alive, qb, P, ord_base, part, g_thr, st);
-            else if (nq == 2) ds_launch<2, true>(di, X, n_rows, dpad, alive, qb, P, ord_base, part, g_thr, st);
-            else ds_launch<1, true>(di, X, n_rows, dpad, alive, qb, P, ord_base, part, g_thr, st);
-        } else {
-            if (nq == 4) ds_launch<4, false>(di, X, n_rows, dpad, alive, qb, P, ord_base, part, g_thr, st);
-            else if (nq == 2) ds_launch<2, false>(di, X, n_rows, dpad, alive, qb, P, ord_base, part, g_thr, st);
-            else ds_launch<1, false>(di, X, n_rows, dpad, alive, qb, P, ord_base, part, g_thr, st);
-        }
+        (split ? (nq == 4 ? ds_launch<4, true> : nq == 2 ? ds_launch<2, true> : ds_launch<1, true>)
+               : (nq == 4 ? ds_launch<4, false> : nq == 2 ? ds_launch<2, false> : ds_launch<1, false>))(
+            di, X, n_rows, dpad, alive, qb, P, ord_base, part, g_thr, st);
         // part is [nq][grid][P]: lists = CTAs
         launch_merge(part, grid, P, nq, P, /*list_stride=*/P, /*batch_stride=*/(int64_t)grid * P,
                      keys_out + (size_t)b * P, st, reinterpret_cast<const uint64_t*>(g_thr));
@@ -203,9 +197,10 @@ int64_t stream_scan_chunk_rows(int dpad)
     return r / 32 * 32;
 }
 
-void launch_dense_scan_streamed(const DeviceInfo& di, const float* X_host, int64_t n_rows, int dpad, const uint32_t* alive,
-                                const float* q, int batch, int P, OrdMap ord_base, uint64_t* part, const ScanStaging& sg,
-                                uint64_t* keys_out, cudaStream_t st)
+// host rows, chunk by chunk through the staging buffers of sg
+static void scan_streamed(const DeviceInfo& di, const float* X_host, int64_t n_rows, int dpad, const uint32_t* alive,
+                          const float* q, int batch, int P, OrdMap ord_base, uint64_t* part, const ScanStaging& sg,
+                          uint64_t* keys_out, cudaStream_t st)
 {
     const int64_t R = sg.chunk_rows;
     const int64_t list = (int64_t)batch * P;
@@ -223,7 +218,7 @@ void launch_dense_scan_streamed(const DeviceInfo& di, const float* X_host, int64
         KRAG_CUDA(cudaEventRecord(sg.copied[b], sg.copy));
         KRAG_CUDA(cudaStreamWaitEvent(st, sg.copied[b], 0));
         const OrdMap om{ord_base + (uint32_t)r0, ord_base.stride};
-        launch_dense_scan(di, sg.buf[b], m, dpad, alive ? alive + r0 / 32 : nullptr, q, batch, P, om, part, i == 0 ? run : chk, st, false);
+        scan_rows(di, sg.buf[b], m, dpad, alive ? alive + r0 / 32 : nullptr, q, batch, P, om, part, i == 0 ? run : chk, st, false);
         KRAG_CUDA(cudaEventRecord(sg.freed[b], st));
         if (i > 0) {
             launch_merge(run, 2, P, batch, P, list, P, keys_out, st);
@@ -231,6 +226,13 @@ void launch_dense_scan_streamed(const DeviceInfo& di, const float* X_host, int64
         }
     }
     if (i == 1) KRAG_CUDA(cudaMemcpyAsync(keys_out, run, sizeof(uint64_t) * (size_t)list, cudaMemcpyDeviceToDevice, st));
+}
+
+void launch_dense_scan(const DeviceInfo& di, const DenseRows& rows, const uint32_t* alive, const float* q, int batch, int P,
+                       OrdMap ord_base, uint64_t* part, uint64_t* keys_out, cudaStream_t st, const ScanStaging* sg)
+{
+    if (rows.host()) scan_streamed(di, rows.host_h(), rows.n, rows.dpad, alive, q, batch, P, ord_base, part, *sg, keys_out, st);
+    else scan_rows(di, rows.dev(), rows.n, rows.dpad, alive, q, batch, P, ord_base, part, keys_out, st, rows.split());
 }
 
 }  // namespace krag

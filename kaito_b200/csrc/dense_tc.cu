@@ -805,10 +805,6 @@ size_t dense_tc_workspace_bytes(const DeviceInfo&, int64_t n_rows, int P, bool h
     return tc_carve(nullptr, nullptr, tc_cap(P), tc_sample_tiles(n_rows) * TC_TILE_M, host_rows);
 }
 bool dense_tc_wants(int64_t n_rows, int batch) { return n_rows >= TC_MIN_ROWS && batch >= 16; }
-bool dense_tc_host_rows_supported(const DeviceInfo& di, int64_t n_rows, int dpad)
-{
-    return n_rows >= TC_MIN_ROWS && n_rows < (1ll << 31) && dpad % (2 * TC_KBLOCK) == 0 && dense_tc_supported(di, dpad);
-}
 
 // Constants of the fetch rule (fetch_compact_kernel).  K1 (dense_scan_kernel, rescore_kernel) computes D = sum (x_i - q_i)^2
 // over nonnegative terms; every term passes through at most m = dpad / 32 + 7 roundings to nearest: its difference (squared:
@@ -846,72 +842,104 @@ static float certify_slack_rel(int dpad)
 static std::atomic<int64_t> g_host_rows_fetched{0};
 int64_t host_rows_fetched() { return g_host_rows_fetched.load(); }
 
-// one launch of a prune kernel (sample pass: DUMP) over n_ltiles tiles, tile_stride apart
-template <int NQ, int MODE, bool DUMP>
-static void tc_launch(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensorMap& tmQ, int64_t n_rows, int dpad,
-                      int64_t n_ltiles, int tile_stride, const float* xnorm, const uint32_t* alive, const float* thr,
-                      uint32_t* cand_count, uint32_t* cand_rows, int cap, float* dump, int64_t S, int dump_min, cudaStream_t st)
+// What a prune operand fixes besides its main kernel and rows (tc_pass): the kernel id krag_last_dense_kernel reports,
+// whether the main pass multiplies bf16 operands (2 bytes per element, the bf16 error bound, a wider candidate margin) and
+// the rows per tile of its kernel
+struct TcOpInfo { int kernel_id; bool bf16; int tile_rows; };
+static constexpr TcOpInfo TC_OPS[] = {{3, false, TC_TILE_M} /* TF32 */, {3, false, TC_TILE_M} /* TF32S */,
+                                      {5, true, TC16_TILE_M} /* BF16_SPLIT */, {4, true, TC16_TILE_M} /* BF16_SHADOW */,
+                                      {6, true, TC16_TILE_M} /* BF16_HOST */};
+
+TcOp tc_operand(const DenseRows& r, bool shadow, bool tf32)
 {
-    using Cfg = TcCfg<NQ, MODE>;
-    static bool attr_set = false;
-    if (!attr_set) {
-        KRAG_CUDA(cudaFuncSetAttribute(dense_tc_kernel<NQ, MODE, DUMP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM));
-        attr_set = true;
-    }
-    const int grid = (int)(n_ltiles < di.sm_count ? n_ltiles : di.sm_count);
-    dense_tc_kernel<NQ, MODE, DUMP><<<grid, TC_THREADS, Cfg::SMEM, st>>>(tmX, tmQ, n_rows, dpad / Cfg::ELEMS, n_ltiles, tile_stride,
-                                                                         xnorm, alive, thr, cand_count, cand_rows, cap, dump, S, dump_min);
-}
-// one launch of the bf16 kernel over the high halves of split rows (split) or over bf16 rows, with the nq bf16 queries qh:
-// n_ltiles tiles, row_step rows apart.  A k-block steps 2 pieces on split rows (high- and low-half pieces interleave), 1 on
-// bf16 rows
-template <int NQ, bool DUMP>
-static void tc16_launch(const DeviceInfo& di, const void* rows, bool split, const uint16_t* qh, int nq, int64_t n_rows, int dpad,
-                        int64_t n_ltiles, int row_step, const float* xnorm, const uint32_t* alive, const float* thr,
-                        uint32_t* cand_count, uint32_t* cand_rows, int cap, float* dump, int64_t S, int dump_min, cudaStream_t st)
-{
-    using Cfg = Tc16Cfg<NQ>;
-    CUtensorMap tmX, tmQ;
-    if (!make_map(&tmQ, (const void*)qh, nq, dpad, NQ, true) || !make_map_pieces(&tmX, rows, n_rows, dpad, split, TC16_TILE_M))
-        throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled(bf16 pass)", __FILE__, __LINE__};
-    static bool attr_set = false;
-    if (!attr_set) {
-        KRAG_CUDA(cudaFuncSetAttribute(dense_tc_bf16_kernel<NQ, DUMP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM));
-        attr_set = true;
-    }
-    const int grid = (int)(n_ltiles < di.sm_count ? n_ltiles : di.sm_count);
-    dense_tc_bf16_kernel<NQ, DUMP><<<grid, TC16_THREADS, Cfg::SMEM, st>>>(tmX, tmQ, n_rows, dpad / Cfg::ELEMS, split ? 2 : 1, n_ltiles,
-                                                                          row_step, xnorm, alive, thr, cand_count, cand_rows,
-                                                                          cap, dump, S, dump_min);
+    if (r.host()) return TC_OP_BF16_HOST;
+    if (shadow && r.bf16() && r.dpad % (2 * TC_KBLOCK) == 0) return TC_OP_BF16_SHADOW;   // bf16 k-blocks are 64 elements wide
+    if (!r.split()) return TC_OP_TF32;
+    return tf32 ? TC_OP_TF32S : TC_OP_BF16_SPLIT;
 }
 
-template <int NQ>
-static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensorMap& tmQ, const float* X, int64_t n_rows,
-                    int dpad, const float* xnorm, const uint32_t* xn_max_bits, const uint32_t* alive, const float* q,
-                    int nq, int P, OrdMap ord_base, const TcWorkspace& w, int cap, int64_t S, uint64_t* keys_out,
-                    const uint16_t* Xh, bool split, bool allow_bf16, const HostRowsView* hr, cudaStream_t st)
+bool dense_tc_serves(const DeviceInfo& di, const DenseRows& r, TcOp op)
 {
-    const bool host = hr != nullptr;             // fp32 rows in pinned host memory: both passes read the bf16 copy Xh
-    // bf16 operands in the prune pass: a bf16 copy Xh (shadow, host rows) or the high halves of split rows (X)
-    const bool bf16 = Xh != nullptr || (split && allow_bf16);
+    return dense_tc_supported(di, r.dpad) && r.n >= TC_MIN_ROWS && r.n < (1ll << 31) &&
+           (!TC_OPS[op].bf16 || r.dpad % (2 * TC_KBLOCK) == 0);   // bf16 k-blocks are 64 elements wide
+}
+
+// the TF32 kernels' map of device rows: 3-D pieces of split rows, 2-D fp32 rows otherwise
+static bool make_rows_map(CUtensorMap* tm, const DenseRows& r)
+{
+    return r.split() ? make_map_pieces(tm, r.dev(), r.n, r.dpad, true, TC_TILE_M) : make_map(tm, r.dev(), r.n, r.dpad, TC_TILE_M);
+}
+
+// the queries as op's bf16 operand: rounded to nearest even, in the split rows' lane order inside each 64-element block for
+// their high halves.  The TF32 kernels read the fp32 queries.
+static void tc_queries(TcOp op, const float* q, int nq, int dpad, uint16_t* qh, cudaStream_t st)
+{
+    if (op == TC_OP_BF16_SPLIT) launch_bf16_split_order(q, qh, (int64_t)nq * dpad, st);
+    else if (TC_OPS[op].bf16) launch_f32_to_bf16(q, qh, (int64_t)nq * dpad, st);
+}
+
+// op's prune kernel over n_tiles tiles, row_step rows apart: the main pass (rows below thr go to the candidate lists), or with
+// DUMP the dump of a (dump_min: per 16-row group, the sample pass; otherwise per row, in the columns up to S).  The bf16
+// kernel reads the high halves of split rows (its k-blocks step 2 pieces: high- and low-half pieces interleave) or bf16 rows,
+// with the bf16 queries qh; the TF32 kernels read the maps tmX and tmQ.
+template <int NQ, bool DUMP>
+static void tc_prune(const DeviceInfo& di, const DenseRows& r, TcOp op, const CUtensorMap& tmX, const CUtensorMap& tmQ,
+                     const uint16_t* qh, int nq, int64_t n_tiles, int row_step, const uint32_t* alive, const float* thr,
+                     uint32_t* cand_count, uint32_t* cand_rows, int cap, float* dump, int64_t S, int dump_min, cudaStream_t st)
+{
+    using C16 = Tc16Cfg<NQ>;
+    using C32 = TcCfg<NQ, TC_TF32>;
+    using C32S = TcCfg<NQ, TC_TF32S>;
+    static bool attr_set = false;
+    if (!attr_set) {
+        KRAG_CUDA(cudaFuncSetAttribute(dense_tc_bf16_kernel<NQ, DUMP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C16::SMEM));
+        KRAG_CUDA(cudaFuncSetAttribute(dense_tc_kernel<NQ, TC_TF32, DUMP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C32::SMEM));
+        KRAG_CUDA(cudaFuncSetAttribute(dense_tc_kernel<NQ, TC_TF32S, DUMP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C32S::SMEM));
+        attr_set = true;
+    }
+    const int grid = (int)(n_tiles < di.sm_count ? n_tiles : di.sm_count);
+    if (TC_OPS[op].bf16) {
+        const bool split = op == TC_OP_BF16_SPLIT;
+        CUtensorMap tmR, tmQh;
+        if (!make_map(&tmQh, qh, nq, r.dpad, NQ, true) ||
+            !make_map_pieces(&tmR, split ? (const void*)r.dev() : (const void*)r.bf16(), r.n, r.dpad, split, TC16_TILE_M))
+            throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled(bf16 pass)", __FILE__, __LINE__};
+        dense_tc_bf16_kernel<NQ, DUMP><<<grid, TC16_THREADS, C16::SMEM, st>>>(tmR, tmQh, r.n, r.dpad / C16::ELEMS, split ? 2 : 1, n_tiles,
+                                                                              row_step, r.norms(), alive, thr, cand_count, cand_rows,
+                                                                              cap, dump, S, dump_min);
+    } else if (op == TC_OP_TF32S) {
+        dense_tc_kernel<NQ, TC_TF32S, DUMP><<<grid, TC_THREADS, C32S::SMEM, st>>>(tmX, tmQ, r.n, r.dpad / C32S::ELEMS, n_tiles,
+                                                                                  row_step / TC_TILE_M, r.norms(), alive, thr,
+                                                                                  cand_count, cand_rows, cap, dump, S, dump_min);
+    } else {
+        dense_tc_kernel<NQ, TC_TF32, DUMP><<<grid, TC_THREADS, C32::SMEM, st>>>(tmX, tmQ, r.n, r.dpad / C32::ELEMS, n_tiles,
+                                                                                row_step / TC_TILE_M, r.norms(), alive, thr,
+                                                                                cand_count, cand_rows, cap, dump, S, dump_min);
+    }
+}
+
+// One K2 pass of nq <= NQ queries.  Besides the main kernel, op decides the sample kernel (TC_TF32 on plain rows, TC_TF32S
+// on split rows, the bf16 kernel on host rows' copy), the rescoring (from device rows, or refined on the copy and fetched
+// from host rows) and eps_rel.
+template <int NQ>
+static void tc_pass(const DeviceInfo& di, const DenseRows& r, TcOp op, const CUtensorMap& tmX, const CUtensorMap& tmQ,
+                    const uint32_t* alive, const float* q, int nq, int P, OrdMap ord_base, const TcWorkspace& w, int cap,
+                    uint64_t* keys_out, cudaStream_t st)
+{
+    const int64_t n_rows = r.n;
+    const int dpad = r.dpad;
+    const bool host = op == TC_OP_BF16_HOST, bf16 = TC_OPS[op].bf16;
+    tc_queries(op, q, nq, dpad, w.q_bf16, st);
     // 1. sample pass, dump a = |x|^2 - 2 x.q: one tile at the start of every TC_SAMPLE_STRIDE 128-row tiles, so every pass
-    // samples the same rows first; bf16 on host rows (192-row tiles), TF32 otherwise (128-row tiles)
+    // samples the same rows first; bf16 on host rows (192-row tiles), TF32 otherwise (128-row tiles).  The sample pass only
+    // chooses thr: its operands do not enter soundness.
     // the dump holds one value per (16-row group of a sampled tile, query): S_min per query
-    const int sample_m = host ? TC16_TILE_M : TC_TILE_M;
+    const TcOp sample_op = host ? op : (r.split() ? TC_OP_TF32S : TC_OP_TF32);
+    const int sample_m = TC_OPS[sample_op].tile_rows;
     const int64_t s_tiles = tc_sample_tiles(n_rows);
     const int64_t S_min = s_tiles * (sample_m / TC_DUMP_GROUP);
-    (void)S;
-    if (host) {   // the sample pass only chooses thr: bf16 operands do not enter soundness
-        launch_f32_to_bf16(q, w.q_bf16, (int64_t)nq * dpad, st);
-        tc16_launch<NQ, true>(di, Xh, false, w.q_bf16, nq, n_rows, dpad, s_tiles, TC_SAMPLE_STRIDE * TC_TILE_M, xnorm, alive,
-                              nullptr, nullptr, nullptr, 0, w.dump, S_min, 1, st);
-    } else if (split) {
-        tc_launch<NQ, TC_TF32S, true>(di, tmX, tmQ, n_rows, dpad, s_tiles, TC_SAMPLE_STRIDE, xnorm, alive, nullptr, nullptr, nullptr, 0,
-                                      w.dump, S_min, 1, st);
-    } else {
-        tc_launch<NQ, TC_TF32, true>(di, tmX, tmQ, n_rows, dpad, s_tiles, TC_SAMPLE_STRIDE, xnorm, alive, nullptr, nullptr, nullptr, 0,
-                                     w.dump, S_min, 1, st);
-    }
+    tc_prune<NQ, true>(di, r, sample_op, tmX, tmQ, w.q_bf16, nq, s_tiles, TC_SAMPLE_STRIDE * TC_TILE_M, alive, nullptr, nullptr,
+                       nullptr, 0, w.dump, S_min, 1, st);
     KRAG_CUDA(cudaGetLastError());
     count_launch();
     // 2. threshold admitting ~C rows: the m-th smallest of the sample, m = C * sample_fraction
@@ -931,22 +959,10 @@ static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensor
     count_launch();
     KRAG_CUDA(cudaMemsetAsync(w.cand_count, 0, 256 * 4, st));
     // 3. main pass: stream the corpus once, prune on the tensor cores
-    // split rows: queries in the rows' lane order inside each 64-element block
-    if (Xh && !host) launch_f32_to_bf16(q, w.q_bf16, (int64_t)nq * dpad, st);
-    else if (bf16 && !host) launch_bf16_split_order(q, w.q_bf16, (int64_t)nq * dpad, st);
-    // kernel ids: 6 host rows' bf16 copy, 4 bf16 shadow, 5 high halves of split rows, 3 tf32
-    dense_timer_begin(st, host ? 6 : (Xh ? 4 : (bf16 ? 5 : 3)), n_rows * (int64_t)dpad * (bf16 ? 2 : 4), 2 * (int64_t)NQ * n_rows * dpad);
-    if (bf16) {
-        const int64_t n_tiles = (n_rows + TC16_TILE_M - 1) / TC16_TILE_M;
-        tc16_launch<NQ, false>(di, Xh ? (const void*)Xh : (const void*)X, Xh == nullptr, w.q_bf16, nq, n_rows, dpad, n_tiles,
-                               TC16_TILE_M, xnorm, alive, w.thr, w.cand_count, w.cand_rows, cap, nullptr, 0, 0, st);
-    } else {
-        const int64_t n_tiles = (n_rows + TC_TILE_M - 1) / TC_TILE_M;
-        if (split) tc_launch<NQ, TC_TF32S, false>(di, tmX, tmQ, n_rows, dpad, n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows,
-                                                  cap, nullptr, 0, 0, st);
-        else tc_launch<NQ, TC_TF32, false>(di, tmX, tmQ, n_rows, dpad, n_tiles, 1, xnorm, alive, w.thr, w.cand_count, w.cand_rows,
-                                           cap, nullptr, 0, 0, st);
-    }
+    dense_timer_begin(st, TC_OPS[op].kernel_id, n_rows * (int64_t)dpad * (bf16 ? 2 : 4), 2 * (int64_t)NQ * n_rows * dpad);
+    const int tile = TC_OPS[op].tile_rows;
+    tc_prune<NQ, false>(di, r, op, tmX, tmQ, w.q_bf16, nq, (n_rows + tile - 1) / tile, tile, alive, w.thr, w.cand_count, w.cand_rows,
+                        cap, nullptr, 0, 0, st);
     dense_timer_end(st);
     KRAG_CUDA(cudaGetLastError());
     count_launch();
@@ -967,7 +983,7 @@ static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensor
             KRAG_CUDA(cudaFuncSetAttribute(rescore_mapped_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 4));
             rf_attr_set = true;
         }
-        refine_kernel<<<rg, 256, (size_t)dpad * 4, st>>>(Xh, hr->xres, dpad, q, w.cand_count, w.cand_rows, cap, w.lo, w.exact_keys);
+        refine_kernel<<<rg, 256, (size_t)dpad * 4, st>>>(r.bf16(), r.res(), dpad, q, w.cand_count, w.cand_rows, cap, w.lo, w.exact_keys);
         KRAG_CUDA(cudaGetLastError());
         count_launch();
         launch_merge(w.exact_keys, 1, cap, nq, P, cap, cap, keys_out, st);
@@ -978,18 +994,18 @@ static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensor
             w.cand_count, w.cand_rows, cap, w.lo, keys_out, P, scale, eta2, w.fetch_count, w.fetch_rows);
         KRAG_CUDA(cudaGetLastError());
         count_launch();
-        rescore_mapped_kernel<<<rg, 256, (size_t)dpad * 4, st>>>(hr->d, dpad, q, w.fetch_count, w.fetch_rows, cap, ord_base,
+        rescore_mapped_kernel<<<rg, 256, (size_t)dpad * 4, st>>>(r.host_d(), dpad, q, w.fetch_count, w.fetch_rows, cap, ord_base,
                                                                  w.exact_keys);
     } else {
-        if (split) rescore_kernel<true><<<rg, 256, (size_t)dpad * 4, st>>>(X, dpad, q, w.cand_count, w.cand_rows, cap, ord_base, w.exact_keys);
-        else rescore_kernel<false><<<rg, 256, (size_t)dpad * 4, st>>>(X, dpad, q, w.cand_count, w.cand_rows, cap, ord_base, w.exact_keys);
+        if (r.split()) rescore_kernel<true><<<rg, 256, (size_t)dpad * 4, st>>>(r.dev(), dpad, q, w.cand_count, w.cand_rows, cap, ord_base, w.exact_keys);
+        else rescore_kernel<false><<<rg, 256, (size_t)dpad * 4, st>>>(r.dev(), dpad, q, w.cand_count, w.cand_rows, cap, ord_base, w.exact_keys);
     }
     KRAG_CUDA(cudaGetLastError());
     count_launch();
     launch_merge(w.exact_keys, 1, cap, nq, P, cap, cap, keys_out, st);
     // 5. certificate: the error bound of the main pass's operands (the sample pass only chooses thr, whatever its value)
     const float eps_rel = bf16 ? (0.0078125f + 0.000244140625f) : (0.001953125f + 0.000244140625f);
-    certify_kernel<<<(nq * 32 + 255) / 256, 256, 0, st>>>(q, dpad, nq, P, w.thr, w.cand_count, cap, keys_out, xn_max_bits, eps_rel,
+    certify_kernel<<<(nq * 32 + 255) / 256, 256, 0, st>>>(q, dpad, nq, P, w.thr, w.cand_count, cap, keys_out, r.norm_max(), eps_rel,
                                                           certify_slack_rel(dpad), w.flags);
     KRAG_CUDA(cudaGetLastError());
     count_launch();
@@ -998,85 +1014,56 @@ static void tc_pass(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensor
 static std::atomic<int64_t> g_tc_fallback_queries{0};   // searches run concurrently (reader lock)
 int64_t dense_tc_fallback_queries() { return g_tc_fallback_queries.load(); }
 
-bool launch_dense_tc(const DeviceInfo& di, const float* X, int64_t n_rows, int dpad, const uint32_t* alive,
-                     const float* xnorm, const uint32_t* xn_max_bits, const float* q, int batch, int P, OrdMap ord_base,
-                     void* workspace, size_t workspace_bytes, uint64_t* part, uint64_t* keys_out, cudaStream_t st,
-                     const uint16_t* Xh, bool allow_bf16, bool split)
+bool launch_dense_tc(const DeviceInfo& di, const DenseRows& r, TcOp op, const uint32_t* alive, const float* q, int batch,
+                     int P, OrdMap ord_base, void* workspace, size_t workspace_bytes, uint64_t* part, const ScanStaging* sg,
+                     uint64_t* keys_out, cudaStream_t st)
 {
-    if (Xh != nullptr && dpad % (2 * TC_KBLOCK) != 0) Xh = nullptr;   // bf16 k-blocks are 64 elements wide
-    // default prune pass on split rows: bf16 wgmma on their high halves; allow_bf16 = false keeps the TF32 pass
-    if (n_rows < TC_MIN_ROWS || n_rows >= (1ll << 31) || xnorm == nullptr) return false;
+    const int64_t n_rows = r.n;
+    const int dpad = r.dpad;
+    const bool host = op == TC_OP_BF16_HOST;
     const int cap = tc_cap(P);
-    const int64_t S = tc_sample_tiles(n_rows) * TC_TILE_M;
     TcWorkspace w;
-    if (tc_carve(&w, (unsigned char*)workspace, cap, S) > workspace_bytes) return false;
-    CUtensorMap tmX;
-    if (!(split ? make_map_pieces(&tmX, X, n_rows, dpad, true, TC_TILE_M) : make_map(&tmX, X, n_rows, dpad, TC_TILE_M))) return false;
+    if (tc_carve(&w, (unsigned char*)workspace, cap, tc_sample_tiles(n_rows) * TC_TILE_M, host) > workspace_bytes) return false;
+    // the maps of the TF32 kernels, which do not run on host rows; tmX is encoded once per call
+    CUtensorMap tmX{}, tmQ{};
+    if (!host && !make_rows_map(&tmX, r)) return false;
     std::vector<int32_t> flags(256);
+    std::vector<uint32_t> fetched(host ? 256 : 0);   // host rows: rows each query fetched from host memory
     for (int b0 = 0; b0 < batch; b0 += 256) {
         const int nq = batch - b0 < 256 ? batch - b0 : 256;
         const int NQ = nq <= 64 ? 64 : (nq <= 128 ? 128 : 256);
         const float* qb = q + (size_t)b0 * dpad;
-        CUtensorMap tmQ;
-        if (!make_map(&tmQ, qb, nq, dpad, NQ)) return false;
+        if (!host && !make_map(&tmQ, qb, nq, dpad, NQ)) return false;
         uint64_t* ko = keys_out + (size_t)b0 * P;
-        if (NQ == 64) tc_pass<64>(di, tmX, tmQ, X, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, Xh, split, allow_bf16, nullptr, st);
-        else if (NQ == 128) tc_pass<128>(di, tmX, tmQ, X, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, Xh, split, allow_bf16, nullptr, st);
-        else tc_pass<256>(di, tmX, tmQ, X, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, Xh, split, allow_bf16, nullptr, st);
-        // uncertified queries (rare) are re-run on the exact scan kernel -- still on the GPU
+        (NQ == 64 ? tc_pass<64> : NQ == 128 ? tc_pass<128> : tc_pass<256>)(di, r, op, tmX, tmQ, alive, qb, nq, P, ord_base, w, cap, ko, st);
         KRAG_CUDA(cudaMemcpyAsync(flags.data(), w.flags, sizeof(int32_t) * (size_t)nq, cudaMemcpyDeviceToHost, st));
+        if (host) KRAG_CUDA(cudaMemcpyAsync(fetched.data(), w.fetch_count, sizeof(uint32_t) * (size_t)nq, cudaMemcpyDeviceToHost, st));
         KRAG_CUDA(cudaStreamSynchronize(st));
-        for (int j = 0; j < nq; ++j) {
-            if (flags[(size_t)j]) continue;
-            ++g_tc_fallback_queries;
-            launch_dense_scan(di, X, n_rows, dpad, alive, qb + (size_t)j * dpad, 1, P, ord_base, part, ko + (size_t)j * P, st, split);
-        }
-    }
-    return true;
-}
-
-// K2 over host-resident rows: sample and main pass on the device bf16 copy, refine + fetch + zero-copy rescoring from the
-// pinned fp32 rows, the same certificate; uncertified queries go through the streamed exact scan together
-bool launch_dense_tc_host(const DeviceInfo& di, const HostRowsView& hr, int64_t n_rows, int dpad, const uint32_t* alive,
-                          const float* xnorm, const uint32_t* xn_max_bits, const float* q, int batch, int P, OrdMap ord_base,
-                          void* workspace, size_t workspace_bytes, uint64_t* part, const ScanStaging& sg, uint64_t* keys_out,
-                          cudaStream_t st)
-{
-    if (!dense_tc_host_rows_supported(di, n_rows, dpad) || xnorm == nullptr) return false;
-    const int cap = tc_cap(P);
-    const int64_t S = tc_sample_tiles(n_rows) * TC_TILE_M;
-    TcWorkspace w;
-    if (tc_carve(&w, (unsigned char*)workspace, cap, S, true) > workspace_bytes) return false;
-    CUtensorMap unused{};   // the fp32 maps are not read in host mode
-    std::vector<int32_t> flags(256);
-    std::vector<uint32_t> fetched(256);
-    for (int b0 = 0; b0 < batch; b0 += 256) {
-        const int nq = batch - b0 < 256 ? batch - b0 : 256;
-        const int NQ = nq <= 64 ? 64 : (nq <= 128 ? 128 : 256);
-        const float* qb = q + (size_t)b0 * dpad;
-        uint64_t* ko = keys_out + (size_t)b0 * P;
-        if (NQ == 64) tc_pass<64>(di, unused, unused, nullptr, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, hr.bf16, false, false, &hr, st);
-        else if (NQ == 128) tc_pass<128>(di, unused, unused, nullptr, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, hr.bf16, false, false, &hr, st);
-        else tc_pass<256>(di, unused, unused, nullptr, n_rows, dpad, xnorm, xn_max_bits, alive, qb, nq, P, ord_base, w, cap, S, ko, hr.bf16, false, false, &hr, st);
-        KRAG_CUDA(cudaMemcpyAsync(flags.data(), w.flags, sizeof(int32_t) * (size_t)nq, cudaMemcpyDeviceToHost, st));
-        KRAG_CUDA(cudaMemcpyAsync(fetched.data(), w.fetch_count, sizeof(uint32_t) * (size_t)nq, cudaMemcpyDeviceToHost, st));
-        KRAG_CUDA(cudaStreamSynchronize(st));
-        int64_t rows = 0;
         int nf = 0;
-        for (int j = 0; j < nq; ++j) {
-            rows += fetched[(size_t)j] < (uint32_t)cap ? fetched[(size_t)j] : (uint32_t)cap;
-            if (flags[(size_t)j]) continue;
-            KRAG_CUDA(cudaMemcpyAsync(sg.q_sel + (size_t)nf * dpad, qb + (size_t)j * dpad, sizeof(float) * (size_t)dpad,
-                                      cudaMemcpyDeviceToDevice, st));
-            flags[(size_t)nf++] = j;   // flags[0, nf) now lists the uncertified queries
+        for (int j = 0; j < nq; ++j)
+            if (!flags[(size_t)j]) flags[(size_t)nf++] = j;   // flags[0, nf) now lists the uncertified queries
+        // uncertified queries (rare) are re-run on the exact scan -- still on the GPU: one by one on device rows, together
+        // in one streamed scan of host rows
+        if (!host) {
+            for (int i = 0; i < nf; ++i) {
+                ++g_tc_fallback_queries;
+                launch_dense_scan(di, r, alive, qb + (size_t)flags[(size_t)i] * dpad, 1, P, ord_base, part, ko + (size_t)flags[(size_t)i] * P, st);
+            }
+            continue;
         }
+        int64_t rows = 0;
+        for (int j = 0; j < nq; ++j) rows += fetched[(size_t)j] < (uint32_t)cap ? fetched[(size_t)j] : (uint32_t)cap;
         g_host_rows_fetched += rows;
-        if (nf == 0) continue;
-        g_tc_fallback_queries += nf;
-        launch_dense_scan_streamed(di, hr.h, n_rows, dpad, alive, sg.q_sel, nf, P, ord_base, part, sg, sg.k_sel, st);
-        for (int i = 0; i < nf; ++i)
-            KRAG_CUDA(cudaMemcpyAsync(ko + (size_t)flags[(size_t)i] * P, sg.k_sel + (size_t)i * P, sizeof(uint64_t) * (size_t)P,
-                                      cudaMemcpyDeviceToDevice, st));
+        if (nf > 0) {
+            g_tc_fallback_queries += nf;
+            for (int i = 0; i < nf; ++i)
+                KRAG_CUDA(cudaMemcpyAsync(sg->q_sel + (size_t)i * dpad, qb + (size_t)flags[(size_t)i] * dpad, sizeof(float) * (size_t)dpad,
+                                          cudaMemcpyDeviceToDevice, st));
+            launch_dense_scan(di, r, alive, sg->q_sel, nf, P, ord_base, part, sg->k_sel, st, sg);
+            for (int i = 0; i < nf; ++i)
+                KRAG_CUDA(cudaMemcpyAsync(ko + (size_t)flags[(size_t)i] * P, sg->k_sel + (size_t)i * P, sizeof(uint64_t) * (size_t)P,
+                                          cudaMemcpyDeviceToDevice, st));
+        }
     }
     return true;
 }
@@ -1104,59 +1091,26 @@ size_t dense_tc_debug_carve(TcDebugWs* w, unsigned char* base, int64_t n_rows, i
     return o;
 }
 
-template <int NQ, int MODE>
-static void tc_debug_launch(const DeviceInfo& di, const CUtensorMap& tmX, const CUtensorMap& tmQ, int64_t n_rows, int dpad,
-                            const float* xnorm, const uint32_t* alive, const TcDebugWs& w, int cap, cudaStream_t st)
+bool dense_tc_debug_pass(const DeviceInfo& di, const DenseRows& r, TcOp op, const uint32_t* alive, const float* q, int nq,
+                         const TcDebugWs& w, int cap, cudaStream_t st)
 {
-    const int64_t n_tiles = (n_rows + TC_TILE_M - 1) / TC_TILE_M;
-    if (cap == 0)   // as a sample pass, but over every tile and every row (dump_min = 0)
-        tc_launch<NQ, MODE, true>(di, tmX, tmQ, n_rows, dpad, n_tiles, 1, xnorm, nullptr, nullptr, nullptr, nullptr, 0,
-                                  w.dump, n_tiles * TC_TILE_M, 0, st);
-    else            // the main pass of tc_pass
-        tc_launch<NQ, MODE, false>(di, tmX, tmQ, n_rows, dpad, n_tiles, 1, xnorm, alive, w.thr, w.cand_count,
-                                   w.cand_rows, cap, nullptr, 0, 0, st);
-}
-
-template <int NQ>
-static bool tc_debug_pass(const DeviceInfo& di, int pass, const float* X, const uint16_t* Xh, bool split, int64_t n_rows, int dpad,
-                          const float* xnorm, const uint32_t* alive, const float* q, int nq, const TcDebugWs& w, int cap, cudaStream_t st)
-{
-    if (pass == 0) {   // TF32: fp32 queries straight from the caller's rows
-        CUtensorMap tmX, tmQ;
-        if (!(split ? make_map_pieces(&tmX, X, n_rows, dpad, true, TC_TILE_M) : make_map(&tmX, X, n_rows, dpad, TC_TILE_M)) ||
-            !make_map(&tmQ, q, nq, dpad, NQ))
-            return false;
-        if (split) tc_debug_launch<NQ, TC_TF32S>(di, tmX, tmQ, n_rows, dpad, xnorm, alive, w, cap, st);
-        else tc_debug_launch<NQ, TC_TF32>(di, tmX, tmQ, n_rows, dpad, xnorm, alive, w, cap, st);
-        return true;
-    }
-    // bf16: the queries converted as tc_pass converts them for the same rows
-    if (pass == 1) launch_bf16_split_order(q, w.q_bf16, (int64_t)nq * dpad, st);
-    else launch_f32_to_bf16(q, w.q_bf16, (int64_t)nq * dpad, st);
-    const void* rows = pass == 1 ? (const void*)X : (const void*)Xh;
-    const int64_t S = (n_rows + TC_TILE_M - 1) / TC_TILE_M * TC_TILE_M;
-    if (cap == 0)   // as the host-rows sample pass, but over every row and the padding columns up to S (dump_min = 0)
-        tc16_launch<NQ, true>(di, rows, pass == 1, w.q_bf16, nq, n_rows, dpad, (S + TC16_TILE_M - 1) / TC16_TILE_M, TC16_TILE_M,
-                              xnorm, nullptr, nullptr, nullptr, nullptr, 0, w.dump, S, 0, st);
-    else
-        tc16_launch<NQ, false>(di, rows, pass == 1, w.q_bf16, nq, n_rows, dpad, (n_rows + TC16_TILE_M - 1) / TC16_TILE_M, TC16_TILE_M, xnorm,
-                               alive, w.thr, w.cand_count, w.cand_rows, cap, nullptr, 0, 0, st);
-    return true;
-}
-
-bool dense_tc_debug_pass(const DeviceInfo& di, int pass, const float* X, const uint16_t* Xh, bool split, int64_t n_rows, int dpad,
-                         const float* xnorm, const uint32_t* alive, const float* q, int nq, const TcDebugWs& w, int cap,
-                         cudaStream_t st)
-{
-    if (!dense_tc_supported(di, dpad) || nq < 1 || nq > 256 || n_rows < 1 || n_rows >= (1ll << 31)) return false;
-    if (pass < 0 || pass > 3 || (pass == 1 && !split) || (pass >= 2 && (Xh == nullptr || dpad % (2 * TC_KBLOCK) != 0))) return false;
+    if (!dense_tc_supported(di, r.dpad) || nq < 1 || nq > 256 || r.n < 1 || r.n >= (1ll << 31)) return false;
+    if (op == TC_OP_BF16_SPLIT ? !r.split() : TC_OPS[op].bf16 && (!r.bf16() || r.dpad % (2 * TC_KBLOCK) != 0)) return false;
     const int NQ = nq <= 64 ? 64 : (nq <= 128 ? 128 : 256);
+    // TF32: fp32 queries straight from the caller's rows; bf16: the queries converted as tc_pass converts them
+    CUtensorMap tmX{}, tmQ{};
+    if (!TC_OPS[op].bf16 && (!make_rows_map(&tmX, r) || !make_map(&tmQ, q, nq, r.dpad, NQ))) return false;
+    tc_queries(op, q, nq, r.dpad, w.q_bf16, st);
+    // cap == 0: as a sample pass, but over every row and the padding columns up to S; cap > 0: the main pass of tc_pass.
+    // w holds the dump or the candidate lists, and null for the other.
+    const int tile = TC_OPS[op].tile_rows;
+    const int64_t S = (r.n + TC_TILE_M - 1) / TC_TILE_M * TC_TILE_M;
     if (cap > 0) KRAG_CUDA(cudaMemsetAsync(w.cand_count, 0, (size_t)NQ * 4, st));
-    bool ok;
-    if (NQ == 64) ok = tc_debug_pass<64>(di, pass, X, Xh, split, n_rows, dpad, xnorm, alive, q, nq, w, cap, st);
-    else if (NQ == 128) ok = tc_debug_pass<128>(di, pass, X, Xh, split, n_rows, dpad, xnorm, alive, q, nq, w, cap, st);
-    else ok = tc_debug_pass<256>(di, pass, X, Xh, split, n_rows, dpad, xnorm, alive, q, nq, w, cap, st);
-    if (!ok) return false;
+    const bool dump = cap == 0;
+    (NQ == 64 ? (dump ? tc_prune<64, true> : tc_prune<64, false>) : NQ == 128 ? (dump ? tc_prune<128, true> : tc_prune<128, false>)
+                                                                   : (dump ? tc_prune<256, true> : tc_prune<256, false>))(
+        di, r, op, tmX, tmQ, w.q_bf16, nq, ((dump ? S : r.n) + tile - 1) / tile, tile, alive, w.thr, w.cand_count, w.cand_rows, cap,
+        w.dump, dump ? S : 0, 0, st);
     KRAG_CUDA(cudaGetLastError());
     count_launch();
     return true;

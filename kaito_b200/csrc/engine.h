@@ -209,21 +209,63 @@ bool dense_timer_read(float* ms, int* kernel_id, int64_t* bytes, int64_t* flops)
 void count_launch(int n = 1);
 int64_t launch_count();
 
-// ---- K1: exact fp32 L2^2 scan + fused top-P (dense_scan.cu)
-// q: device [batch, dpad] zero-padded.  part: workspace >= dense_scan_part_elems() u64.
-// keys_out: device [batch, P], ascending, KEY_PAD padded, ordinals already global.  split: X holds split rows (split_rows.cuh).
-size_t dense_scan_part_elems(const DeviceInfo& di, int P);
-void launch_dense_scan(const DeviceInfo& di, const float* X, int64_t n_rows, int dpad, const uint32_t* alive,
-                       const float* q, int batch, int P, OrdMap ord_base, uint64_t* part, uint64_t* keys_out,
-                       cudaStream_t st, bool split);
+// ---- the dense rows of an index (dense_rows.cu): the rows in one of three layouts, and what is kept per row beside them
+struct CompactPlan;
+struct RedealRows;
+// PLAIN: fp32 rows on the device (dpad % 64 == 32).  SPLIT: split rows on the device (split_rows.cuh, dpad % 64 == 0).
+// HOST: fp32 rows in pinned host memory (KRAG_ROWS_HOST), with a bf16 copy and its residuals on the device.
+enum class RowsLayout { PLAIN, SPLIT, HOST };
+class DenseRows {
+public:
+    int dim = 0, dpad = 0;
+    int64_t n = 0;                           // rows held
+    RowsLayout layout = RowsLayout::PLAIN;   // decided once, by init
 
-// ---- host-resident rows (KRAG_ROWS_HOST): fp32 rows in pinned host memory, bf16 copy + residual norms on the device
-struct HostRowsView {
-    const float* h;          // host address of the fp32 rows [n_rows, dpad] (DMA source)
-    const float* d;          // the same memory through its mapped device address (zero-copy reads)
-    const uint16_t* bf16;    // device bf16 copy [n_rows, dpad]
-    const float* xres;       // device |x - bf16(x)| per row, rounded up
+    void init(int dim, bool host_rows);
+    bool host() const { return layout == RowsLayout::HOST; }
+    bool split() const { return layout == RowsLayout::SPLIT; }
+    // whether the rows keep a bf16 copy under this dense mode: host rows always; device rows as the KRAG_DENSE_TC_BF16
+    // shadow, which stays once built unless release asks to drop it.  Whenever the copy exists it covers every row.
+    bool keeps_bf16(int dense_mode, bool release = false) const;
+    // room for `rows` rows; a bf16 copy that keeps_bf16 asks for and that does not exist yet is built from the rows held
+    void reserve(int64_t rows, int dense_mode, cudaStream_t st);
+    // rows [n, n + m): host fp32 rows [m, dim] (append) or the synthetic rows of global rows row_base + r (synth), with their
+    // |x|^2, the running max, the bf16 copy and the stored layout.  The caller raises n once the rest of its update holds.
+    void append(const float* vecs, int64_t m, int dense_mode, cudaStream_t st);
+    void synth(int64_t m, int64_t row_base, uint64_t seed, int dense_mode, cudaStream_t st);
+    // rows [row0, row0 + m) as fp32 [m, dim] on the host; read_stored: device rows as stored, [m, dpad]
+    void read(int64_t row0, int64_t m, float* out) const;
+    void read_stored(int64_t row0, int64_t m, float* out) const;
+    // the bf16 shadow of device rows: built from the rows held when missing (on), or released (off); host rows keep their copy
+    void set_shadow(bool on, cudaStream_t st);
+    // row d <- row plan.src[d] in every array, in place; returns the bytes moved.  shrink: n = rows, the running max of
+    // |x|^2 over them, and exact-size buffers where they fit; synchronises st.
+    int64_t compact(const CompactPlan& plan, cudaStream_t st);
+    void shrink(int64_t rows, cudaStream_t st);
+    // a redeal's row view: these rows and the given term lists (null without)
+    RedealRows redeal_rows(uint32_t* dlen, const int64_t* toff, const uint32_t* tid, const uint16_t* ttf) const;
+    int64_t device_bytes() const;
+
+    // what the kernels read
+    const float* dev() const { return X.p; }        // device rows (PLAIN, SPLIT)
+    const float* host_h() const { return Xp.h; }    // host rows: their host address (DMA source)
+    const float* host_d() const { return Xp.d; }    // host rows: their mapped device address (zero-copy reads)
+    const uint16_t* bf16() const { return Xh.p; }   // the bf16 copy [n, dpad], or null
+    const float* res() const { return xres.p; }     // host rows: |x - bf16(x)| per row, rounded up
+    const float* norms() const { return xnorm.p; }  // |x|^2 per row (K2 epilogue), from the fp32 rows
+    const uint32_t* norm_max() const { return xn_max.p; }   // bits of max |x|^2 (K2 certificate)
+
+private:
+    DevArray<float> X;          // device rows [n, dpad], zero padded; split rows when SPLIT
+    HostArray<float> Xp;        // host rows [n, dpad], zero padded
+    DevArray<uint16_t> Xh;      // bf16 copy of the rows: optional shadow of device rows, always present for host rows
+    DevArray<float> xres;       // host rows only
+    DevArray<float> xnorm;
+    DevArray<uint32_t> xn_max;  // [1]
+    void derive(int64_t m, const uint64_t* gen_seed, int64_t row_base, cudaStream_t st);
+    void reserve_bf16(int64_t elems, cudaStream_t st);
 };
+
 // device staging of the streamed exact scan, owned by the search slot
 struct ScanStaging {
     float* buf[2];           // two chunks of chunk_rows rows (double buffering)
@@ -235,47 +277,46 @@ struct ScanStaging {
     uint64_t* k_sel;         // [256, P]
 };
 int64_t stream_scan_chunk_rows(int dpad);
-// K1, unchanged, over chunks of host rows copied in by DMA; each chunk's top P folded into the running list.  Exact.
-void launch_dense_scan_streamed(const DeviceInfo& di, const float* X_host, int64_t n_rows, int dpad, const uint32_t* alive,
-                                const float* q, int batch, int P, OrdMap ord_base, uint64_t* part, const ScanStaging& sg,
-                                uint64_t* keys_out, cudaStream_t st);
+
+// ---- K1: exact fp32 L2^2 scan + fused top-P (dense_scan.cu)
+// q: device [batch, dpad] zero-padded.  part: workspace >= dense_scan_part_elems() u64.
+// keys_out: device [batch, P], ascending, KEY_PAD padded, ordinals already global.  Device rows are scanned in place; host
+// rows are copied in by DMA in chunks through sg (required then), each chunk's top P folded into the running list.  Exact.
+size_t dense_scan_part_elems(const DeviceInfo& di, int P);
+void launch_dense_scan(const DeviceInfo& di, const DenseRows& rows, const uint32_t* alive, const float* q, int batch, int P,
+                       OrdMap ord_base, uint64_t* part, uint64_t* keys_out, cudaStream_t st, const ScanStaging* sg = nullptr);
 void launch_bf16_residual(const float* X, int64_t n, int dpad, uint16_t* Xh, float* xres, cudaStream_t st);
-bool dense_tc_host_rows_supported(const DeviceInfo& di, int64_t n_rows, int dpad);
-// returns false when K2 cannot serve the index (the caller runs the streamed scan)
-bool launch_dense_tc_host(const DeviceInfo& di, const HostRowsView& hr, int64_t n_rows, int dpad, const uint32_t* alive,
-                          const float* xnorm, const uint32_t* xn_max_bits, const float* q, int batch, int P, OrdMap ord_base,
-                          void* workspace, size_t workspace_bytes, uint64_t* part, const ScanStaging& sg, uint64_t* keys_out,
-                          cudaStream_t st);
 int64_t host_rows_fetched();   // rows rescored from host memory, process-wide
 
 // ---- K2: wgmma candidate generation + exact fp32 rescoring (dense_tc.cu)
+// The prune operand of a K2 pass: every choice that follows from it is a row of TC_OPS or a branch of tc_pass (dense_tc.cu).
+// The bf16 operands are KRAG_TC_PASS_* + 1.
+enum TcOp { TC_OP_TF32, TC_OP_TF32S, TC_OP_BF16_SPLIT, TC_OP_BF16_SHADOW, TC_OP_BF16_HOST };
+// the operand for these rows: shadow = prune on the bf16 shadow when there is one; tf32 = keep split rows on the TF32 pass
+TcOp tc_operand(const DenseRows& rows, bool shadow, bool tf32);
 bool dense_tc_supported(const DeviceInfo& di, int dpad);
 bool dense_tc_wants(int64_t n_rows, int batch);   // size heuristics: is K2 the better kernel for this call?
+bool dense_tc_serves(const DeviceInfo& di, const DenseRows& rows, TcOp op);   // can launch_dense_tc run op on these rows?
 size_t dense_tc_workspace_bytes(const DeviceInfo& di, int64_t n_rows, int P, bool host_rows = false);
 // |x|^2 per row (+ running max) maintained at index time for K2's epilogue and certificate
 void launch_row_norms(const float* X, int64_t row0, int64_t n, int dpad, float* xnorm, uint32_t* xn_max_bits,
                       cudaStream_t st);
-// returns false when the tensor-core path cannot serve the request (caller falls back to K1 -- still GPU)
-bool launch_dense_tc(const DeviceInfo& di, const float* X, int64_t n_rows, int dpad, const uint32_t* alive,
-                     const float* xnorm, const uint32_t* xn_max_bits, const float* q, int batch, int P,
-                     OrdMap ord_base, void* workspace, size_t workspace_bytes, uint64_t* part, uint64_t* keys_out,
-                     cudaStream_t st, const uint16_t* Xh /* optional bf16 shadow of X for the prune pass */,
-                     bool allow_bf16 /* split rows: bf16 wgmma on their high halves instead of tf32 wgmma */,
-                     bool split /* X holds split rows (split_rows.cuh) */);
+// For rows dense_tc_serves.  Returns false when the workspace or a tensor map does not fit (the caller runs K1 -- still GPU).
+// Queries the certificate rejects are re-run on K1 inside: one by one on device rows, together through sg on host rows.
+bool launch_dense_tc(const DeviceInfo& di, const DenseRows& rows, TcOp op, const uint32_t* alive, const float* q, int batch,
+                     int P, OrdMap ord_base, void* workspace, size_t workspace_bytes, uint64_t* part, const ScanStaging* sg,
+                     uint64_t* keys_out, cudaStream_t st);
 void launch_f32_to_bf16(const float* in, uint16_t* out, int64_t n_elems, cudaStream_t st);
 int64_t dense_tc_fallback_queries();   // queries re-run on K1 because the exactness certificate failed
-// diagnostics (tests only): one prune pass of K2 over every tile of the rows, in the production instantiation.
-// pass (KRAG_TC_PASS_*): 0 the TF32 pass (TC_TF32S on split rows, TC_TF32 on plain rows), 1 the bf16 pass on the high halves
-// of split rows, 2 the bf16 pass on the shadow Xh, 3 the bf16 pass on a host-rows index's device copy Xh.
+// diagnostics (tests only): one prune pass of K2 on operand op over every tile of the rows, in the production instantiation.
 // cap == 0: the DUMP instantiation writes a[j][r] = |x_r|^2 - 2 x_r.q_j for ALL rows and NQ_pad query columns to w.dump
 // [NQ_pad][S] (rows past n_rows: +inf); cap > 0: the main pass appends the alive rows with a < w.thr[j] to w.cand_rows
 // [NQ_pad][cap] and counts them in w.cand_count [NQ_pad].  w is carved by dense_tc_debug_carve (base == nullptr: size only).
 struct TcDebugWs { uint16_t* q_bf16; float* dump; float* thr; uint32_t* cand_count; uint32_t* cand_rows; };
 size_t dense_tc_debug_carve(TcDebugWs* w, unsigned char* base, int64_t n_rows, int dpad, int nq, int cap, int64_t* S_out,
                             int* nq_pad_out);
-bool dense_tc_debug_pass(const DeviceInfo& di, int pass, const float* X, const uint16_t* Xh, bool split, int64_t n_rows, int dpad,
-                         const float* xnorm, const uint32_t* alive, const float* q, int nq, const TcDebugWs& w, int cap,
-                         cudaStream_t st);
+bool dense_tc_debug_pass(const DeviceInfo& di, const DenseRows& rows, TcOp op, const uint32_t* alive, const float* q, int nq,
+                         const TcDebugWs& w, int cap, cudaStream_t st);
 
 // ---- merge / fuse (merge_fuse.cu)
 // per query: n_lists lists of list_len keys (element (l,i) at in[b*batch_stride + l*list_stride + i]) -> the P smallest
