@@ -382,6 +382,26 @@ int32_t krag_debug_rotary_cos_sin(float base, int32_t dh, int32_t pos, float* co
 int32_t krag_rerank(krag_embedder* e, int32_t n_queries, const int32_t* pair_offsets, const int32_t* tok_ids,
                     const int32_t* tok_offsets, const int32_t* seg_b, int32_t activation, int32_t top_k, int32_t* out_pos,
                     float* out_score);
+/* Late-interaction reranking (ColBERT: colbertv2.0, answerai-colbert-small).  krag_embedder_set_late_interaction, before
+ * krag_embedder_finalize: the projection linear.weight [dim, hidden] (no bias; dim a multiple of 16 in [16, 256]).
+ * KRAG_E_INVALID, naming linear.weight, when n_elems is not dim * hidden.  Every token row of the last layer then maps to
+ * v = W h / max(|W h|, 1e-12); the forward gives each sequence bits that depend on its own tokens alone (no split-K GEMM
+ * plan, the 64-key attention blocking at every length). */
+int32_t krag_embedder_set_late_interaction(krag_embedder* e, int32_t dim, const float* weight, int64_t n_elems);
+/* Query i is query_tok[i * query_len .. (i+1) * query_len) (query_len <= 32; ColBERT's [CLS] [Q] q... [SEP] [MASK]...) whose
+ * keys are its first query_keys[i] rows (1 .. query_len; every row is a query and an output row).  Passage p is
+ * passage_tok[passage_offsets[p] .. passage_offsets[p+1]); row t enters the max iff passage_keep[t] != 0 (at least one row
+ * of every passage must).  Query i owns pairs pair_offsets[i] .. pair_offsets[i+1] (0 to 300), pair j scores passage
+ * pair_passage[j]: score = sum over the query's rows r, in order, of the max over kept passage rows of the fp32 dot product
+ * of their unit vectors.  Each query and passage is encoded once per call, however many pairs name it.  out_pos /
+ * out_score [n_queries, top_k] as for krag_rerank.  All arguments are HOST memory; the call returns synchronised. */
+int32_t krag_late_rerank(krag_embedder* e, int32_t n_queries, int32_t query_len, const int32_t* query_tok, const int32_t* query_keys,
+                         int32_t n_passages, const int32_t* passage_tok, const int32_t* passage_offsets, const uint8_t* passage_keep,
+                         const int32_t* pair_offsets, const int32_t* pair_passage, int32_t top_k, int32_t* out_pos, float* out_score);
+/* The unit token vectors [tok_offsets[batch], dim] of packed sequences (key_lens [batch] or NULL: every row a key), as
+ * krag_late_rerank computes them.  Test hook. */
+int32_t krag_debug_late_vectors(krag_embedder* e, int32_t batch, const int32_t* tok_ids, const int32_t* tok_offsets, const int32_t* key_lens,
+                                float* out);
 int32_t krag_embedder_destroy(krag_embedder* e);
 
 /* ------------------------------------------------- host-side text analysis (no GPU involved; ASCII input) */

@@ -44,6 +44,7 @@ SYMBOLS = [
     "krag_embedder_set_position_offset", "krag_text_unigram_create", "krag_text_unigram_encode_batch",
     "krag_text_unigram_destroy", "krag_debug_tc_dump_pass", "krag_debug_tc_prune", "krag_debug_relative_bucket",
     "krag_wordpiece_create_specials", "krag_embedder_set_rotary", "krag_debug_rotary_cos_sin",
+    "krag_embedder_set_late_interaction", "krag_late_rerank", "krag_debug_late_vectors",
 ]
 # krag_debug_tc_dump_pass / krag_debug_tc_prune: the prune pass to run (KRAG_TC_PASS_*)
 TC_PASS_TF32, TC_PASS_BF16_SPLIT, TC_PASS_BF16_SHADOW, TC_PASS_BF16_HOST = 0, 1, 2, 3
@@ -152,6 +153,9 @@ def load() -> C.CDLL:
     L.krag_debug_relative_bucket.argtypes = [i32]
     L.krag_embedder_set_rotary.argtypes = [vp, C.c_float]
     L.krag_debug_rotary_cos_sin.argtypes = [C.c_float, i32, i32, vp, vp]
+    L.krag_embedder_set_late_interaction.argtypes = [vp, i32, vp, i64]
+    L.krag_late_rerank.argtypes = [vp, i32, i32, vp, vp, i32, vp, vp, vp, vp, vp, i32, vp, vp]
+    L.krag_debug_late_vectors.argtypes = [vp, i32, vp, vp, vp, vp]
     L.krag_wordpiece_encode_batch.argtypes = [vp, i64, C.c_char_p, vp, i32, vp, vp]
     L.krag_wordpiece_destroy.argtypes = [vp]
     L.krag_text_unigram_create.argtypes = [C.c_char_p, vp, vp, i64, i32, C.c_char_p, i64, i32, C.c_char_p, vp, vp, vp, i32,
@@ -390,6 +394,37 @@ class Embedder:
         check(self._L.krag_rerank(self._h, nq, ptr(pair_offsets), ptr(flat_tokens), ptr(tok_offsets), ptr(seg_b), activation, top_k,
                                   ptr(pos), ptr(sc)))
         return pos, sc
+
+    def set_late_interaction(self, weight):
+        """the ColBERT projection linear.weight [dim, hidden] (no bias) every token row maps through before its L2
+        normalisation (krag_embedder_set_late_interaction); before load_state_dict, which finalizes"""
+        w = np.ascontiguousarray(weight, np.float32)
+        self.li_dim = int(w.shape[0])
+        check(self._L.krag_embedder_set_late_interaction(self._h, self.li_dim, ptr(w), w.size))
+
+    def late_rerank(self, q_tokens, q_keys, p_tokens, p_offsets, p_keep, pair_offsets, pair_passage, top_k: int):
+        """krag_late_rerank: q_tokens int32 [n_queries, query_len], q_keys [n_queries]; packed passages with their uint8 keep
+        mask; pair_passage [n_pairs] indexes the passages.  (positions int32 [n_queries, top_k], scores float32 [n_queries,
+        top_k]); -1 / NaN past a query's pair count"""
+        q_tokens = np.ascontiguousarray(q_tokens, np.int32)
+        nq, ql = q_tokens.shape
+        q_keys = np.ascontiguousarray(q_keys, np.int32)
+        p_tokens = np.ascontiguousarray(p_tokens, np.int32); p_offsets = np.ascontiguousarray(p_offsets, np.int32)
+        p_keep = np.ascontiguousarray(p_keep, np.uint8)
+        pair_offsets = np.ascontiguousarray(pair_offsets, np.int32); pair_passage = np.ascontiguousarray(pair_passage, np.int32)
+        pos = np.empty((nq, top_k), np.int32)
+        sc = np.empty((nq, top_k), np.float32)
+        check(self._L.krag_late_rerank(self._h, nq, ql, ptr(q_tokens), ptr(q_keys), len(p_offsets) - 1, ptr(p_tokens), ptr(p_offsets),
+                                       ptr(p_keep), ptr(pair_offsets), ptr(pair_passage), top_k, ptr(pos), ptr(sc)))
+        return pos, sc
+
+    def debug_late_vectors(self, flat_tokens, offsets, key_lens=None) -> np.ndarray:
+        """the unit token vectors [tokens, dim] of packed sequences (krag_debug_late_vectors); key_lens None: every row a key"""
+        flat_tokens = np.ascontiguousarray(flat_tokens, np.int32); offsets = np.ascontiguousarray(offsets, np.int32)
+        kl = None if key_lens is None else np.ascontiguousarray(key_lens, np.int32)
+        out = np.empty((int(offsets[-1]), self.li_dim), np.float32)
+        check(self._L.krag_debug_late_vectors(self._h, len(offsets) - 1, ptr(flat_tokens), ptr(offsets), ptr(kl), ptr(out)))
+        return out
 
     def debug_cls_rows(self, on: bool):
         """test hook: False runs the last layer over every token under CLS pooling too (same embeddings)"""

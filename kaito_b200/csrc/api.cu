@@ -1705,6 +1705,36 @@ int32_t krag_rerank(krag_embedder* h, int32_t n_queries, const int32_t* pair_off
         embedder_rerank(h->e, n_queries, pair_offsets, tok_ids, tok_offsets, seg_b, activation, top_k, out_pos, out_score);
     });
 }
+int32_t krag_embedder_set_late_interaction(krag_embedder* h, int32_t dim, const float* weight, int64_t n_elems)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(h && weight, KRAG_E_INVALID, "null argument");
+        KRAG_CUDA(cudaSetDevice(h->ctx->di.device));
+        embedder_set_late_interaction(h->e, dim, weight, n_elems);
+    });
+}
+int32_t krag_late_rerank(krag_embedder* h, int32_t n_queries, int32_t query_len, const int32_t* query_tok, const int32_t* query_keys,
+                         int32_t n_passages, const int32_t* passage_tok, const int32_t* passage_offsets, const uint8_t* passage_keep,
+                         const int32_t* pair_offsets, const int32_t* pair_passage, int32_t top_k, int32_t* out_pos, float* out_score)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(h && query_tok && query_keys && pair_offsets && out_pos && out_score && n_queries >= 1, KRAG_E_INVALID, "bad argument");
+        KRAG_REQUIRE(pair_offsets[n_queries] == 0 || (passage_tok && passage_offsets && passage_keep && pair_passage), KRAG_E_INVALID,
+                     "bad argument");
+        KRAG_CUDA(cudaSetDevice(h->ctx->di.device));
+        embedder_late_rerank(h->e, n_queries, query_len, query_tok, query_keys, n_passages, passage_tok, passage_offsets, passage_keep,
+                             pair_offsets, pair_passage, top_k, out_pos, out_score);
+    });
+}
+int32_t krag_debug_late_vectors(krag_embedder* h, int32_t batch, const int32_t* tok_ids, const int32_t* tok_offsets, const int32_t* key_lens,
+                                float* out)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(h && tok_ids && tok_offsets && out && batch >= 1, KRAG_E_INVALID, "bad argument");
+        KRAG_CUDA(cudaSetDevice(h->ctx->di.device));
+        embedder_late_vectors(h->e, batch, tok_ids, tok_offsets, key_lens, out);
+    });
+}
 int32_t krag_embedder_destroy(krag_embedder* h)
 {
     return guarded([&] {

@@ -9,6 +9,8 @@
 //   tokens (packed, variable length: no padding rows)  ->  word+position+type embeddings -> LayerNorm
 //   L x [ QKV GEMM -> attention -> O GEMM (+bias +residual) -> LayerNorm -> FFN1 GEMM (+bias, erf-GELU)
 //         -> FFN2 GEMM (+bias +residual) -> LayerNorm ]  ->  CLS row or token mean (krag_embedder_set_pooling)  ->  L2 normalise
+// Late interaction (ColBERT, krag_late_rerank): every token row of the last layer -> hidden x dim projection -> L2 normalise,
+// then maxsim_kernel scores (query, passage) pairs from the token vectors.
 //
 // The four GEMMs per layer (24 S d^2 of the 24 S d^2 + 4 S^2 d flops) run on fp16 wgmma over split operands (see
 // gemm_f16s_kernel) with fp32 accumulation in registers, operands staged by TMA; bias / GELU / residual are fused into
@@ -18,6 +20,7 @@
 #include <math_constants.h>
 
 #include <cmath>
+#include <algorithm>
 #include <cstring>
 #include <map>
 #include <memory>
@@ -549,6 +552,10 @@ template <int N> __device__ __forceinline__ void am_wait() { asm volatile("cp.as
 // REL (MPNet): every score gets its head's learned bias at the key - query distance, clamped to [-REL_MAX, REL_MAX]:
 // rel_tab [heads][REL_TAB] holds it at index distance + REL_MAX (embedder_finalize builds it from the 32-bucket table).  The
 // head's row is staged after the K / V stages in shared memory.  REL = false ignores rel_tab and is the BERT kernel.
+//
+// KVL (ColBERT queries with attend_to_mask_tokens false): sequence b's keys are its first kv_len[b] rows (1 <= kv_len[b] <=
+// len); keys at or past it score -inf before the online softmax, key blocks past it are not visited, and every row of the
+// sequence stays a query row.  KVL = false ignores kv_len.
 constexpr int REL_MAX = 128, REL_TAB = 2 * REL_MAX + 1;
 template <int DH, int WARPS, int KB, int STAGES, int PLANES> struct AmCfg {
     static constexpr int LDH = DH + 8;                                   // row stride in halfs (16 bytes of padding)
@@ -556,10 +563,11 @@ template <int DH, int WARPS, int KB, int STAGES, int PLANES> struct AmCfg {
     static constexpr int KV_HALFS = PLANES * KB * LDH;                   // hi | lo of one operand of one stage
     static constexpr size_t SMEM = 2 * (size_t)(Q_HALFS + 2 * STAGES * KV_HALFS);
 };
-template <int DH, int WARPS, int KB, int STAGES, int PLANES, bool REL>
+template <int DH, int WARPS, int KB, int STAGES, int PLANES, bool REL, bool KVL>
 __global__ void __launch_bounds__(WARPS * 32)
 attention_mma_kernel(const uint16_t* __restrict__ qkv_hi, const uint16_t* __restrict__ qkv_lo, const int32_t* __restrict__ seq_off,
-                     uint16_t* __restrict__ out_hi, uint16_t* __restrict__ out_lo, int d, int heads, const float* __restrict__ rel_tab)
+                     uint16_t* __restrict__ out_hi, uint16_t* __restrict__ out_lo, int d, int heads, const float* __restrict__ rel_tab,
+                     const int32_t* __restrict__ kv_len)
 {
     using Cfg = AmCfg<DH, WARPS, KB, STAGES, PLANES>;
     constexpr int LDH = Cfg::LDH, QROWS = 16 * WARPS, THREADS = WARPS * 32, CH = DH / 8 /* 16-byte chunks per row */;
@@ -595,7 +603,8 @@ attention_mma_kernel(const uint16_t* __restrict__ qkv_hi, const uint16_t* __rest
     if constexpr (REL) {                                   // read after the first key block's __syncthreads
         for (int i = tid; i < REL_TAB; i += THREADS) sRel[i] = rel_tab[(size_t)h * REL_TAB + i];
     }
-    const int nkb = (len + KB - 1) / KB;
+    const int n_keys = KVL ? kv_len[b] : len;
+    const int nkb = (n_keys + KB - 1) / KB;
     uint32_t qh[DH / 16][4], ql[DH / 16][4];
     float om[DH / 8][4], oc[PLANES == 2 ? DH / 8 : 1][4];  // output accumulators: main and correction products
 #pragma unroll
@@ -654,7 +663,7 @@ attention_mma_kernel(const uint16_t* __restrict__ qkv_hi, const uint16_t* __rest
         for (int j = 0; j < KB / 8; ++j)
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-                const bool in = k0 + j * 8 + 2 * t + (e & 1) < len;
+                const bool in = k0 + j * 8 + 2 * t + (e & 1) < n_keys;
                 if constexpr (REL) {                       // transformers' order: scale, then + position bias, then the mask
                     const int c = dist0 + j * 8 + (e & 1) - 8 * (e >> 1);
                     const float bias = sRel[min(max(c, -REL_MAX), REL_MAX) + REL_MAX];
@@ -899,6 +908,79 @@ rerank_select_kernel(const float* __restrict__ scores, const int32_t* __restrict
     }
 }
 
+// ------------------------------------------------------------------------------------ late interaction (ColBERT)
+// MaxSim: score(q, P) = sum_{i < q_rows} max_{j in P, keep[j]} q_i . d_j over unit token vectors (rows of stride ld floats,
+// dim columns read).  One CTA per (query, slice of its pairs): query q's q_rows vectors are staged in shared memory once,
+// then each pair p of the slice (pair_pass[p] = its passage) streams the passage's rows 32 at a time.  Thread (i, jl) =
+// (tid / 8, tid % 8) owns query row i and passage rows jl + 8 u of a chunk (u < 4): every dot product is one fp32 fmaf chain
+// over k = 0 .. dim - 1 in order, the max over rows is exact (so the row order does not matter), and one thread adds the
+// q_rows maxima in row order.  A pair's score therefore depends on its two token matrices alone.  Rows are padded by 4 floats
+// in shared memory, so the 16-byte reads of 8 rows at one k hit 8 distinct bank groups.
+constexpr int MS_QROWS = 32, MS_CHUNK = 32, MS_THREADS = 256;
+__global__ void __launch_bounds__(MS_THREADS)
+maxsim_kernel(const float* __restrict__ qv, int q_rows, const float* __restrict__ pv, const int32_t* __restrict__ p_off,
+              const uint8_t* __restrict__ keep, const int32_t* __restrict__ pair_off, const int32_t* __restrict__ pair_pass, int dim,
+              int ld, float* __restrict__ scores)
+{
+    extern __shared__ __align__(16) float ms_sm[];
+    const int LDS = dim + 4;
+    float* sQ = ms_sm;                                  // [MS_QROWS][LDS]
+    float* sD = sQ + MS_QROWS * LDS;                    // [MS_CHUNK][LDS]
+    float* sMax = sD + MS_CHUNK * LDS;                  // [MS_QROWS]
+    int* sKeep = reinterpret_cast<int*>(sMax + MS_QROWS);   // [MS_CHUNK]
+    const int q = blockIdx.x, tid = threadIdx.x, i = tid >> 3, jl = tid & 7, c4 = dim / 4;
+    const int p_begin = pair_off[q], p_end = pair_off[q + 1];
+    if (p_begin + (int)blockIdx.y >= p_end) return;
+    for (int x = tid; x < q_rows * c4; x += MS_THREADS) {
+        const int r = x / c4, c = x % c4;
+        *reinterpret_cast<float4*>(sQ + r * LDS + 4 * c) = *reinterpret_cast<const float4*>(qv + ((size_t)q * q_rows + r) * ld + 4 * c);
+    }
+    for (int p = p_begin + (int)blockIdx.y; p < p_end; p += gridDim.y) {
+        const int pp = pair_pass[p], r0 = p_off[pp], r1 = p_off[pp + 1];
+        float m = -CUDART_INF_F;
+        for (int c0 = r0; c0 < r1; c0 += MS_CHUNK) {
+            const int n = r1 - c0 < MS_CHUNK ? r1 - c0 : MS_CHUNK;
+            __syncthreads();                            // the previous chunk (and the query rows) are staged / consumed
+            for (int x = tid; x < n * c4; x += MS_THREADS) {
+                const int r = x / c4, c = x % c4;
+                *reinterpret_cast<float4*>(sD + r * LDS + 4 * c) = *reinterpret_cast<const float4*>(pv + ((size_t)c0 + r) * ld + 4 * c);
+            }
+            if (tid < MS_CHUNK) sKeep[tid] = tid < n ? (int)keep[c0 + tid] : 0;
+            __syncthreads();
+            if (i < q_rows) {
+                float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+                const float* qr = sQ + i * LDS;
+                for (int k = 0; k < c4; ++k) {
+                    const float4 a = *reinterpret_cast<const float4*>(qr + 4 * k);
+                    const float4 b0 = *reinterpret_cast<const float4*>(sD + jl * LDS + 4 * k);
+                    const float4 b1 = *reinterpret_cast<const float4*>(sD + (jl + 8) * LDS + 4 * k);
+                    const float4 b2 = *reinterpret_cast<const float4*>(sD + (jl + 16) * LDS + 4 * k);
+                    const float4 b3 = *reinterpret_cast<const float4*>(sD + (jl + 24) * LDS + 4 * k);
+                    a0 = fmaf(a.x, b0.x, a0); a0 = fmaf(a.y, b0.y, a0); a0 = fmaf(a.z, b0.z, a0); a0 = fmaf(a.w, b0.w, a0);
+                    a1 = fmaf(a.x, b1.x, a1); a1 = fmaf(a.y, b1.y, a1); a1 = fmaf(a.z, b1.z, a1); a1 = fmaf(a.w, b1.w, a1);
+                    a2 = fmaf(a.x, b2.x, a2); a2 = fmaf(a.y, b2.y, a2); a2 = fmaf(a.z, b2.z, a2); a2 = fmaf(a.w, b2.w, a2);
+                    a3 = fmaf(a.x, b3.x, a3); a3 = fmaf(a.y, b3.y, a3); a3 = fmaf(a.z, b3.z, a3); a3 = fmaf(a.w, b3.w, a3);
+                }
+                if (sKeep[jl]) m = fmaxf(m, a0);
+                if (sKeep[jl + 8]) m = fmaxf(m, a1);
+                if (sKeep[jl + 16]) m = fmaxf(m, a2);
+                if (sKeep[jl + 24]) m = fmaxf(m, a3);
+            }
+        }
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));   // the 8 threads of a query row are adjacent lanes
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
+        if (jl == 0 && i < q_rows) sMax[i] = m;
+        __syncthreads();
+        if (tid == 0) {
+            float s = 0.f;
+            for (int r = 0; r < q_rows; ++r) s += sMax[r];
+            scores[p] = s;
+        }
+    }
+}
+static size_t maxsim_smem(int dim) { return sizeof(float) * ((size_t)(MS_QROWS + MS_CHUNK) * (dim + 4) + MS_QROWS) + sizeof(int) * MS_CHUNK; }
+
 // ------------------------------------------------------------------------------------ host
 // launch with programmatic stream serialization (see pdl_wait in tc_ptx.cuh); only for kernels that call pdl_wait()
 template <typename... KArgs, typename... Args>
@@ -915,39 +997,46 @@ static void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
     count_launch();
 }
 
-template <int DH, int WARPS, int KB, int STAGES, int PLANES, bool REL>
+template <int DH, int WARPS, int KB, int STAGES, int PLANES, bool REL, bool KVL>
 static void launch_attention_mma(const uint16_t* q_hi, const uint16_t* q_lo, const int32_t* seq_off, uint16_t* out_hi, uint16_t* out_lo, int d,
-                                 int heads, int batch, int max_len, bool first_rows, const float* rel_tab, cudaStream_t st)
+                                 int heads, int batch, int max_len, bool first_rows, const float* rel_tab, const int32_t* kv_len, cudaStream_t st)
 {
     using Cfg = AmCfg<DH, WARPS, KB, STAGES, PLANES>;
     constexpr size_t smem = Cfg::SMEM + (REL ? sizeof(float) * REL_TAB : 0);
     static bool attr_set = false;
     if (!attr_set) {
-        KRAG_CUDA(cudaFuncSetAttribute(attention_mma_kernel<DH, WARPS, KB, STAGES, PLANES, REL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        KRAG_CUDA(cudaFuncSetAttribute(attention_mma_kernel<DH, WARPS, KB, STAGES, PLANES, REL, KVL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set = true;
     }
     const unsigned q_blocks = first_rows ? 1u : (unsigned)((max_len + 16 * WARPS - 1) / (16 * WARPS));
-    launch_pdl(attention_mma_kernel<DH, WARPS, KB, STAGES, PLANES, REL>, dim3(q_blocks, (unsigned)heads, (unsigned)batch),
-               dim3(WARPS * 32), smem, st, q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, rel_tab);
+    launch_pdl(attention_mma_kernel<DH, WARPS, KB, STAGES, PLANES, REL, KVL>, dim3(q_blocks, (unsigned)heads, (unsigned)batch),
+               dim3(WARPS * 32), smem, st, q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, rel_tab, kv_len);
 }
-template <int DH, int PLANES, bool REL>
+template <int DH, int PLANES, bool REL, bool KVL>
 static void attention_mma_blocks(const uint16_t* q_hi, const uint16_t* q_lo, const int32_t* seq_off, uint16_t* out_hi, uint16_t* out_lo, int d,
-                                 int heads, int batch, int max_len, bool first_rows, const float* rel_tab, cudaStream_t st)
+                                 int heads, int batch, int max_len, bool first_rows, const float* rel_tab, const int32_t* kv_len, cudaStream_t st)
 {
-    if (max_len <= 32) launch_attention_mma<DH, 2, 32, 1, PLANES, REL>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, rel_tab, st);
-    else if (max_len <= 64) launch_attention_mma<DH, 4, 64, 1, PLANES, REL>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, rel_tab, st);
-    else launch_attention_mma<DH, 4, 64, 2, PLANES, REL>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, rel_tab, st);
+    if constexpr (KVL) {                   // the late-interaction forward's blocking (encoder_forward: max_len > 64)
+        launch_attention_mma<DH, 4, 64, 2, PLANES, REL, KVL>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, rel_tab, kv_len, st);
+    } else if (max_len <= 32)
+        launch_attention_mma<DH, 2, 32, 1, PLANES, REL, KVL>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, rel_tab, kv_len, st);
+    else if (max_len <= 64)
+        launch_attention_mma<DH, 4, 64, 1, PLANES, REL, KVL>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, rel_tab, kv_len, st);
+    else launch_attention_mma<DH, 4, 64, 2, PLANES, REL, KVL>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, rel_tab, kv_len, st);
 }
 // queries (<= 32 tokens): 2 warps, one key block; <= 64: 4 warps, one block; chunks: 4 warps, 64-key blocks, double-buffered.
 // first_rows: only the first block of query rows of every sequence (the [CLS] row among them); a query row's result does
 // not depend on which other rows run, and the key blocking follows max_len either way.  PLANES == 1: q_lo / out_lo are not used.
-// rel_tab: the MPNet relative-position bias table (REL instantiations), null for BERT.
+// rel_tab: the MPNet relative-position bias table (REL instantiations), null for BERT.  kv_len: per-sequence key counts
+// (device, KVL instantiations; BERT only), null: every row is a key.
 template <int DH, int PLANES>
 static void attention_mma(const uint16_t* q_hi, const uint16_t* q_lo, const int32_t* seq_off, uint16_t* out_hi, uint16_t* out_lo, int d, int heads,
-                          int batch, int max_len, bool first_rows, const float* rel_tab, cudaStream_t st)
+                          int batch, int max_len, bool first_rows, const float* rel_tab, const int32_t* kv_len, cudaStream_t st)
 {
-    if (rel_tab) attention_mma_blocks<DH, PLANES, true>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, rel_tab, st);
-    else attention_mma_blocks<DH, PLANES, false>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, nullptr, st);
+    if (rel_tab && kv_len) throw std::runtime_error("embedder: key lengths are not combined with the relative-position bias");
+    if (rel_tab) attention_mma_blocks<DH, PLANES, true, false>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, rel_tab, nullptr, st);
+    else if (kv_len) attention_mma_blocks<DH, PLANES, false, true>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, nullptr, kv_len, st);
+    else attention_mma_blocks<DH, PLANES, false, false>(q_hi, q_lo, seq_off, out_hi, out_lo, d, heads, batch, max_len, first_rows, nullptr, nullptr, st);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -1141,12 +1230,20 @@ struct Embedder {
     bool gated = false;
     std::vector<DevArray<float>> bf1;
     bool has_head = false;
+    // late interaction (ColBERT): li_dim > 0 (krag_embedder_set_late_interaction); finalize splits linear.weight [li_dim][hidden]
+    // zero-padded to li_pad = the next multiple of 128 rows (the padded outputs are exact zeros), li_bias is li_pad zeros
+    int li_dim = 0, li_pad = 0;
+    SplitMat s_li{nullptr, nullptr};
+    DevArray<float> li_bias;
+    DevArray<float> li_c, li_q, li_p;     // projection scratch [cap_tok][li_pad]; query / passage unit vectors, rows of li_pad
+    DevArray<int32_t> d_kvl, li_off, li_pp;
+    DevArray<uint8_t> li_keep;
     bool finalized = false;
     cudaStream_t st = nullptr;
     cudaEvent_t done = nullptr, in_ev = nullptr;
-    // captured forward per (n_tok, batch, max_len, cls_rows, head, precision): head = 1 for cross-encoder pairs (token types
-    // uploaded); the two precisions run different kernels
-    using GraphKey = std::tuple<int, int, int, int, int, int>;
+    // captured forward per (n_tok, batch, max_len, cls_rows, head, precision, late): head = 1 for cross-encoder pairs (token
+    // types uploaded); the two precisions run different kernels; late = 1 for a late-interaction forward, 2 with key lengths
+    using GraphKey = std::tuple<int, int, int, int, int, int, int>;
     std::map<GraphKey, cudaGraphExec_t> graphs;
     std::map<GraphKey, int> seen;
     int precision = EMB_PREC_FP32;        // EMB_PREC_FP16: single-plane products (the hi planes of weights and activations)
@@ -1238,6 +1335,7 @@ int relative_bucket(int rel)
     return base + (v < 15 ? v : 15);
 }
 static const char* const REL_BIAS = "encoder.relative_attention_bias.weight";   // MPNet: [32 buckets][heads]
+static const char* const LI_WEIGHT = "linear.weight";                           // ColBERT: [dim][hidden], no bias
 constexpr int REL_BUCKETS = 32;
 
 // transformers' default RoPE (NomicBertRotaryEmbedding): inv_freq[i] = 1 / base^(2i / dh) and the angle fp32(pos) *
@@ -1252,6 +1350,17 @@ void rotary_cos_sin(float base, int dh, int pos, float* cos_out, float* sin_out)
         cos_out[i] = (float)std::cos((double)theta);
         sin_out[i] = (float)std::sin((double)theta);
     }
+}
+
+void embedder_set_late_interaction(Embedder* e, int dim, const float* weight, int64_t n)
+{
+    if (dim < 16 || dim > 256 || dim % 16)
+        throw std::runtime_error("embedder: the late-interaction dim must be a multiple of 16 in [16, 256]");
+    if (n != (int64_t)dim * e->cfg.hidden)
+        throw std::runtime_error(std::string("embedder: ") + LI_WEIGHT + " must hold dim x hidden = " + std::to_string((int64_t)dim * e->cfg.hidden) +
+                                 " elements, not " + std::to_string(n));
+    embedder_load(e, LI_WEIGHT, weight, n);
+    e->li_dim = dim;
 }
 
 void embedder_set_rotary(Embedder* e, float base)
@@ -1292,6 +1401,7 @@ void embedder_finalize(Embedder* e)
     e->bqkv.clear(); e->planes.clear(); e->s_qkv.clear(); e->s_o.clear(); e->s_f1.clear(); e->s_f2.clear();
     e->s_pool = SplitMat{nullptr, nullptr}; e->has_head = false;
     e->rel_tab.release(); e->rope.release(); e->bf1.clear(); e->gated = false;
+    e->s_li = SplitMat{nullptr, nullptr}; e->li_pad = 0; e->li_bias.release();
     e->drop_graphs(); e->seen.clear();   // captured weight pointers are about to change
     const BertConfig& c = e->cfg;
     const int dh = d / c.heads;
@@ -1299,6 +1409,7 @@ void embedder_finalize(Embedder* e)
     const auto rit = e->t.find(REL_BIAS);
     const bool rel = rit != e->t.end() && rit->second.p;   // an MPNet encoder: loaded with the relative-position bias
     if (rel) emb_get(e, REL_BIAS, (int64_t)REL_BUCKETS * c.heads);
+    if (e->li_dim) emb_get(e, LI_WEIGHT, (int64_t)e->li_dim * d);
     const bool rotary = e->rope_base > 0.f;
     // a gated FFN: every layer loaded with intermediate.gate.weight [inter][hidden] (and its bias), or none
     const bool gated = emb_has(e, lname(0, "intermediate.gate.weight"));
@@ -1385,6 +1496,19 @@ void embedder_finalize(Embedder* e)
         e->s_pool = emb_split_weight(e, emb_get(e, "pooler.dense.weight", (int64_t)d * d), (size_t)d * d);
         e->has_head = true;
     }
+    if (e->li_dim) {
+        const int pad = (e->li_dim + GM_TILE - 1) / GM_TILE * GM_TILE;
+        DevArray<float> w;
+        w.alloc((int64_t)pad * d);
+        KRAG_CUDA(cudaMemsetAsync(w.p, 0, sizeof(float) * (size_t)pad * d, e->st));
+        KRAG_CUDA(cudaMemcpyAsync(w.p, emb_get(e, LI_WEIGHT, (int64_t)e->li_dim * d), sizeof(float) * (size_t)e->li_dim * d,
+                                  cudaMemcpyDeviceToDevice, e->st));
+        e->s_li = emb_split_weight(e, w.p, (size_t)pad * d);
+        e->li_bias.alloc(pad);
+        KRAG_CUDA(cudaMemsetAsync(e->li_bias.p, 0, sizeof(float) * (size_t)pad, e->st));
+        KRAG_CUDA(cudaStreamSynchronize(e->st));   // w is freed at scope end
+        e->li_pad = pad;
+    }
     if (rel) {
         // the bias by distance, [heads][REL_TAB]: the kernel looks a score's bias up without computing its bucket
         std::vector<float> w((size_t)REL_BUCKETS * c.heads), tab((size_t)c.heads * REL_TAB);
@@ -1466,7 +1590,13 @@ static void launch_pool(const Embedder* e, int batch, bool cls_rows, float* out,
 // seg_b (host, [batch] or null): index of the first token of segment B of each sequence; tokens from there on add token
 // type row 1, the others row 0 (null: row 0 everywhere, the single-sequence embedding).  cls_ok: only the [CLS] rows of the
 // last layer are read.  Returns whether the last layer ran on the [CLS] rows only (then in cx / cxs, else x / xs).
-static bool encoder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int32_t* tok_offsets, const int32_t* seg_b, bool cls_ok)
+// late (late-interaction token vectors): every row of the last layer is read, and each sequence's rows get bits that depend
+// on its own tokens alone -- every GEMM runs the one plan LATE_PLAN (linear_plan picks the tile width and K split from the
+// token count) and attention the 64-key blocking whatever the batch's longest sequence.  kv_len (host, [batch] or null; late only): the
+// keys of sequence b are its first kv_len[b] rows.
+constexpr GemmPlan LATE_PLAN{128, 1, false};   // 128 x 128 tiles, the whole K range: valid for every N % 128 == 0 (hidden, 3 hidden, FFN)
+static bool encoder_forward(Embedder* e, int batch, const int32_t* tok_ids, const int32_t* tok_offsets, const int32_t* seg_b, bool cls_ok,
+                            bool late = false, const int32_t* kv_len = nullptr)
 {
     if (!e->finalized) throw std::runtime_error("embedder: call finalize after loading the weights");
     const BertConfig& c = e->cfg;
@@ -1482,6 +1612,7 @@ static bool encoder_forward(Embedder* e, int batch, const int32_t* tok_ids, cons
         if (len < 1 || len > c.max_pos - off)
             throw std::runtime_error("embedder: sequence length must be in [1, max_position - position offset]");
         max_len = len > max_len ? len : max_len;
+        if (kv_len && (kv_len[b] < 1 || kv_len[b] > len)) throw std::runtime_error("embedder: a key length must be in [1, sequence length]");
         for (int i = 0; i < len; ++i) pos[(size_t)tok_offsets[b] + i] = off + i;
         if (seg_b) {
             if (seg_b[b] < 1 || seg_b[b] > len) throw std::runtime_error("embedder: segment B must start in [1, sequence length]");
@@ -1495,10 +1626,10 @@ static bool encoder_forward(Embedder* e, int batch, const int32_t* tok_ids, cons
         // all old buffers go before the first new one is allocated (the peak is the new set only); a grow that fails
         // half-way leaves no workspace and capacity 0, so the next call grows again
         e->cap_tok = e->cap_batch = 0;
-        e->d_tok.release(); e->d_pos.release(); e->d_off.release(); e->d_typ.release(); e->x.release(); e->x2.release(); e->qkv.release();
+        e->d_tok.release(); e->d_pos.release(); e->d_off.release(); e->d_typ.release(); e->d_kvl.release(); e->x.release(); e->x2.release(); e->qkv.release();
         e->xs.release(); e->cs.release(); e->fs.release(); e->out.release();
         e->cx.release(); e->cx2.release(); e->ccs.release(); e->cxs.release(); e->cfs.release();
-        e->d_tok.alloc(T); e->d_pos.alloc(T); e->d_off.alloc(Bc + 1); e->d_typ.alloc(T);
+        e->d_tok.alloc(T); e->d_pos.alloc(T); e->d_off.alloc(Bc + 1); e->d_typ.alloc(T); e->d_kvl.alloc(Bc);
         e->x.alloc(T * d); e->x2.alloc(T * d); e->qkv.alloc(2 * T * 3 * d);
         e->xs.alloc(2 * T * d); e->cs.alloc(2 * T * d); e->fs.alloc(2 * T * c.inter);
         e->out.alloc(Bc * d);
@@ -1515,12 +1646,16 @@ static bool encoder_forward(Embedder* e, int batch, const int32_t* tok_ids, cons
     KRAG_CUDA(cudaMemcpyAsync(e->d_pos.p, pos.data(), 4 * (size_t)n_tok, cudaMemcpyHostToDevice, st));
     KRAG_CUDA(cudaMemcpyAsync(e->d_off.p, tok_offsets, 4 * (size_t)(batch + 1), cudaMemcpyHostToDevice, st));
     if (seg_b) KRAG_CUDA(cudaMemcpyAsync(e->d_typ.p, typ.data(), 4 * (size_t)n_tok, cudaMemcpyHostToDevice, st));
+    if (kv_len) KRAG_CUDA(cudaMemcpyAsync(e->d_kvl.p, kv_len, 4 * (size_t)batch, cudaMemcpyHostToDevice, st));
+    const GemmPlan* const plan = late ? &LATE_PLAN : nullptr;
+    const int att_len = late && max_len <= 64 ? 65 : max_len;   // the attention blocking of sequences over 64 tokens
+    const int32_t* const d_kvl = kv_len ? e->d_kvl.p : nullptr;
 
     // CLS pooling reads one row per sequence of the last layer's output.  K and V of every token are still needed, so the
     // last QKV projection runs over all tokens; attention then runs for the first query rows only, and the O projection,
     // FFN and LayerNorms run on the gathered [CLS] rows.  Those GEMMs keep the plan (tile width, K split) of the full
     // token count, so every [CLS] row gets the same bits as in the full layer.  Taken when it saves a 128-row tile.
-    const bool cls_rows = cls_ok && e->cls_rows_only && (n_tok + GM_TILE - 1) / GM_TILE > (batch + GM_TILE - 1) / GM_TILE;
+    const bool cls_rows = !late && cls_ok && e->cls_rows_only && (n_tok + GM_TILE - 1) / GM_TILE > (batch + GM_TILE - 1) / GM_TILE;
     // The forward is ~7 kernels per layer; for a handful of query tokens it is bound by launch gaps and kernel
     // prologues, so each (n_tok, batch, max_len, cls_rows, head) shape is captured into a CUDA graph the second time it is seen.
     const int dh = d / c.heads;
@@ -1548,13 +1683,13 @@ static bool encoder_forward(Embedder* e, int batch, const int32_t* tok_ids, cons
         const size_t L = (size_t)l;
         const bool last_cls = cls_rows && l == c.layers - 1;
         launch_linear(e->di, xs, e->s_qkv[L], n_tok, 3 * d, d, e->bqkv[L].p, nullptr, false, nullptr, q_hi, q_lo, nullptr, nullptr, 0.f,
-                      nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st, nullptr, planes, &ep_qkv);
+                      nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st, plan, planes, &ep_qkv);
         const float* rel = e->rel_tab.p;                  // null: BERT
         if (planes == 1) {
-            if (dh == 64) attention_mma<64, 1>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, rel, st);
-            else attention_mma<32, 1>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, rel, st);
-        } else if (dh == 64) attention_mma<64, 2>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, rel, st);
-        else attention_mma<32, 2>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, max_len, last_cls, rel, st);
+            if (dh == 64) attention_mma<64, 1>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, att_len, last_cls, rel, d_kvl, st);
+            else attention_mma<32, 1>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, att_len, last_cls, rel, d_kvl, st);
+        } else if (dh == 64) attention_mma<64, 2>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, att_len, last_cls, rel, d_kvl, st);
+        else attention_mma<32, 2>(q_hi, q_lo, e->d_off.p, cs.hi, cs.lo, d, c.heads, batch, att_len, last_cls, rel, d_kvl, st);
         if (last_cls) {
             const SplitMat ccs{e->ccs.p, lo_of(e->ccs.p, (size_t)batch * d)}, cxs{e->cxs.p, lo_of(e->cxs.p, (size_t)batch * d)},
                            cfs{e->cfs.p, lo_of(e->cfs.p, (size_t)batch * c.inter)};
@@ -1576,17 +1711,17 @@ static bool encoder_forward(Embedder* e, int batch, const int32_t* tok_ids, cons
         // O projection (+bias +residual) -> LayerNorm -> x (fp32 residual stream) + its split planes
         launch_linear(e->di, cs, e->s_o[L], n_tok, d, d, e->t[lname(l, "attention.output.dense.bias")].p, e->x.p, false, e->x2.p, nullptr, nullptr,
                       e->t[lname(l, "attention.output.LayerNorm.weight")].p, e->t[lname(l, "attention.output.LayerNorm.bias")].p, c.eps, e->x.p, xs.hi, xs.lo,
-                      e->ws.p, Embedder::WS_FLOATS, st, nullptr, planes);
+                      e->ws.p, Embedder::WS_FLOATS, st, plan, planes);
         // FFN1 (+bias, GELU; gated: silu(gate) * up): only the split planes are written (FFN2 is the sole consumer)
         launch_linear(e->di, xs, e->s_f1[L], n_tok, n_f1, d, f1_bias(l), nullptr, !e->gated, nullptr, fs.hi, fs.lo,
-                      nullptr, nullptr, 0.f, nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st, nullptr, planes, &ep_f1);
+                      nullptr, nullptr, 0.f, nullptr, nullptr, nullptr, e->ws.p, Embedder::WS_FLOATS, st, plan, planes, &ep_f1);
         // FFN2 (+bias +residual) -> LayerNorm -> x + split planes
         launch_linear(e->di, fs, e->s_f2[L], n_tok, d, c.inter, e->t[lname(l, "output.dense.bias")].p, e->x.p, false, e->x2.p, nullptr, nullptr,
                       e->t[lname(l, "output.LayerNorm.weight")].p, e->t[lname(l, "output.LayerNorm.bias")].p, c.eps, e->x.p, xs.hi, xs.lo, e->ws.p,
-                      Embedder::WS_FLOATS, st, nullptr, planes);
+                      Embedder::WS_FLOATS, st, plan, planes);
     }
     };   // run_layers
-    const Embedder::GraphKey key(n_tok, batch, max_len, cls_rows ? 1 : 0, seg_b ? 1 : 0, e->precision);
+    const Embedder::GraphKey key(n_tok, batch, max_len, cls_rows ? 1 : 0, seg_b ? 1 : 0, e->precision, late ? (kv_len ? 2 : 1) : 0);
     auto git = e->graphs.find(key);
     if (git != e->graphs.end()) {
         KRAG_CUDA(cudaGraphLaunch(git->second, st));
@@ -1693,6 +1828,130 @@ void embedder_rerank(Embedder* e, int n_queries, const int32_t* pair_off, const 
     const size_t nk = (size_t)n_queries * top_k;
     rerank_select_kernel<<<(unsigned)n_queries, 256, 0, st>>>(e->scores.p, e->d_poff.p, top_k, e->sel.p,
                                                              reinterpret_cast<float*>(e->sel.p + nk));
+    KRAG_CUDA(cudaGetLastError());
+    count_launch();
+    std::vector<int32_t> h(2 * nk);
+    KRAG_CUDA(cudaMemcpyAsync(h.data(), e->sel.p, 4 * 2 * nk, cudaMemcpyDeviceToHost, st));
+    KRAG_CUDA(cudaStreamSynchronize(st));
+    std::memcpy(out_pos, h.data(), 4 * nk);
+    std::memcpy(out_score, h.data() + nk, 4 * nk);
+}
+
+
+// ---- late interaction (ColBERT)
+// Unit token vectors of packed sequences: the late-interaction forward (every row of the last layer, bits per sequence),
+// the projection W . h through the split-fp16 GEMM with zero bias into [n_tok][li_pad] (columns past li_dim are exact zeros),
+// then cls_normalize_kernel over every row (one warp per row, fixed fp32 order; the zero columns add nothing to the norm),
+// written to rows of `out` (device, stride li_pad).  Sequences go through forwards of at most RERANK_MAX_TOKENS tokens.
+static void late_vectors(Embedder* e, int batch, const int32_t* tok_ids, const int32_t* tok_off, const int32_t* kv_len, float* out)
+{
+    const int d = e->cfg.hidden, pad = e->li_pad;
+    const int planes = e->precision == EMB_PREC_FP16 ? 1 : 2;
+    std::vector<int32_t> offs;
+    for (int b0 = 0; b0 < batch;) {
+        int b1 = b0 + 1;
+        while (b1 < batch && tok_off[b1 + 1] - tok_off[b0] <= RERANK_MAX_TOKENS) ++b1;
+        const int nb = b1 - b0, n_tok = tok_off[b1] - tok_off[b0];
+        offs.assign((size_t)nb + 1, 0);
+        for (int j = 0; j <= nb; ++j) offs[(size_t)j] = tok_off[b0 + j] - tok_off[b0];
+        encoder_forward(e, nb, tok_ids + tok_off[b0], offs.data(), nullptr, false, true, kv_len ? kv_len + b0 : nullptr);
+        if (e->li_c.cap < (int64_t)e->cap_tok * pad) e->li_c.alloc((int64_t)e->cap_tok * pad);
+        const SplitMat xs{e->xs.p, planes == 2 ? e->xs.p + (size_t)e->cap_tok * d : nullptr};
+        launch_linear(e->di, xs, e->s_li, n_tok, pad, d, e->li_bias.p, nullptr, false, e->li_c.p, nullptr, nullptr, nullptr, nullptr, 0.f,
+                      nullptr, nullptr, nullptr, nullptr, 0, e->st, &LATE_PLAN, planes);
+        cls_normalize_kernel<<<(unsigned)((n_tok * 32 + 255) / 256), 256, 0, e->st>>>(e->li_c.p, nullptr, out + (size_t)tok_off[b0] * pad,
+                                                                                     n_tok, pad, pad);
+        KRAG_CUDA(cudaGetLastError());
+        count_launch();
+        b0 = b1;
+    }
+}
+
+static void late_check(const Embedder* e, int batch, const int32_t* tok_off)
+{
+    if (!e->finalized) throw std::runtime_error("embedder: call finalize after loading the weights");
+    if (!e->li_pad) throw std::runtime_error("embedder: late interaction needs krag_embedder_set_late_interaction before finalize");
+    if (batch < 1 || tok_off[0] != 0) throw std::runtime_error("embedder: token offsets must start at 0");
+    for (int b = 0; b < batch; ++b) {
+        const int len = tok_off[b + 1] - tok_off[b];
+        if (len < 1 || len > e->cfg.max_pos - e->pos_off)
+            throw std::runtime_error("embedder: sequence length must be in [1, max_position - position offset]");
+    }
+}
+
+void embedder_late_vectors(Embedder* e, int batch, const int32_t* tok_ids, const int32_t* tok_off, const int32_t* kv_len, float* out_host)
+{
+    late_check(e, batch, tok_off);
+    const int64_t n_tok = tok_off[batch];
+    if (e->li_q.cap < n_tok * e->li_pad) e->li_q.alloc(n_tok * e->li_pad);
+    late_vectors(e, batch, tok_ids, tok_off, kv_len, e->li_q.p);
+    KRAG_CUDA(cudaMemcpy2DAsync(out_host, sizeof(float) * (size_t)e->li_dim, e->li_q.p, sizeof(float) * (size_t)e->li_pad,
+                                sizeof(float) * (size_t)e->li_dim, (size_t)n_tok, cudaMemcpyDeviceToHost, e->st));
+    KRAG_CUDA(cudaStreamSynchronize(e->st));
+}
+
+// Late-interaction reranking.  n_queries queries of q_rows tokens each (q_tok [n_queries * q_rows], keys q_kv[i] <= q_rows),
+// n_pass distinct passages (p_tok packed by p_off [n_pass + 1], p_keep[t] = 1 where row t enters the max), query i owns pairs
+// pair_off[i] .. pair_off[i + 1], pair p scores passage pair_pass[p].  Each query and each passage is encoded once; maxsim_kernel
+// writes every pair's score at its offset, rerank_select_kernel orders each query's scores as for krag_rerank.
+void embedder_late_rerank(Embedder* e, int n_queries, int q_rows, const int32_t* q_tok, const int32_t* q_kv, int n_pass, const int32_t* p_tok,
+                          const int32_t* p_off, const uint8_t* p_keep, const int32_t* pair_off, const int32_t* pair_pass, int top_k,
+                          int32_t* out_pos, float* out_score)
+{
+    if (q_rows < 1 || q_rows > MS_QROWS) throw std::runtime_error("embedder: a late-interaction query holds 1 to 32 tokens");
+    if (top_k < 1 || top_k > RERANK_MAX_CANDIDATES) throw std::runtime_error("embedder: top_k must be in [1, 300]");
+    if (n_queries < 1 || pair_off[0] != 0) throw std::runtime_error("embedder: pair offsets must start at 0");
+    for (int q = 0; q < n_queries; ++q) {
+        const int n = pair_off[q + 1] - pair_off[q];
+        if (n < 0 || n > RERANK_MAX_CANDIDATES) throw std::runtime_error("embedder: a query has 0 to 300 candidate pairs");
+    }
+    const int n_pairs = pair_off[n_queries];
+    std::vector<int32_t> q_off((size_t)n_queries + 1);
+    for (int q = 0; q <= n_queries; ++q) q_off[(size_t)q] = q * q_rows;
+    late_check(e, n_queries, q_off.data());
+    if (n_pairs > 0) {
+        if (n_pass < 1) throw std::runtime_error("embedder: pairs need passages");
+        late_check(e, n_pass, p_off);
+        for (int p = 0; p < n_pass; ++p) {
+            int kept = 0;
+            for (int t = p_off[p]; t < p_off[p + 1]; ++t) kept += p_keep[t] != 0;
+            if (!kept) throw std::runtime_error("embedder: every passage needs at least one row that enters the max");
+        }
+        for (int p = 0; p < n_pairs; ++p)
+            if (pair_pass[p] < 0 || pair_pass[p] >= n_pass) throw std::runtime_error("embedder: a pair's passage index is out of range");
+    }
+    cudaStream_t st = e->st;
+    const int64_t pad = e->li_pad, nq_tok = (int64_t)n_queries * q_rows, np_tok = n_pairs > 0 ? p_off[n_pass] : 0;
+    if (e->li_q.cap < nq_tok * pad) e->li_q.alloc(nq_tok * pad);
+    if (np_tok > 0 && e->li_p.cap < np_tok * pad) e->li_p.alloc(np_tok * pad);
+    if (e->scores.cap < (n_pairs > 0 ? n_pairs : 1)) e->scores.alloc(n_pairs > 0 ? n_pairs : 1);
+    if (e->d_poff.cap < n_queries + 1) e->d_poff.alloc(n_queries + 1);
+    if (e->sel.cap < 2 * (int64_t)n_queries * top_k) e->sel.alloc(2 * (int64_t)n_queries * top_k);
+    late_vectors(e, n_queries, q_tok, q_off.data(), q_kv, e->li_q.p);
+    KRAG_CUDA(cudaMemcpyAsync(e->d_poff.p, pair_off, 4 * (size_t)(n_queries + 1), cudaMemcpyHostToDevice, st));
+    if (n_pairs > 0) {
+        late_vectors(e, n_pass, p_tok, p_off, nullptr, e->li_p.p);
+        if (e->li_off.cap < n_pass + 1) e->li_off.alloc(n_pass + 1);
+        if (e->li_pp.cap < n_pairs) e->li_pp.alloc(n_pairs);
+        if (e->li_keep.cap < np_tok) e->li_keep.alloc(np_tok);
+        KRAG_CUDA(cudaMemcpyAsync(e->li_off.p, p_off, 4 * (size_t)(n_pass + 1), cudaMemcpyHostToDevice, st));
+        KRAG_CUDA(cudaMemcpyAsync(e->li_pp.p, pair_pass, 4 * (size_t)n_pairs, cudaMemcpyHostToDevice, st));
+        KRAG_CUDA(cudaMemcpyAsync(e->li_keep.p, p_keep, (size_t)np_tok, cudaMemcpyHostToDevice, st));
+        int max_pairs = 0;
+        for (int q = 0; q < n_queries; ++q) max_pairs = std::max(max_pairs, pair_off[q + 1] - pair_off[q]);
+        // slices per query: about two CTAs per SM over the call, one pair per CTA at most
+        const int want = (2 * e->di.sm_count + n_queries - 1) / n_queries;
+        const int slices = std::max(1, std::min(max_pairs, want));
+        const size_t smem = maxsim_smem(e->li_dim);
+        static bool attr = false;
+        if (!attr) { KRAG_CUDA(cudaFuncSetAttribute(maxsim_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)maxsim_smem(256))); attr = true; }
+        maxsim_kernel<<<dim3((unsigned)n_queries, (unsigned)slices), MS_THREADS, smem, st>>>(e->li_q.p, q_rows, e->li_p.p, e->li_off.p, e->li_keep.p,
+                                                                                         e->d_poff.p, e->li_pp.p, e->li_dim, (int)pad, e->scores.p);
+        KRAG_CUDA(cudaGetLastError());
+        count_launch();
+    }
+    const size_t nk = (size_t)n_queries * top_k;
+    rerank_select_kernel<<<(unsigned)n_queries, 256, 0, st>>>(e->scores.p, e->d_poff.p, top_k, e->sel.p, reinterpret_cast<float*>(e->sel.p + nk));
     KRAG_CUDA(cudaGetLastError());
     count_launch();
     std::vector<int32_t> h(2 * nk);

@@ -537,6 +537,13 @@ constexpr int RERANK_MAX_CANDIDATES = 300;           // pairs per query (= KRAG_
 constexpr int RERANK_MAX_TOKENS = 65536;             // tokens per forward of a rerank call
 void embedder_rerank(Embedder* e, int n_queries, const int32_t* pair_off, const int32_t* tok_ids, const int32_t* tok_off,
                      const int32_t* seg_b, int act, int top_k, int32_t* out_pos, float* out_score);
+// late interaction (ColBERT): the hidden -> dim projection (linear.weight [dim][hidden], no bias; before finalize), the unit
+// token vectors of packed sequences (kv_len: keys per sequence, or null), and MaxSim reranking (see embed.cu)
+void embedder_set_late_interaction(Embedder* e, int dim, const float* weight, int64_t n);
+void embedder_late_vectors(Embedder* e, int batch, const int32_t* tok_ids, const int32_t* tok_off, const int32_t* kv_len, float* out_host);
+void embedder_late_rerank(Embedder* e, int n_queries, int q_rows, const int32_t* q_tok, const int32_t* q_kv, int n_pass, const int32_t* p_tok,
+                          const int32_t* p_off, const uint8_t* p_keep, const int32_t* pair_off, const int32_t* pair_pass, int top_k,
+                          int32_t* out_pos, float* out_score);
 // A fp32 matrix carried as two fp16 planes: v = hi + lo * 2^-11 (see embed.cu: split operands of the K5 GEMMs)
 struct SplitMat { uint16_t* hi; uint16_t* lo; };
 void launch_split_f16(const float* in, uint16_t* hi, uint16_t* lo, int64_t n /* % 8 == 0 */, cudaStream_t st);

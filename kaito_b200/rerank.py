@@ -269,3 +269,226 @@ class GpuCrossEncoder:
         flat, toff, seg, poff = build_pairs(self.tokenizer.cls, self.tokenizer.sep, qs, docs, self.max_length, self.specials - 2)
         with self._mu:
             return self._emb.rerank(poff, flat, toff, seg, top_k, self._act)
+
+
+# ------------------------------------------------------------------ late interaction (ColBERT)
+# Stanford ColBERT (colbert.modeling) restated: a query is [CLS] [Q] q... [SEP] cut to query_maxlen and padded with [MASK] to
+# exactly query_maxlen (ColBERT tokenises ". " + text and overwrites the "." at position 1 with the marker); a passage is
+# [CLS] [D] d... [SEP] cut to doc_maxlen.  Every token row becomes normalize(W h); score = sum over query rows of the max over
+# passage rows (skiplist rows excluded) of their dot product.  K5 computes all of it (krag_late_rerank).
+COLBERT_QUERY_ROWS = 32          # the longest query_maxlen maxsim_kernel stages
+
+
+def is_colbert_snapshot(model_dir: str) -> bool:
+    """a Stanford ColBERT checkpoint (artifact.metadata, or config.json architectures HF_ColBERT) or a PyLate one (modules.json
+    with a Dense module after the Transformer)"""
+    join = os.path.join
+    if os.path.isfile(join(model_dir, "artifact.metadata")):
+        return True
+    cfg = _json(join(model_dir, "config.json"), required=False) or {}
+    if "HF_ColBERT" in (cfg.get("architectures") or []):
+        return True
+    mods = _json(join(model_dir, "modules.json"), required=False)
+    return isinstance(mods, list) and any(isinstance(m, dict) and str(m.get("type", "")).endswith("Dense") for m in mods)
+
+
+def _int_field(where: str, meta: dict, field: str, lo: int, hi: int) -> int:
+    v = meta.get(field)
+    if not isinstance(v, int) or isinstance(v, bool) or not lo <= v <= hi:
+        raise ValueError(f"{where}: {field} {v!r}: must be an integer in [{lo}, {hi}]")
+    return v
+
+
+def _marker(where: str, field: str, v, vocab: list[str]) -> int:
+    """a marker token given as its vocabulary string ("[unused0]") or its id"""
+    if isinstance(v, str) and v in vocab:
+        return vocab.index(v)
+    if isinstance(v, int) and not isinstance(v, bool) and 0 <= v < len(vocab):
+        return v
+    raise ValueError(f"{where}: {field} {v!r}: not a token of vocab.txt")
+
+
+def read_colbert_spec(model_dir: str) -> dict:
+    """What Stanford ColBERT computes from a checkpoint, or a ValueError naming the file and field K5 does not restate.
+    Reads JSON and vocab.txt only (no weights, no GPU).  Forms:
+      Stanford  config.json (a BERT inside K5's shapes) + artifact.metadata (query_maxlen, doc_maxlen, dim,
+                mask_punctuation, attend_to_mask_tokens, query_token_id, doc_token_id, similarity); linear.weight in the
+                checkpoint's weights
+      PyLate    modules.json (Transformer, then a Dense module at `path`), <path>/config.json (out_features, bias false,
+                Identity activation), config_sentence_transformers.json (query_prefix, document_prefix, query_length,
+                document_length, attend_to_expansion_tokens, skiplist_words, do_query_expansion true) [3P-unverified]
+    Stanford's `interaction` must be "colbert" (MaxSim) when present.  Returns query_maxlen, doc_maxlen, dim, attend_to_mask_tokens, q_marker / d_marker (ids), mask_punctuation,
+    skip_words (None: string.punctuation), do_lower_case, weight (file, tensor name) of the projection."""
+    import string
+    join = os.path.join
+    cpath = join(model_dir, "config.json")
+    cfg = _json(cpath)
+    check_bert_config(cpath, cfg)
+    vpath = join(model_dir, "vocab.txt")
+    if not os.path.isfile(vpath):
+        raise ValueError(f"{vpath}: file missing (K5 takes WordPiece vocabularies)")
+    with open(vpath, encoding="utf-8") as f:
+        vocab = [line.rstrip("\n") for line in f]
+    if "[MASK]" not in vocab:
+        raise ValueError(f"{vpath}: no [MASK] token (ColBERT pads queries with [MASK])")
+    tc = _json(join(model_dir, "tokenizer_config.json"), required=False) or {}
+    lower = bool(tc.get("do_lower_case", True))
+    max_pos = cfg.get("max_position_embeddings", 512)
+    mpath = join(model_dir, "artifact.metadata")
+    if os.path.isfile(mpath):
+        meta = _json(mpath)
+        sim = meta.get("similarity", "cosine")
+        if sim != "cosine":
+            raise ValueError(f"{mpath}: similarity {sim!r}: K5 scores with ColBERT's cosine MaxSim only")
+        inter = meta.get("interaction", "colbert")
+        if inter != "colbert":
+            raise ValueError(f"{mpath}: interaction {inter!r}: K5 scores with ColBERT's MaxSim interaction only")
+        spec = {"query_maxlen": _int_field(mpath, meta, "query_maxlen", 3, COLBERT_QUERY_ROWS),
+                "doc_maxlen": _int_field(mpath, meta, "doc_maxlen", 3, max_pos),
+                "dim": _int_field(mpath, meta, "dim", 16, 256),
+                "q_marker": _marker(mpath, "query_token_id", meta.get("query_token_id", "[unused0]"), vocab),
+                "d_marker": _marker(mpath, "doc_token_id", meta.get("doc_token_id", "[unused1]"), vocab),
+                "skip_words": None, "do_lower_case": lower}
+        for flag, default in (("mask_punctuation", True), ("attend_to_mask_tokens", False)):
+            v = meta.get(flag, default)
+            if not isinstance(v, bool):
+                raise ValueError(f"{mpath}: {flag} {v!r}: must be true or false")
+            spec[flag] = v
+        if spec["dim"] % 16:
+            raise ValueError(f"{mpath}: dim {spec['dim']}: K5 projects to multiples of 16")
+        st = join(model_dir, "model.safetensors")
+        spec["weight"] = (st if os.path.exists(st) else join(model_dir, "pytorch_model.bin"), "linear.weight")
+        return spec
+    mods = _json(join(model_dir, "modules.json"), required=False)
+    dense = [m for m in (mods or []) if isinstance(m, dict) and str(m.get("type", "")).endswith("Dense")]
+    if not dense:
+        raise ValueError(f"{mpath}: file missing (a ColBERT snapshot has artifact.metadata, or a PyLate modules.json with a Dense module)")
+    if (len(mods) != 2 or len(dense) != 1 or mods[1] is not dense[0]
+            or not str(mods[0].get("type", "")).endswith("models.Transformer")):
+        raise ValueError(f"{join(model_dir, 'modules.json')}: {[m.get('type') for m in mods]!r}: K5 runs a Transformer followed by one Dense module")
+    dpath = join(model_dir, dense[0].get("path", ""), "config.json")
+    dc = _json(dpath)
+    if dc.get("bias", True):
+        raise ValueError(f"{dpath}: bias {dc.get('bias', True)!r}: ColBERT's projection has no bias")
+    act = str(dc.get("activation_function", "torch.nn.modules.linear.Identity"))
+    if not act.endswith("Identity"):
+        raise ValueError(f"{dpath}: activation_function {act!r}: ColBERT's projection is linear")
+    if dc.get("in_features") != cfg["hidden_size"]:
+        raise ValueError(f"{dpath}: in_features {dc.get('in_features')!r}: config.json hidden_size is {cfg['hidden_size']}")
+    spath = join(model_dir, "config_sentence_transformers.json")
+    sc = _json(spath)
+    if sc.get("do_query_expansion", True) is not True:
+        raise ValueError(f"{spath}: do_query_expansion {sc.get('do_query_expansion')!r}: ColBERT pads queries with [MASK]")
+    att = sc.get("attend_to_expansion_tokens", False)
+    if not isinstance(att, bool):
+        raise ValueError(f"{spath}: attend_to_expansion_tokens {att!r}: must be true or false")
+    words = sc.get("skiplist_words", list(string.punctuation))
+    if not isinstance(words, list) or not all(isinstance(w, str) for w in words):
+        raise ValueError(f"{spath}: skiplist_words {words!r}: must be a list of strings")
+    spec = {"query_maxlen": _int_field(spath, sc, "query_length", 3, COLBERT_QUERY_ROWS),
+            "doc_maxlen": _int_field(spath, sc, "document_length", 3, max_pos),
+            "dim": _int_field(dpath, dc, "out_features", 16, 256),
+            "q_marker": _marker(spath, "query_prefix", sc.get("query_prefix", "[unused0]"), vocab),
+            "d_marker": _marker(spath, "document_prefix", sc.get("document_prefix", "[unused1]"), vocab),
+            "mask_punctuation": bool(words), "attend_to_mask_tokens": att, "skip_words": words, "do_lower_case": lower}
+    if spec["dim"] % 16:
+        raise ValueError(f"{dpath}: out_features {spec['dim']}: K5 projects to multiples of 16")
+    wdir = join(model_dir, dense[0].get("path", ""))
+    st = join(wdir, "model.safetensors")
+    spec["weight"] = (st if os.path.exists(st) else join(wdir, "pytorch_model.bin"), "linear.weight")
+    return spec
+
+
+def colbert_query_ids(tokenizer, texts: list[str], query_maxlen: int, q_marker: int, mask_id: int, attend_to_mask: bool):
+    """(ids int32 [n, query_maxlen], key counts int32 [n]): [CLS] [Q] q... [SEP] cut to query_maxlen, [MASK] up to it; the
+    keys are the rows before the [MASK] padding, or all rows when attend_to_mask"""
+    ids = np.full((len(texts), query_maxlen), mask_id, np.int32)
+    keys = np.empty(len(texts), np.int32)
+    for i, t in enumerate(tokenizer.encode_batch_plain(list(texts))):
+        t = t[:query_maxlen - 3]
+        n = len(t) + 3
+        ids[i, 0], ids[i, 1], ids[i, 2:n - 1], ids[i, n - 1] = tokenizer.cls, q_marker, t, tokenizer.sep
+        keys[i] = query_maxlen if attend_to_mask else n
+    return ids, keys
+
+
+def colbert_skip_ids(tokenizer, words) -> np.ndarray:
+    """ColBERT's skiplist as ids: the first token id of each word (string.punctuation's characters by default)"""
+    import string
+    words = list(string.punctuation) if words is None else list(words)
+    return np.unique(np.asarray([t[0] for t in tokenizer.encode_batch_plain(words) if len(t)], np.int32))
+
+
+class GpuLateInteractionReranker:
+    """A ColBERT late-interaction model on the GPU (krag_late_rerank), with GpuCrossEncoder's interface: rerank(queries,
+    candidate ordinals per query, top_k, passages) and encode_passages for the store's per-ordinal token cache.  Each distinct
+    candidate ordinal of a call is encoded once."""
+
+    def __init__(self, engine, tokenizer, config: dict, state_dict: dict, weight: np.ndarray, spec: dict, precision: str = "fp32"):
+        from . import _native
+        if precision not in PRECISIONS:
+            raise ValueError(f"precision {precision!r}: expected 'fp32' or 'fp16'")
+        self.tokenizer, self.spec, self.precision = tokenizer, spec, precision
+        self.mask_id = tokenizer.vocab["[MASK]"]
+        self.skip = colbert_skip_ids(tokenizer, spec["skip_words"]) if spec["mask_punctuation"] else np.zeros(0, np.int32)
+        self._emb = _native.Embedder(engine, config["num_hidden_layers"], config["hidden_size"], config["num_attention_heads"],
+                                     config["intermediate_size"], config["vocab_size"], config.get("max_position_embeddings", 512),
+                                     config.get("type_vocab_size", 2), config.get("layer_norm_eps", 1e-12))
+        self._emb.set_late_interaction(weight)
+        self._emb.load_state_dict({k: v for k, v in state_dict.items() if k != "linear.weight"})
+        self._emb.set_precision(precision)
+        self._mu = threading.Lock()
+
+    @classmethod
+    def from_pretrained(cls, engine, model_dir: str, **kw):
+        """model_dir: a ColBERT snapshot (read_colbert_spec); raises ValueError when it asks for what K5 does not compute"""
+        from .embedding import _k5_name
+        from .text import WordPieceTokenizer
+        spec = read_colbert_spec(model_dir)
+        cfg = _json(os.path.join(model_dir, "config.json"))
+        state = load_state(model_dir)
+        wfile, wname = spec["weight"]
+        if os.path.dirname(wfile) != model_dir.rstrip(os.sep):          # PyLate: the Dense module's own weights file
+            wstate = {_k5_name(k): v for k, v in load_state(os.path.dirname(wfile)).items()}
+        else:
+            wstate = state
+        w = wstate.get(wname)
+        if w is None:
+            raise ValueError(f"{wfile}: tensor {wname} missing (the ColBERT projection)")
+        if tuple(np.shape(w)) != (spec["dim"], cfg["hidden_size"]):
+            raise ValueError(f"{wfile}: tensor {wname} has shape {tuple(np.shape(w))}, expected {(spec['dim'], cfg['hidden_size'])}")
+        for k in list(wstate):
+            if k.startswith("linear.") and k != "linear.weight":
+                raise ValueError(f"{wfile}: tensor {k}: ColBERT's projection has no bias")
+        tok = WordPieceTokenizer.from_file(os.path.join(model_dir, "vocab.txt"), do_lower_case=spec["do_lower_case"],
+                                           max_length=max(spec["doc_maxlen"], spec["query_maxlen"]))
+        return cls(engine, tok, cfg, state, np.asarray(w, np.float32), spec, **kw)
+
+    def query_ids(self, texts: list[str]):
+        s = self.spec
+        return colbert_query_ids(self.tokenizer, texts, s["query_maxlen"], s["q_marker"], self.mask_id, s["attend_to_mask_tokens"])
+
+    def encode_passages(self, texts: list[str]) -> list[tuple[np.ndarray, np.ndarray]]:
+        """(ids [CLS] [D] d... [SEP] cut to doc_maxlen, keep mask uint8: 0 on skiplist rows) of each text"""
+        keep_n = self.spec["doc_maxlen"] - 3
+        out = []
+        for t in self.tokenizer.encode_batch_plain(texts):
+            ids = np.concatenate([[self.tokenizer.cls, self.spec["d_marker"]], t[:keep_n], [self.tokenizer.sep]]).astype(np.int32)
+            out.append((ids, (~np.isin(ids, self.skip)).astype(np.uint8)))
+        return out
+
+    def rerank(self, queries: list[str], candidates: list, top_k: int, passages):
+        """(positions int32 [n_queries, top_k], scores float32 [n_queries, top_k]) of each query's best top_k candidates
+        (position within its candidate list; -1 / NaN past its count), ties by position ascending"""
+        q_ids, q_keys = self.query_ids(list(queries))
+        poff = np.zeros(len(candidates) + 1, np.int32)
+        np.cumsum([len(c) for c in candidates], out=poff[1:])
+        flat = np.concatenate([np.asarray(c, np.int64) for c in candidates]) if len(candidates) else np.zeros(0, np.int64)
+        uniq, pair_pass = np.unique(flat, return_inverse=True)
+        docs = passages(uniq, self.encode_passages) if len(uniq) else []
+        d_off = np.zeros(len(docs) + 1, np.int32)
+        np.cumsum([len(d[0]) for d in docs], out=d_off[1:])
+        d_tok = np.concatenate([d[0] for d in docs]) if docs else np.zeros(0, np.int32)
+        d_keep = np.concatenate([d[1] for d in docs]) if docs else np.zeros(0, np.uint8)
+        with self._mu:
+            return self._emb.late_rerank(q_ids, q_keys, d_tok, d_off, d_keep, poff, pair_pass.astype(np.int32), top_k)

@@ -140,10 +140,11 @@ class _IndexState:
         self.n_dead = 0                          # tombstoned nodes still in `nodes` (and rows in the engine)
         self._filter_cache: dict[str, tuple[int, np.ndarray]] = {}   # filter json -> (nodes covered, allow bitmap)
         self._frag_cache: dict[int, tuple[bytes, bytes]] = {}        # ordinal -> serialised halves of its NodeWithScore
-        self._pair_cache: dict[int, tuple] = {}                      # ordinal -> its cross-encoder tokens (ids, full length)
+        self._pair_cache: dict[int, tuple] = {}                      # ordinal -> its reranker tokens (encode_passages)
 
     def pair_passages(self, ordinals, encode) -> list[tuple]:
-        """the cross-encoder tokens of nodes `ordinals` (embed_text of each, as the embedder saw it): cached per ordinal,
+        """the reranker's tokens of nodes `ordinals` (embed_text of each, as the embedder saw it; `encode` is the reranker's
+        encode_passages: a cross-encoder's ids and full length, or a ColBERT model's ids and keep mask): cached per ordinal,
         misses tokenised in one `encode` call.  Two dispatcher threads may fill the cache at once under the store's reader
         lock: nodes are immutable and the tokeniser deterministic, so both compute the same entry, and a dict item assignment
         is atomic under the GIL -- the worst case is a node tokenised twice.  Compaction renumbers ordinals under the writer
@@ -217,8 +218,8 @@ class HybridRetriever:
         self._filter_pushdown = filter_pushdown
         self.want_components = True          # VectorStore turns this off unless KRAG_COMPONENT_SCORES=1 (saves 10 dicts per query)
         self.last_components: list[dict] = []
-        # cross-encoder (kaito_b200.rerank.GpuCrossEncoder or None): the fused max_results candidates are rescored and the
-        # rerank_top_k best kept
+        # reranker (kaito_b200.rerank.GpuCrossEncoder, GpuLateInteractionReranker or None): the fused max_results candidates
+        # are rescored and the rerank_top_k best kept
         self._reranker, self._rerank_top_k = reranker, rerank_top_k
 
     def _allow_bitmap(self):
@@ -268,8 +269,8 @@ class HybridRetriever:
         return out
 
     def _rerank(self, queries: list[str], out: dict) -> dict:
-        """the engine's arrays cut to the rerank_top_k fused candidates the cross-encoder scores highest, in that order
-        (equal scores: fused position ascending); "final" becomes the cross-encoder score, "dense" / "sparse" follow their
+        """the engine's arrays cut to the rerank_top_k fused candidates the reranker scores highest, in that order
+        (equal scores: fused position ascending); "final" becomes the reranker's score, "dense" / "sparse" follow their
         candidates (they describe the fusion stage)"""
         counts = np.asarray(out["count"])
         cands = [np.asarray(out["ordinal"][b, :int(counts[b])]) for b in range(len(queries))]
@@ -293,8 +294,8 @@ class VectorStore:
     def __init__(self, embed_model, engine, reranker=None):
         self.embed_model = embed_model
         self.engine = engine
-        # optional cross-encoder (KRAG_RERANK_MODEL_DIR): /retrieve fuses N = min(max(top_k, KRAG_RERANK_CANDIDATES),
-        # RAG_MAX_TOP_K) candidates and returns the top_k the cross-encoder scores highest
+        # optional reranker (KRAG_RERANK_MODEL_DIR: a cross-encoder or ColBERT): /retrieve fuses N = min(max(top_k, KRAG_RERANK_CANDIDATES),
+        # RAG_MAX_TOP_K) candidates and returns the top_k the reranker scores highest
         self.reranker = reranker
         self.rerank_candidates = int(os.getenv("KRAG_RERANK_CANDIDATES", "30"))
         self.dimension = embed_model.get_embedding_dimension()   # faiss_store.py:28
