@@ -146,3 +146,87 @@ def test_passage_ids_and_keep_mask(tmp_path):
         assert keep.tolist() == [0 if x in skip else 1 for x in want], t
     all_punct = r.encode_passages(["!!! ... ?"])[0]
     assert all_punct[1].tolist() == [1, 1, 0, 0, 0, 0, 0, 0, 0, 1]          # [CLS] [D] and [SEP] stay
+
+
+# ------------------------------------------------------------------------------------ the fmaf yardstick
+def _round_f32(x):
+    """the Fraction x rounded to the nearest fp32, ties to even (subnormals included), as a Python float"""
+    from fractions import Fraction
+    if x == 0:
+        return 0.0
+    sign, x = (-1.0 if x < 0 else 1.0), abs(x)
+    e = x.numerator.bit_length() - x.denominator.bit_length()
+    while Fraction(2) ** e > x:
+        e -= 1
+    while Fraction(2) ** (e + 1) <= x:
+        e += 1
+    ulp = Fraction(2) ** (max(e, -126) - 23)
+    m = x / ulp
+    n = m.numerator // m.denominator
+    r = m - n
+    if r > Fraction(1, 2) or (r == Fraction(1, 2) and n % 2):
+        n += 1
+    v = n * ulp
+    return sign * (float("inf") if v >= 2 ** 128 else float(v))
+
+
+def _exact_fmaf(a, b, c):
+    from fractions import Fraction
+    return np.float32(_round_f32(Fraction(float(a)) * Fraction(float(b)) + Fraction(float(c))))
+
+
+def _check_fmaf(a, b, c):
+    from tests import colbert_reference as cr
+    got = cr.fmaf(a, b, c)
+    want = np.array([_exact_fmaf(x, y, z) for x, y, z in zip(a, b, c)], np.float32)
+    bad = np.flatnonzero(got.view(np.int32) != want.view(np.int32))
+    assert not len(bad), [(float(a[i]), float(b[i]), float(c[i]), float(got[i]), float(want[i])) for i in bad[:5]]
+
+
+@pytest.mark.skipif(np.finfo(np.longdouble).nmant < 63, reason="needs a 64-bit long double significand")
+def test_fmaf_emulation_is_one_rounding_on_random_triples():
+    """tests/colbert_reference.fmaf (the yardstick of the exact MaxSim tests) against a Fraction fma rounded once to fp32:
+    unit-vector components (the kernel's operands) and accumulators of all sizes, and triples whose product is far above
+    or far below the addend, so the exact sum needs more than 64 bits"""
+    g = np.random.default_rng(0)
+    n = 6000
+    a = (g.standard_normal(n) / 8).astype(np.float32)
+    b = (g.standard_normal(n) / 8).astype(np.float32)
+    c = (g.standard_normal(n) * np.exp2(g.integers(-40, 12, n))).astype(np.float32)
+    _check_fmaf(a, b, c)
+    e = np.exp2(g.integers(-60, 60, (3, n)))
+    _check_fmaf(*[(g.standard_normal(n) * e[i]).astype(np.float32) for i in range(3)])
+
+
+@pytest.mark.skipif(np.finfo(np.longdouble).nmant < 63, reason="needs a 64-bit long double significand")
+def test_fmaf_emulation_near_fp32_midpoints():
+    """addends c of both parities and signs, and products that put c + a b exactly on the midpoint to c's neighbour (ties
+    to even), or 2^-k of an ulp to either side of it for k = 2 .. 24; fmaf(a, b, -fl(a b)) (the product's exact rounding
+    error); and the limit of the yardstick: a sum 2^-47 ulp below a midpoint, which the 64-bit intermediate rounds onto
+    the midpoint, so the emulation rounds an odd c the wrong way -- the error class of about 2^-40 the exact tests accept"""
+    g = np.random.default_rng(1)
+    cs = (g.standard_normal(64) * np.exp2(g.integers(-20, 20, 64))).astype(np.float32)
+    bits = cs.view(np.int32)
+    bits[::2] |= 1                                                 # odd significands ...
+    bits[1::2] &= ~1                                               # ... and even ones
+    assert (bits[::2] % 2 == 1).all() and (bits[1::2] % 2 == 0).all()
+    cs = np.concatenate([cs, -cs])
+    a, b, c = [], [], []
+    for x in cs:
+        half = np.float32(np.spacing(np.abs(x)) / 2) * np.sign(x)    # towards the neighbour away from zero
+        for k in range(2, 25):
+            for f in (1.0, 1.0 + 2.0 ** -(k - 1), 1.0 - 2.0 ** -(k - 1)):
+                a.append(half); b.append(np.float32(f)); c.append(x)
+        a.append(half); b.append(np.float32(-1.0)); c.append(x)     # the midpoint towards zero
+    a, b, c = (np.asarray(v, np.float32) for v in (a, b, c))
+    assert np.isfinite(a * b).all()
+    _check_fmaf(a, b, c)
+    p, q = (g.standard_normal((2, 2000)) / 8).astype(np.float32)
+    _check_fmaf(p, q, -(p * q))
+    from tests import colbert_reference as cr
+    for x in (np.float32(1.0), np.float32(1.0 + 2.0 ** -23)):
+        u = np.float32(np.spacing(x))
+        a1, b1 = np.float32(u / 2 * np.float32(1 + 2.0 ** -23)), np.float32(1 - 2.0 ** -23)   # a b = u / 2 (1 - 2^-46)
+        want, got = _exact_fmaf(a1, b1, x), cr.fmaf(a1, b1, x)
+        assert want == x
+        assert got == (x if x.view(np.int32) % 2 == 0 else np.nextafter(x, np.float32(2)))
