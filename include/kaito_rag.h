@@ -402,6 +402,37 @@ int32_t krag_late_rerank(krag_embedder* e, int32_t n_queries, int32_t query_len,
  * krag_late_rerank computes them.  Test hook. */
 int32_t krag_debug_late_vectors(krag_embedder* e, int32_t batch, const int32_t* tok_ids, const int32_t* tok_offsets, const int32_t* key_lens,
                                 float* out);
+/* Passage vector stores.  A store keeps, per ordinal, a passage's kept unit vectors (the rows krag_late_rerank lets into the
+ * max, in row order, fp32 [rows, dim]) in device slabs of at most 256 MB; they have the bits krag_debug_late_vectors gives
+ * for that passage alone, so a pair scored from a stored passage has the score it has when the passage is encoded in the
+ * call.  Every store created from one embedder draws its slabs from one budget of device bytes
+ * (krag_embedder_set_store_budget, default 0: nothing is stored; KRAG_E_INVALID when negative).  A store records the
+ * embedder's precision mode; an append or rerank under another mode is KRAG_E_INVALID.  The embedder cannot be destroyed
+ * while it has stores (KRAG_E_INVALID). */
+typedef struct krag_late_store krag_late_store;
+int32_t krag_embedder_set_store_budget(krag_embedder* e, int64_t bytes);
+int32_t krag_late_store_create(krag_embedder* e, krag_late_store** out);
+int32_t krag_late_store_destroy(krag_late_store* s);
+/* Passages p < n (passage_tok / passage_offsets / passage_keep as for krag_late_rerank, with its checks) become the next n
+ * ordinals, in order.  stored_out [n]: 1 where the passage was stored, 0 where the budget (or the device) had no room; an
+ * unstored ordinal is then scored by encoding it in the call, as without a store. */
+int32_t krag_late_store_append(krag_late_store* s, int32_t n, const int32_t* passage_tok, const int32_t* passage_offsets,
+                               const uint8_t* passage_keep, uint8_t* stored_out);
+/* Drops ordinals n_ordinals and up (rolls an append back), freeing slabs left empty. */
+int32_t krag_late_store_truncate(krag_late_store* s, int64_t n_ordinals);
+/* Keeps the ordinals whose bit is set in alive_bitmap (bit o % 32 of word o / 32; n_ordinals must be the store's ordinal
+ * count), renumbered 0 .. n_live - 1 in order; their rows move down on the device and slabs left empty are freed. */
+int32_t krag_late_store_compact(krag_late_store* s, const uint32_t* alive_bitmap, int64_t n_ordinals);
+/* ordinals, stored passages, stored rows and the slabs' device bytes (counted by krag_device_bytes); any pointer may be NULL */
+int32_t krag_late_store_stats(const krag_late_store* s, int64_t* ordinals, int64_t* stored, int64_t* rows, int64_t* device_bytes);
+/* krag_late_rerank with pair_source[j] >= 0 naming a stored ordinal (KRAG_E_INVALID when the store does not hold it) and
+ * pair_source[j] < 0 naming passage ~pair_source[j] of the call (n_passages may be 0 when every pair names an ordinal). */
+int32_t krag_late_rerank_stored(krag_embedder* e, const krag_late_store* s, int32_t n_queries, int32_t query_len, const int32_t* query_tok,
+                                const int32_t* query_keys, int32_t n_passages, const int32_t* passage_tok, const int32_t* passage_offsets,
+                                const uint8_t* passage_keep, const int32_t* pair_offsets, const int32_t* pair_source, int32_t top_k,
+                                int32_t* out_pos, float* out_score);
+/* The n_rows stored rows [n_rows, dim] of a stored ordinal (n_rows must be its row count).  Test hook. */
+int32_t krag_debug_late_store_vectors(const krag_late_store* s, int64_t ordinal, float* out, int64_t n_rows);
 int32_t krag_embedder_destroy(krag_embedder* e);
 
 /* ------------------------------------------------- host-side text analysis (no GPU involved; ASCII input) */

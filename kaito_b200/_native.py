@@ -45,6 +45,9 @@ SYMBOLS = [
     "krag_text_unigram_destroy", "krag_debug_tc_dump_pass", "krag_debug_tc_prune", "krag_debug_relative_bucket",
     "krag_wordpiece_create_specials", "krag_embedder_set_rotary", "krag_debug_rotary_cos_sin",
     "krag_embedder_set_late_interaction", "krag_late_rerank", "krag_debug_late_vectors",
+    "krag_embedder_set_store_budget", "krag_late_store_create", "krag_late_store_destroy", "krag_late_store_append",
+    "krag_late_store_truncate", "krag_late_store_compact", "krag_late_store_stats", "krag_late_rerank_stored",
+    "krag_debug_late_store_vectors",
 ]
 # krag_debug_tc_dump_pass / krag_debug_tc_prune: the prune pass to run (KRAG_TC_PASS_*)
 TC_PASS_TF32, TC_PASS_BF16_SPLIT, TC_PASS_BF16_SHADOW, TC_PASS_BF16_HOST = 0, 1, 2, 3
@@ -156,6 +159,15 @@ def load() -> C.CDLL:
     L.krag_embedder_set_late_interaction.argtypes = [vp, i32, vp, i64]
     L.krag_late_rerank.argtypes = [vp, i32, i32, vp, vp, i32, vp, vp, vp, vp, vp, i32, vp, vp]
     L.krag_debug_late_vectors.argtypes = [vp, i32, vp, vp, vp, vp]
+    L.krag_embedder_set_store_budget.argtypes = [vp, i64]
+    L.krag_late_store_create.argtypes = [vp, C.POINTER(vp)]
+    L.krag_late_store_destroy.argtypes = [vp]
+    L.krag_late_store_append.argtypes = [vp, i32, vp, vp, vp, vp]
+    L.krag_late_store_truncate.argtypes = [vp, i64]
+    L.krag_late_store_compact.argtypes = [vp, vp, i64]
+    L.krag_late_store_stats.argtypes = [vp, vp, vp, vp, vp]
+    L.krag_late_rerank_stored.argtypes = [vp, vp, i32, i32, vp, vp, i32, vp, vp, vp, vp, vp, i32, vp, vp]
+    L.krag_debug_late_store_vectors.argtypes = [vp, i64, vp, i64]
     L.krag_wordpiece_encode_batch.argtypes = [vp, i64, C.c_char_p, vp, i32, vp, vp]
     L.krag_wordpiece_destroy.argtypes = [vp]
     L.krag_text_unigram_create.argtypes = [C.c_char_p, vp, vp, i64, i32, C.c_char_p, i64, i32, C.c_char_p, vp, vp, vp, i32,
@@ -426,6 +438,28 @@ class Embedder:
         check(self._L.krag_debug_late_vectors(self._h, len(offsets) - 1, ptr(flat_tokens), ptr(offsets), ptr(kl), ptr(out)))
         return out
 
+    def set_store_budget(self, nbytes: int):
+        """device bytes every LateStore of this embedder may hold in all (krag_embedder_set_store_budget; 0: none)"""
+        check(self._L.krag_embedder_set_store_budget(self._h, int(nbytes)))
+
+    def late_rerank_stored(self, store: "LateStore", q_tokens, q_keys, p_tokens, p_offsets, p_keep, pair_offsets, pair_source,
+                           top_k: int):
+        """krag_late_rerank_stored: late_rerank with pair_source[j] >= 0 a stored ordinal of `store`, < 0 passage
+        ~pair_source[j] of the call (the packed passages may be empty)"""
+        q_tokens = np.ascontiguousarray(q_tokens, np.int32)
+        nq, ql = q_tokens.shape
+        q_keys = np.ascontiguousarray(q_keys, np.int32)
+        p_tokens = np.ascontiguousarray(p_tokens, np.int32); p_offsets = np.ascontiguousarray(p_offsets, np.int32)
+        p_keep = np.ascontiguousarray(p_keep, np.uint8)
+        pair_offsets = np.ascontiguousarray(pair_offsets, np.int32); pair_source = np.ascontiguousarray(pair_source, np.int32)
+        pos = np.empty((nq, top_k), np.int32)
+        sc = np.empty((nq, top_k), np.float32)
+        n_pass = max(len(p_offsets) - 1, 0)
+        check(self._L.krag_late_rerank_stored(self._h, store._h, nq, ql, ptr(q_tokens), ptr(q_keys), n_pass, ptr(p_tokens) if n_pass else None,
+                                              ptr(p_offsets) if n_pass else None, ptr(p_keep) if n_pass else None, ptr(pair_offsets),
+                                              ptr(pair_source), top_k, ptr(pos), ptr(sc)))
+        return pos, sc
+
     def debug_cls_rows(self, on: bool):
         """test hook: False runs the last layer over every token under CLS pooling too (same embeddings)"""
         check(self._L.krag_debug_embedder_cls_rows(self._h, 1 if on else 0))
@@ -433,6 +467,51 @@ class Embedder:
     def destroy(self):
         if self._h:
             check(self._L.krag_embedder_destroy(self._h))
+            self._h = None
+
+
+class LateStore:
+    """krag_late_store: the kept token vectors of passages, per ordinal, on the embedder's GPU (see kaito_rag.h).  Holds its
+    embedder, which cannot be destroyed before it."""
+
+    def __init__(self, emb: Embedder):
+        self.emb, self._L = emb, emb._L
+        h = C.c_void_p()
+        check(self._L.krag_late_store_create(emb._h, C.byref(h)))
+        self._h = h
+
+    def append(self, p_tokens, p_offsets, p_keep) -> np.ndarray:
+        """the next len(p_offsets) - 1 ordinals; uint8 [n]: 1 where the passage was stored"""
+        p_tokens = np.ascontiguousarray(p_tokens, np.int32); p_offsets = np.ascontiguousarray(p_offsets, np.int32)
+        p_keep = np.ascontiguousarray(p_keep, np.uint8)
+        out = np.zeros(len(p_offsets) - 1, np.uint8)
+        check(self._L.krag_late_store_append(self._h, len(out), ptr(p_tokens), ptr(p_offsets), ptr(p_keep), ptr(out)))
+        return out
+
+    def truncate(self, n_ordinals: int):
+        check(self._L.krag_late_store_truncate(self._h, int(n_ordinals)))
+
+    def compact(self, alive: np.ndarray):
+        """alive: bool [ordinals]; the live ordinals keep their order and become 0 .. n_live - 1"""
+        alive = np.asarray(alive, bool)
+        bm = np.zeros((len(alive) + 31) // 32, np.uint32)
+        idx = np.flatnonzero(alive)
+        np.bitwise_or.at(bm, idx >> 5, (np.uint32(1) << (idx & 31).astype(np.uint32)))
+        check(self._L.krag_late_store_compact(self._h, ptr(bm), len(alive)))
+
+    def stats(self) -> dict:
+        v = [C.c_int64() for _ in range(4)]
+        check(self._L.krag_late_store_stats(self._h, *[C.byref(x) for x in v]))
+        return dict(zip(("ordinals", "stored", "rows", "device_bytes"), (int(x.value) for x in v)))
+
+    def debug_vectors(self, ordinal: int, n_rows: int) -> np.ndarray:
+        out = np.empty((n_rows, self.emb.li_dim), np.float32)
+        check(self._L.krag_debug_late_store_vectors(self._h, int(ordinal), ptr(out), int(n_rows)))
+        return out
+
+    def destroy(self):
+        if self._h:
+            check(self._L.krag_late_store_destroy(self._h))
             self._h = None
 
 

@@ -1735,6 +1735,89 @@ int32_t krag_debug_late_vectors(krag_embedder* h, int32_t batch, const int32_t* 
         embedder_late_vectors(h->e, batch, tok_ids, tok_offsets, key_lens, out);
     });
 }
+struct krag_late_store { krag_embedder* emb; LateStore* s; };
+int32_t krag_embedder_set_store_budget(krag_embedder* h, int64_t bytes)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(h, KRAG_E_INVALID, "null embedder");
+        embedder_set_store_budget(h->e, bytes);
+    });
+}
+int32_t krag_late_store_create(krag_embedder* h, krag_late_store** out)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(h && out, KRAG_E_INVALID, "null argument");
+        *out = new krag_late_store{h, late_store_create(h->e)};
+    });
+}
+int32_t krag_late_store_destroy(krag_late_store* s)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(s, KRAG_E_INVALID, "null store");
+        cudaSetDevice(s->emb->ctx->di.device);
+        late_store_destroy(s->s);
+        delete s;
+    });
+}
+int32_t krag_late_store_append(krag_late_store* s, int32_t n, const int32_t* passage_tok, const int32_t* passage_offsets,
+                               const uint8_t* passage_keep, uint8_t* stored_out)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(s && passage_tok && passage_offsets && passage_keep && stored_out && n >= 1, KRAG_E_INVALID, "bad argument");
+        KRAG_CUDA(cudaSetDevice(s->emb->ctx->di.device));
+        late_store_append(s->s, n, passage_tok, passage_offsets, passage_keep, stored_out);
+    });
+}
+int32_t krag_late_store_truncate(krag_late_store* s, int64_t n_ordinals)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(s, KRAG_E_INVALID, "null store");
+        KRAG_CUDA(cudaSetDevice(s->emb->ctx->di.device));
+        late_store_truncate(s->s, n_ordinals);
+    });
+}
+int32_t krag_late_store_compact(krag_late_store* s, const uint32_t* alive_bitmap, int64_t n_ordinals)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(s && (alive_bitmap || n_ordinals == 0), KRAG_E_INVALID, "bad argument");
+        KRAG_CUDA(cudaSetDevice(s->emb->ctx->di.device));
+        late_store_compact(s->s, alive_bitmap, n_ordinals);
+    });
+}
+int32_t krag_late_store_stats(const krag_late_store* s, int64_t* ordinals, int64_t* stored, int64_t* rows, int64_t* device_bytes)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(s, KRAG_E_INVALID, "null store");
+        int64_t v[4];
+        late_store_stats(s->s, &v[0], &v[1], &v[2], &v[3]);
+        if (ordinals) *ordinals = v[0];
+        if (stored) *stored = v[1];
+        if (rows) *rows = v[2];
+        if (device_bytes) *device_bytes = v[3];
+    });
+}
+int32_t krag_late_rerank_stored(krag_embedder* h, const krag_late_store* s, int32_t n_queries, int32_t query_len, const int32_t* query_tok,
+                                const int32_t* query_keys, int32_t n_passages, const int32_t* passage_tok, const int32_t* passage_offsets,
+                                const uint8_t* passage_keep, const int32_t* pair_offsets, const int32_t* pair_source, int32_t top_k,
+                                int32_t* out_pos, float* out_score)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(h && s && query_tok && query_keys && pair_offsets && out_pos && out_score && n_queries >= 1, KRAG_E_INVALID, "bad argument");
+        KRAG_REQUIRE(pair_offsets[n_queries] == 0 || pair_source, KRAG_E_INVALID, "bad argument");
+        KRAG_REQUIRE(n_passages == 0 || (passage_tok && passage_offsets && passage_keep), KRAG_E_INVALID, "bad argument");
+        KRAG_CUDA(cudaSetDevice(h->ctx->di.device));
+        late_store_rerank(h->e, s->s, n_queries, query_len, query_tok, query_keys, n_passages, passage_tok, passage_offsets, passage_keep,
+                          pair_offsets, pair_source, top_k, out_pos, out_score);
+    });
+}
+int32_t krag_debug_late_store_vectors(const krag_late_store* s, int64_t ordinal, float* out, int64_t n_rows)
+{
+    return guarded([&] {
+        KRAG_REQUIRE(s && out, KRAG_E_INVALID, "null argument");
+        KRAG_CUDA(cudaSetDevice(s->emb->ctx->di.device));
+        late_store_vectors(s->s, ordinal, out, n_rows);
+    });
+}
 int32_t krag_embedder_destroy(krag_embedder* h)
 {
     return guarded([&] {

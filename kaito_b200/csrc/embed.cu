@@ -10,7 +10,7 @@
 //   L x [ QKV GEMM -> attention -> O GEMM (+bias +residual) -> LayerNorm -> FFN1 GEMM (+bias, erf-GELU)
 //         -> FFN2 GEMM (+bias +residual) -> LayerNorm ]  ->  CLS row or token mean (krag_embedder_set_pooling)  ->  L2 normalise
 // Late interaction (ColBERT, krag_late_rerank): every token row of the last layer -> hidden x dim projection -> L2 normalise,
-// then maxsim_kernel scores (query, passage) pairs from the token vectors.
+// then maxsim_kernel scores (query, passage) pairs from the kept token vectors, of the call's passages or of a LateStore.
 //
 // The four GEMMs per layer (24 S d^2 of the 24 S d^2 + 4 S^2 d flops) run on fp16 wgmma over split operands (see
 // gemm_f16s_kernel) with fp32 accumulation in registers, operands staged by TMA; bias / GELU / residual are fused into
@@ -909,77 +909,114 @@ rerank_select_kernel(const float* __restrict__ scores, const int32_t* __restrict
 }
 
 // ------------------------------------------------------------------------------------ late interaction (ColBERT)
-// MaxSim: score(q, P) = sum_{i < q_rows} max_{j in P, keep[j]} q_i . d_j over unit token vectors (rows of stride ld floats,
-// dim columns read).  One CTA per (query, slice of its pairs): query q's q_rows vectors are staged in shared memory once,
-// then each pair p of the slice (pair_pass[p] = its passage) streams the passage's rows 32 at a time.  Thread (i, jl) =
-// (tid / 8, tid % 8) owns query row i and passage rows jl + 8 u of a chunk (u < 4): every dot product is one fp32 fmaf chain
-// over k = 0 .. dim - 1 in order, the max over rows is exact (so the row order does not matter), and one thread adds the
-// q_rows maxima in row order.  A pair's score therefore depends on its two token matrices alone.  Rows are padded by 4 floats
-// in shared memory, so the 16-byte reads of 8 rows at one k hit 8 distinct bank groups.
-constexpr int MS_QROWS = 32, MS_CHUNK = 32, MS_THREADS = 256;
+// MaxSim over a pair table: pair p scores the rows tab[p].rows [tab[p].n][dim] (stride dim; every row enters the max: the
+// kept rows of a stored passage, or of a passage encoded in the call) against its query's q_rows unit vectors (rows of
+// stride ld): score = sum_{i < q_rows} max_{j < n} q_i . d_j.  Query q owns pairs pair_off[q] .. pair_off[q + 1].  One CTA
+// per (query, slice of its pairs): the query's rows are staged in shared memory once, then the CTA walks the 32-row chunks of
+// its pairs as one sequence, with the next MS_STAGES - 1 chunks in flight by cp.async across pair boundaries.  Thread (i, jl)
+// = (tid / 8, tid % 8) owns query row i and chunk rows jl + 8 u (u < 4): every dot product is one fp32 fmaf chain over
+// k = 0 .. dim - 1 in order, the max over rows is exact (so the row order does not matter), and one thread adds the q_rows
+// maxima in row order.  A pair's score therefore depends on its two token matrices alone, wherever its rows live.  Rows are
+// padded by 4 floats in shared memory, so the 16-byte reads of 8 rows at one k hit 8 distinct bank groups.
+struct MsPair { const float* rows; int32_t n, unused; };
+constexpr int MS_QROWS = 32, MS_CHUNK = 32, MS_THREADS = 256, MS_STAGES = 3;
 __global__ void __launch_bounds__(MS_THREADS)
-maxsim_kernel(const float* __restrict__ qv, int q_rows, const float* __restrict__ pv, const int32_t* __restrict__ p_off,
-              const uint8_t* __restrict__ keep, const int32_t* __restrict__ pair_off, const int32_t* __restrict__ pair_pass, int dim,
-              int ld, float* __restrict__ scores)
+maxsim_kernel(const float* __restrict__ qv, int q_rows, int ld, const MsPair* __restrict__ tab, const int32_t* __restrict__ pair_off,
+              int dim, float* __restrict__ scores)
 {
     extern __shared__ __align__(16) float ms_sm[];
-    const int LDS = dim + 4;
+    const int LDS = dim + 4, c4 = dim / 4;
     float* sQ = ms_sm;                                  // [MS_QROWS][LDS]
-    float* sD = sQ + MS_QROWS * LDS;                    // [MS_CHUNK][LDS]
-    float* sMax = sD + MS_CHUNK * LDS;                  // [MS_QROWS]
-    int* sKeep = reinterpret_cast<int*>(sMax + MS_QROWS);   // [MS_CHUNK]
-    const int q = blockIdx.x, tid = threadIdx.x, i = tid >> 3, jl = tid & 7, c4 = dim / 4;
-    const int p_begin = pair_off[q], p_end = pair_off[q + 1];
-    if (p_begin + (int)blockIdx.y >= p_end) return;
+    float* sD = sQ + MS_QROWS * LDS;                    // [MS_STAGES][MS_CHUNK][LDS]
+    float* sMax = sD + MS_STAGES * MS_CHUNK * LDS;      // [MS_QROWS]
+    const int q = blockIdx.x, tid = threadIdx.x, i = tid >> 3, jl = tid & 7, step = (int)gridDim.y;
+    const int p_end = pair_off[q + 1];
+    int lp = pair_off[q] + (int)blockIdx.y, lc = 0;     // the next chunk to load: rows lc .. of pair lp
+    if (lp >= p_end) return;
+    MsPair lt = tab[lp];
+    int cp = lp, cc = 0, cn = lt.n;                     // the chunk to score: rows cc .. of pair cp (cn rows)
     for (int x = tid; x < q_rows * c4; x += MS_THREADS) {
-        const int r = x / c4, c = x % c4;
+        const int r = x / c4, c = x - r * c4;
         *reinterpret_cast<float4*>(sQ + r * LDS + 4 * c) = *reinterpret_cast<const float4*>(qv + ((size_t)q * q_rows + r) * ld + 4 * c);
     }
-    for (int p = p_begin + (int)blockIdx.y; p < p_end; p += gridDim.y) {
-        const int pp = pair_pass[p], r0 = p_off[pp], r1 = p_off[pp + 1];
-        float m = -CUDART_INF_F;
-        for (int c0 = r0; c0 < r1; c0 += MS_CHUNK) {
-            const int n = r1 - c0 < MS_CHUNK ? r1 - c0 : MS_CHUNK;
-            __syncthreads();                            // the previous chunk (and the query rows) are staged / consumed
+    // one commit group per chunk slot, empty once the slice's chunks are all issued
+    auto issue = [&](int stage) {
+        if (lp < p_end) {
+            const int n = lt.n - lc < MS_CHUNK ? lt.n - lc : MS_CHUNK;
+            const float* src = lt.rows + (size_t)lc * dim;
+            const uint32_t dst = (uint32_t)__cvta_generic_to_shared(sD + stage * MS_CHUNK * LDS);
             for (int x = tid; x < n * c4; x += MS_THREADS) {
-                const int r = x / c4, c = x % c4;
-                *reinterpret_cast<float4*>(sD + r * LDS + 4 * c) = *reinterpret_cast<const float4*>(pv + ((size_t)c0 + r) * ld + 4 * c);
+                const int r = x / c4, c = x - r * c4;
+                cp_async16_zfill(dst + 4u * (uint32_t)(r * LDS + 4 * c), src + 4 * (size_t)x, true);
             }
-            if (tid < MS_CHUNK) sKeep[tid] = tid < n ? (int)keep[c0 + tid] : 0;
-            __syncthreads();
-            if (i < q_rows) {
-                float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-                const float* qr = sQ + i * LDS;
-                for (int k = 0; k < c4; ++k) {
-                    const float4 a = *reinterpret_cast<const float4*>(qr + 4 * k);
-                    const float4 b0 = *reinterpret_cast<const float4*>(sD + jl * LDS + 4 * k);
-                    const float4 b1 = *reinterpret_cast<const float4*>(sD + (jl + 8) * LDS + 4 * k);
-                    const float4 b2 = *reinterpret_cast<const float4*>(sD + (jl + 16) * LDS + 4 * k);
-                    const float4 b3 = *reinterpret_cast<const float4*>(sD + (jl + 24) * LDS + 4 * k);
-                    a0 = fmaf(a.x, b0.x, a0); a0 = fmaf(a.y, b0.y, a0); a0 = fmaf(a.z, b0.z, a0); a0 = fmaf(a.w, b0.w, a0);
-                    a1 = fmaf(a.x, b1.x, a1); a1 = fmaf(a.y, b1.y, a1); a1 = fmaf(a.z, b1.z, a1); a1 = fmaf(a.w, b1.w, a1);
-                    a2 = fmaf(a.x, b2.x, a2); a2 = fmaf(a.y, b2.y, a2); a2 = fmaf(a.z, b2.z, a2); a2 = fmaf(a.w, b2.w, a2);
-                    a3 = fmaf(a.x, b3.x, a3); a3 = fmaf(a.y, b3.y, a3); a3 = fmaf(a.z, b3.z, a3); a3 = fmaf(a.w, b3.w, a3);
-                }
-                if (sKeep[jl]) m = fmaxf(m, a0);
-                if (sKeep[jl + 8]) m = fmaxf(m, a1);
-                if (sKeep[jl + 16]) m = fmaxf(m, a2);
-                if (sKeep[jl + 24]) m = fmaxf(m, a3);
+            lc += MS_CHUNK;
+            if (lc >= lt.n) {
+                lp += step; lc = 0;
+                if (lp < p_end) lt = tab[lp];
             }
         }
-        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));   // the 8 threads of a query row are adjacent lanes
-        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
-        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
-        if (jl == 0 && i < q_rows) sMax[i] = m;
-        __syncthreads();
-        if (tid == 0) {
-            float s = 0.f;
-            for (int r = 0; r < q_rows; ++r) s += sMax[r];
-            scores[p] = s;
+        am_commit();
+    };
+#pragma unroll
+    for (int s = 0; s < MS_STAGES - 1; ++s) issue(s);
+    float m = -CUDART_INF_F;
+    for (int t = 0; cp < p_end; ++t) {
+        am_wait<MS_STAGES - 2>();
+        __syncthreads();                                // chunk t (and the query rows) staged; chunk t - 1's stage consumed
+        issue((t + MS_STAGES - 1) % MS_STAGES);
+        const float* sC = sD + (t % MS_STAGES) * MS_CHUNK * LDS;
+        const int n = cn - cc;                          // rows of this chunk: min(n, MS_CHUNK)
+        if (i < q_rows) {
+            float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+            const float* qr = sQ + i * LDS;
+            for (int k = 0; k < c4; ++k) {
+                const float4 a = *reinterpret_cast<const float4*>(qr + 4 * k);
+                const float4 b0 = *reinterpret_cast<const float4*>(sC + jl * LDS + 4 * k);
+                const float4 b1 = *reinterpret_cast<const float4*>(sC + (jl + 8) * LDS + 4 * k);
+                const float4 b2 = *reinterpret_cast<const float4*>(sC + (jl + 16) * LDS + 4 * k);
+                const float4 b3 = *reinterpret_cast<const float4*>(sC + (jl + 24) * LDS + 4 * k);
+                a0 = fmaf(a.x, b0.x, a0); a0 = fmaf(a.y, b0.y, a0); a0 = fmaf(a.z, b0.z, a0); a0 = fmaf(a.w, b0.w, a0);
+                a1 = fmaf(a.x, b1.x, a1); a1 = fmaf(a.y, b1.y, a1); a1 = fmaf(a.z, b1.z, a1); a1 = fmaf(a.w, b1.w, a1);
+                a2 = fmaf(a.x, b2.x, a2); a2 = fmaf(a.y, b2.y, a2); a2 = fmaf(a.z, b2.z, a2); a2 = fmaf(a.w, b2.w, a2);
+                a3 = fmaf(a.x, b3.x, a3); a3 = fmaf(a.y, b3.y, a3); a3 = fmaf(a.z, b3.z, a3); a3 = fmaf(a.w, b3.w, a3);
+            }
+            if (jl < n) m = fmaxf(m, a0);
+            if (jl + 8 < n) m = fmaxf(m, a1);
+            if (jl + 16 < n) m = fmaxf(m, a2);
+            if (jl + 24 < n) m = fmaxf(m, a3);
+        }
+        cc += MS_CHUNK;
+        if (cc >= cn) {                                 // the pair's last chunk
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));   // the 8 threads of a query row are adjacent lanes
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
+            if (jl == 0 && i < q_rows) sMax[i] = m;
+            __syncthreads();
+            if (tid == 0) {
+                float s = 0.f;
+                for (int r = 0; r < q_rows; ++r) s += sMax[r];
+                scores[cp] = s;
+            }
+            m = -CUDART_INF_F;
+            cp += step; cc = 0;
+            if (cp < p_end) cn = tab[cp].n;
         }
     }
+    am_wait<0>();
 }
-static size_t maxsim_smem(int dim) { return sizeof(float) * ((size_t)(MS_QROWS + MS_CHUNK) * (dim + 4) + MS_QROWS) + sizeof(int) * MS_CHUNK; }
+static size_t maxsim_smem(int dim) { return sizeof(float) * ((size_t)(MS_QROWS + MS_STAGES * MS_CHUNK) * (dim + 4) + MS_QROWS); }
+
+// Row r of the output, dst[r] (dim floats), is row src[r] of `in` (stride ld): the kept rows of passages encoded at stride
+// li_pad, gathered into a store's slabs or a call's compact scratch.  One warp per row; a copy, so the bits do not change.
+__global__ void __launch_bounds__(256)
+late_gather_kernel(const float* __restrict__ in, int ld, const int32_t* __restrict__ src, float* const* __restrict__ dst, int n_rows, int dim)
+{
+    const int r = (int)((blockIdx.x * 256u + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+    if (r >= n_rows) return;
+    const float4* a = reinterpret_cast<const float4*>(in + (size_t)src[r] * ld);
+    float4* b = reinterpret_cast<float4*>(dst[r]);
+    for (int c = lane; c < dim / 4; c += 32) b[c] = a[c];
+}
 
 // ------------------------------------------------------------------------------------ host
 // launch with programmatic stream serialization (see pdl_wait in tc_ptx.cuh); only for kernels that call pdl_wait()
@@ -1236,8 +1273,13 @@ struct Embedder {
     SplitMat s_li{nullptr, nullptr};
     DevArray<float> li_bias;
     DevArray<float> li_c, li_q, li_p;     // projection scratch [cap_tok][li_pad]; query / passage unit vectors, rows of li_pad
-    DevArray<int32_t> d_kvl, li_off, li_pp;
-    DevArray<uint8_t> li_keep;
+    DevArray<float> li_k;                 // the kept rows of a call's passages, rows of li_dim (late_gather_kernel)
+    DevArray<int32_t> d_kvl, li_src;      // li_src / li_dst: a gather's source row and destination of every kept row
+    DevArray<float*> li_dst;
+    DevArray<MsPair> li_tab;              // maxsim_kernel's pair table
+    // stores of passage vectors (LateStore) made from this embedder: their slabs share one budget of device bytes
+    int64_t store_budget = 0, store_bytes = 0;
+    int n_stores = 0;
     bool finalized = false;
     cudaStream_t st = nullptr;
     cudaEvent_t done = nullptr, in_ev = nullptr;
@@ -1532,7 +1574,11 @@ void embedder_finalize(Embedder* e)
     e->finalized = true;
 }
 
-void embedder_destroy(Embedder* e) { delete e; }
+void embedder_destroy(Embedder* e)
+{
+    if (e->n_stores) throw std::runtime_error("embedder: destroy its passage vector stores first");
+    delete e;
+}
 
 int embedder_hidden(const Embedder* e) { return e->cfg.hidden; }
 
@@ -1890,14 +1936,261 @@ void embedder_late_vectors(Embedder* e, int batch, const int32_t* tok_ids, const
     KRAG_CUDA(cudaStreamSynchronize(e->st));
 }
 
-// Late-interaction reranking.  n_queries queries of q_rows tokens each (q_tok [n_queries * q_rows], keys q_kv[i] <= q_rows),
-// n_pass distinct passages (p_tok packed by p_off [n_pass + 1], p_keep[t] = 1 where row t enters the max), query i owns pairs
-// pair_off[i] .. pair_off[i + 1], pair p scores passage pair_pass[p].  Each query and each passage is encoded once; maxsim_kernel
-// writes every pair's score at its offset, rerank_select_kernel orders each query's scores as for krag_rerank.
-void embedder_late_rerank(Embedder* e, int n_queries, int q_rows, const int32_t* q_tok, const int32_t* q_kv, int n_pass, const int32_t* p_tok,
-                          const int32_t* p_off, const uint8_t* p_keep, const int32_t* pair_off, const int32_t* pair_pass, int top_k,
-                          int32_t* out_pos, float* out_score)
+static void late_gather(Embedder* e, const float* in, const std::vector<int32_t>& src, const std::vector<float*>& dst)
 {
+    const int64_t n = (int64_t)src.size();
+    if (n == 0) return;
+    if (e->li_src.cap < n) e->li_src.alloc(n);
+    if (e->li_dst.cap < n) e->li_dst.alloc(n);
+    KRAG_CUDA(cudaMemcpyAsync(e->li_src.p, src.data(), sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, e->st));
+    KRAG_CUDA(cudaMemcpyAsync(e->li_dst.p, dst.data(), sizeof(float*) * (size_t)n, cudaMemcpyHostToDevice, e->st));
+    late_gather_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, e->st>>>(in, e->li_pad, e->li_src.p, e->li_dst.p, (int)n, e->li_dim);
+    KRAG_CUDA(cudaGetLastError());
+    count_launch();
+}
+
+static int kept_rows(const int32_t* p_off, const uint8_t* p_keep, int p)
+{
+    int kept = 0;
+    for (int t = p_off[p]; t < p_off[p + 1]; ++t) kept += p_keep[t] != 0;
+    return kept;
+}
+static void check_passages(const Embedder* e, int n_pass, const int32_t* p_off, const uint8_t* p_keep)
+{
+    late_check(e, n_pass, p_off);
+    for (int p = 0; p < n_pass; ++p)
+        if (!kept_rows(p_off, p_keep, p)) throw std::runtime_error("embedder: every passage needs at least one row that enters the max");
+}
+
+// ---- passage vector stores
+// A LateStore holds the kept rows of passages, per ordinal, in fixed-size device slabs (skiplist rows never enter the max,
+// so they are not stored): passage o is tab[o].rows unit vectors of dim floats, contiguous from float offset tab[o].off of
+// slab tab[o].slab (-1: not stored).  Passages fill the last slab in ordinal order; one that does not fit there opens a new
+// slab of min(LATE_SLAB_BYTES, what the embedder's budget has left) bytes, or stays unstored when that is too small (it is
+// then encoded per call).  A passage never straddles two slabs and a slab never moves, so growing the store copies nothing.
+// Positions grow with the ordinal (next fit), which compaction relies on.
+constexpr int64_t LATE_SLAB_BYTES = (int64_t)256 << 20;
+struct LateStore {
+    struct Slab { DevArray<float> a; int64_t used = 0; };
+    struct Entry { int32_t slab, rows; int64_t off; };
+    Embedder* e = nullptr;
+    int precision = EMB_PREC_FP32, dim = 0;
+    std::vector<Slab> slabs;
+    std::vector<Entry> tab;
+};
+
+void embedder_set_store_budget(Embedder* e, int64_t bytes)
+{
+    if (bytes < 0) throw std::runtime_error("embedder: the store budget must be >= 0 bytes");
+    e->store_budget = bytes;
+}
+
+LateStore* late_store_create(Embedder* e)
+{
+    if (!e->finalized || !e->li_pad) throw std::runtime_error("embedder: a passage vector store needs a finalized late-interaction embedder");
+    LateStore* s = new LateStore;
+    s->e = e; s->precision = e->precision; s->dim = e->li_dim;
+    ++e->n_stores;
+    return s;
+}
+
+static void store_pop_slab(LateStore* s)
+{
+    s->e->store_bytes -= s->slabs.back().a.bytes();
+    s->slabs.pop_back();
+}
+
+void late_store_destroy(LateStore* s)
+{
+    while (!s->slabs.empty()) store_pop_slab(s);
+    --s->e->n_stores;
+    delete s;
+}
+
+static void store_check(const LateStore* s, const Embedder* e)
+{
+    if (s->e != e) throw std::runtime_error("embedder: the store belongs to another embedder");
+    if (s->precision != e->precision) throw std::runtime_error("embedder: the store holds vectors of another precision mode");
+}
+
+// room for `rows` rows in the last slab or a new one; false: the budget (or the device) has no room
+static bool store_place(LateStore* s, int rows, LateStore::Entry& en)
+{
+    const int64_t need = (int64_t)rows * s->dim;
+    if (s->slabs.empty() || s->slabs.back().a.cap - s->slabs.back().used < need) {
+        const int64_t room = std::min(LATE_SLAB_BYTES, s->e->store_budget - s->e->store_bytes) / (int64_t)sizeof(float);
+        if (room < need) return false;
+        LateStore::Slab sl;
+        try {
+            sl.a.alloc(room);
+        } catch (const DevOom&) {
+            return false;
+        }
+        s->e->store_bytes += sl.a.bytes();
+        s->slabs.push_back(std::move(sl));
+    }
+    LateStore::Slab& sl = s->slabs.back();
+    en.slab = (int32_t)s->slabs.size() - 1;
+    en.off = sl.used;
+    sl.used += need;
+    return true;
+}
+
+// slabs past the last stored passage are freed; the last one's fill ends after that passage
+static void store_trim(LateStore* s)
+{
+    int last = -1;
+    int64_t end = 0;
+    for (auto it = s->tab.rbegin(); it != s->tab.rend(); ++it)
+        if (it->slab >= 0) { last = it->slab; end = it->off + (int64_t)it->rows * s->dim; break; }
+    while ((int)s->slabs.size() > last + 1) store_pop_slab(s);
+    if (last >= 0) s->slabs[(size_t)last].used = end;
+}
+
+// Passages p < n (tok packed by off, keep: rows that enter the max) become ordinals tab.size() + p; each is stored while
+// the budget allows (stored_out[p] = 1).  Forwards follow late_vectors' RERANK_MAX_TOKENS split, and a batch without a
+// stored passage runs none; late_gather_kernel copies each stored passage's kept rows into its slab, in row order.
+void late_store_append(LateStore* s, int n, const int32_t* tok, const int32_t* off, const uint8_t* keep, uint8_t* stored_out)
+{
+    Embedder* e = s->e;
+    store_check(s, e);
+    check_passages(e, n, off, keep);
+    const size_t n0 = s->tab.size();
+    try {
+        std::vector<int32_t> src, loff;
+        std::vector<float*> dst;
+        for (int b0 = 0; b0 < n;) {
+            int b1 = b0 + 1;
+            while (b1 < n && off[b1 + 1] - off[b0] <= RERANK_MAX_TOKENS) ++b1;
+            src.clear(); dst.clear();
+            for (int p = b0; p < b1; ++p) {
+                LateStore::Entry en{-1, kept_rows(off, keep, p), 0};
+                if (store_place(s, en.rows, en)) {
+                    float* base = s->slabs[(size_t)en.slab].a.p + en.off;
+                    int r = 0;
+                    for (int t = off[p]; t < off[p + 1]; ++t)
+                        if (keep[t]) { src.push_back(t - off[b0]); dst.push_back(base + (size_t)r++ * s->dim); }
+                }
+                s->tab.push_back(en);
+                stored_out[p] = en.slab >= 0;
+            }
+            if (!src.empty()) {
+                const int64_t n_tok = off[b1] - off[b0];
+                loff.resize((size_t)(b1 - b0) + 1);
+                for (int j = 0; j <= b1 - b0; ++j) loff[(size_t)j] = off[b0 + j] - off[b0];
+                if (e->li_p.cap < n_tok * e->li_pad) e->li_p.alloc(n_tok * e->li_pad);
+                late_vectors(e, b1 - b0, tok + off[b0], loff.data(), nullptr, e->li_p.p);
+                late_gather(e, e->li_p.p, src, dst);
+            }
+            b0 = b1;
+        }
+        KRAG_CUDA(cudaStreamSynchronize(e->st));
+    } catch (...) {
+        s->tab.resize(n0);
+        store_trim(s);
+        throw;
+    }
+}
+
+void late_store_truncate(LateStore* s, int64_t n)
+{
+    if (n < 0 || n > (int64_t)s->tab.size()) throw std::runtime_error("embedder: truncate to at most the store's ordinal count");
+    s->tab.resize((size_t)n);
+    store_trim(s);
+}
+
+// Keeps the ordinals whose bit is set in alive (bit o % 32 of word o / 32), renumbered 0 .. n_live - 1 in order, and moves
+// their stored rows down in the same order by next fit over the same slabs: a passage goes to the first slab, from the write
+// position on, with room for it.  Slabs differ in size (one opened when the budget was nearly spent is small), so that may
+// skip a slab; the passage's own slab always has room at or before its old offset, so no passage moves up and the moves run
+// front to back.  A move within a slab that overlaps its own source goes through a scratch buffer.  Slabs left without a
+// passage are freed.  A CUDA error part way leaves rows moved under the old table: the store is then unusable (the service
+// destroys it and reranks the index per call).
+void late_store_compact(LateStore* s, const uint32_t* alive, int64_t n)
+{
+    if (n != (int64_t)s->tab.size()) throw std::runtime_error("embedder: the alive bitmap must cover every ordinal of the store");
+    cudaStream_t st = s->e->st;
+    std::vector<LateStore::Entry> nt;
+    DevArray<float> bounce;
+    int ws = 0;
+    int64_t wo = 0;
+    for (int64_t o = 0; o < n; ++o) {
+        if (!((alive[o >> 5] >> (o & 31)) & 1u)) continue;
+        LateStore::Entry en = s->tab[(size_t)o];
+        if (en.slab >= 0) {
+            const int64_t need = (int64_t)en.rows * s->dim;
+            while (s->slabs[(size_t)ws].a.cap - wo < need) { ++ws; wo = 0; }   // stops at en.slab at the latest
+            float* to = s->slabs[(size_t)ws].a.p + wo;
+            const float* from = s->slabs[(size_t)en.slab].a.p + en.off;
+            if (to != from) {
+                const size_t bytes = sizeof(float) * (size_t)need;
+                if (ws == en.slab && en.off - wo < need) {           // overlapping: source -> scratch -> destination
+                    if (bounce.cap < need) {
+                        KRAG_CUDA(cudaStreamSynchronize(st));       // the previous scratch's copies are done before it goes
+                        bounce.alloc(need);
+                    }
+                    KRAG_CUDA(cudaMemcpyAsync(bounce.p, from, bytes, cudaMemcpyDeviceToDevice, st));
+                    KRAG_CUDA(cudaMemcpyAsync(to, bounce.p, bytes, cudaMemcpyDeviceToDevice, st));
+                } else {
+                    KRAG_CUDA(cudaMemcpyAsync(to, from, bytes, cudaMemcpyDeviceToDevice, st));
+                }
+            }
+            en.slab = ws; en.off = wo;
+            wo += need;
+        }
+        nt.push_back(en);
+    }
+    KRAG_CUDA(cudaStreamSynchronize(st));
+    std::vector<int32_t> keep_slab(s->slabs.size(), -1);
+    for (const auto& en : nt)
+        if (en.slab >= 0) keep_slab[(size_t)en.slab] = 0;
+    std::vector<LateStore::Slab> kept;
+    for (size_t k = 0; k < s->slabs.size(); ++k) {
+        if (keep_slab[k] < 0) {
+            s->e->store_bytes -= s->slabs[k].a.bytes();
+            continue;                                               // freed when s->slabs is replaced below
+        }
+        keep_slab[k] = (int32_t)kept.size();
+        kept.push_back(std::move(s->slabs[k]));
+    }
+    for (auto& en : nt)
+        if (en.slab >= 0) en.slab = keep_slab[(size_t)en.slab];
+    s->slabs = std::move(kept);
+    s->tab = std::move(nt);
+    store_trim(s);
+}
+
+void late_store_stats(const LateStore* s, int64_t* ordinals, int64_t* stored, int64_t* rows, int64_t* bytes)
+{
+    int64_t k = 0, r = 0, b = 0;
+    for (const auto& en : s->tab)
+        if (en.slab >= 0) { ++k; r += en.rows; }
+    for (const auto& sl : s->slabs) b += sl.a.bytes();
+    *ordinals = (int64_t)s->tab.size(); *stored = k; *rows = r; *bytes = b;
+}
+
+void late_store_vectors(const LateStore* s, int64_t ordinal, float* out_host, int64_t n_rows)
+{
+    if (ordinal < 0 || ordinal >= (int64_t)s->tab.size() || s->tab[(size_t)ordinal].slab < 0)
+        throw std::runtime_error("embedder: the store does not hold ordinal " + std::to_string(ordinal));
+    const LateStore::Entry& en = s->tab[(size_t)ordinal];
+    if (n_rows != en.rows) throw std::runtime_error("embedder: the ordinal holds " + std::to_string(en.rows) + " rows");
+    KRAG_CUDA(cudaMemcpyAsync(out_host, s->slabs[(size_t)en.slab].a.p + en.off, sizeof(float) * (size_t)n_rows * s->dim,
+                              cudaMemcpyDeviceToHost, s->e->st));
+    KRAG_CUDA(cudaStreamSynchronize(s->e->st));
+}
+
+// Late-interaction reranking.  n_queries queries of q_rows tokens each (q_tok [n_queries * q_rows], keys q_kv[i] <= q_rows),
+// n_pass passages of the call (p_tok packed by p_off [n_pass + 1], p_keep[t] = 1 where row t enters the max), query i owns
+// pairs pair_off[i] .. pair_off[i + 1].  Without a store, pair p scores passage pair_src[p] of the call; with one, pair_src[p]
+// >= 0 names a stored ordinal and < 0 passage ~pair_src[p] of the call.  Each query and each passage of the call is encoded
+// once and its kept rows gathered into li_k; maxsim_kernel writes every pair's score at its offset from the pair table, and
+// rerank_select_kernel orders each query's scores as for krag_rerank.
+static void late_rerank(Embedder* e, const LateStore* s, int n_queries, int q_rows, const int32_t* q_tok, const int32_t* q_kv, int n_pass,
+                        const int32_t* p_tok, const int32_t* p_off, const uint8_t* p_keep, const int32_t* pair_off, const int32_t* pair_src,
+                        int top_k, int32_t* out_pos, float* out_score)
+{
+    if (s) store_check(s, e);
     if (q_rows < 1 || q_rows > MS_QROWS) throw std::runtime_error("embedder: a late-interaction query holds 1 to 32 tokens");
     if (top_k < 1 || top_k > RERANK_MAX_CANDIDATES) throw std::runtime_error("embedder: top_k must be in [1, 300]");
     if (n_queries < 1 || pair_off[0] != 0) throw std::runtime_error("embedder: pair offsets must start at 0");
@@ -1909,44 +2202,68 @@ void embedder_late_rerank(Embedder* e, int n_queries, int q_rows, const int32_t*
     std::vector<int32_t> q_off((size_t)n_queries + 1);
     for (int q = 0; q <= n_queries; ++q) q_off[(size_t)q] = q * q_rows;
     late_check(e, n_queries, q_off.data());
-    if (n_pairs > 0) {
-        if (n_pass < 1) throw std::runtime_error("embedder: pairs need passages");
-        late_check(e, n_pass, p_off);
-        for (int p = 0; p < n_pass; ++p) {
-            int kept = 0;
-            for (int t = p_off[p]; t < p_off[p + 1]; ++t) kept += p_keep[t] != 0;
-            if (!kept) throw std::runtime_error("embedder: every passage needs at least one row that enters the max");
+    if (n_pairs == 0) n_pass = 0;
+    if (n_pairs > 0 && !s && n_pass < 1) throw std::runtime_error("embedder: pairs need passages");
+    if (n_pass < 0) throw std::runtime_error("embedder: the passage count must be >= 0");
+    if (n_pass > 0) check_passages(e, n_pass, p_off, p_keep);
+    for (int p = 0; p < n_pairs; ++p) {
+        const int32_t x = pair_src[p];
+        if (!s || x < 0) {
+            const int32_t c = s ? ~x : x;
+            if (c < 0 || c >= n_pass) throw std::runtime_error("embedder: a pair's passage index is out of range");
+        } else if (x >= (int64_t)s->tab.size() || s->tab[(size_t)x].slab < 0) {
+            throw std::runtime_error("embedder: a pair names ordinal " + std::to_string(x) + ", which the store does not hold");
         }
-        for (int p = 0; p < n_pairs; ++p)
-            if (pair_pass[p] < 0 || pair_pass[p] >= n_pass) throw std::runtime_error("embedder: a pair's passage index is out of range");
     }
     cudaStream_t st = e->st;
-    const int64_t pad = e->li_pad, nq_tok = (int64_t)n_queries * q_rows, np_tok = n_pairs > 0 ? p_off[n_pass] : 0;
+    const int64_t pad = e->li_pad, dim = e->li_dim, nq_tok = (int64_t)n_queries * q_rows;
     if (e->li_q.cap < nq_tok * pad) e->li_q.alloc(nq_tok * pad);
-    if (np_tok > 0 && e->li_p.cap < np_tok * pad) e->li_p.alloc(np_tok * pad);
     if (e->scores.cap < (n_pairs > 0 ? n_pairs : 1)) e->scores.alloc(n_pairs > 0 ? n_pairs : 1);
     if (e->d_poff.cap < n_queries + 1) e->d_poff.alloc(n_queries + 1);
     if (e->sel.cap < 2 * (int64_t)n_queries * top_k) e->sel.alloc(2 * (int64_t)n_queries * top_k);
     late_vectors(e, n_queries, q_tok, q_off.data(), q_kv, e->li_q.p);
     KRAG_CUDA(cudaMemcpyAsync(e->d_poff.p, pair_off, 4 * (size_t)(n_queries + 1), cudaMemcpyHostToDevice, st));
     if (n_pairs > 0) {
-        late_vectors(e, n_pass, p_tok, p_off, nullptr, e->li_p.p);
-        if (e->li_off.cap < n_pass + 1) e->li_off.alloc(n_pass + 1);
-        if (e->li_pp.cap < n_pairs) e->li_pp.alloc(n_pairs);
-        if (e->li_keep.cap < np_tok) e->li_keep.alloc(np_tok);
-        KRAG_CUDA(cudaMemcpyAsync(e->li_off.p, p_off, 4 * (size_t)(n_pass + 1), cudaMemcpyHostToDevice, st));
-        KRAG_CUDA(cudaMemcpyAsync(e->li_pp.p, pair_pass, 4 * (size_t)n_pairs, cudaMemcpyHostToDevice, st));
-        KRAG_CUDA(cudaMemcpyAsync(e->li_keep.p, p_keep, (size_t)np_tok, cudaMemcpyHostToDevice, st));
+        std::vector<int64_t> koff((size_t)n_pass + 1, 0);        // kept rows of the call's passages, packed in li_k
+        if (n_pass > 0) {
+            const int64_t np_tok = p_off[n_pass];
+            for (int p = 0; p < n_pass; ++p) koff[(size_t)p + 1] = koff[(size_t)p] + kept_rows(p_off, p_keep, p);
+            if (e->li_p.cap < np_tok * pad) e->li_p.alloc(np_tok * pad);
+            if (e->li_k.cap < koff[(size_t)n_pass] * dim) e->li_k.alloc(koff[(size_t)n_pass] * dim);
+            late_vectors(e, n_pass, p_tok, p_off, nullptr, e->li_p.p);
+            std::vector<int32_t> src;
+            std::vector<float*> dst;
+            src.reserve((size_t)koff[(size_t)n_pass]); dst.reserve((size_t)koff[(size_t)n_pass]);
+            for (int t = 0; t < np_tok; ++t)
+                if (p_keep[t]) { dst.push_back(e->li_k.p + (size_t)src.size() * dim); src.push_back(t); }
+            late_gather(e, e->li_p.p, src, dst);
+        }
+        std::vector<MsPair> tab((size_t)n_pairs);
+        for (int p = 0; p < n_pairs; ++p) {
+            const int32_t x = pair_src[p];
+            if (!s || x < 0) {
+                const int32_t c = s ? ~x : x;
+                tab[(size_t)p] = MsPair{e->li_k.p + koff[(size_t)c] * dim, (int32_t)(koff[(size_t)c + 1] - koff[(size_t)c]), 0};
+            } else {
+                const LateStore::Entry& en = s->tab[(size_t)x];
+                tab[(size_t)p] = MsPair{s->slabs[(size_t)en.slab].a.p + en.off, en.rows, 0};
+            }
+        }
+        if (e->li_tab.cap < n_pairs) e->li_tab.alloc(n_pairs);
+        KRAG_CUDA(cudaMemcpyAsync(e->li_tab.p, tab.data(), sizeof(MsPair) * (size_t)n_pairs, cudaMemcpyHostToDevice, st));
         int max_pairs = 0;
         for (int q = 0; q < n_queries; ++q) max_pairs = std::max(max_pairs, pair_off[q + 1] - pair_off[q]);
-        // slices per query: about two CTAs per SM over the call, one pair per CTA at most
-        const int want = (2 * e->di.sm_count + n_queries - 1) / n_queries;
-        const int slices = std::max(1, std::min(max_pairs, want));
         const size_t smem = maxsim_smem(e->li_dim);
         static bool attr = false;
         if (!attr) { KRAG_CUDA(cudaFuncSetAttribute(maxsim_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)maxsim_smem(256))); attr = true; }
-        maxsim_kernel<<<dim3((unsigned)n_queries, (unsigned)slices), MS_THREADS, smem, st>>>(e->li_q.p, q_rows, e->li_p.p, e->li_off.p, e->li_keep.p,
-                                                                                         e->d_poff.p, e->li_pp.p, e->li_dim, (int)pad, e->scores.p);
+        // slices per query: about four resident waves of CTAs over the call, so the last wave's tail is short
+        int per_sm = 1;
+        KRAG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, maxsim_kernel, MS_THREADS, smem));
+        const int resident = std::max(1, per_sm) * e->di.sm_count;
+        const int want = (4 * resident + n_queries - 1) / n_queries;
+        const int slices = std::max(1, std::min(max_pairs, want));
+        maxsim_kernel<<<dim3((unsigned)n_queries, (unsigned)slices), MS_THREADS, smem, st>>>(e->li_q.p, q_rows, (int)pad, e->li_tab.p, e->d_poff.p,
+                                                                                         e->li_dim, e->scores.p);
         KRAG_CUDA(cudaGetLastError());
         count_launch();
     }
@@ -1959,6 +2276,20 @@ void embedder_late_rerank(Embedder* e, int n_queries, int q_rows, const int32_t*
     KRAG_CUDA(cudaStreamSynchronize(st));
     std::memcpy(out_pos, h.data(), 4 * nk);
     std::memcpy(out_score, h.data() + nk, 4 * nk);
+}
+
+void embedder_late_rerank(Embedder* e, int n_queries, int q_rows, const int32_t* q_tok, const int32_t* q_kv, int n_pass, const int32_t* p_tok,
+                          const int32_t* p_off, const uint8_t* p_keep, const int32_t* pair_off, const int32_t* pair_pass, int top_k,
+                          int32_t* out_pos, float* out_score)
+{
+    late_rerank(e, nullptr, n_queries, q_rows, q_tok, q_kv, n_pass, p_tok, p_off, p_keep, pair_off, pair_pass, top_k, out_pos, out_score);
+}
+
+void late_store_rerank(Embedder* e, const LateStore* s, int n_queries, int q_rows, const int32_t* q_tok, const int32_t* q_kv, int n_pass,
+                       const int32_t* p_tok, const int32_t* p_off, const uint8_t* p_keep, const int32_t* pair_off, const int32_t* pair_src,
+                       int top_k, int32_t* out_pos, float* out_score)
+{
+    late_rerank(e, s, n_queries, q_rows, q_tok, q_kv, n_pass, p_tok, p_off, p_keep, pair_off, pair_src, top_k, out_pos, out_score);
 }
 
 }  // namespace krag

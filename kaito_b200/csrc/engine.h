@@ -544,6 +544,21 @@ void embedder_late_vectors(Embedder* e, int batch, const int32_t* tok_ids, const
 void embedder_late_rerank(Embedder* e, int n_queries, int q_rows, const int32_t* q_tok, const int32_t* q_kv, int n_pass, const int32_t* p_tok,
                           const int32_t* p_off, const uint8_t* p_keep, const int32_t* pair_off, const int32_t* pair_pass, int top_k,
                           int32_t* out_pos, float* out_score);
+// Stores of passage token vectors (kept rows only, fp32, per ordinal in device slabs) filled from a late-interaction
+// embedder; their slabs share the embedder's budget of device bytes.  late_store_rerank: pair_src >= 0 names a stored
+// ordinal, < 0 passage ~pair_src of the call (see embed.cu)
+struct LateStore;
+void embedder_set_store_budget(Embedder* e, int64_t bytes);
+LateStore* late_store_create(Embedder* e);
+void late_store_destroy(LateStore* s);
+void late_store_append(LateStore* s, int n, const int32_t* tok, const int32_t* off, const uint8_t* keep, uint8_t* stored_out);
+void late_store_truncate(LateStore* s, int64_t n);
+void late_store_compact(LateStore* s, const uint32_t* alive, int64_t n);
+void late_store_stats(const LateStore* s, int64_t* ordinals, int64_t* stored, int64_t* rows, int64_t* bytes);
+void late_store_vectors(const LateStore* s, int64_t ordinal, float* out_host, int64_t n_rows);
+void late_store_rerank(Embedder* e, const LateStore* s, int n_queries, int q_rows, const int32_t* q_tok, const int32_t* q_kv, int n_pass,
+                       const int32_t* p_tok, const int32_t* p_off, const uint8_t* p_keep, const int32_t* pair_off, const int32_t* pair_src,
+                       int top_k, int32_t* out_pos, float* out_score);
 // A fp32 matrix carried as two fp16 planes: v = hi + lo * 2^-11 (see embed.cu: split operands of the K5 GEMMs)
 struct SplitMat { uint16_t* hi; uint16_t* lo; };
 void launch_split_f16(const float* in, uint16_t* hi, uint16_t* lo, int64_t n /* % 8 == 0 */, cudaStream_t st);

@@ -29,6 +29,22 @@ def precision_from_env() -> str:
     return p
 
 
+def store_bytes_from_env(colbert: bool) -> int:
+    """KRAG_RERANK_STORE_GB (default 0: off): the device bytes (GB = 10^9 bytes) a ColBERT reranker may spend on stored
+    passage vectors, over all indexes; a ValueError for a value that is not a number, is negative, or asks a
+    cross-encoder to store (its passages are scored with their queries, so there is nothing to store)"""
+    raw = os.getenv("KRAG_RERANK_STORE_GB") or "0"
+    try:
+        gb = float(raw)
+    except ValueError:
+        raise ValueError(f"KRAG_RERANK_STORE_GB {raw!r}: expected a number of GB") from None
+    if not gb >= 0 or gb == float("inf"):
+        raise ValueError(f"KRAG_RERANK_STORE_GB {raw!r}: must be a finite number >= 0")
+    if gb > 0 and not colbert:
+        raise ValueError(f"KRAG_RERANK_STORE_GB {raw!r}: only a ColBERT reranker stores passage vectors (this one is a cross-encoder)")
+    return int(gb * 1e9)
+
+
 def _activation(cpath: str, cfg: dict) -> str:
     st = cfg.get("sentence_transformers") if isinstance(cfg.get("sentence_transformers"), dict) else {}
     fn = st.get("activation_fn") or cfg.get("sbert_ce_default_activation_function") or "torch.nn.modules.activation.Sigmoid"
@@ -419,12 +435,67 @@ def colbert_skip_ids(tokenizer, words) -> np.ndarray:
     return np.unique(np.asarray([t[0] for t in tokenizer.encode_batch_plain(words) if len(t)], np.int32))
 
 
+def _pack(docs):
+    """(tokens, offsets, keep) of encode_passages' output, packed"""
+    off = np.zeros(len(docs) + 1, np.int32)
+    np.cumsum([len(d[0]) for d in docs], out=off[1:])
+    tok = np.concatenate([d[0] for d in docs]) if docs else np.zeros(0, np.int32)
+    keep = np.concatenate([d[1] for d in docs]) if docs else np.zeros(0, np.uint8)
+    return tok, off, keep
+
+
+class PassageStore:
+    """One index's ColBERT passage vectors on the reranker's GPU (a _native.LateStore, one entry per node ordinal) and the
+    host's record of which ordinals it holds: GpuLateInteractionReranker.rerank scores those from the store and encodes the
+    others in the call.  Every call holds the reranker's lock (the store works on the embedder's stream and scratch)."""
+
+    APPEND_BATCH = 8192              # passages tokenised and appended per native call (bounds the host's token arrays)
+
+    def __init__(self, reranker: "GpuLateInteractionReranker", native):
+        self._rr, self.native = reranker, native
+        self.stored = np.zeros(0, bool)
+
+    def __len__(self) -> int:
+        return len(self.stored)
+
+    def append(self, texts: list[str]):
+        """the next len(texts) ordinals: encode_passages of each text (as rerank() would encode it), stored while the
+        budget allows"""
+        for i in range(0, len(texts), self.APPEND_BATCH):
+            tok, off, keep = _pack(self._rr.encode_passages(texts[i:i + self.APPEND_BATCH]))
+            with self._rr._mu:
+                got = self.native.append(tok, off, keep)
+            self.stored = np.concatenate([self.stored, got.astype(bool)])
+
+    def truncate(self, n: int):
+        with self._rr._mu:
+            self.native.truncate(n)
+        self.stored = self.stored[:n]
+
+    def compact(self, alive):
+        """keep the ordinals where alive (bool per ordinal) is set, renumbered in order"""
+        alive = np.asarray(alive, bool)
+        with self._rr._mu:
+            self.native.compact(alive)
+        self.stored = self.stored[alive]
+
+    def stats(self) -> dict:
+        with self._rr._mu:
+            return self.native.stats()
+
+    def destroy(self):
+        with self._rr._mu:
+            self.native.destroy()
+
+
 class GpuLateInteractionReranker:
     """A ColBERT late-interaction model on the GPU (krag_late_rerank), with GpuCrossEncoder's interface: rerank(queries,
     candidate ordinals per query, top_k, passages) and encode_passages for the store's per-ordinal token cache.  Each distinct
-    candidate ordinal of a call is encoded once."""
+    candidate ordinal of a call is encoded once.  With store_bytes > 0 (KRAG_RERANK_STORE_GB), create_store gives each index
+    a PassageStore, filled at /index, and rerank(..., store=) encodes only the candidates it does not hold."""
 
-    def __init__(self, engine, tokenizer, config: dict, state_dict: dict, weight: np.ndarray, spec: dict, precision: str = "fp32"):
+    def __init__(self, engine, tokenizer, config: dict, state_dict: dict, weight: np.ndarray, spec: dict, precision: str = "fp32",
+                 store_bytes: int = 0):
         from . import _native
         if precision not in PRECISIONS:
             raise ValueError(f"precision {precision!r}: expected 'fp32' or 'fp16'")
@@ -437,7 +508,18 @@ class GpuLateInteractionReranker:
         self._emb.set_late_interaction(weight)
         self._emb.load_state_dict({k: v for k, v in state_dict.items() if k != "linear.weight"})
         self._emb.set_precision(precision)
+        self.store_bytes = int(store_bytes)
+        if self.store_bytes > 0:
+            self._emb.set_store_budget(self.store_bytes)
         self._mu = threading.Lock()
+
+    def create_store(self):
+        """a PassageStore for one index, or None when storing is off (store_bytes 0)"""
+        if self.store_bytes <= 0:
+            return None
+        from . import _native
+        with self._mu:
+            return PassageStore(self, _native.LateStore(self._emb))
 
     @classmethod
     def from_pretrained(cls, engine, model_dir: str, **kw):
@@ -477,18 +559,24 @@ class GpuLateInteractionReranker:
             out.append((ids, (~np.isin(ids, self.skip)).astype(np.uint8)))
         return out
 
-    def rerank(self, queries: list[str], candidates: list, top_k: int, passages):
+    def rerank(self, queries: list[str], candidates: list, top_k: int, passages, store: PassageStore | None = None):
         """(positions int32 [n_queries, top_k], scores float32 [n_queries, top_k]) of each query's best top_k candidates
-        (position within its candidate list; -1 / NaN past its count), ties by position ascending"""
+        (position within its candidate list; -1 / NaN past its count), ties by position ascending.  With a store, its
+        ordinals are scored from their stored vectors (the same bits) and only the others go through `passages`."""
         q_ids, q_keys = self.query_ids(list(queries))
         poff = np.zeros(len(candidates) + 1, np.int32)
         np.cumsum([len(c) for c in candidates], out=poff[1:])
         flat = np.concatenate([np.asarray(c, np.int64) for c in candidates]) if len(candidates) else np.zeros(0, np.int64)
         uniq, pair_pass = np.unique(flat, return_inverse=True)
-        docs = passages(uniq, self.encode_passages) if len(uniq) else []
-        d_off = np.zeros(len(docs) + 1, np.int32)
-        np.cumsum([len(d[0]) for d in docs], out=d_off[1:])
-        d_tok = np.concatenate([d[0] for d in docs]) if docs else np.zeros(0, np.int32)
-        d_keep = np.concatenate([d[1] for d in docs]) if docs else np.zeros(0, np.uint8)
+        if store is None:
+            d_tok, d_off, d_keep = _pack(passages(uniq, self.encode_passages) if len(uniq) else [])
+            with self._mu:
+                return self._emb.late_rerank(q_ids, q_keys, d_tok, d_off, d_keep, poff, pair_pass.astype(np.int32), top_k)
+        held = uniq < len(store.stored)
+        held[held] = store.stored[uniq[held]]
+        encode = np.flatnonzero(~held)
+        source = uniq.astype(np.int32)                    # a stored ordinal names itself, the others ~(position in `encode`)
+        source[encode] = ~np.arange(len(encode), dtype=np.int32)
+        d_tok, d_off, d_keep = _pack(passages(uniq[encode], self.encode_passages) if len(encode) else [])
         with self._mu:
-            return self._emb.late_rerank(q_ids, q_keys, d_tok, d_off, d_keep, poff, pair_pass.astype(np.int32), top_k)
+            return self._emb.late_rerank_stored(store.native, q_ids, q_keys, d_tok, d_off, d_keep, poff, source[pair_pass], top_k)

@@ -432,11 +432,13 @@ def main():
             raise SystemExit(f"embedding model '{cfg['embedding_model']}' is not supported by this image: {e}")
     rerank_dir = os.getenv("KRAG_RERANK_MODEL_DIR") or None
     if rerank_dir:
-        from .rerank import is_colbert_snapshot, precision_from_env, read_colbert_spec, read_cross_encoder_spec
+        from .rerank import is_colbert_snapshot, precision_from_env, read_colbert_spec, read_cross_encoder_spec, store_bytes_from_env
         try:
             # refuse a reranker K5 cannot run before any GPU work starts
-            (read_colbert_spec if is_colbert_snapshot(rerank_dir) else read_cross_encoder_spec)(rerank_dir)
+            colbert = is_colbert_snapshot(rerank_dir)
+            (read_colbert_spec if colbert else read_cross_encoder_spec)(rerank_dir)
             rerank_precision = precision_from_env()
+            rerank_store = store_bytes_from_env(colbert)
             if int(os.getenv("KRAG_RERANK_CANDIDATES", "30")) < 1:
                 raise ValueError("KRAG_RERANK_CANDIDATES must be >= 1")
         except ValueError as e:
@@ -472,8 +474,10 @@ def main():
         from .rerank import GpuCrossEncoder, GpuLateInteractionReranker, is_colbert_snapshot
         try:
             # on rank 0 after the exchange: K5 + MaxSim (ColBERT) or K5 + classifier head (cross-encoder)
-            kind = GpuLateInteractionReranker if is_colbert_snapshot(rerank_dir) else GpuCrossEncoder
-            reranker = kind.from_pretrained(ctx, rerank_dir, precision=rerank_precision)
+            if is_colbert_snapshot(rerank_dir):
+                reranker = GpuLateInteractionReranker.from_pretrained(ctx, rerank_dir, precision=rerank_precision, store_bytes=rerank_store)
+            else:
+                reranker = GpuCrossEncoder.from_pretrained(ctx, rerank_dir, precision=rerank_precision)
         except ValueError as e:
             raise SystemExit(f"reranker '{rerank_dir}' is not supported by this image: {e}")
     app = create_app(vs.VectorStore(embed, engine, reranker=reranker), cfg)

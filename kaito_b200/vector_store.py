@@ -130,8 +130,11 @@ class _Node:
 
 
 class _IndexState:
-    def __init__(self, index):
+    def __init__(self, index, late_store=None):
         self.index = index                       # kaito_b200._native.Index (or a test double)
+        # the ColBERT reranker's stored passage vectors of this index (kaito_b200.rerank.PassageStore, one entry per ordinal), or
+        # None: created by the reranker when KRAG_RERANK_STORE_GB > 0; lives on rank 0 beside the reranker
+        self.late_store = late_store
         self.vocab = _text.Vocabulary()
         self.nodes: list[_Node] = []             # by ordinal (== insertion order == engine row)
         self.ref_docs: dict[str, dict] = {}      # doc_id -> {"text", "metadata", "nodes": [ordinal]}
@@ -275,7 +278,9 @@ class HybridRetriever:
         counts = np.asarray(out["count"])
         cands = [np.asarray(out["ordinal"][b, :int(counts[b])]) for b in range(len(queries))]
         k = self._rerank_top_k
-        pos, score = self._reranker.rerank(queries, cands, k, self._state.pair_passages)
+        store = self._state.late_store
+        kw = {"store": store} if store is not None else {}
+        pos, score = self._reranker.rerank(queries, cands, k, self._state.pair_passages, **kw)
         pos = np.asarray(pos, np.int64)
         valid = pos >= 0
         take = np.where(valid, pos, 0)
@@ -316,7 +321,7 @@ class VectorStore:
         with self._rw.writer():
             st = self.index_map.get(index_name)
             if st is None:
-                st = _IndexState(self.engine.create_index(index_name, self.dimension))
+                st = _IndexState(self.engine.create_index(index_name, self.dimension), self._new_late_store())
                 self.index_map[index_name] = st
             ids, fresh, fresh_ids = [], [], set()
             for doc in documents:
@@ -329,6 +334,22 @@ class VectorStore:
             if fresh:
                 self._insert(st, fresh)
             return ids
+
+    def _new_late_store(self):
+        """the reranker's passage vector store for a new index, or None (no ColBERT reranker, or storing off)"""
+        create = getattr(self.reranker, "create_store", None)
+        return create() if create is not None else None
+
+    @staticmethod
+    def _drop_store(st: _IndexState):
+        store, st.late_store = st.late_store, None
+        if store is not None:
+            store.destroy()
+
+    @staticmethod
+    def _drop_state(st: _IndexState):
+        st.index.drop()
+        VectorStore._drop_store(st)
 
     def _insert(self, st: _IndexState, docs, replace: bool = False):
         """Chunk, analyse, embed and append `docs`; the host docstore is published only after the embedder and the
@@ -354,9 +375,17 @@ class VectorStore:
                 ords.append(ordinal)
             new_refs[doc_id] = {"text": text, "metadata": metadata, "nodes": ords}
         vecs = np.asarray(self.embed_model.get_text_embedding_batch(texts), np.float32)
-        st.index.add(np.asarray(node_ids, np.uint64), vecs, np.asarray(offs, np.int64),
-                     np.concatenate(tids) if tids else np.zeros(0, np.uint32),
-                     np.concatenate(tfs) if tfs else np.zeros(0, np.uint16), np.asarray(dls, np.uint32))
+        store = st.late_store
+        try:
+            if store is not None:               # ordinals base .. : the texts rerank() would encode for them
+                store.append(texts)
+            st.index.add(np.asarray(node_ids, np.uint64), vecs, np.asarray(offs, np.int64),
+                         np.concatenate(tids) if tids else np.zeros(0, np.uint32),
+                         np.concatenate(tfs) if tfs else np.zeros(0, np.uint16), np.asarray(dls, np.uint32))
+        except BaseException:
+            if store is not None:
+                store.truncate(base)
+            raise
         # the rows are in the engine: publish.  (A failing commit below leaves the index "uncommitted": /retrieve takes
         # the reference's vector-only fallback until the next successful commit.)
         st.nodes.extend(new_nodes)
@@ -394,6 +423,14 @@ class VectorStore:
                 or not hasattr(st.index, "compact")):      # an engine without compaction keeps its tombstones
             return
         st.index.compact()
+        if st.late_store is not None:           # the same renumbering as below: live ordinals in order
+            try:
+                st.late_store.compact([n.alive for n in st.nodes])
+            except Exception:
+                # the engine has compacted, so the host renumbers below whatever happens here; a store that could not
+                # follow (a device error, possibly part way through its moves) no longer matches the ordinals: drop it,
+                # and the index is reranked per call, with the same scores
+                self._drop_store(st)
         live = [n for n in st.nodes if n.alive]
         # the sharded engine's node ids are the ordinals: its compaction renumbers them too, and the next node gets n_live
         renumber = getattr(st.index, "compact_renumbers_keys", False)
@@ -629,7 +666,7 @@ class VectorStore:
         if index_name not in self.index_map:
             raise HTTPException(404, f"No such index: '{index_name}' exists.")
         with self._rw.writer():
-            self.index_map.pop(index_name).index.drop()
+            self._drop_state(self.index_map.pop(index_name))
 
     # -------------------------------------------------------- persist / load
     def persist(self, index_name: str, path: str):
@@ -672,13 +709,21 @@ class VectorStore:
                     fresh.next_key = max(keys) + 1 if keys else len(fresh.nodes)
                     fresh.n_dead = sum(1 for n in fresh.nodes if not n.alive)
                     fresh.committed = True
+                    # the snapshot holds no passage vectors: every node, dead ones too (compaction drops them), in ordinal order.
+                    # The index being replaced gives its stored vectors back to the shared budget first (it keeps serving,
+                    # reranked per call, should this load still fail), so the fresh store can take their room.
+                    if index_name in self.index_map:
+                        self._drop_store(self.index_map[index_name])
+                    fresh.late_store = self._new_late_store()
+                    if fresh.late_store is not None:
+                        fresh.late_store.append([embed_text(n.text, n.metadata) for n in fresh.nodes])
                 except Exception:
-                    fresh.index.drop()
+                    self._drop_state(fresh)
                     raise
                 old = self.index_map.get(index_name)
                 self.index_map[index_name] = fresh
                 if old is not None:
-                    old.index.drop()
+                    self._drop_state(old)
         except HTTPException:
             raise
         except Exception as e:
